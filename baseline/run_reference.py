@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Time the UNMODIFIED reference (staged under ``baseline/_ref`` by ``baseline/stage_reference.py``) on the hot path:
+"""Time the UNMODIFIED reference (staged under ``oracle/_ref`` by ``oracle/stage_reference.py``) on the hot path:
 ``MAMLFewShotClassifier.run_train_iter`` (reference few_shot_learning_system.py:338-369) through the reference's own
 public API and stock code path -- none of this repo's kernels, engine or model code runs here.  What this repo
 contributes is the workload description only: the args Bunch of a BASELINE configuration (the reference's own JSON
@@ -23,7 +23,7 @@ import time
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF = os.path.join(HERE, "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 
 def cpu_model():
@@ -52,7 +52,7 @@ def main():
     cli = ap.parse_args()
 
     if not os.path.isdir(REF) or not os.path.exists(os.path.join(REF, "few_shot_learning_system.py")):
-        print(json.dumps({"unavailable": "baseline/_ref is not staged (run baseline/stage_reference.py where /root/reference exists)"}))
+        print(json.dumps({"unavailable": "oracle/_ref is not staged (run oracle/stage_reference.py)"}))
         return 0
     if cli.device == "cpu":
         os.environ["CUDA_VISIBLE_DEVICES"] = ""
@@ -129,7 +129,7 @@ def main():
     except Exception:
         pass
     out = {
-        "impl": "reference (unmodified, baseline/_ref)", "commit": commit, "config": cli.config, "device": str(dev),
+        "impl": "reference (unmodified, oracle/_ref)", "commit": commit, "config": cli.config, "device": str(dev),
         "batch_size": int(args.batch_size), "tasks_per_sec": args.batch_size / med, "ms_per_iter": 1e3 * med,
         "times_s": times, "warmup": max(1, cli.warmup), "threads": (threads if dev.type == "cpu" else None),
         "host_threads": ncpu, "cpu_model": cpu_model(), "thread_probe_s": tuned, "last_loss": loss,

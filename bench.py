@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the MAML / MAML++ hot path (BASELINE.json metric: meta-tasks/sec, 5-way, 5 inner steps).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--config NAME] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--config NAME] [--impl ours|reference] [--dump-outputs DIR]
 
 One "step" = one ``run_train_iter`` over one meta-batch of synthetic episodes: inner-loop unroll for every
 task, second-order meta-gradient, (all-reduce over ranks), clamp + Adam, running-stat EMA.
@@ -16,6 +16,8 @@ task, second-order meta-gradient, (all-reduce over ranks), clamp + Adam, running
              the reference -- the reference itself is Python and cannot travel to the GPU box), timed on the
              host cores on a bounded sample of the same workload.
 ``--impl reference`` prints the CPU arm as its own line (rank 0 only under torchrun).
+``--dump-outputs DIR`` writes what the last timed step computed (see ``dump_outputs``) so that two builds can be
+compared output for output on identical seeded inputs.
 Weak scaling: every rank holds ``batch_size`` tasks (tasks are sharded over GPUs, one all-reduce of the flat
 meta-gradient per iteration); the global meta-batch is N x batch_size.
 """
@@ -32,7 +34,7 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 METRIC = "meta-tasks/sec (5-way, 5 inner steps, second order)"
-DEFAULT_CONFIG = "omniglot_mamlpp_5w1s"          # BASELINE.json configs[1]: the 1xB200 headline workload
+DEFAULT_CONFIG = "omniglot_mamlpp_5w1s"          # BASELINE.json configs[1]: the single-GPU headline workload
 SCALING = {}                                      # config -> "weak" / "strong" (filled by main from the CLI)
 
 
@@ -69,7 +71,7 @@ def flops_per_task(args):
 
 
 class ClockSampler(object):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -120,7 +122,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback (B200_PROFILING.md)"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "fallback (NVIDIA H100 SXM data sheet, dense, 700 W; not measured)"
 
 
 def _cpu_port_iteration_times(args, iters, warmup, threads):
@@ -217,7 +219,7 @@ def _visible_gpu_token(local_rank):
 
 
 def run_unmodified_reference(config, batch_size, device, steps, warmup, local_rank=0, tune=True, max_seconds=240.0):
-    """Run ``baseline/run_reference.py`` (the UNMODIFIED reference staged under baseline/_ref, its own public API and
+    """Run ``baseline/run_reference.py`` (the UNMODIFIED reference staged under oracle/_ref, its own public API and
     stock code path) in a child process and return its JSON dict, or {"unavailable": why}."""
     script = os.path.join(ROOT, "baseline", "run_reference.py")
     cmd = [sys.executable, script, "--config", config, "--device", device, "--steps", str(steps), "--warmup", str(warmup),
@@ -246,7 +248,7 @@ def run_unmodified_reference(config, batch_size, device, steps, warmup, local_ra
 
 def reference_cpu_baseline(cli, args, steps, warmup):
     """cpu_baseline dict (+ raw run) from the unmodified reference on the host cores; falls back to the oracle port
-    (stated in ``kind``) only when baseline/_ref was not staged."""
+    (stated in ``kind``) only when oracle/_ref was not staged."""
     ref = run_unmodified_reference(cli.config, int(args.batch_size), "cpu", steps, warmup)
     if "unavailable" not in ref:
         sample = "%d timed iterations of %d tasks (median), %d warm-up, %d of %d host threads (1 probe iteration each at 8/16/32/64/all, fastest kept)" % (
@@ -261,7 +263,7 @@ def reference_cpu_baseline(cli, args, steps, warmup):
 
 
 def run_reference_arm(cli, args, rank, world):
-    """--impl reference: the reference's own CPU implementation of the path (unmodified, baseline/_ref) on the host
+    """--impl reference: the reference's own CPU implementation of the path (unmodified, oracle/_ref) on the host
     cores, same config / metric / unit; rank 0 only."""
     if rank != 0:
         return
@@ -278,7 +280,7 @@ def run_reference_arm(cli, args, rank, world):
         "e2e": {"value": cb["value"], "unit": "tasks/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "gpu_launches": 0,
         "note": "reference = the unmodified reference's run_train_iter (few_shot_learning_system.py:338-369) imported from "
-                "baseline/_ref with CUDA_VISIBLE_DEVICES='' (BASELINE.md section 4); one step = one meta-batch of %d tasks; "
+                "oracle/_ref with CUDA_VISIBLE_DEVICES='' (BASELINE.md section 4); one step = one meta-batch of %d tasks; "
                 "wall %.1f s" % (int(args.batch_size), time.perf_counter() - t0),
     }
     _emit(line)
@@ -318,11 +320,12 @@ def measure_device_loop(model, args, dev, rank, world, K, W, flush, n_pool=8, sa
     barrier()
     wall0 = time.perf_counter()
     loop0.record()
+    last = None
     for i in range(K):
         if flush is not None:
             flush.zero_()
         ev[i][0].record()
-        device_step(W + i)
+        last = device_step(W + i)
         ev[i][1].record()
         if sync_each_step:
             torch.cuda.synchronize()
@@ -331,7 +334,33 @@ def measure_device_loop(model, args, dev, rank, world, K, W, flush, n_pool=8, sa
     wall = time.perf_counter() - wall0
     step_ms = [a.elapsed_time(b) for a, b in ev]
     return {"step_ms": step_ms, "sum_ms": sum(step_ms), "loop_ms": loop0.elapsed_time(loop1), "wall_s": wall,
-            "host_batches": host_batches, "device_step": device_step, "barrier": barrier}
+            "host_batches": host_batches, "device_step": device_step, "barrier": barrier, "last": last}
+
+
+DUMP_LIMIT_BYTES = 64 * 2 ** 20
+
+
+def dump_outputs(model, last, out_dir):
+    """What a caller of the timed path receives from its last step, as ``<name>.npy``: ``result`` = [loss, n_correct],
+    ``logits`` = the target-set logits, ``state.<name>`` = every parameter and running statistic after the update.
+    float64 arrays stay float64, everything else is written as float32."""
+    import numpy as np
+    import torch
+    torch.cuda.synchronize()
+    head, logits = last[0], last[1]
+    arrays = [("result", head[0]), ("logits", logits)]
+    arrays += [("state." + k, v) for k, v in model.state_dict().items()]
+    out = []
+    for name, t in arrays:
+        if torch.is_tensor(t):
+            a = t.detach().cpu().numpy()
+            out.append((name, a.astype(np.float64 if a.dtype == np.float64 else np.float32)))
+    total = sum(a.nbytes for _, a in out)
+    if total > DUMP_LIMIT_BYTES:          # checked before anything is written: no partial directory
+        raise SystemExit("--dump-outputs: outputs take %d bytes, more than %d" % (total, DUMP_LIMIT_BYTES))
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in out:
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def gather_rank_stats(step_ms, loop_ms, coll_us, dev, world):
@@ -360,7 +389,7 @@ def roofline_from_profile(prof, prof_steps, peaks, peak_src, value, fpt, world, 
     achieved = dom_fl / (dom_ms * 1e-3) / 1e12 if dom_ms > 0 else 0.0
     all_ms, all_fl = dom_ms + c0_ms + w0_ms, dom_fl + c0_fl + w0_fl
     return {
-        "bound": "tensor", "kernel": "3x3 conv contractions of blocks >= 1: conv_tc_kernel (forward / dgrad / tangent) + wgrad_tc_kernel (weight gradient), both tcgen05 3xTF32 fed by TMA",
+        "bound": "tensor", "kernel": "3x3 conv contractions of blocks >= 1: conv_tc_kernel (forward / dgrad / tangent: wgmma 3xTF32 fed by TMA) + wgrad_row_kernel (weight gradient, fp32 FFMA)",
         "achieved": achieved, "peak": peak_3x, "unit": "TFLOP/s", "frac": achieved / peak_3x,
         "traffic": traffic,
         "peak_source": peak_src + ": bf16_tflops %.1f / 2 (tf32) / 3 (3xTF32 split)" % peaks["bf16_tflops"],
@@ -426,6 +455,8 @@ def main():
                     help="weak: every GPU holds the config's meta-batch; strong: the config's meta-batch is split over the GPUs")
     ap.add_argument("--no-flush", action="store_true", help="diagnostic: do not flush L2 between timed steps")
     ap.add_argument("--sync-each-step", action="store_true", help="diagnostic: synchronize after every timed step")
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (rank 0)")
     cli = ap.parse_args()
 
     # The contract is ONE JSON line on stdout.  Libraries write there too (NCCL prints its version banner to fd 1 when
@@ -468,7 +499,9 @@ def main():
     if world > 1:
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         dist.init_process_group("nccl", rank=rank, world_size=world, device_id=dev)
-    W, K = max(3, cli.warmup), max(1, cli.steps)
+    if cli.steps < 1:
+        raise SystemExit("--steps must be >= 1")
+    W, K = max(3, cli.warmup), cli.steps
 
     model = MAMLFewShotClassifier(im_shape=(2, args.image_channels, args.image_height, args.image_width), device=dev, args=args)
     B = int(args.batch_size)
@@ -478,6 +511,8 @@ def main():
     sampler = ClockSampler(local_rank) if rank == 0 else None
     r = measure_device_loop(model, args, dev, rank, world, K, W, flush, sampler=sampler, sync_each_step=cli.sync_each_step)
     step_ms, device_step, barrier = r["step_ms"], r["device_step"], r["barrier"]
+    if cli.dump_outputs and rank == 0:
+        dump_outputs(model, r["last"], cli.dump_outputs)
     host_batches = r["host_batches"]
     n_pool = len(host_batches)
     pinned_batches = [tuple(t.pin_memory() for t in hb) for hb in host_batches]
@@ -541,17 +576,7 @@ def main():
         value = tasks_total / (total_ms * 1e-3)
         e2e_value = tasks_total / (e2e_ms * 1e-3)
         fpt = flops_per_task(args)
-        traffic, traffic_note = None, None
-        for cand in ("ncu_summary_r2.json", "ncu_summary_r1.json"):
-            try:
-                d = json.load(open(os.path.join(ROOT, "profiles", cand)))
-                traffic = d["dominant_kernel_traffic_bytes_per_launch"]
-                traffic_note = d.get("traffic_note", "dram__bytes_read+write of one dominant-kernel launch (ncu --set full, cold cache; profiles/%s)" % cand)
-                break
-            except Exception:
-                continue
-        roofline = roofline_from_profile(prof, prof_steps, peaks, peak_src, value, fpt, world, traffic)
-        roofline["traffic_note"] = traffic_note
+        roofline = roofline_from_profile(prof, prof_steps, peaks, peak_src, value, fpt, world, None)
         line = {
             "metric": METRIC, "value": value, "unit": "tasks/s", "n_gpus": world, "steps": K, "warmup": W,
             "ms_per_step": total_ms / K, "higher_is_better": True, "scaling": cli.scaling, "vs_baseline": None,
@@ -573,7 +598,7 @@ def main():
         }
         if not cli.no_cpu_baseline and world == 1:
             # the reference's own GPU path (it self-selects CUDA, few_shot_learning_system.py:73-81): the library-kernel
-            # baseline on the same B200; then its CPU path on the host cores (bounded sample)
+            # baseline on the same GPU; then its CPU path on the host cores (bounded sample)
             g = run_unmodified_reference(cli.config, B, "cuda", steps=3, warmup=2, local_rank=local_rank)
             if "unavailable" in g:
                 try:
@@ -584,7 +609,7 @@ def main():
             else:
                 line["torch_gpu_baseline"] = {
                     "value": g["tasks_per_sec"], "unit": "tasks/s", "ms_per_step": g["ms_per_iter"],
-                    "kind": "reference (unmodified, baseline/_ref) on its own GPU path: eager PyTorch cuDNN / ATen, fp32, TF32 off",
+                    "kind": "reference (unmodified, oracle/_ref) on its own GPU path: eager PyTorch cuDNN / ATen, fp32, TF32 off",
                     "sample": "%d timed iterations of %d tasks (median), %d warm-up" % (len(g["times_s"]), g["batch_size"], g["warmup"]),
                     "gpu": g.get("gpu")}
             line["cpu_baseline"], _ = reference_cpu_baseline(cli, args, steps=8, warmup=2)

@@ -1,4 +1,4 @@
-"""B200-native MAML / MAML++ inner-loop engine behind the reference's Python surface.
+"""H100-native MAML / MAML++ inner-loop engine behind the reference's Python surface.
 
 Public surface (same names as the reference repo's modules):
   few_shot_learning_system.MAMLFewShotClassifier      -- B0: run_train_iter / run_validation_iter

@@ -144,7 +144,7 @@ class Engine(object):
                  per_step_bn, max_tasks, keep_target_passes=False, force_fp32_convs=False):
         import torch
         if not torch.cuda.is_available():
-            raise NativeLibraryError("the MAML engine needs a CUDA (sm_100a) device; there is no CPU fallback")
+            raise NativeLibraryError("the MAML engine needs a CUDA (sm_90a) device; there is no CPU fallback")
         self.lib = load_library()
         self.cfg = Config(n_way=n_way, k_shot=k_shot, t_target=t_target, channels=channels, height=height, width=width,
                           filters=filters, num_stages=num_stages, inner_steps=inner_steps,

@@ -47,7 +47,7 @@ CONFIGS = {
     # configs[0]: Omniglot MAML 5-way 1-shot, meta-batch 8 (the reference's CPU-runnable case)
     "omniglot_maml_5w1s": _mk(_OMNIGLOT, _MAML, batch_size=8, num_classes_per_set=5,
                               num_samples_per_class=1, experiment_name="omniglot_maml_5w1s"),
-    # configs[1]: Omniglot MAML++ 5-way 1-shot, meta-batch 8, 1xB200 (the headline workload)
+    # configs[1]: Omniglot MAML++ 5-way 1-shot, meta-batch 8, one GPU (the headline workload)
     "omniglot_mamlpp_5w1s": _mk(_OMNIGLOT, _MAML_PP, batch_size=8, num_classes_per_set=5,
                                 num_samples_per_class=1, experiment_name="omniglot_mamlpp_5w1s"),
     # configs[2]: Mini-ImageNet MAML++ 5-way 1-shot, 48 filters, meta-batch 2

@@ -1,4 +1,4 @@
-// Shared declarations for the B200 MAML engine (sm_100a only).
+// Shared declarations for the MAML engine (sm_90a: H100).
 //
 // Activation layout ("padded pixel grid"): every activation-like tensor of block l lives as a
 // row-major matrix [n * G_l, C] with G_l = (h_l + 1) * (w_l + 1) (zero padding shared between neighbours): one row per position of the
@@ -83,6 +83,8 @@ struct WgradArgs {
   FusedReduce fr;
   const float* A[2]; long long a_stride[2];    // conv inputs (guarded matrices) [rows][kc]
   const float* D[2]; long long d_stride[2];    // output gradients (zero-border matrices) [rows][ncols]
+  long long a_plane[2], d_plane[2];            // tensor-core path: distance (floats) from the fp32 plane to its TF32 hi plane
+                                               // (the lo plane follows at the same distance)
   int nsrc;
   int kc, ncols, rows, gw;
   int rows_per_chunk, nchunks;
@@ -297,8 +299,8 @@ enum { PASS_SUP_FWD = 0, PASS_SUP_BWD = 1, PASS_TGT_FWD = 2, PASS_TGT_BWD = 3, P
 // Programmatic dependent launch: every kernel is launched with the programmatic-stream-serialization attribute and
 // starts with `griddepcontrol.launch_dependents; griddepcontrol.wait;` -- the next kernel of the stream is scheduled
 // while this one still runs (its launch latency and set-up overlap) and blocks until this grid has completed and
-// flushed.  Measured on B200 inside the captured CUDA graph: no gain (4.16 ms vs 4.02 ms per iteration) -- the kernels'
-// own durations, not the launch gaps, set the critical path -- so the attribute is OFF unless MAML_B200_PDL=1.
+// flushed.  Inside the captured CUDA graph the kernels' own durations, not the launch gaps, set the critical path, so
+// the attribute is OFF unless MAML_B200_PDL=1.
 // ---------------------------------------------------------------------------------------------
 extern int g_use_pdl;               // 0: off, 1: every launch, 2: only launches on the iteration's main chain (g_pdl_main_stream),
                                     // 3: every stream except the weight-gradient side stream (g_pdl_wg_stream)
@@ -308,15 +310,14 @@ inline bool pdl_allowed(cudaStream_t st) {
   return g_use_pdl == 1 || (g_use_pdl == 2 && st == g_pdl_main_stream) || (g_use_pdl == 3 && st != g_pdl_wg_stream);
 }
 extern int g_launch_prio;
+int num_sms();                     // streaming multiprocessors of the current device (queried once)
 
 // Device-side launch trace (debug; maml_b200_trace): CTA (0,0,0) of every kernel appends (globaltimer ns << 8 | kernel
 // id) to a buffer -> the start-time sequence of one captured iteration, the only timeline available without nsys.
 // One pointer copy per translation unit (no relocatable device code), all set to the same buffer; null = off.
 // The trace is armed through a bit of the launch tag, i.e. a kernel ARGUMENT: with tracing off no kernel touches memory for
 // it.  Before, every thread of every kernel began with a load of the buffer pointer (a __device__ variable) and a branch on
-// it -- a dependent global load in front of the first useful instruction: 2.663 -> 2.586 ms per iteration without it (same
-// box, scripts/build_variant.sh).  Moving the pointer to __constant__ memory + reading it from one thread only was SLOWER
-// (2.683 ms).  Enabling the trace drops the handle's cached CUDA graphs so that they are re-captured with armed tags.
+// it -- a dependent global load in front of the first useful instruction.  Enabling the trace drops the handle's cached CUDA graphs so that they are re-captured with armed tags.
 #define MAML_TRACE_ARMED 0x40000000
 static __device__ unsigned long long* t_trace_buf = nullptr;
 #define MAML_TRACE_SETTER(fn) void fn(unsigned long long* p) { cudaMemcpyToSymbol(t_trace_buf, &p, sizeof(p)); }
@@ -337,7 +338,6 @@ void trace_set_bn(unsigned long long* p);
 void trace_set_head(unsigned long long* p);
 void trace_set_param(unsigned long long* p);
 void trace_set_tc(unsigned long long* p);
-void trace_set_wgtc(unsigned long long* p);
 
 __device__ __forceinline__ void pdl_prologue(int kid = 0, int tag = 0) {
   trace_mark(kid, tag);

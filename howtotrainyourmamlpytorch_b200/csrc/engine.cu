@@ -1,4 +1,4 @@
-// Host-side orchestration + C ABI (include/maml_b200.h) of the B200 MAML / MAML++ engine.
+// Host-side orchestration + C ABI (include/maml_b200.h) of the H100 MAML / MAML++ engine.
 //
 // One call of maml_b200_meta_batch_fwd_bwd replaces, for the local shard of tasks, the reference's
 //   forward()   few_shot_learning_system.py:170-263  (task loop x inner-step loop, Python, autograd)
@@ -59,20 +59,17 @@ struct PassSet {            // activation buffers of one kind of pass (support: 
   float* dz[MAML_MAX_LAYERS] = {}; long long dz_sz[MAML_MAX_LAYERS] = {};
   float* dp[MAML_MAX_LAYERS] = {}; long long dp_sz[MAML_MAX_LAYERS] = {};
   // conv inputs of blocks l >= 1 (ain) and output gradients (dz) are stored as three planes: fp32, TF32-hi, TF32-lo
-  // (the hi/lo planes feed the tcgen05 kernels through TMA; same geometry incl. guards)
+  // (the hi/lo planes feed the wgmma conv kernel through TMA; same geometry incl. guards)
   float* ain_base[MAML_MAX_LAYERS + 1] = {}; long long ain_plane[MAML_MAX_LAYERS + 1] = {};
   float* dz_base[MAML_MAX_LAYERS] = {}; long long dz_plane[MAML_MAX_LAYERS] = {};
   CUtensorMap ain_map[MAML_MAX_LAYERS][2];   // [layer][hi/lo]
   CUtensorMap dz_map[MAML_MAX_LAYERS][2];
-  // the same planes seen by the tcgen05 weight-gradient kernel (MN-major operands: swizzle 128B_ATOM_32B, other boxes)
-  CUtensorMap ain_wg_map[MAML_MAX_LAYERS][2];
-  CUtensorMap dz_wg_map[MAML_MAX_LAYERS][2];
 };
 
 struct ChunkPlan { int rows_per_chunk[MAML_MAX_LAYERS]; int nchunks[MAML_MAX_LAYERS]; PartialDesc pd; long long size; int head_groups; };
 // rows of a batch one head CTA handles: small batches (<= 16 rows: the Omniglot 5-way passes) stay in ONE CTA so that the
 // last block / head / BatchNorm-backward fusion applies; larger ones are cut into groups of 4 rows -- the head of a 75-row
-// Mini-ImageNet target pass ran as 5 CTAs per task (latency-bound, 1.0 -> 0.55 ms per iteration with 19)
+// Mini-ImageNet target pass would otherwise run as 5 latency-bound CTAs per task
 static inline int head_rows(int n) {
   static const int forced = getenv("MAML_B200_HEAD_ROWS") ? atoi(getenv("MAML_B200_HEAD_ROWS")) : 0;
   if (forced > 0) return forced;
@@ -99,7 +96,7 @@ struct maml_b200_handle {
   long long* zero_labels = nullptr;   // [max(n_s, n_t)] zeros (label-free forward)
   unsigned* wg0_counters = nullptr;   // [maxT] arrival counters of the fused first-block reduction (self-resetting)
   bool fuse_wg0_reduce = false;       // env MAML_B200_WG0_FUSE=1: first-block parameter reduction fused into wgrad0 (last CTA of a
-                                      // task); measured slower than the separate launch (2.817 vs 2.788 ms), so off by default
+                                      // task); off by default
   float* pinned = nullptr;            // host staging ring for small per-call scalars (16 slots x 32 floats)
   int pin_slot = 0;
   long long last_launches = 0;
@@ -115,7 +112,7 @@ struct maml_b200_handle {
   bool use_graphs = true;
   cudaStream_t main_stream = nullptr;                 // stream of the iteration's main chain while it is being enqueued
   int pdl_mode = 0, pdl_cluster = 0;                  // programmatic dependent launch (see common.cuh), chosen per handle
-  int nb_main = 8, wg_nstage = 4;                     // shared-memory ring depths of the tcgen05 conv / weight-gradient kernels (see maml_b200_create)
+  int nb_main = 8;                                    // shared-memory B ring depth of the tensor-core conv kernel (see maml_b200_create)
   int nb_side = 0;                                    // env MAML_B200_TC_NB_SIDE: B ring depth cap of side-stream convs (0 = the global cap)
   int side_bn_cap = 0;                                // env MAML_B200_BN_SIDE_CAP: CTA cap of grid-stride BatchNorm launches on side streams
   int split_cap_side = 0, split_cap_l1 = 0;           // env MAML_B200_TC_SPLIT_SIDE / _L1: split-K caps (0 = none) for side-stream convs / main-chain block 1
@@ -127,9 +124,7 @@ struct maml_b200_handle {
   unsigned long long graph_clock = 0;
   // tensor-core path (blocks l >= 1 when F % 32 == 0)
   bool use_tc = false;
-  bool wgrad_tc = true;    // tcgen05 weight gradient for blocks l >= 1 (env MAML_B200_WGRAD_TC=0: the FFMA filter-row kernel)
-  int tc_stack = 1;        // N-stacked 3xTF32 MMAs (env MAML_B200_TC_STACK=0: three MMAs per k-step)
-  int tc_bo_mode = 0;      // 0: row-shifted UMMA descriptors keep base_offset = 0 (correct on B200); 1: experiment (env MAML_B200_TC_BO)
+  bool wgrad_tc = true;    // wgmma weight gradient for blocks l >= 1 (env MAML_B200_WGRAD_TC=0: the FFMA filter-row kernel)
   float *pack_theta = nullptr, *pack_u = nullptr;       // [4 planes][steps][T][(L-1)*9*F*F]
   long long pack_theta_plane = 0, pack_u_plane = 0, pack_task = 0;
   CUtensorMap theta_map[4], u_map[4];                   // planes: W hi, W lo, WT hi, WT lo
@@ -139,6 +134,15 @@ struct maml_b200_handle {
   void* comm_opened[MAML_MAX_RANKS] = {};               // peer blocks mapped with cudaIpcOpenMemHandle
   bool comm_connected = false;
 };
+
+int num_sms() {
+  static int n = 0;
+  if (n == 0) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+  }
+  return n;
+}
 
 extern "C" int maml_b200_abi_version(void) { return MAML_B200_ABI_VERSION; }
 extern "C" const char* maml_b200_last_error(void) { return g_err.c_str(); }
@@ -205,22 +209,14 @@ static void plan_chunks(maml_b200_handle* h, int n, ChunkPlan* cp) {
     } else {
       // ONE wgrad CTA per SM (wgrad_row_kernel<4,4>: 105 registers x 256 threads; its 48 independent accumulators per thread keep
       // the FMA pipe fed with 8 warps): a second CTA per SM would take the register file away from the main chain's kernels
-      // running beside it (measured 3.057 -> 3.038 ms per iteration); 3 filter rows x tasks x
-      // chunks should just fill 148 x 4 slots -- 720 CTAs (128-row chunks at 8 tasks) ran as 1.2 waves = 2x the time
-      static const int wg_slots = getenv("MAML_B200_WG_SLOTS") ? atoi(getenv("MAML_B200_WG_SLOTS")) : 148;
+      // running beside it; 3 filter rows x tasks x
+      // chunks should just fill one slot per SM -- 720 CTAs (128-row chunks at 8 tasks) ran as 1.2 waves = 2x the time
+      static const int wg_slots = getenv("MAML_B200_WG_SLOTS") ? atoi(getenv("MAML_B200_WG_SLOTS")) : num_sms();
       static const int wg_per_chunk = (getenv("MAML_B200_WGRAD_ROW") && atoi(getenv("MAML_B200_WGRAD_ROW")) == 0) ? 9 : 3;
       long long want = std::max<long long>(1, wg_slots / ((long long)wg_per_chunk * h->maxT));
       nch = (int)std::min<long long>(std::min<long long>(64, want), std::max<long long>(1, (rows + 15) / 16));
-      if (h->use_tc && h->wgrad_tc) {
-        // tcgen05 weight gradient: 3 CTAs (filter rows) per chunk, stages of 32 rows, accumulators drained every 64 rows
-        // (so chunk length is a scheduling choice only): one wave of CTAs, chunks of at least 64 rows to amortise a
-        // CTA's fixed cost, at most 64 chunks per task.
-        long long r = rup((rows + want - 1) / want, 32);
-        r = std::max<long long>(64, r);
-        nch = (int)std::min<long long>(64, (rows + r - 1) / r);
-      }
     }
-    rpc = (int)rup((rows + nch - 1) / nch, (l > 0 && h->use_tc && h->wgrad_tc) ? 32 : 16);
+    rpc = (int)rup((rows + nch - 1) / nch, 16);
     nch = (int)((rows + rpc - 1) / rpc);
     cp->rows_per_chunk[l] = rpc; cp->nchunks[l] = nch;
     const long long cs = 9LL * h->geo[l].cin * h->F + h->F;
@@ -279,10 +275,6 @@ static int make_pass_maps(maml_b200_handle* h, PassSet& ps, bool has_dz) {
       const int rp = tc_conv_rpad(h->geo[l].gw);       // one TMA box = the 128-row tile plus its halo
       if (make_map(&ps.ain_map[l][pl], ps.ain_base[l] + (pl + 1) * ps.ain_plane[l], ps.ain_plane[l] / h->F, h->F, rp)) return 1;
       if (has_dz && make_map(&ps.dz_map[l][pl], ps.dz_base[l] + (pl + 1) * ps.dz_plane[l], ps.dz_plane[l] / h->F, h->F, rp)) return 1;
-      if (make_map(&ps.ain_wg_map[l][pl], ps.ain_base[l] + (pl + 1) * ps.ain_plane[l], ps.ain_plane[l] / h->F, h->F, 40,
-                   CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)) return 1;
-      if (has_dz && make_map(&ps.dz_wg_map[l][pl], ps.dz_base[l] + (pl + 1) * ps.dz_plane[l], ps.dz_plane[l] / h->F, h->F, 32,
-                             CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)) return 1;
     }
   }
   return 0;
@@ -294,8 +286,7 @@ static int make_all_maps(maml_b200_handle* h) {
     if (make_map(&h->theta_map[pl], h->pack_theta + pl * h->pack_theta_plane, h->pack_theta_plane / h->F, h->F, h->F)) return 1;
     if (make_map(&h->u_map[pl], h->pack_u + pl * h->pack_u_plane, h->pack_u_plane / h->F, h->F, h->F)) return 1;
   }
-  if (tc_conv_prepare()) return fail("cudaFuncSetAttribute(max dynamic shared memory) failed for the tcgen05 conv kernel");
-  if (wgrad_tc_prepare()) return fail("cudaFuncSetAttribute(max dynamic shared memory) failed for the tcgen05 wgrad kernel");
+  if (tc_conv_prepare()) return fail("cudaFuncSetAttribute(max dynamic shared memory) failed for the wgmma conv kernel");
   return 0;
 }
 
@@ -390,10 +381,8 @@ extern "C" int maml_b200_create(const maml_b200_config* cfg, maml_b200_handle** 
   h->C = cfg->channels; h->H = cfg->height; h->W = cfg->width; h->n_s = n_s; h->n_t = n_t; h->maxT = cfg->max_tasks;
   build_geometry(h);
   build_layout(h);
-  // tensor-core (tcgen05 / TMA, 3xTF32) convolutions for blocks l >= 1; reserved bit 1 forces the fp32 FFMA kernels (tests)
+  // tensor-core (wgmma / TMA, 3xTF32) convolutions for blocks l >= 1; reserved bit 1 forces the fp32 FFMA kernels (tests)
   h->use_tc = (h->L > 1) && !(cfg->reserved & 2);
-  if (const char* bo = getenv("MAML_B200_TC_BO")) h->tc_bo_mode = atoi(bo);
-  if (const char* sk = getenv("MAML_B200_TC_STACK")) h->tc_stack = atoi(sk) != 0;
   if (const char* wt = getenv("MAML_B200_WGRAD_TC")) h->wgrad_tc = atoi(wt) != 0;
   if (const char* sp = getenv("MAML_B200_TC_SPLIT")) tc_conv_set_split(atoi(sp));
   tc_conv_set_zstage(getenv("MAML_B200_TC_ZSTAGE") ? atoi(getenv("MAML_B200_TC_ZSTAGE")) : 1);
@@ -429,27 +418,23 @@ extern "C" int maml_b200_create(const maml_b200_config* cfg, maml_b200_handle** 
   h->use_graphs = !(cfg->reserved & 4) && !getenv("MAML_B200_NO_GRAPH");
   // Two regimes, told apart by whether one iteration's block-1 tiles (support + target, all tasks) fit one wave of SMs.
   //  * latency-bound (Omniglot 5-way at 8 tasks: 144 tiles): programmatic dependent launch on the MAIN chain only (the next
-  //    kernel of the support / tangent chain is scheduled while the current one drains, ~1 us per link: 2.742 -> 2.671 ms;
-  //    on every stream 2.89 ms, with cluster launches included 2.91 ms -- early-launched CTAs hold the SM slots the other
-  //    streams want), deep shared-memory rings (all B stages of a short pipeline prefetched at once; ring = 3 / 4: 2.82 ms;
-  //    a ring cut to the stages one CTA has in flight, which lets other kernels share the SM: 2.69 -> 2.73 ms).
-  //  * throughput-bound (Mini-ImageNet, 20-way): no PDL (11.75 -> 11.97 ms, 19.66 -> 19.89 ms), shallow rings (conv ring 4 +
-  //    wgrad ring 2: 19.73 -> 19.10 ms, 11.79 -> 11.58 ms -- the shared memory they give up lets the BatchNorm / first-block
-  //    kernels of the other streams share the SM).
-  // All numbers: profiles/ab_contention_r2.txt (scripts/ab_inproc.py).
+  //    kernel of the support / tangent chain is scheduled while the current one drains; on every stream, early-launched
+  //    CTAs hold the SM slots the other streams want), deep shared-memory rings (all B stages of a short pipeline
+  //    prefetched at once).
+  //  * throughput-bound (Mini-ImageNet, 20-way): no PDL, conv ring 4 (the shared memory it gives up lets the BatchNorm /
+  //    first-block kernels of the other streams share the SM).
   {
     const int l1 = h->L > 1 ? 1 : 0;
     const long long tiles = (((long long)h->n_s * h->geo[l1].G + 127) / 128 + ((long long)h->n_t * h->geo[l1].G + 127) / 128) * h->maxT;
-    const bool small = tiles <= 160;
+    const bool small = tiles <= num_sms();
     h->pdl_mode = getenv("MAML_B200_PDL") ? atoi(getenv("MAML_B200_PDL")) : (small ? 2 : 0);
     h->pdl_cluster = getenv("MAML_B200_PDL_CLUSTER") ? atoi(getenv("MAML_B200_PDL_CLUSTER")) : 0;
     h->nb_main = getenv("MAML_B200_TC_NB") ? std::max(2, std::min(8, atoi(getenv("MAML_B200_TC_NB")))) : (small ? 8 : 4);
-    h->wg_nstage = getenv("MAML_B200_WG_NSTAGE") ? std::max(2, std::min(4, atoi(getenv("MAML_B200_WG_NSTAGE")))) : (small ? 4 : 2);
     g_use_pdl = h->pdl_mode; g_pdl_cluster = h->pdl_cluster;
   }
   // Priorities: the support chain (capture stream) is the critical path; the weight-gradient and target streams only
   // have to finish by the end of a step.  Their many small CTAs would otherwise occupy every SM and keep the
-  // whole-SM tcgen05 conv CTAs of the critical path waiting (measured: ~20 us per step).
+  // whole-SM tensor-core conv CTAs of the critical path waiting.
   int prio_lo = 0, prio_hi = 0;
   cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);      // lo = numerically largest = least urgent
   const bool use_prio = getenv("MAML_B200_NO_PRIO") == nullptr;
@@ -624,9 +609,8 @@ static void tc_conv(maml_b200_handle* h, int l, int n, int nsrc, const TcOp* ops
   TcMaps maps;
   TcConvArgs a{};
   a.nsrc = nsrc; a.kc = h->F; a.rows = n * g.G; a.gw = g.gw; a.G = g.G; a.h = g.h; a.w = g.w; a.ncols = h->F; a.mode = mode; a.tasks = T; a.plan_tasks = h->maxT;
-  a.stack = h->tc_stack;
   a.split_cap = (h->main_stream && st != h->main_stream) ? h->split_cap_side : (l == 1 ? h->split_cap_l1 : 0);
-  a.halo = g.gw + 1; a.rpad = tc_conv_rpad(g.gw); a.nb = std::min(tc_conv_ring(h->F, g.gw), h->nb_main); if (h->nb_side >= 2 && h->main_stream && st != h->main_stream && a.nb > h->nb_side) a.nb = h->nb_side; a.bo_mode = h->tc_bo_mode; { const char* tl = getenv("MAML_B200_TC_TIMELINE"); a.timeline = (tl && (atoi(tl) <= 0 || atoi(tl) == l)) ? 1 : 0; }
+  a.halo = g.gw + 1; a.rpad = tc_conv_rpad(g.gw); a.nb = std::min(tc_conv_ring(h->F, g.gw), h->nb_main); if (h->nb_side >= 2 && h->main_stream && st != h->main_stream && a.nb > h->nb_side) a.nb = h->nb_side; { const char* tl = getenv("MAML_B200_TC_TIMELINE"); a.timeline = (tl && (atoi(tl) <= 0 || atoi(tl) == l)) ? 1 : 0; }
   for (int s = 0; s < nsrc; ++s) {
     maps.m[s * 4 + 0] = ops[s].a_maps[0]; maps.m[s * 4 + 1] = ops[s].a_maps[1];
     maps.m[s * 4 + 2] = ops[s].b_maps[ops[s].b_pair]; maps.m[s * 4 + 3] = ops[s].b_maps[ops[s].b_pair + 1];
@@ -638,30 +622,6 @@ static void tc_conv(maml_b200_handle* h, int l, int n, int nsrc, const TcOp* ops
   a.zh = zh; a.zh_stride = zh_stride; a.stats = stats; a.stats_stride = h->stats_task_stride;
   a.alg_flops = conv_flops(h, l, n, T, nsrc);
   launch_conv_tc(maps, a, st);
-}
-
-// tcgen05 weight gradient of block l >= 1: sum over sources of A(ain of a_ps/a_slot)^T-shifted x D(dz of d_ps/d_slot)
-struct WgSrc { const PassSet* a_ps; int a_slot; const PassSet* d_ps; int d_slot; };
-static void tc_wgrad(maml_b200_handle* h, int l, int n, int nsrc, const WgSrc* src, float* partial, const ChunkPlan& cp, int T,
-                     cudaStream_t st) {
-  const LayerGeom& g = h->geo[l];
-  TcMaps maps;
-  WgTcArgs a{};
-  a.nsrc = nsrc; a.kc = h->F; a.ncols = h->F; a.rows = n * g.G; a.gw = g.gw;
-  a.rows_per_chunk = cp.rows_per_chunk[l]; a.nchunks = cp.nchunks[l];
-  { static const int lite = getenv("MAML_B200_WGRAD_LITE") ? atoi(getenv("MAML_B200_WGRAD_LITE")) : 1; a.force_flush = lite ? 0 : 1; }
-  for (int s = 0; s < nsrc; ++s) {
-    const PassSet& ap = *src[s].a_ps; const PassSet& dp = *src[s].d_ps;
-    maps.m[s * 4 + 0] = ap.ain_wg_map[l][0]; maps.m[s * 4 + 1] = ap.ain_wg_map[l][1];
-    maps.m[s * 4 + 2] = dp.dz_wg_map[l][0]; maps.m[s * 4 + 3] = dp.dz_wg_map[l][1];
-    a.a_row_base[s] = a_row_base_of(h, ap.ain_sz[l], l, src[s].a_slot); a.a_task_rows[s] = (int)(ap.ain_sz[l] * ap.slots / h->F);
-    a.b_row_base[s] = a_row_base_of(h, dp.dz_sz[l], l, src[s].d_slot); a.b_task_rows[s] = (int)(dp.dz_sz[l] * dp.slots / h->F);
-  }
-  if (nsrc == 1) for (int k = 4; k < 8; ++k) maps.m[k] = maps.m[k - 4];
-  a.partial = partial + cp.pd.off[2 * l]; a.partial_task_stride = cp.pd.task_stride; a.chunk_stride = cp.pd.cstride[2 * l];
-  a.tasks = T; a.nstage = h->wg_nstage;
-  a.alg_flops = conv_flops(h, l, n, T, nsrc);
-  launch_wgrad_tc(maps, a, st);
 }
 
 // primal forward of one pass: conv -> stats -> BN/leaky/pool for every block
@@ -770,8 +730,8 @@ static void backward_pass(maml_b200_handle* h, const PassSet& ps, int slot, cons
         launch_conv_rows(a, st);
       }
       if (h->use_tc && h->wgrad_tc) {
-        WgSrc ws{&ps, slot, &ps, slot};
-        tc_wgrad(h, l, ps.n, 1, &ws, partial, cp, T, wst);
+        w.a_plane[0] = ps.ain_plane[l]; w.d_plane[0] = ps.dz_plane[l];
+        launch_wgrad_tc(w, wst);
       } else {
         launch_wgrad(w, wst);
       }
@@ -939,8 +899,9 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
         launch_conv_rows(a, st);
       }
       if (h->use_tc && h->wgrad_tc) {
-        WgSrc ws[2] = {{&sp, s, &tn, 0}, {&tn, 0, &sp, s}};        // (a_in, dz_dot) + (a_in_dot, dz)
-        tc_wgrad(h, l, sp.n, 2, ws, h->sup_partial, cp, T, h->s_wg);
+        w.a_plane[0] = sp.ain_plane[l]; w.d_plane[0] = tn.dz_plane[l];
+        w.a_plane[1] = tn.ain_plane[l]; w.d_plane[1] = sp.dz_plane[l];
+        launch_wgrad_tc(w, h->s_wg);
       } else {
         launch_wgrad(w, h->s_wg);
       }
@@ -989,7 +950,7 @@ static int enqueue_iteration(maml_b200_handle* h, const maml_b200_iter_args* it,
   launch_prep_x(x_support, h->sup.xg, h->sup.xg_stride, T, h->n_s, h->C, h->H, h->W, st);
   launch_import_theta(h->pl, meta, h->theta, h->Ppad, T, st);
   // The target images and the tensor-core packs of theta^0 are first needed after block 0 of the first support pass: both
-  // go to the side stream (15 us off the head of the main chain).  Every consumer already waits for ev_wg: the main chain
+  // go to the side stream (off the head of the main chain).  Every consumer already waits for ev_wg: the main chain
   // through join_pending before block 1, the target streams before each pass.
   CK(cudaEventRecord(h->ev_fork, st));
   CK(cudaStreamWaitEvent(h->s_wg, h->ev_fork, 0));
@@ -1425,7 +1386,7 @@ extern "C" int maml_b200_profile_read(maml_b200_handle* h, double* ms_by_cat, do
 // device-side launch trace (common.cuh: trace_mark): start timestamps of every kernel of the following calls
 static unsigned long long* g_trace_dev = nullptr;
 static void trace_set_all(unsigned long long* p) {
-  trace_set_conv(p); trace_set_bn(p); trace_set_head(p); trace_set_param(p); trace_set_tc(p); trace_set_wgtc(p);
+  trace_set_conv(p); trace_set_bn(p); trace_set_head(p); trace_set_param(p); trace_set_tc(p);
 }
 extern "C" int maml_b200_trace(maml_b200_handle* h, int32_t enable) {
   if (!h) return fail("null argument");

@@ -16,8 +16,8 @@ __device__ __forceinline__ float warp_sum(float v) {
 // chunks in order.  `smh`: 5 * rows_per_cta * N floats of shared memory; 256 threads.  Also called by the fused
 // last-block kernels (kernels_bn.cu).
 // COMPACT = true: every loop stays rolled.  The fused last-block kernels and the small-D heads (Omniglot: D = 64) execute this
-// code ONCE per launch and were measured instruction-fetch bound (34 % of the stall samples, ncu); rolled loops cut their SASS
-// from ~6.2 k to ~3.8 k instructions (headline 2.767 -> 2.755 ms).  Large-D heads (Mini-ImageNet: D = 1200) keep the
+// code ONCE per launch and are instruction-fetch bound; rolled loops cut their SASS
+// from ~6.2 k to ~3.8 k instructions.  Large-D heads (Mini-ImageNet: D = 1200) keep the
 // compiler's unrolling: rolled, their D-loops ran 2x slower.
 #define HEAD_LOOP _Pragma("unroll 1")
 #define HEAD_BODY_NAME head_body_compact

@@ -119,7 +119,7 @@ static inline dim3 bn_grid(const BnGeom& g, int tasks, int* block) {
   *block = wpb * F4;
   const int NW = g.n * ((g.h + 1) / 2) * ((g.w + 1) / 2);
   int bx = (NW + wpb - 1) / wpb;
-  if (bx > 592) bx = 592;
+  if (bx > 4 * num_sms()) bx = 4 * num_sms();
   if (g_bn_cta_cap > 0 && (long long)bx * tasks > g_bn_cta_cap) bx = g_bn_cta_cap / tasks;
   if (bx < 1) bx = 1;
   return dim3(bx, tasks);
@@ -279,7 +279,7 @@ __global__ void __launch_bounds__(256) bnbwd_reduce_kernel(BnBwdArgs a) {
 void launch_bnbwd_reduce(const BnBwdArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
   int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
-  if (grid.x > 148) grid.x = 148;
+  if ((int)grid.x > num_sms()) grid.x = num_sms();
   launch_pdl(bnbwd_reduce_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();
 }
@@ -547,7 +547,7 @@ __global__ void __launch_bounds__(256) bnbwd_tan_reduce_kernel(BnBwdTanArgs a) {
 void launch_bnbwd_tan_reduce(const BnBwdTanArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
   int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
-  if (grid.x > 148) grid.x = 148;
+  if ((int)grid.x > num_sms()) grid.x = num_sms();
   launch_pdl(bnbwd_tan_reduce_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();
 }
@@ -670,7 +670,7 @@ void launch_bnbwd_tan(const BnBwdTanArgs& a, cudaStream_t st) {
 // BatchNorm/activation/pool, the classifier head (logits, loss gradient, weight-gradient chunk, feature gradient) and
 // the BatchNorm backward of the same block are ONE kernel with one CTA per task: the three stages exchange their data
 // through global memory written and re-read by the same CTA (visible after __syncthreads), the backward sums need no
-// cluster.  Replaces three dependent launches (5 + 7 + 7 us) on the critical path of every support / tangent pass.
+// cluster.  Replaces three dependent launches on the critical path of every support / tangent pass.
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) tail_fused_kernel(BnActArgs fa, HeadArgs ha, BnBwdArgs ba) {
   pdl_prologue(23, fa.tag);

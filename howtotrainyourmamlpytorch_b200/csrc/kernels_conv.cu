@@ -5,7 +5,7 @@
 // (convolution_backward / double backward) -- see SURVEY.md appendix A1-A3.
 //
 // These kernels are the exact-fp32 path: used for the first block (K = 9*C_in is 9 or 27) and
-// for shapes the tcgen05 3xTF32 kernels (kernels_tc.cu) do not cover.
+// for shapes the wgmma 3xTF32 kernel (kernels_tc.cu) does not cover.
 #include <algorithm>
 #include "common.cuh"
 
@@ -394,7 +394,7 @@ static bool launch_conv0_rb(const Conv0Args& a, cudaStream_t st) {
   // tiles per CTA: as many as keep >= ~3 CTAs per SM in flight (fixed per-CTA cost -- weights, window, fp64 statistics
   // reduction -- is then paid once per `tiles` x 128 rows); 1 for the small launches that sit on the latency-critical chain
   const long long t128 = (a.rows + 127) / 128;
-  int tiles = (int)std::min<long long>(8, std::max<long long>(1, t128 * a.tasks / (3 * 148)));
+  int tiles = (int)std::min<long long>(8, std::max<long long>(1, t128 * a.tasks / (3LL * num_sms())));
   dim3 grid((unsigned)((t128 + tiles - 1) / tiles), a.tasks);
   const size_t smem = (size_t)(9 * C0 * a.ncols + (128 * tiles + 2 * (a.gw + 1)) * C0) * sizeof(float);
   switch (a.ncols / 16) {

@@ -79,7 +79,6 @@ __global__ void param_reduce_kernel(ParamLayout pl, PartialDesc pd, const float*
   const float* p = partial + (long long)task * pd.task_stride + pd.off[seg] + (i - pl.seg_off[seg]);
   float s = 0.f;
   for (int c = 0; c < pd.nchunks[seg]; ++c) s += p[(long long)c * pd.cstride[seg]];   // fixed order: deterministic
-  // (issuing the loads of 8 chunks together was measured slower: param class 0.88 -> 0.93 ms on the headline, 2.0 -> 3.1 ms on Mini-ImageNet)
   const long long o = (long long)task * task_stride + i;
   if (mode == PR_UPDATE) {
     const float alpha = meta[pl.m_lslr + (long long)seg * (pl.S + 1) + step];
@@ -192,7 +191,7 @@ __device__ __forceinline__ void comm_signal_when_last(const CommDev& c, unsigned
 
 // __grid_constant__: the argument block (~0.9 KB, indexed dynamically by layer / segment) is read in place from the
 // constant bank.  By value -- and with the result pointer patched in the struct -- every thread first copied all of it to
-// its local-memory stack: 808 B x 278 k threads = 159 MB of DRAM writes per launch and 42 us (ncu, profiles/ncu_r2b_export.txt).
+// its local-memory stack: 808 B x 278 k threads = 159 MB of DRAM writes per launch.
 __global__ void export_kernel(const __grid_constant__ ExportArgs a) {
   pdl_prologue(18, a.tag);
   unsigned seq = 0;
@@ -210,7 +209,7 @@ __global__ void export_kernel(const __grid_constant__ ExportArgs a) {
 // blocks = range 2, one WARP per remaining entry of the result vector (BatchNorm beta / gamma, LSLR, loss, accuracy count,
 // running-stat partial sums): the lanes share the (task, step) terms of the entry and a fixed shuffle tree adds them
 // (fp64, deterministic).  Each of those entries is a sum of 8..80 scattered fp64 loads (+ a pow() per term for the
-// running statistics); as a sequential per-thread loop they were the tail of the kernel (export alone: 50 us).
+// running statistics); as a sequential per-thread loop they were the tail of the kernel.
 __device__ __forceinline__ long long export_range1_blocks(const ParamLayout& pl) { return (pl.P + 255) / 256; }
 __device__ __forceinline__ double warp_sum_f64(double v) {
 #pragma unroll

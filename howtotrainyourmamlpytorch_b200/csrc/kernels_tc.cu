@@ -1,4 +1,4 @@
-// tcgen05 / TMA implicit-GEMM 3x3 convolution for sm_100a, fp32-faithful via the 3xTF32 operand split.
+// wgmma / TMA implicit-GEMM 3x3 convolution for sm_90a, fp32-faithful via the 3xTF32 operand split.
 //
 //   out[j, n] = sum_src sum_tap sum_k A_src[j +/- s_tap, k] * B_src[tap][n][k]        (fp32 result)
 //
@@ -11,17 +11,16 @@
 //
 // Precision: single-pass TF32 is not acceptable for this path (SURVEY.md appendix C: 40-130 % meta-gradient
 // error).  Every operand x is pre-split by its producer kernel into hi = rna_tf32(x), lo = rna_tf32(x - hi);
-// the kernel accumulates A_hi*B_hi and (A_lo*B_hi + A_hi*B_lo) in SEPARATE fp32 TMEM accumulators.
+// the kernel accumulates A_hi*B_hi and (A_lo*B_hi + A_hi*B_lo) in SEPARATE fp32 register accumulators.
 // The tensor core's fp32 accumulation truncates when it aligns addends, so error grows with the number of
-// sequential accumulations into one accumulator (measured: one accumulator for all 216 MMAs of a 64-channel
-// layer gave ~5x the fp32-FFMA error).  The big term is therefore spread round-robin over 4 accumulators
-// (18 accumulations each instead of 216), the small terms get a fifth, and the epilogue adds the five with
-// IEEE fp32 adds.
+// sequential accumulations into one accumulator (one accumulator for all 216 MMAs of a 64-channel layer gave ~5x
+// the fp32-FFMA error).  The big term is therefore spread round-robin over 4 accumulators (18 accumulations each
+// instead of 216), the small terms get a fifth, and the epilogue adds the five with IEEE fp32 adds.
 //
-// CTA = one 128-row M tile x all N (<= 64) columns.  Warp roles: warp 0 / warp 6 = TMA producers for B / A (one thread each),
-// warp 1 = TMEM allocator + MMA issuer (one thread), warps 2..5 = epilogue (TMEM -> registers -> shared ->
-// coalesced global store, + bias, + fp64 BatchNorm statistics).  4-stage smem ring, mbarrier full/empty,
-// tcgen05.commit frees stages and publishes the accumulator.
+// CTA = one 128-row M tile x all N (<= 64) columns, 384 threads.  Warps 0..7 = two consumer warpgroups (rows 0..63 and
+// 64..127 of the tile: wgmma m64nNk8, accumulators in registers, 5 x N / 2 per thread), warps 8..11 = producer
+// warpgroup (one TMA thread; setmaxnreg moves its registers to the consumers).  Warps 0..3 then run the epilogue (+ bias, coalesced global store, fp64 BatchNorm statistics).  Shared-memory
+// B ring with mbarrier full/empty pairs; a stage is released once wgmma.wait_group shows its MMAs complete.
 #include <cuda.h>
 #include <map>
 #include <utility>
@@ -55,37 +54,81 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                ::"r"(dst), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tc_mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-               ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// accumulator registers stay live across asynchronous wgmma groups: keep the compiler from moving their uses
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_mma_tf32_acc(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-               ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc) : "memory");
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, sm_100):
+// K-major, SWIZZLE_128B shared-memory matrix descriptor (sm_90 wgmma):
 //   [0,14) start address >> 4 | [16,30) LBO >> 4 (unused: one swizzle atom along K) | [32,46) SBO >> 4 = 1024 B
-//   (8 rows x 128 B) | [46,48) version = 1 | [61,64) layout type = 2 (SWIZZLE_128B)
+//   (8 rows x 128 B) | [49,52) base offset = 0 | [62,64) layout type = 1 (SWIZZLE_128B)
 __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
+  d |= (uint64_t)1 << 16;
   d |= (uint64_t)((1024u >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-                 "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-               : "r"(taddr));
+// wgmma.mma_async m64nNk8 tf32 x tf32 -> f32, D += A * B (accumulators are zero-initialised by the caller)
+__device__ __forceinline__ void wgmma_tf32_n16(float (&d)[8], uint64_t adesc, uint64_t bdesc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+               : "l"(adesc), "l"(bdesc), "r"(1) : "memory");
 }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_tf32_n32(float (&d)[16], uint64_t adesc, uint64_t bdesc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+               : "l"(adesc), "l"(bdesc), "r"(1) : "memory");
+}
+__device__ __forceinline__ void wgmma_tf32_n48(float (&d)[24], uint64_t adesc, uint64_t bdesc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+               : "l"(adesc), "l"(bdesc), "r"(1) : "memory");
+}
+__device__ __forceinline__ void wgmma_tf32_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+               : "l"(adesc), "l"(bdesc), "r"(1) : "memory");
+}
+
+// the same with the A fragment in registers (m64k8 tf32 layout per warp: see wgrad_tc_kernel)
+__device__ __forceinline__ void wgmma_tf32_rs_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t bdesc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1) : "memory");
+}
+__device__ __forceinline__ void wgmma_tf32_rs_n32(float (&d)[16], const uint32_t (&a)[4], uint64_t bdesc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1) : "memory");
+}
+__device__ __forceinline__ void wgmma_tf32_rs_n48(float (&d)[24], const uint32_t (&a)[4], uint64_t bdesc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %29, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, {%24, %25, %26, %27}, %28, p, 1, 1;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1) : "memory");
+}
+__device__ __forceinline__ void wgmma_tf32_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1) : "memory");
+}
 
 // thread-block-cluster helpers (split-K over the CTAs of one cluster, reduction through distributed shared memory)
 __device__ __forceinline__ void cluster_sync_all() {
@@ -172,34 +215,41 @@ __device__ __forceinline__ void splitk_reduce_local(const float* __restrict__ re
   }
 }
 
-// K-major SWIZZLE_128B descriptor whose start is `row_off` rows into a 1024B-aligned tile.  Measured on B200: the
-// 128B swizzle XOR is a function of the ABSOLUTE shared-memory address bits [7,10) (as for TMA writes), so a start
-// address moved by row_off * 128 B addresses rows row_off .. row_off+127 of the tile correctly with the
-// matrix-base-offset field left at 0; setting base_offset = row_off mod 8 (bo_mode = 1) gives wrong results.
+// K-major SWIZZLE_128B descriptor whose start is `row_off` rows into a 1024B-aligned tile.  The 128B swizzle XOR is a
+// function of the ABSOLUTE shared-memory address bits [7,10) (as for TMA writes), so a start address moved by
+// row_off * 128 B addresses rows row_off .. row_off+63 of the tile correctly with the base-offset field left at 0.
 // This is what lets ONE halo tile serve all nine filter taps.
-// (the issuer below adds row_off * 128 B >> 4 to the descriptor's address field)
+// (the consumers add row_off * 128 B >> 4 to the descriptor's address field)
 
 // debug timeline (clock64 at pipeline milestones of CTA (0,0)); written only when TcConvArgs::timeline != 0
 __device__ long long g_tc_timeline[16];
 #define TC_MARK(i) do { if (a.timeline && blockIdx.x == 0 && blockIdx.y == 0) g_tc_timeline[i] = clock64(); } while (0)
 
 template <int NCOLS>
-__global__ void __launch_bounds__(224, 1) conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcConvArgs a) {
+__device__ __forceinline__ void wgmma_tf32(float (&d)[NCOLS / 2], uint64_t adesc, uint64_t bdesc) {
+  if constexpr (NCOLS == 16) wgmma_tf32_n16(d, adesc, bdesc);
+  else if constexpr (NCOLS == 32) wgmma_tf32_n32(d, adesc, bdesc);
+  else if constexpr (NCOLS == 48) wgmma_tf32_n48(d, adesc, bdesc);
+  else wgmma_tf32_n64(d, adesc, bdesc);
+}
+
+constexpr int TC_THREADS = 384;      // 2 consumer warpgroups + 1 producer warpgroup
+
+template <int NCOLS>
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcConvArgs a) {
   pdl_trigger();
   trace_mark(22, a.tag);
   constexpr int B_BYTES = NCOLS * 128;
   constexpr int BSTAGE = 2 * B_BYTES;            // B_hi + B_lo of one (tap, k-chunk)
-  // accumulators: plain mode 4 x hi*hi (round-robin over k-steps) + 1 x (lo*hi + hi*lo) = 5 * NCOLS columns;
-  // stacked mode 4 x [hi*hi | hi*lo + lo*hi] = 8 * NCOLS columns (see the MMA issuer)
-  constexpr int TMEM_COLS = NCOLS <= 16 ? 128 : (NCOLS <= 32 ? 256 : 512);   // power of two >= 8 * NCOLS
-  constexpr int PITCH = NCOLS + 1;
+  constexpr int P4 = NCOLS + 4;                  // pitch (floats) of every tile / buffer row: 16-byte aligned rows
+  constexpr int R = NCOLS / 2;                   // accumulator registers per thread of one m64nNk8 accumulator
   constexpr int MAXB = 8;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ uint64_t a_full[2], a_empty[2], b_full[MAXB], b_empty[MAXB], accum_bar;
-  __shared__ uint32_t tmem_base_s;
+  __shared__ uint64_t a_full[2], a_empty[2], b_full[MAXB], b_empty[MAXB];
   __shared__ int row_ok[128];
   __shared__ double sred[2][NCOLS][2];
+  __shared__ float s_bias[NCOLS];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int task = blockIdx.y;
@@ -212,55 +262,59 @@ __global__ void __launch_bounds__(224, 1) conv_tc_kernel(const __grid_constant__
   // nph * 9 (phase, tap) stages and the partial tiles are summed through distributed shared memory in the epilogue
   const int nsplit = (int)gridDim.z, zrank = (int)blockIdx.z;
   const int st_lo = zrank * (nph * 9) / nsplit, st_hi = (zrank + 1) * (nph * 9) / nsplit;
-  const int ph_lo = st_lo / 9, ph_hi = (st_hi - 1) / 9;
+  const int ph_lo = st_lo / 9;
   // push variant: a CTA writes into its peers' shared memory as soon as ITS accumulators are done, so every CTA of the
   // cluster must be known to have started by then: arrive here, wait right before the first remote store (free by then)
   if (nsplit > 1 && a.push) cluster_arrive_relaxed();
   const int abuf = a.rpad * 128;                 // bytes of one A halo buffer (hi or lo)
   uint8_t* bring = smem + 4 * (size_t)abuf;
+  float* zbuf = reinterpret_cast<float*>(bring + (size_t)nb * BSTAGE + ((nsplit > 1 && a.push) ? (size_t)128 * P4 * 4 : 0));
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < 2; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
-    for (int s = 0; s < nb; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 1); }
-    mbar_init(&accum_bar, 1);
+    for (int s = 0; s < 2; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 8); }
+    for (int s = 0; s < nb; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 8); }   // empty: one arrival per consumer warp
     fence_barrier_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"((uint32_t)TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+  if (threadIdx.x < 128) {
+    // epilogue row flags (interior pixel of the padded grid) and the bias
+    const int et = threadIdx.x;
+    const int row = j0 + et;
+    int ok = 0;
+    if (row < a.rows) {
+      const int rr = row % a.G;
+      const int yy = rr / a.gw, xx = rr - yy * a.gw;
+      ok = (yy >= 1 && yy <= a.h && xx >= 1 && xx <= a.w) ? 1 : 0;
+    }
+    row_ok[et] = ok;
+    if (et < NCOLS) s_bias[et] = a.bias ? a.bias[(long long)task * a.bias_stride + et] : 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
   pdl_wait();          // set-up above overlapped the previous kernel's tail; its results are needed from here on
   if (threadIdx.x == 0) TC_MARK(1);
 
-  if (warp == 6) {
-    if (lane == 0) {
-      // ===== TMA producer A: per phase (source, k-chunk) ONE halo tile of A (hi, lo); all 9 taps read it at row
-      // offsets.  Double-buffered, so phase ph+1 streams in while the MMAs of phase ph run.
-      for (int ph = ph_lo; ph <= ph_hi; ++ph) {
-        const int s = ph / kchunks;
-        const int kc0 = (ph - s * kchunks) << 5;
-        const int lp = ph - ph_lo;
-        const int ab = lp & 1;
-        mbar_wait(&a_empty[ab], (((uint32_t)lp >> 1) & 1u) ^ 1u);
-        const int arow = a.a_row_base[s] + task * a.a_task_rows[s] + j0 - a.halo;
-        const uint32_t ad = smem_u32(smem + (size_t)ab * 2 * abuf);
-        mbar_arrive_expect_tx(&a_full[ab], 2u * (uint32_t)abuf);
-        tma_load_2d(ad, &maps.m[s * 4 + 0], &a_full[ab], kc0, arow);
-        tma_load_2d(ad + abuf, &maps.m[s * 4 + 1], &a_full[ab], kc0, arow);
-      }
-    }
-  } else if (warp == 0) {
-    if (lane == 0) {
-      // ===== TMA producer B: one (B_hi, B_lo) stage per (phase, tap) through the ring
+  float* tile = reinterpret_cast<float*>(smem);  // the finished tile, once all MMAs have completed (operand buffers are free)
+  if (warp >= 8) {
+    // producer warpgroup: gives registers to the consumers (their five accumulators take 5 x NCOLS / 2 per thread)
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp == 8 && lane == 0) {
+      // ===== TMA producer: per phase (source, k-chunk) ONE halo tile of A (hi, lo) that all 9 taps read at row offsets,
+      // double-buffered so that phase ph+1 streams in while the MMAs of phase ph run; per (phase, tap) one (B_hi, B_lo)
+      // stage through the ring
       int stage = 0; uint32_t bphase = 0;
       for (int st = st_lo; st < st_hi; ++st) {
         const int ph = st / 9, tap = st - ph * 9;
         const int s = ph / kchunks;
         const int kc0 = (ph - s * kchunks) << 5;
+        if (tap == 0 || st == st_lo) {
+          const int lp = ph - ph_lo;
+          const int ab = lp & 1;
+          mbar_wait(&a_empty[ab], (((uint32_t)lp >> 1) & 1u) ^ 1u);
+          const int arow = a.a_row_base[s] + task * a.a_task_rows[s] + j0 - a.halo;
+          const uint32_t ad = smem_u32(smem + (size_t)ab * 2 * abuf);
+          mbar_arrive_expect_tx(&a_full[ab], 2u * (uint32_t)abuf);
+          tma_load_2d(ad, &maps.m[s * 4 + 0], &a_full[ab], kc0, arow);
+          tma_load_2d(ad + abuf, &maps.m[s * 4 + 1], &a_full[ab], kc0, arow);
+        }
         mbar_wait(&b_empty[stage], bphase ^ 1u);
         const int brow = a.b_row_base[s] + task * a.b_task_rows[s] + tap * NCOLS;
         const uint32_t bd = smem_u32(bring + (size_t)stage * BSTAGE);
@@ -270,282 +324,364 @@ __global__ void __launch_bounds__(224, 1) conv_tc_kernel(const __grid_constant__
         if (++stage == nb) { stage = 0; bphase ^= 1u; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      // instruction descriptor (cute::UMMA::InstrDescriptor): D=F32 (1<<4), A=B=TF32 (2<<7, 2<<10), both K-major,
-      // N>>3 at bit 17, M>>4 at bit 24
-      constexpr uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(NCOLS >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      // The issuing thread is the serial resource of this kernel: descriptors are built once per phase / stage and
-      // advanced with 64-bit adds on the 16-byte-unit address field (K step: +32 B = +2; tap: row_off * 128 B).
-      const uint64_t desc_base = make_desc_sw128(0);
-      int stage = 0; uint32_t bphase = 0; int kstep = 0;
-      uint64_t ahd = 0, ald = 0;
-      int sgn = 1, ab = 0;
-      for (int st = st_lo; st < st_hi; ++st) {
-        const int ph = st / 9, tap = st - ph * 9;
-        if (tap == 0 || st == st_lo) {
-          const int lp = ph - ph_lo;
-          ab = lp & 1;
-          mbar_wait(&a_full[ab], ((uint32_t)lp >> 1) & 1u);
-          if (st == st_lo) TC_MARK(2);
-          const uint32_t a_hi = smem_u32(smem + (size_t)ab * 2 * abuf);
-          ahd = desc_base + (uint64_t)(a_hi >> 4);
-          ald = ahd + (uint64_t)(abuf >> 4);
-          sgn = a.sign[ph / kchunks];
-        }
-        mbar_wait(&b_full[stage], bphase);
-        if (st == st_lo) TC_MARK(3);
-        if (st == st_lo + 9) TC_MARK(4);
-        tc_fence_after();
-        const int ty = tap / 3;
-        const int row_off = a.halo + sgn * ((ty - 1) * a.gw + (tap - 3 * ty - 1));    // in [0, 2 * halo]
-        const uint64_t ah0 = ahd + (uint64_t)(row_off * 8);
-        const uint64_t al0 = ald + (uint64_t)(row_off * 8);
-        const uint64_t bh0 = desc_base + (uint64_t)(smem_u32(bring + (size_t)stage * BSTAGE) >> 4);
-        const uint64_t bl0 = bh0 + (uint64_t)(B_BYTES >> 4);
-        if (a.stack) {
-          // N-stacked 3xTF32: B_hi and B_lo of a stage are adjacent K-major tiles, so ONE descriptor with N = 2 * NCOLS
-          // reads [B_hi; B_lo] and A_hi x [B_hi; B_lo]^T lands as [hi*hi | hi*lo] in 2 * NCOLS adjacent TMEM columns:
-          // two instructions per k-step instead of three, and A_hi crosses the shared-memory port once instead of twice
-          // (14 KB instead of 18 KB of operand fetch per k-step at N = 64 -- the measured floor of this kernel).
-          // lo*hi is added to the small block.  Round-robin over 4 such column blocks keeps <= 18 sequential
-          // accumulations per accumulator (the tensor core's fp32 accumulation truncates, see the header).
-          constexpr uint32_t idesc2 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)((2 * NCOLS) >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-          const uint32_t first = (kstep == 0) ? 0u : 1u;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            tc_mma_tf32(tmem_base + (uint32_t)k * 2 * NCOLS, ah0 + 2 * k, bh0 + 2 * k, idesc2, first);
-            tc_mma_tf32_acc(tmem_base + (uint32_t)k * 2 * NCOLS + NCOLS, al0 + 2 * k, bh0 + 2 * k, idesc);
-          }
-        } else if (kstep == 0) {
-          // first four k-steps initialise the five accumulators
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            tc_mma_tf32(tmem_base + 4 * NCOLS, al0 + 2 * k, bh0 + 2 * k, idesc, k > 0 ? 1u : 0u);
-            tc_mma_tf32_acc(tmem_base + 4 * NCOLS, ah0 + 2 * k, bl0 + 2 * k, idesc);
-            tc_mma_tf32(tmem_base + (uint32_t)k * NCOLS, ah0 + 2 * k, bh0 + 2 * k, idesc, 0u);
-          }
-        } else {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            tc_mma_tf32_acc(tmem_base + 4 * NCOLS, al0 + 2 * k, bh0 + 2 * k, idesc);
-            tc_mma_tf32_acc(tmem_base + 4 * NCOLS, ah0 + 2 * k, bl0 + 2 * k, idesc);
-            tc_mma_tf32_acc(tmem_base + (uint32_t)k * NCOLS, ah0 + 2 * k, bh0 + 2 * k, idesc);
-          }
-        }
-        kstep += 4;
-        tc_commit(&b_empty[stage]);              // frees this B stage once the MMAs above have read it
-        if (++stage == nb) { stage = 0; bphase ^= 1u; }
-        if (tap == 8 || st == st_hi - 1) tc_commit(&a_empty[ab]);   // A halo buffer pair reusable after this phase's MMAs
-      }
-      TC_MARK(5);
-      tc_commit(&accum_bar);                     // accumulators complete
+    __syncwarp();
+    if (nsplit > 1) {                            // the cluster barriers of the consumers' split-K epilogue, same sequence
+      if (a.push) cluster_wait();
+      cluster_sync_all();
+      if (!a.push) cluster_sync_all();
     }
   } else {
-    // ===== epilogue: warps 2..5, TMEM lane quarter = warp % 4.  Thread (q, lane) owns tile row r = 32 q + lane:
-    // it sums the five accumulators, adds the bias and stores its 4*NCOLS contiguous bytes straight to global;
-    // a shared-memory copy of the tile is kept only when BatchNorm statistics are wanted (column sums).
-    const int et = threadIdx.x - 64;             // 0..127
-    const int q = warp & 3;
-    const int r = q * 32 + lane;
-    __shared__ float s_bias[NCOLS];
-    {
-      const int row = j0 + et;
-      int ok = 0;
-      if (row < a.rows) {
-        const int rr = row % a.G;
-        const int yy = rr / a.gw, xx = rr - yy * a.gw;
-        ok = (yy >= 1 && yy <= a.h && xx >= 1 && xx <= a.w) ? 1 : 0;
-      }
-      row_ok[et] = ok;
-      if (et < NCOLS) s_bias[et] = a.bias ? a.bias[(long long)task * a.bias_stride + et] : 0.f;
-    }
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-    if (a.zstage) {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+    // ===== consumers: warpgroup wg computes tile rows [64 wg, 64 wg + 64)
+    const int wg = warp >> 2;
+    if (a.zstage && threadIdx.x < 128) {
       // tangent mode: the statistics below need the primal zh of the rows this CTA finishes.  Copy them into shared
-      // memory NOW (coalesced float4 loads, a region of its own behind the ring / receive buffer) while the MMAs run --
-      // the statistics loop then reads shared memory instead of one dependent global load per row (tangent-mode launches
-      // ran 5.0 / 3.1 / 1.7 us longer than forward-mode launches of the same grid, ncu)
-      constexpr int ZP = NCOLS + 4, Q = NCOLS / 4;
-      float* zbuf = reinterpret_cast<float*>(bring + (size_t)nb * BSTAGE + ((nsplit > 1 && a.push) ? (size_t)128 * (NCOLS + 4) * 4 : 0));
+      // memory first (coalesced float4 loads, a region of its own behind the ring / receive buffer) -- the statistics
+      // loop then reads shared memory instead of one dependent global load per row
+      constexpr int Q = NCOLS / 4;
       const float* zhg = a.zh + (long long)task * a.zh_stride;
       const int rows_own = 128 / nsplit, row0 = j0 + zrank * rows_own;
-      for (int idx = et; idx < rows_own * Q; idx += 128) {
+      for (int idx = threadIdx.x; idx < rows_own * Q; idx += 128) {
         const int rr = idx / Q, c4 = idx - rr * Q;
         const int gr = row0 + rr;
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
         if (gr < a.rows) v = *reinterpret_cast<const float4*>(zhg + (long long)gr * NCOLS + c4 * 4);
-        *reinterpret_cast<float4*>(zbuf + rr * ZP + c4 * 4) = v;
+        *reinterpret_cast<float4*>(zbuf + rr * P4 + c4 * 4) = v;
       }
     }
-    mbar_wait(&accum_bar, 0);
-    if (et == 0) TC_MARK(6);
-    tc_fence_after();
-    float* tile = reinterpret_cast<float*>(smem);  // all MMAs have completed: operand buffers are free
-    const bool want_stats = (a.mode != CONV_PLAIN);
-    const int grow = j0 + r;
-    float* orow = a.out + (long long)task * a.out_stride + (long long)grow * NCOLS;
-    float* push_local = nullptr;
-    uint32_t push_row = 0;                       // split-K, push variant: this thread's row inside the owner's receive buffer
-    if (nsplit > 1 && a.push) {
-      cluster_wait();                            // phase 1 (arrived at kernel start): all peers are running
-      const int rows_per = 128 / nsplit, owner = r / rows_per, rloc = r - owner * rows_per;
-      push_row = dsmem_addr(smem_u32(bring + (size_t)nb * BSTAGE) + (uint32_t)(((zrank * rows_per + rloc) * (NCOLS + 4)) * 4), (uint32_t)owner);
-      if (owner == zrank) push_local = reinterpret_cast<float*>(bring + (size_t)nb * BSTAGE) + (zrank * rows_per + rloc) * (NCOLS + 4);   // own rows: plain st.shared
-    }
+    // accumulators 0..3: hi*hi, round-robin over the k-steps of a stage; 4: lo*hi + hi*lo
+    float acc[5][R];
 #pragma unroll
-    for (int c0 = 0; c0 < NCOLS; c0 += 16) {
-      uint32_t v0[16], v1[16], v2[16], v3[16], v4[16];
-      const uint32_t ta = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0;
-      if (a.stack) {
-        // blocks k = 0..3 at columns k * 2N: [hi*hi | small]; sum the four small blocks first (into v4), then load the big ones
-        tc_ld16(ta + NCOLS, v0);
-        tc_ld16(ta + 3 * NCOLS, v1);
-        tc_ld16(ta + 5 * NCOLS, v2);
-        tc_ld16(ta + 7 * NCOLS, v3);
-        tc_wait_ld();
+    for (int q = 0; q < 5; ++q)
 #pragma unroll
-        for (int i = 0; i < 16; ++i)
-          v4[i] = __float_as_uint((__uint_as_float(v0[i]) + __uint_as_float(v1[i])) + (__uint_as_float(v2[i]) + __uint_as_float(v3[i])));
-        tc_ld16(ta, v0);
-        tc_ld16(ta + 2 * NCOLS, v1);
-        tc_ld16(ta + 4 * NCOLS, v2);
-        tc_ld16(ta + 6 * NCOLS, v3);
-      } else {
-        tc_ld16(ta, v0);
-        tc_ld16(ta + NCOLS, v1);
-        tc_ld16(ta + 2 * NCOLS, v2);
-        tc_ld16(ta + 3 * NCOLS, v3);
-        tc_ld16(ta + 4 * NCOLS, v4);
+      for (int i = 0; i < R; ++i) acc[q][i] = 0.f;
+    const uint64_t desc_base = make_desc_sw128(0);
+    int stage = 0; uint32_t bphase = 0;
+    int prev_stage = -1, prev_ab = -1;           // operands of the previous stage, released once its MMAs have completed
+    uint64_t ahd = 0, ald = 0;
+    int sgn = 1, ab = 0;
+    for (int st = st_lo; st < st_hi; ++st) {
+      const int ph = st / 9, tap = st - ph * 9;
+      if (tap == 0 || st == st_lo) {
+        const int lp = ph - ph_lo;
+        ab = lp & 1;
+        mbar_wait(&a_full[ab], ((uint32_t)lp >> 1) & 1u);
+        if (st == st_lo && threadIdx.x == 0) TC_MARK(2);
+        const uint32_t a_hi = smem_u32(smem + (size_t)ab * 2 * abuf) + (uint32_t)(wg * 64 * 128);
+        ahd = desc_base + (uint64_t)(a_hi >> 4);
+        ald = ahd + (uint64_t)(abuf >> 4);
+        sgn = a.sign[ph / kchunks];
       }
-      tc_wait_ld();
-      float o[16];
-      if (nsplit == 1) {
+      mbar_wait(&b_full[stage], bphase);
+      if (threadIdx.x == 0) { if (st == st_lo) TC_MARK(3); if (st == st_lo + 9) TC_MARK(4); }
+      const int ty = tap / 3;
+      const int row_off = a.halo + sgn * ((ty - 1) * a.gw + (tap - 3 * ty - 1));    // in [0, 2 * halo]
+      const uint64_t ah0 = ahd + (uint64_t)(row_off * 8);
+      const uint64_t al0 = ald + (uint64_t)(row_off * 8);
+      const uint64_t bh0 = desc_base + (uint64_t)(smem_u32(bring + (size_t)stage * BSTAGE) >> 4);
+      const uint64_t bl0 = bh0 + (uint64_t)(B_BYTES >> 4);
+      wgmma_fence();
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float big = (__uint_as_float(v0[i]) + __uint_as_float(v1[i])) + (__uint_as_float(v2[i]) + __uint_as_float(v3[i]));
-          o[i] = (big + __uint_as_float(v4[i])) + s_bias[c0 + i];
-        }
-        if (grow < a.rows) {
+      for (int k = 0; k < 4; ++k) {              // K step: +32 B = +2 in the 16-byte address field
+        wgmma_tf32<NCOLS>(acc[4], al0 + 2 * k, bh0 + 2 * k);
+        wgmma_tf32<NCOLS>(acc[4], ah0 + 2 * k, bl0 + 2 * k);
+        wgmma_tf32<NCOLS>(acc[k], ah0 + 2 * k, bh0 + 2 * k);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                           // the previous stage's MMAs have completed: hand its buffers back
+      if (prev_stage >= 0 && lane == 0) {
+        mbar_arrive(&b_empty[prev_stage]);
+        if (prev_ab >= 0) mbar_arrive(&a_empty[prev_ab]);
+      }
+      prev_stage = stage;
+      prev_ab = (tap == 8 || st == st_hi - 1) ? ab : -1;
+      if (++stage == nb) { stage = 0; bphase ^= 1u; }
+    }
+    wgmma_wait<0>();
 #pragma unroll
-          for (int i = 0; i < 16; i += 4) *reinterpret_cast<float4*>(orow + c0 + i) = make_float4(o[i], o[i + 1], o[i + 2], o[i + 3]);
-        }
-        if (want_stats) {
+    for (int q = 0; q < 5; ++q) reg_fence<R>(acc[q]);
+    if (threadIdx.x == 0) TC_MARK(5);
+    // both warpgroups' MMAs have completed before the tile overwrites the operand buffers
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    if (threadIdx.x == 0) TC_MARK(6);
+    {
+      // accumulator fragment: register 4 i + 2 h + e holds row 16 (warp % 4) + lane / 4 + 8 h, column 8 i + 2 (lane % 4) + e
+      const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+      const int cq = (lane & 3) * 2;
 #pragma unroll
-          for (int i = 0; i < 16; ++i) tile[r * PITCH + c0 + i] = o[i];
-        }
-      } else {
-        // split-K partial (no bias): parked in shared memory (16-byte aligned rows) for the cluster reduction below
+      for (int i = 0; i < NCOLS / 8; ++i) {
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float big = (__uint_as_float(v0[i]) + __uint_as_float(v1[i])) + (__uint_as_float(v2[i]) + __uint_as_float(v3[i]));
-          o[i] = big + __uint_as_float(v4[i]);
-        }
-        if (a.push) {
-          // row r of the tile belongs to cluster rank r / (128 / nsplit): straight into that CTA's receive buffer
-          if (push_local != nullptr) {
+        for (int hh = 0; hh < 2; ++hh) {
+          float o[2];
 #pragma unroll
-            for (int i = 0; i < 16; i += 4) *reinterpret_cast<float4*>(push_local + c0 + i) = make_float4(o[i], o[i + 1], o[i + 2], o[i + 3]);
-          } else {
-#pragma unroll
-            for (int i = 0; i < 16; i += 4) dsmem_st4(push_row + (uint32_t)((c0 + i) * 4), make_float4(o[i], o[i + 1], o[i + 2], o[i + 3]));
+          for (int e = 0; e < 2; ++e) {
+            const int x = 4 * i + 2 * hh + e;
+            const float big = (acc[0][x] + acc[1][x]) + (acc[2][x] + acc[3][x]);
+            o[e] = big + acc[4][x];
           }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 16; i += 4)
-            *reinterpret_cast<float4*>(tile + r * (NCOLS + 4) + c0 + i) = make_float4(o[i], o[i + 1], o[i + 2], o[i + 3]);
+          *reinterpret_cast<float2*>(tile + (rbase + 8 * hh) * P4 + 8 * i + cq) = make_float2(o[0], o[1]);
         }
       }
     }
-    if (et == 0) TC_MARK(7);
-  }
-
-  // rows [row_lo, row_lo + row_n) of the tile are finished by this CTA (all 128 without split-K)
-  int row_lo = 0, row_n = 128, spitch = PITCH;
-  const float* sbuf = reinterpret_cast<const float*>(smem);   // where those rows live (row index relative to row_lo)
-  if (nsplit > 1) {
-    __syncwarp();
-    if (a.push && !(warp >= 2 && warp < 6)) cluster_wait();     // phase 1 for the non-epilogue warps
-    cluster_sync_all();                            // pull: every CTA's partial tile is in its shared memory; push: every receive buffer is complete
-    if (threadIdx.x == 64) TC_MARK(10);
-    row_n = 128 / nsplit; row_lo = zrank * row_n; spitch = NCOLS + 4;
-    float* tile2 = reinterpret_cast<float*>(smem + 40 * 1024);
-    sbuf = tile2;
-    if (warp >= 2 && warp < 6) {
-      const int et = threadIdx.x - 64;
-      const uint32_t tile_local = smem_u32(smem);
-      const float* bias = a.bias ? a.bias + (long long)task * a.bias_stride : nullptr;
-      float* outp = a.out + (long long)task * a.out_stride;
-      if (a.push) {
-        const float* recv = reinterpret_cast<const float*>(bring + (size_t)nb * BSTAGE);
-        if (nsplit == 2) splitk_reduce_local<NCOLS, 2>(recv, zrank, et, bias, tile2, outp, j0, a.rows);
-        else if (nsplit == 4) splitk_reduce_local<NCOLS, 4>(recv, zrank, et, bias, tile2, outp, j0, a.rows);
-        else splitk_reduce_local<NCOLS, 8>(recv, zrank, et, bias, tile2, outp, j0, a.rows);
-      } else if (nsplit == 2) splitk_reduce<NCOLS, 2>(tile_local, zrank, et, bias, tile2, outp, j0, a.rows);
-      else if (nsplit == 4) splitk_reduce<NCOLS, 4>(tile_local, zrank, et, bias, tile2, outp, j0, a.rows);
-      else splitk_reduce<NCOLS, 8>(tile_local, zrank, et, bias, tile2, outp, j0, a.rows);
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    if (warp < 4) {
+      // ===== epilogue: thread r owns tile row r.  Without split-K: + bias, store its 4 * NCOLS contiguous bytes, keep the
+      // biased row in the tile for the statistics.  Split-K (push): the row goes into the owner CTA's receive buffer;
+      // (pull): the partial tile stays where it is.
+      const int r = threadIdx.x;
+      const int grow = j0 + r;
+      float* trow = tile + r * P4;
+      if (nsplit == 1) {
+        float* orow = a.out + (long long)task * a.out_stride + (long long)grow * NCOLS;
+        const bool want_stats = (a.mode != CONV_PLAIN);
+#pragma unroll
+        for (int c = 0; c < NCOLS; c += 4) {
+          float4 v = *reinterpret_cast<const float4*>(trow + c);
+          v.x += s_bias[c]; v.y += s_bias[c + 1]; v.z += s_bias[c + 2]; v.w += s_bias[c + 3];
+          if (grow < a.rows) *reinterpret_cast<float4*>(orow + c) = v;
+          if (want_stats) *reinterpret_cast<float4*>(trow + c) = v;
+        }
+      } else if (a.push) {
+        cluster_wait();                          // phase 1 (arrived at kernel start): all peers are running
+        const int rows_per = 128 / nsplit, owner = r / rows_per, rloc = r - owner * rows_per;
+        const uint32_t recv_off = (uint32_t)(((zrank * rows_per + rloc) * P4) * 4);
+        const uint32_t push_row = dsmem_addr(smem_u32(bring + (size_t)nb * BSTAGE) + recv_off, (uint32_t)owner);
+        float* push_local = reinterpret_cast<float*>(bring + (size_t)nb * BSTAGE + recv_off);
+#pragma unroll
+        for (int c = 0; c < NCOLS; c += 4) {
+          const float4 v = *reinterpret_cast<const float4*>(trow + c);
+          if (owner == zrank) *reinterpret_cast<float4*>(push_local + c) = v;    // own rows: plain st.shared
+          else dsmem_st4(push_row + (uint32_t)(c * 4), v);
+        }
+      }
+      if (r == 0) TC_MARK(7);
     }
-  }
 
-  if (threadIdx.x == 64) TC_MARK(11);
-  if (warp >= 2 && warp < 6) {
-    const int et = threadIdx.x - 64;
-    const bool want_stats = (a.mode != CONV_PLAIN);
-    if (want_stats) {
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      const float* zh = a.zh ? a.zh + (long long)task * a.zh_stride : nullptr;
-      const float* zbuf_s = reinterpret_cast<const float*>(bring + (size_t)nb * BSTAGE + ((nsplit > 1 && a.push) ? (size_t)128 * (NCOLS + 4) * 4 : 0));
-      constexpr int PARTS = 128 / NCOLS;           // 2 for 64 and 48, 4 for 32, 8 for 16
-      const int col = et % NCOLS, part = et / NCOLS;
-      double s1 = 0.0, s2 = 0.0;
-      if (part < PARTS) {
-        // (a 4-row-batched variant of this loop -- all loads of a batch issued before the first add, four independent fp64
-        // chains -- and an integer re-bias instead of F2F.F64.F32 both measured SLOWER: 11.6 -> 12.0 ms on Mini-ImageNet,
-        // 19.1 -> 19.7 / 20.0 ms on 20-way; see DESIGN.md, negative results)
-        for (int rr = part; rr < row_n; rr += PARTS) {
-          if (row_ok[row_lo + rr]) {
-            const float v = sbuf[rr * spitch + col];
-            if (a.mode == CONV_FWD_STATS) { s1 += (double)v; s2 += (double)v * (double)v; }
-            else {
-              const float zv = a.zstage ? zbuf_s[rr * (NCOLS + 4) + col] : zh[(long long)(j0 + row_lo + rr) * NCOLS + col];
-              s1 += (double)v; s2 += (double)zv * (double)v;
+    // rows [row_lo, row_lo + row_n) of the tile are finished by this CTA (all 128 without split-K)
+    int row_lo = 0, row_n = 128;
+    const float* sbuf = tile;                      // where those rows live (row index relative to row_lo)
+    if (nsplit > 1) {
+      __syncwarp();
+      if (a.push && warp >= 4) cluster_wait();       // phase 1 for the consumer warps that did not push
+      cluster_sync_all();                            // pull: every CTA's partial tile is in its shared memory; push: every receive buffer is complete
+      if (threadIdx.x == 0) TC_MARK(10);
+      row_n = 128 / nsplit; row_lo = zrank * row_n;
+      float* tile2 = reinterpret_cast<float*>(smem + 40 * 1024);
+      sbuf = tile2;
+      if (warp < 4) {
+        const int et = threadIdx.x;
+        const uint32_t tile_local = smem_u32(smem);
+        const float* bias = a.bias ? a.bias + (long long)task * a.bias_stride : nullptr;
+        float* outp = a.out + (long long)task * a.out_stride;
+        if (a.push) {
+          const float* recv = reinterpret_cast<const float*>(bring + (size_t)nb * BSTAGE);
+          if (nsplit == 2) splitk_reduce_local<NCOLS, 2>(recv, zrank, et, bias, tile2, outp, j0, a.rows);
+          else if (nsplit == 4) splitk_reduce_local<NCOLS, 4>(recv, zrank, et, bias, tile2, outp, j0, a.rows);
+          else splitk_reduce_local<NCOLS, 8>(recv, zrank, et, bias, tile2, outp, j0, a.rows);
+        } else if (nsplit == 2) splitk_reduce<NCOLS, 2>(tile_local, zrank, et, bias, tile2, outp, j0, a.rows);
+        else if (nsplit == 4) splitk_reduce<NCOLS, 4>(tile_local, zrank, et, bias, tile2, outp, j0, a.rows);
+        else splitk_reduce<NCOLS, 8>(tile_local, zrank, et, bias, tile2, outp, j0, a.rows);
+      }
+    }
+
+    if (threadIdx.x == 0) TC_MARK(11);
+    if (warp < 4) {
+      const int et = threadIdx.x;
+      const bool want_stats = (a.mode != CONV_PLAIN);
+      if (want_stats) {
+        asm volatile("bar.sync 2, 128;" ::: "memory");
+        const float* zh = a.zh ? a.zh + (long long)task * a.zh_stride : nullptr;
+        constexpr int PARTS = 128 / NCOLS;           // 2 for 64 and 48, 4 for 32, 8 for 16
+        const int col = et % NCOLS, part = et / NCOLS;
+        double s1 = 0.0, s2 = 0.0;
+        if (part < PARTS) {
+          for (int rr = part; rr < row_n; rr += PARTS) {
+            if (row_ok[row_lo + rr]) {
+              const float v = sbuf[rr * P4 + col];
+              if (a.mode == CONV_FWD_STATS) { s1 += (double)v; s2 += (double)v * (double)v; }
+              else {
+                const float zv = a.zstage ? zbuf[rr * P4 + col] : zh[(long long)(j0 + row_lo + rr) * NCOLS + col];
+                s1 += (double)v; s2 += (double)zv * (double)v;
+              }
             }
           }
+          if (part < 2) { sred[part][col][0] = s1; sred[part][col][1] = s2; }
         }
-        if (part < 2) { sred[part][col][0] = s1; sred[part][col][1] = s2; }
-      }
-      if (PARTS > 2) {
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (part >= 2 && part < PARTS) { atomicAdd(&sred[part & 1][col][0], s1); atomicAdd(&sred[part & 1][col][1], s2); }
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (et < NCOLS * 2) {
-        const int c = et >> 1, which = et & 1;
-        double* stats = a.stats + (long long)task * a.stats_stride;
-        atomicAdd(&stats[c * 2 + which], sred[0][c][which] + sred[1][c][which]);
+        if (PARTS > 2) {
+          asm volatile("bar.sync 2, 128;" ::: "memory");
+          if (part >= 2 && part < PARTS) { atomicAdd(&sred[part & 1][col][0], s1); atomicAdd(&sred[part & 1][col][1], s2); }
+        }
+        asm volatile("bar.sync 2, 128;" ::: "memory");
+        if (et < NCOLS * 2) {
+          const int c = et >> 1, which = et & 1;
+          double* stats = a.stats + (long long)task * a.stats_stride;
+          atomicAdd(&stats[c * 2 + which], sred[0][c][which] + sred[1][c][which]);
+        }
       }
     }
-  }
-  if (threadIdx.x == 64) TC_MARK(12);
-  if (nsplit > 1 && !a.push) {
-    __syncwarp();
-    cluster_sync_all();                            // pull variant: nobody leaves while a peer still reads its partial tile
-  }
-
-  if (threadIdx.x == 64) TC_MARK(8);
-  tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x == 0) TC_MARK(9);
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TMEM_COLS) : "memory");
+    if (threadIdx.x == 0) TC_MARK(12);
+    if (nsplit > 1 && !a.push) {
+      __syncwarp();
+      cluster_sync_all();                            // pull variant: nobody leaves while a peer still reads its partial tile
+    }
+    if (threadIdx.x == 0) TC_MARK(8);
   }
   trace_mark(22 | 0x80, a.tag);     // end of CTA (0,0,0)
 }
 
+// ---------------------------------------------------------------------------------------------
+// wgmma weight gradient of the 3x3 convolutions of blocks l >= 1, fp32-faithful via the 3xTF32 operand split:
+//
+//   dW[tap][c][f] = sum_src sum_j  A_src[j + s_tap, c] * D_src[j, f]            (+ db[f] = sum_j D_0[j, f])
+//
+// GEMM M = c, N = f, K = j (pixels).  Both operands are stored pixel-major ([grid row][channel], common.cuh), i.e.
+// MN-major for this GEMM, and TF32 wgmma reads shared-memory operands K-major only.  So A comes from REGISTERS (any
+// layout: each thread loads its m64k8 fragment straight from the hi / lo planes, the tap shift is a row offset) and the
+// warpgroup transposes every 32-row stage of D into K-major SWIZZLE_128B tiles ([f][32 j], the conv kernel's B layout).
+// CTA = one warpgroup per (row chunk, tap, task).  Per K step of 8 rows: A_hi*D_hi into one accumulator, A_hi*D_lo and
+// A_lo*D_hi into a second; after every 32-row stage (4 K steps) both are drained into fp32 register totals with IEEE adds
+// (the tensor core's accumulation truncates, so no accumulator takes more than 8 accumulations).  The dead conv-bias gradient (column sums
+// of D_0) is summed in fp32 by the centre-tap CTA.
+// ---------------------------------------------------------------------------------------------
+template <int NC>
+__device__ __forceinline__ void wgmma_tf32_rs(float (&d)[NC / 2], const uint32_t (&a)[4], uint64_t bdesc) {
+  if constexpr (NC == 16) wgmma_tf32_rs_n16(d, a, bdesc);
+  else if constexpr (NC == 32) wgmma_tf32_rs_n32(d, a, bdesc);
+  else if constexpr (NC == 48) wgmma_tf32_rs_n48(d, a, bdesc);
+  else wgmma_tf32_rs_n64(d, a, bdesc);
+}
+
+template <int NC>
+__global__ void __launch_bounds__(128) wgrad_tc_kernel(const WgradArgs a) {
+  pdl_prologue(27, a.tag);
+  constexpr int R = NC / 2;
+  constexpr int BT = NC * 128;                   // one K-major [NC][32] SWIZZLE_128B tile (bytes)
+  constexpr int DV = NC / 16;                    // float4 of one 32-row D stage per thread and plane
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  const int task = blockIdx.y;
+  const int chunk = blockIdx.x / 9, tap = blockIdx.x - chunk * 9;
+  const int ky = tap / 3, kx = tap - 3 * ky;
+  const int sh = (ky - 1) * a.gw + (kx - 1);
+  const int r_begin = chunk * a.rows_per_chunk;
+  const int r_end = min(a.rows, r_begin + a.rows_per_chunk);
+  const int guard = a.gw + 2;
+  const int KC = a.kc;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int c0 = 16 * warp + (lane >> 2), t4 = lane & 3;   // A fragment: channels c0 (+8), pixels t4 (+4) of a K step
+  const int steps = (r_end - r_begin + 31) / 32;
+  const int nit = steps * a.nsrc;
+
+  float big[R], small[R], tot[R];
+#pragma unroll
+  for (int i = 0; i < R; ++i) { big[i] = 0.f; small[i] = 0.f; tot[i] = 0.f; }
+  float4 dh[DV], dl[DV];
+  auto fetch_d = [&](int it) {
+    const int s = it / steps;
+    const int r0 = r_begin + (it - s * steps) * 32;
+    const float* Dh = a.D[s] + (long long)task * a.d_stride[s] + a.d_plane[s];
+    const float* Dl = Dh + a.d_plane[s];
+#pragma unroll
+    for (int v = 0; v < DV; ++v) {
+      const int e = tid + 128 * v, r = e / (NC / 4), f4 = e - r * (NC / 4);
+      const int jr = r0 + r;
+      const bool ok = jr < r_end;
+      dh[v] = ok ? *reinterpret_cast<const float4*>(Dh + (long long)jr * NC + f4 * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
+      dl[v] = ok ? *reinterpret_cast<const float4*>(Dl + (long long)jr * NC + f4 * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  };
+  auto drain = [&]() {
+    wgmma_wait<0>();
+    reg_fence<R>(big);
+    reg_fence<R>(small);
+#pragma unroll
+    for (int i = 0; i < R; ++i) { tot[i] += big[i] + small[i]; big[i] = 0.f; small[i] = 0.f; }
+  };
+
+  const uint64_t desc_h = make_desc_sw128(smem_u32(smem)), desc_l = desc_h + (uint64_t)(BT >> 4);
+  if (nit > 0) fetch_d(0);
+  for (int it = 0; it < nit; ++it) {
+    const int s = it / steps;
+    const int r0 = r_begin + (it - s * steps) * 32;
+    // D stage -> K-major tiles: element (f, j) at f * 128 + ((j / 4) ^ (f % 8)) * 16 + (j % 4) * 4
+#pragma unroll
+    for (int v = 0; v < DV; ++v) {
+      const int e = tid + 128 * v, r = e / (NC / 4), f4 = e - r * (NC / 4);
+      const float hv[4] = {dh[v].x, dh[v].y, dh[v].z, dh[v].w}, lv[4] = {dl[v].x, dl[v].y, dl[v].z, dl[v].w};
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int f = f4 * 4 + q;
+        const int off = f * 128 + (((r >> 2) ^ (f & 7)) << 4) + (r & 3) * 4;
+        *reinterpret_cast<float*>(smem + off) = hv[q];
+        *reinterpret_cast<float*>(smem + BT + off) = lv[q];
+      }
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma
+    __syncthreads();
+    // A fragments of the stage's 4 K steps (m64k8 tf32: a0 (c0, t4), a1 (c0 + 8, t4), a2 (c0, t4 + 4), a3 (c0 + 8, t4 + 4))
+    const float* Ah = a.A[s] + (long long)task * a.a_stride[s] + a.a_plane[s];
+    const float* Al = Ah + a.a_plane[s];
+    uint32_t ah[4][4], al[4][4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int row = r0 + 8 * k + t4 + ((q & 2) ? 4 : 0);
+        const int c = c0 + ((q & 1) ? 8 : 0);
+        const int jr = row + sh;
+        const bool ok = row < r_end && c < KC && jr >= -guard && jr < a.rows + guard;
+        ah[k][q] = ok ? __float_as_uint(Ah[(long long)jr * KC + c]) : 0u;
+        al[k][q] = ok ? __float_as_uint(Al[(long long)jr * KC + c]) : 0u;
+      }
+    const int ks = min(4, (r_end - r0 + 7) >> 3);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if (k < ks) {
+        wgmma_fence();
+        wgmma_tf32_rs<NC>(big, ah[k], desc_h + 2 * k);       // K step: +32 B = +2 in the 16-byte address field
+        wgmma_tf32_rs<NC>(small, ah[k], desc_l + 2 * k);
+        wgmma_tf32_rs<NC>(small, al[k], desc_h + 2 * k);
+        wgmma_commit();
+      }
+    }
+    if (it + 1 < nit) fetch_d(it + 1);           // next stage's global loads overlap this stage's MMAs
+    drain();
+    __syncthreads();                             // every MMA has read the tiles before they are overwritten
+  }
+
+  float* P = a.partial + (long long)task * a.partial_task_stride + (long long)chunk * a.chunk_stride;
+  // accumulator register 4 i + 2 h + e: channel c0 + 8 h, filter 8 i + 2 t4 + e
+#pragma unroll
+  for (int i = 0; i < NC / 8; ++i)
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int c = c0 + 8 * hh;
+      if (c < KC)
+        *reinterpret_cast<float2*>(P + (long long)(tap * KC + c) * NC + 8 * i + 2 * t4) = make_float2(tot[4 * i + 2 * hh], tot[4 * i + 2 * hh + 1]);
+    }
+  if (tap == 4 && tid < NC) {
+    const float* D0 = a.D[0] + (long long)task * a.d_stride[0];
+    float bacc = 0.f;
+    for (int j = r_begin; j < r_end; ++j) bacc += D0[(long long)j * NC + tid];
+    P[(long long)9 * KC * NC + tid] = bacc;
+  }
+}
+
+
 }  // namespace
 
 int tc_read_timeline(long long* out16) { return cudaMemcpyFromSymbol(out16, g_tc_timeline, 16 * sizeof(long long)) == cudaSuccess ? 0 : 1; }
+
+void launch_wgrad_tc(const WgradArgs& a, cudaStream_t st) {
+  ProfScope prof_scope__(PROF_WGRAD, a.alg_flops, st);
+  dim3 grid(a.nchunks * 9, a.tasks);
+  const size_t smem = (size_t)2 * a.ncols * 128 + 1024;
+  if (a.ncols == 64) launch_pdl(wgrad_tc_kernel<64>, grid, dim3(128), smem, st, tagged(a));
+  else if (a.ncols == 48) launch_pdl(wgrad_tc_kernel<48>, grid, dim3(128), smem, st, tagged(a));
+  else if (a.ncols == 32) launch_pdl(wgrad_tc_kernel<32>, grid, dim3(128), smem, st, tagged(a));
+  else launch_pdl(wgrad_tc_kernel<16>, grid, dim3(128), smem, st, tagged(a));
+  CUDA_CHECK_LAUNCH();
+}
 
 // halo tile rows (multiple of 8) for a grid of pitch gw, and the deepest B ring that fits next to 4 halo buffers
 int tc_conv_rpad(int gw) { return ((128 + 2 * (gw + 1)) + 7) / 8 * 8; }
@@ -588,7 +724,7 @@ static int max_clusters(size_t smem, int S) {
   auto it = cache.find({smem, S});
   if (it != cache.end()) return it->second;
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(1, 1, S); cfg.blockDim = dim3(224); cfg.dynamicSmemBytes = smem;
+  cfg.gridDim = dim3(1, 1, S); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = smem;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = 1; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = S;
@@ -644,11 +780,11 @@ static void launch_conv_tc_n(const TcMaps& maps, const TcConvArgs& a_in, size_t 
   }
   smem = tc_conv_smem_for(NCOLS, a.gw, a.nb) + (a.push ? recv_bytes : 0) + zbytes;
   if (S == 1) {
-    launch_pdl(conv_tc_kernel<NCOLS>, grid, dim3(224), smem, st, maps, tagged(a));
+    launch_pdl(conv_tc_kernel<NCOLS>, grid, dim3(TC_THREADS), smem, st, maps, tagged(a));
     return;
   }
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = grid; cfg.blockDim = dim3(224); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cfg.gridDim = grid; cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = st;
   cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = 1; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = S;

@@ -1,4 +1,4 @@
-// Declarations shared by the tcgen05 kernels (kernels_tc.cu) and the engine.
+// Declarations shared by the wgmma conv kernel (kernels_tc.cu) and the engine.
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
@@ -12,8 +12,7 @@ struct TcConvArgs {
   int push;              // split-K only, set by the launcher: 1 = partial rows are pushed into the owner CTA's receive buffer
   int zstage;            // tangent mode, set by the launcher: 1 = the primal zh rows are staged in shared memory during the MMAs
   int split_cap;         // > 0: largest split-K cluster size for THIS launch (side-stream launches: fewer, longer CTAs)
-  int stack;             // 1: N-stacked 3xTF32 (A_hi x [B_hi; B_lo] as one N = 2 * ncols MMA), 0: three MMAs per k-step
-  int halo, rpad, nb, bo_mode, timeline;   // halo = gw + 1 rows; rpad = halo-tile rows (multiple of 8); nb = B ring depth
+  int halo, rpad, nb, timeline;   // halo = gw + 1 rows; rpad = halo-tile rows (multiple of 8); nb = B ring depth
   int a_row_base[2];     // row (in the A tensor map) of grid row 0 of task 0 for this pass slot (includes the guard)
   int a_task_rows[2];    // rows per task in the A tensor map
   int sign[2];           // +1 conv, -1 dgrad
@@ -40,22 +39,4 @@ int tc_read_timeline(long long* out16);
 void launch_conv_tc(const TcMaps& maps, const TcConvArgs& a, cudaStream_t st);
 void launch_pack_weights(const ParamLayout& pl, const float* theta, long long theta_task_stride, float* pack,
                          long long pack_task_stride, long long plane_stride, int tasks, cudaStream_t st);
-
-// tcgen05 weight gradient (kernels_wgrad_tc.cu).  maps.m[s * 4 + {0,1,2,3}] = A_hi, A_lo, D_hi, D_lo of source s, all with
-// swizzle 128B_ATOM_32B and boxes [40 rows][32] (A) / [32 rows][32] (D) over the same planes the conv kernel reads.
-struct WgTcArgs {
-  int nsrc, kc, ncols, rows, gw;
-  int rows_per_chunk, nchunks;          // rows_per_chunk is a multiple of 32
-  int nstage;                           // stage ring depth (set by the launcher)
-  int force_flush;                      // 1: always the draining variant (env MAML_B200_WGRAD_LITE=0)
-  int a_row_base[2], a_task_rows[2];    // row (in the A map) of grid row 0 of task 0 for this pass slot; rows per task
-  int b_row_base[2], b_task_rows[2];
-  float* partial; long long partial_task_stride; long long chunk_stride;    // [task][chunk][9 * kc * ncols + ncols]
-  int tasks;
-  double alg_flops;
-  int tag;
-};
-size_t wgrad_tc_smem_bytes();
-int wgrad_tc_prepare();
-void wgrad_tc_set_stages(int n);        // stage ring depth in [2, 4]
-void launch_wgrad_tc(const TcMaps& maps, const WgTcArgs& a, cudaStream_t st);
+void launch_wgrad_tc(const WgradArgs& a, cudaStream_t st);   // wgmma weight gradient of blocks l >= 1 (needs a_plane / d_plane)

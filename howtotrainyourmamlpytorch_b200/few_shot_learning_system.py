@@ -1,4 +1,4 @@
-"""MAML / MAML++ meta-learning system on the B200 engine (level B0 of the drop-in boundary).
+"""MAML / MAML++ meta-learning system on the H100 engine (level B0 of the drop-in boundary).
 
 ``MAMLFewShotClassifier`` keeps the reference's public contract (reference
 ``few_shot_learning_system.py:26-424``; SURVEY.md section 8b): constructor
@@ -9,7 +9,7 @@
 
 What is different underneath: the reference runs ~3500 eager autograd ops per task; here one call of
 the C ABI (``include/maml_b200.h``) runs the whole meta-batch -- inner-loop unroll, hand-rolled
-gradients, LSLR updates, second-order reverse sweep -- as hand-written sm_100a kernels, one
+gradients, LSLR updates, second-order reverse sweep -- as hand-written sm_90a kernels, one
 all-reduce sums the flat meta-gradient over ranks (tasks are sharded over GPUs), and a fused kernel
 applies clamp + Adam.  All parameters live in ONE flat fp32 device buffer; the ``nn.Parameter``s
 are views into it.
@@ -271,7 +271,7 @@ class MAMLFewShotClassifier(nn.Module):
     def _ensure_engine(self, n_tasks):
         if self.device.type != "cuda":
             raise _native.NativeLibraryError(
-                "MAMLFewShotClassifier needs a CUDA (sm_100a) device: the hot path has no CPU fallback")
+                "MAMLFewShotClassifier needs a CUDA (sm_90a) device: the hot path has no CPU fallback")
         if self._engine is None or n_tasks > self._engine_tasks:
             a = self.args
             with torch.cuda.device(self.device):
@@ -384,7 +384,7 @@ class MAMLFewShotClassifier(nn.Module):
     def _run(self, data_batch, epoch, training_phase, apply_update):
         if self.device.type != "cuda":
             raise _native.NativeLibraryError(
-                "MAMLFewShotClassifier needs a CUDA (sm_100a) device: the hot path has no CPU fallback")
+                "MAMLFewShotClassifier needs a CUDA (sm_90a) device: the hot path has no CPU fallback")
         # _shard_override = (rank, world): test hook -- act as one rank of a sharded job without a process group
         self.rank, self.world_size = getattr(self, "_shard_override", None) or self._dist()
         xs, xt, ys, yt = self._stage_batch(data_batch)

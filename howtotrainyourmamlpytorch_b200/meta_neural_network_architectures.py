@@ -21,7 +21,7 @@ class MetaConv2dLayer(nn.Module):
     def __init__(self, in_channels, out_channels, kernel_size, stride, padding, use_bias, groups=1, dilation_rate=1):
         super().__init__()
         if int(kernel_size) != 3 or int(stride) != 1 or int(padding) != 1 or int(groups) != 1 or int(dilation_rate) != 1:
-            raise NotImplementedError("the B200 engine implements the shipped configuration only: 3x3, stride 1, "
+            raise NotImplementedError("the engine implements the shipped configuration only: 3x3, stride 1, "
                                       "padding 1 (max_pooling=true, conv_padding=true)")
         self.stride, self.padding, self.dilation_rate, self.groups, self.use_bias = 1, 1, 1, 1, bool(use_bias)
         self.weight = nn.Parameter(torch.empty(out_channels, in_channels, 3, 3))
@@ -158,7 +158,7 @@ class VGGReLUNormNetwork(nn.Module):
         number of classes (episode shaped)."""
         from . import _native
         if x.device.type != "cuda":
-            raise _native.NativeLibraryError("VGGReLUNormNetwork.forward needs a CUDA (sm_100a) device: no CPU fallback")
+            raise _native.NativeLibraryError("VGGReLUNormNetwork.forward needs a CUDA (sm_90a) device: no CPU fallback")
         n = int(x.shape[0])
         if n % self.num_output_classes != 0:
             raise ValueError("batch size %d is not a multiple of num_output_classes %d" % (n, self.num_output_classes))

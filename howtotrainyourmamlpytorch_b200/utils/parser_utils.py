@@ -1,4 +1,4 @@
-"""Config / flag handling for the B200 MAML hot path.
+"""Config / flag handling for the H100 MAML hot path.
 
 Mirrors the reference's flag system (``utils/parser_utils.py:4-106`` of the reference):
 argparse defaults overridden by the keys of a JSON file (except keys containing
@@ -145,7 +145,7 @@ def get_args(argv=None):
     """
     import torch
 
-    parser = argparse.ArgumentParser(description="B200-native MAML++ training system")
+    parser = argparse.ArgumentParser(description="H100-native MAML++ training system")
     for name, typ, default in _DEFAULTS:
         if name in ("gpu_to_use", "experiment_name", "architecture_name"):
             parser.add_argument("--" + name, nargs="?", type=typ)

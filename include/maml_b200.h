@@ -1,5 +1,5 @@
 /*
- * maml_b200.h -- C ABI of the B200-native MAML / MAML++ inner-loop engine.
+ * maml_b200.h -- C ABI of the H100-native MAML / MAML++ inner-loop engine.
  *
  * Drop-in boundary for ONE hot path of AntreasAntoniou/HowToTrainYourMAMLPytorch:
  *   MAMLFewShotClassifier.run_train_iter / run_validation_iter
@@ -46,7 +46,7 @@ typedef struct maml_b200_config {
   int32_t per_step_bn;  /* per_step_bn_statistics (MAML++) 0/1         */
   int32_t max_tasks;    /* max tasks per call on this GPU (workspace)  */
   int32_t reserved;     /* test switches. bit 0: keep the activations of EVERY target pass for debug_read;
-                           bit 1: run blocks l >= 1 on the fp32 FFMA kernels instead of tcgen05 3xTF32 */
+                           bit 1: run blocks l >= 1 on the fp32 FFMA kernels instead of wgmma 3xTF32 */
 } maml_b200_config;
 
 /* Per-call schedule: what reference forward(...) derives from epoch / phase (:232-244,:304-305). */

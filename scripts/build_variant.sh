@@ -5,8 +5,8 @@ set -e
 cd "$(dirname "$0")/../howtotrainyourmamlpytorch_b200"
 NAME=$1; shift
 mkdir -p lib/var_$NAME
-for f in kernels_conv kernels_bn kernels_head kernels_param kernels_tc kernels_wgrad_tc engine; do
-  nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC "$@" -c csrc/$f.cu -o lib/var_$NAME/$f.o &
+for f in kernels_conv kernels_bn kernels_head kernels_param kernels_tc engine; do
+  nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC "$@" -c csrc/$f.cu -o lib/var_$NAME/$f.o &
 done
 wait
 nvcc -shared -o lib/libmaml_b200_$NAME.so lib/var_$NAME/*.o -lcudart

@@ -1,6 +1,6 @@
 """Longest dependency path of the captured iteration graph.
 
-Inputs (made on a B200):
+Inputs:
   graph.dot     MAML_B200_GRAPH_DOT=<file> python scripts/trace_timeline.py            (cudaGraphDebugDotPrint)
   serial trace  MAML_B200_ONE_STREAM=1 python scripts/trace_timeline.py --full > <file>  (true kernel durations: one stream)
 Kernel nodes of the graph (creation order) and trace entries (launch order) are the same sequence, so node i gets the

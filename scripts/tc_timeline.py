@@ -1,7 +1,7 @@
-"""Diagnostic: clock64 timeline of CTA (0,0) of the LAST tcgen05 conv launch of an eval iteration
-(MAML_B200_TC_TIMELINE=1, graphs off).  Marks: 0 start, 1 setup done (barriers, TMEM alloc), 2 first A tile landed,
-3 first B stage landed, 4 B stage 9 landed, 5 last MMA issued, 6 accumulators complete (epilogue wakes),
-7 TMEM drained to smem, 8 epilogue done, 9 all warps joined."""
+"""Diagnostic: clock64 timeline of CTA (0,0) of the LAST wgmma conv launch of an eval iteration
+(MAML_B200_TC_TIMELINE=1, graphs off).  Marks: 0 start, 1 setup done (barriers, row flags), 2 first A tile landed,
+3 first B stage landed, 4 B stage 9 landed, 5 last MMA complete, 6 both warpgroups done (tile overwrites operands),
+7 epilogue rows stored / pushed, 8 epilogue done."""
 import os, sys
 os.environ["MAML_B200_TC_TIMELINE"] = sys.argv[3] if len(sys.argv) > 3 else "0"     # block to record (0 = any)
 os.environ["MAML_B200_NO_GRAPH"] = "1"

@@ -20,7 +20,7 @@ ALL_CASES = TINY_CASES + BIG_CASES
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA (B200) device")
+    config.addinivalue_line("markers", "gpu: needs a CUDA (H100) device")
 
 
 class Golden(object):
