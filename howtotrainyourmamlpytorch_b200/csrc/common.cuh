@@ -11,6 +11,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string>
 
 #define MAML_MAX_LAYERS 4
 #define MAML_MAX_STEPS 8
@@ -67,20 +68,7 @@ struct Conv0Args {                             // first block: K = 9 * C0 is tin
   int tag;          // launch sequence number inside the iteration (device trace)
 };
 
-// Optional tail of the first-block weight-gradient kernel: the LAST CTA of a task to finish sums that task's chunks (fixed
-// order) and applies what param_reduce would have (segments 0, 1 = first-block weight and bias) -- one launch less on
-// the critical path of every backward pass.
-struct FusedReduce {
-  int mode;                                    // -1: off; PR_UPDATE / PR_SUB
-  const float* theta_in; float* theta_out; float* g_out; float* tbar;
-  const float* alpha;                          // meta + m_lslr + step: alpha of segment k at alpha[k * (S + 1)]
-  int alpha_stride;                            // S + 1
-  long long task_stride;                       // Ppad
-  unsigned* counters;                          // [tasks], zero between launches (self-resetting)
-};
-
 struct WgradArgs {
-  FusedReduce fr;
   const float* A[2]; long long a_stride[2];    // conv inputs (guarded matrices) [rows][kc]
   const float* D[2]; long long d_stride[2];    // output gradients (zero-border matrices) [rows][ncols]
   long long a_plane[2], d_plane[2];            // tensor-core path: distance (floats) from the fp32 plane to its TF32 hi plane
@@ -207,12 +195,8 @@ void launch_prep_x(const float* x, float* xg, long long xg_task_stride, int task
                    cudaStream_t st);
 void launch_conv_rows(const ConvArgs& a, cudaStream_t st);
 void launch_conv0(const Conv0Args& a, cudaStream_t st);
-void conv0_set_rb(int on);
-void wgrad0_set_rb(int on);
 void launch_wgrad(const WgradArgs& a, cudaStream_t st);
-void wgrad_set_row_variant(int on);
 void launch_wgrad0(const WgradArgs& a, cudaStream_t st);
-bool wgrad0_can_fuse_reduce(int kc, int ncols, int nsrc);
 void launch_bnact(const BnActArgs& a, cudaStream_t st);
 void launch_bnact_tan(const BnActTanArgs& a, cudaStream_t st);
 void launch_bnbwd_reduce(const BnBwdArgs& a, cudaStream_t st);
@@ -221,11 +205,7 @@ void launch_bnbwd_tan_reduce(const BnBwdTanArgs& a, cudaStream_t st);
 void launch_bnbwd_tan_apply(const BnBwdTanArgs& a, cudaStream_t st);
 void launch_bnbwd(const BnBwdArgs& a, cudaStream_t st);          // reduce + apply (one cluster kernel for small blocks)
 void launch_bnbwd_tan(const BnBwdTanArgs& a, cudaStream_t st);
-extern int g_bn_cta_cap;            // see kernels_bn.cu (bn_grid)
-void bn_set_fuse(int on);
-void bn_set_fuse_max(int v);
 bool tail_fusable(const BnGeom& g, int n_rows, int rows_per_cta);
-void tail_set_onchip(int on);
 void launch_tail_fused(const BnActArgs& fa, const HeadArgs& ha, const BnBwdArgs& ba, cudaStream_t st);
 void launch_tail_tan_fused(const BnActTanArgs& fa, const HeadArgs& ha, const BnBwdTanArgs& ba, cudaStream_t st);
 void launch_head(const HeadArgs& a, cudaStream_t st);
@@ -296,20 +276,61 @@ enum { PASS_SUP_FWD = 0, PASS_SUP_BWD = 1, PASS_TGT_FWD = 2, PASS_TGT_BWD = 3, P
        PASS_KINDS = 6 };
 
 // ---------------------------------------------------------------------------------------------
-// Programmatic dependent launch: every kernel is launched with the programmatic-stream-serialization attribute and
-// starts with `griddepcontrol.launch_dependents; griddepcontrol.wait;` -- the next kernel of the stream is scheduled
-// while this one still runs (its launch latency and set-up overlap) and blocks until this grid has completed and
-// flushed.  Inside the captured CUDA graph the kernels' own durations, not the launch gaps, set the critical path, so
-// the attribute is OFF unless MAML_B200_PDL=1.
+// Diagnostic switches of one engine handle (environment variables MAML_B200_<NAME>, read once when the handle is
+// created: engine.cu read_options).  The value written here is the default.
 // ---------------------------------------------------------------------------------------------
-extern int g_use_pdl;               // 0: off, 1: every launch, 2: only launches on the iteration's main chain (g_pdl_main_stream),
-                                    // 3: every stream except the weight-gradient side stream (g_pdl_wg_stream)
-extern cudaStream_t g_pdl_main_stream, g_pdl_wg_stream;
-extern int g_pdl_cluster;           // cluster launches that take the attribute too: bit 0 fused BatchNorm backward, bit 1 split-K convs
+struct EngineOptions {
+  bool no_graph = false;     // NO_GRAPH (set): eager launches instead of the captured CUDA graph
+  bool one_stream = false;   // ONE_STREAM (set): every kernel on the caller's stream
+  bool wgrad_tc = true;      // WGRAD_TC=0: FFMA weight gradient for blocks l >= 1
+  bool wgrad_row = true;     // WGRAD_ROW=0: one filter tap per FFMA weight-gradient CTA instead of one filter row
+  int tc_split = 8;          // TC_SPLIT: largest split-K cluster size of the wgmma conv, in [1, 8] (1 = off)
+  int tc_split_side = 0;     // TC_SPLIT_SIDE: split-K cap of side-stream convs (0 = none)
+  int tc_nb = 0;             // TC_NB: B ring depth of main-chain convs, in [2, 8] (0 = by regime)
+  int tc_nb_side = 0;        // TC_NB_SIDE: B ring depth cap of side-stream convs (< 2 = none)
+  bool tc_nb_fit = false;    // TC_NB_FIT=1: cut the ring to the B stages one CTA ever has in flight
+  bool tc_push = true;       // TC_PUSH=0: pull-based split-K reduction (two cluster barriers)
+  bool tc_zstage = true;     // TC_ZSTAGE=0: tangent-mode statistics read the primal zh from global memory
+  bool bn_fuse = true;       // BN_FUSE=0: BatchNorm backward always as two kernels (reduce, apply)
+  int bn_side_cap = 0;       // BN_SIDE_CAP: CTA cap of grid-stride BatchNorm launches on side streams (0 = none)
+  bool tail_fuse = true;     // TAIL_FUSE=0: last block / head / its BatchNorm backward as separate kernels
+  int tail_onchip = 3;       // TAIL_ONCHIP: fused last-block kernels on chip, bit 0 primal, bit 1 tangent
+  bool tan_split = true;     // TAN_SPLIT=0: two-source tangent convs on the main chain
+  int tgt_slots = 2;         // TGT_SLOTS: target-pass buffers / streams (>= 1)
+  int pdl = -1;              // PDL: programmatic dependent launch mode, in [0, 3] (-1 = by regime)
+  int pdl_cluster = 0;       // PDL_CLUSTER: cluster launches that take PDL too, bit 0 fused BatchNorm backward, bit 1 split-K convs
+  int tc_timeline = -1;      // TC_TIMELINE: clock64 milestones of one conv CTA of block l (0 = any block, -1 = off)
+  std::string graph_dot;     // GRAPH_DOT: file the captured graph is written to (empty = none)
+};
+
+// ---------------------------------------------------------------------------------------------
+// Launch context: what the launchers need to know about the handle whose call is enqueueing work.  The engine installs
+// it for the duration of each handle call (engine.cu LaunchScope); with none installed PDL is off, the options are the
+// defaults and nothing is profiled.
+// ---------------------------------------------------------------------------------------------
+struct Profiler;
+struct LaunchContext {
+  const EngineOptions* opt;
+  int pdl_mode;                    // 0: off, 1: every launch, 2: only launches on main_stream, 3: every stream but wg_stream
+  cudaStream_t main_stream;        // stream of the call's main chain (null: the call has none)
+  cudaStream_t wg_stream;          // the handle's weight-gradient side stream
+  Profiler* prof;                  // non-null while the handle is profiling
+};
+const LaunchContext& launch_ctx();
+// a launch on a side stream of the current iteration (target passes, weight gradients, pre-computed tangent addends)
+inline bool on_side_stream(cudaStream_t st) { return launch_ctx().main_stream && st != launch_ctx().main_stream; }
+
+// ---------------------------------------------------------------------------------------------
+// Programmatic dependent launch: a kernel launched with the programmatic-stream-serialization attribute starts with
+// `griddepcontrol.launch_dependents; griddepcontrol.wait;` -- the next kernel of the stream is scheduled while this one
+// still runs (its launch latency and set-up overlap) and blocks until this grid has completed and flushed.  Which
+// launches take the attribute is the handle's PDL mode: main chain only in the latency-bound regime, none in the
+// throughput-bound one (maml_b200_create), or MAML_B200_PDL.
+// ---------------------------------------------------------------------------------------------
 inline bool pdl_allowed(cudaStream_t st) {
-  return g_use_pdl == 1 || (g_use_pdl == 2 && st == g_pdl_main_stream) || (g_use_pdl == 3 && st != g_pdl_wg_stream);
+  const LaunchContext& c = launch_ctx();
+  return c.pdl_mode == 1 || (c.pdl_mode == 2 && st == c.main_stream) || (c.pdl_mode == 3 && st != c.wg_stream);
 }
-extern int g_launch_prio;
 int num_sms();                     // streaming multiprocessors of the current device (queried once)
 
 // Device-side launch trace (debug; maml_b200_trace): CTA (0,0,0) of every kernel appends (globaltimer ns << 8 | kernel
@@ -350,16 +371,10 @@ template <typename... KArgs, typename... Args>
 inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute attr[2];
+  cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = pdl_allowed(st) ? 1 : 0;
   cfg.attrs = attr; cfg.numAttrs = 1;
-  if (g_launch_prio) {          // explicit per-launch priority = the stream's (captured graph nodes keep it)
-    int prio = 0;
-    cudaStreamGetPriority(st, &prio);
-    attr[1].id = cudaLaunchAttributePriority; attr[1].val.priority = prio;
-    cfg.numAttrs = 2;
-  }
   cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
@@ -376,12 +391,10 @@ template <class A> inline A tagged(const A& a) { A t = a; t.tag = launch_tag(); 
 // ---------------------------------------------------------------------------------------------
 enum { PROF_CONV = 0, PROF_CONV0 = 1, PROF_WGRAD = 2, PROF_WGRAD0 = 3, PROF_BN = 4, PROF_HEAD = 5, PROF_PARAM = 6,
        PROF_CATS = 7 };
-struct Profiler;
-extern Profiler* g_prof;                       // non-null while profiling is on
-void prof_begin(int cat, double flops, cudaStream_t st);
-void prof_end(cudaStream_t st);
+void prof_begin(Profiler* p, int cat, double flops, cudaStream_t st);
+void prof_end(Profiler* p, cudaStream_t st);
 struct ProfScope {
-  cudaStream_t st; bool on;
-  ProfScope(int cat, double flops, cudaStream_t s) : st(s), on(g_prof != nullptr) { if (on) prof_begin(cat, flops, st); }
-  ~ProfScope() { if (on) prof_end(st); }
+  cudaStream_t st; Profiler* prof;
+  ProfScope(int cat, double flops, cudaStream_t s) : st(s), prof(launch_ctx().prof) { if (prof) prof_begin(prof, cat, flops, st); }
+  ~ProfScope() { if (prof) prof_end(prof, st); }
 };

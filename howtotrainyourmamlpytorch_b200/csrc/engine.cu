@@ -43,13 +43,42 @@ struct Profiler {
   void reset() { recs.clear(); used = 0; }
   ~Profiler() { for (auto e : pool) cudaEventDestroy(e); }
 };
-Profiler* g_prof = nullptr;
-void prof_begin(int cat, double flops, cudaStream_t st) {
-  Profiler::Rec r; r.cat = cat; r.flops = flops; r.a = g_prof->get(); r.b = g_prof->get();
+void prof_begin(Profiler* p, int cat, double flops, cudaStream_t st) {
+  Profiler::Rec r; r.cat = cat; r.flops = flops; r.a = p->get(); r.b = p->get();
   cudaEventRecord(r.a, st);
-  g_prof->recs.push_back(r);
+  p->recs.push_back(r);
 }
-void prof_end(cudaStream_t st) { cudaEventRecord(g_prof->recs.back().b, st); }
+void prof_end(Profiler* p, cudaStream_t st) { cudaEventRecord(p->recs.back().b, st); }
+
+// Every diagnostic switch of the engine, read from the environment once per handle (maml_b200_create).
+static EngineOptions read_options() {
+  auto flag = [](const char* name, bool def) { const char* v = getenv(name); return v ? atoi(v) != 0 : def; };
+  auto num = [](const char* name, int def) { const char* v = getenv(name); return v ? atoi(v) : def; };
+  auto clamp = [](int v, int lo, int hi) { return std::max(lo, std::min(hi, v)); };
+  EngineOptions o;
+  o.no_graph = getenv("MAML_B200_NO_GRAPH") != nullptr;
+  o.one_stream = getenv("MAML_B200_ONE_STREAM") != nullptr;
+  o.wgrad_tc = flag("MAML_B200_WGRAD_TC", o.wgrad_tc);
+  o.wgrad_row = flag("MAML_B200_WGRAD_ROW", o.wgrad_row);
+  o.tc_split = clamp(num("MAML_B200_TC_SPLIT", o.tc_split), 1, 8);
+  o.tc_split_side = num("MAML_B200_TC_SPLIT_SIDE", o.tc_split_side);
+  if (getenv("MAML_B200_TC_NB")) o.tc_nb = clamp(num("MAML_B200_TC_NB", 0), 2, 8);
+  o.tc_nb_side = num("MAML_B200_TC_NB_SIDE", o.tc_nb_side);
+  o.tc_nb_fit = flag("MAML_B200_TC_NB_FIT", o.tc_nb_fit);
+  o.tc_push = flag("MAML_B200_TC_PUSH", o.tc_push);
+  o.tc_zstage = flag("MAML_B200_TC_ZSTAGE", o.tc_zstage);
+  o.bn_fuse = flag("MAML_B200_BN_FUSE", o.bn_fuse);
+  o.bn_side_cap = num("MAML_B200_BN_SIDE_CAP", o.bn_side_cap);
+  o.tail_fuse = flag("MAML_B200_TAIL_FUSE", o.tail_fuse);
+  o.tail_onchip = num("MAML_B200_TAIL_ONCHIP", o.tail_onchip);
+  o.tan_split = flag("MAML_B200_TAN_SPLIT", o.tan_split);
+  o.tgt_slots = std::max(1, num("MAML_B200_TGT_SLOTS", o.tgt_slots));
+  o.pdl = num("MAML_B200_PDL", o.pdl);
+  o.pdl_cluster = num("MAML_B200_PDL_CLUSTER", o.pdl_cluster);
+  if (getenv("MAML_B200_TC_TIMELINE")) o.tc_timeline = std::max(0, num("MAML_B200_TC_TIMELINE", 0));
+  if (const char* v = getenv("MAML_B200_GRAPH_DOT")) o.graph_dot = v;
+  return o;
+}
 
 struct PassSet {            // activation buffers of one kind of pass (support: S slots, target / tangent: 1)
   int n = 0, slots = 0;
@@ -70,14 +99,11 @@ struct ChunkPlan { int rows_per_chunk[MAML_MAX_LAYERS]; int nchunks[MAML_MAX_LAY
 // rows of a batch one head CTA handles: small batches (<= 16 rows: the Omniglot 5-way passes) stay in ONE CTA so that the
 // last block / head / BatchNorm-backward fusion applies; larger ones are cut into groups of 4 rows -- the head of a 75-row
 // Mini-ImageNet target pass would otherwise run as 5 latency-bound CTAs per task
-static inline int head_rows(int n) {
-  static const int forced = getenv("MAML_B200_HEAD_ROWS") ? atoi(getenv("MAML_B200_HEAD_ROWS")) : 0;
-  if (forced > 0) return forced;
-  return n <= 16 ? 16 : 4;
-}
+static inline int head_rows(int n) { return n <= 16 ? 16 : 4; }
 
 struct maml_b200_handle {
   maml_b200_config cfg;
+  EngineOptions opt;
   int L, F, N, S, C, H, W, n_s, n_t, maxT, D, pix;
   LayerGeom geo[MAML_MAX_LAYERS];
   ParamLayout pl;
@@ -94,28 +120,20 @@ struct maml_b200_handle {
   float *losses = nullptr, *correct = nullptr, *decay_dev = nullptr;
   double* abar = nullptr;
   long long* zero_labels = nullptr;   // [max(n_s, n_t)] zeros (label-free forward)
-  unsigned* wg0_counters = nullptr;   // [maxT] arrival counters of the fused first-block reduction (self-resetting)
-  bool fuse_wg0_reduce = false;       // env MAML_B200_WG0_FUSE=1: first-block parameter reduction fused into wgrad0 (last CTA of a
-                                      // task); off by default
   float* pinned = nullptr;            // host staging ring for small per-call scalars (16 slots x 32 floats)
   int pin_slot = 0;
   long long last_launches = 0;
   int last_tasks = 0;
   Profiler prof;
+  bool profiling = false;             // maml_b200_profile(h, 1): this handle's launches are recorded into prof
   // side streams / events for fork-join inside one iteration, CUDA-graph cache
   cudaStream_t s_cap = nullptr, s_tgt = nullptr, s_tgt2 = nullptr, s_wg = nullptr;
   int tgt_slots = 1;       // target passes of consecutive steps are independent: double-buffered on two streams
   cudaEvent_t ev_fork = nullptr, ev_wg = nullptr, ev_pack = nullptr, ev_tgt[MAML_MAX_STEPS] = {};
   cudaEvent_t ev_pre[2 * MAML_MAX_LAYERS] = {};     // tangent pre-computed addends: [l] forward conv, [MAX_LAYERS + l] dgrad
-  bool tail_fuse = true;                              // env MAML_B200_TAIL_FUSE=0: last block / head / its BN backward as separate kernels
-  bool tan_split = true;                              // env MAML_B200_TAN_SPLIT=0: two-source tangent convs on the main chain
   bool use_graphs = true;
-  cudaStream_t main_stream = nullptr;                 // stream of the iteration's main chain while it is being enqueued
-  int pdl_mode = 0, pdl_cluster = 0;                  // programmatic dependent launch (see common.cuh), chosen per handle
+  int pdl_mode = 0;                                   // programmatic dependent launch (see common.cuh), chosen per handle
   int nb_main = 8;                                    // shared-memory B ring depth of the tensor-core conv kernel (see maml_b200_create)
-  int nb_side = 0;                                    // env MAML_B200_TC_NB_SIDE: B ring depth cap of side-stream convs (0 = the global cap)
-  int side_bn_cap = 0;                                // env MAML_B200_BN_SIDE_CAP: CTA cap of grid-stride BatchNorm launches on side streams
-  int split_cap_side = 0, split_cap_l1 = 0;           // env MAML_B200_TC_SPLIT_SIDE / _L1: split-K caps (0 = none) for side-stream convs / main-chain block 1
   // results produced on s_wg (upper-block parameter reduction, weight packs) that the main chain has not joined yet:
   // consumed right before the first kernel that reads them (block 1's convolution / the head)
   bool wg_pending = false;
@@ -124,7 +142,6 @@ struct maml_b200_handle {
   unsigned long long graph_clock = 0;
   // tensor-core path (blocks l >= 1 when F % 32 == 0)
   bool use_tc = false;
-  bool wgrad_tc = true;    // wgmma weight gradient for blocks l >= 1 (env MAML_B200_WGRAD_TC=0: the FFMA filter-row kernel)
   float *pack_theta = nullptr, *pack_u = nullptr;       // [4 planes][steps][T][(L-1)*9*F*F]
   long long pack_theta_plane = 0, pack_u_plane = 0, pack_task = 0;
   CUtensorMap theta_map[4], u_map[4];                   // planes: W hi, W lo, WT hi, WT lo
@@ -133,6 +150,24 @@ struct maml_b200_handle {
   char* comm_block = nullptr; long long comm_bytes = 0;
   void* comm_opened[MAML_MAX_RANKS] = {};               // peer blocks mapped with cudaIpcOpenMemHandle
   bool comm_connected = false;
+};
+
+// launch context of the handle call in progress on this thread (common.cuh); the default one has PDL off
+static const EngineOptions g_default_options;
+static thread_local LaunchContext g_launch_ctx{&g_default_options, 0, nullptr, nullptr, nullptr};
+const LaunchContext& launch_ctx() { return g_launch_ctx; }
+
+// Installs a handle's launch context for the duration of one call and restores the previous one.  Calls that enqueue an
+// iteration chain pass its main stream and launch with the handle's PDL mode; the other calls launch without PDL.
+struct LaunchScope {
+  LaunchContext saved;
+  explicit LaunchScope(maml_b200_handle* h) : LaunchScope(h, 0, nullptr) {}
+  LaunchScope(maml_b200_handle* h, cudaStream_t main) : LaunchScope(h, h->pdl_mode, main) {}
+  ~LaunchScope() { g_launch_ctx = saved; }
+ private:
+  LaunchScope(maml_b200_handle* h, int pdl_mode, cudaStream_t main) : saved(g_launch_ctx) {
+    g_launch_ctx = LaunchContext{&h->opt, pdl_mode, main, h->s_wg, h->profiling ? &h->prof : nullptr};
+  }
 };
 
 int num_sms() {
@@ -211,9 +246,8 @@ static void plan_chunks(maml_b200_handle* h, int n, ChunkPlan* cp) {
       // the FMA pipe fed with 8 warps): a second CTA per SM would take the register file away from the main chain's kernels
       // running beside it; 3 filter rows x tasks x
       // chunks should just fill one slot per SM -- 720 CTAs (128-row chunks at 8 tasks) ran as 1.2 waves = 2x the time
-      static const int wg_slots = getenv("MAML_B200_WG_SLOTS") ? atoi(getenv("MAML_B200_WG_SLOTS")) : num_sms();
-      static const int wg_per_chunk = (getenv("MAML_B200_WGRAD_ROW") && atoi(getenv("MAML_B200_WGRAD_ROW")) == 0) ? 9 : 3;
-      long long want = std::max<long long>(1, wg_slots / ((long long)wg_per_chunk * h->maxT));
+      const int wg_per_chunk = h->opt.wgrad_row ? 3 : 9;
+      long long want = std::max<long long>(1, num_sms() / ((long long)wg_per_chunk * h->maxT));
       nch = (int)std::min<long long>(std::min<long long>(64, want), std::max<long long>(1, (rows + 15) / 16));
     }
     rpc = (int)rup((rows + nch - 1) / nch, 16);
@@ -330,7 +364,7 @@ static void carve_pass(maml_b200_handle* h, Bump& b, PassSet& ps, int n, int slo
 static void carve(maml_b200_handle* h, Bump& b) {
   const long long T = h->maxT;
   carve_pass(h, b, h->sup, h->n_s, h->S, true, true);
-  h->tgt_slots = std::min(h->S, getenv("MAML_B200_TGT_SLOTS") ? std::max(1, atoi(getenv("MAML_B200_TGT_SLOTS"))) : 2);
+  h->tgt_slots = std::min(h->S, h->opt.tgt_slots);
   carve_pass(h, b, h->tgt, h->n_t, (h->cfg.reserved & 1) ? h->S : h->tgt_slots, true, true);   // reserved bit 0: keep every target pass (tests)
   carve_pass(h, b, h->tan, h->n_s, 1, false, true);
   carve_pass(h, b, h->tan2, h->n_s, 1, false, true);
@@ -358,7 +392,6 @@ static void carve(maml_b200_handle* h, Bump& b) {
   h->abar = b.d(T * h->pl.nseg_inner * MAML_MAX_STEPS);
   h->decay_dev = b.f(MAML_MAX_STEPS);
   h->zero_labels = (long long*)b.d(std::max(h->n_s, h->n_t));
-  h->wg0_counters = (unsigned*)b.f(h->maxT);
 }
 
 extern "C" int maml_b200_create(const maml_b200_config* cfg, maml_b200_handle** out) {
@@ -377,28 +410,13 @@ extern "C" int maml_b200_create(const maml_b200_config* cfg, maml_b200_handle** 
   }
   maml_b200_handle* h = new maml_b200_handle();
   h->cfg = *cfg;
+  h->opt = read_options();
   h->L = cfg->num_stages; h->F = cfg->filters; h->N = cfg->n_way; h->S = cfg->inner_steps;
   h->C = cfg->channels; h->H = cfg->height; h->W = cfg->width; h->n_s = n_s; h->n_t = n_t; h->maxT = cfg->max_tasks;
   build_geometry(h);
   build_layout(h);
   // tensor-core (wgmma / TMA, 3xTF32) convolutions for blocks l >= 1; reserved bit 1 forces the fp32 FFMA kernels (tests)
   h->use_tc = (h->L > 1) && !(cfg->reserved & 2);
-  if (const char* wt = getenv("MAML_B200_WGRAD_TC")) h->wgrad_tc = atoi(wt) != 0;
-  if (const char* sp = getenv("MAML_B200_TC_SPLIT")) tc_conv_set_split(atoi(sp));
-  tc_conv_set_zstage(getenv("MAML_B200_TC_ZSTAGE") ? atoi(getenv("MAML_B200_TC_ZSTAGE")) : 1);
-  tc_conv_set_push(getenv("MAML_B200_TC_PUSH") ? atoi(getenv("MAML_B200_TC_PUSH")) : 1);
-  tc_conv_set_ring_fit(getenv("MAML_B200_TC_NB_FIT") ? atoi(getenv("MAML_B200_TC_NB_FIT")) : 0);
-  if (const char* sp = getenv("MAML_B200_TC_NB_SIDE")) h->nb_side = atoi(sp);
-  if (const char* sp = getenv("MAML_B200_TC_SPLIT_SIDE")) h->split_cap_side = atoi(sp);
-  if (const char* sp = getenv("MAML_B200_TC_SPLIT_L1")) h->split_cap_l1 = atoi(sp);
-  if (const char* sp = getenv("MAML_B200_BN_SIDE_CAP")) h->side_bn_cap = atoi(sp);
-  g_launch_prio = (getenv("MAML_B200_LAUNCH_PRIO") && atoi(getenv("MAML_B200_LAUNCH_PRIO")) != 0) ? 1 : 0;
-  if (const char* wr = getenv("MAML_B200_WGRAD_ROW")) wgrad_set_row_variant(atoi(wr));
-  if (const char* bf = getenv("MAML_B200_BN_FUSE")) bn_set_fuse(atoi(bf));
-  if (const char* bf = getenv("MAML_B200_BN_FUSE_MAX")) bn_set_fuse_max(atoi(bf));
-  if (const char* rb = getenv("MAML_B200_CONV0_RB")) conv0_set_rb(atoi(rb));
-  if (const char* rb = getenv("MAML_B200_WGRAD0_RB")) wgrad0_set_rb(atoi(rb));
-  if (const char* fz = getenv("MAML_B200_WG0_FUSE")) h->fuse_wg0_reduce = atoi(fz) != 0;
   for (int l = 1; l < h->L && h->use_tc; ++l)
     if (tc_conv_rpad(h->geo[l].gw) > 256 || tc_conv_ring(h->F, h->geo[l].gw) < 2) h->use_tc = false;   // image too wide for one halo box      // F in {16, 32, 48, 64}: ragged K chunks are zero-filled by TMA
   plan_chunks(h, h->n_s, &h->plan_sup);
@@ -415,7 +433,7 @@ extern "C" int maml_b200_create(const maml_b200_config* cfg, maml_b200_handle** 
   if (make_all_maps(h)) { cudaFree(h->ws); delete h; return 1; }
   e = cudaMallocHost((void**)&h->pinned, 16 * 32 * sizeof(float));
   if (e != cudaSuccess) { cudaFree(h->ws); delete h; return fail(std::string("cudaMallocHost: ") + cudaGetErrorString(e)); }
-  h->use_graphs = !(cfg->reserved & 4) && !getenv("MAML_B200_NO_GRAPH");
+  h->use_graphs = !(cfg->reserved & 4) && !h->opt.no_graph;
   // Two regimes, told apart by whether one iteration's block-1 tiles (support + target, all tasks) fit one wave of SMs.
   //  * latency-bound (Omniglot 5-way at 8 tasks: 144 tiles): programmatic dependent launch on the MAIN chain only (the next
   //    kernel of the support / tangent chain is scheduled while the current one drains; on every stream, early-launched
@@ -427,18 +445,15 @@ extern "C" int maml_b200_create(const maml_b200_config* cfg, maml_b200_handle** 
     const int l1 = h->L > 1 ? 1 : 0;
     const long long tiles = (((long long)h->n_s * h->geo[l1].G + 127) / 128 + ((long long)h->n_t * h->geo[l1].G + 127) / 128) * h->maxT;
     const bool small = tiles <= num_sms();
-    h->pdl_mode = getenv("MAML_B200_PDL") ? atoi(getenv("MAML_B200_PDL")) : (small ? 2 : 0);
-    h->pdl_cluster = getenv("MAML_B200_PDL_CLUSTER") ? atoi(getenv("MAML_B200_PDL_CLUSTER")) : 0;
-    h->nb_main = getenv("MAML_B200_TC_NB") ? std::max(2, std::min(8, atoi(getenv("MAML_B200_TC_NB")))) : (small ? 8 : 4);
-    g_use_pdl = h->pdl_mode; g_pdl_cluster = h->pdl_cluster;
+    h->pdl_mode = h->opt.pdl >= 0 ? h->opt.pdl : (small ? 2 : 0);
+    h->nb_main = h->opt.tc_nb > 0 ? h->opt.tc_nb : (small ? 8 : 4);
   }
   // Priorities: the support chain (capture stream) is the critical path; the weight-gradient and target streams only
   // have to finish by the end of a step.  Their many small CTAs would otherwise occupy every SM and keep the
   // whole-SM tensor-core conv CTAs of the critical path waiting.
   int prio_lo = 0, prio_hi = 0;
   cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);      // lo = numerically largest = least urgent
-  const bool use_prio = getenv("MAML_B200_NO_PRIO") == nullptr;
-  const int p_main = use_prio ? prio_hi : 0, p_tgt = use_prio ? std::min(prio_lo, prio_hi + 1) : 0, p_wg = use_prio ? prio_lo : 0;
+  const int p_main = prio_hi, p_tgt = std::min(prio_lo, prio_hi + 1), p_wg = prio_lo;
   bool ok = cudaStreamCreateWithPriority(&h->s_cap, cudaStreamNonBlocking, p_main) == cudaSuccess &&
             cudaStreamCreateWithPriority(&h->s_tgt, cudaStreamNonBlocking, p_tgt) == cudaSuccess &&
             cudaStreamCreateWithPriority(&h->s_tgt2, cudaStreamNonBlocking, p_tgt) == cudaSuccess &&
@@ -448,9 +463,6 @@ extern "C" int maml_b200_create(const maml_b200_config* cfg, maml_b200_handle** 
             cudaEventCreateWithFlags(&h->ev_pack, cudaEventDisableTiming) == cudaSuccess;
   for (int s = 0; ok && s < MAML_MAX_STEPS; ++s) ok = cudaEventCreateWithFlags(&h->ev_tgt[s], cudaEventDisableTiming) == cudaSuccess;
   for (int s = 0; ok && s < 2 * MAML_MAX_LAYERS; ++s) ok = cudaEventCreateWithFlags(&h->ev_pre[s], cudaEventDisableTiming) == cudaSuccess;
-  if (const char* ts = getenv("MAML_B200_TAN_SPLIT")) h->tan_split = atoi(ts) != 0;
-  if (const char* tf = getenv("MAML_B200_TAIL_FUSE")) h->tail_fuse = atoi(tf) != 0;
-  tail_set_onchip(getenv("MAML_B200_TAIL_ONCHIP") ? atoi(getenv("MAML_B200_TAIL_ONCHIP")) : 3);      // bit 0 primal, bit 1 tangent
   if (!ok) { maml_b200_destroy(h); return fail("stream / event creation failed"); }
   *out = h;
   return 0;
@@ -580,16 +592,6 @@ static void reduce_upper_on_side(maml_b200_handle* h, const ReduceSpec& rs, cons
   cudaEventRecord(h->ev_wg, h->s_wg);
   h->wg_pending = true;
 }
-// first-block reduction fused into the weight-gradient kernel (see FusedReduce); false -> the caller launches reduce_lower
-static bool fuse_lower_into_wgrad0(maml_b200_handle* h, const ReduceSpec& rs, const float* meta, WgradArgs& w) {
-  w.fr.mode = -1;
-  if (!h->fuse_wg0_reduce || !wgrad0_can_fuse_reduce(w.kc, w.ncols, w.nsrc)) return false;
-  w.fr.mode = rs.mode;
-  w.fr.theta_in = rs.theta_in; w.fr.theta_out = rs.theta_out; w.fr.g_out = rs.g_out; w.fr.tbar = rs.tbar;
-  w.fr.alpha = meta + h->pl.m_lslr + rs.step; w.fr.alpha_stride = h->S + 1;
-  w.fr.task_stride = h->Ppad; w.fr.counters = h->wg0_counters;
-  return true;
-}
 
 static void reduce_lower(maml_b200_handle* h, const ReduceSpec& rs, const PartialDesc& pd, const float* partial,
                          const float* meta, int T, cudaStream_t st) {
@@ -609,8 +611,11 @@ static void tc_conv(maml_b200_handle* h, int l, int n, int nsrc, const TcOp* ops
   TcMaps maps;
   TcConvArgs a{};
   a.nsrc = nsrc; a.kc = h->F; a.rows = n * g.G; a.gw = g.gw; a.G = g.G; a.h = g.h; a.w = g.w; a.ncols = h->F; a.mode = mode; a.tasks = T; a.plan_tasks = h->maxT;
-  a.split_cap = (h->main_stream && st != h->main_stream) ? h->split_cap_side : (l == 1 ? h->split_cap_l1 : 0);
-  a.halo = g.gw + 1; a.rpad = tc_conv_rpad(g.gw); a.nb = std::min(tc_conv_ring(h->F, g.gw), h->nb_main); if (h->nb_side >= 2 && h->main_stream && st != h->main_stream && a.nb > h->nb_side) a.nb = h->nb_side; { const char* tl = getenv("MAML_B200_TC_TIMELINE"); a.timeline = (tl && (atoi(tl) <= 0 || atoi(tl) == l)) ? 1 : 0; }
+  const bool side = on_side_stream(st);
+  a.split_cap = side ? h->opt.tc_split_side : 0;
+  a.halo = g.gw + 1; a.rpad = tc_conv_rpad(g.gw); a.nb = std::min(tc_conv_ring(h->F, g.gw), h->nb_main);
+  if (side && h->opt.tc_nb_side >= 2 && a.nb > h->opt.tc_nb_side) a.nb = h->opt.tc_nb_side;
+  a.timeline = (h->opt.tc_timeline == 0 || h->opt.tc_timeline == l) ? 1 : 0;
   for (int s = 0; s < nsrc; ++s) {
     maps.m[s * 4 + 0] = ops[s].a_maps[0]; maps.m[s * 4 + 1] = ops[s].a_maps[1];
     maps.m[s * 4 + 2] = ops[s].b_maps[ops[s].b_pair]; maps.m[s * 4 + 3] = ops[s].b_maps[ops[s].b_pair + 1];
@@ -627,8 +632,6 @@ static void tc_conv(maml_b200_handle* h, int l, int n, int nsrc, const TcOp* ops
 // primal forward of one pass: conv -> stats -> BN/leaky/pool for every block
 static void forward_pass(maml_b200_handle* h, const PassSet& ps, int slot, const float* theta, int th_step, const float* meta,
                          int bn_step, int stat_kind, int T, cudaStream_t st, BnActArgs* defer_last = nullptr) {
-  struct CapScope { CapScope(int v) { g_bn_cta_cap = v; } ~CapScope() { g_bn_cta_cap = 0; } }
-      cap_scope((h->main_stream && st != h->main_stream) ? h->side_bn_cap : 0);
   for (int l = 0; l < h->L; ++l) {
     const LayerGeom& g = h->geo[l];
     if (l == 1 && st != h->s_tgt && st != h->s_tgt2) join_pending(h, st);
@@ -678,11 +681,8 @@ static void backward_pass(maml_b200_handle* h, const PassSet& ps, int slot, cons
   // wgrad of block l >= 1 only feeds the parameter-space reduction: it runs on a side stream, concurrently with
   // dgrad(l) and the BatchNorm backward of block l-1.  With a ReduceSpec the reduction itself is split (see
   // reduce_upper_on_side); without one the caller reduces after this function returns.
-  struct CapScope { CapScope(int v) { g_bn_cta_cap = v; } ~CapScope() { g_bn_cta_cap = 0; } }
-      cap_scope((h->main_stream && st != h->main_stream) ? h->side_bn_cap : 0);
   cudaStream_t wst = fork_wgrad ? h->s_wg : st;
   const bool split = fork_wgrad && rs != nullptr;
-  bool lower_fused = false;
   for (int l = h->L - 1; l >= 0; --l) {
     const LayerGeom& g = h->geo[l];
     BnBwdArgs b{};
@@ -709,8 +709,6 @@ static void backward_pass(maml_b200_handle* h, const PassSet& ps, int slot, cons
       w.A[0] = ps.xg; w.a_stride[0] = ps.xg_stride; w.kc = h->C;
       w.alg_flops = conv_flops(h, 0, ps.n, T, 1);
       if (split && h->L == 1) reduce_upper_on_side(h, *rs, cp.pd, partial, meta, T);
-      w.fr.mode = -1;
-      if (split) lower_fused = fuse_lower_into_wgrad0(h, *rs, meta, w);
       launch_wgrad0(w, split ? st : wst);
     } else {
       w.A[0] = AIN(ps, l, slot); w.a_stride[0] = STRIDE(ps, ain, l); w.kc = h->F;
@@ -729,7 +727,7 @@ static void backward_pass(maml_b200_handle* h, const PassSet& ps, int slot, cons
         a.alg_flops = conv_flops(h, l, ps.n, T, 1);
         launch_conv_rows(a, st);
       }
-      if (h->use_tc && h->wgrad_tc) {
+      if (h->use_tc && h->opt.wgrad_tc) {
         w.a_plane[0] = ps.ain_plane[l]; w.d_plane[0] = ps.dz_plane[l];
         launch_wgrad_tc(w, wst);
       } else {
@@ -738,8 +736,8 @@ static void backward_pass(maml_b200_handle* h, const PassSet& ps, int slot, cons
       if (split && l == 1) reduce_upper_on_side(h, *rs, cp.pd, partial, meta, T);
     }
   }
-  if (split && !lower_fused) reduce_lower(h, *rs, cp.pd, partial, meta, T, st);
-  else if (fork_wgrad && !split) { cudaEventRecord(h->ev_wg, h->s_wg); cudaStreamWaitEvent(st, h->ev_wg, 0); }
+  if (split) reduce_lower(h, *rs, cp.pd, partial, meta, T, st);
+  else if (fork_wgrad) { cudaEventRecord(h->ev_wg, h->s_wg); cudaStreamWaitEvent(st, h->ev_wg, 0); }
 }
 
 // forward-mode tangent of (support forward + support backward) at step s in direction u  =>  H u into `partial`
@@ -751,8 +749,8 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
   // u packs) into the tan2 buffers -- BatchNorm statistics contributions included, they are linear -- and the
   // consumers (bnact_tan / bnbwd_tan) add the two addends.  The main chain keeps the single-pair half: 18 instead of
   // 36 stages per tile on the critical path.
-  const bool split = h->use_tc && h->tan_split;
-  const bool fuse_tail = h->tail_fuse && tail_fusable(bn_geom(h, h->L - 1, sp.n), sp.n, head_rows(sp.n));
+  const bool split = h->use_tc && h->opt.tan_split;
+  const bool fuse_tail = h->opt.tail_fuse && tail_fusable(bn_geom(h, h->L - 1, sp.n), sp.n, head_rows(sp.n));
   BnActTanArgs last_act{};
   HeadArgs hd{};
   if (split) {
@@ -822,7 +820,6 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
     else launch_bnact_tan(b, st);
   }
   const ChunkPlan& cp = h->plan_sup;
-  bool lower_fused = false;
   join_pending(h, st);
   {
     HeadArgs& a = hd;
@@ -870,7 +867,6 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
       w.A[0] = sp.xg; w.a_stride[0] = sp.xg_stride; w.kc = h->C;
       w.alg_flops = conv_flops(h, 0, sp.n, T, 1);
       if (h->L == 1) reduce_upper_on_side(h, rs, cp.pd, h->sup_partial, meta, T);
-      lower_fused = fuse_lower_into_wgrad0(h, rs, meta, w);
       launch_wgrad0(w, st);
     } else {
       w.nsrc = 2;
@@ -898,7 +894,7 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
         a.alg_flops = conv_flops(h, l, sp.n, T, 2);
         launch_conv_rows(a, st);
       }
-      if (h->use_tc && h->wgrad_tc) {
+      if (h->use_tc && h->opt.wgrad_tc) {
         w.a_plane[0] = sp.ain_plane[l]; w.d_plane[0] = tn.dz_plane[l];
         w.a_plane[1] = tn.ain_plane[l]; w.d_plane[1] = sp.dz_plane[l];
         launch_wgrad_tc(w, h->s_wg);
@@ -908,7 +904,7 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
       if (l == 1) reduce_upper_on_side(h, rs, cp.pd, h->sup_partial, meta, T);
     }
   }
-  if (!lower_fused) reduce_lower(h, rs, cp.pd, h->sup_partial, meta, T, st);
+  reduce_lower(h, rs, cp.pd, h->sup_partial, meta, T, st);
 }
 
 static void pack_theta_step(maml_b200_handle* h, int step, int T, cudaStream_t st) {
@@ -927,14 +923,14 @@ static int enqueue_iteration(maml_b200_handle* h, const maml_b200_iter_args* it,
                              const long long* ys, const float* x_target, const long long* yt, float* result, float* last_logits,
                              cudaStream_t st) {
   g_launch_base = g_launch_counter;      // launch tags (device trace) count from the start of the iteration
-  h->main_stream = st; g_pdl_main_stream = st; g_pdl_wg_stream = h->s_wg; g_use_pdl = h->pdl_mode; g_pdl_cluster = h->pdl_cluster;
+  LaunchScope launch_scope(h, st);
   const int T = it->n_tasks;
   const unsigned mask = it->target_mask & ((1u << it->num_steps) - 1u);
   const long long TP = (long long)h->maxT * h->Ppad;
   // diagnostic (MAML_B200_ONE_STREAM=1): everything on one stream -> the device trace shows true kernel durations
   struct StreamSwap {
     maml_b200_handle* h; cudaStream_t tgt, tgt2, wg; bool on;
-    StreamSwap(maml_b200_handle* h_, cudaStream_t st) : h(h_), tgt(h_->s_tgt), tgt2(h_->s_tgt2), wg(h_->s_wg), on(getenv("MAML_B200_ONE_STREAM") != nullptr) {
+    StreamSwap(maml_b200_handle* h_, cudaStream_t st) : h(h_), tgt(h_->s_tgt), tgt2(h_->s_tgt2), wg(h_->s_wg), on(h_->opt.one_stream) {
       if (on) { h->s_tgt = st; h->s_tgt2 = st; h->s_wg = st; }
     }
     ~StreamSwap() { if (on) { h->s_tgt = tgt; h->s_tgt2 = tgt2; h->s_wg = wg; } }
@@ -964,7 +960,7 @@ static int enqueue_iteration(maml_b200_handle* h, const maml_b200_iter_args* it,
   for (int s = 0; s < it->num_steps; ++s) {
     const float* th = h->theta + (long long)s * TP;
     float* th_next = h->theta + (long long)(s + 1) * TP;
-    const bool fuse_tail = h->tail_fuse && tail_fusable(bn_geom(h, h->L - 1, h->n_s), h->n_s, head_rows(h->n_s));
+    const bool fuse_tail = h->opt.tail_fuse && tail_fusable(bn_geom(h, h->L - 1, h->n_s), h->n_s, head_rows(h->n_s));
     BnActArgs last_act{};
     forward_pass(h, h->sup, s, th, s, meta, s, PASS_SUP_FWD, T, st, fuse_tail ? &last_act : nullptr);
     join_pending(h, st);
@@ -1041,7 +1037,7 @@ static int enqueue_iteration(maml_b200_handle* h, const maml_b200_iter_args* it,
         // while the main chain runs block 0
         // ... on a target stream (idle in phase B) when the u-weight convs are pre-computed there too, so that they do
         // not queue in front of the weight gradients on the wgrad stream
-        cudaStream_t spre = (h->use_tc && h->tan_split && !getenv("MAML_B200_PRE_ON_WG")) ? h->s_tgt : h->s_wg;
+        cudaStream_t spre = (h->use_tc && h->opt.tan_split) ? h->s_tgt : h->s_wg;
         CK(cudaEventRecord(h->ev_fork, st));
         CK(cudaStreamWaitEvent(spre, h->ev_fork, 0));
         pack_u(h, T, spre);
@@ -1093,7 +1089,7 @@ extern "C" int maml_b200_meta_batch_fwd_bwd(maml_b200_handle* h, const maml_b200
   const long long* yt = (const long long*)y_target;
   h->last_tasks = T;
 
-  if (!h->use_graphs || g_prof) {
+  if (!h->use_graphs || h->profiling) {
     // eager: launches go straight to the caller's stream (side streams fork / join through events)
     const long long launches0 = g_launch_counter;
     if (enqueue_iteration(h, it, meta, x_support, ys, x_target, yt, result, last_logits, st)) return 1;
@@ -1121,7 +1117,7 @@ extern "C" int maml_b200_meta_batch_fwd_bwd(maml_b200_handle* h, const maml_b200
     cudaError_t e = cudaStreamEndCapture(h->s_cap, &graph);
     if (rc) { if (graph) cudaGraphDestroy(graph); return 1; }
     if (e != cudaSuccess) return fail(std::string("cudaStreamEndCapture: ") + cudaGetErrorString(e));
-    if (const char* dot = getenv("MAML_B200_GRAPH_DOT")) cudaGraphDebugDotPrint(graph, dot, cudaGraphDebugDotFlagsKernelNodeParams);
+    if (!h->opt.graph_dot.empty()) cudaGraphDebugDotPrint(graph, h->opt.graph_dot.c_str(), cudaGraphDebugDotFlagsKernelNodeParams);
     maml_b200_handle::GraphEntry ge;
     ge.it = *it; memcpy(ge.p, ptrs, sizeof(ptrs)); ge.exec = nullptr; ge.launches = g_launch_counter - launches0; ge.stamp = 0;
     e = cudaGraphInstantiate(&ge.exec, graph, 0);
@@ -1146,7 +1142,7 @@ extern "C" int maml_b200_net_forward(maml_b200_handle* h, int32_t n_tasks, int32
   if (n_tasks < 1 || n_tasks > h->maxT) return fail("n_tasks out of range");
   if (num_step < 0 || num_step >= h->S) return fail("num_step out of range");
   cudaStream_t st = (cudaStream_t)stream;
-  h->main_stream = st; g_pdl_main_stream = st; g_use_pdl = h->pdl_mode; g_pdl_cluster = h->pdl_cluster;
+  LaunchScope launch_scope(h, st);
   const int T = n_tasks;
   CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
   CK(cudaMemsetAsync(h->losses, 0, (size_t)h->maxT * MAML_MAX_STEPS * sizeof(float), st));
@@ -1180,7 +1176,7 @@ extern "C" int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int3
   if (n_tasks < 1 || n_tasks > h->maxT) return fail("n_tasks out of range");
   if (num_step < 0 || num_step >= h->S) return fail("num_step out of range");
   cudaStream_t st = (cudaStream_t)stream;
-  h->main_stream = st; g_pdl_main_stream = st; g_use_pdl = h->pdl_mode; g_pdl_cluster = h->pdl_cluster;
+  LaunchScope launch_scope(h, st);
   const int T = n_tasks;
   // backward statistics (and the tangent ones export subtracts) start from zero; forward statistics are kept
   for (int kind : {PASS_TGT_BWD, PASS_TAN_BWD})
@@ -1230,6 +1226,7 @@ extern "C" int maml_b200_net_running_update(maml_b200_handle* h, int32_t n_tasks
   if (n_tasks < 1 || n_tasks > h->maxT) return fail("n_tasks out of range");
   if (num_step < 0 || num_step >= h->S) return fail("num_step out of range");
   if (!h->cfg.per_step_bn) return 0;
+  LaunchScope launch_scope(h);
   int hw[MAML_MAX_LAYERS];
   for (int l = 0; l < h->L; ++l) hw[l] = h->geo[l].h * h->geo[l].w;
   launch_running_ema_from_stats(stat_at(h, PASS_TGT_FWD, num_step, 0), h->stats_task_stride, h->st_layer_stride, n_tasks, running_mean,
@@ -1242,6 +1239,7 @@ extern "C" int maml_b200_adam_step(maml_b200_handle* h, float* meta, const float
                                    float lr, int32_t step, uint32_t trainable_mask, uint32_t clamp_mask, void* stream) {
   if (!h || !meta || !grad || !exp_avg || !exp_avg_sq) return fail("null argument");
   if (step < 1) return fail("step must be >= 1");
+  LaunchScope launch_scope(h);
   std::vector<long long> ends;
   for (size_t k = 0; k < h->seg_off.size(); ++k) ends.push_back(h->seg_off[k] + h->seg_size[k]);
   const float bc1 = (float)(1.0 - pow(0.9, (double)step));
@@ -1256,6 +1254,7 @@ extern "C" int maml_b200_running_stats_update(maml_b200_handle* h, const float* 
                                               const float* decay_host, void* stream) {
   if (!h || !result || !running_mean || !running_var || !decay_host) return fail("null argument");
   if (!h->cfg.per_step_bn) return 0;    // shared-BN mode passes running stats = None in the reference: no update
+  LaunchScope launch_scope(h);
   cudaStream_t st = (cudaStream_t)stream;
   float* pin = h->pinned + 32 * (h->pin_slot++ & 15);
   for (int s = 0; s < h->S; ++s) pin[s] = decay_host[s];
@@ -1331,6 +1330,7 @@ extern "C" int maml_b200_all_reduce(maml_b200_handle* h, float* vec, void* strea
   if (!h || !vec) return fail("null argument");
   if (!h->comm_connected) return fail("all_reduce: communicator not connected");
   if ((reinterpret_cast<uintptr_t>(vec) & 15u) != 0) return fail("all_reduce: vector must be 16-byte aligned");
+  LaunchScope launch_scope(h);
   cudaStream_t st = (cudaStream_t)stream;
   launch_publish(h->comm, vec, maml_b200_result_size(h), st);
   launch_allreduce(h->comm, vec, maml_b200_result_size(h), st);
@@ -1364,7 +1364,8 @@ extern "C" int maml_b200_episode_gather(const float* dataset, const int64_t* ima
 
 extern "C" int maml_b200_profile(maml_b200_handle* h, int32_t enable) {
   if (!h) return fail("null argument");
-  if (enable) { h->prof.reset(); g_prof = &h->prof; } else { g_prof = nullptr; }
+  if (enable) h->prof.reset();
+  h->profiling = enable != 0;
   return 0;
 }
 

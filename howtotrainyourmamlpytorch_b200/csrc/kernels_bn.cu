@@ -110,24 +110,24 @@ __global__ void __launch_bounds__(256) bnact_kernel(BnActArgs a) {
   bnact_phase(a, g, task, blockIdx.x, gridDim.x, it, s_mu, s_r, s_g, s_b);
 }
 
-// > 0: launches enqueued right now sit on a side stream (target passes): at most this many CTAs per launch, so that the
-// grid-stride BatchNorm kernels leave SM slots to the main chain (set by the engine around side-stream passes)
-int g_bn_cta_cap = 0;
-static inline dim3 bn_grid(const BnGeom& g, int tasks, int* block) {
+// launches on a side stream (target passes) take at most the BN_SIDE_CAP option's CTAs, so that the grid-stride
+// BatchNorm kernels can leave SM slots to the main chain
+static inline dim3 bn_grid(const BnGeom& g, int tasks, int* block, cudaStream_t st) {
   const int F4 = g.F / 4;
   const int wpb = 256 / F4;
   *block = wpb * F4;
   const int NW = g.n * ((g.h + 1) / 2) * ((g.w + 1) / 2);
   int bx = (NW + wpb - 1) / wpb;
   if (bx > 4 * num_sms()) bx = 4 * num_sms();
-  if (g_bn_cta_cap > 0 && (long long)bx * tasks > g_bn_cta_cap) bx = g_bn_cta_cap / tasks;
+  const int cap = on_side_stream(st) ? launch_ctx().opt->bn_side_cap : 0;
+  if (cap > 0 && (long long)bx * tasks > cap) bx = cap / tasks;
   if (bx < 1) bx = 1;
   return dim3(bx, tasks);
 }
 
 void launch_bnact(const BnActArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
+  int block; dim3 grid = bn_grid(a.g, a.tasks, &block, st);
   launch_pdl(bnact_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();
 }
@@ -278,7 +278,7 @@ __global__ void __launch_bounds__(256) bnbwd_reduce_kernel(BnBwdArgs a) {
 
 void launch_bnbwd_reduce(const BnBwdArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
+  int block; dim3 grid = bn_grid(a.g, a.tasks, &block, st);
   if ((int)grid.x > num_sms()) grid.x = num_sms();
   launch_pdl(bnbwd_reduce_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();
@@ -369,14 +369,14 @@ __global__ void __launch_bounds__(256) bnbwd_fused_kernel(BnBwdArgs a) {
   bnbwd_apply_phase(a, g, task, blockIdx.x, gridDim.x, it, s_r, s_g, s_b, s_c1, s_c2);
 }
 
-// cluster size for the fused kernels: enough CTAs for <= 4 windows per thread, else 0 (two-kernel path)
-static int g_bn_fuse_max = 32;       // env MAML_B200_BN_FUSE_MAX: largest "CTAs needed at one window per thread" still fused
-void bn_set_fuse_max(int v) { g_bn_fuse_max = v; }
+// cluster size for the fused kernels: enough CTAs for <= 4 windows per thread, else 0 (two-kernel path: the block needs
+// more than 32 CTAs at one window per thread, or the handle's BN_FUSE option is off)
 static inline int bn_fused_cluster(const BnGeom& g) {
+  if (!launch_ctx().opt->bn_fuse) return 0;
   const int F4 = g.F / 4, wpb = 256 / F4;
   const int NW = g.n * ((g.h + 1) / 2) * ((g.w + 1) / 2);
   const int need = (NW + wpb - 1) / wpb;
-  if (need > g_bn_fuse_max) return 0;
+  if (need > 32) return 0;
   int cl = 1;
   while (cl < need && cl < 8) cl <<= 1;
   return cl;
@@ -390,25 +390,23 @@ static inline void launch_cluster(void (*kernel)(A), const A& a, int cl, int tas
   attr[0].val.clusterDim.x = cl; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
   attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = ((g_pdl_cluster & 1) && pdl_allowed(st)) ? 2 : 1;
+  cfg.attrs = attr; cfg.numAttrs = ((launch_ctx().opt->pdl_cluster & 1) && pdl_allowed(st)) ? 2 : 1;
   cudaLaunchKernelEx(&cfg, kernel, a);
 }
-static int g_bn_fuse = 1;            // env MAML_B200_BN_FUSE=0 -> always the two-kernel path
-void bn_set_fuse(int on) { g_bn_fuse = on; }
 
 // BatchNorm backward of one block (reduce + apply), fused into one cluster kernel when the block is small
 void launch_bnbwd(const BnBwdArgs& a, cudaStream_t st) {
-  const int cl = g_bn_fuse ? bn_fused_cluster(a.g) : 0;
+  const int cl = bn_fused_cluster(a.g);
   if (cl == 0) { launch_bnbwd_reduce(a, st); launch_bnbwd_apply(a, st); return; }
   ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; bn_grid(a.g, a.tasks, &block);
+  int block; bn_grid(a.g, a.tasks, &block, st);
   launch_cluster(bnbwd_fused_kernel, tagged(a), cl, a.tasks, block, st);
   CUDA_CHECK_LAUNCH();
 }
 
 void launch_bnbwd_apply(const BnBwdArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
+  int block; dim3 grid = bn_grid(a.g, a.tasks, &block, st);
   launch_pdl(bnbwd_apply_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();
 }
@@ -486,7 +484,7 @@ __global__ void __launch_bounds__(256) bnact_tan_kernel(BnActTanArgs a) {
 
 void launch_bnact_tan(const BnActTanArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
+  int block; dim3 grid = bn_grid(a.g, a.tasks, &block, st);
   launch_pdl(bnact_tan_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();
 }
@@ -546,7 +544,7 @@ __global__ void __launch_bounds__(256) bnbwd_tan_reduce_kernel(BnBwdTanArgs a) {
 
 void launch_bnbwd_tan_reduce(const BnBwdTanArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
+  int block; dim3 grid = bn_grid(a.g, a.tasks, &block, st);
   if ((int)grid.x > num_sms()) grid.x = num_sms();
   launch_pdl(bnbwd_tan_reduce_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();
@@ -651,16 +649,16 @@ __global__ void __launch_bounds__(256) bnbwd_tan_fused_kernel(BnBwdTanArgs a) {
 
 void launch_bnbwd_tan_apply(const BnBwdTanArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
+  int block; dim3 grid = bn_grid(a.g, a.tasks, &block, st);
   launch_pdl(bnbwd_tan_apply_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();
 }
 
 void launch_bnbwd_tan(const BnBwdTanArgs& a, cudaStream_t st) {
-  const int cl = g_bn_fuse ? bn_fused_cluster(a.g) : 0;
+  const int cl = bn_fused_cluster(a.g);
   if (cl == 0) { launch_bnbwd_tan_reduce(a, st); launch_bnbwd_tan_apply(a, st); return; }
   ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; bn_grid(a.g, a.tasks, &block);
+  int block; bn_grid(a.g, a.tasks, &block, st);
   launch_cluster(bnbwd_tan_fused_kernel, tagged(a), cl, a.tasks, block, st);
   CUDA_CHECK_LAUNCH();
 }
@@ -1042,14 +1040,11 @@ __global__ void __launch_bounds__(256) tail_tan_onchip_kernel(BnActTanArgs fa, H
   }
 }
 
-static int g_tail_onchip = 3;          // env MAML_B200_TAIL_ONCHIP: bit 0 primal, bit 1 tangent on-chip kernels (0: stages exchange data through L2)
-void tail_set_onchip(int on) { g_tail_onchip = on; }
-
 // the last block of `n` images is small enough for the fused kernels
 bool tail_fusable(const BnGeom& g, int n_rows, int rows_per_cta) {
   const int F4 = g.F / 4, wpb = 256 / F4;
   const int NW = g.n * ((g.h + 1) / 2) * ((g.w + 1) / 2);
-  return g_bn_fuse && g.F <= 64 && n_rows <= rows_per_cta && NW <= 4 * wpb;
+  return launch_ctx().opt->bn_fuse && g.F <= 64 && n_rows <= rows_per_cta && NW <= 4 * wpb;
 }
 
 void launch_tail_fused(const BnActArgs& fa, const HeadArgs& ha, const BnBwdArgs& ba, cudaStream_t st) {
@@ -1058,7 +1053,7 @@ void launch_tail_fused(const BnActArgs& fa, const HeadArgs& ha, const BnBwdArgs&
     const int F4 = fa.g.F / 4, wpb = 256 / F4;
     const int NW = fa.g.n * ((fa.g.h + 1) / 2) * ((fa.g.w + 1) / 2);
     const size_t words = (size_t)5 * ha.rows_per_cta * ha.N + 2 * (size_t)ha.n * ha.D + (size_t)ha.N * ha.D + ha.N;
-    if ((g_tail_onchip & 1) && fa.g.pb == 0 && fa.p_hi == nullptr && NW <= 2 * wpb && words * sizeof(float) <= 40 * 1024) {
+    if ((launch_ctx().opt->tail_onchip & 1) && fa.g.pb == 0 && fa.p_hi == nullptr && NW <= 2 * wpb && words * sizeof(float) <= 40 * 1024) {
       if (NW <= wpb) launch_pdl(tail_onchip_kernel<1>, dim3(1, fa.tasks), dim3(256), words * sizeof(float), st, tagged(fa), ha, ba);
       else launch_pdl(tail_onchip_kernel<2>, dim3(1, fa.tasks), dim3(256), words * sizeof(float), st, tagged(fa), ha, ba);
       CUDA_CHECK_LAUNCH();
@@ -1076,7 +1071,7 @@ void launch_tail_tan_fused(const BnActTanArgs& fa, const HeadArgs& ha, const BnB
     const int F4 = fa.g.F / 4, wpb = 256 / F4;
     const int NW = fa.g.n * ((fa.g.h + 1) / 2) * ((fa.g.w + 1) / 2);
     const size_t words = (size_t)5 * ha.rows_per_cta * ha.N + 3 * (size_t)ha.n * ha.D + 2 * (size_t)ha.N * ha.D + 2 * ha.N;
-    if ((g_tail_onchip & 2) && fa.g.pb == 0 && fa.pdot_hi == nullptr && ba.dpdot2 == nullptr && NW <= 2 * wpb && words * sizeof(float) <= 40 * 1024) {
+    if ((launch_ctx().opt->tail_onchip & 2) && fa.g.pb == 0 && fa.pdot_hi == nullptr && ba.dpdot2 == nullptr && NW <= 2 * wpb && words * sizeof(float) <= 40 * 1024) {
       if (NW <= wpb) launch_pdl(tail_tan_onchip_kernel<1>, dim3(1, fa.tasks), dim3(256), words * sizeof(float), st, tagged(fa), ha, ba);
       else launch_pdl(tail_tan_onchip_kernel<2>, dim3(1, fa.tasks), dim3(256), words * sizeof(float), st, tagged(fa), ha, ba);
       CUDA_CHECK_LAUNCH();

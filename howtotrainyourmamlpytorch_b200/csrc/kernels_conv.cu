@@ -11,11 +11,7 @@
 
 long long g_launch_counter = 0;
 long long g_launch_base = 0;
-int g_use_pdl = 0;
-cudaStream_t g_pdl_main_stream = nullptr, g_pdl_wg_stream = nullptr;
-int g_launch_prio = 0;
 int g_trace_flag = 0;
-int g_pdl_cluster = 1;
 
 __device__ __forceinline__ int tap_shift(int tap, int gw) { return (tap / 3 - 1) * gw + (tap % 3 - 1); }
 
@@ -386,9 +382,6 @@ __global__ void __launch_bounds__(256) conv0_rb_kernel(Conv0Args a, int tiles) {
   }
 }
 
-static int g_conv0_rb = 1;               // env MAML_B200_CONV0_RB=0 -> the 64-row kernel
-void conv0_set_rb(int on) { g_conv0_rb = on; }
-
 template <int C0>
 static bool launch_conv0_rb(const Conv0Args& a, cudaStream_t st) {
   // tiles per CTA: as many as keep >= ~3 CTAs per SM in flight (fixed per-CTA cost -- weights, window, fp64 statistics
@@ -408,7 +401,7 @@ static bool launch_conv0_rb(const Conv0Args& a, cudaStream_t st) {
 
 void launch_conv0(const Conv0Args& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_CONV0, a.alg_flops, st);
-  if (g_conv0_rb && (a.c0 == 1 || a.c0 == 3)) {
+  if (a.c0 == 1 || a.c0 == 3) {
     if (a.c0 == 1) launch_conv0_rb<1>(a, st); else launch_conv0_rb<3>(a, st);
     CUDA_CHECK_LAUNCH();
     return;
@@ -628,13 +621,10 @@ __global__ void __launch_bounds__(256) wgrad_row_kernel(WgradArgs a) {
   if (ky == 1 && tid < NC) P[(long long)9 * KC * NC + tid] = bacc;
 }
 
-static int g_wgrad_rows3 = 1;            // env MAML_B200_WGRAD_ROW=0 -> one tap per CTA
-void wgrad_set_row_variant(int on) { g_wgrad_rows3 = on; }
-
 void launch_wgrad(const WgradArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_WGRAD, a.alg_flops, st);
   const int cn = a.kc / 16, fn = a.ncols / 16;
-  if (g_wgrad_rows3) {
+  if (launch_ctx().opt->wgrad_row) {
     dim3 grid(a.nchunks * 3, a.tasks);
 #define WGR_CASE(C, F_) if (cn == C && fn == F_) { launch_pdl(wgrad_row_kernel<C, F_>, dim3(grid), dim3(256), (size_t)(0), st, tagged(a)); CUDA_CHECK_LAUNCH(); return; }
     WGR_CASE(1, 1) WGR_CASE(2, 2) WGR_CASE(3, 3) WGR_CASE(4, 4)
@@ -723,8 +713,9 @@ __global__ void __launch_bounds__(256) wgrad0_kernel(WgradArgs a) {
 // The CTA's threads form NS "row streams" of 3 * F/4 threads; a stream walks CONSECUTIVE rows of the staged tile, so the
 // three x positions of a row slide by one per row: per row C0 broadcast loads + one LDS.128 of dz feed 12 * C0 FMAs
 // (wgrad0_kernel: 7 loads per 6 FMAs).  Streams are summed through shared memory in stream order (deterministic).
+// C0 = 1 is held to 48 registers (5 CTAs per SM); left to itself ptxas gives it 58 (4 CTAs).  0: no bound for C0 = 3.
 template <int C0>
-__global__ void __launch_bounds__(256) wgrad0_rb_kernel(WgradArgs a) {
+__global__ void __launch_bounds__(256, C0 == 1 ? 5 : 0) wgrad0_rb_kernel(WgradArgs a) {
   pdl_prologue(4, a.tag);
   extern __shared__ float smw[];
   const int task = blockIdx.y, chunk = blockIdx.x;
@@ -817,44 +808,12 @@ __global__ void __launch_bounds__(256) wgrad0_rb_kernel(WgradArgs a) {
     for (int st = 0; st < NS; ++st) t += red[(long long)st * (ncombo + 1) * Fc + i];
     P[i] = t;
   }
-  if (a.fr.mode < 0) return;
-  // fused parameter-space reduction: the last CTA of this task sums the chunks in order and applies the update
-  __shared__ unsigned s_last;
-  __threadfence();
-  __syncthreads();
-  if (tid == 0) {
-    const unsigned done = atomicAdd(&a.fr.counters[task], 1u);
-    s_last = (done == gridDim.x - 1) ? 1u : 0u;
-    if (s_last) a.fr.counters[task] = 0;
-  }
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
-  const float* P0 = a.partial + (long long)task * a.partial_task_stride;
-  const int nw = ncombo * Fc;                       // internal fast-weight index: [W_0 (tap, c, f) | b_0 (f)] starts at 0
-  for (int i = tid; i < nw + Fc; i += 256) {
-    float sum = 0.f;
-    for (int ch = 0; ch < a.nchunks; ++ch) sum += __ldcg(P0 + (long long)ch * a.chunk_stride + i);
-    const long long o = (long long)task * a.fr.task_stride + i;
-    if (a.fr.mode == PR_UPDATE) {
-      const float alpha = a.fr.alpha[(i < nw ? 0 : 1) * a.fr.alpha_stride];
-      a.fr.g_out[o] = sum;
-      a.fr.theta_out[o] = a.fr.theta_in[o] - alpha * sum;
-    } else {
-      a.fr.tbar[o] -= sum;
-    }
-  }
 }
-
-static int g_wgrad0_rb = 1;              // env MAML_B200_WGRAD0_RB=0 -> wgrad0_kernel
-void wgrad0_set_rb(int on) { g_wgrad0_rb = on; }
-
-bool wgrad0_can_fuse_reduce(int kc, int ncols, int nsrc) { return g_wgrad0_rb && (kc == 1 || kc == 3) && nsrc == 1 && (ncols % 4) == 0; }
 
 void launch_wgrad0(const WgradArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_WGRAD0, a.alg_flops, st);
   dim3 grid(a.nchunks, a.tasks);
-  if (g_wgrad0_rb && (a.kc == 1 || a.kc == 3) && a.nsrc == 1 && (a.ncols % 4) == 0) {
+  if ((a.kc == 1 || a.kc == 3) && a.nsrc == 1 && (a.ncols % 4) == 0) {
     const int tps = 3 * (a.ncols / 4), ns = 256 / tps, rt = ns * 16;
     const size_t stage = (size_t)(rt * a.ncols + (rt + 2 * (a.gw + 1)) * a.kc) * sizeof(float);
     const size_t red = (size_t)ns * (9 * a.kc + 1) * a.ncols * sizeof(float);

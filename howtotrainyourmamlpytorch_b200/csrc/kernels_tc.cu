@@ -683,14 +683,13 @@ void launch_wgrad_tc(const WgradArgs& a, cudaStream_t st) {
   CUDA_CHECK_LAUNCH();
 }
 
-// halo tile rows (multiple of 8) for a grid of pitch gw, and the deepest B ring that fits next to 4 halo buffers
+// halo tile rows (multiple of 8) for a grid of pitch gw, and the deepest B ring (at most 8 stages) that fits next to 4
+// halo buffers
 int tc_conv_rpad(int gw) { return ((128 + 2 * (gw + 1)) + 7) / 8 * 8; }
-static int g_tc_ring_cap = 8;         // env MAML_B200_TC_NB: B ring depth cap (a shallower ring leaves shared memory to co-resident kernels)
-void tc_conv_set_ring_cap(int nb) { g_tc_ring_cap = nb < 2 ? 2 : (nb > 8 ? 8 : nb); }
 int tc_conv_ring(int ncols, int gw) {
   const long long avail = 227LL * 1024 - 4096 /* static smem */ - 1024 /* alignment */ - 4LL * tc_conv_rpad(gw) * 128;
   long long nb = avail / (2LL * ncols * 128);
-  if (nb > g_tc_ring_cap) nb = g_tc_ring_cap;
+  if (nb > 8) nb = 8;
   return (int)nb;
 }
 size_t tc_conv_smem_bytes(int ncols, int gw) {
@@ -710,14 +709,8 @@ int tc_conv_prepare() {
 // Split-K factor: small layers have fewer tiles than SMs (Omniglot block 3: 8 tiles, block 2: 32), and one tile's
 // serial pipeline (~18 stages x ~1000 cycles) is then the whole kernel.  Spreading the (phase, tap) stages of a tile
 // over a cluster of S CTAs shortens that to 18 / S stages + one distributed-shared-memory reduction.  S is the largest
-// of {8, 4, 2} whose clusters are all co-resident (asked from the occupancy calculator once per shape).
-static int g_tc_zstage = 1;          // env MAML_B200_TC_ZSTAGE=0: tangent-mode statistics read the primal zh from global memory row by row
-void tc_conv_set_zstage(int on) { g_tc_zstage = on; }
-static int g_tc_push = 1;            // env MAML_B200_TC_PUSH=0: pull-based split-K reduction (two cluster barriers)
-void tc_conv_set_push(int on) { g_tc_push = on; }
-static int g_tc_ring_fit = 1;        // env MAML_B200_TC_NB_FIT=0: keep the full ring for short pipelines
-void tc_conv_set_ring_fit(int on) { g_tc_ring_fit = on; }
-static int g_tc_split_max = 8;       // env MAML_B200_TC_SPLIT (1 disables split-K)
+// of {8, 4, 2} (at most the handle's TC_SPLIT option) whose clusters are all co-resident (asked from the occupancy
+// calculator once per shape).
 template <int NCOLS>
 static int max_clusters(size_t smem, int S) {
   static std::map<std::pair<size_t, int>, int> cache;
@@ -738,6 +731,7 @@ static int max_clusters(size_t smem, int S) {
 template <int NCOLS>
 static void launch_conv_tc_n(const TcMaps& maps, const TcConvArgs& a_in, size_t smem, cudaStream_t st) {
   TcConvArgs a = a_in;
+  const EngineOptions& opt = *launch_ctx().opt;
   const int tiles = ((a.rows + 127) / 128) * (a.plan_tasks > a.tasks ? a.plan_tasks : a.tasks);
   const int stages = a.nsrc * ((a.kc + 31) / 32) * 9;
   int S = 1;
@@ -750,9 +744,9 @@ static void launch_conv_tc_n(const TcMaps& maps, const TcConvArgs& a_in, size_t 
     const long long fit = avail / (2LL * NCOLS * 128);
     if (fit < nb_push) nb_push = (int)fit;
   }
-  const bool push = g_tc_push && nb_push >= 2;
+  const bool push = opt.tc_push && nb_push >= 2;
   if (push) smem = tc_conv_smem_for(NCOLS, a.gw, nb_push) + recv_bytes;
-  int smax = g_tc_split_max;
+  int smax = opt.tc_split;
   if (a.split_cap > 0 && a.split_cap < smax) { smax = 1; while (smax * 2 <= a.split_cap) smax *= 2; }
   for (int cand = smax; cand >= 2; cand >>= 1) {
     if (cand > 8 || stages < 2 * cand) continue;
@@ -761,7 +755,7 @@ static void launch_conv_tc_n(const TcMaps& maps, const TcConvArgs& a_in, size_t 
   dim3 grid((a.rows + 127) / 128, a.tasks, S);
   // a CTA never has more than ceil(stages / S) B stages in flight: a ring deeper than that only takes shared memory
   // away from the kernels of the other streams that could share the SM (block-0 / BatchNorm kernels need 10-27 KB)
-  if (g_tc_ring_fit) {
+  if (opt.tc_nb_fit) {
     const int per_cta = (stages + S - 1) / S;
     if (a.nb > per_cta) a.nb = per_cta < 2 ? 2 : per_cta;
   }
@@ -770,7 +764,7 @@ static void launch_conv_tc_n(const TcMaps& maps, const TcConvArgs& a_in, size_t 
   // tangent mode: room for the primal zh rows this CTA finishes (see the kernel); the ring gives up stages if it must
   a.zstage = 0;
   size_t zbytes = 0;
-  if (g_tc_zstage && a.mode == CONV_TAN_STATS && a.zh != nullptr) {
+  if (opt.tc_zstage && a.mode == CONV_TAN_STATS && a.zh != nullptr) {
     zbytes = (size_t)(128 / S) * (NCOLS + 4) * 4;
     const long long limit = 227LL * 1024 - 4096;
     int nb2 = a.nb;
@@ -790,11 +784,9 @@ static void launch_conv_tc_n(const TcMaps& maps, const TcConvArgs& a_in, size_t 
   attr[0].val.clusterDim.x = 1; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = S;
   attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = ((g_pdl_cluster & 2) && pdl_allowed(st)) ? 2 : 1;
+  cfg.attrs = attr; cfg.numAttrs = ((opt.pdl_cluster & 2) && pdl_allowed(st)) ? 2 : 1;
   cudaLaunchKernelEx(&cfg, conv_tc_kernel<NCOLS>, maps, tagged(a));
 }
-
-void tc_conv_set_split(int max_split) { g_tc_split_max = max_split < 1 ? 1 : (max_split > 8 ? 8 : max_split); }
 
 void launch_conv_tc(const TcMaps& maps, const TcConvArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_CONV, a.alg_flops, st);

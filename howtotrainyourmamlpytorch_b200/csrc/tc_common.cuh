@@ -28,13 +28,8 @@ struct TcConvArgs {
 
 int tc_conv_rpad(int gw);
 int tc_conv_ring(int ncols, int gw);
-void tc_conv_set_ring_cap(int nb);
-void tc_conv_set_push(int on);         // split-K reduction: 1 push (one cluster barrier), 0 pull (two)
-void tc_conv_set_zstage(int on);       // tangent-mode statistics: 1 = primal zh staged in shared memory, 0 = read from global
-void tc_conv_set_ring_fit(int on);     // 1: ring depth = min(cap, B stages one CTA ever has in flight)     // B ring depth cap in [2, 8]
 size_t tc_conv_smem_bytes(int ncols, int gw);
 int tc_conv_prepare();
-void tc_conv_set_split(int max_split);   // largest split-K cluster size (1 = off)
 int tc_read_timeline(long long* out16);
 void launch_conv_tc(const TcMaps& maps, const TcConvArgs& a, cudaStream_t st);
 void launch_pack_weights(const ParamLayout& pl, const float* theta, long long theta_task_stride, float* pack,
