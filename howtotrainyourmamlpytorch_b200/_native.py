@@ -24,6 +24,7 @@ EXPORTED_SYMBOLS = [
     "maml_b200_trace", "maml_b200_trace_read",
     "maml_b200_comm_init", "maml_b200_comm_connect", "maml_b200_comm_world", "maml_b200_all_reduce",
     "maml_b200_comm_status", "maml_b200_net_backward", "maml_b200_net_running_update", "maml_b200_episode_gather",
+    "maml_b200_net_hvp",
 ]
 PROF_CATS = ["conv_igemm", "conv_first_block", "wgrad", "wgrad_first_block", "bn_act_pool", "head", "param"]
 
@@ -80,6 +81,8 @@ def load_library():
     lib.maml_b200_net_forward.restype = ctypes.c_int
     lib.maml_b200_net_backward.argtypes = [vp, i32, i32, vp, vp, vp, vp]
     lib.maml_b200_net_backward.restype = ctypes.c_int
+    lib.maml_b200_net_hvp.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
+    lib.maml_b200_net_hvp.restype = ctypes.c_int
     lib.maml_b200_net_running_update.argtypes = [vp, i32, i32, vp, vp, vp]
     lib.maml_b200_net_running_update.restype = ctypes.c_int
     lib.maml_b200_episode_gather.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, ctypes.POINTER(f32),
@@ -206,6 +209,12 @@ class Engine(object):
         rc = self.lib.maml_b200_net_backward(self.h, int(n_tasks), int(num_step), meta_like.data_ptr(), dlogits.data_ptr(),
                                              grad_out.data_ptr(), self._stream())
         _check(self.lib, rc, "maml_b200_net_backward")
+
+    def net_hvp(self, n_tasks, num_step, meta_like, x, dlogits, v_like, jv_out, hv_out):
+        rc = self.lib.maml_b200_net_hvp(self.h, int(n_tasks), int(num_step), meta_like.data_ptr(), x.data_ptr(),
+                                        dlogits.data_ptr(), v_like.data_ptr(), jv_out.data_ptr(), hv_out.data_ptr(),
+                                        self._stream())
+        _check(self.lib, rc, "maml_b200_net_hvp")
 
     def net_running_update(self, n_tasks, num_step, running_mean, running_var):
         rc = self.lib.maml_b200_net_running_update(self.h, int(n_tasks), int(num_step), running_mean.data_ptr(),

@@ -138,24 +138,26 @@ struct BnBwdTanArgs {             // backward reduce / apply (tangent)
 };
 
 enum { HEAD_SUPPORT = 0, HEAD_TARGET_FWD = 1, HEAD_TARGET_BWD = 2, HEAD_TANGENT = 3,
-       HEAD_EXTERNAL_BWD = 4 };     // backward of the linear layer for an externally supplied d(loss)/d(logits) (functional operator)
+       HEAD_EXTERNAL_BWD = 4,       // backward of the linear layer for an externally supplied d(loss)/d(logits) (functional operator)
+       HEAD_EXTERNAL_TAN = 5 };     // tangent of HEAD_EXTERNAL_BWD with d(loss)/d(logits) held constant; the logits tangent
+                                    // goes to logits_out (second-order functional operator)
 
 struct HeadArgs {
   int mode;
   int n, N, D;
   const float* f; long long f_stride;             // [n][D] features (grid order: pixel-major, channel-minor)
-  const float* fdot; long long fdot_stride;       // tangent of f (HEAD_TANGENT)
+  const float* fdot; long long fdot_stride;       // tangent of f (HEAD_TANGENT, HEAD_EXTERNAL_TAN)
   const float* Wfc; const float* bfc; long long theta_stride;     // [N][D], [N] (internal order), per task
-  const float* uW; const float* ub; long long u_stride;           // tangent direction (HEAD_TANGENT)
+  const float* uW; const float* ub; long long u_stride;           // tangent direction (HEAD_TANGENT, HEAD_EXTERNAL_TAN)
   const long long* y; long long y_stride;         // labels [n]
-  const float* dl_ext; long long dl_ext_stride;   // HEAD_EXTERNAL_BWD: upstream gradient w.r.t. the logits [n][N], per task
+  const float* dl_ext; long long dl_ext_stride;   // HEAD_EXTERNAL_*: upstream gradient w.r.t. the logits [n][N], per task
   float scale;                                    // loss weight folded into dlogits (1 for the support loss)
   float* gW; float* gb; long long g_stride;       // gradient (or H*u) output for the head tensors (chunk 0)
   long long g_chunk_stride;                       // stride between the row-group chunks of gW / gb
   int rows_per_cta;                               // rows of the batch handled by one CTA (grid.x = row groups)
   float* df; long long df_stride;                 // [n][D] gradient (or its tangent) w.r.t. features
   float* loss_out; long long loss_stride;         // per-task scalar (HEAD_TARGET_FWD)
-  float* logits_out; long long logits_stride;     // nullable [n][N]
+  float* logits_out; long long logits_stride;     // nullable [n][N] (HEAD_EXTERNAL_TAN: the logits tangent, required)
   float* correct_out; long long correct_stride;   // nullable per-task count
   int tasks;
   int tag;          // launch sequence number inside the iteration (device trace)

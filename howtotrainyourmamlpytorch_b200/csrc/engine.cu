@@ -740,9 +740,21 @@ static void backward_pass(maml_b200_handle* h, const PassSet& ps, int slot, cons
   else if (fork_wgrad) { cudaEventRecord(h->ev_wg, h->s_wg); cudaStreamWaitEvent(st, h->ev_wg, 0); }
 }
 
+// What a tangent pass differentiates at its head, and where its BatchNorm gamma / beta sums go (export adds the
+// PASS_TGT_BWD sums and subtracts the PASS_TAN_BWD ones).
+//   fused iteration:       HEAD_TANGENT, support labels y, PASS_TAN_BWD   (gamma-bar -= H_gamma u)
+//   functional operator:   HEAD_EXTERNAL_TAN, dl_ext held constant, the logits tangent into jv_out, PASS_TGT_BWD
+//                          (+H_gamma v)
+struct TangentHead {
+  int mode;
+  const long long* y;
+  const float* dl_ext; float* jv_out;
+  int kind_tbwd;
+};
+
 // forward-mode tangent of (support forward + support backward) at step s in direction u  =>  H u into `partial`
 static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const float* u, const float* meta,
-                         const long long* y_support, int T, cudaStream_t st, const ReduceSpec& rs, cudaStream_t spre) {
+                         const TangentHead& th, int T, cudaStream_t st, const ReduceSpec& rs, cudaStream_t spre) {
   const PassSet& sp = h->sup; const PassSet& tn = h->tan; const PassSet& t2 = h->tan2;
   // Tangent convs of blocks >= 1 have two operand pairs; the pair (primal activation, u weights) depends only on u and
   // on what phase A saved, not on the tangent chain.  It is computed up front on the side stream (right behind the
@@ -750,7 +762,8 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
   // consumers (bnact_tan / bnbwd_tan) add the two addends.  The main chain keeps the single-pair half: 18 instead of
   // 36 stages per tile on the critical path.
   const bool split = h->use_tc && h->opt.tan_split;
-  const bool fuse_tail = h->opt.tail_fuse && tail_fusable(bn_geom(h, h->L - 1, sp.n), sp.n, head_rows(sp.n));
+  // the fused last-block kernels implement the cross-entropy tangent head only
+  const bool fuse_tail = th.mode == HEAD_TANGENT && h->opt.tail_fuse && tail_fusable(bn_geom(h, h->L - 1, sp.n), sp.n, head_rows(sp.n));
   BnActTanArgs last_act{};
   HeadArgs hd{};
   if (split) {
@@ -823,12 +836,18 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
   join_pending(h, st);
   {
     HeadArgs& a = hd;
-    a.mode = HEAD_TANGENT; a.n = h->n_s; a.N = h->N; a.D = h->D; a.scale = 1.f;
+    a.mode = th.mode; a.n = h->n_s; a.N = h->N; a.D = h->D; a.scale = 1.f;
     a.f = AIN(sp, h->L, s); a.f_stride = STRIDE(sp, ain, h->L);
     a.fdot = AIN(tn, h->L, 0); a.fdot_stride = STRIDE(tn, ain, h->L);
     a.Wfc = theta + h->pl.fcw_off; a.bfc = theta + h->pl.fcb_off; a.theta_stride = h->Ppad;
     a.uW = u + h->pl.fcw_off; a.ub = u + h->pl.fcb_off; a.u_stride = h->Ppad;
-    a.y = y_support; a.y_stride = h->n_s;
+    if (th.mode == HEAD_TANGENT) {
+      a.y = th.y; a.y_stride = h->n_s;
+    } else {
+      a.y = h->zero_labels; a.y_stride = 0;
+      a.dl_ext = th.dl_ext; a.dl_ext_stride = (long long)h->n_s * h->N;
+      a.logits_out = th.jv_out; a.logits_stride = (long long)h->n_s * h->N;
+    }
     a.gW = h->sup_partial + cp.pd.off[2 * h->L]; a.gb = h->sup_partial + cp.pd.off[2 * h->L + 1]; a.g_stride = cp.pd.task_stride;
     a.g_chunk_stride = cp.pd.cstride[2 * h->L]; a.rows_per_cta = head_rows(a.n);
     a.df = DP(tn, h->L - 1, 0); a.df_stride = STRIDE(tn, dp, h->L - 1);
@@ -847,7 +866,7 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
     b.stats_fwd = stat_at(h, PASS_SUP_FWD, s, l); b.stats_fwd_stride = h->stats_task_stride;
     b.stats_bwd = stat_at(h, PASS_SUP_BWD, s, l); b.stats_bwd_stride = h->stats_task_stride;
     b.stats_tan = stat_at(h, PASS_TAN_FWD, s, l); b.stats_tan_stride = h->stats_task_stride;
-    b.stats_tbwd = stat_at(h, PASS_TAN_BWD, s, l); b.stats_tbwd_stride = h->stats_task_stride;
+    b.stats_tbwd = stat_at(h, th.kind_tbwd, s, l); b.stats_tbwd_stride = h->stats_task_stride;
     b.gamma = gamma_at(h, meta, l, s); b.beta = beta_at(h, meta, l, s);
     b.dzdot = DZ(tn, l, 0); b.dzdot_stride = STRIDE(tn, dz, l);
     if (h->use_tc && l >= 1) { b.dzdot_hi = DZ_HI(tn, l, 0); b.dzdot_lo = DZ_LO(tn, l, 0); }
@@ -1044,7 +1063,7 @@ static int enqueue_iteration(maml_b200_handle* h, const maml_b200_iter_args* it,
         CK(cudaEventRecord(h->ev_wg, spre));
         h->wg_pending = true;
         ReduceSpec rs{PR_SUB, nullptr, nullptr, nullptr, h->tbar, s, -1};
-        tangent_pass(h, s, th, h->u, meta, ys, T, st, rs, spre);
+        tangent_pass(h, s, th, h->u, meta, TangentHead{HEAD_TANGENT, ys, nullptr, nullptr, PASS_TAN_BWD}, T, st, rs, spre);
       }
     }
     join_pending(h, st);
@@ -1216,10 +1235,78 @@ extern "C" int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int3
   return 0;
 }
 
+// Second-order companion of maml_b200_net_backward: what torch.autograd needs to differentiate the backward of the
+// functional operator once more (the reference's loss.backward() through torch.autograd.grad(..., create_graph=True),
+// few_shot_learning_system.py:138-139).  Self-contained: meta_like is imported into theta[num_step] and the whole chain
+// runs at support slot s = num_step, exactly as the fused iteration's support chain does at step s -- forward, backward of
+// the external dlogits, then the tangent pass along v_like with dlogits held constant (HEAD_EXTERNAL_TAN).  Batches of
+// N*K images (the handle's support shape).  jv_out [n_tasks, N*K, N] = J v.  hv_out: result_size floats; the first meta_size
+// hold d/d(meta_like) <dlogits, J v> in the meta layout, summed over the batches: conv / linear entries are stored into
+// tbar by the parameter reduction, the BatchNorm gamma / beta sums go to the PASS_TGT_BWD statistics, which export adds
+// (+H_gamma v, +H_beta v); LSLR entries 0.  v_like's BatchNorm and LSLR entries are not read.  Overwrites the batch
+// statistics maml_b200_net_running_update reads; no running-statistics side effect of its own.
+extern "C" int maml_b200_net_hvp(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
+                                 const float* dlogits, const float* v_like, float* jv_out, float* hv_out, void* stream) {
+  if (!h || !meta_like || !x || !dlogits || !v_like || !jv_out || !hv_out) return fail("null argument");
+  if (n_tasks < 1 || n_tasks > h->maxT) return fail("n_tasks out of range");
+  if (num_step < 0 || num_step >= h->S) return fail("num_step out of range");
+  cudaStream_t st = (cudaStream_t)stream;
+  LaunchScope launch_scope(h, st);
+  const int T = n_tasks, s = num_step;
+  float* th = h->theta + (long long)s * h->maxT * h->Ppad;
+  CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
+  CK(cudaMemsetAsync(h->abar, 0, (size_t)h->maxT * h->pl.nseg_inner * MAML_MAX_STEPS * sizeof(double), st));
+  CK(cudaMemsetAsync(h->losses, 0, (size_t)h->maxT * MAML_MAX_STEPS * sizeof(float), st));
+  CK(cudaMemsetAsync(h->correct, 0, (size_t)h->maxT * sizeof(float), st));
+  launch_prep_x(x, h->sup.xg, h->sup.xg_stride, T, h->n_s, h->C, h->H, h->W, st);
+  launch_import_theta(h->pl, meta_like, th, h->Ppad, T, st);
+  launch_import_theta(h->pl, v_like, h->u, h->Ppad, T, st);
+  pack_theta_step(h, s, T, st);
+  forward_pass(h, h->sup, s, th, s, meta_like, s, PASS_SUP_FWD, T, st);
+  HeadArgs a{};
+  a.mode = HEAD_EXTERNAL_BWD; a.n = h->n_s; a.N = h->N; a.D = h->D; a.scale = 1.f;
+  a.f = AIN(h->sup, h->L, s); a.f_stride = STRIDE(h->sup, ain, h->L);
+  a.Wfc = th + h->pl.fcw_off; a.bfc = th + h->pl.fcb_off; a.theta_stride = h->Ppad;
+  a.y = h->zero_labels; a.y_stride = 0;
+  a.dl_ext = dlogits; a.dl_ext_stride = (long long)h->n_s * h->N;
+  a.gW = h->sup_partial + h->plan_sup.pd.off[2 * h->L]; a.gb = h->sup_partial + h->plan_sup.pd.off[2 * h->L + 1];
+  a.g_stride = h->plan_sup.pd.task_stride; a.g_chunk_stride = h->plan_sup.pd.cstride[2 * h->L];
+  a.rows_per_cta = head_rows(a.n);
+  a.df = DP(h->sup, h->L - 1, s); a.df_stride = STRIDE(h->sup, dp, h->L - 1);
+  a.tasks = T;
+  launch_head(a, st);
+  // the tangent pass reads this backward's dz / dp and statistics; its weight-gradient chunks are overwritten unread
+  backward_pass(h, h->sup, s, th, s, meta_like, s, PASS_SUP_FWD, PASS_SUP_BWD, h->sup_partial, h->plan_sup, T, st, false);
+  cudaStream_t spre = (h->use_tc && h->opt.tan_split) ? h->s_tgt : h->s_wg;     // as in the fused reverse sweep
+  CK(cudaEventRecord(h->ev_fork, st));
+  CK(cudaStreamWaitEvent(spre, h->ev_fork, 0));
+  pack_u(h, T, spre);
+  CK(cudaEventRecord(h->ev_wg, spre));
+  h->wg_pending = true;
+  ReduceSpec rs{PR_STORE, nullptr, nullptr, h->tbar, nullptr, s, -1};
+  tangent_pass(h, s, th, h->u, meta_like, TangentHead{HEAD_EXTERNAL_TAN, nullptr, dlogits, jv_out, PASS_TGT_BWD}, T, st, rs, spre);
+  join_pending(h, st);
+  ExportArgs e{};
+  e.pl = h->pl;
+  e.tbar = h->tbar; e.task_stride = h->Ppad;
+  e.abar = h->abar;
+  e.stats = h->stats; e.stats_task_stride = h->stats_task_stride; e.st_pass_stride = h->st_pass_stride; e.st_layer_stride = h->st_layer_stride;
+  e.losses = h->losses; e.correct = h->correct;
+  e.target_mask = 0; e.num_steps = h->S; e.training = 1;
+  e.tasks = T; e.task_offset = 0; e.tasks_global = 1;            // plain sum over the batches, no 1/B
+  e.n_s = h->n_s; e.n_t = h->n_t;
+  for (int l = 0; l < h->L; ++l) e.hw[l] = h->geo[l].h * h->geo[l].w;
+  e.result = hv_out;
+  launch_export(e, st);
+  CK(cudaGetLastError());
+  return 0;
+}
+
 // Side effect of the functional forward in the reference: F.batch_norm's EMA update of running_mean / running_var at
 // `num_step` (meta_neural_network_architectures.py:226-247), from the batch statistics of the last maml_b200_net_forward
 // call (one update per batch, in order).  running_mean / running_var: [stages][S][F] device.  No-op for shared BatchNorm
-// (the reference passes running stats = None there).
+// (the reference passes running stats = None there).  A maml_b200_net_hvp call on the same handle in between overwrites
+// those statistics: apply the update right after the forward.
 extern "C" int maml_b200_net_running_update(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, float* running_mean,
                                            float* running_var, void* stream) {
   if (!h || !running_mean || !running_var) return fail("null argument");

@@ -30,8 +30,10 @@ __device__ __forceinline__ float warp_sum(float v) {
 #undef HEAD_LOOP
 #undef HEAD_BODY_NAME
 
-template <bool COMPACT>
+// EXT_TAN = false compiles the HEAD_EXTERNAL_TAN branch out, so the kernels that run the fused iteration's modes (the fused
+// last-block kernels, the head kernel's default instantiations) keep their code; launch_head picks EXT_TAN by mode.
+template <bool COMPACT, bool EXT_TAN = false>
 __device__ __forceinline__ void head_body(const HeadArgs& a, int task, int group, float* smh, float* s_rowloss, float* s_rowcorrect) {
-  if constexpr (COMPACT) head_body_compact(a, task, group, smh, s_rowloss, s_rowcorrect);
-  else head_body_unrolled(a, task, group, smh, s_rowloss, s_rowcorrect);
+  if constexpr (COMPACT) head_body_compact<EXT_TAN>(a, task, group, smh, s_rowloss, s_rowcorrect);
+  else head_body_unrolled<EXT_TAN>(a, task, group, smh, s_rowloss, s_rowcorrect);
 }

@@ -10,13 +10,13 @@
 
 #include "head_body.cuh"
 
-template <bool COMPACT>
+template <bool COMPACT, bool EXT_TAN>
 __global__ void __launch_bounds__(256) head_kernel(HeadArgs a) {
   pdl_prologue(14, a.tag);
   extern __shared__ float smh[];
   __shared__ float s_rowloss[64];
   __shared__ float s_rowcorrect[64];
-  head_body<COMPACT>(a, blockIdx.y, blockIdx.x, smh, s_rowloss, s_rowcorrect);
+  head_body<COMPACT, EXT_TAN>(a, blockIdx.y, blockIdx.x, smh, s_rowloss, s_rowcorrect);
 }
 
 void launch_head(const HeadArgs& a, cudaStream_t st) {
@@ -25,8 +25,14 @@ void launch_head(const HeadArgs& a, cudaStream_t st) {
   dim3 grid((a.n + a.rows_per_cta - 1) / a.rows_per_cta, a.tasks);
   // small feature vectors (Omniglot: D = 64): the rolled-loop body (less code to fetch for a kernel that runs once);
   // large ones (Mini-ImageNet: D = 1200): the compiler's unrolled D-loops
-  if (a.D <= 256) launch_pdl(head_kernel<true>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
-  else launch_pdl(head_kernel<false>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
+  // HEAD_EXTERNAL_TAN (functional operator only) has instantiations of its own: the iteration's heads keep their code
+  if (a.mode == HEAD_EXTERNAL_TAN) {
+    if (a.D <= 256) launch_pdl(head_kernel<true, true>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
+    else launch_pdl(head_kernel<false, true>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
+  } else {
+    if (a.D <= 256) launch_pdl(head_kernel<true, false>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
+    else launch_pdl(head_kernel<false, false>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
+  }
   CUDA_CHECK_LAUNCH();
 }
 

@@ -7,7 +7,8 @@ the reference's module tree and parameter names -- so ``state_dict`` keys, shape
 order (= Adam parameter order) and initialisation RNG consumption are identical -- but they are
 parameter containers: the arithmetic of the path runs in the CUDA engine (``csrc/``), which sees
 these parameters as one flat buffer.  ``VGGReLUNormNetwork.forward`` is the functional-network operator of the
-boundary (level B1): forward and (first-order) backward both run on the engine through ``torch.autograd.Function``.
+boundary (level B1): forward, backward and the backward of that backward (second-order MAML) all run on the engine
+through ``torch.autograd.Function``.
 
 Initialisation restates reference ``:62-66`` (xavier_uniform_ conv weight, zero bias),
 ``:114-118`` (xavier_uniform_ linear weights), ``:177-192`` (running_mean zeros; running_var ones
@@ -142,6 +143,26 @@ class VGGReLUNormNetwork(nn.Module):
                           "run": torch.zeros(2, self.num_stages, S, self.cnn_filters, dtype=torch.float32, device=x.device)}
         return cache[key]
 
+    def _hvp_engine(self, x):
+        """Engine of ``maml_b200_net_hvp`` for this batch shape, created on the first double backward: a second handle whose
+        SUPPORT buffers (those the tangent pass runs on) hold the batch, so the operator's first-order handle and its
+        users pay nothing for them."""
+        from . import _native
+        st = self._operator_engine(x)
+        if "hvp" not in st:
+            a, n, N = self.args, int(x.shape[0]), self.num_output_classes
+            with torch.cuda.device(x.device):
+                eng = _native.Engine(n_way=N, k_shot=n // N, t_target=1, channels=int(x.shape[1]), height=int(x.shape[2]),
+                                     width=int(x.shape[3]), filters=self.cnn_filters, num_stages=self.num_stages,
+                                     inner_steps=int(a.number_of_training_steps_per_iter),
+                                     per_step_bn=bool(a.per_step_bn_statistics), max_tasks=1)
+            st["hvp"] = {"eng": eng,
+                         "meta": torch.zeros(eng.meta_size, dtype=torch.float32, device=x.device),
+                         "v": torch.zeros(eng.meta_size, dtype=torch.float32, device=x.device),
+                         "jv": torch.empty(1, n, N, dtype=torch.float32, device=x.device),
+                         "hv": torch.zeros(eng.result_size, dtype=torch.float32, device=x.device)}
+        return st["hvp"]
+
     def forward(self, x, num_step, params=None, training=False, backup_running_statistics=False):
         """Logits of a batch under externally supplied ("fast") weights -- reference
         ``VGGReLUNormNetwork.forward`` (:620-660): ``params`` maps ``layer_dict.conv{i}.conv.{weight,bias}`` /
@@ -153,9 +174,11 @@ class VGGReLUNormNetwork(nn.Module):
         Runs on the CUDA engine (C ABI ``maml_b200_net_forward`` / ``maml_b200_net_backward``) and is differentiable
         through ``torch.autograd`` with respect to every weight it uses (conv / linear fast weights, BatchNorm gamma /
         beta), which is what the reference's ``apply_inner_loop_update`` needs (``torch.autograd.grad`` of the support
-        loss, few_shot_learning_system.py:138-139).  First order only: the second-order terms live in the fused
-        iteration (``MAMLFewShotClassifier``).  No gradient flows to ``x``.  The batch size must be a multiple of the
-        number of classes (episode shaped)."""
+        loss, few_shot_learning_system.py:138-139).  Twice differentiable: with ``create_graph=True`` the returned
+        gradients are differentiable w.r.t. the weights (and the upstream d(logits)) through ``maml_b200_net_hvp``, so the
+        reference's second-order loop runs on this operator; a BatchNorm gamma / beta gradient is not (see
+        ``_FunctionalBackward``).  No gradient flows to ``x``.  The batch size must be a multiple of the number of classes
+        (episode shaped)."""
         from . import _native
         if x.device.type != "cuda":
             raise _native.NativeLibraryError("VGGReLUNormNetwork.forward needs a CUDA (sm_90a) device: no CPU fallback")
@@ -199,10 +222,10 @@ class VGGReLUNormNetwork(nn.Module):
 
 class _FunctionalForward(torch.autograd.Function):
     """``VGGReLUNormNetwork.forward`` as an autograd node: forward = ``maml_b200_net_forward``, backward =
-    ``maml_b200_net_backward`` (head backward for an external d(logits), BatchNorm / pool / leaky-ReLU backward, dgrad and
-    wgrad kernels of the engine).  The engine keeps the activations of its LAST forward only, so a backward that arrives
-    after another forward of the same shape first replays its own forward (cheap) -- correctness does not depend on the
-    call order."""
+    ``_FunctionalBackward`` (``maml_b200_net_backward``: head backward for an external d(logits), BatchNorm / pool / leaky-ReLU
+    backward, dgrad and wgrad kernels of the engine), itself differentiable once more.  The engine keeps the activations of
+    its LAST forward only, so a backward that arrives after another forward of the same shape first replays its own forward
+    (cheap) -- correctness does not depend on the call order."""
 
     @staticmethod
     def forward(ctx, net, x, num_step, *tensors):
@@ -217,25 +240,77 @@ class _FunctionalForward(torch.autograd.Function):
             net._apply_running_ema(st, num_step)
         st["gen"] += 1
         ctx.net, ctx.num_step, ctx.gen = net, num_step, st["gen"]
-        ctx.save_for_backward(xin, *[t.detach() for t in tensors])
+        ctx.save_for_backward(xin, *tensors)       # the weights themselves: a double backward differentiates w.r.t. them
         return logits[0].clone()
 
     @staticmethod
-    @torch.autograd.function.once_differentiable
     def backward(ctx, dlogits):
-        net, num_step = ctx.net, ctx.num_step
         xin, tensors = ctx.saved_tensors[0], ctx.saved_tensors[1:]
+        return (None, None, None) + tuple(_FunctionalBackward.apply(ctx, xin, dlogits, *tensors))
+
+
+class _FunctionalBackward(torch.autograd.Function):
+    """Backward of ``_FunctionalForward`` as an autograd node of its own, so that ``torch.autograd.grad(...,
+    create_graph=True)`` of a loss on the operator's logits can be differentiated again (second-order MAML, reference
+    few_shot_learning_system.py:138-139 and the outer ``loss.backward()``).
+
+    forward  = ``maml_b200_net_backward``: B(dl, theta) = J^T dl for every tensor (conv / linear, BatchNorm gamma / beta of
+               ``num_step``).  With grad mode off this is the whole first-order backward.
+    backward = ``maml_b200_net_hvp`` along the cotangents v of the conv / linear gradients: one forward-over-reverse pass with
+               dl held constant gives J v (the cotangent of dl) and d/dtheta <dl, J v> (that of every tensor).  torch carries
+               J v on through the loss's own double backward.  Third order is not supported.
+    A cotangent on a BatchNorm gamma / beta GRADIENT would need gamma / beta tangent directions, which the engine's BatchNorm
+    tangent kernels do not have: refused (it only arises when BatchNorm parameters are inner-loop fast weights,
+    enable_inner_loop_optimizable_bn_params, which the network refuses too)."""
+
+    @staticmethod
+    def forward(ctx, fwd_ctx, xin, dlogits, *tensors):
+        net, num_step = fwd_ctx.net, fwd_ctx.num_step
         st = net._operator_engine(xin)
         eng, meta_like, logits, grad = st["eng"], st["meta"], st["logits"], st["grad"]
         with torch.cuda.device(xin.device):
-            if st["gen"] != ctx.gen:                 # another forward ran since: replay ours (no EMA side effect again)
+            if st["gen"] != fwd_ctx.gen:             # another forward ran since: replay ours (no EMA side effect again)
                 for (off, size), t in zip(eng.segments, tensors):
-                    meta_like[off:off + size].copy_(t.reshape(-1).to(torch.float32))
+                    meta_like[off:off + size].copy_(t.detach().reshape(-1).to(torch.float32))
                 eng.net_forward(1, num_step, meta_like, xin, logits)
                 st["gen"] += 1
-                ctx.gen = st["gen"]
+                fwd_ctx.gen = st["gen"]
             eng.net_backward(1, num_step, meta_like, dlogits.detach().to(torch.float32).contiguous().view(1, *dlogits.shape), grad)
+        ctx.set_materialize_grads(False)
+        ctx.net, ctx.num_step, ctx.x = net, num_step, xin
+        ctx.save_for_backward(dlogits, *tensors)
+        grads = []
+        for (off, size), t, need in zip(eng.segments, tensors, fwd_ctx.needs_input_grad[3:]):
+            grads.append(grad[off:off + size].view(t.shape).clone() if need else None)
+        return tuple(grads)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, *cotangents):
+        net, num_step, xin = ctx.net, ctx.num_step, ctx.x
+        dlogits, tensors = ctx.saved_tensors[0], ctx.saved_tensors[1:]
+        n_conv = 4 * net.num_stages
+        for i, c in enumerate(cotangents[:n_conv]):
+            if c is not None and i % 4 >= 2:
+                raise NotImplementedError(
+                    "differentiating through the gradient of a BatchNorm gamma / beta needs gamma / beta tangent "
+                    "directions, which the engine does not implement (BatchNorm parameters as inner-loop fast weights, "
+                    "enable_inner_loop_optimizable_bn_params, are outside the accelerated path)")
+        if all(c is None for c in cotangents):
+            return (None,) * (3 + len(tensors))
+        hs = net._hvp_engine(xin)
+        eng, meta_like, v_like, jv, hv = hs["eng"], hs["meta"], hs["v"], hs["jv"], hs["hv"]
+        with torch.no_grad():
+            v_like.zero_()
+            for (off, size), t, c in zip(eng.segments, tensors, cotangents):
+                meta_like[off:off + size].copy_(t.reshape(-1).to(torch.float32))
+                if c is not None:
+                    v_like[off:off + size].copy_(c.reshape(-1).to(torch.float32))
+        with torch.cuda.device(xin.device):
+            eng.net_hvp(1, num_step, meta_like, xin, dlogits.to(torch.float32).contiguous().view(1, *dlogits.shape), v_like,
+                        jv, hv)
+        d_dlogits = jv[0].to(dlogits.dtype).clone() if ctx.needs_input_grad[2] else None
         grads = []
         for (off, size), t, need in zip(eng.segments, tensors, ctx.needs_input_grad[3:]):
-            grads.append(grad[off:off + size].view(t.shape).clone() if need else None)
-        return (None, None, None) + tuple(grads)
+            grads.append(hv[off:off + size].view(t.shape).to(t.dtype).clone() if need else None)
+        return (None, None, d_dlogits) + tuple(grads)

@@ -122,8 +122,23 @@ int maml_b200_net_forward(maml_b200_handle* h, int32_t n_tasks, int32_t num_step
 int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
                            const float* dlogits, float* grad_out, void* stream);
 
+/* Second-order companion of maml_b200_net_backward: for the batch x, weights meta_like and upstream dlogits, one
+ * forward-over-reverse pass along v_like (meta layout; its BatchNorm and LSLR entries are not read: there are no
+ * gamma / beta tangent directions).  Self-contained: it recomputes the forward and the backward of dlogits itself, so it
+ * needs no earlier call.  The batch has the handle's SUPPORT shape: N*K images (create the handle with k_shot = batch / N).
+ *   x          [n_tasks, N*K, C, H, W]
+ *   dlogits    [n_tasks, N*K, N]  d(loss) / d(logits), held constant along v
+ *   jv_out     [n_tasks, N*K, N]  = J(meta_like) v           (tangent of the logits)
+ *   hv_out     result_size floats; first meta_size = d/d(meta_like) <dlogits, J v> in the meta layout
+ *              (conv / linear weights and biases, BatchNorm gamma / beta of num_step; LSLR entries 0), summed over the
+ *              n_tasks batches
+ * No running-statistics side effect; it overwrites the batch statistics maml_b200_net_running_update reads. */
+int maml_b200_net_hvp(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
+                      const float* dlogits, const float* v_like, float* jv_out, float* hv_out, void* stream);
+
 /* EMA side effect of the functional forward (F.batch_norm updating running_mean / running_var at num_step, reference
- * meta_neural_network_architectures.py:226-247) from the batch statistics of the last maml_b200_net_forward call.
+ * meta_neural_network_architectures.py:226-247) from the batch statistics of the last maml_b200_net_forward call, which
+ * must not be followed by a maml_b200_net_hvp call on the same handle before this one (apply it right after the forward).
  * running_mean / running_var: [stages][S][F] device.  No-op without per-step BatchNorm. */
 int maml_b200_net_running_update(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, float* running_mean,
                                  float* running_var, void* stream);

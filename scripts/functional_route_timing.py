@@ -1,0 +1,127 @@
+"""Time one outer training iteration (forward + meta-gradient) of the headline config (Omniglot MAML++ 5-way 1-shot,
+meta-batch 8, second order) three ways, on one GPU:
+
+  operator  the reference's training loop (per task, per inner step: torch.autograd.grad(create_graph=True), LSLR
+            update, MSL target losses; then the outer backward) on this repository's VGGReLUNormNetwork.forward
+            (integration route B1: engine forward / backward / Hessian-vector product);
+  torch     the same loop on torch ops on the GPU (oracle._net_forward: F.conv2d / F.batch_norm / ..., fp32, TF32 off);
+  fused     MAMLFewShotClassifier.run_train_iter (route B0: the whole iteration as one engine call, Adam step included).
+
+Warm-up first; every timed iteration ends in a device synchronise; the three legs alternate within each repeat.  Prints
+one JSON line: per leg the median / min / max milliseconds per iteration, plus the GPU name and power limit read in
+the same run.
+
+  python scripts/functional_route_timing.py [--repeats 20] [--warmup 3]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+
+import torch                                         # noqa: E402
+import torch.nn.functional as Fnn                    # noqa: E402
+
+CONFIG, META_BATCH = "omniglot_mamlpp_5w1s", 8
+
+
+def reference_loop(net_forward, params, a, batch, epoch, O):
+    """oracle.autograd_train_iter's loop with a pluggable network forward; returns the outer gradients."""
+    S = int(a.number_of_training_steps_per_iter)
+    second_order = bool(a.second_order) and epoch > a.first_order_to_second_order_epoch
+    sched = O.target_pass_schedule(a, epoch, True, S)
+    w_msl = torch.from_numpy(O.msl_weights(a, epoch)).to(batch[0].device)
+    inner = O.inner_param_names(a)
+    xs, xt, ys, yt = batch
+    total = []
+    for b in range(xs.shape[0]):
+        fast = {n: params[n] for n in inner}
+        x_s, y_s = xs[b].reshape(-1, *xs.shape[-3:]), ys[b].reshape(-1)
+        x_t, y_t = xt[b].reshape(-1, *xt.shape[-3:]), yt[b].reshape(-1)
+        task_losses = []
+        for s in range(S):
+            loss_s = Fnn.cross_entropy(net_forward(x_s, fast, s), y_s)
+            grads = torch.autograd.grad(loss_s, [fast[n] for n in inner], create_graph=second_order)
+            fast = {n: fast[n] - params[O.lslr_name(n)][s] * g for n, g in zip(inner, grads)}
+            if sched[s] is not None:
+                loss_t = Fnn.cross_entropy(net_forward(x_t, fast, s), y_t)
+                task_losses.append(w_msl[s] * loss_t if sched[s] == "msl" else loss_t)
+        total.append(torch.stack(task_losses).sum())
+    loss = torch.stack(total).mean()
+    names = O.trainable_names(a)
+    return torch.autograd.grad(loss, [params[n] for n in names], allow_unused=True)
+
+
+def gpu_info():
+    out = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                         stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True).stdout.strip()
+    name, _, power = out.partition(",")
+    return name.strip() or torch.cuda.get_device_name(0), power.strip() or "unknown"
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--repeats", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=3)
+    cli = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("functional_route_timing.py needs a CUDA device")
+    from howtotrainyourmamlpytorch_b200 import MAMLFewShotClassifier, make_args, synthetic_batch
+    from oracle import maml_oracle as O
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    dev = torch.device("cuda", 0)
+    a = make_args(CONFIG, batch_size=META_BATCH)
+    epoch = 0
+    batch = synthetic_batch(a, iteration=0)
+    dbatch = tuple(t.to(dev) for t in batch)
+    dbatch = (dbatch[0].float(), dbatch[1].float(), dbatch[2].long(), dbatch[3].long())
+    m_op = MAMLFewShotClassifier(im_shape=(2, a.image_channels, a.image_height, a.image_width), device=dev, args=a)
+    m_fused = MAMLFewShotClassifier(im_shape=(2, a.image_channels, a.image_height, a.image_width), device=dev, args=a)
+    m_fused.load_state_dict(m_op.state_dict())
+    op_params = dict(m_op.named_parameters())
+    t_params = {k: v.detach().clone().requires_grad_(v.requires_grad) for k, v in m_op.state_dict().items()}
+    t_params.update({k: v.detach().clone().requires_grad_(True) for k, v in op_params.items() if v.requires_grad})
+    pre = len("classifier.")
+
+    def op_forward(x, fast, s):
+        return m_op.classifier.forward(x, num_step=s, training=True, params={n[pre:]: w.unsqueeze(0) for n, w in fast.items()})
+
+    def torch_forward(x, fast, s):
+        return O._net_forward(x, fast, t_params, a, s)
+
+    legs = {
+        "operator": lambda: reference_loop(op_forward, op_params, a, dbatch, epoch, O),
+        "torch": lambda: reference_loop(torch_forward, t_params, a, dbatch, epoch, O),
+        "fused": lambda: m_fused.run_train_iter(batch, epoch),
+    }
+    for _ in range(cli.warmup):
+        for f in legs.values():
+            f()
+    torch.cuda.synchronize()
+    times = {k: [] for k in legs}
+    for _ in range(cli.repeats):
+        for k, f in legs.items():
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            f()
+            torch.cuda.synchronize()
+            times[k].append(1e3 * (time.perf_counter() - t0))
+    name, power = gpu_info()
+
+    def summary(v):
+        v = sorted(v)
+        return {"median_ms": round(v[len(v) // 2], 3), "min_ms": round(v[0], 3), "max_ms": round(v[-1], 3)}
+
+    print(json.dumps({"config": CONFIG, "meta_batch": META_BATCH, "second_order": True, "gpu": name,
+                      "power_limit": power, "repeats": cli.repeats, "warmup": cli.warmup,
+                      "legs": {k: summary(v) for k, v in times.items()}}))
+
+
+if __name__ == "__main__":
+    main()
