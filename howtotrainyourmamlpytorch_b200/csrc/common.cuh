@@ -285,22 +285,12 @@ struct EngineOptions {
   bool no_graph = false;     // NO_GRAPH (set): eager launches instead of the captured CUDA graph
   bool one_stream = false;   // ONE_STREAM (set): every kernel on the caller's stream
   bool wgrad_tc = true;      // WGRAD_TC=0: FFMA weight gradient for blocks l >= 1
-  bool wgrad_row = true;     // WGRAD_ROW=0: one filter tap per FFMA weight-gradient CTA instead of one filter row
   int tc_split = 8;          // TC_SPLIT: largest split-K cluster size of the wgmma conv, in [1, 8] (1 = off)
-  int tc_split_side = 0;     // TC_SPLIT_SIDE: split-K cap of side-stream convs (0 = none)
   int tc_nb = 0;             // TC_NB: B ring depth of main-chain convs, in [2, 8] (0 = by regime)
-  int tc_nb_side = 0;        // TC_NB_SIDE: B ring depth cap of side-stream convs (< 2 = none)
-  bool tc_nb_fit = false;    // TC_NB_FIT=1: cut the ring to the B stages one CTA ever has in flight
-  bool tc_push = true;       // TC_PUSH=0: pull-based split-K reduction (two cluster barriers)
-  bool tc_zstage = true;     // TC_ZSTAGE=0: tangent-mode statistics read the primal zh from global memory
   bool bn_fuse = true;       // BN_FUSE=0: BatchNorm backward always as two kernels (reduce, apply)
-  int bn_side_cap = 0;       // BN_SIDE_CAP: CTA cap of grid-stride BatchNorm launches on side streams (0 = none)
   bool tail_fuse = true;     // TAIL_FUSE=0: last block / head / its BatchNorm backward as separate kernels
   int tail_onchip = 3;       // TAIL_ONCHIP: fused last-block kernels on chip, bit 0 primal, bit 1 tangent
-  bool tan_split = true;     // TAN_SPLIT=0: two-source tangent convs on the main chain
-  int tgt_slots = 2;         // TGT_SLOTS: target-pass buffers / streams (>= 1)
-  int pdl = -1;              // PDL: programmatic dependent launch mode, in [0, 3] (-1 = by regime)
-  int pdl_cluster = 0;       // PDL_CLUSTER: cluster launches that take PDL too, bit 0 fused BatchNorm backward, bit 1 split-K convs
+  int pdl = -1;              // PDL: programmatic dependent launch on the main chain, 0 off / 1 on (-1 = by regime)
   int tc_timeline = -1;      // TC_TIMELINE: clock64 milestones of one conv CTA of block l (0 = any block, -1 = off)
   std::string graph_dot;     // GRAPH_DOT: file the captured graph is written to (empty = none)
 };
@@ -313,25 +303,22 @@ struct EngineOptions {
 struct Profiler;
 struct LaunchContext {
   const EngineOptions* opt;
-  int pdl_mode;                    // 0: off, 1: every launch, 2: only launches on main_stream, 3: every stream but wg_stream
+  bool pdl;                        // launches on main_stream take programmatic dependent launch
   cudaStream_t main_stream;        // stream of the call's main chain (null: the call has none)
-  cudaStream_t wg_stream;          // the handle's weight-gradient side stream
   Profiler* prof;                  // non-null while the handle is profiling
 };
 const LaunchContext& launch_ctx();
-// a launch on a side stream of the current iteration (target passes, weight gradients, pre-computed tangent addends)
-inline bool on_side_stream(cudaStream_t st) { return launch_ctx().main_stream && st != launch_ctx().main_stream; }
 
 // ---------------------------------------------------------------------------------------------
 // Programmatic dependent launch: a kernel launched with the programmatic-stream-serialization attribute starts with
 // `griddepcontrol.launch_dependents; griddepcontrol.wait;` -- the next kernel of the stream is scheduled while this one
-// still runs (its launch latency and set-up overlap) and blocks until this grid has completed and flushed.  Which
-// launches take the attribute is the handle's PDL mode: main chain only in the latency-bound regime, none in the
-// throughput-bound one (maml_b200_create), or MAML_B200_PDL.
+// still runs (its launch latency and set-up overlap) and blocks until this grid has completed and flushed.  Only
+// non-cluster launches on the main chain take the attribute, and only in the latency-bound regime (maml_b200_create)
+// unless MAML_B200_PDL says otherwise.
 // ---------------------------------------------------------------------------------------------
 inline bool pdl_allowed(cudaStream_t st) {
   const LaunchContext& c = launch_ctx();
-  return c.pdl_mode == 1 || (c.pdl_mode == 2 && st == c.main_stream) || (c.pdl_mode == 3 && st != c.wg_stream);
+  return c.pdl && st == c.main_stream;
 }
 int num_sms();                     // streaming multiprocessors of the current device (queried once)
 

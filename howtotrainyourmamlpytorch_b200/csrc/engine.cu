@@ -59,22 +59,12 @@ static EngineOptions read_options() {
   o.no_graph = getenv("MAML_B200_NO_GRAPH") != nullptr;
   o.one_stream = getenv("MAML_B200_ONE_STREAM") != nullptr;
   o.wgrad_tc = flag("MAML_B200_WGRAD_TC", o.wgrad_tc);
-  o.wgrad_row = flag("MAML_B200_WGRAD_ROW", o.wgrad_row);
   o.tc_split = clamp(num("MAML_B200_TC_SPLIT", o.tc_split), 1, 8);
-  o.tc_split_side = num("MAML_B200_TC_SPLIT_SIDE", o.tc_split_side);
   if (getenv("MAML_B200_TC_NB")) o.tc_nb = clamp(num("MAML_B200_TC_NB", 0), 2, 8);
-  o.tc_nb_side = num("MAML_B200_TC_NB_SIDE", o.tc_nb_side);
-  o.tc_nb_fit = flag("MAML_B200_TC_NB_FIT", o.tc_nb_fit);
-  o.tc_push = flag("MAML_B200_TC_PUSH", o.tc_push);
-  o.tc_zstage = flag("MAML_B200_TC_ZSTAGE", o.tc_zstage);
   o.bn_fuse = flag("MAML_B200_BN_FUSE", o.bn_fuse);
-  o.bn_side_cap = num("MAML_B200_BN_SIDE_CAP", o.bn_side_cap);
   o.tail_fuse = flag("MAML_B200_TAIL_FUSE", o.tail_fuse);
   o.tail_onchip = num("MAML_B200_TAIL_ONCHIP", o.tail_onchip);
-  o.tan_split = flag("MAML_B200_TAN_SPLIT", o.tan_split);
-  o.tgt_slots = std::max(1, num("MAML_B200_TGT_SLOTS", o.tgt_slots));
-  o.pdl = num("MAML_B200_PDL", o.pdl);
-  o.pdl_cluster = num("MAML_B200_PDL_CLUSTER", o.pdl_cluster);
+  if (const char* v = getenv("MAML_B200_PDL")) o.pdl = atoi(v) != 0 ? 1 : 0;
   if (getenv("MAML_B200_TC_TIMELINE")) o.tc_timeline = std::max(0, num("MAML_B200_TC_TIMELINE", 0));
   if (const char* v = getenv("MAML_B200_GRAPH_DOT")) o.graph_dot = v;
   return o;
@@ -128,11 +118,11 @@ struct maml_b200_handle {
   bool profiling = false;             // maml_b200_profile(h, 1): this handle's launches are recorded into prof
   // side streams / events for fork-join inside one iteration, CUDA-graph cache
   cudaStream_t s_cap = nullptr, s_tgt = nullptr, s_tgt2 = nullptr, s_wg = nullptr;
-  int tgt_slots = 1;       // target passes of consecutive steps are independent: double-buffered on two streams
+  int tgt_slots = 1;       // target passes of consecutive steps are independent: double-buffered on two streams (min(S, 2))
   cudaEvent_t ev_fork = nullptr, ev_wg = nullptr, ev_pack = nullptr, ev_tgt[MAML_MAX_STEPS] = {};
   cudaEvent_t ev_pre[2 * MAML_MAX_LAYERS] = {};     // tangent pre-computed addends: [l] forward conv, [MAX_LAYERS + l] dgrad
   bool use_graphs = true;
-  int pdl_mode = 0;                                   // programmatic dependent launch (see common.cuh), chosen per handle
+  bool pdl = false;                                   // programmatic dependent launch on the main chain (see common.cuh)
   int nb_main = 8;                                    // shared-memory B ring depth of the tensor-core conv kernel (see maml_b200_create)
   // results produced on s_wg (upper-block parameter reduction, weight packs) that the main chain has not joined yet:
   // consumed right before the first kernel that reads them (block 1's convolution / the head)
@@ -154,19 +144,19 @@ struct maml_b200_handle {
 
 // launch context of the handle call in progress on this thread (common.cuh); the default one has PDL off
 static const EngineOptions g_default_options;
-static thread_local LaunchContext g_launch_ctx{&g_default_options, 0, nullptr, nullptr, nullptr};
+static thread_local LaunchContext g_launch_ctx{&g_default_options, false, nullptr, nullptr};
 const LaunchContext& launch_ctx() { return g_launch_ctx; }
 
 // Installs a handle's launch context for the duration of one call and restores the previous one.  Calls that enqueue an
 // iteration chain pass its main stream and launch with the handle's PDL mode; the other calls launch without PDL.
 struct LaunchScope {
   LaunchContext saved;
-  explicit LaunchScope(maml_b200_handle* h) : LaunchScope(h, 0, nullptr) {}
-  LaunchScope(maml_b200_handle* h, cudaStream_t main) : LaunchScope(h, h->pdl_mode, main) {}
+  explicit LaunchScope(maml_b200_handle* h) : LaunchScope(h, false, nullptr) {}
+  LaunchScope(maml_b200_handle* h, cudaStream_t main) : LaunchScope(h, h->pdl, main) {}
   ~LaunchScope() { g_launch_ctx = saved; }
  private:
-  LaunchScope(maml_b200_handle* h, int pdl_mode, cudaStream_t main) : saved(g_launch_ctx) {
-    g_launch_ctx = LaunchContext{&h->opt, pdl_mode, main, h->s_wg, h->profiling ? &h->prof : nullptr};
+  LaunchScope(maml_b200_handle* h, bool pdl, cudaStream_t main) : saved(g_launch_ctx) {
+    g_launch_ctx = LaunchContext{&h->opt, pdl, main, h->profiling ? &h->prof : nullptr};
   }
 };
 
@@ -246,8 +236,7 @@ static void plan_chunks(maml_b200_handle* h, int n, ChunkPlan* cp) {
       // the FMA pipe fed with 8 warps): a second CTA per SM would take the register file away from the main chain's kernels
       // running beside it; 3 filter rows x tasks x
       // chunks should just fill one slot per SM -- 720 CTAs (128-row chunks at 8 tasks) ran as 1.2 waves = 2x the time
-      const int wg_per_chunk = h->opt.wgrad_row ? 3 : 9;
-      long long want = std::max<long long>(1, num_sms() / ((long long)wg_per_chunk * h->maxT));
+      long long want = std::max<long long>(1, num_sms() / (3LL * h->maxT));
       nch = (int)std::min<long long>(std::min<long long>(64, want), std::max<long long>(1, (rows + 15) / 16));
     }
     rpc = (int)rup((rows + nch - 1) / nch, 16);
@@ -364,7 +353,7 @@ static void carve_pass(maml_b200_handle* h, Bump& b, PassSet& ps, int n, int slo
 static void carve(maml_b200_handle* h, Bump& b) {
   const long long T = h->maxT;
   carve_pass(h, b, h->sup, h->n_s, h->S, true, true);
-  h->tgt_slots = std::min(h->S, h->opt.tgt_slots);
+  h->tgt_slots = std::min(h->S, 2);
   carve_pass(h, b, h->tgt, h->n_t, (h->cfg.reserved & 1) ? h->S : h->tgt_slots, true, true);   // reserved bit 0: keep every target pass (tests)
   carve_pass(h, b, h->tan, h->n_s, 1, false, true);
   carve_pass(h, b, h->tan2, h->n_s, 1, false, true);
@@ -417,8 +406,13 @@ extern "C" int maml_b200_create(const maml_b200_config* cfg, maml_b200_handle** 
   build_layout(h);
   // tensor-core (wgmma / TMA, 3xTF32) convolutions for blocks l >= 1; reserved bit 1 forces the fp32 FFMA kernels (tests)
   h->use_tc = (h->L > 1) && !(cfg->reserved & 2);
-  for (int l = 1; l < h->L && h->use_tc; ++l)
-    if (tc_conv_rpad(h->geo[l].gw) > 256 || tc_conv_ring(h->F, h->geo[l].gw) < 2) h->use_tc = false;   // image too wide for one halo box      // F in {16, 32, 48, 64}: ragged K chunks are zero-filled by TMA
+  // (any F in {16, 32, 48, 64}: ragged K chunks are zero-filled by TMA).  The image must fit one halo box, and a ring of
+  // 2 B stages must fit next to the halo buffers and the largest buffer behind the ring, which is that of split-K over 2
+  // CTAs in tangent mode (receive buffer + 64 staged primal zh rows; S = 1 stages 128 rows, larger S fewer)
+  for (int l = 1; l < h->L && h->use_tc; ++l) {
+    const int gw = h->geo[l].gw;
+    if (tc_conv_rpad(gw) > 256 || tc_conv_ring(h->F, gw, tc_conv_extra_bytes(h->F, 2, true)) < 2) h->use_tc = false;
+  }
   plan_chunks(h, h->n_s, &h->plan_sup);
   plan_chunks(h, h->n_t, &h->plan_tgt);
   Bump sz{nullptr, 0};
@@ -445,7 +439,7 @@ extern "C" int maml_b200_create(const maml_b200_config* cfg, maml_b200_handle** 
     const int l1 = h->L > 1 ? 1 : 0;
     const long long tiles = (((long long)h->n_s * h->geo[l1].G + 127) / 128 + ((long long)h->n_t * h->geo[l1].G + 127) / 128) * h->maxT;
     const bool small = tiles <= num_sms();
-    h->pdl_mode = h->opt.pdl >= 0 ? h->opt.pdl : (small ? 2 : 0);
+    h->pdl = h->opt.pdl >= 0 ? h->opt.pdl != 0 : small;
     h->nb_main = h->opt.tc_nb > 0 ? h->opt.tc_nb : (small ? 8 : 4);
   }
   // Priorities: the support chain (capture stream) is the critical path; the weight-gradient and target streams only
@@ -604,28 +598,22 @@ static void join_pending(maml_b200_handle* h, cudaStream_t st) {
   h->wg_pending = false;
 }
 
-static void tc_conv(maml_b200_handle* h, int l, int n, int nsrc, const TcOp* ops, const float* bias, long long bias_stride,
+static void tc_conv(maml_b200_handle* h, int l, int n, const TcOp& op, const float* bias, long long bias_stride,
                     float* out, long long out_stride, int mode, const float* zh, long long zh_stride, double* stats, int T,
                     cudaStream_t st) {
   const LayerGeom& g = h->geo[l];
   TcMaps maps;
   TcConvArgs a{};
-  a.nsrc = nsrc; a.kc = h->F; a.rows = n * g.G; a.gw = g.gw; a.G = g.G; a.h = g.h; a.w = g.w; a.ncols = h->F; a.mode = mode; a.tasks = T; a.plan_tasks = h->maxT;
-  const bool side = on_side_stream(st);
-  a.split_cap = side ? h->opt.tc_split_side : 0;
+  a.kc = h->F; a.rows = n * g.G; a.gw = g.gw; a.G = g.G; a.h = g.h; a.w = g.w; a.ncols = h->F; a.mode = mode; a.tasks = T; a.plan_tasks = h->maxT;
   a.halo = g.gw + 1; a.rpad = tc_conv_rpad(g.gw); a.nb = std::min(tc_conv_ring(h->F, g.gw), h->nb_main);
-  if (side && h->opt.tc_nb_side >= 2 && a.nb > h->opt.tc_nb_side) a.nb = h->opt.tc_nb_side;
   a.timeline = (h->opt.tc_timeline == 0 || h->opt.tc_timeline == l) ? 1 : 0;
-  for (int s = 0; s < nsrc; ++s) {
-    maps.m[s * 4 + 0] = ops[s].a_maps[0]; maps.m[s * 4 + 1] = ops[s].a_maps[1];
-    maps.m[s * 4 + 2] = ops[s].b_maps[ops[s].b_pair]; maps.m[s * 4 + 3] = ops[s].b_maps[ops[s].b_pair + 1];
-    a.a_row_base[s] = ops[s].a_row_base; a.a_task_rows[s] = ops[s].a_task_rows; a.sign[s] = ops[s].sign;
-    a.b_row_base[s] = ops[s].b_row_base; a.b_task_rows[s] = ops[s].b_task_rows;
-  }
-  if (nsrc == 1) for (int k = 4; k < 8; ++k) maps.m[k] = maps.m[k - 4];
+  maps.m[0] = op.a_maps[0]; maps.m[1] = op.a_maps[1];
+  maps.m[2] = op.b_maps[op.b_pair]; maps.m[3] = op.b_maps[op.b_pair + 1];
+  a.a_row_base = op.a_row_base; a.a_task_rows = op.a_task_rows; a.sign = op.sign;
+  a.b_row_base = op.b_row_base; a.b_task_rows = op.b_task_rows;
   a.bias = bias; a.bias_stride = bias_stride; a.out = out; a.out_stride = out_stride;
   a.zh = zh; a.zh_stride = zh_stride; a.stats = stats; a.stats_stride = h->stats_task_stride;
-  a.alg_flops = conv_flops(h, l, n, T, nsrc);
+  a.alg_flops = conv_flops(h, l, n, T, 1);
   launch_conv_tc(maps, a, st);
 }
 
@@ -646,8 +634,8 @@ static void forward_pass(maml_b200_handle* h, const PassSet& ps, int slot, const
       a.alg_flops = conv_flops(h, 0, ps.n, T, 1);
       launch_conv0(a, st);
     } else if (h->use_tc) {
-      TcOp op = tc_op_ain(h, ps, l, slot, h->theta_map, th_step, +1, 2);
-      tc_conv(h, l, ps.n, 1, &op, theta + h->pl.b_off[l], h->Ppad, ZH(ps, l, slot), STRIDE(ps, zh, l), CONV_FWD_STATS, nullptr, 0,
+      tc_conv(h, l, ps.n, tc_op_ain(h, ps, l, slot, h->theta_map, th_step, +1, 2), theta + h->pl.b_off[l], h->Ppad,
+              ZH(ps, l, slot), STRIDE(ps, zh, l), CONV_FWD_STATS, nullptr, 0,
               stat_at(h, stat_kind, bn_step, l), T, st);
     } else {
       ConvArgs a{};
@@ -715,8 +703,8 @@ static void backward_pass(maml_b200_handle* h, const PassSet& ps, int slot, cons
       w.alg_flops = conv_flops(h, l, ps.n, T, 1);
       // dgrad (critical path) is enqueued before the side-stream wgrad so that its CTAs get SMs first
       if (h->use_tc) {
-        TcOp op = tc_op_dz(h, ps, l, slot, h->theta_map, th_step, -1, 0);
-        tc_conv(h, l, ps.n, 1, &op, nullptr, 0, DP(ps, l - 1, slot), STRIDE(ps, dp, l - 1), CONV_PLAIN, nullptr, 0, nullptr, T, st);
+        tc_conv(h, l, ps.n, tc_op_dz(h, ps, l, slot, h->theta_map, th_step, -1, 0), nullptr, 0, DP(ps, l - 1, slot),
+                STRIDE(ps, dp, l - 1), CONV_PLAIN, nullptr, 0, nullptr, T, st);
       } else {
         ConvArgs a{};
         a.nsrc = 1;
@@ -760,22 +748,21 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
   // on what phase A saved, not on the tangent chain.  It is computed up front on the side stream (right behind the
   // u packs) into the tan2 buffers -- BatchNorm statistics contributions included, they are linear -- and the
   // consumers (bnact_tan / bnbwd_tan) add the two addends.  The main chain keeps the single-pair half: 18 instead of
-  // 36 stages per tile on the critical path.
-  const bool split = h->use_tc && h->opt.tan_split;
+  // 36 stages per tile on the critical path.  The FFMA convs (no tensor-core path) take both pairs in one launch.
   // the fused last-block kernels implement the cross-entropy tangent head only
   const bool fuse_tail = th.mode == HEAD_TANGENT && h->opt.tail_fuse && tail_fusable(bn_geom(h, h->L - 1, sp.n), sp.n, head_rows(sp.n));
   BnActTanArgs last_act{};
   HeadArgs hd{};
-  if (split) {
+  if (h->use_tc) {
     for (int l = 1; l < h->L; ++l) {
-      TcOp op = tc_op_ain(h, sp, l, s, h->u_map, 0, +1, 2);          // conv(a_in, u_W) + u_b
-      tc_conv(h, l, sp.n, 1, &op, u + h->pl.b_off[l], h->Ppad, ZH(t2, l, 0), STRIDE(t2, zh, l), CONV_TAN_STATS, ZH(sp, l, s),
+      tc_conv(h, l, sp.n, tc_op_ain(h, sp, l, s, h->u_map, 0, +1, 2),          // conv(a_in, u_W) + u_b
+              u + h->pl.b_off[l], h->Ppad, ZH(t2, l, 0), STRIDE(t2, zh, l), CONV_TAN_STATS, ZH(sp, l, s),
               STRIDE(sp, zh, l), stat_at(h, PASS_TAN_FWD, s, l), T, spre);
       cudaEventRecord(h->ev_pre[l], spre);
     }
     for (int l = h->L - 1; l >= 1; --l) {
-      TcOp op = tc_op_dz(h, sp, l, s, h->u_map, 0, -1, 0);           // dgrad(u_W, dz)
-      tc_conv(h, l, sp.n, 1, &op, nullptr, 0, DP(t2, l - 1, 0), STRIDE(t2, dp, l - 1), CONV_PLAIN, nullptr, 0, nullptr, T, spre);
+      tc_conv(h, l, sp.n, tc_op_dz(h, sp, l, s, h->u_map, 0, -1, 0),           // dgrad(u_W, dz)
+              nullptr, 0, DP(t2, l - 1, 0), STRIDE(t2, dp, l - 1), CONV_PLAIN, nullptr, 0, nullptr, T, spre);
       cudaEventRecord(h->ev_pre[MAML_MAX_LAYERS + l], spre);
     }
   }
@@ -793,17 +780,11 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
       a.stats = stat_at(h, PASS_TAN_FWD, s, 0); a.stats_stride = h->stats_task_stride; a.tasks = T;
       a.alg_flops = conv_flops(h, 0, sp.n, T, 1);
       launch_conv0(a, st);
-    } else if (split) {
-      TcOp op = tc_op_ain(h, tn, l, 0, h->theta_map, s, +1, 2);       // conv(a_in_dot, W); the other addend is in tan2
-      tc_conv(h, l, sp.n, 1, &op, nullptr, 0, ZH(tn, l, 0), STRIDE(tn, zh, l), CONV_TAN_STATS, ZH(sp, l, s),
+    } else if (h->use_tc) {
+      tc_conv(h, l, sp.n, tc_op_ain(h, tn, l, 0, h->theta_map, s, +1, 2),       // conv(a_in_dot, W); the other addend is in tan2
+              nullptr, 0, ZH(tn, l, 0), STRIDE(tn, zh, l), CONV_TAN_STATS, ZH(sp, l, s),
               STRIDE(sp, zh, l), stat_at(h, PASS_TAN_FWD, s, l), T, st);
       cudaStreamWaitEvent(st, h->ev_pre[l], 0);
-    } else if (h->use_tc) {
-      TcOp ops[2];
-      ops[0] = tc_op_ain(h, sp, l, s, h->u_map, 0, +1, 2);          // conv(a_in, u_W)
-      ops[1] = tc_op_ain(h, tn, l, 0, h->theta_map, s, +1, 2);      // conv(a_in_dot, W)
-      tc_conv(h, l, sp.n, 2, ops, u + h->pl.b_off[l], h->Ppad, ZH(tn, l, 0), STRIDE(tn, zh, l), CONV_TAN_STATS, ZH(sp, l, s),
-              STRIDE(sp, zh, l), stat_at(h, PASS_TAN_FWD, s, l), T, st);
     } else {
       ConvArgs a{};
       a.nsrc = 2;
@@ -821,7 +802,7 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
     }
     BnActTanArgs b{};
     b.zdot = ZH(tn, l, 0); b.zdot_stride = STRIDE(tn, zh, l);
-    if (split && l >= 1) b.zdot2 = ZH(t2, l, 0);
+    if (h->use_tc && l >= 1) b.zdot2 = ZH(t2, l, 0);
     b.zh = ZH(sp, l, s); b.zh_stride = STRIDE(sp, zh, l);
     b.stats_fwd = stat_at(h, PASS_SUP_FWD, s, l); b.stats_fwd_stride = h->stats_task_stride;
     b.stats_tan = stat_at(h, PASS_TAN_FWD, s, l); b.stats_tan_stride = h->stats_task_stride;
@@ -859,7 +840,7 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
     BnBwdTanArgs b{};
     b.dp = DP(sp, l, s); b.dp_stride = STRIDE(sp, dp, l);
     b.dpdot = DP(tn, l, 0); b.dpdot_stride = STRIDE(tn, dp, l);
-    if (split && l + 1 < h->L) { b.dpdot2 = DP(t2, l, 0); cudaStreamWaitEvent(st, h->ev_pre[MAML_MAX_LAYERS + l + 1], 0); }
+    if (h->use_tc && l + 1 < h->L) { b.dpdot2 = DP(t2, l, 0); cudaStreamWaitEvent(st, h->ev_pre[MAML_MAX_LAYERS + l + 1], 0); }
     b.zh = ZH(sp, l, s); b.zh_stride = STRIDE(sp, zh, l);
     b.zhdot = ZH(tn, l, 0); b.zhdot_stride = STRIDE(tn, zh, l);
     b.dz = DZ(sp, l, s); b.dz_stride = STRIDE(sp, dz, l);
@@ -893,14 +874,9 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
       w.A[1] = AIN(tn, l, 0); w.a_stride[1] = STRIDE(tn, ain, l);
       w.D[1] = DZ(sp, l, s); w.d_stride[1] = STRIDE(sp, dz, l);
       w.alg_flops = conv_flops(h, l, sp.n, T, 2);
-      if (split) {
-        TcOp op = tc_op_dz(h, tn, l, 0, h->theta_map, s, -1, 0);      // dgrad(W, dz_dot); the other addend is in tan2
-        tc_conv(h, l, sp.n, 1, &op, nullptr, 0, DP(tn, l - 1, 0), STRIDE(tn, dp, l - 1), CONV_PLAIN, nullptr, 0, nullptr, T, st);
-      } else if (h->use_tc) {
-        TcOp ops[2];
-        ops[0] = tc_op_dz(h, tn, l, 0, h->theta_map, s, -1, 0);     // dgrad(W, dz_dot)
-        ops[1] = tc_op_dz(h, sp, l, s, h->u_map, 0, -1, 0);         // dgrad(u_W, dz)
-        tc_conv(h, l, sp.n, 2, ops, nullptr, 0, DP(tn, l - 1, 0), STRIDE(tn, dp, l - 1), CONV_PLAIN, nullptr, 0, nullptr, T, st);
+      if (h->use_tc) {
+        tc_conv(h, l, sp.n, tc_op_dz(h, tn, l, 0, h->theta_map, s, -1, 0),      // dgrad(W, dz_dot); the other addend is in tan2
+                nullptr, 0, DP(tn, l - 1, 0), STRIDE(tn, dp, l - 1), CONV_PLAIN, nullptr, 0, nullptr, T, st);
       } else {
         ConvArgs a{};
         a.nsrc = 2;
@@ -1056,7 +1032,7 @@ static int enqueue_iteration(maml_b200_handle* h, const maml_b200_iter_args* it,
         // while the main chain runs block 0
         // ... on a target stream (idle in phase B) when the u-weight convs are pre-computed there too, so that they do
         // not queue in front of the weight gradients on the wgrad stream
-        cudaStream_t spre = (h->use_tc && h->opt.tan_split) ? h->s_tgt : h->s_wg;
+        cudaStream_t spre = h->use_tc ? h->s_tgt : h->s_wg;
         CK(cudaEventRecord(h->ev_fork, st));
         CK(cudaStreamWaitEvent(spre, h->ev_fork, 0));
         pack_u(h, T, spre);
@@ -1277,7 +1253,7 @@ extern "C" int maml_b200_net_hvp(maml_b200_handle* h, int32_t n_tasks, int32_t n
   launch_head(a, st);
   // the tangent pass reads this backward's dz / dp and statistics; its weight-gradient chunks are overwritten unread
   backward_pass(h, h->sup, s, th, s, meta_like, s, PASS_SUP_FWD, PASS_SUP_BWD, h->sup_partial, h->plan_sup, T, st, false);
-  cudaStream_t spre = (h->use_tc && h->opt.tan_split) ? h->s_tgt : h->s_wg;     // as in the fused reverse sweep
+  cudaStream_t spre = h->use_tc ? h->s_tgt : h->s_wg;     // as in the fused reverse sweep
   CK(cudaEventRecord(h->ev_fork, st));
   CK(cudaStreamWaitEvent(spre, h->ev_fork, 0));
   pack_u(h, T, spre);

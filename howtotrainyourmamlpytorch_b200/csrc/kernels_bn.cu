@@ -110,24 +110,20 @@ __global__ void __launch_bounds__(256) bnact_kernel(BnActArgs a) {
   bnact_phase(a, g, task, blockIdx.x, gridDim.x, it, s_mu, s_r, s_g, s_b);
 }
 
-// launches on a side stream (target passes) take at most the BN_SIDE_CAP option's CTAs, so that the grid-stride
-// BatchNorm kernels can leave SM slots to the main chain
-static inline dim3 bn_grid(const BnGeom& g, int tasks, int* block, cudaStream_t st) {
+static inline dim3 bn_grid(const BnGeom& g, int tasks, int* block) {
   const int F4 = g.F / 4;
   const int wpb = 256 / F4;
   *block = wpb * F4;
   const int NW = g.n * ((g.h + 1) / 2) * ((g.w + 1) / 2);
   int bx = (NW + wpb - 1) / wpb;
   if (bx > 4 * num_sms()) bx = 4 * num_sms();
-  const int cap = on_side_stream(st) ? launch_ctx().opt->bn_side_cap : 0;
-  if (cap > 0 && (long long)bx * tasks > cap) bx = cap / tasks;
   if (bx < 1) bx = 1;
   return dim3(bx, tasks);
 }
 
 void launch_bnact(const BnActArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; dim3 grid = bn_grid(a.g, a.tasks, &block, st);
+  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
   launch_pdl(bnact_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();
 }
@@ -278,7 +274,7 @@ __global__ void __launch_bounds__(256) bnbwd_reduce_kernel(BnBwdArgs a) {
 
 void launch_bnbwd_reduce(const BnBwdArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; dim3 grid = bn_grid(a.g, a.tasks, &block, st);
+  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
   if ((int)grid.x > num_sms()) grid.x = num_sms();
   launch_pdl(bnbwd_reduce_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();
@@ -385,12 +381,10 @@ template <class A>
 static inline void launch_cluster(void (*kernel)(A), const A& a, int cl, int tasks, int block, cudaStream_t st) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(cl, tasks); cfg.blockDim = dim3(block); cfg.dynamicSmemBytes = 0; cfg.stream = st;
-  cudaLaunchAttribute attr[2];
+  cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = cl; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = ((launch_ctx().opt->pdl_cluster & 1) && pdl_allowed(st)) ? 2 : 1;
+  cfg.attrs = attr; cfg.numAttrs = 1;
   cudaLaunchKernelEx(&cfg, kernel, a);
 }
 
@@ -399,14 +393,14 @@ void launch_bnbwd(const BnBwdArgs& a, cudaStream_t st) {
   const int cl = bn_fused_cluster(a.g);
   if (cl == 0) { launch_bnbwd_reduce(a, st); launch_bnbwd_apply(a, st); return; }
   ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; bn_grid(a.g, a.tasks, &block, st);
+  int block; bn_grid(a.g, a.tasks, &block);
   launch_cluster(bnbwd_fused_kernel, tagged(a), cl, a.tasks, block, st);
   CUDA_CHECK_LAUNCH();
 }
 
 void launch_bnbwd_apply(const BnBwdArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; dim3 grid = bn_grid(a.g, a.tasks, &block, st);
+  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
   launch_pdl(bnbwd_apply_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();
 }
@@ -484,7 +478,7 @@ __global__ void __launch_bounds__(256) bnact_tan_kernel(BnActTanArgs a) {
 
 void launch_bnact_tan(const BnActTanArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; dim3 grid = bn_grid(a.g, a.tasks, &block, st);
+  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
   launch_pdl(bnact_tan_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();
 }
@@ -544,7 +538,7 @@ __global__ void __launch_bounds__(256) bnbwd_tan_reduce_kernel(BnBwdTanArgs a) {
 
 void launch_bnbwd_tan_reduce(const BnBwdTanArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; dim3 grid = bn_grid(a.g, a.tasks, &block, st);
+  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
   if ((int)grid.x > num_sms()) grid.x = num_sms();
   launch_pdl(bnbwd_tan_reduce_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();
@@ -649,7 +643,7 @@ __global__ void __launch_bounds__(256) bnbwd_tan_fused_kernel(BnBwdTanArgs a) {
 
 void launch_bnbwd_tan_apply(const BnBwdTanArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; dim3 grid = bn_grid(a.g, a.tasks, &block, st);
+  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
   launch_pdl(bnbwd_tan_apply_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();
 }
@@ -658,7 +652,7 @@ void launch_bnbwd_tan(const BnBwdTanArgs& a, cudaStream_t st) {
   const int cl = bn_fused_cluster(a.g);
   if (cl == 0) { launch_bnbwd_tan_reduce(a, st); launch_bnbwd_tan_apply(a, st); return; }
   ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; bn_grid(a.g, a.tasks, &block, st);
+  int block; bn_grid(a.g, a.tasks, &block);
   launch_cluster(bnbwd_tan_fused_kernel, tagged(a), cl, a.tasks, block, st);
   CUDA_CHECK_LAUNCH();
 }

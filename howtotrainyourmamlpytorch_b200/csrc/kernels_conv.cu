@@ -419,98 +419,12 @@ void launch_conv0(const Conv0Args& a, cudaStream_t st) {
 
 // ---------------------------------------------------------------------------------------------
 // wgrad:  partial[chunk][tap][c][f] = sum_{j in chunk} sum_src A_src[j + s_tap, c] * D_src[j, f]
-//         partial[chunk][bias][f]   = sum_{j in chunk} D_0[j, f]                 (tap 4 CTA)
-// grid (nchunks * 9, tasks); chunks are reduced (in fixed order => deterministic) by the
-// parameter-space kernel that consumes the partial buffer.
+//         partial[chunk][bias][f]   = sum_{j in chunk} D_0[j, f]                 (centre filter row CTA)
+// chunks are reduced (in fixed order => deterministic) by the parameter-space kernel that consumes the partial buffer.
 // ---------------------------------------------------------------------------------------------
-template <int CN, int FN>
-__global__ void __launch_bounds__(256) wgrad_kernel(WgradArgs a) {
-  pdl_prologue(3, a.tag);
-  constexpr int KC = 16 * CN, NC = 16 * FN;
-  __shared__ __align__(16) float As[16][KC];
-  __shared__ __align__(16) float Ds[16][NC];
-  const int task = blockIdx.y;
-  const int chunk = blockIdx.x / 9, tap = blockIdx.x - chunk * 9;
-  const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
-  const int sh = tap_shift(tap, a.gw);
-  const int r_begin = chunk * a.rows_per_chunk;
-  const int r_end = min(a.rows, r_begin + a.rows_per_chunk);
-
-  float acc[CN][FN];
-#pragma unroll
-  for (int i = 0; i < CN; ++i)
-#pragma unroll
-    for (int jn = 0; jn < FN; ++jn) acc[i][jn] = 0.f;
-  float bacc = 0.f;
-
-  const int steps = (r_end > r_begin) ? (r_end - r_begin + 15) / 16 : 0;
-  const int nit = steps * a.nsrc;
-  float4 ra = make_float4(0.f, 0.f, 0.f, 0.f), rd = make_float4(0.f, 0.f, 0.f, 0.f);
-
-  auto fetch = [&](int it) {
-    const int s = it / steps;
-    const int r0 = r_begin + (it - s * steps) * 16;
-    if (tid < 4 * KC) {
-      const int r = tid / (KC / 4), c4 = tid - r * (KC / 4);
-      const int jr = r0 + r;
-      if (jr < r_end)
-        ra = *reinterpret_cast<const float4*>(a.A[s] + (long long)task * a.a_stride[s] + (long long)(jr + sh) * KC + c4 * 4);
-      else
-        ra = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    if (tid < 4 * NC) {
-      const int r = tid / (NC / 4), f4 = tid - r * (NC / 4);
-      const int jr = r0 + r;
-      if (jr < r_end)
-        rd = *reinterpret_cast<const float4*>(a.D[s] + (long long)task * a.d_stride[s] + (long long)jr * NC + f4 * 4);
-      else
-        rd = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-  };
-
-  if (nit > 0) fetch(0);
-  for (int it = 0; it < nit; ++it) {
-    if (tid < 4 * KC) {
-      const int r = tid / (KC / 4), c4 = tid - r * (KC / 4);
-      *reinterpret_cast<float4*>(&As[r][c4 * 4]) = ra;
-    }
-    if (tid < 4 * NC) {
-      const int r = tid / (NC / 4), f4 = tid - r * (NC / 4);
-      *reinterpret_cast<float4*>(&Ds[r][f4 * 4]) = rd;
-    }
-    __syncthreads();
-    const bool bias_src = (it / steps) == 0;
-    if (it + 1 < nit) fetch(it + 1);
-#pragma unroll
-    for (int r = 0; r < 16; ++r) {
-      float av[CN], b[FN];
-#pragma unroll
-      for (int i = 0; i < CN; ++i) av[i] = As[r][ty * CN + i];
-#pragma unroll
-      for (int jn = 0; jn < FN; ++jn) b[jn] = Ds[r][tx * FN + jn];
-#pragma unroll
-      for (int i = 0; i < CN; ++i)
-#pragma unroll
-        for (int jn = 0; jn < FN; ++jn) acc[i][jn] = fmaf(av[i], b[jn], acc[i][jn]);
-    }
-    if (tap == 4 && bias_src && tid < NC) {
-#pragma unroll
-      for (int r = 0; r < 16; ++r) bacc += Ds[r][tid];
-    }
-    __syncthreads();
-  }
-
-  float* P = a.partial + (long long)task * a.partial_task_stride + (long long)chunk * a.chunk_stride;
-#pragma unroll
-  for (int i = 0; i < CN; ++i)
-#pragma unroll
-    for (int jn = 0; jn < FN; ++jn) P[(long long)(tap * KC + ty * CN + i) * NC + tx * FN + jn] = acc[i][jn];
-  if (tap == 4 && tid < NC) P[(long long)9 * KC * NC + tid] = bacc;
-}
-
-// Filter-row variant: one CTA handles the three taps (ky, kx = -1, 0, +1) of a chunk.  Their A rows are CONSECUTIVE
+// One CTA handles the three taps (ky, kx = -1, 0, +1) of one filter row and chunk.  Their A rows are CONSECUTIVE
 // (shifts s-1, s, s+1), so while a thread walks the rows of a K step it keeps a sliding window of three A rows in
-// registers: per row 2 x LDS.128 feed 3 x CN x FN FMAs (the one-tap kernel above needs 2 x LDS.128 per CN x FN), the
+// registers: per row 2 x LDS.128 feed 3 x CN x FN FMAs (one tap per CTA would need 2 x LDS.128 per CN x FN), the
 // dz tile is staged once for three taps and the number of barriers per FMA drops 3x.  grid (nchunks * 3, tasks).
 template <int CN, int FN>
 __global__ void __launch_bounds__(256) wgrad_row_kernel(WgradArgs a) {
@@ -624,16 +538,10 @@ __global__ void __launch_bounds__(256) wgrad_row_kernel(WgradArgs a) {
 void launch_wgrad(const WgradArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_WGRAD, a.alg_flops, st);
   const int cn = a.kc / 16, fn = a.ncols / 16;
-  if (launch_ctx().opt->wgrad_row) {
-    dim3 grid(a.nchunks * 3, a.tasks);
+  dim3 grid(a.nchunks * 3, a.tasks);
 #define WGR_CASE(C, F_) if (cn == C && fn == F_) { launch_pdl(wgrad_row_kernel<C, F_>, dim3(grid), dim3(256), (size_t)(0), st, tagged(a)); CUDA_CHECK_LAUNCH(); return; }
-    WGR_CASE(1, 1) WGR_CASE(2, 2) WGR_CASE(3, 3) WGR_CASE(4, 4)
+  WGR_CASE(1, 1) WGR_CASE(2, 2) WGR_CASE(3, 3) WGR_CASE(4, 4)
 #undef WGR_CASE
-  }
-  dim3 grid(a.nchunks * 9, a.tasks);
-#define WG_CASE(C, F_) if (cn == C && fn == F_) { launch_pdl(wgrad_kernel<C, F_>, dim3(grid), dim3(256), (size_t)(0), st, tagged(a)); CUDA_CHECK_LAUNCH(); return; }
-  WG_CASE(1, 1) WG_CASE(2, 2) WG_CASE(3, 3) WG_CASE(4, 4)
-#undef WG_CASE
 }
 
 // first block wgrad: A = image matrix [rows][c0] (c0 <= 4), D = dz [rows][F].

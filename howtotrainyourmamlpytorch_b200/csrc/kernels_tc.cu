@@ -1,9 +1,10 @@
 // wgmma / TMA implicit-GEMM 3x3 convolution for sm_90a, fp32-faithful via the 3xTF32 operand split.
 //
-//   out[j, n] = sum_src sum_tap sum_k A_src[j +/- s_tap, k] * B_src[tap][n][k]        (fp32 result)
+//   out[j, n] = sum_tap sum_k A[j +/- s_tap, k] * B[tap][n][k]        (fp32 result)
 //
-// Used for the forward conv, the tangent conv (two operand pairs), dgrad and tangent dgrad of blocks
-// l >= 1 (reference meta_neural_network_architectures.py:89-97 and its autograd derivatives).
+// Used for the forward conv, the tangent conv, dgrad and tangent dgrad of blocks l >= 1 (reference
+// meta_neural_network_architectures.py:89-97 and its autograd derivatives).  One operand pair per launch: the two pairs
+// of a tangent conv run as two launches whose outputs the BatchNorm kernels add.
 //
 // Why it maps to plain 2-D TMA tiles: activations live on the zero-padded pixel grid (common.cuh), so the A
 // operand of filter tap (ky,kx) is the SAME [rows, C] matrix shifted by s_tap rows -- every (tap, k-chunk)
@@ -22,6 +23,7 @@
 // warpgroup (one TMA thread; setmaxnreg moves its registers to the consumers).  Warps 0..3 then run the epilogue (+ bias, coalesced global store, fp64 BatchNorm statistics).  Shared-memory
 // B ring with mbarrier full/empty pairs; a stage is released once wgmma.wait_group shows its MMAs complete.
 #include <cuda.h>
+#include <algorithm>
 #include <map>
 #include <utility>
 #include "common.cuh"
@@ -144,56 +146,16 @@ __device__ __forceinline__ uint32_t dsmem_addr(uint32_t local, uint32_t rank) {
 __device__ __forceinline__ void dsmem_st4(uint32_t addr, float4 v) {
   asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
-__device__ __forceinline__ float4 dsmem_ld4(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-  return v;
-}
 
-// Split-K reduction of one output tile across the S CTAs of a cluster.  CTA `zrank` finishes rows [zrank * 128/S, ...):
-// every thread first issues ALL its distributed-shared-memory loads (S per float4 item, compile-time unrolled), then
-// sums them in rank order (deterministic), adds the bias and writes global memory + a local copy for the statistics.
-template <int NCOLS, int S>
-__device__ __forceinline__ void splitk_reduce(uint32_t tile_local, int zrank, int et, const float* __restrict__ bias,
-                                              float* __restrict__ tile2, float* __restrict__ out, int j0, int rows) {
-  constexpr int P4 = NCOLS + 4;                         // partial-tile pitch (floats), keeps rows 16-byte aligned
-  constexpr int ROWS = 128 / S;
-  constexpr int TOTAL4 = ROWS * (NCOLS / 4);
-  constexpr int ITEMS = (TOTAL4 + 127) / 128;
-  float4 v[ITEMS][S];
-#pragma unroll
-  for (int it = 0; it < ITEMS; ++it) {
-    const int idx = et + it * 128;
-    const int rr = idx / (NCOLS / 4), c4 = idx - rr * (NCOLS / 4);
-    const uint32_t off = (uint32_t)(((zrank * ROWS + rr) * P4 + c4 * 4) * 4);
-#pragma unroll
-    for (int z = 0; z < S; ++z)
-      v[it][z] = (idx < TOTAL4) ? dsmem_ld4(dsmem_addr(tile_local + off, (uint32_t)z)) : make_float4(0.f, 0.f, 0.f, 0.f);
-  }
-#pragma unroll
-  for (int it = 0; it < ITEMS; ++it) {
-    const int idx = et + it * 128;
-    if (idx >= TOTAL4) continue;
-    const int rr = idx / (NCOLS / 4), c4 = idx - rr * (NCOLS / 4);
-    float4 acc = v[it][0];
-#pragma unroll
-    for (int z = 1; z < S; ++z) { acc.x += v[it][z].x; acc.y += v[it][z].y; acc.z += v[it][z].z; acc.w += v[it][z].w; }
-    if (bias) { acc.x += bias[c4 * 4]; acc.y += bias[c4 * 4 + 1]; acc.z += bias[c4 * 4 + 2]; acc.w += bias[c4 * 4 + 3]; }
-    *reinterpret_cast<float4*>(tile2 + rr * P4 + c4 * 4) = acc;
-    const int g = j0 + zrank * ROWS + rr;
-    if (g < rows) *reinterpret_cast<float4*>(out + (long long)g * NCOLS + c4 * 4) = acc;
-  }
-}
-
-
-// Push-based variant (default): every CTA has already WRITTEN the rows it does not own into the owner's receive buffer
+// Split-K reduction of one output tile across the S CTAs of a cluster.  CTA `zrank` finishes rows [zrank * 128/S, ...).
+// Every CTA has already WRITTEN the rows it does not own into the owner's receive buffer
 // recv[source rank][128 / S rows][NCOLS + 4] (st.shared::cluster, before the one cluster barrier), so the owner sums S
-// LOCAL buffers -- no remote load latency, and nobody reads a peer's shared memory after the barrier, so the second
-// cluster barrier ("do not exit while a peer still reads") is gone.  Same summation order as the pull variant.
+// LOCAL buffers in rank order (deterministic), adds the bias and writes global memory + a local copy for the statistics.
+// Nobody reads a peer's shared memory after the barrier, so no second barrier keeps a CTA alive for its peers.
 template <int NCOLS, int S>
-__device__ __forceinline__ void splitk_reduce_local(const float* __restrict__ recv, int zrank, int et, const float* __restrict__ bias,
-                                                    float* __restrict__ tile2, float* __restrict__ out, int j0, int rows) {
-  constexpr int P4 = NCOLS + 4;
+__device__ __forceinline__ void splitk_reduce(const float* __restrict__ recv, int zrank, int et, const float* __restrict__ bias,
+                                              float* __restrict__ tile2, float* __restrict__ out, int j0, int rows) {
+  constexpr int P4 = NCOLS + 4;                         // receive / tile pitch (floats), keeps rows 16-byte aligned
   constexpr int ROWS = 128 / S;
   constexpr int TOTAL4 = ROWS * (NCOLS / 4);
   constexpr int ITEMS = (TOTAL4 + 127) / 128;
@@ -255,20 +217,21 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
   const int task = blockIdx.y;
   const int j0 = blockIdx.x * 128;
   if (threadIdx.x == 0) TC_MARK(0);
-  const int kchunks = (a.kc + 31) >> 5;          // a ragged last chunk (kc = 16 or 48) is zero-filled by TMA
-  const int nph = a.nsrc * kchunks;              // A phases: (source, k-chunk); 9 taps each
+  const int nph = (a.kc + 31) >> 5;              // A phases = k-chunks (a ragged last one, kc = 16 or 48, is zero-filled
+                                                 // by TMA); 9 taps each
   const int nb = a.nb;                           // B ring depth
   // split-K: the gridDim.z CTAs of a cluster share one output tile; CTA z accumulates stages [st_lo, st_hi) of the
   // nph * 9 (phase, tap) stages and the partial tiles are summed through distributed shared memory in the epilogue
   const int nsplit = (int)gridDim.z, zrank = (int)blockIdx.z;
   const int st_lo = zrank * (nph * 9) / nsplit, st_hi = (zrank + 1) * (nph * 9) / nsplit;
   const int ph_lo = st_lo / 9;
-  // push variant: a CTA writes into its peers' shared memory as soon as ITS accumulators are done, so every CTA of the
-  // cluster must be known to have started by then: arrive here, wait right before the first remote store (free by then)
-  if (nsplit > 1 && a.push) cluster_arrive_relaxed();
+  // a CTA writes into its peers' shared memory as soon as ITS accumulators are done, so every CTA of the cluster must be
+  // known to have started by then: arrive here, wait right before the first remote store (free by then)
+  if (nsplit > 1) cluster_arrive_relaxed();
   const int abuf = a.rpad * 128;                 // bytes of one A halo buffer (hi or lo)
   uint8_t* bring = smem + 4 * (size_t)abuf;
-  float* zbuf = reinterpret_cast<float*>(bring + (size_t)nb * BSTAGE + ((nsplit > 1 && a.push) ? (size_t)128 * P4 * 4 : 0));
+  float* recv = reinterpret_cast<float*>(bring + (size_t)nb * BSTAGE);   // split-K receive buffer [128][P4]
+  float* zbuf = recv + (nsplit > 1 ? 128 * P4 : 0);                       // tangent mode: primal zh rows [128 / S][P4]
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < 2; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 8); }
@@ -297,44 +260,42 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     // producer warpgroup: gives registers to the consumers (their five accumulators take 5 x NCOLS / 2 per thread)
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
     if (warp == 8 && lane == 0) {
-      // ===== TMA producer: per phase (source, k-chunk) ONE halo tile of A (hi, lo) that all 9 taps read at row offsets,
+      // ===== TMA producer: per phase (k-chunk) ONE halo tile of A (hi, lo) that all 9 taps read at row offsets,
       // double-buffered so that phase ph+1 streams in while the MMAs of phase ph run; per (phase, tap) one (B_hi, B_lo)
       // stage through the ring
       int stage = 0; uint32_t bphase = 0;
       for (int st = st_lo; st < st_hi; ++st) {
         const int ph = st / 9, tap = st - ph * 9;
-        const int s = ph / kchunks;
-        const int kc0 = (ph - s * kchunks) << 5;
+        const int kc0 = ph << 5;
         if (tap == 0 || st == st_lo) {
           const int lp = ph - ph_lo;
           const int ab = lp & 1;
           mbar_wait(&a_empty[ab], (((uint32_t)lp >> 1) & 1u) ^ 1u);
-          const int arow = a.a_row_base[s] + task * a.a_task_rows[s] + j0 - a.halo;
+          const int arow = a.a_row_base + task * a.a_task_rows + j0 - a.halo;
           const uint32_t ad = smem_u32(smem + (size_t)ab * 2 * abuf);
           mbar_arrive_expect_tx(&a_full[ab], 2u * (uint32_t)abuf);
-          tma_load_2d(ad, &maps.m[s * 4 + 0], &a_full[ab], kc0, arow);
-          tma_load_2d(ad + abuf, &maps.m[s * 4 + 1], &a_full[ab], kc0, arow);
+          tma_load_2d(ad, &maps.m[0], &a_full[ab], kc0, arow);
+          tma_load_2d(ad + abuf, &maps.m[1], &a_full[ab], kc0, arow);
         }
         mbar_wait(&b_empty[stage], bphase ^ 1u);
-        const int brow = a.b_row_base[s] + task * a.b_task_rows[s] + tap * NCOLS;
+        const int brow = a.b_row_base + task * a.b_task_rows + tap * NCOLS;
         const uint32_t bd = smem_u32(bring + (size_t)stage * BSTAGE);
         mbar_arrive_expect_tx(&b_full[stage], BSTAGE);
-        tma_load_2d(bd, &maps.m[s * 4 + 2], &b_full[stage], kc0, brow);
-        tma_load_2d(bd + B_BYTES, &maps.m[s * 4 + 3], &b_full[stage], kc0, brow);
+        tma_load_2d(bd, &maps.m[2], &b_full[stage], kc0, brow);
+        tma_load_2d(bd + B_BYTES, &maps.m[3], &b_full[stage], kc0, brow);
         if (++stage == nb) { stage = 0; bphase ^= 1u; }
       }
     }
     __syncwarp();
     if (nsplit > 1) {                            // the cluster barriers of the consumers' split-K epilogue, same sequence
-      if (a.push) cluster_wait();
+      cluster_wait();
       cluster_sync_all();
-      if (!a.push) cluster_sync_all();
     }
   } else {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
     // ===== consumers: warpgroup wg computes tile rows [64 wg, 64 wg + 64)
     const int wg = warp >> 2;
-    if (a.zstage && threadIdx.x < 128) {
+    if (a.mode == CONV_TAN_STATS && threadIdx.x < 128) {
       // tangent mode: the statistics below need the primal zh of the rows this CTA finishes.  Copy them into shared
       // memory first (coalesced float4 loads, a region of its own behind the ring / receive buffer) -- the statistics
       // loop then reads shared memory instead of one dependent global load per row
@@ -359,7 +320,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     int stage = 0; uint32_t bphase = 0;
     int prev_stage = -1, prev_ab = -1;           // operands of the previous stage, released once its MMAs have completed
     uint64_t ahd = 0, ald = 0;
-    int sgn = 1, ab = 0;
+    int ab = 0;
     for (int st = st_lo; st < st_hi; ++st) {
       const int ph = st / 9, tap = st - ph * 9;
       if (tap == 0 || st == st_lo) {
@@ -370,12 +331,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
         const uint32_t a_hi = smem_u32(smem + (size_t)ab * 2 * abuf) + (uint32_t)(wg * 64 * 128);
         ahd = desc_base + (uint64_t)(a_hi >> 4);
         ald = ahd + (uint64_t)(abuf >> 4);
-        sgn = a.sign[ph / kchunks];
       }
       mbar_wait(&b_full[stage], bphase);
       if (threadIdx.x == 0) { if (st == st_lo) TC_MARK(3); if (st == st_lo + 9) TC_MARK(4); }
       const int ty = tap / 3;
-      const int row_off = a.halo + sgn * ((ty - 1) * a.gw + (tap - 3 * ty - 1));    // in [0, 2 * halo]
+      const int row_off = a.halo + a.sign * ((ty - 1) * a.gw + (tap - 3 * ty - 1));    // in [0, 2 * halo]
       const uint64_t ah0 = ahd + (uint64_t)(row_off * 8);
       const uint64_t al0 = ald + (uint64_t)(row_off * 8);
       const uint64_t bh0 = desc_base + (uint64_t)(smem_u32(bring + (size_t)stage * BSTAGE) >> 4);
@@ -426,8 +386,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     asm volatile("bar.sync 1, 256;" ::: "memory");
     if (warp < 4) {
       // ===== epilogue: thread r owns tile row r.  Without split-K: + bias, store its 4 * NCOLS contiguous bytes, keep the
-      // biased row in the tile for the statistics.  Split-K (push): the row goes into the owner CTA's receive buffer;
-      // (pull): the partial tile stays where it is.
+      // biased row in the tile for the statistics.  Split-K: the row goes into the owner CTA's receive buffer.
       const int r = threadIdx.x;
       const int grow = j0 + r;
       float* trow = tile + r * P4;
@@ -441,12 +400,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
           if (grow < a.rows) *reinterpret_cast<float4*>(orow + c) = v;
           if (want_stats) *reinterpret_cast<float4*>(trow + c) = v;
         }
-      } else if (a.push) {
+      } else {
         cluster_wait();                          // phase 1 (arrived at kernel start): all peers are running
         const int rows_per = 128 / nsplit, owner = r / rows_per, rloc = r - owner * rows_per;
-        const uint32_t recv_off = (uint32_t)(((zrank * rows_per + rloc) * P4) * 4);
-        const uint32_t push_row = dsmem_addr(smem_u32(bring + (size_t)nb * BSTAGE) + recv_off, (uint32_t)owner);
-        float* push_local = reinterpret_cast<float*>(bring + (size_t)nb * BSTAGE + recv_off);
+        const int recv_off = (zrank * rows_per + rloc) * P4;
+        const uint32_t push_row = dsmem_addr(smem_u32(recv + recv_off), (uint32_t)owner);
+        float* push_local = recv + recv_off;
 #pragma unroll
         for (int c = 0; c < NCOLS; c += 4) {
           const float4 v = *reinterpret_cast<const float4*>(trow + c);
@@ -462,25 +421,19 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     const float* sbuf = tile;                      // where those rows live (row index relative to row_lo)
     if (nsplit > 1) {
       __syncwarp();
-      if (a.push && warp >= 4) cluster_wait();       // phase 1 for the consumer warps that did not push
-      cluster_sync_all();                            // pull: every CTA's partial tile is in its shared memory; push: every receive buffer is complete
+      if (warp >= 4) cluster_wait();                 // phase 1 for the consumer warps that did not push
+      cluster_sync_all();                            // every receive buffer is complete
       if (threadIdx.x == 0) TC_MARK(10);
       row_n = 128 / nsplit; row_lo = zrank * row_n;
       float* tile2 = reinterpret_cast<float*>(smem + 40 * 1024);
       sbuf = tile2;
       if (warp < 4) {
         const int et = threadIdx.x;
-        const uint32_t tile_local = smem_u32(smem);
         const float* bias = a.bias ? a.bias + (long long)task * a.bias_stride : nullptr;
         float* outp = a.out + (long long)task * a.out_stride;
-        if (a.push) {
-          const float* recv = reinterpret_cast<const float*>(bring + (size_t)nb * BSTAGE);
-          if (nsplit == 2) splitk_reduce_local<NCOLS, 2>(recv, zrank, et, bias, tile2, outp, j0, a.rows);
-          else if (nsplit == 4) splitk_reduce_local<NCOLS, 4>(recv, zrank, et, bias, tile2, outp, j0, a.rows);
-          else splitk_reduce_local<NCOLS, 8>(recv, zrank, et, bias, tile2, outp, j0, a.rows);
-        } else if (nsplit == 2) splitk_reduce<NCOLS, 2>(tile_local, zrank, et, bias, tile2, outp, j0, a.rows);
-        else if (nsplit == 4) splitk_reduce<NCOLS, 4>(tile_local, zrank, et, bias, tile2, outp, j0, a.rows);
-        else splitk_reduce<NCOLS, 8>(tile_local, zrank, et, bias, tile2, outp, j0, a.rows);
+        if (nsplit == 2) splitk_reduce<NCOLS, 2>(recv, zrank, et, bias, tile2, outp, j0, a.rows);
+        else if (nsplit == 4) splitk_reduce<NCOLS, 4>(recv, zrank, et, bias, tile2, outp, j0, a.rows);
+        else splitk_reduce<NCOLS, 8>(recv, zrank, et, bias, tile2, outp, j0, a.rows);
       }
     }
 
@@ -490,7 +443,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
       const bool want_stats = (a.mode != CONV_PLAIN);
       if (want_stats) {
         asm volatile("bar.sync 2, 128;" ::: "memory");
-        const float* zh = a.zh ? a.zh + (long long)task * a.zh_stride : nullptr;
         constexpr int PARTS = 128 / NCOLS;           // 2 for 64 and 48, 4 for 32, 8 for 16
         const int col = et % NCOLS, part = et / NCOLS;
         double s1 = 0.0, s2 = 0.0;
@@ -499,10 +451,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
             if (row_ok[row_lo + rr]) {
               const float v = sbuf[rr * P4 + col];
               if (a.mode == CONV_FWD_STATS) { s1 += (double)v; s2 += (double)v * (double)v; }
-              else {
-                const float zv = a.zstage ? zbuf[rr * P4 + col] : zh[(long long)(j0 + row_lo + rr) * NCOLS + col];
-                s1 += (double)v; s2 += (double)zv * (double)v;
-              }
+              else { s1 += (double)v; s2 += (double)zbuf[rr * P4 + col] * (double)v; }
             }
           }
           if (part < 2) { sred[part][col][0] = s1; sred[part][col][1] = s2; }
@@ -520,10 +469,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
       }
     }
     if (threadIdx.x == 0) TC_MARK(12);
-    if (nsplit > 1 && !a.push) {
-      __syncwarp();
-      cluster_sync_all();                            // pull variant: nobody leaves while a peer still reads its partial tile
-    }
     if (threadIdx.x == 0) TC_MARK(8);
   }
   trace_mark(22 | 0x80, a.tag);     // end of CTA (0,0,0)
@@ -684,16 +629,20 @@ void launch_wgrad_tc(const WgradArgs& a, cudaStream_t st) {
 }
 
 // halo tile rows (multiple of 8) for a grid of pitch gw, and the deepest B ring (at most 8 stages) that fits next to 4
-// halo buffers
+// halo buffers and `extra` bytes behind the ring
 int tc_conv_rpad(int gw) { return ((128 + 2 * (gw + 1)) + 7) / 8 * 8; }
-int tc_conv_ring(int ncols, int gw) {
-  const long long avail = 227LL * 1024 - 4096 /* static smem */ - 1024 /* alignment */ - 4LL * tc_conv_rpad(gw) * 128;
+int tc_conv_ring(int ncols, int gw, size_t extra) {
+  const long long avail = 227LL * 1024 - 4096 /* static smem */ - 1024 /* alignment */ - 4LL * tc_conv_rpad(gw) * 128 - (long long)extra;
   long long nb = avail / (2LL * ncols * 128);
   if (nb > 8) nb = 8;
   return (int)nb;
 }
-size_t tc_conv_smem_bytes(int ncols, int gw) {
-  return (size_t)4 * tc_conv_rpad(gw) * 128 + (size_t)tc_conv_ring(ncols, gw) * 2 * ncols * 128 + 1024;
+// shared memory behind the B ring: with split-K (S > 1) the receive buffer [128 rows][ncols + 4] (peers write it while
+// this CTA's MMAs may still read the operand buffers, so it cannot alias them); in tangent mode the primal zh rows the
+// CTA finishes [128 / S][ncols + 4]
+size_t tc_conv_extra_bytes(int ncols, int S, bool tangent) {
+  const size_t row = (size_t)(ncols + 4) * 4;
+  return (S > 1 ? 128 * row : 0) + (tangent ? (size_t)(128 / S) * row : 0);
 }
 static size_t tc_conv_smem_for(int ncols, int gw, int nb) { return (size_t)4 * tc_conv_rpad(gw) * 128 + (size_t)nb * 2 * ncols * 128 + 1024; }
 
@@ -729,72 +678,42 @@ static int max_clusters(size_t smem, int S) {
 }
 
 template <int NCOLS>
-static void launch_conv_tc_n(const TcMaps& maps, const TcConvArgs& a_in, size_t smem, cudaStream_t st) {
+static void launch_conv_tc_n(const TcMaps& maps, const TcConvArgs& a_in, cudaStream_t st) {
   TcConvArgs a = a_in;
-  const EngineOptions& opt = *launch_ctx().opt;
   const int tiles = ((a.rows + 127) / 128) * (a.plan_tasks > a.tasks ? a.plan_tasks : a.tasks);
-  const int stages = a.nsrc * ((a.kc + 31) / 32) * 9;
+  const int stages = ((a.kc + 31) / 32) * 9;
+  // co-residency is asked for the split-K shape: the ring gives up the stages that the receive buffer takes
+  const size_t recv_bytes = tc_conv_extra_bytes(NCOLS, 2, false);
+  const size_t split_smem = tc_conv_smem_for(NCOLS, a.gw, std::min(a.nb, tc_conv_ring(NCOLS, a.gw, recv_bytes))) + recv_bytes;
   int S = 1;
-  // push-based split-K epilogue: a receive buffer [128 rows][NCOLS + 4] behind the B ring (peers write it while this CTA's
-  // MMAs may still read the operand buffers, so it cannot alias them); the ring gives up the stages that no longer fit
-  const size_t recv_bytes = (size_t)128 * (NCOLS + 4) * 4;
-  int nb_push = a.nb;
-  {
-    const long long avail = 227LL * 1024 - 4096 - 1024 - 4LL * tc_conv_rpad(a.gw) * 128 - (long long)recv_bytes;
-    const long long fit = avail / (2LL * NCOLS * 128);
-    if (fit < nb_push) nb_push = (int)fit;
-  }
-  const bool push = opt.tc_push && nb_push >= 2;
-  if (push) smem = tc_conv_smem_for(NCOLS, a.gw, nb_push) + recv_bytes;
-  int smax = opt.tc_split;
-  if (a.split_cap > 0 && a.split_cap < smax) { smax = 1; while (smax * 2 <= a.split_cap) smax *= 2; }
-  for (int cand = smax; cand >= 2; cand >>= 1) {
+  for (int cand = launch_ctx().opt->tc_split; cand >= 2; cand >>= 1) {
     if (cand > 8 || stages < 2 * cand) continue;
-    if (tiles <= max_clusters<NCOLS>(smem, cand)) { S = cand; break; }
+    if (tiles <= max_clusters<NCOLS>(split_smem, cand)) { S = cand; break; }
   }
   dim3 grid((a.rows + 127) / 128, a.tasks, S);
-  // a CTA never has more than ceil(stages / S) B stages in flight: a ring deeper than that only takes shared memory
-  // away from the kernels of the other streams that could share the SM (block-0 / BatchNorm kernels need 10-27 KB)
-  if (opt.tc_nb_fit) {
-    const int per_cta = (stages + S - 1) / S;
-    if (a.nb > per_cta) a.nb = per_cta < 2 ? 2 : per_cta;
-  }
-  a.push = (S > 1 && push) ? 1 : 0;
-  if (a.push) a.nb = nb_push;
-  // tangent mode: room for the primal zh rows this CTA finishes (see the kernel); the ring gives up stages if it must
-  a.zstage = 0;
-  size_t zbytes = 0;
-  if (opt.tc_zstage && a.mode == CONV_TAN_STATS && a.zh != nullptr) {
-    zbytes = (size_t)(128 / S) * (NCOLS + 4) * 4;
-    const long long limit = 227LL * 1024 - 4096;
-    int nb2 = a.nb;
-    auto total = [&](int nbx) { return (long long)tc_conv_smem_for(NCOLS, a.gw, nbx) + (long long)(a.push ? recv_bytes : 0) + (long long)zbytes; };
-    while (nb2 > 2 && total(nb2) > limit) --nb2;
-    if (total(nb2) <= limit) { a.nb = nb2; a.zstage = 1; } else zbytes = 0;
-  }
-  smem = tc_conv_smem_for(NCOLS, a.gw, a.nb) + (a.push ? recv_bytes : 0) + zbytes;
+  // maml_b200_create admits a geometry only if a ring of 2 stages fits next to the largest extra (S = 2, tangent mode)
+  const size_t extra = tc_conv_extra_bytes(NCOLS, S, a.mode == CONV_TAN_STATS);
+  a.nb = std::min(a.nb, tc_conv_ring(NCOLS, a.gw, extra));
+  const size_t smem = tc_conv_smem_for(NCOLS, a.gw, a.nb) + extra;
   if (S == 1) {
     launch_pdl(conv_tc_kernel<NCOLS>, grid, dim3(TC_THREADS), smem, st, maps, tagged(a));
     return;
   }
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid; cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute attr[2];
+  cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = 1; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = S;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = ((opt.pdl_cluster & 2) && pdl_allowed(st)) ? 2 : 1;
+  cfg.attrs = attr; cfg.numAttrs = 1;
   cudaLaunchKernelEx(&cfg, conv_tc_kernel<NCOLS>, maps, tagged(a));
 }
 
 void launch_conv_tc(const TcMaps& maps, const TcConvArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_CONV, a.alg_flops, st);
-  const size_t smem = tc_conv_smem_bytes(a.ncols, a.gw);
-  if (a.ncols == 64) launch_conv_tc_n<64>(maps, a, smem, st);
-  else if (a.ncols == 48) launch_conv_tc_n<48>(maps, a, smem, st);
-  else if (a.ncols == 32) launch_conv_tc_n<32>(maps, a, smem, st);
-  else launch_conv_tc_n<16>(maps, a, smem, st);
+  if (a.ncols == 64) launch_conv_tc_n<64>(maps, a, st);
+  else if (a.ncols == 48) launch_conv_tc_n<48>(maps, a, st);
+  else if (a.ncols == 32) launch_conv_tc_n<32>(maps, a, st);
+  else launch_conv_tc_n<16>(maps, a, st);
   CUDA_CHECK_LAUNCH();
 }
 

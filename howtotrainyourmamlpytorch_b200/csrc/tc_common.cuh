@@ -3,21 +3,18 @@
 #include <cuda.h>
 #include "common.cuh"
 
-struct alignas(64) TcMaps { CUtensorMap m[8]; };   // per source: A_hi, A_lo, B_hi, B_lo
+struct alignas(64) TcMaps { CUtensorMap m[4]; };   // A_hi, A_lo, B_hi, B_lo
 
 struct TcConvArgs {
-  int nsrc, kc, rows, gw, G, h, w, ncols, mode, tasks;
+  int kc, rows, gw, G, h, w, ncols, mode, tasks;
   int plan_tasks;        // split-K is planned for this many tasks (the handle's max_tasks) so that a task's arithmetic
                          // does not depend on how many tasks share the call
-  int push;              // split-K only, set by the launcher: 1 = partial rows are pushed into the owner CTA's receive buffer
-  int zstage;            // tangent mode, set by the launcher: 1 = the primal zh rows are staged in shared memory during the MMAs
-  int split_cap;         // > 0: largest split-K cluster size for THIS launch (side-stream launches: fewer, longer CTAs)
   int halo, rpad, nb, timeline;   // halo = gw + 1 rows; rpad = halo-tile rows (multiple of 8); nb = B ring depth
-  int a_row_base[2];     // row (in the A tensor map) of grid row 0 of task 0 for this pass slot (includes the guard)
-  int a_task_rows[2];    // rows per task in the A tensor map
-  int sign[2];           // +1 conv, -1 dgrad
-  int b_row_base[2];     // row (in the B tensor map) of (task 0, tap 0, n 0)
-  int b_task_rows[2];    // rows per task in the B tensor map
+  int a_row_base;        // row (in the A tensor map) of grid row 0 of task 0 for this pass slot (includes the guard)
+  int a_task_rows;       // rows per task in the A tensor map
+  int sign;              // +1 conv, -1 dgrad
+  int b_row_base;        // row (in the B tensor map) of (task 0, tap 0, n 0)
+  int b_task_rows;       // rows per task in the B tensor map
   const float* bias; long long bias_stride;
   float* out; long long out_stride;
   const float* zh; long long zh_stride;
@@ -27,8 +24,8 @@ struct TcConvArgs {
 };
 
 int tc_conv_rpad(int gw);
-int tc_conv_ring(int ncols, int gw);
-size_t tc_conv_smem_bytes(int ncols, int gw);
+int tc_conv_ring(int ncols, int gw, size_t extra = 0);
+size_t tc_conv_extra_bytes(int ncols, int S, bool tangent);
 int tc_conv_prepare();
 int tc_read_timeline(long long* out16);
 void launch_conv_tc(const TcMaps& maps, const TcConvArgs& a, cudaStream_t st);

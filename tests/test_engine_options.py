@@ -77,7 +77,7 @@ def test_switches_do_not_leak_between_handles(cuda_device, monkeypatch):
     launches_a = a._engine.last_launch_count()
 
     with monkeypatch.context() as env:
-        for k, v in {"BN_FUSE": "0", "TAIL_FUSE": "0", "TC_SPLIT": "1", "WGRAD_ROW": "0", "WGRAD_TC": "0"}.items():
+        for k, v in {"BN_FUSE": "0", "TAIL_FUSE": "0", "TC_SPLIT": "1", "WGRAD_TC": "0"}.items():
             env.setenv("MAML_B200_" + k, v)
         b = _model(g, cuda_device)
         b.meta_gradient(batch, epoch)

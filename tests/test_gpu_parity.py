@@ -632,13 +632,11 @@ def test_functional_network_operator_is_differentiable(case, cuda_device):
 
 def test_fused_and_cluster_paths_match_plain_paths(cuda_device):
     """The scheduling / fusion variants (cluster split-K convs, wgmma weight gradient, fused
-    BatchNorm backward, tangent conv split, double-buffered target passes, fused last block + head) against the plain
-    one-kernel-per-op paths (one-tap FFMA wgrad included) they replaced
+    BatchNorm backward, fused last block + head) against the plain one-kernel-per-op paths they replaced
     (selected through the diagnostic environment switches, read when the engine handle is created)."""
     g = load_golden("tiny_pp")
     batch, epoch = g.batch(0), g.iters[0][0]
-    plain = {"MAML_B200_TC_SPLIT": "1", "MAML_B200_BN_FUSE": "0", "MAML_B200_TAN_SPLIT": "0", "MAML_B200_TGT_SLOTS": "1",
-             "MAML_B200_WGRAD_ROW": "0", "MAML_B200_TAIL_FUSE": "0", "MAML_B200_WGRAD_TC": "0"}
+    plain = {"MAML_B200_TC_SPLIT": "1", "MAML_B200_BN_FUSE": "0", "MAML_B200_TAIL_FUSE": "0", "MAML_B200_WGRAD_TC": "0"}
     saved = {k: os.environ.get(k) for k in plain}
     try:
         os.environ.update(plain)
@@ -662,21 +660,21 @@ def test_fused_and_cluster_paths_match_plain_paths(cuda_device):
 
 _POLICY_SWITCHES = [
     {"MAML_B200_PDL": "0"},                                  # no programmatic dependent launch
-    {"MAML_B200_PDL": "1", "MAML_B200_PDL_CLUSTER": "3"},    # ... on every stream, cluster launches included
-    {"MAML_B200_TC_PUSH": "0"},                              # pull-based split-K reduction (two cluster barriers)
-    {"MAML_B200_TC_ZSTAGE": "0"},                            # tangent-mode statistics read the primal zh from global memory
+    {"MAML_B200_TC_SPLIT": "2"},                             # 2-CTA split-K: the largest receive buffer + staged zh rows
     {"MAML_B200_TAIL_ONCHIP": "0"},                          # last-block kernels that exchange their stages through L2
-    {"MAML_B200_TC_NB": "3", "MAML_B200_TC_NB_FIT": "1"},    # shallow shared-memory rings
-    {"MAML_B200_TC_SPLIT_SIDE": "1", "MAML_B200_TC_NB_SIDE": "2", "MAML_B200_BN_SIDE_CAP": "16"},   # side-stream caps
+    {"MAML_B200_TC_NB": "3"},                                # shallow shared-memory rings
+    {"MAML_B200_TC_NB": "2"},                                # the shallowest ring a handle admits
 ]
 
 
-@pytest.mark.parametrize("case", ["tiny_pp", "tiny_bern"])
+# tiny_maml: another geometry (16x16x1), plain MAML with shared BatchNorm statistics; tiny_pp_first: a first-order
+# iteration, whose schedule has no tangent passes
+@pytest.mark.parametrize("case", ["tiny_pp", "tiny_bern", "tiny_maml", "tiny_pp_first"])
 @pytest.mark.parametrize("switches", _POLICY_SWITCHES, ids=lambda d: "+".join("%s=%s" % (k[10:], v) for k, v in d.items()))
 def test_launch_policy_switches_do_not_change_results(case, switches, cuda_device):
-    """Round-2 launch policy (programmatic dependent launch, push-based split-K epilogue, on-chip last-block kernels,
-    shared-memory ring depths, side-stream caps): every switch is scheduling only -- the meta-gradient must agree with
-    the default build to summation-order noise."""
+    """Launch policy (programmatic dependent launch, split-K cluster size, on-chip last-block kernels, shared-memory
+    ring depths): every switch is scheduling only -- the meta-gradient must agree with the default build to
+    summation-order noise."""
     g = load_golden(case)
     batch, epoch = g.batch(0), g.iters[0][0]
     m1 = _model(g, cuda_device)
