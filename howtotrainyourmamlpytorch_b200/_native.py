@@ -24,7 +24,7 @@ EXPORTED_SYMBOLS = [
     "maml_b200_trace", "maml_b200_trace_read",
     "maml_b200_comm_init", "maml_b200_comm_connect", "maml_b200_comm_world", "maml_b200_all_reduce",
     "maml_b200_comm_status", "maml_b200_net_backward", "maml_b200_net_running_update", "maml_b200_episode_gather",
-    "maml_b200_net_hvp",
+    "maml_b200_net_hvp", "maml_b200_net_input_grad", "maml_b200_net_hvp_input_grad",
 ]
 PROF_CATS = ["conv_igemm", "conv_first_block", "wgrad", "wgrad_first_block", "bn_act_pool", "head", "param"]
 
@@ -83,6 +83,10 @@ def load_library():
     lib.maml_b200_net_backward.restype = ctypes.c_int
     lib.maml_b200_net_hvp.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.maml_b200_net_hvp.restype = ctypes.c_int
+    lib.maml_b200_net_input_grad.argtypes = [vp, i32, vp, vp]
+    lib.maml_b200_net_input_grad.restype = ctypes.c_int
+    lib.maml_b200_net_hvp_input_grad.argtypes = [vp, i32, vp, vp]
+    lib.maml_b200_net_hvp_input_grad.restype = ctypes.c_int
     lib.maml_b200_net_running_update.argtypes = [vp, i32, i32, vp, vp, vp]
     lib.maml_b200_net_running_update.restype = ctypes.c_int
     lib.maml_b200_episode_gather.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, ctypes.POINTER(f32),
@@ -215,6 +219,14 @@ class Engine(object):
                                         dlogits.data_ptr(), v_like.data_ptr(), jv_out.data_ptr(), hv_out.data_ptr(),
                                         self._stream())
         _check(self.lib, rc, "maml_b200_net_hvp")
+
+    def net_input_grad(self, n_tasks, dx_out):
+        rc = self.lib.maml_b200_net_input_grad(self.h, int(n_tasks), dx_out.data_ptr(), self._stream())
+        _check(self.lib, rc, "maml_b200_net_input_grad")
+
+    def net_hvp_input_grad(self, n_tasks, dxdot_out):
+        rc = self.lib.maml_b200_net_hvp_input_grad(self.h, int(n_tasks), dxdot_out.data_ptr(), self._stream())
+        _check(self.lib, rc, "maml_b200_net_hvp_input_grad")
 
     def net_running_update(self, n_tasks, num_step, running_mean, running_var):
         rc = self.lib.maml_b200_net_running_update(self.h, int(n_tasks), int(num_step), running_mean.data_ptr(),

@@ -82,6 +82,17 @@ struct WgradArgs {
   int tag;          // launch sequence number inside the iteration (device trace)
 };
 
+struct InputGradArgs {                         // first-block data gradient, written as NCHW images
+  const float* D[2]; long long d_stride[2];    // output gradients of the first conv: row 0 of [rows][ncols], per task
+  const float* W[2]; long long w_stride;       // first-block weights [9][C0][ncols], per task (D[s] pairs with W[s])
+  float* dx; long long dx_stride;              // [n][C0][h][w], per task
+  int nsrc;                                    // operand pairs summed into dx (1 or 2)
+  int rows, gw, G, h, w, c0, ncols;
+  int tasks;
+  double alg_flops;
+  int tag;          // launch sequence number inside the iteration (device trace)
+};
+
 struct BnGeom { int n, h, w, gw, G, ph, pw, pgw, pG, pb, F; };
 
 struct BnActArgs {                // forward: z -> zh (in place), pooled activation p
@@ -199,6 +210,7 @@ void launch_conv_rows(const ConvArgs& a, cudaStream_t st);
 void launch_conv0(const Conv0Args& a, cudaStream_t st);
 void launch_wgrad(const WgradArgs& a, cudaStream_t st);
 void launch_wgrad0(const WgradArgs& a, cudaStream_t st);
+void launch_input_grad0(const InputGradArgs& a, cudaStream_t st);
 void launch_bnact(const BnActArgs& a, cudaStream_t st);
 void launch_bnact_tan(const BnActTanArgs& a, cudaStream_t st);
 void launch_bnbwd_reduce(const BnBwdArgs& a, cudaStream_t st);

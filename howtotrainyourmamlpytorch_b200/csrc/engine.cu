@@ -114,6 +114,9 @@ struct maml_b200_handle {
   int pin_slot = 0;
   long long last_launches = 0;
   int last_tasks = 0;
+  // the functional call (net_forward / net_backward / net_hvp) whose buffers the handle holds; FN_NONE after an
+  // iteration or a call that failed.  The image-gradient entries read those buffers and check this record first.
+  int fn_kind = 0, fn_tasks = 0, fn_step = 0;
   Profiler prof;
   bool profiling = false;             // maml_b200_profile(h, 1): this handle's launches are recorded into prof
   // side streams / events for fork-join inside one iteration, CUDA-graph cache
@@ -141,6 +144,11 @@ struct maml_b200_handle {
   void* comm_opened[MAML_MAX_RANKS] = {};               // peer blocks mapped with cudaIpcOpenMemHandle
   bool comm_connected = false;
 };
+
+enum { FN_NONE = 0, FN_FORWARD = 1, FN_BACKWARD = 2, FN_HVP = 3 };
+static void record_call(maml_b200_handle* h, int kind, int n_tasks, int num_step) {
+  h->fn_kind = kind; h->fn_tasks = n_tasks; h->fn_step = num_step;
+}
 
 // launch context of the handle call in progress on this thread (common.cuh); the default one has PDL off
 static const EngineOptions g_default_options;
@@ -1083,6 +1091,7 @@ extern "C" int maml_b200_meta_batch_fwd_bwd(maml_b200_handle* h, const maml_b200
   const long long* ys = (const long long*)y_support;
   const long long* yt = (const long long*)y_target;
   h->last_tasks = T;
+  record_call(h, FN_NONE, 0, 0);           // the iteration reuses the functional calls' buffers
 
   if (!h->use_graphs || h->profiling) {
     // eager: launches go straight to the caller's stream (side streams fork / join through events)
@@ -1139,6 +1148,7 @@ extern "C" int maml_b200_net_forward(maml_b200_handle* h, int32_t n_tasks, int32
   cudaStream_t st = (cudaStream_t)stream;
   LaunchScope launch_scope(h, st);
   const int T = n_tasks;
+  record_call(h, FN_NONE, 0, 0);
   CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
   CK(cudaMemsetAsync(h->losses, 0, (size_t)h->maxT * MAML_MAX_STEPS * sizeof(float), st));
   CK(cudaMemsetAsync(h->correct, 0, (size_t)h->maxT * sizeof(float), st));
@@ -1156,6 +1166,7 @@ extern "C" int maml_b200_net_forward(maml_b200_handle* h, int32_t n_tasks, int32
   a.tasks = T;
   launch_head(a, st);
   CK(cudaGetLastError());
+  record_call(h, FN_FORWARD, T, num_step);
   return 0;
 }
 
@@ -1173,6 +1184,7 @@ extern "C" int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int3
   cudaStream_t st = (cudaStream_t)stream;
   LaunchScope launch_scope(h, st);
   const int T = n_tasks;
+  record_call(h, FN_NONE, 0, 0);
   // backward statistics (and the tangent ones export subtracts) start from zero; forward statistics are kept
   for (int kind : {PASS_TGT_BWD, PASS_TAN_BWD})
     CK(cudaMemset2DAsync(h->stats + (long long)kind * MAML_MAX_STEPS * h->st_pass_stride, (size_t)h->stats_task_stride * sizeof(double), 0,
@@ -1208,6 +1220,7 @@ extern "C" int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int3
   e.result = grad_out;
   launch_export(e, st);
   CK(cudaGetLastError());
+  record_call(h, FN_BACKWARD, T, num_step);
   return 0;
 }
 
@@ -1230,6 +1243,7 @@ extern "C" int maml_b200_net_hvp(maml_b200_handle* h, int32_t n_tasks, int32_t n
   LaunchScope launch_scope(h, st);
   const int T = n_tasks, s = num_step;
   float* th = h->theta + (long long)s * h->maxT * h->Ppad;
+  record_call(h, FN_NONE, 0, 0);                 // at num_step 0 this overwrites the weights net_forward imported
   CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
   CK(cudaMemsetAsync(h->abar, 0, (size_t)h->maxT * h->pl.nseg_inner * MAML_MAX_STEPS * sizeof(double), st));
   CK(cudaMemsetAsync(h->losses, 0, (size_t)h->maxT * MAML_MAX_STEPS * sizeof(float), st));
@@ -1275,7 +1289,53 @@ extern "C" int maml_b200_net_hvp(maml_b200_handle* h, int32_t n_tasks, int32_t n
   e.result = hv_out;
   launch_export(e, st);
   CK(cudaGetLastError());
+  record_call(h, FN_HVP, T, num_step);
   return 0;
+}
+
+// First-block data gradient of a functional call, straight into NCHW images: dx = sum over the pairs (W_k, D_k) of
+// W_k^T applied to D_k, where D_k is a gradient at the first conv's output.
+static int input_grad(maml_b200_handle* h, int n_tasks, const Slot* D, const float* const* W, int nsrc, float* dx_out,
+                      cudaStream_t st) {
+  LaunchScope launch_scope(h, st);
+  const LayerGeom& g = h->geo[0];
+  const PassSet& ps = *D[0].ps;
+  InputGradArgs a{};
+  for (int k = 0; k < nsrc; ++k) {
+    a.D[k] = DZ(*D[k].ps, 0, D[k].slot); a.d_stride[k] = STRIDE(*D[k].ps, dz, 0); a.W[k] = W[k];
+  }
+  a.w_stride = h->Ppad;
+  a.dx = dx_out; a.dx_stride = (long long)ps.n * h->C * h->H * h->W;
+  a.nsrc = nsrc; a.rows = ps.n * g.G; a.gw = g.gw; a.G = g.G; a.h = g.h; a.w = g.w; a.c0 = h->C; a.ncols = h->F;
+  a.tasks = n_tasks;
+  a.alg_flops = conv_flops(h, 0, ps.n, n_tasks, nsrc);
+  launch_input_grad0(a, st);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+// d(loss)/d(x) of the immediately preceding maml_b200_net_backward on this handle: W_0^T applied to the first block's
+// output gradient of that backward (target pass, theta slot 0 as imported by net_forward).
+extern "C" int maml_b200_net_input_grad(maml_b200_handle* h, int32_t n_tasks, float* dx_out, void* stream) {
+  if (!h || !dx_out) return fail("null argument");
+  if (h->fn_kind != FN_BACKWARD) return fail("maml_b200_net_input_grad must immediately follow maml_b200_net_backward on this handle");
+  if (n_tasks != h->fn_tasks) return fail("maml_b200_net_input_grad: n_tasks differs from the preceding maml_b200_net_backward");
+  const Slot D[1] = {{&h->tgt, 0}};
+  const float* W[1] = {h->theta + h->pl.w_off[0]};
+  return input_grad(h, n_tasks, D, W, 1, dx_out, (cudaStream_t)stream);
+}
+
+// d/dx <dlogits, J v> of the immediately preceding maml_b200_net_hvp on this handle: the tangent of the image gradient
+// along v, W_0^T applied to the tangent of the first block's output gradient plus U_0^T applied to that gradient itself
+// (support pass and theta slot num_step of the hvp call, u = v's weights).
+extern "C" int maml_b200_net_hvp_input_grad(maml_b200_handle* h, int32_t n_tasks, float* dxdot_out, void* stream) {
+  if (!h || !dxdot_out) return fail("null argument");
+  if (h->fn_kind != FN_HVP) return fail("maml_b200_net_hvp_input_grad must immediately follow maml_b200_net_hvp on this handle");
+  if (n_tasks != h->fn_tasks) return fail("maml_b200_net_hvp_input_grad: n_tasks differs from the preceding maml_b200_net_hvp");
+  const int s = h->fn_step;
+  const Slot D[2] = {{&h->tan, 0}, {&h->sup, s}};
+  const float* W[2] = {h->theta + (long long)s * h->maxT * h->Ppad + h->pl.w_off[0], h->u + h->pl.w_off[0]};
+  return input_grad(h, n_tasks, D, W, 2, dxdot_out, (cudaStream_t)stream);
 }
 
 // Side effect of the functional forward in the reference: F.batch_norm's EMA update of running_mean / running_var at

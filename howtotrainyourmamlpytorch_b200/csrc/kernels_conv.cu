@@ -741,6 +741,124 @@ void launch_wgrad0(const WgradArgs& a, cudaStream_t st) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// first-block data gradient (d loss / d images), written straight into NCHW [tasks][n][C0][h][w]:
+//   dx[img][c][y][x] = sum_src sum_tap sum_f W_src[tap][c][f] * D_src[row(img, y, x) - s_tap][f]
+// N = C0 <= 4 is below wgmma's smallest N (8) and K = 9 * F: register-blocked FFMA.  Thread (rg, fl) owns IG_R
+// consecutive grid rows x all C0 outputs for the filter slice f = f0 + fl of each 16-wide chunk f0.  For a filter row ky
+// the source rows of its IG_R rows and three kx taps are IG_R + 2 consecutive rows: read once from shared memory, they
+// feed 3 x C0 x IG_R FMAs.  The 16 f lanes of a half-warp are summed by a fixed xor butterfly (no atomics: bit-identical
+// run to run).  Source rows outside the valid h x w window (pad columns, pad rows, guard rows) are zero by index test:
+// the kernel never reads what other passes left in the border rows of D.
+// ---------------------------------------------------------------------------------------------
+constexpr int IG_R = 8, IG_GROUPS = 32, IG_ROWS = IG_R * IG_GROUPS, IG_FC = 16;
+constexpr int IG_P = IG_FC + 2;   // shared row pitch: the two half-warps of a warp (rows 8 apart) hit disjoint banks
+
+template <int C0, int NSRC>
+__global__ void __launch_bounds__(IG_GROUPS * 16) input_grad0_kernel(InputGradArgs a) {
+  pdl_prologue(31, a.tag);
+  extern __shared__ float smi[];
+  const int task = blockIdx.y;
+  const int j0 = blockIdx.x * IG_ROWS;
+  const int tid = threadIdx.x, rg = tid >> 4, fl = tid & 15;
+  const int F = a.ncols, halo = a.gw + 1, wrows = IG_ROWS + 2 * halo;
+  float* Ws = smi;                                   // [NSRC][9][C0][F]
+  float* Ds = Ws + NSRC * 9 * C0 * F;                // [wrows][IG_P]: one 16-wide filter chunk of the window
+  int* vm = reinterpret_cast<int*>(Ds + wrows * IG_P);   // [wrows]: window row is a valid pixel
+  for (int s = 0; s < NSRC; ++s) {
+    const float* W = (s == 0 ? a.W[0] : a.W[1]) + (long long)task * a.w_stride;   // (no dynamic index into the parameters)
+    for (int i = tid; i < 9 * C0 * F; i += IG_GROUPS * 16) Ws[s * 9 * C0 * F + i] = W[i];
+  }
+  for (int r = tid; r < wrows; r += IG_GROUPS * 16) {
+    const int row = j0 - halo + r;
+    int ok = 0;
+    if (row >= 0 && row < a.rows) {
+      const int rr = row % a.G, yy = rr / a.gw, xx = rr - yy * a.gw;
+      ok = yy >= 1 && yy <= a.h && xx >= 1 && xx <= a.w;
+    }
+    vm[r] = ok;
+  }
+  float acc[IG_R][C0];
+#pragma unroll
+  for (int k = 0; k < IG_R; ++k)
+#pragma unroll
+    for (int c = 0; c < C0; ++c) acc[k][c] = 0.f;
+
+  for (int s = 0; s < NSRC; ++s) {
+    const float* D = s == 0 ? a.D[0] + (long long)task * a.d_stride[0] : a.D[1] + (long long)task * a.d_stride[1];
+    for (int f0 = 0; f0 < F; f0 += IG_FC) {
+      __syncthreads();                               // the previous chunk has been consumed
+      for (int i = tid; i < wrows * (IG_FC / 4); i += IG_GROUPS * 16) {
+        const int r = i >> 2, q = i & 3;
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (vm[r]) v = *reinterpret_cast<const float4*>(D + (long long)(j0 - halo + r) * F + f0 + q * 4);
+        float* d = Ds + r * IG_P + q * 4;
+        d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
+      }
+      __syncthreads();
+      const float* wp = Ws + s * 9 * C0 * F + f0 + fl;
+#pragma unroll
+      for (int ky = 0; ky < 3; ++ky) {
+        // window rows rg*IG_R + halo - (ky-1)*gw - 1 .. + IG_R + 1: tap kx of local row k reads entry k + 2 - kx
+        const float* dp = Ds + (rg * IG_R + halo - (ky - 1) * a.gw - 1) * IG_P + fl;
+        float xw[IG_R + 2];
+#pragma unroll
+        for (int i = 0; i < IG_R + 2; ++i) xw[i] = dp[i * IG_P];
+#pragma unroll
+        for (int kx = 0; kx < 3; ++kx)
+#pragma unroll
+          for (int c = 0; c < C0; ++c) {
+            const float wv = wp[((ky * 3 + kx) * C0 + c) * F];
+#pragma unroll
+            for (int k = 0; k < IG_R; ++k) acc[k][c] = fmaf(xw[k + 2 - kx], wv, acc[k][c]);
+          }
+      }
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < IG_R; ++k)
+#pragma unroll
+    for (int c = 0; c < C0; ++c)
+#pragma unroll
+      for (int o = 8; o >= 1; o >>= 1) acc[k][c] += __shfl_xor_sync(0xffffffffu, acc[k][c], o);
+
+  // every lane of the half-warp now holds the same sums: lane fl stores row k = fl % 8, channels fl / 8, fl / 8 + 2
+  const int k = fl & (IG_R - 1), ch = fl >> 3;
+  const int row = j0 + rg * IG_R + k;
+  if (row >= a.rows) return;
+  const int img = row / a.G, rr = row - img * a.G, yy = rr / a.gw, xx = rr - yy * a.gw;
+  if (yy < 1 || yy > a.h || xx < 1 || xx > a.w) return;
+  const long long plane = (long long)a.h * a.w;
+  float* out = a.dx + (long long)task * a.dx_stride + (long long)img * C0 * plane + (long long)(yy - 1) * a.w + (xx - 1);
+#pragma unroll
+  for (int cp = 0; cp < C0; cp += 2) {
+    if (cp + ch < C0) {
+      float v = 0.f;
+#pragma unroll
+      for (int kk = 0; kk < IG_R; ++kk)
+        if (kk == k) v = ch ? acc[kk][cp + 1 < C0 ? cp + 1 : cp] : acc[kk][cp];
+      out[(cp + ch) * plane] = v;
+    }
+  }
+}
+
+template <int C0, int NSRC>
+static void launch_input_grad0_c(const InputGradArgs& a, cudaStream_t st) {
+  const int wrows = IG_ROWS + 2 * (a.gw + 1);
+  const size_t smem = (size_t)(NSRC * 9 * C0 * a.ncols + wrows * IG_P + wrows) * sizeof(float);
+  if (smem > 48 * 1024) cudaFuncSetAttribute(input_grad0_kernel<C0, NSRC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  dim3 grid((a.rows + IG_ROWS - 1) / IG_ROWS, a.tasks);
+  launch_pdl(input_grad0_kernel<C0, NSRC>, dim3(grid), dim3(IG_GROUPS * 16), smem, st, tagged(a));
+}
+
+void launch_input_grad0(const InputGradArgs& a, cudaStream_t st) {
+  ProfScope prof_scope__(PROF_CONV0, a.alg_flops, st);
+#define IG_CASE(C, S) if (a.c0 == C && a.nsrc == S) launch_input_grad0_c<C, S>(a, st); else
+  IG_CASE(1, 1) IG_CASE(2, 1) IG_CASE(3, 1) IG_CASE(4, 1) IG_CASE(1, 2) IG_CASE(2, 2) IG_CASE(3, 2) IG_CASE(4, 2) {}
+#undef IG_CASE
+  CUDA_CHECK_LAUNCH();
+}
+
+// ---------------------------------------------------------------------------------------------
 // image NCHW [tasks][n][C][H][W] -> padded-grid matrix [tasks][n*G][C] (valid positions only)
 // ---------------------------------------------------------------------------------------------
 __global__ void prep_x_kernel(const float* __restrict__ x, float* __restrict__ xg, long long xg_task_stride, int n,

@@ -177,8 +177,11 @@ class VGGReLUNormNetwork(nn.Module):
         loss, few_shot_learning_system.py:138-139).  Twice differentiable: with ``create_graph=True`` the returned
         gradients are differentiable w.r.t. the weights (and the upstream d(logits)) through ``maml_b200_net_hvp``, so the
         reference's second-order loop runs on this operator; a BatchNorm gamma / beta gradient is not (see
-        ``_FunctionalBackward``).  No gradient flows to ``x``.  The batch size must be a multiple of the number of classes
-        (episode shaped)."""
+        ``_FunctionalBackward``).  When ``x`` requires grad the operator is differentiable w.r.t. the images too
+        (``maml_b200_net_input_grad``), and with ``create_graph=True`` the weight gradients are differentiable w.r.t. ``x``
+        (``maml_b200_net_hvp_input_grad``: the mixed term an outer loss needs to reach support images through the inner
+        loop); the image gradient itself is not differentiable again.  With ``x`` not requiring grad none of this runs.
+        The batch size must be a multiple of the number of classes (episode shaped)."""
         from . import _native
         if x.device.type != "cuda":
             raise _native.NativeLibraryError("VGGReLUNormNetwork.forward needs a CUDA (sm_90a) device: no CPU fallback")
@@ -240,13 +243,15 @@ class _FunctionalForward(torch.autograd.Function):
             net._apply_running_ema(st, num_step)
         st["gen"] += 1
         ctx.net, ctx.num_step, ctx.gen = net, num_step, st["gen"]
-        ctx.save_for_backward(xin, *tensors)       # the weights themselves: a double backward differentiates w.r.t. them
+        # x and the weights themselves: a double backward differentiates w.r.t. them
+        ctx.save_for_backward(x, *tensors)
         return logits[0].clone()
 
     @staticmethod
     def backward(ctx, dlogits):
-        xin, tensors = ctx.saved_tensors[0], ctx.saved_tensors[1:]
-        return (None, None, None) + tuple(_FunctionalBackward.apply(ctx, xin, dlogits, *tensors))
+        x, tensors = ctx.saved_tensors[0], ctx.saved_tensors[1:]
+        out = _FunctionalBackward.apply(ctx, x, dlogits, *tensors)
+        return (None, out[0], None) + tuple(out[1:])
 
 
 class _FunctionalBackward(torch.autograd.Function):
@@ -255,17 +260,22 @@ class _FunctionalBackward(torch.autograd.Function):
     few_shot_learning_system.py:138-139 and the outer ``loss.backward()``).
 
     forward  = ``maml_b200_net_backward``: B(dl, theta) = J^T dl for every tensor (conv / linear, BatchNorm gamma / beta of
-               ``num_step``).  With grad mode off this is the whole first-order backward.
+               ``num_step``), and -- only when x requires grad -- ``maml_b200_net_input_grad``: J_x^T dl (else None).  With
+               grad mode off this is the whole first-order backward.
     backward = ``maml_b200_net_hvp`` along the cotangents v of the conv / linear gradients: one forward-over-reverse pass with
-               dl held constant gives J v (the cotangent of dl) and d/dtheta <dl, J v> (that of every tensor).  torch carries
-               J v on through the loss's own double backward.  Third order is not supported.
-    A cotangent on a BatchNorm gamma / beta GRADIENT would need gamma / beta tangent directions, which the engine's BatchNorm
-    tangent kernels do not have: refused (it only arises when BatchNorm parameters are inner-loop fast weights,
-    enable_inner_loop_optimizable_bn_params, which the network refuses too)."""
+               dl held constant gives J v (the cotangent of dl) and d/dtheta <dl, J v> (that of every tensor); when x
+               requires grad, ``maml_b200_net_hvp_input_grad`` on the same handle gives d/dx <dl, J v> (that of x).  torch
+               carries J v on through the loss's own double backward.  Third order is not supported.
+    A cotangent on a BatchNorm gamma / beta GRADIENT would need gamma / beta tangent directions, and one on the image
+    gradient dx would need image tangent directions (the first conv's tangent driven by x-dot); the engine's tangent pass
+    has neither: both are refused (the first only arises when BatchNorm parameters are inner-loop fast weights,
+    enable_inner_loop_optimizable_bn_params, which the network refuses too; the second e.g. for a penalty on the image
+    gradient's norm that is differentiated again)."""
 
     @staticmethod
-    def forward(ctx, fwd_ctx, xin, dlogits, *tensors):
+    def forward(ctx, fwd_ctx, x, dlogits, *tensors):
         net, num_step = fwd_ctx.net, fwd_ctx.num_step
+        xin = x.detach().to(torch.float32).contiguous()
         st = net._operator_engine(xin)
         eng, meta_like, logits, grad = st["eng"], st["meta"], st["logits"], st["grad"]
         with torch.cuda.device(xin.device):
@@ -276,19 +286,29 @@ class _FunctionalBackward(torch.autograd.Function):
                 st["gen"] += 1
                 fwd_ctx.gen = st["gen"]
             eng.net_backward(1, num_step, meta_like, dlogits.detach().to(torch.float32).contiguous().view(1, *dlogits.shape), grad)
+            dx = None
+            if fwd_ctx.needs_input_grad[1]:
+                dx = st.setdefault("dx", torch.empty((1,) + tuple(xin.shape), dtype=torch.float32, device=xin.device))
+                eng.net_input_grad(1, dx)
+                dx = dx[0].to(x.dtype, copy=True)
         ctx.set_materialize_grads(False)
-        ctx.net, ctx.num_step, ctx.x = net, num_step, xin
-        ctx.save_for_backward(dlogits, *tensors)
+        ctx.net, ctx.num_step = net, num_step
+        ctx.save_for_backward(x, dlogits, *tensors)
         grads = []
         for (off, size), t, need in zip(eng.segments, tensors, fwd_ctx.needs_input_grad[3:]):
             grads.append(grad[off:off + size].view(t.shape).clone() if need else None)
-        return tuple(grads)
+        return (dx,) + tuple(grads)
 
     @staticmethod
     @torch.autograd.function.once_differentiable
-    def backward(ctx, *cotangents):
-        net, num_step, xin = ctx.net, ctx.num_step, ctx.x
-        dlogits, tensors = ctx.saved_tensors[0], ctx.saved_tensors[1:]
+    def backward(ctx, dx_cotangent, *cotangents):
+        net, num_step = ctx.net, ctx.num_step
+        x, dlogits, tensors = ctx.saved_tensors[0], ctx.saved_tensors[1], ctx.saved_tensors[2:]
+        if dx_cotangent is not None:
+            raise NotImplementedError(
+                "differentiating through the gradient with respect to the images needs image tangent directions, which "
+                "the engine's tangent pass does not implement")
+        xin = x.detach().to(torch.float32).contiguous()
         n_conv = 4 * net.num_stages
         for i, c in enumerate(cotangents[:n_conv]):
             if c is not None and i % 4 >= 2:
@@ -309,8 +329,13 @@ class _FunctionalBackward(torch.autograd.Function):
         with torch.cuda.device(xin.device):
             eng.net_hvp(1, num_step, meta_like, xin, dlogits.to(torch.float32).contiguous().view(1, *dlogits.shape), v_like,
                         jv, hv)
+            d_x = None
+            if ctx.needs_input_grad[1]:
+                dxdot = hs.setdefault("dxdot", torch.empty((1,) + tuple(xin.shape), dtype=torch.float32, device=xin.device))
+                eng.net_hvp_input_grad(1, dxdot)
+                d_x = dxdot[0].to(x.dtype, copy=True)
         d_dlogits = jv[0].to(dlogits.dtype).clone() if ctx.needs_input_grad[2] else None
         grads = []
         for (off, size), t, need in zip(eng.segments, tensors, ctx.needs_input_grad[3:]):
             grads.append(hv[off:off + size].view(t.shape).to(t.dtype).clone() if need else None)
-        return (None, None, d_dlogits) + tuple(grads)
+        return (None, d_x, d_dlogits) + tuple(grads)

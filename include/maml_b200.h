@@ -118,7 +118,8 @@ int maml_b200_net_forward(maml_b200_handle* h, int32_t n_tasks, int32_t num_step
  *   dlogits  [n_tasks, N*T, N]   d(loss) / d(logits)
  *   grad_out [result_size]       (out) first meta_size floats = d(loss) / d(meta_like) in the meta layout (conv / linear
  *                                weights and biases, BatchNorm beta / gamma rows of num_step; LSLR entries 0), summed over
- *                                the n_tasks batches.  No gradient with respect to the images is produced. */
+ *                                the n_tasks batches.  The gradient with respect to the images is a separate call,
+ *                                maml_b200_net_input_grad. */
 int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
                            const float* dlogits, float* grad_out, void* stream);
 
@@ -135,6 +136,15 @@ int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int32_t num_ste
  * No running-statistics side effect; it overwrites the batch statistics maml_b200_net_running_update reads. */
 int maml_b200_net_hvp(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
                       const float* dlogits, const float* v_like, float* jv_out, float* hv_out, void* stream);
+
+/* Gradients with respect to the images.  Each reads the buffers of the functional call that ran last on this handle and
+ * must follow it immediately, with the same n_tasks: another call on the handle in between (a functional call, an
+ * iteration) makes it fail with an error and launch nothing.
+ *   net_input_grad      after maml_b200_net_backward:  dx_out    [n_tasks, N*T, C, H, W] = J_x^T dlogits
+ *   net_hvp_input_grad  after maml_b200_net_hvp:       dxdot_out [n_tasks, N*K, C, H, W] = d/dx <dlogits, J v>
+ *                       (the mixed second-order term: the tangent of the image gradient along v) */
+int maml_b200_net_input_grad(maml_b200_handle* h, int32_t n_tasks, float* dx_out, void* stream);
+int maml_b200_net_hvp_input_grad(maml_b200_handle* h, int32_t n_tasks, float* dxdot_out, void* stream);
 
 /* EMA side effect of the functional forward (F.batch_norm updating running_mean / running_var at num_step, reference
  * meta_neural_network_architectures.py:226-247) from the batch statistics of the last maml_b200_net_forward call, which
