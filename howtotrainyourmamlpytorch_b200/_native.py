@@ -25,6 +25,7 @@ EXPORTED_SYMBOLS = [
     "maml_b200_comm_init", "maml_b200_comm_connect", "maml_b200_comm_world", "maml_b200_all_reduce",
     "maml_b200_comm_status", "maml_b200_net_backward", "maml_b200_net_running_update", "maml_b200_episode_gather",
     "maml_b200_net_hvp", "maml_b200_net_input_grad", "maml_b200_net_hvp_input_grad",
+    "maml_b200_net_hvp_image", "maml_b200_net_jvp",
 ]
 PROF_CATS = ["conv_igemm", "conv_first_block", "wgrad", "wgrad_first_block", "bn_act_pool", "head", "param"]
 
@@ -83,6 +84,10 @@ def load_library():
     lib.maml_b200_net_backward.restype = ctypes.c_int
     lib.maml_b200_net_hvp.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.maml_b200_net_hvp.restype = ctypes.c_int
+    lib.maml_b200_net_hvp_image.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.maml_b200_net_hvp_image.restype = ctypes.c_int
+    lib.maml_b200_net_jvp.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp]
+    lib.maml_b200_net_jvp.restype = ctypes.c_int
     lib.maml_b200_net_input_grad.argtypes = [vp, i32, vp, vp]
     lib.maml_b200_net_input_grad.restype = ctypes.c_int
     lib.maml_b200_net_hvp_input_grad.argtypes = [vp, i32, vp, vp]
@@ -219,6 +224,20 @@ class Engine(object):
                                         dlogits.data_ptr(), v_like.data_ptr(), jv_out.data_ptr(), hv_out.data_ptr(),
                                         self._stream())
         _check(self.lib, rc, "maml_b200_net_hvp")
+
+    def net_hvp_image(self, n_tasks, num_step, meta_like, x, xdot, dlogits, v_like, jv_out, hv_out):
+        """``net_hvp`` along (v_like, xdot); ``xdot`` None is ``net_hvp``."""
+        rc = self.lib.maml_b200_net_hvp_image(self.h, int(n_tasks), int(num_step), meta_like.data_ptr(), x.data_ptr(),
+                                              None if xdot is None else xdot.data_ptr(), dlogits.data_ptr(),
+                                              v_like.data_ptr(), jv_out.data_ptr(), hv_out.data_ptr(), self._stream())
+        _check(self.lib, rc, "maml_b200_net_hvp_image")
+
+    def net_jvp(self, n_tasks, num_step, meta_like, x, t_like, xdot, jv_out):
+        """Logits tangent J_theta t + J_x xdot (``xdot`` may be None)."""
+        rc = self.lib.maml_b200_net_jvp(self.h, int(n_tasks), int(num_step), meta_like.data_ptr(), x.data_ptr(),
+                                        t_like.data_ptr(), None if xdot is None else xdot.data_ptr(), jv_out.data_ptr(),
+                                        self._stream())
+        _check(self.lib, rc, "maml_b200_net_jvp")
 
     def net_input_grad(self, n_tasks, dx_out):
         rc = self.lib.maml_b200_net_input_grad(self.h, int(n_tasks), dx_out.data_ptr(), self._stream())

@@ -207,12 +207,16 @@ struct PartialDesc {              // where each inner segment's gradient chunks 
 void launch_prep_x(const float* x, float* xg, long long xg_task_stride, int tasks, int n, int C, int H, int W,
                    cudaStream_t st);
 void launch_conv_rows(const ConvArgs& a, cudaStream_t st);
-void launch_conv0(const Conv0Args& a, cudaStream_t st);
+// X2 / W2 (nullable, same strides as X / W): a second operand pair summed into the output -- the image tangent of the
+// first block's tangent conv, W_0 applied to x-dot.  Kernel arguments of their own (not Conv0Args fields), so the
+// one-pair kernels keep their parameter layout.
+void launch_conv0(const Conv0Args& a, cudaStream_t st, const float* X2 = nullptr, const float* W2 = nullptr);
 void launch_wgrad(const WgradArgs& a, cudaStream_t st);
-void launch_wgrad0(const WgradArgs& a, cudaStream_t st);
+void launch_wgrad0(const WgradArgs& a, cudaStream_t st);     // nsrc = 2: pair 1 adds A[1] (x) D[1]; the bias row sums D[0]
 void launch_input_grad0(const InputGradArgs& a, cudaStream_t st);
 void launch_bnact(const BnActArgs& a, cudaStream_t st);
-void launch_bnact_tan(const BnActTanArgs& a, cudaStream_t st);
+// gdot / bdot (nullable, [F]): tangents of gamma / beta, pdot = slope * (gamma zhdot + gdot zh + bdot) at the arg-max
+void launch_bnact_tan(const BnActTanArgs& a, cudaStream_t st, const float* gdot = nullptr, const float* bdot = nullptr);
 void launch_bnbwd_reduce(const BnBwdArgs& a, cudaStream_t st);
 void launch_bnbwd_apply(const BnBwdArgs& a, cudaStream_t st);
 void launch_bnbwd_tan_reduce(const BnBwdTanArgs& a, cudaStream_t st);

@@ -117,6 +117,10 @@ struct maml_b200_handle {
   // the functional call (net_forward / net_backward / net_hvp) whose buffers the handle holds; FN_NONE after an
   // iteration or a call that failed.  The image-gradient entries read those buffers and check this record first.
   int fn_kind = 0, fn_tasks = 0, fn_step = 0;
+  // forward-mode buffers outside the workspace, allocated by the first call that needs them (handles that never see
+  // forward mode keep their footprint): the image tangent on the support grid, zero d(logits) for the logits-tangent head
+  float* xdot_g = nullptr;
+  float* zero_dl = nullptr;
   Profiler prof;
   bool profiling = false;             // maml_b200_profile(h, 1): this handle's launches are recorded into prof
   // side streams / events for fork-join inside one iteration, CUDA-graph cache
@@ -490,6 +494,8 @@ extern "C" void maml_b200_destroy(maml_b200_handle* h) {
   for (int s = 0; s < MAML_MAX_STEPS; ++s) if (h->ev_tgt[s]) cudaEventDestroy(h->ev_tgt[s]);
   for (int s = 0; s < 2 * MAML_MAX_LAYERS; ++s) if (h->ev_pre[s]) cudaEventDestroy(h->ev_pre[s]);
   if (h->ws) cudaFree(h->ws);
+  if (h->xdot_g) cudaFree(h->xdot_g - (long long)h->geo[0].guard * h->C);
+  if (h->zero_dl) cudaFree(h->zero_dl);
   if (h->pinned) cudaFreeHost(h->pinned);
   delete h;
 }
@@ -748,19 +754,21 @@ struct TangentHead {
   int kind_tbwd;
 };
 
-// forward-mode tangent of (support forward + support backward) at step s in direction u  =>  H u into `partial`
-static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const float* u, const float* meta,
-                         const TangentHead& th, int T, cudaStream_t st, const ReduceSpec& rs, cudaStream_t spre) {
+// Forward half of the tangent pass at support slot s: the tangent of the support forward in direction u (weights), plus
+// the image tangent xdot_g (padded grid, nullable: W_0 applied to it joins block 0's tangent conv as a second operand
+// pair) and the BatchNorm gamma / beta tangents of step s read from the meta-layout vector t_bn (nullable).  Leaves the
+// normalised tangents in tan.zh and the pooled ones in tan.ain; the features' tangent is tan.ain[L].
+// pre_dgrad: also enqueue the u-weight dgrad convs of the backward half on spre, right behind the forward ones.
+// defer_last: the last block's BatchNorm tangent is not launched but returned (the fused last-block kernel runs it).
+static void tangent_forward(maml_b200_handle* h, int s, const float* theta, const float* u, const float* meta,
+                            const float* xdot_g, const float* t_bn, int T, cudaStream_t st, cudaStream_t spre, bool pre_dgrad,
+                            BnActTanArgs* defer_last) {
   const PassSet& sp = h->sup; const PassSet& tn = h->tan; const PassSet& t2 = h->tan2;
   // Tangent convs of blocks >= 1 have two operand pairs; the pair (primal activation, u weights) depends only on u and
   // on what phase A saved, not on the tangent chain.  It is computed up front on the side stream (right behind the
   // u packs) into the tan2 buffers -- BatchNorm statistics contributions included, they are linear -- and the
   // consumers (bnact_tan / bnbwd_tan) add the two addends.  The main chain keeps the single-pair half: 18 instead of
   // 36 stages per tile on the critical path.  The FFMA convs (no tensor-core path) take both pairs in one launch.
-  // the fused last-block kernels implement the cross-entropy tangent head only
-  const bool fuse_tail = th.mode == HEAD_TANGENT && h->opt.tail_fuse && tail_fusable(bn_geom(h, h->L - 1, sp.n), sp.n, head_rows(sp.n));
-  BnActTanArgs last_act{};
-  HeadArgs hd{};
   if (h->use_tc) {
     for (int l = 1; l < h->L; ++l) {
       tc_conv(h, l, sp.n, tc_op_ain(h, sp, l, s, h->u_map, 0, +1, 2),          // conv(a_in, u_W) + u_b
@@ -768,7 +776,7 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
               STRIDE(sp, zh, l), stat_at(h, PASS_TAN_FWD, s, l), T, spre);
       cudaEventRecord(h->ev_pre[l], spre);
     }
-    for (int l = h->L - 1; l >= 1; --l) {
+    for (int l = h->L - 1; l >= 1 && pre_dgrad; --l) {
       tc_conv(h, l, sp.n, tc_op_dz(h, sp, l, s, h->u_map, 0, -1, 0),           // dgrad(u_W, dz)
               nullptr, 0, DP(t2, l - 1, 0), STRIDE(t2, dp, l - 1), CONV_PLAIN, nullptr, 0, nullptr, T, spre);
       cudaEventRecord(h->ev_pre[MAML_MAX_LAYERS + l], spre);
@@ -786,8 +794,8 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
       a.rows = sp.n * g.G; a.gw = g.gw; a.G = g.G; a.h = g.h; a.w = g.w; a.c0 = h->C; a.ncols = h->F; a.mode = CONV_TAN_STATS;
       a.zh = ZH(sp, 0, s); a.zh_stride = STRIDE(sp, zh, 0);
       a.stats = stat_at(h, PASS_TAN_FWD, s, 0); a.stats_stride = h->stats_task_stride; a.tasks = T;
-      a.alg_flops = conv_flops(h, 0, sp.n, T, 1);
-      launch_conv0(a, st);
+      a.alg_flops = conv_flops(h, 0, sp.n, T, xdot_g ? 2 : 1);
+      launch_conv0(a, st, xdot_g, xdot_g ? theta + h->pl.w_off[0] : nullptr);     // + conv(x_dot, W_0)
     } else if (h->use_tc) {
       tc_conv(h, l, sp.n, tc_op_ain(h, tn, l, 0, h->theta_map, s, +1, 2),       // conv(a_in_dot, W); the other addend is in tan2
               nullptr, 0, ZH(tn, l, 0), STRIDE(tn, zh, l), CONV_TAN_STATS, ZH(sp, l, s),
@@ -818,9 +826,22 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
     b.pdot = AIN(tn, l + 1, 0); b.pdot_stride = STRIDE(tn, ain, l + 1);
     if (h->use_tc && l + 1 < h->L) { b.pdot_hi = AIN_HI(tn, l + 1, 0); b.pdot_lo = AIN_LO(tn, l + 1, 0); }
     b.g = bn_geom(h, l, sp.n); b.tasks = T;
-    if (fuse_tail && l == h->L - 1) last_act = b;
-    else launch_bnact_tan(b, st);
+    if (defer_last && l == h->L - 1) *defer_last = b;
+    else launch_bnact_tan(b, st, t_bn ? gamma_at(h, t_bn, l, s) : nullptr, t_bn ? beta_at(h, t_bn, l, s) : nullptr);
   }
+}
+
+// forward-mode tangent of (support forward + support backward) at step s in direction u (and, with xdot_g, in the
+// images' direction x-dot: pass the padded grid of x-dot)  =>  H u into `partial`
+static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const float* u, const float* meta,
+                         const TangentHead& th, int T, cudaStream_t st, const ReduceSpec& rs, cudaStream_t spre,
+                         const float* xdot_g = nullptr) {
+  const PassSet& sp = h->sup; const PassSet& tn = h->tan; const PassSet& t2 = h->tan2;
+  // the fused last-block kernels implement the cross-entropy tangent head only
+  const bool fuse_tail = th.mode == HEAD_TANGENT && h->opt.tail_fuse && tail_fusable(bn_geom(h, h->L - 1, sp.n), sp.n, head_rows(sp.n));
+  BnActTanArgs last_act{};
+  HeadArgs hd{};
+  tangent_forward(h, s, theta, u, meta, xdot_g, nullptr, T, st, spre, true, fuse_tail ? &last_act : nullptr);
   const ChunkPlan& cp = h->plan_sup;
   join_pending(h, st);
   {
@@ -873,7 +894,12 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
     if (l == 0) {
       w.nsrc = 1;
       w.A[0] = sp.xg; w.a_stride[0] = sp.xg_stride; w.kc = h->C;
-      w.alg_flops = conv_flops(h, 0, sp.n, T, 1);
+      if (xdot_g) {                                                    // + x_dot (x) dz: the image tangent's part
+        w.nsrc = 2;
+        w.A[1] = xdot_g; w.a_stride[1] = sp.xg_stride;
+        w.D[1] = DZ(sp, 0, s); w.d_stride[1] = STRIDE(sp, dz, 0);
+      }
+      w.alg_flops = conv_flops(h, 0, sp.n, T, w.nsrc);
       if (h->L == 1) reduce_upper_on_side(h, rs, cp.pd, h->sup_partial, meta, T);
       launch_wgrad0(w, st);
     } else {
@@ -1224,6 +1250,26 @@ extern "C" int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int3
   return 0;
 }
 
+// A forward-mode buffer allocated on first use and zeroed on the call's stream (the kernels that read it run there; a
+// plain cudaMemset would not be ordered before them on a non-blocking stream).  Nothing is kept if a step fails.
+static int alloc_zeroed(float** out, size_t bytes, cudaStream_t st) {
+  float* p = nullptr;
+  CK(cudaMalloc((void**)&p, bytes));
+  const cudaError_t e = cudaMemsetAsync(p, 0, bytes, st);
+  if (e != cudaSuccess) { cudaFree(p); return fail(std::string("cudaMemsetAsync: ") + cudaGetErrorString(e)); }
+  *out = p;
+  return 0;
+}
+
+// The support-grid buffer of the image tangent x-dot (guard rows included, as sup.xg; zero outside the images).
+static int ensure_xdot(maml_b200_handle* h, cudaStream_t st) {
+  if (h->xdot_g) return 0;
+  float* p = nullptr;
+  if (alloc_zeroed(&p, (size_t)h->sup.xg_stride * h->maxT * sizeof(float), st)) return 1;
+  h->xdot_g = p + (long long)h->geo[0].guard * h->C;
+  return 0;
+}
+
 // Second-order companion of maml_b200_net_backward: what torch.autograd needs to differentiate the backward of the
 // functional operator once more (the reference's loss.backward() through torch.autograd.grad(..., create_graph=True),
 // few_shot_learning_system.py:138-139).  Self-contained: meta_like is imported into theta[num_step] and the whole chain
@@ -1234,8 +1280,8 @@ extern "C" int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int3
 // tbar by the parameter reduction, the BatchNorm gamma / beta sums go to the PASS_TGT_BWD statistics, which export adds
 // (+H_gamma v, +H_beta v); LSLR entries 0.  v_like's BatchNorm and LSLR entries are not read.  Overwrites the batch
 // statistics maml_b200_net_running_update reads; no running-statistics side effect of its own.
-extern "C" int maml_b200_net_hvp(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
-                                 const float* dlogits, const float* v_like, float* jv_out, float* hv_out, void* stream) {
+static int net_hvp_impl(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
+                        const float* xdot, const float* dlogits, const float* v_like, float* jv_out, float* hv_out, void* stream) {
   if (!h || !meta_like || !x || !dlogits || !v_like || !jv_out || !hv_out) return fail("null argument");
   if (n_tasks < 1 || n_tasks > h->maxT) return fail("n_tasks out of range");
   if (num_step < 0 || num_step >= h->S) return fail("num_step out of range");
@@ -1244,11 +1290,13 @@ extern "C" int maml_b200_net_hvp(maml_b200_handle* h, int32_t n_tasks, int32_t n
   const int T = n_tasks, s = num_step;
   float* th = h->theta + (long long)s * h->maxT * h->Ppad;
   record_call(h, FN_NONE, 0, 0);                 // at num_step 0 this overwrites the weights net_forward imported
+  if (xdot && ensure_xdot(h, st)) return 1;
   CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
   CK(cudaMemsetAsync(h->abar, 0, (size_t)h->maxT * h->pl.nseg_inner * MAML_MAX_STEPS * sizeof(double), st));
   CK(cudaMemsetAsync(h->losses, 0, (size_t)h->maxT * MAML_MAX_STEPS * sizeof(float), st));
   CK(cudaMemsetAsync(h->correct, 0, (size_t)h->maxT * sizeof(float), st));
   launch_prep_x(x, h->sup.xg, h->sup.xg_stride, T, h->n_s, h->C, h->H, h->W, st);
+  if (xdot) launch_prep_x(xdot, h->xdot_g, h->sup.xg_stride, T, h->n_s, h->C, h->H, h->W, st);
   launch_import_theta(h->pl, meta_like, th, h->Ppad, T, st);
   launch_import_theta(h->pl, v_like, h->u, h->Ppad, T, st);
   pack_theta_step(h, s, T, st);
@@ -1274,7 +1322,8 @@ extern "C" int maml_b200_net_hvp(maml_b200_handle* h, int32_t n_tasks, int32_t n
   CK(cudaEventRecord(h->ev_wg, spre));
   h->wg_pending = true;
   ReduceSpec rs{PR_STORE, nullptr, nullptr, h->tbar, nullptr, s, -1};
-  tangent_pass(h, s, th, h->u, meta_like, TangentHead{HEAD_EXTERNAL_TAN, nullptr, dlogits, jv_out, PASS_TGT_BWD}, T, st, rs, spre);
+  tangent_pass(h, s, th, h->u, meta_like, TangentHead{HEAD_EXTERNAL_TAN, nullptr, dlogits, jv_out, PASS_TGT_BWD}, T, st, rs, spre,
+               xdot ? h->xdot_g : nullptr);
   join_pending(h, st);
   ExportArgs e{};
   e.pl = h->pl;
@@ -1290,6 +1339,74 @@ extern "C" int maml_b200_net_hvp(maml_b200_handle* h, int32_t n_tasks, int32_t n
   launch_export(e, st);
   CK(cudaGetLastError());
   record_call(h, FN_HVP, T, num_step);
+  return 0;
+}
+
+extern "C" int maml_b200_net_hvp(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
+                                 const float* dlogits, const float* v_like, float* jv_out, float* hv_out, void* stream) {
+  return net_hvp_impl(h, n_tasks, num_step, meta_like, x, nullptr, dlogits, v_like, jv_out, hv_out, stream);
+}
+
+// maml_b200_net_hvp along the images too: the tangent direction is (v_like's weights, xdot).  jv_out = J_theta v +
+// J_x xdot; hv_out = d/d(meta_like) <dlogits, jv_out>.  The first block's tangent conv takes W_0 applied to xdot as a
+// second operand pair and its weight-gradient tangent adds xdot (x) dz_0.  xdot NULL is maml_b200_net_hvp.
+extern "C" int maml_b200_net_hvp_image(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
+                                       const float* x, const float* xdot, const float* dlogits, const float* v_like, float* jv_out,
+                                       float* hv_out, void* stream) {
+  return net_hvp_impl(h, n_tasks, num_step, meta_like, x, xdot, dlogits, v_like, jv_out, hv_out, stream);
+}
+
+// Forward mode of the functional operator: jv_out [n_tasks, N*K, N] = J_theta t + J_x xdot at the weights meta_like, for
+// batches of N*K images (the handle's support shape).  Self-contained: the primal forward at support slot num_step, then
+// the forward half of the tangent pass (no backward).  t_like in the meta layout: conv / linear entries are the weight
+// tangents, the BatchNorm beta / gamma rows of num_step their tangents; LSLR entries are not read.  xdot may be NULL.
+// The logits tangent comes from the HEAD_EXTERNAL_TAN head with d(logits) = 0, whose gradient outputs are discarded.
+// Overwrites the batch statistics maml_b200_net_running_update reads; no running-statistics side effect of its own.
+extern "C" int maml_b200_net_jvp(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
+                                 const float* t_like, const float* xdot, float* jv_out, void* stream) {
+  if (!h || !meta_like || !x || !t_like || !jv_out) return fail("null argument");
+  if (n_tasks < 1 || n_tasks > h->maxT) return fail("n_tasks out of range");
+  if (num_step < 0 || num_step >= h->S) return fail("num_step out of range");
+  cudaStream_t st = (cudaStream_t)stream;
+  LaunchScope launch_scope(h, st);
+  const int T = n_tasks, s = num_step;
+  float* th = h->theta + (long long)s * h->maxT * h->Ppad;
+  record_call(h, FN_NONE, 0, 0);
+  if (xdot && ensure_xdot(h, st)) return 1;
+  // zero d(logits) of one batch, read with a task stride of 0
+  if (!h->zero_dl && alloc_zeroed(&h->zero_dl, (size_t)h->n_s * h->N * sizeof(float), st)) return 1;
+  CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
+  launch_prep_x(x, h->sup.xg, h->sup.xg_stride, T, h->n_s, h->C, h->H, h->W, st);
+  if (xdot) launch_prep_x(xdot, h->xdot_g, h->sup.xg_stride, T, h->n_s, h->C, h->H, h->W, st);
+  launch_import_theta(h->pl, meta_like, th, h->Ppad, T, st);
+  launch_import_theta(h->pl, t_like, h->u, h->Ppad, T, st);
+  pack_theta_step(h, s, T, st);
+  forward_pass(h, h->sup, s, th, s, meta_like, s, PASS_SUP_FWD, T, st);
+  cudaStream_t spre = h->use_tc ? h->s_tgt : h->s_wg;
+  CK(cudaEventRecord(h->ev_fork, st));
+  CK(cudaStreamWaitEvent(spre, h->ev_fork, 0));
+  pack_u(h, T, spre);
+  CK(cudaEventRecord(h->ev_wg, spre));
+  h->wg_pending = true;
+  tangent_forward(h, s, th, h->u, meta_like, xdot ? h->xdot_g : nullptr, t_like, T, st, spre, false, nullptr);
+  join_pending(h, st);
+  const PassSet& sp = h->sup; const PassSet& tn = h->tan;
+  HeadArgs a{};
+  a.mode = HEAD_EXTERNAL_TAN; a.n = h->n_s; a.N = h->N; a.D = h->D; a.scale = 1.f;
+  a.f = AIN(sp, h->L, s); a.f_stride = STRIDE(sp, ain, h->L);
+  a.fdot = AIN(tn, h->L, 0); a.fdot_stride = STRIDE(tn, ain, h->L);
+  a.Wfc = th + h->pl.fcw_off; a.bfc = th + h->pl.fcb_off; a.theta_stride = h->Ppad;
+  a.uW = h->u + h->pl.fcw_off; a.ub = h->u + h->pl.fcb_off; a.u_stride = h->Ppad;
+  a.y = h->zero_labels; a.y_stride = 0;
+  a.dl_ext = h->zero_dl; a.dl_ext_stride = 0;
+  a.logits_out = jv_out; a.logits_stride = (long long)h->n_s * h->N;
+  a.gW = h->sup_partial + h->plan_sup.pd.off[2 * h->L]; a.gb = h->sup_partial + h->plan_sup.pd.off[2 * h->L + 1];
+  a.g_stride = h->plan_sup.pd.task_stride; a.g_chunk_stride = h->plan_sup.pd.cstride[2 * h->L];
+  a.rows_per_cta = head_rows(a.n);
+  a.df = DP(tn, h->L - 1, 0); a.df_stride = STRIDE(tn, dp, h->L - 1);
+  a.tasks = T;
+  launch_head(a, st);
+  CK(cudaGetLastError());
   return 0;
 }
 

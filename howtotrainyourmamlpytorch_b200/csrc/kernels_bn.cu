@@ -417,11 +417,15 @@ __device__ __forceinline__ void bnact_tan_setup(const BnActTanArgs& a, const BnG
   }
 }
 
+// GB: gamma / beta carry tangents (s_gd, s_bd): pdot = slope * (gamma zhdot + gdot zh + bdot) at the arg-max
+template <bool GB = false>
 __device__ __forceinline__ void bnact_tan_phase(const BnActTanArgs& a, const BnGeom& g, int task, int cta, int ncta, const WinIter& it,
                                                 const float* s_r, const float* s_g, const float* s_b, const float* s_md,
-                                                const float* s_q) {
+                                                const float* s_q, const float* s_gd = nullptr, const float* s_bd = nullptr) {
   if (it.lane >= it.WPB) return;
   const float4 r = ld4s(s_r, it.q), ga = ld4s(s_g, it.q), be = ld4s(s_b, it.q), md = ld4s(s_md, it.q), qq = ld4s(s_q, it.q);
+  float4 gd = make_float4(0.f, 0.f, 0.f, 0.f), bd = gd;
+  if constexpr (GB) { gd = ld4s(s_gd, it.q); bd = ld4s(s_bd, it.q); }
   float* zd = a.zdot + (long long)task * a.zdot_stride;
   const float* zd2 = a.zdot2 ? a.zdot2 + (long long)task * a.zdot_stride : nullptr;
   const float* zhp = a.zh + (long long)task * a.zh_stride;
@@ -446,8 +450,13 @@ __device__ __forceinline__ void bnact_tan_phase(const BnActTanArgs& a, const BnG
         float4 y, act, pdv;
         y.x = fmaf(ga.x, zh.x, be.x); y.y = fmaf(ga.y, zh.y, be.y); y.z = fmaf(ga.z, zh.z, be.z); y.w = fmaf(ga.w, zh.w, be.w);
         act.x = leaky(y.x); act.y = leaky(y.y); act.z = leaky(y.z); act.w = leaky(y.w);
-        pdv.x = slope_of(y.x) * ga.x * zhd.x; pdv.y = slope_of(y.y) * ga.y * zhd.y;
-        pdv.z = slope_of(y.z) * ga.z * zhd.z; pdv.w = slope_of(y.w) * ga.w * zhd.w;
+        if constexpr (GB) {
+          pdv.x = slope_of(y.x) * (ga.x * zhd.x + fmaf(gd.x, zh.x, bd.x)); pdv.y = slope_of(y.y) * (ga.y * zhd.y + fmaf(gd.y, zh.y, bd.y));
+          pdv.z = slope_of(y.z) * (ga.z * zhd.z + fmaf(gd.z, zh.z, bd.z)); pdv.w = slope_of(y.w) * (ga.w * zhd.w + fmaf(gd.w, zh.w, bd.w));
+        } else {
+          pdv.x = slope_of(y.x) * ga.x * zhd.x; pdv.y = slope_of(y.y) * ga.y * zhd.y;
+          pdv.z = slope_of(y.z) * ga.z * zhd.z; pdv.w = slope_of(y.w) * ga.w * zhd.w;
+        }
         if (k == 0) { best = act; pbest = pdv; }
         else {
           if (act.x > best.x) { best.x = act.x; pbest.x = pdv.x; }
@@ -476,10 +485,25 @@ __global__ void __launch_bounds__(256) bnact_tan_kernel(BnActTanArgs a) {
   bnact_tan_phase(a, g, task, blockIdx.x, gridDim.x, it, s_r, s_g, s_b, s_md, s_q);
 }
 
-void launch_bnact_tan(const BnActTanArgs& a, cudaStream_t st) {
+// forward tangent with gamma / beta tangents (functional operator's forward mode); a kernel of its own, so that the
+// fused iteration's bnact_tan_kernel keeps its code
+__global__ void __launch_bounds__(256) bnact_tan_gb_kernel(BnActTanArgs a, const float* gdot, const float* bdot) {
+  pdl_prologue(32, a.tag);
+  __shared__ float s_mu[64], s_r[64], s_g[64], s_b[64], s_md[64], s_q[64], s_gd[64], s_bd[64];
+  const BnGeom g = a.g;
+  const int task = blockIdx.y;
+  bnact_tan_setup(a, g, task, (double)g.n * g.h * g.w, s_mu, s_r, s_g, s_b, s_md, s_q);
+  if (threadIdx.x < g.F) { s_gd[threadIdx.x] = gdot[threadIdx.x]; s_bd[threadIdx.x] = bdot[threadIdx.x]; }
+  __syncthreads();
+  WinIter it(g);
+  bnact_tan_phase<true>(a, g, task, blockIdx.x, gridDim.x, it, s_r, s_g, s_b, s_md, s_q, s_gd, s_bd);
+}
+
+void launch_bnact_tan(const BnActTanArgs& a, cudaStream_t st, const float* gdot, const float* bdot) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
   int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
-  launch_pdl(bnact_tan_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
+  if (gdot) launch_pdl(bnact_tan_gb_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a), gdot, bdot);
+  else launch_pdl(bnact_tan_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();
 }
 

@@ -201,9 +201,14 @@ void launch_conv_rows(const ConvArgs& a, cudaStream_t st) {
 
 // ---------------------------------------------------------------------------------------------
 // first block: K = 9 * C0 (9 or 27) -- all weights and the image window live in shared memory
+// The two-pair instantiations (NSRC = 2: the image tangent of the functional operator) repeat the staging and the inner
+// loop of the first pair in `if constexpr (NSRC == 2)` blocks.  The copies are deliberate: one force-inlined helper or
+// lambda called once per pair changes the register allocation and instruction order of the one-pair instantiations,
+// which the fused iteration runs.
 // ---------------------------------------------------------------------------------------------
-template <int FN>
-__global__ void __launch_bounds__(256) conv0_kernel(Conv0Args a) {
+// NSRC = 2 adds the pair (X2, W2) (image tangent): its weights and window are staged behind the first pair's
+template <int FN, int NSRC>
+__global__ void __launch_bounds__(256) conv0_kernel(Conv0Args a, const float* X2, const float* W2) {
   pdl_prologue(2, a.tag);
   constexpr int NC = 16 * FN;
   extern __shared__ float sm0[];
@@ -225,6 +230,19 @@ __global__ void __launch_bounds__(256) conv0_kernel(Conv0Args a) {
     float v = 0.f;
     if (r >= -guard && r < a.rows + guard) v = X[(long long)(j0 - halo) * c0 + i];
     xs[i] = v;
+  }
+  if constexpr (NSRC == 2) {
+    float* Ws2 = xs + wrows * c0;        // [9*c0][NC], then the window [(64 + 2*(gw+1))][c0]
+    float* xs2 = Ws2 + 9 * c0 * NC;
+    const float* W2t = W2 + (long long)task * a.w_stride;
+    for (int i = tid; i < 9 * c0 * NC; i += 256) Ws2[i] = W2t[i];
+    const float* X2t = X2 + (long long)task * a.x_stride;
+    for (int i = tid; i < wrows * c0; i += 256) {
+      const int r = j0 - halo + i / c0;
+      float v = 0.f;
+      if (r >= -guard && r < a.rows + guard) v = X2t[(long long)(j0 - halo) * c0 + i];
+      xs2[i] = v;
+    }
   }
   __syncthreads();
 
@@ -248,6 +266,24 @@ __global__ void __launch_bounds__(256) conv0_kernel(Conv0Args a) {
       }
     }
   }
+  if constexpr (NSRC == 2) {                 // the second pair: the same loop over its staged weights and window
+    const float* Ws2 = xs + wrows * c0;
+    const float* xs2 = Ws2 + 9 * c0 * NC;
+    for (int tap = 0; tap < 9; ++tap) {
+      const int sh = tap_shift(tap, a.gw) + halo;
+      for (int c = 0; c < c0; ++c) {
+        float b[FN];
+#pragma unroll
+        for (int jn = 0; jn < FN; ++jn) b[jn] = Ws2[(tap * c0 + c) * NC + tx * FN + jn];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float av = xs2[(ty * 4 + i + sh) * c0 + c];
+#pragma unroll
+          for (int jn = 0; jn < FN; ++jn) acc[i][jn] = fmaf(av, b[jn], acc[i][jn]);
+        }
+      }
+    }
+  }
   conv_epilogue<FN>(acc, j0, a.rows, a.gw, a.G, a.h, a.w, a.mode,
                     a.bias ? a.bias + (long long)task * a.bias_stride : nullptr,
                     a.out + (long long)task * a.out_stride,
@@ -260,8 +296,9 @@ __global__ void __launch_bounds__(256) conv0_kernel(Conv0Args a) {
 // registers (10 * C0 broadcast loads) and feed 8 x 3 x C0 x FN FMAs, the weights of the row come as 3 * C0 vector loads
 // -- ~4 FMAs per shared-memory load instead of 12 per 7 in conv0_kernel, 128 rows per CTA instead of 64.
 // Measured on Mini-ImageNet target passes (75 images of 84x84x3 -> 48 channels per task): see DESIGN.md.
-template <int FN, int C0>
-__global__ void __launch_bounds__(256) conv0_rb_kernel(Conv0Args a, int tiles) {
+// NSRC = 2 adds the pair (X2, W2) (image tangent): its weights and window are staged behind the first pair's
+template <int FN, int C0, int NSRC>
+__global__ void __launch_bounds__(256) conv0_rb_kernel(Conv0Args a, int tiles, const float* X2, const float* W2) {
   pdl_prologue(2, a.tag);
   constexpr int NC = 16 * FN, R = 8, ROWS = 16 * R;
   extern __shared__ float sm0[];
@@ -282,6 +319,19 @@ __global__ void __launch_bounds__(256) conv0_rb_kernel(Conv0Args a, int tiles) {
     float v = 0.f;
     if (r >= -guard && r < a.rows + guard) v = X[(long long)(j00 - halo) * C0 + i];
     xs[i] = v;
+  }
+  if constexpr (NSRC == 2) {
+    float* Ws2 = xs + wrows * C0;        // [9*C0][NC], then the window [(ROWS*tiles + 2*(gw+1))][C0]
+    float* xs2 = Ws2 + 9 * C0 * NC;
+    const float* W2t = W2 + (long long)task * a.w_stride;
+    for (int i = tid; i < 9 * C0 * NC; i += 256) Ws2[i] = W2t[i];
+    const float* X2t = X2 + (long long)task * a.x_stride;
+    for (int i = tid; i < wrows * C0; i += 256) {
+      const int r = j00 - halo + i / C0;
+      float v = 0.f;
+      if (r >= -guard && r < a.rows + guard) v = X2t[(long long)(j00 - halo) * C0 + i];
+      xs2[i] = v;
+    }
   }
   float bv[FN];
   {
@@ -324,6 +374,34 @@ __global__ void __launch_bounds__(256) conv0_rb_kernel(Conv0Args a, int tiles) {
             const float av = xw[(i + kx) * C0 + c];
 #pragma unroll
             for (int jn = 0; jn < FN; ++jn) acc[i][jn] = fmaf(av, b[jn], acc[i][jn]);
+          }
+        }
+      }
+    }
+    if constexpr (NSRC == 2) {               // the second pair: the same loop over its staged weights and window
+      const float* Ws2 = xs + wrows * C0;
+      const float* xs2 = Ws2 + 9 * C0 * NC;
+#pragma unroll
+      for (int ky = 0; ky < 3; ++ky) {
+        // positions t*ROWS + ty*R + (ky-1)*gw - 1 + halo .. + R + 1 of the window (always inside it)
+        const float* xp = xs2 + (t * ROWS + ty * R + (ky - 1) * a.gw - 1 + halo) * C0;
+        float xw[(R + 2) * C0];
+#pragma unroll
+        for (int i = 0; i < (R + 2) * C0; ++i) xw[i] = xp[i];
+#pragma unroll
+        for (int kx = 0; kx < 3; ++kx) {
+#pragma unroll
+          for (int c = 0; c < C0; ++c) {
+            float b[FN];
+            const float* wp = Ws2 + ((ky * 3 + kx) * C0 + c) * NC + tx * FN;
+#pragma unroll
+            for (int jn = 0; jn < FN; ++jn) b[jn] = wp[jn];
+#pragma unroll
+            for (int i = 0; i < R; ++i) {
+              const float av = xw[(i + kx) * C0 + c];
+#pragma unroll
+              for (int jn = 0; jn < FN; ++jn) acc[i][jn] = fmaf(av, b[jn], acc[i][jn]);
+            }
           }
         }
       }
@@ -382,38 +460,55 @@ __global__ void __launch_bounds__(256) conv0_rb_kernel(Conv0Args a, int tiles) {
   }
 }
 
-template <int C0>
-static bool launch_conv0_rb(const Conv0Args& a, cudaStream_t st) {
+// dynamic shared memory beyond the default 48 KB (two-pair launches of large windows) has to be opted into per kernel
+template <class K>
+static K smem_optin(K kernel, size_t smem) {
+  if (smem > 48 * 1024) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  return kernel;
+}
+template <class K>
+static void launch_conv0_k(K kernel, dim3 grid, size_t smem, cudaStream_t st, const Conv0Args& a, int tiles, const float* X2,
+                           const float* W2) {
+  launch_pdl(smem_optin(kernel, smem), grid, dim3(256), smem, st, tagged(a), tiles, X2, W2);
+}
+
+template <int C0, int NSRC>
+static bool launch_conv0_rb(const Conv0Args& a, cudaStream_t st, const float* X2, const float* W2) {
   // tiles per CTA: as many as keep >= ~3 CTAs per SM in flight (fixed per-CTA cost -- weights, window, fp64 statistics
   // reduction -- is then paid once per `tiles` x 128 rows); 1 for the small launches that sit on the latency-critical chain
   const long long t128 = (a.rows + 127) / 128;
   int tiles = (int)std::min<long long>(8, std::max<long long>(1, t128 * a.tasks / (3LL * num_sms())));
   dim3 grid((unsigned)((t128 + tiles - 1) / tiles), a.tasks);
-  const size_t smem = (size_t)(9 * C0 * a.ncols + (128 * tiles + 2 * (a.gw + 1)) * C0) * sizeof(float);
+  const size_t smem = (size_t)NSRC * (9 * C0 * a.ncols + (128 * tiles + 2 * (a.gw + 1)) * C0) * sizeof(float);
   switch (a.ncols / 16) {
-    case 1: launch_pdl(conv0_rb_kernel<1, C0>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a), tiles); break;
-    case 2: launch_pdl(conv0_rb_kernel<2, C0>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a), tiles); break;
-    case 3: launch_pdl(conv0_rb_kernel<3, C0>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a), tiles); break;
-    default: launch_pdl(conv0_rb_kernel<4, C0>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a), tiles); break;
+    case 1: launch_conv0_k(conv0_rb_kernel<1, C0, NSRC>, grid, smem, st, a, tiles, X2, W2); break;
+    case 2: launch_conv0_k(conv0_rb_kernel<2, C0, NSRC>, grid, smem, st, a, tiles, X2, W2); break;
+    case 3: launch_conv0_k(conv0_rb_kernel<3, C0, NSRC>, grid, smem, st, a, tiles, X2, W2); break;
+    default: launch_conv0_k(conv0_rb_kernel<4, C0, NSRC>, grid, smem, st, a, tiles, X2, W2); break;
   }
   return true;
 }
 
-void launch_conv0(const Conv0Args& a, cudaStream_t st) {
-  ProfScope prof_scope__(PROF_CONV0, a.alg_flops, st);
+template <int NSRC>
+static void launch_conv0_n(const Conv0Args& a, cudaStream_t st, const float* X2, const float* W2) {
   if (a.c0 == 1 || a.c0 == 3) {
-    if (a.c0 == 1) launch_conv0_rb<1>(a, st); else launch_conv0_rb<3>(a, st);
-    CUDA_CHECK_LAUNCH();
+    if (a.c0 == 1) launch_conv0_rb<1, NSRC>(a, st, X2, W2); else launch_conv0_rb<3, NSRC>(a, st, X2, W2);
     return;
   }
   dim3 grid((a.rows + 63) / 64, a.tasks);
-  const size_t smem = (size_t)(9 * a.c0 * a.ncols + (64 + 2 * (a.gw + 1)) * a.c0) * sizeof(float);
+  const size_t smem = (size_t)NSRC * (9 * a.c0 * a.ncols + (64 + 2 * (a.gw + 1)) * a.c0) * sizeof(float);
   switch (a.ncols / 16) {
-    case 1: launch_pdl(conv0_kernel<1>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a)); break;
-    case 2: launch_pdl(conv0_kernel<2>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a)); break;
-    case 3: launch_pdl(conv0_kernel<3>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a)); break;
-    default: launch_pdl(conv0_kernel<4>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a)); break;
+    case 1: launch_pdl(smem_optin(conv0_kernel<1, NSRC>, smem), dim3(grid), dim3(256), (size_t)(smem), st, tagged(a), X2, W2); break;
+    case 2: launch_pdl(smem_optin(conv0_kernel<2, NSRC>, smem), dim3(grid), dim3(256), (size_t)(smem), st, tagged(a), X2, W2); break;
+    case 3: launch_pdl(smem_optin(conv0_kernel<3, NSRC>, smem), dim3(grid), dim3(256), (size_t)(smem), st, tagged(a), X2, W2); break;
+    default: launch_pdl(smem_optin(conv0_kernel<4, NSRC>, smem), dim3(grid), dim3(256), (size_t)(smem), st, tagged(a), X2, W2); break;
   }
+}
+
+void launch_conv0(const Conv0Args& a, cudaStream_t st, const float* X2, const float* W2) {
+  ProfScope prof_scope__(PROF_CONV0, a.alg_flops, st);
+  if (X2) launch_conv0_n<2>(a, st, X2, W2);
+  else launch_conv0_n<1>(a, st, nullptr, nullptr);
   CUDA_CHECK_LAUNCH();
 }
 
@@ -547,7 +642,8 @@ void launch_wgrad(const WgradArgs& a, cudaStream_t st) {
 // first block wgrad: A = image matrix [rows][c0] (c0 <= 4), D = dz [rows][F].
 // Per 64-row sub-tile the dz rows and the image window (rows +/- halo) are staged in shared memory; thread
 // (grp, f) accumulates the (tap, c) combinations q = grp, grp + NG, ... for output channel f.
-template <int MAXQ>
+// NSRC = 2 adds pair 1, A[1] (x) D[1], staged behind pair 0's arrays (the bias row sums D[0] only)
+template <int MAXQ, int NSRC>
 __global__ void __launch_bounds__(256) wgrad0_kernel(WgradArgs a) {
   pdl_prologue(4, a.tag);
   extern __shared__ float smw[];
@@ -590,6 +686,17 @@ __global__ void __launch_bounds__(256) wgrad0_kernel(WgradArgs a) {
       if (r >= -guard && r < a.rows + guard) v = A[(long long)(r0 - halo) * c0 + i];
       Xs[i] = v;
     }
+    if constexpr (NSRC == 2) {
+      float* Ds2 = Xs + (((RT + 2 * halo) * c0 + 3) & ~3);   // [RT][Fc], then [(RT + 2*halo)][c0] (pair 0's window padded)
+      float* Xs2 = Ds2 + RT * Fc;
+      const float* A2 = a.A[1] + (long long)task * a.a_stride[1];
+      const float* D2 = a.D[1] + (long long)task * a.d_stride[1];
+      for (int i = tid; i < RT * Fc; i += 256) Ds2[i] = (i / Fc < nr) ? D2[(long long)r0 * Fc + i] : 0.f;
+      for (int i = tid; i < (RT + 2 * halo) * c0; i += 256) {
+        const int r = r0 - halo + i / c0;
+        Xs2[i] = (r >= -guard && r < a.rows + guard) ? A2[(long long)(r0 - halo) * c0 + i] : 0.f;
+      }
+    }
     __syncthreads();
     if (active) {
       for (int r = 0; r < nr; ++r) {
@@ -599,6 +706,16 @@ __global__ void __launch_bounds__(256) wgrad0_kernel(WgradArgs a) {
         for (int i = 0; i < MAXQ; ++i) {
           const int q = grp + i * NG;
           if (q < ncombo) acc[i] = fmaf(xr[off[i]], d, acc[i]);
+        }
+        if constexpr (NSRC == 2) {
+          const float* Ds2 = Xs + (((RT + 2 * halo) * c0 + 3) & ~3);
+          const float d2 = Ds2[r * Fc + f];
+          const float* xr2 = Ds2 + RT * Fc + r * c0;
+#pragma unroll
+          for (int i = 0; i < MAXQ; ++i) {
+            const int q = grp + i * NG;
+            if (q < ncombo) acc[i] = fmaf(xr2[off[i]], d2, acc[i]);
+          }
         }
         bacc += d;
       }
@@ -622,8 +739,10 @@ __global__ void __launch_bounds__(256) wgrad0_kernel(WgradArgs a) {
 // three x positions of a row slide by one per row: per row C0 broadcast loads + one LDS.128 of dz feed 12 * C0 FMAs
 // (wgrad0_kernel: 7 loads per 6 FMAs).  Streams are summed through shared memory in stream order (deterministic).
 // C0 = 1 is held to 48 registers (5 CTAs per SM); left to itself ptxas gives it 58 (4 CTAs).  0: no bound for C0 = 3.
-template <int C0>
-__global__ void __launch_bounds__(256, C0 == 1 ? 5 : 0) wgrad0_rb_kernel(WgradArgs a) {
+// NSRC = 2 adds pair 1, A[1] (x) D[1] (forward-over-reverse with an image tangent), staged behind pair 0 and walked by the
+// same row streams; the bias row sums D[0] only.  No register bound: it is not on the fused iteration's path.
+template <int C0, int NSRC>
+__global__ void __launch_bounds__(256, (C0 == 1 && NSRC == 1) ? 5 : 0) wgrad0_rb_kernel(WgradArgs a) {
   pdl_prologue(4, a.tag);
   extern __shared__ float smw[];
   const int task = blockIdx.y, chunk = blockIdx.x;
@@ -666,6 +785,18 @@ __global__ void __launch_bounds__(256, C0 == 1 ? 5 : 0) wgrad0_rb_kernel(WgradAr
       if (r >= -guard && r < a.rows + guard) v = A[(long long)(r0 - halo) * C0 + i];
       Xs[i] = v;
     }
+    if constexpr (NSRC == 2) {
+      // [RT][Fc], then [(RT + 2*halo)][C0]; pair 0's window is padded to 4 floats: Ds2 is read as float4
+      float* Ds2 = Xs + (((RT + 2 * halo) * C0 + 3) & ~3);
+      float* Xs2 = Ds2 + RT * Fc;
+      const float* A2 = a.A[1] + (long long)task * a.a_stride[1];
+      const float* D2 = a.D[1] + (long long)task * a.d_stride[1];
+      for (int i = tid; i < RT * Fc; i += 256) Ds2[i] = (i / Fc < nr) ? D2[(long long)r0 * Fc + i] : 0.f;
+      for (int i = tid; i < (RT + 2 * halo) * C0; i += 256) {
+        const int r = r0 - halo + i / C0;
+        Xs2[i] = (r >= -guard && r < a.rows + guard) ? A2[(long long)(r0 - halo) * C0 + i] : 0.f;
+      }
+    }
     __syncthreads();
     if (active) {
       const int rs = stream * L;                                        // first row of this stream in the tile
@@ -689,6 +820,33 @@ __global__ void __launch_bounds__(256, C0 == 1 ? 5 : 0) wgrad0_rb_kernel(WgradAr
             acc[kx][c][3] = fmaf(xw[kx][c], d.w, acc[kx][c][3]);
           }
         bacc[0] += d.x; bacc[1] += d.y; bacc[2] += d.z; bacc[3] += d.w;
+      }
+    }
+    if constexpr (NSRC == 2) {               // pair 1 on the same row streams (the bias row sums pair 0 only)
+      const float* Ds2 = Xs + (((RT + 2 * halo) * C0 + 3) & ~3);
+      const float* Xs2 = Ds2 + RT * Fc;
+      if (active) {
+        const int rs = stream * L;                                        // first row of this stream in the tile
+        // window row index of tap (ky, kx) for tile row r: r + halo + (ky-1)*gw + (kx-1)
+        const float* xp = Xs2 + (rs + halo + (ky - 1) * a.gw - 1) * C0;
+        float xw[3][C0];
+#pragma unroll
+        for (int c = 0; c < C0; ++c) { xw[1][c] = xp[c]; xw[2][c] = xp[C0 + c]; }
+#pragma unroll 4
+        for (int r = 0; r < L; ++r) {
+#pragma unroll
+          for (int c = 0; c < C0; ++c) { xw[0][c] = xw[1][c]; xw[1][c] = xw[2][c]; xw[2][c] = xp[(r + 2) * C0 + c]; }
+          const float4 d = *reinterpret_cast<const float4*>(Ds2 + (rs + r) * Fc + f4 * 4);
+#pragma unroll
+          for (int kx = 0; kx < 3; ++kx)
+#pragma unroll
+            for (int c = 0; c < C0; ++c) {
+              acc[kx][c][0] = fmaf(xw[kx][c], d.x, acc[kx][c][0]);
+              acc[kx][c][1] = fmaf(xw[kx][c], d.y, acc[kx][c][1]);
+              acc[kx][c][2] = fmaf(xw[kx][c], d.z, acc[kx][c][2]);
+              acc[kx][c][3] = fmaf(xw[kx][c], d.w, acc[kx][c][3]);
+            }
+        }
       }
     }
     __syncthreads();
@@ -721,22 +879,36 @@ __global__ void __launch_bounds__(256, C0 == 1 ? 5 : 0) wgrad0_rb_kernel(WgradAr
 void launch_wgrad0(const WgradArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_WGRAD0, a.alg_flops, st);
   dim3 grid(a.nchunks, a.tasks);
-  if ((a.kc == 1 || a.kc == 3) && a.nsrc == 1 && (a.ncols % 4) == 0) {
+  if ((a.kc == 1 || a.kc == 3) && (a.ncols % 4) == 0) {
     const int tps = 3 * (a.ncols / 4), ns = 256 / tps, rt = ns * 16;
-    const size_t stage = (size_t)(rt * a.ncols + (rt + 2 * (a.gw + 1)) * a.kc) * sizeof(float);
+    const size_t win = (size_t)(rt + 2 * (a.gw + 1)) * a.kc;      // a second pair starts at a 4-float boundary
+    const size_t stage = (rt * a.ncols + win + (a.nsrc == 2 ? rt * a.ncols + ((win + 3) & ~(size_t)3) : 0)) * sizeof(float);
     const size_t red = (size_t)ns * (9 * a.kc + 1) * a.ncols * sizeof(float);
     const size_t smem = stage > red ? stage : red;
-    if (a.kc == 1) launch_pdl(wgrad0_rb_kernel<1>, dim3(grid), dim3(256), smem, st, tagged(a));
-    else launch_pdl(wgrad0_rb_kernel<3>, dim3(grid), dim3(256), smem, st, tagged(a));
+    if (a.nsrc == 2) {
+      if (a.kc == 1) launch_pdl(smem_optin(wgrad0_rb_kernel<1, 2>, smem), dim3(grid), dim3(256), smem, st, tagged(a));
+      else launch_pdl(smem_optin(wgrad0_rb_kernel<3, 2>, smem), dim3(grid), dim3(256), smem, st, tagged(a));
+    } else {
+      if (a.kc == 1) launch_pdl(wgrad0_rb_kernel<1, 1>, dim3(grid), dim3(256), smem, st, tagged(a));
+      else launch_pdl(wgrad0_rb_kernel<3, 1>, dim3(grid), dim3(256), smem, st, tagged(a));
+    }
     CUDA_CHECK_LAUNCH();
     return;
   }
-  const size_t smem = (size_t)(64 * a.ncols + (64 + 2 * (a.gw + 1)) * a.kc) * sizeof(float);
+  const size_t win = (size_t)(64 + 2 * (a.gw + 1)) * a.kc;        // a second pair starts at a 4-float boundary
+  const size_t smem = (64 * a.ncols + win + (a.nsrc == 2 ? 64 * a.ncols + ((win + 3) & ~(size_t)3) : 0)) * sizeof(float);
   const int need = (9 * a.kc + (256 / a.ncols) - 1) / (256 / a.ncols);      // (tap, c) combinations per thread
-  if (need <= 3) launch_pdl(wgrad0_kernel<3>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
-  else if (need <= 6) launch_pdl(wgrad0_kernel<6>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
-  else if (need <= 9) launch_pdl(wgrad0_kernel<9>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
-  else launch_pdl(wgrad0_kernel<36>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
+  if (a.nsrc == 2) {
+    if (need <= 3) launch_pdl(smem_optin(wgrad0_kernel<3, 2>, smem), dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
+    else if (need <= 6) launch_pdl(smem_optin(wgrad0_kernel<6, 2>, smem), dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
+    // F <= 64 and C0 <= 4 (maml_b200_create) give need <= 9: the two-pair form has no MAXQ = 36 instantiation
+    else launch_pdl(smem_optin(wgrad0_kernel<9, 2>, smem), dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
+  } else {
+    if (need <= 3) launch_pdl(wgrad0_kernel<3, 1>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
+    else if (need <= 6) launch_pdl(wgrad0_kernel<6, 1>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
+    else if (need <= 9) launch_pdl(wgrad0_kernel<9, 1>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
+    else launch_pdl(wgrad0_kernel<36, 1>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
+  }
   CUDA_CHECK_LAUNCH();
 }
 

@@ -15,6 +15,7 @@ Initialisation restates reference ``:62-66`` (xavier_uniform_ conv weight, zero 
 per-step but ZEROS in shared mode; beta zeros; gamma ones).
 """
 import torch
+import torch.autograd.forward_ad as fwAD
 import torch.nn as nn
 
 
@@ -243,15 +244,72 @@ class _FunctionalForward(torch.autograd.Function):
             net._apply_running_ema(st, num_step)
         st["gen"] += 1
         ctx.net, ctx.num_step, ctx.gen = net, num_step, st["gen"]
-        # x and the weights themselves: a double backward differentiates w.r.t. them
+        # x and the weights themselves: a double backward differentiates w.r.t. them, forward mode at them
         ctx.save_for_backward(x, *tensors)
+        ctx.save_for_forward(x, *tensors)
         return logits[0].clone()
 
     @staticmethod
     def backward(ctx, dlogits):
         x, tensors = ctx.saved_tensors[0], ctx.saved_tensors[1:]
+        for i, t in enumerate(tensors[:4 * ctx.net.num_stages]):
+            if i % 4 >= 2 and fwAD.unpack_dual(t).tangent is not None:
+                raise NotImplementedError(
+                    "differentiating the gradient in forward mode along a BatchNorm gamma / beta tangent needs gamma / beta "
+                    "tangent directions in the backward tangent pass, which the engine does not implement (BatchNorm "
+                    "parameters as inner-loop fast weights, enable_inner_loop_optimizable_bn_params, are outside the "
+                    "accelerated path)")
         out = _FunctionalBackward.apply(ctx, x, dlogits, *tensors)
         return (None, out[0], None) + tuple(out[1:])
+
+    @staticmethod
+    def jvp(ctx, _net_t, x_t, _step_t, *tangents):
+        """Forward mode (``torch.autograd.forward_ad``): the logits tangent J_theta t + J_x x_t through
+        ``maml_b200_net_jvp`` on the second (HVP) handle -- one primal forward and one tangent forward.  Tangents may sit
+        on the images, the conv / linear weights and the BatchNorm gamma / beta."""
+        x, tensors = ctx.saved_tensors[0], ctx.saved_tensors[1:]
+        xin = x.detach().to(torch.float32).contiguous()
+        hs = ctx.net._hvp_engine(xin)
+        eng, meta_like, t_like, jv = hs["eng"], hs["meta"], hs["v"], hs["jv"]
+        _fill_meta(eng, meta_like, tensors, t_like, tangents)
+        xdot = None if x_t is None else x_t.detach().to(torch.float32).contiguous()
+        with torch.cuda.device(xin.device):
+            eng.net_jvp(1, ctx.num_step, meta_like, xin, t_like, xdot, jv)
+        return jv[0].clone()
+
+
+def _fill_meta(eng, meta_like, tensors, v_like, directions):
+    """meta_like <- the tensors, v_like <- the directions (None: zero) in the engine's meta layout."""
+    with torch.no_grad():
+        v_like.zero_()
+        for (off, size), t, d in zip(eng.segments, tensors, directions):
+            meta_like[off:off + size].copy_(t.detach().reshape(-1).to(torch.float32))
+            if d is not None:
+                v_like[off:off + size].copy_(d.detach().reshape(-1).to(torch.float32))
+
+
+def _net_backward(fwd_ctx, xin, tensors, dl, x_dtype):
+    """J^T dl on the operator's handle (``maml_b200_net_backward``), after replaying ``fwd_ctx``'s forward when another
+    forward of this shape ran since (the handle keeps the activations of its last forward only; the replay has no EMA side
+    effect), and J_x^T dl (``maml_b200_net_input_grad``) when x requires grad.  Returns (the handle's state, whose "grad"
+    holds the weight gradients in the meta layout; dx or None)."""
+    net, num_step = fwd_ctx.net, fwd_ctx.num_step
+    st = net._operator_engine(xin)
+    eng, meta_like, logits, grad = st["eng"], st["meta"], st["logits"], st["grad"]
+    with torch.no_grad(), torch.cuda.device(xin.device):
+        if st["gen"] != fwd_ctx.gen:
+            for (off, size), t in zip(eng.segments, tensors):
+                meta_like[off:off + size].copy_(t.detach().reshape(-1).to(torch.float32))
+            eng.net_forward(1, num_step, meta_like, xin, logits)
+            st["gen"] += 1
+            fwd_ctx.gen = st["gen"]
+        eng.net_backward(1, num_step, meta_like, dl.detach().to(torch.float32).contiguous().view(1, *dl.shape), grad)
+        dx = None
+        if fwd_ctx.needs_input_grad[1]:
+            dx = st.setdefault("dx", torch.empty((1,) + tuple(xin.shape), dtype=torch.float32, device=xin.device))
+            eng.net_input_grad(1, dx)
+            dx = dx[0].to(x_dtype, copy=True)
+    return st, dx
 
 
 class _FunctionalBackward(torch.autograd.Function):
@@ -276,28 +334,56 @@ class _FunctionalBackward(torch.autograd.Function):
     def forward(ctx, fwd_ctx, x, dlogits, *tensors):
         net, num_step = fwd_ctx.net, fwd_ctx.num_step
         xin = x.detach().to(torch.float32).contiguous()
-        st = net._operator_engine(xin)
-        eng, meta_like, logits, grad = st["eng"], st["meta"], st["logits"], st["grad"]
-        with torch.cuda.device(xin.device):
-            if st["gen"] != fwd_ctx.gen:             # another forward ran since: replay ours (no EMA side effect again)
-                for (off, size), t in zip(eng.segments, tensors):
-                    meta_like[off:off + size].copy_(t.detach().reshape(-1).to(torch.float32))
-                eng.net_forward(1, num_step, meta_like, xin, logits)
-                st["gen"] += 1
-                fwd_ctx.gen = st["gen"]
-            eng.net_backward(1, num_step, meta_like, dlogits.detach().to(torch.float32).contiguous().view(1, *dlogits.shape), grad)
-            dx = None
-            if fwd_ctx.needs_input_grad[1]:
-                dx = st.setdefault("dx", torch.empty((1,) + tuple(xin.shape), dtype=torch.float32, device=xin.device))
-                eng.net_input_grad(1, dx)
-                dx = dx[0].to(x.dtype, copy=True)
+        st, dx = _net_backward(fwd_ctx, xin, tensors, dlogits, x.dtype)
+        eng, grad = st["eng"], st["grad"]
         ctx.set_materialize_grads(False)
-        ctx.net, ctx.num_step = net, num_step
+        ctx.net, ctx.num_step, ctx.fwd_ctx = net, num_step, fwd_ctx
         ctx.save_for_backward(x, dlogits, *tensors)
+        ctx.save_for_forward(x, dlogits, *tensors)
         grads = []
         for (off, size), t, need in zip(eng.segments, tensors, fwd_ctx.needs_input_grad[3:]):
             grads.append(grad[off:off + size].view(t.shape).clone() if need else None)
         return (dx,) + tuple(grads)
+
+    @staticmethod
+    def jvp(ctx, _fwd_ctx_t, x_t, dl_t, *tangents):
+        """Forward-over-reverse: the tangent of every gradient this node returned, along (x_t, dl_t, tangents).  For a
+        weight gradient J_theta^T dl_t + d/dtheta <dl, J_theta t + J_x x_t>; for dx the same with d/dx.  The first term is
+        ``maml_b200_net_backward`` (+ ``net_input_grad``) of dl_t on the operator's handle, the second
+        ``maml_b200_net_hvp_image`` (+ ``net_hvp_input_grad``) on the HVP handle; a term whose tangents are all None is
+        skipped.  A tangent on a BatchNorm gamma / beta input never gets here: ``_FunctionalForward.backward`` refuses it
+        before this node runs."""
+        net, num_step, fwd_ctx = ctx.net, ctx.num_step, ctx.fwd_ctx
+        x, dlogits, tensors = ctx.saved_tensors[0], ctx.saved_tensors[1], ctx.saved_tensors[2:]
+        need_x = fwd_ctx.needs_input_grad[1]
+        needs = fwd_ctx.needs_input_grad[3:]
+        xin = x.detach().to(torch.float32).contiguous()
+        dx_t, grads_t = None, [None] * len(tensors)
+
+        def add(acc, v):
+            return v if acc is None else acc + v
+        with torch.cuda.device(xin.device):
+            if dl_t is not None:                              # J^T dl_t on the operator's handle
+                st, dx_t = _net_backward(fwd_ctx, xin, tensors, dl_t, x.dtype)
+                eng, grad = st["eng"], st["grad"]
+                for k, ((off, size), t) in enumerate(zip(eng.segments, tensors)):
+                    if needs[k]:
+                        grads_t[k] = add(grads_t[k], grad[off:off + size].view(t.shape).clone())
+            if x_t is not None or any(t is not None for t in tangents):    # d/d(theta, x) <dl, J_theta t + J_x x_t>
+                hs = net._hvp_engine(xin)
+                eng, meta_like, v_like, jv, hv = hs["eng"], hs["meta"], hs["v"], hs["jv"], hs["hv"]
+                _fill_meta(eng, meta_like, tensors, v_like, tangents)
+                xdot = None if x_t is None else x_t.detach().to(torch.float32).contiguous()
+                eng.net_hvp_image(1, num_step, meta_like, xin, xdot,
+                                  dlogits.detach().to(torch.float32).contiguous().view(1, *dlogits.shape), v_like, jv, hv)
+                if need_x:
+                    dxdot = hs.setdefault("dxdot", torch.empty((1,) + tuple(xin.shape), dtype=torch.float32, device=xin.device))
+                    eng.net_hvp_input_grad(1, dxdot)
+                    dx_t = add(dx_t, dxdot[0].to(x.dtype, copy=True))
+                for k, ((off, size), t) in enumerate(zip(eng.segments, tensors)):
+                    if needs[k]:
+                        grads_t[k] = add(grads_t[k], hv[off:off + size].view(t.shape).clone())
+        return (dx_t if need_x else None,) + tuple(grads_t)
 
     @staticmethod
     @torch.autograd.function.once_differentiable

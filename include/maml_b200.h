@@ -137,6 +137,26 @@ int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int32_t num_ste
 int maml_b200_net_hvp(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
                       const float* dlogits, const float* v_like, float* jv_out, float* hv_out, void* stream);
 
+/* maml_b200_net_hvp with an image tangent as well: the tangent direction is (v_like, xdot), xdot [n_tasks, N*K, C, H, W]
+ * or NULL (then exactly maml_b200_net_hvp).  jv_out = J_theta v + J_x xdot; hv_out = d/d(meta_like) <dlogits, jv_out>,
+ * laid out as in maml_b200_net_hvp.  Like it, it may be followed by maml_b200_net_hvp_input_grad, which then gives
+ * d/dx <dlogits, jv_out>.  The image-tangent buffer is allocated by the first call with xdot != NULL, outside the
+ * workspace. */
+int maml_b200_net_hvp_image(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
+                            const float* xdot, const float* dlogits, const float* v_like, float* jv_out, float* hv_out,
+                            void* stream);
+
+/* Forward mode of the functional operator: the logits tangent J_theta t + J_x xdot at the weights meta_like, for batches of
+ * the handle's SUPPORT shape (N*K images).  Self-contained: one primal forward, then one tangent forward; no backward.
+ *   x, xdot    [n_tasks, N*K, C, H, W]; xdot may be NULL (no image tangent)
+ *   t_like     meta layout: conv / linear tangents and the BatchNorm beta / gamma tangents of num_step; LSLR entries
+ *              are not read
+ *   jv_out     [n_tasks, N*K, N]
+ * No running-statistics side effect; it overwrites the batch statistics maml_b200_net_running_update reads.  Its small
+ * buffers (zero d(logits), the image tangent) are allocated by the first call that needs them, outside the workspace. */
+int maml_b200_net_jvp(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
+                      const float* t_like, const float* xdot, float* jv_out, void* stream);
+
 /* Gradients with respect to the images.  Each reads the buffers of the functional call that ran last on this handle and
  * must follow it immediately, with the same n_tasks: another call on the handle in between (a functional call, an
  * iteration) makes it fail with an error and launch nothing.
