@@ -114,8 +114,8 @@ struct maml_b200_handle {
   int pin_slot = 0;
   long long last_launches = 0;
   int last_tasks = 0;
-  // the functional call (net_forward / net_backward / net_hvp) whose buffers the handle holds; FN_NONE after an
-  // iteration or a call that failed.  The image-gradient entries read those buffers and check this record first.
+  // the functional call (net_forward / net_backward / net_hvp) whose buffers the handle holds; FN_NONE after any other
+  // call that launched, or failed after launching.  The entries that read those buffers check it first (require_call).
   int fn_kind = 0, fn_tasks = 0, fn_step = 0;
   // forward-mode buffers outside the workspace, allocated by the first call that needs them (handles that never see
   // forward mode keep their footprint): the image tangent on the support grid, zero d(logits) for the logits-tangent head
@@ -149,9 +149,25 @@ struct maml_b200_handle {
   bool comm_connected = false;
 };
 
-enum { FN_NONE = 0, FN_FORWARD = 1, FN_BACKWARD = 2, FN_HVP = 3 };
+enum { FN_NONE = 0, FN_FORWARD = 1, FN_BACKWARD = 2, FN_HVP = 4 };     // bits: require_call takes a set of kinds
 static void record_call(maml_b200_handle* h, int kind, int n_tasks, int num_step) {
   h->fn_kind = kind; h->fn_tasks = n_tasks; h->fn_step = num_step;
+}
+static std::string call_names(int kinds) {
+  std::string s;
+  for (int k : {FN_FORWARD, FN_BACKWARD, FN_HVP})
+    if (kinds & k)
+      s += std::string(s.empty() ? "" : " or ") + (k == FN_FORWARD ? "maml_b200_net_forward" : k == FN_BACKWARD ? "maml_b200_net_backward" : "maml_b200_net_hvp");
+  return s;
+}
+// An entry that reads the buffers of an earlier functional call first checks the handle's record of that call: its kind
+// must be one of `kinds`, with the same n_tasks and (num_step >= 0) the same num_step.  Fails without touching the record.
+static int require_call(const maml_b200_handle* h, int kinds, int n_tasks, int num_step, const char* entry) {
+  const std::string e(entry), last = call_names(h->fn_kind);
+  if (!(h->fn_kind & kinds)) return fail(e + " must immediately follow " + call_names(kinds) + " on this handle");
+  if (n_tasks != h->fn_tasks) return fail(e + ": n_tasks differs from the preceding " + last);
+  if (num_step >= 0 && num_step != h->fn_step) return fail(e + ": num_step differs from the preceding " + last);
+  return 0;
 }
 
 // launch context of the handle call in progress on this thread (common.cuh); the default one has PDL off
@@ -947,6 +963,36 @@ static void pack_u(maml_b200_handle* h, int T, cudaStream_t st) {
   launch_pack_weights(h->pl, h->u, h->Ppad, h->pack_u, h->pack_task, h->pack_u_plane, T, st);
 }
 
+// Forks the pre-stream of a tangent pass off `st` and packs u there (first needed by block 1 of the tangent forward, while
+// the main chain runs block 0).  With the tensor-core path that is a target stream (idle then), so that the u-weight convs
+// pre-computed there too do not queue in front of the weight gradients on the wgrad stream.
+static int fork_direction(maml_b200_handle* h, int T, cudaStream_t st, cudaStream_t* spre) {
+  *spre = h->use_tc ? h->s_tgt : h->s_wg;
+  CK(cudaEventRecord(h->ev_fork, st));
+  CK(cudaStreamWaitEvent(*spre, h->ev_fork, 0));
+  pack_u(h, T, *spre);
+  CK(cudaEventRecord(h->ev_wg, *spre));
+  h->wg_pending = true;
+  return 0;
+}
+
+// Export of a functional call: a plain sum over the n_tasks batches (tasks_global 1, no 1/B) into `result`, no target
+// losses.  The fused iteration sets its schedule on top.
+static ExportArgs export_args(const maml_b200_handle* h, int T, float* result) {
+  ExportArgs e{};
+  e.pl = h->pl;
+  e.tbar = h->tbar; e.task_stride = h->Ppad;
+  e.abar = h->abar;
+  e.stats = h->stats; e.stats_task_stride = h->stats_task_stride; e.st_pass_stride = h->st_pass_stride; e.st_layer_stride = h->st_layer_stride;
+  e.losses = h->losses; e.correct = h->correct;
+  e.target_mask = 0; e.num_steps = h->S; e.training = 1;
+  e.tasks = T; e.task_offset = 0; e.tasks_global = 1;
+  e.n_s = h->n_s; e.n_t = h->n_t;
+  for (int l = 0; l < h->L; ++l) e.hw[l] = h->geo[l].h * h->geo[l].w;
+  e.result = result;
+  return e;
+}
+
 // enqueue one whole iteration; `st` is either the caller's stream (eager / profiling) or the capture stream
 static int enqueue_iteration(maml_b200_handle* h, const maml_b200_iter_args* it, const float* meta, const float* x_support,
                              const long long* ys, const float* x_target, const long long* yt, float* result, float* last_logits,
@@ -1062,16 +1108,8 @@ static int enqueue_iteration(maml_b200_handle* h, const maml_b200_iter_args* it,
       join_pending(h, st);                               // g^s / tbar parts reduced on the side stream
       launch_dots_u(h->pl, h->tbar, tg, h->g + (long long)s * TP, h->u, h->abar, meta, s, h->Ppad, T, st);
       if (it->second_order) {
-        // the tensor-core packs of u are first needed by block 1 of the tangent forward: pack on the side stream
-        // while the main chain runs block 0
-        // ... on a target stream (idle in phase B) when the u-weight convs are pre-computed there too, so that they do
-        // not queue in front of the weight gradients on the wgrad stream
-        cudaStream_t spre = h->use_tc ? h->s_tgt : h->s_wg;
-        CK(cudaEventRecord(h->ev_fork, st));
-        CK(cudaStreamWaitEvent(spre, h->ev_fork, 0));
-        pack_u(h, T, spre);
-        CK(cudaEventRecord(h->ev_wg, spre));
-        h->wg_pending = true;
+        cudaStream_t spre;
+        if (fork_direction(h, T, st, &spre)) return 1;
         ReduceSpec rs{PR_SUB, nullptr, nullptr, nullptr, h->tbar, s, -1};
         tangent_pass(h, s, th, h->u, meta, TangentHead{HEAD_TANGENT, ys, nullptr, nullptr, PASS_TAN_BWD}, T, st, rs, spre);
       }
@@ -1082,18 +1120,10 @@ static int enqueue_iteration(maml_b200_handle* h, const maml_b200_iter_args* it,
     for (int s = 0; s < it->num_steps; ++s) if (mask & (1u << s)) CK(cudaStreamWaitEvent(st, h->ev_tgt[s], 0));
   }
 
-  ExportArgs e{};
-  e.pl = h->pl;
-  e.tbar = h->tbar; e.task_stride = h->Ppad;
-  e.abar = h->abar;
-  e.stats = h->stats; e.stats_task_stride = h->stats_task_stride; e.st_pass_stride = h->st_pass_stride; e.st_layer_stride = h->st_layer_stride;
-  e.losses = h->losses; e.correct = h->correct;
+  ExportArgs e = export_args(h, T, result);
   for (int s = 0; s < MAML_MAX_STEPS; ++s) e.weights[s] = it->target_weight[s];
   e.target_mask = mask; e.num_steps = it->num_steps; e.training = it->training;
-  e.tasks = T; e.task_offset = it->task_offset; e.tasks_global = it->tasks_global;
-  e.n_s = h->n_s; e.n_t = h->n_t;
-  for (int l = 0; l < h->L; ++l) e.hw[l] = h->geo[l].h * h->geo[l].w;
-  e.result = result;
+  e.task_offset = it->task_offset; e.tasks_global = it->tasks_global;
   // sharded call with a connected communicator: export publishes into the peer-visible slot and the all-reduce kernel
   // (same stream, same captured graph) leaves the SUM over ranks in `result` -- no host round trip, no library call
   const bool reduce = h->comm_connected && it->tasks_global > it->n_tasks;
@@ -1162,15 +1192,56 @@ extern "C" int maml_b200_meta_batch_fwd_bwd(maml_b200_handle* h, const maml_b200
   return 0;
 }
 
+// Argument checks of the functional entries; `ptrs`: the entry's required pointers are all non-null.
+static int check_call(const maml_b200_handle* h, bool ptrs, int n_tasks, int num_step) {
+  if (!h || !ptrs) return fail("null argument");
+  if (n_tasks < 1 || n_tasks > h->maxT) return fail("n_tasks out of range");
+  if (num_step < 0 || num_step >= h->S) return fail("num_step out of range");
+  return 0;
+}
+
+// Stages a functional call's batch and runs its primal forward on pass set `ps` at `slot`: x (and the image tangent xdot,
+// support grid only) onto the block-0 grid, meta_like into theta slot `slot` (and dir_like into u), the tensor-core packs
+// of that slot, then the forward with the BatchNorm gamma / beta of num_step.  Returns the theta slot.
+static const float* stage_forward(maml_b200_handle* h, const PassSet& ps, int slot, int stat_kind, int num_step, const float* meta_like,
+                                  const float* x, const float* xdot, const float* dir_like, int T, cudaStream_t st) {
+  float* th = h->theta + (long long)slot * h->maxT * h->Ppad;
+  launch_prep_x(x, ps.xg, ps.xg_stride, T, ps.n, h->C, h->H, h->W, st);
+  if (xdot) launch_prep_x(xdot, h->xdot_g, ps.xg_stride, T, ps.n, h->C, h->H, h->W, st);
+  launch_import_theta(h->pl, meta_like, th, h->Ppad, T, st);
+  if (dir_like) launch_import_theta(h->pl, dir_like, h->u, h->Ppad, T, st);
+  pack_theta_step(h, slot, T, st);
+  forward_pass(h, ps, slot, th, slot, meta_like, num_step, stat_kind, T, st);
+  return th;
+}
+
+// Backward of an external d(logits) [T][ps.n][N] through pass set `ps` at `slot` (theta slot `slot`, BatchNorm gamma / beta
+// of num_step): the HEAD_EXTERNAL_BWD head, then backward_pass into the weight-gradient chunks `partial`.
+static void external_backward(maml_b200_handle* h, const PassSet& ps, int slot, int num_step, int kind_fwd, int kind_bwd,
+                              const float* meta_like, const float* dlogits, float* partial, const ChunkPlan& cp, int T, cudaStream_t st) {
+  const float* th = h->theta + (long long)slot * h->maxT * h->Ppad;
+  HeadArgs a{};
+  a.mode = HEAD_EXTERNAL_BWD; a.n = ps.n; a.N = h->N; a.D = h->D; a.scale = 1.f;
+  a.f = AIN(ps, h->L, slot); a.f_stride = STRIDE(ps, ain, h->L);
+  a.Wfc = th + h->pl.fcw_off; a.bfc = th + h->pl.fcb_off; a.theta_stride = h->Ppad;
+  a.y = h->zero_labels; a.y_stride = 0;
+  a.dl_ext = dlogits; a.dl_ext_stride = (long long)ps.n * h->N;
+  a.gW = partial + cp.pd.off[2 * h->L]; a.gb = partial + cp.pd.off[2 * h->L + 1];
+  a.g_stride = cp.pd.task_stride; a.g_chunk_stride = cp.pd.cstride[2 * h->L];
+  a.rows_per_cta = head_rows(a.n);
+  a.df = DP(ps, h->L - 1, slot); a.df_stride = STRIDE(ps, dp, h->L - 1);
+  a.tasks = T;
+  launch_head(a, st);
+  backward_pass(h, ps, slot, th, slot, meta_like, num_step, kind_fwd, kind_bwd, partial, cp, T, st, false);
+}
+
 // Stand-alone functional forward (level B1 of the boundary): logits of `n_tasks` independent batches of N*T images
 // under externally supplied weights.  `meta_like` has the layout of the meta vector (conv / linear entries = the
 // weights to use, BatchNorm entries = gamma / beta; LSLR entries ignored).  BatchNorm uses batch statistics and the
 // gamma / beta of `num_step`, exactly like reference VGGReLUNormNetwork.forward (training flag is ignored there too).
 extern "C" int maml_b200_net_forward(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
                                     const float* x, float* logits, void* stream) {
-  if (!h || !meta_like || !x || !logits) return fail("null argument");
-  if (n_tasks < 1 || n_tasks > h->maxT) return fail("n_tasks out of range");
-  if (num_step < 0 || num_step >= h->S) return fail("num_step out of range");
+  if (check_call(h, meta_like && x && logits, n_tasks, num_step)) return 1;
   cudaStream_t st = (cudaStream_t)stream;
   LaunchScope launch_scope(h, st);
   const int T = n_tasks;
@@ -1178,10 +1249,7 @@ extern "C" int maml_b200_net_forward(maml_b200_handle* h, int32_t n_tasks, int32
   CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
   CK(cudaMemsetAsync(h->losses, 0, (size_t)h->maxT * MAML_MAX_STEPS * sizeof(float), st));
   CK(cudaMemsetAsync(h->correct, 0, (size_t)h->maxT * sizeof(float), st));
-  launch_prep_x(x, h->tgt.xg, h->tgt.xg_stride, T, h->n_t, h->C, h->H, h->W, st);
-  launch_import_theta(h->pl, meta_like, h->theta, h->Ppad, T, st);
-  pack_theta_step(h, 0, T, st);
-  forward_pass(h, h->tgt, 0, h->theta, 0, meta_like, num_step, PASS_TGT_FWD, T, st);
+  stage_forward(h, h->tgt, 0, PASS_TGT_FWD, num_step, meta_like, x, nullptr, nullptr, T, st);
   HeadArgs a{};
   a.mode = HEAD_TARGET_FWD; a.n = h->n_t; a.N = h->N; a.D = h->D; a.scale = 1.f;
   a.f = AIN(h->tgt, h->L, 0); a.f_stride = STRIDE(h->tgt, ain, h->L);
@@ -1198,15 +1266,15 @@ extern "C" int maml_b200_net_forward(maml_b200_handle* h, int32_t n_tasks, int32
 
 // Backward of the functional forward above (level B1: lets torch.autograd differentiate through the operator, the way the
 // reference's apply_inner_loop_update does with torch.autograd.grad, few_shot_learning_system.py:138-139, first order).
-// Must follow maml_b200_net_forward on the same handle with the same (n_tasks, num_step, meta_like): the activations of
-// that call are what this one differentiates.  dlogits [n_tasks, N*T, N] = d(loss)/d(logits).  grad_out: result_size
-// floats; the first meta_size hold d(loss)/d(meta_like) in the meta layout (conv / linear weights and biases, BatchNorm
-// beta / gamma of `num_step`; LSLR entries 0), summed over the n_tasks batches.  No gradient w.r.t. the images.
+// Must follow maml_b200_net_forward (or another net_backward of it) on the same handle with the same (n_tasks, num_step,
+// meta_like): the activations of that call are what this one differentiates.  The handle's call record refuses another
+// order, n_tasks or num_step (meta_like it cannot check).  dlogits [n_tasks, N*T, N] = d(loss)/d(logits).  grad_out:
+// result_size floats; the first meta_size hold d(loss)/d(meta_like) in the meta layout (conv / linear weights and biases,
+// BatchNorm beta / gamma of `num_step`; LSLR entries 0), summed over the n_tasks batches.  No gradient w.r.t. the images.
 extern "C" int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
                                      const float* dlogits, float* grad_out, void* stream) {
-  if (!h || !meta_like || !dlogits || !grad_out) return fail("null argument");
-  if (n_tasks < 1 || n_tasks > h->maxT) return fail("n_tasks out of range");
-  if (num_step < 0 || num_step >= h->S) return fail("num_step out of range");
+  if (check_call(h, meta_like && dlogits && grad_out, n_tasks, num_step)) return 1;
+  if (require_call(h, FN_FORWARD | FN_BACKWARD, n_tasks, num_step, "maml_b200_net_backward")) return 1;
   cudaStream_t st = (cudaStream_t)stream;
   LaunchScope launch_scope(h, st);
   const int T = n_tasks;
@@ -1218,33 +1286,10 @@ extern "C" int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int3
   CK(cudaMemsetAsync(h->abar, 0, (size_t)h->maxT * h->pl.nseg_inner * MAML_MAX_STEPS * sizeof(double), st));
   CK(cudaMemsetAsync(h->losses, 0, (size_t)h->maxT * MAML_MAX_STEPS * sizeof(float), st));
   CK(cudaMemsetAsync(h->correct, 0, (size_t)h->maxT * sizeof(float), st));
-  float* tpart = h->tgt_partial;
-  HeadArgs a{};
-  a.mode = HEAD_EXTERNAL_BWD; a.n = h->n_t; a.N = h->N; a.D = h->D; a.scale = 1.f;
-  a.f = AIN(h->tgt, h->L, 0); a.f_stride = STRIDE(h->tgt, ain, h->L);
-  a.Wfc = h->theta + h->pl.fcw_off; a.bfc = h->theta + h->pl.fcb_off; a.theta_stride = h->Ppad;
-  a.y = h->zero_labels; a.y_stride = 0;
-  a.dl_ext = dlogits; a.dl_ext_stride = (long long)h->n_t * h->N;
-  a.gW = tpart + h->plan_tgt.pd.off[2 * h->L]; a.gb = tpart + h->plan_tgt.pd.off[2 * h->L + 1];
-  a.g_stride = h->plan_tgt.pd.task_stride; a.g_chunk_stride = h->plan_tgt.pd.cstride[2 * h->L];
-  a.rows_per_cta = head_rows(a.n);
-  a.df = DP(h->tgt, h->L - 1, 0); a.df_stride = STRIDE(h->tgt, dp, h->L - 1);
-  a.tasks = T;
-  launch_head(a, st);
-  backward_pass(h, h->tgt, 0, h->theta, 0, meta_like, num_step, PASS_TGT_FWD, PASS_TGT_BWD, tpart, h->plan_tgt, T, st, false);
-  launch_param_reduce(h->pl, h->plan_tgt.pd, tpart, PR_STORE, nullptr, nullptr, h->tbar, nullptr, meta_like, num_step, h->Ppad, T, st);
-  ExportArgs e{};
-  e.pl = h->pl;
-  e.tbar = h->tbar; e.task_stride = h->Ppad;
-  e.abar = h->abar;
-  e.stats = h->stats; e.stats_task_stride = h->stats_task_stride; e.st_pass_stride = h->st_pass_stride; e.st_layer_stride = h->st_layer_stride;
-  e.losses = h->losses; e.correct = h->correct;
-  e.target_mask = 0; e.num_steps = h->S; e.training = 1;
-  e.tasks = T; e.task_offset = 0; e.tasks_global = 1;            // plain sum over the batches, no 1/B
-  e.n_s = h->n_s; e.n_t = h->n_t;
-  for (int l = 0; l < h->L; ++l) e.hw[l] = h->geo[l].h * h->geo[l].w;
-  e.result = grad_out;
-  launch_export(e, st);
+  external_backward(h, h->tgt, 0, num_step, PASS_TGT_FWD, PASS_TGT_BWD, meta_like, dlogits, h->tgt_partial, h->plan_tgt, T, st);
+  launch_param_reduce(h->pl, h->plan_tgt.pd, h->tgt_partial, PR_STORE, nullptr, nullptr, h->tbar, nullptr, meta_like, num_step,
+                      h->Ppad, T, st);
+  launch_export(export_args(h, T, grad_out), st);
   CK(cudaGetLastError());
   record_call(h, FN_BACKWARD, T, num_step);
   return 0;
@@ -1282,61 +1327,26 @@ static int ensure_xdot(maml_b200_handle* h, cudaStream_t st) {
 // statistics maml_b200_net_running_update reads; no running-statistics side effect of its own.
 static int net_hvp_impl(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
                         const float* xdot, const float* dlogits, const float* v_like, float* jv_out, float* hv_out, void* stream) {
-  if (!h || !meta_like || !x || !dlogits || !v_like || !jv_out || !hv_out) return fail("null argument");
-  if (n_tasks < 1 || n_tasks > h->maxT) return fail("n_tasks out of range");
-  if (num_step < 0 || num_step >= h->S) return fail("num_step out of range");
+  if (check_call(h, meta_like && x && dlogits && v_like && jv_out && hv_out, n_tasks, num_step)) return 1;
   cudaStream_t st = (cudaStream_t)stream;
   LaunchScope launch_scope(h, st);
   const int T = n_tasks, s = num_step;
-  float* th = h->theta + (long long)s * h->maxT * h->Ppad;
   record_call(h, FN_NONE, 0, 0);                 // at num_step 0 this overwrites the weights net_forward imported
   if (xdot && ensure_xdot(h, st)) return 1;
   CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
   CK(cudaMemsetAsync(h->abar, 0, (size_t)h->maxT * h->pl.nseg_inner * MAML_MAX_STEPS * sizeof(double), st));
   CK(cudaMemsetAsync(h->losses, 0, (size_t)h->maxT * MAML_MAX_STEPS * sizeof(float), st));
   CK(cudaMemsetAsync(h->correct, 0, (size_t)h->maxT * sizeof(float), st));
-  launch_prep_x(x, h->sup.xg, h->sup.xg_stride, T, h->n_s, h->C, h->H, h->W, st);
-  if (xdot) launch_prep_x(xdot, h->xdot_g, h->sup.xg_stride, T, h->n_s, h->C, h->H, h->W, st);
-  launch_import_theta(h->pl, meta_like, th, h->Ppad, T, st);
-  launch_import_theta(h->pl, v_like, h->u, h->Ppad, T, st);
-  pack_theta_step(h, s, T, st);
-  forward_pass(h, h->sup, s, th, s, meta_like, s, PASS_SUP_FWD, T, st);
-  HeadArgs a{};
-  a.mode = HEAD_EXTERNAL_BWD; a.n = h->n_s; a.N = h->N; a.D = h->D; a.scale = 1.f;
-  a.f = AIN(h->sup, h->L, s); a.f_stride = STRIDE(h->sup, ain, h->L);
-  a.Wfc = th + h->pl.fcw_off; a.bfc = th + h->pl.fcb_off; a.theta_stride = h->Ppad;
-  a.y = h->zero_labels; a.y_stride = 0;
-  a.dl_ext = dlogits; a.dl_ext_stride = (long long)h->n_s * h->N;
-  a.gW = h->sup_partial + h->plan_sup.pd.off[2 * h->L]; a.gb = h->sup_partial + h->plan_sup.pd.off[2 * h->L + 1];
-  a.g_stride = h->plan_sup.pd.task_stride; a.g_chunk_stride = h->plan_sup.pd.cstride[2 * h->L];
-  a.rows_per_cta = head_rows(a.n);
-  a.df = DP(h->sup, h->L - 1, s); a.df_stride = STRIDE(h->sup, dp, h->L - 1);
-  a.tasks = T;
-  launch_head(a, st);
+  const float* th = stage_forward(h, h->sup, s, PASS_SUP_FWD, s, meta_like, x, xdot, v_like, T, st);
   // the tangent pass reads this backward's dz / dp and statistics; its weight-gradient chunks are overwritten unread
-  backward_pass(h, h->sup, s, th, s, meta_like, s, PASS_SUP_FWD, PASS_SUP_BWD, h->sup_partial, h->plan_sup, T, st, false);
-  cudaStream_t spre = h->use_tc ? h->s_tgt : h->s_wg;     // as in the fused reverse sweep
-  CK(cudaEventRecord(h->ev_fork, st));
-  CK(cudaStreamWaitEvent(spre, h->ev_fork, 0));
-  pack_u(h, T, spre);
-  CK(cudaEventRecord(h->ev_wg, spre));
-  h->wg_pending = true;
+  external_backward(h, h->sup, s, s, PASS_SUP_FWD, PASS_SUP_BWD, meta_like, dlogits, h->sup_partial, h->plan_sup, T, st);
+  cudaStream_t spre;
+  if (fork_direction(h, T, st, &spre)) return 1;
   ReduceSpec rs{PR_STORE, nullptr, nullptr, h->tbar, nullptr, s, -1};
   tangent_pass(h, s, th, h->u, meta_like, TangentHead{HEAD_EXTERNAL_TAN, nullptr, dlogits, jv_out, PASS_TGT_BWD}, T, st, rs, spre,
                xdot ? h->xdot_g : nullptr);
   join_pending(h, st);
-  ExportArgs e{};
-  e.pl = h->pl;
-  e.tbar = h->tbar; e.task_stride = h->Ppad;
-  e.abar = h->abar;
-  e.stats = h->stats; e.stats_task_stride = h->stats_task_stride; e.st_pass_stride = h->st_pass_stride; e.st_layer_stride = h->st_layer_stride;
-  e.losses = h->losses; e.correct = h->correct;
-  e.target_mask = 0; e.num_steps = h->S; e.training = 1;
-  e.tasks = T; e.task_offset = 0; e.tasks_global = 1;            // plain sum over the batches, no 1/B
-  e.n_s = h->n_s; e.n_t = h->n_t;
-  for (int l = 0; l < h->L; ++l) e.hw[l] = h->geo[l].h * h->geo[l].w;
-  e.result = hv_out;
-  launch_export(e, st);
+  launch_export(export_args(h, T, hv_out), st);
   CK(cudaGetLastError());
   record_call(h, FN_HVP, T, num_step);
   return 0;
@@ -1364,30 +1374,18 @@ extern "C" int maml_b200_net_hvp_image(maml_b200_handle* h, int32_t n_tasks, int
 // Overwrites the batch statistics maml_b200_net_running_update reads; no running-statistics side effect of its own.
 extern "C" int maml_b200_net_jvp(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
                                  const float* t_like, const float* xdot, float* jv_out, void* stream) {
-  if (!h || !meta_like || !x || !t_like || !jv_out) return fail("null argument");
-  if (n_tasks < 1 || n_tasks > h->maxT) return fail("n_tasks out of range");
-  if (num_step < 0 || num_step >= h->S) return fail("num_step out of range");
+  if (check_call(h, meta_like && x && t_like && jv_out, n_tasks, num_step)) return 1;
   cudaStream_t st = (cudaStream_t)stream;
   LaunchScope launch_scope(h, st);
   const int T = n_tasks, s = num_step;
-  float* th = h->theta + (long long)s * h->maxT * h->Ppad;
   record_call(h, FN_NONE, 0, 0);
   if (xdot && ensure_xdot(h, st)) return 1;
   // zero d(logits) of one batch, read with a task stride of 0
   if (!h->zero_dl && alloc_zeroed(&h->zero_dl, (size_t)h->n_s * h->N * sizeof(float), st)) return 1;
   CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
-  launch_prep_x(x, h->sup.xg, h->sup.xg_stride, T, h->n_s, h->C, h->H, h->W, st);
-  if (xdot) launch_prep_x(xdot, h->xdot_g, h->sup.xg_stride, T, h->n_s, h->C, h->H, h->W, st);
-  launch_import_theta(h->pl, meta_like, th, h->Ppad, T, st);
-  launch_import_theta(h->pl, t_like, h->u, h->Ppad, T, st);
-  pack_theta_step(h, s, T, st);
-  forward_pass(h, h->sup, s, th, s, meta_like, s, PASS_SUP_FWD, T, st);
-  cudaStream_t spre = h->use_tc ? h->s_tgt : h->s_wg;
-  CK(cudaEventRecord(h->ev_fork, st));
-  CK(cudaStreamWaitEvent(spre, h->ev_fork, 0));
-  pack_u(h, T, spre);
-  CK(cudaEventRecord(h->ev_wg, spre));
-  h->wg_pending = true;
+  const float* th = stage_forward(h, h->sup, s, PASS_SUP_FWD, s, meta_like, x, xdot, t_like, T, st);
+  cudaStream_t spre;
+  if (fork_direction(h, T, st, &spre)) return 1;
   tangent_forward(h, s, th, h->u, meta_like, xdot ? h->xdot_g : nullptr, t_like, T, st, spre, false, nullptr);
   join_pending(h, st);
   const PassSet& sp = h->sup; const PassSet& tn = h->tan;
@@ -1435,8 +1433,7 @@ static int input_grad(maml_b200_handle* h, int n_tasks, const Slot* D, const flo
 // output gradient of that backward (target pass, theta slot 0 as imported by net_forward).
 extern "C" int maml_b200_net_input_grad(maml_b200_handle* h, int32_t n_tasks, float* dx_out, void* stream) {
   if (!h || !dx_out) return fail("null argument");
-  if (h->fn_kind != FN_BACKWARD) return fail("maml_b200_net_input_grad must immediately follow maml_b200_net_backward on this handle");
-  if (n_tasks != h->fn_tasks) return fail("maml_b200_net_input_grad: n_tasks differs from the preceding maml_b200_net_backward");
+  if (require_call(h, FN_BACKWARD, n_tasks, -1, "maml_b200_net_input_grad")) return 1;
   const Slot D[1] = {{&h->tgt, 0}};
   const float* W[1] = {h->theta + h->pl.w_off[0]};
   return input_grad(h, n_tasks, D, W, 1, dx_out, (cudaStream_t)stream);
@@ -1447,8 +1444,7 @@ extern "C" int maml_b200_net_input_grad(maml_b200_handle* h, int32_t n_tasks, fl
 // (support pass and theta slot num_step of the hvp call, u = v's weights).
 extern "C" int maml_b200_net_hvp_input_grad(maml_b200_handle* h, int32_t n_tasks, float* dxdot_out, void* stream) {
   if (!h || !dxdot_out) return fail("null argument");
-  if (h->fn_kind != FN_HVP) return fail("maml_b200_net_hvp_input_grad must immediately follow maml_b200_net_hvp on this handle");
-  if (n_tasks != h->fn_tasks) return fail("maml_b200_net_hvp_input_grad: n_tasks differs from the preceding maml_b200_net_hvp");
+  if (require_call(h, FN_HVP, n_tasks, -1, "maml_b200_net_hvp_input_grad")) return 1;
   const int s = h->fn_step;
   const Slot D[2] = {{&h->tan, 0}, {&h->sup, s}};
   const float* W[2] = {h->theta + (long long)s * h->maxT * h->Ppad + h->pl.w_off[0], h->u + h->pl.w_off[0]};
@@ -1458,13 +1454,12 @@ extern "C" int maml_b200_net_hvp_input_grad(maml_b200_handle* h, int32_t n_tasks
 // Side effect of the functional forward in the reference: F.batch_norm's EMA update of running_mean / running_var at
 // `num_step` (meta_neural_network_architectures.py:226-247), from the batch statistics of the last maml_b200_net_forward
 // call (one update per batch, in order).  running_mean / running_var: [stages][S][F] device.  No-op for shared BatchNorm
-// (the reference passes running stats = None there).  A maml_b200_net_hvp call on the same handle in between overwrites
-// those statistics: apply the update right after the forward.
+// (the reference passes running stats = None there).  Another functional call on the same handle in between overwrites
+// those statistics (net_backward keeps them): the handle's call record refuses any other order, n_tasks or num_step.
 extern "C" int maml_b200_net_running_update(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, float* running_mean,
                                            float* running_var, void* stream) {
-  if (!h || !running_mean || !running_var) return fail("null argument");
-  if (n_tasks < 1 || n_tasks > h->maxT) return fail("n_tasks out of range");
-  if (num_step < 0 || num_step >= h->S) return fail("num_step out of range");
+  if (check_call(h, running_mean && running_var, n_tasks, num_step)) return 1;
+  if (require_call(h, FN_FORWARD | FN_BACKWARD, n_tasks, num_step, "maml_b200_net_running_update")) return 1;
   if (!h->cfg.per_step_bn) return 0;
   LaunchScope launch_scope(h);
   int hw[MAML_MAX_LAYERS];

@@ -123,46 +123,13 @@ class VGGReLUNormNetwork(nn.Module):
             out.append(fast.get(n, own[n]))
         return out
 
-    def _operator_engine(self, x):
-        """(engine, meta-layout scratch, logits out, gradient out, running-stat scratch) for this batch shape."""
-        from . import _native
-        n, N = int(x.shape[0]), self.num_output_classes
-        key = (n, x.device.index)
-        cache = self.__dict__.setdefault("_engines", {})
+    def _handles(self, x):
+        """The operator's engine handles for x's batch size and device (``_OperatorHandles``), created on first use."""
+        cache = self.__dict__.setdefault("_operator_handles", {})
+        key = (int(x.shape[0]), x.device.index)
         if key not in cache:
-            a = self.args
-            with torch.cuda.device(x.device):
-                eng = _native.Engine(n_way=N, k_shot=1, t_target=n // N, channels=int(x.shape[1]), height=int(x.shape[2]),
-                                     width=int(x.shape[3]), filters=self.cnn_filters, num_stages=self.num_stages,
-                                     inner_steps=int(a.number_of_training_steps_per_iter),
-                                     per_step_bn=bool(a.per_step_bn_statistics), max_tasks=1)
-            S = int(a.number_of_training_steps_per_iter) if a.per_step_bn_statistics else 1
-            cache[key] = {"eng": eng, "gen": 0,
-                          "meta": torch.zeros(eng.meta_size, dtype=torch.float32, device=x.device),
-                          "logits": torch.empty(1, n, N, dtype=torch.float32, device=x.device),
-                          "grad": torch.zeros(eng.result_size, dtype=torch.float32, device=x.device),
-                          "run": torch.zeros(2, self.num_stages, S, self.cnn_filters, dtype=torch.float32, device=x.device)}
+            cache[key] = _OperatorHandles(self, x)
         return cache[key]
-
-    def _hvp_engine(self, x):
-        """Engine of ``maml_b200_net_hvp`` for this batch shape, created on the first double backward: a second handle whose
-        SUPPORT buffers (those the tangent pass runs on) hold the batch, so the operator's first-order handle and its
-        users pay nothing for them."""
-        from . import _native
-        st = self._operator_engine(x)
-        if "hvp" not in st:
-            a, n, N = self.args, int(x.shape[0]), self.num_output_classes
-            with torch.cuda.device(x.device):
-                eng = _native.Engine(n_way=N, k_shot=n // N, t_target=1, channels=int(x.shape[1]), height=int(x.shape[2]),
-                                     width=int(x.shape[3]), filters=self.cnn_filters, num_stages=self.num_stages,
-                                     inner_steps=int(a.number_of_training_steps_per_iter),
-                                     per_step_bn=bool(a.per_step_bn_statistics), max_tasks=1)
-            st["hvp"] = {"eng": eng,
-                         "meta": torch.zeros(eng.meta_size, dtype=torch.float32, device=x.device),
-                         "v": torch.zeros(eng.meta_size, dtype=torch.float32, device=x.device),
-                         "jv": torch.empty(1, n, N, dtype=torch.float32, device=x.device),
-                         "hv": torch.zeros(eng.result_size, dtype=torch.float32, device=x.device)}
-        return st["hvp"]
 
     def forward(self, x, num_step, params=None, training=False, backup_running_statistics=False):
         """Logits of a batch under externally supplied ("fast") weights -- reference
@@ -192,21 +159,6 @@ class VGGReLUNormNetwork(nn.Module):
         tensors = self._segment_tensors(params)
         return _FunctionalForward.apply(self, x, int(num_step), *tensors)
 
-    def _apply_running_ema(self, st, num_step):
-        if not self.args.per_step_bn_statistics:
-            return
-        run = st["run"]
-        with torch.no_grad():
-            for l in range(self.num_stages):
-                bn = self.layer_dict["conv%d" % l].norm_layer
-                run[0, l].copy_(bn.running_mean.data)
-                run[1, l].copy_(bn.running_var.data)
-            st["eng"].net_running_update(1, num_step, run[0], run[1])
-            for l in range(self.num_stages):
-                bn = self.layer_dict["conv%d" % l].norm_layer
-                bn.running_mean.data.copy_(run[0, l])
-                bn.running_var.data.copy_(run[1, l])
-
     def zero_grad(self, params=None):
         """Reference :662-677: clears the gradients of ``params`` (or of the module's own parameters)."""
         if params is None:
@@ -224,6 +176,140 @@ class VGGReLUNormNetwork(nn.Module):
         return None
 
 
+def _f32(t):
+    """What the engine reads of a tensor: its values, float32, contiguous."""
+    return t.detach().to(torch.float32).contiguous()
+
+
+def _fill(eng, meta_like, tensors, v_like=None, directions=None):
+    """meta_like <- the tensors and, with v_like, v_like <- the directions (None: zero) in the engine's meta layout."""
+    with torch.no_grad():
+        if v_like is not None:
+            v_like.zero_()
+        for (off, size), t, d in zip(eng.segments, tensors, directions or [None] * len(tensors)):
+            meta_like[off:off + size].copy_(t.detach().reshape(-1).to(torch.float32))
+            if d is not None:
+                v_like[off:off + size].copy_(d.detach().reshape(-1).to(torch.float32))
+
+
+def _unpack(eng, buf, tensors, needs, cast=False):
+    """A meta-layout buffer cut into per-tensor copies (None where not needed), in each tensor's dtype when `cast`."""
+    return [buf[off:off + size].view(t.shape).to(t.dtype if cast else buf.dtype, copy=True) if need else None
+            for (off, size), t, need in zip(eng.segments, tensors, needs)]
+
+
+def _image_buffer(buf, x):
+    """`buf`, or on first use an engine output buffer for the image gradient of x (one batch)."""
+    return buf if buf is not None else torch.empty((1,) + tuple(x.shape), dtype=torch.float32, device=x.device)
+
+
+def _add(a, b):
+    return a if b is None else b if a is None else a + b
+
+
+class _OperatorHandles:
+    """The engine handles behind ``VGGReLUNormNetwork.forward`` for one batch size on one device, one method per use.
+
+    The first-order handle holds the batch as its target pass (``maml_b200_net_forward`` / ``net_backward`` /
+    ``net_input_grad``, the running-statistics update).  It keeps the activations of its LAST forward only: ``gen`` counts
+    its forwards, so that a backward of an older forward replays it first.  The second-order handle, created on first use,
+    holds the batch as its SUPPORT pass, the buffers the tangent pass runs on (``net_hvp_image`` /
+    ``net_hvp_input_grad`` / ``net_jvp``): a model that is only differentiated once pays nothing for it."""
+
+    def __init__(self, net, x):
+        a = net.args
+        self.n, self.N, self.device = int(x.shape[0]), net.num_output_classes, x.device
+        self.cfg = dict(n_way=self.N, channels=int(x.shape[1]), height=int(x.shape[2]), width=int(x.shape[3]),
+                        filters=net.cnn_filters, num_stages=net.num_stages, inner_steps=int(a.number_of_training_steps_per_iter),
+                        per_step_bn=bool(a.per_step_bn_statistics), max_tasks=1)
+        self.first_order = eng = self._engine(k_shot=1, t_target=self.n // self.N)
+        self.gen = 0
+        self.meta = torch.zeros(eng.meta_size, dtype=torch.float32, device=self.device)
+        self.logits = torch.empty(1, self.n, self.N, dtype=torch.float32, device=self.device)
+        self.grad = torch.zeros(eng.result_size, dtype=torch.float32, device=self.device)
+        S = int(a.number_of_training_steps_per_iter) if a.per_step_bn_statistics else 1
+        self.run = torch.zeros(2, net.num_stages, S, net.cnn_filters, dtype=torch.float32, device=self.device)
+        self.dx = self.second_order = self.dxdot = None
+
+    def _engine(self, **shape):
+        from . import _native
+        with torch.cuda.device(self.device):
+            return _native.Engine(**shape, **self.cfg)
+
+    def _second(self):
+        if self.second_order is None:
+            eng = self._engine(k_shot=self.n // self.N, t_target=1)
+            self.meta2 = torch.zeros(eng.meta_size, dtype=torch.float32, device=self.device)
+            self.v = torch.zeros(eng.meta_size, dtype=torch.float32, device=self.device)
+            self.jv = torch.empty(1, self.n, self.N, dtype=torch.float32, device=self.device)
+            self.hv = torch.zeros(eng.result_size, dtype=torch.float32, device=self.device)
+            self.second_order = eng
+        return self.second_order
+
+    def forward(self, net, x, num_step, tensors):
+        """The logits (``net_forward``), and F.batch_norm's EMA of net's running statistics at num_step (per-step
+        BatchNorm only)."""
+        eng = self.first_order
+        _fill(eng, self.meta, tensors)
+        with torch.cuda.device(self.device):
+            eng.net_forward(1, num_step, self.meta, _f32(x), self.logits)
+            if net.args.per_step_bn_statistics:
+                bns = [net.layer_dict["conv%d" % l].norm_layer for l in range(net.num_stages)]
+                with torch.no_grad():
+                    for l, bn in enumerate(bns):
+                        self.run[0, l].copy_(bn.running_mean.data)
+                        self.run[1, l].copy_(bn.running_var.data)
+                    eng.net_running_update(1, num_step, self.run[0], self.run[1])
+                    for l, bn in enumerate(bns):
+                        bn.running_mean.data.copy_(self.run[0, l])
+                        bn.running_var.data.copy_(self.run[1, l])
+        self.gen += 1
+        return self.logits[0].clone()
+
+    def backward(self, fwd_ctx, x, tensors, dl):
+        """J^T dl (``net_backward``) at the forward of ``fwd_ctx``, replayed first when another forward of this shape ran
+        since (the replay has no EMA side effect), and J_x^T dl (``net_input_grad``) when x requires grad.  Returns (dx or
+        None, the per-tensor gradients in float32, None where not needed)."""
+        eng, num_step = self.first_order, fwd_ctx.num_step
+        with torch.no_grad(), torch.cuda.device(self.device):
+            if self.gen != fwd_ctx.gen:
+                _fill(eng, self.meta, tensors)
+                eng.net_forward(1, num_step, self.meta, _f32(x), self.logits)
+                self.gen += 1
+                fwd_ctx.gen = self.gen
+            eng.net_backward(1, num_step, self.meta, _f32(dl).view(1, *dl.shape), self.grad)
+            dx = None
+            if fwd_ctx.needs_input_grad[1]:
+                self.dx = _image_buffer(self.dx, x)
+                eng.net_input_grad(1, self.dx)
+                dx = self.dx[0].to(x.dtype, copy=True)
+            return dx, _unpack(eng, self.grad, tensors, fwd_ctx.needs_input_grad[3:])
+
+    def hvp(self, num_step, x, xdot, dlogits, tensors, directions, need_x, needs, cast=False):
+        """Along the weight directions and the image tangent xdot (None: none; then this is ``net_hvp``): J v and
+        d/dtheta <dlogits, J v> (``net_hvp_image``), and d/dx <dlogits, J v> (``net_hvp_input_grad``) when need_x.  Returns
+        (d/dx or None, J v as float32 [n, N], the per-tensor d/dtheta as by ``_unpack(..., needs, cast)``)."""
+        eng = self._second()
+        _fill(eng, self.meta2, tensors, self.v, directions)
+        with torch.cuda.device(self.device):
+            eng.net_hvp_image(1, num_step, self.meta2, _f32(x), None if xdot is None else _f32(xdot),
+                              _f32(dlogits).view(1, *dlogits.shape), self.v, self.jv, self.hv)
+            d_x = None
+            if need_x:
+                self.dxdot = _image_buffer(self.dxdot, x)
+                eng.net_hvp_input_grad(1, self.dxdot)
+                d_x = self.dxdot[0].to(x.dtype, copy=True)
+        return d_x, self.jv[0], _unpack(eng, self.hv, tensors, needs, cast)
+
+    def jvp(self, num_step, x, xdot, tensors, tangents):
+        """The logits tangent J_theta t + J_x xdot (``net_jvp``; xdot may be None)."""
+        eng = self._second()
+        _fill(eng, self.meta2, tensors, self.v, tangents)
+        with torch.cuda.device(self.device):
+            eng.net_jvp(1, num_step, self.meta2, _f32(x), self.v, None if xdot is None else _f32(xdot), self.jv)
+        return self.jv[0].clone()
+
+
 class _FunctionalForward(torch.autograd.Function):
     """``VGGReLUNormNetwork.forward`` as an autograd node: forward = ``maml_b200_net_forward``, backward =
     ``_FunctionalBackward`` (``maml_b200_net_backward``: head backward for an external d(logits), BatchNorm / pool / leaky-ReLU
@@ -233,21 +319,13 @@ class _FunctionalForward(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, net, x, num_step, *tensors):
-        st = net._operator_engine(x)
-        eng, meta_like, logits = st["eng"], st["meta"], st["logits"]
-        xin = x.detach().to(torch.float32).contiguous()
-        with torch.no_grad():
-            for (off, size), t in zip(eng.segments, tensors):
-                meta_like[off:off + size].copy_(t.detach().reshape(-1).to(torch.float32))
-        with torch.cuda.device(x.device):
-            eng.net_forward(1, num_step, meta_like, xin, logits)
-            net._apply_running_ema(st, num_step)
-        st["gen"] += 1
-        ctx.net, ctx.num_step, ctx.gen = net, num_step, st["gen"]
+        ops = net._handles(x)
+        logits = ops.forward(net, x, num_step, tensors)
+        ctx.net, ctx.ops, ctx.num_step, ctx.gen = net, ops, num_step, ops.gen
         # x and the weights themselves: a double backward differentiates w.r.t. them, forward mode at them
         ctx.save_for_backward(x, *tensors)
         ctx.save_for_forward(x, *tensors)
-        return logits[0].clone()
+        return logits
 
     @staticmethod
     def backward(ctx, dlogits):
@@ -265,51 +343,9 @@ class _FunctionalForward(torch.autograd.Function):
     @staticmethod
     def jvp(ctx, _net_t, x_t, _step_t, *tangents):
         """Forward mode (``torch.autograd.forward_ad``): the logits tangent J_theta t + J_x x_t through
-        ``maml_b200_net_jvp`` on the second (HVP) handle -- one primal forward and one tangent forward.  Tangents may sit
+        ``maml_b200_net_jvp`` on the second-order handle -- one primal forward and one tangent forward.  Tangents may sit
         on the images, the conv / linear weights and the BatchNorm gamma / beta."""
-        x, tensors = ctx.saved_tensors[0], ctx.saved_tensors[1:]
-        xin = x.detach().to(torch.float32).contiguous()
-        hs = ctx.net._hvp_engine(xin)
-        eng, meta_like, t_like, jv = hs["eng"], hs["meta"], hs["v"], hs["jv"]
-        _fill_meta(eng, meta_like, tensors, t_like, tangents)
-        xdot = None if x_t is None else x_t.detach().to(torch.float32).contiguous()
-        with torch.cuda.device(xin.device):
-            eng.net_jvp(1, ctx.num_step, meta_like, xin, t_like, xdot, jv)
-        return jv[0].clone()
-
-
-def _fill_meta(eng, meta_like, tensors, v_like, directions):
-    """meta_like <- the tensors, v_like <- the directions (None: zero) in the engine's meta layout."""
-    with torch.no_grad():
-        v_like.zero_()
-        for (off, size), t, d in zip(eng.segments, tensors, directions):
-            meta_like[off:off + size].copy_(t.detach().reshape(-1).to(torch.float32))
-            if d is not None:
-                v_like[off:off + size].copy_(d.detach().reshape(-1).to(torch.float32))
-
-
-def _net_backward(fwd_ctx, xin, tensors, dl, x_dtype):
-    """J^T dl on the operator's handle (``maml_b200_net_backward``), after replaying ``fwd_ctx``'s forward when another
-    forward of this shape ran since (the handle keeps the activations of its last forward only; the replay has no EMA side
-    effect), and J_x^T dl (``maml_b200_net_input_grad``) when x requires grad.  Returns (the handle's state, whose "grad"
-    holds the weight gradients in the meta layout; dx or None)."""
-    net, num_step = fwd_ctx.net, fwd_ctx.num_step
-    st = net._operator_engine(xin)
-    eng, meta_like, logits, grad = st["eng"], st["meta"], st["logits"], st["grad"]
-    with torch.no_grad(), torch.cuda.device(xin.device):
-        if st["gen"] != fwd_ctx.gen:
-            for (off, size), t in zip(eng.segments, tensors):
-                meta_like[off:off + size].copy_(t.detach().reshape(-1).to(torch.float32))
-            eng.net_forward(1, num_step, meta_like, xin, logits)
-            st["gen"] += 1
-            fwd_ctx.gen = st["gen"]
-        eng.net_backward(1, num_step, meta_like, dl.detach().to(torch.float32).contiguous().view(1, *dl.shape), grad)
-        dx = None
-        if fwd_ctx.needs_input_grad[1]:
-            dx = st.setdefault("dx", torch.empty((1,) + tuple(xin.shape), dtype=torch.float32, device=xin.device))
-            eng.net_input_grad(1, dx)
-            dx = dx[0].to(x_dtype, copy=True)
-    return st, dx
+        return ctx.ops.jvp(ctx.num_step, ctx.saved_tensors[0], x_t, ctx.saved_tensors[1:], tangents)
 
 
 class _FunctionalBackward(torch.autograd.Function):
@@ -332,71 +368,44 @@ class _FunctionalBackward(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, fwd_ctx, x, dlogits, *tensors):
-        net, num_step = fwd_ctx.net, fwd_ctx.num_step
-        xin = x.detach().to(torch.float32).contiguous()
-        st, dx = _net_backward(fwd_ctx, xin, tensors, dlogits, x.dtype)
-        eng, grad = st["eng"], st["grad"]
+        dx, grads = fwd_ctx.ops.backward(fwd_ctx, x, tensors, dlogits)
         ctx.set_materialize_grads(False)
-        ctx.net, ctx.num_step, ctx.fwd_ctx = net, num_step, fwd_ctx
+        ctx.fwd_ctx = fwd_ctx
         ctx.save_for_backward(x, dlogits, *tensors)
         ctx.save_for_forward(x, dlogits, *tensors)
-        grads = []
-        for (off, size), t, need in zip(eng.segments, tensors, fwd_ctx.needs_input_grad[3:]):
-            grads.append(grad[off:off + size].view(t.shape).clone() if need else None)
         return (dx,) + tuple(grads)
 
     @staticmethod
     def jvp(ctx, _fwd_ctx_t, x_t, dl_t, *tangents):
         """Forward-over-reverse: the tangent of every gradient this node returned, along (x_t, dl_t, tangents).  For a
         weight gradient J_theta^T dl_t + d/dtheta <dl, J_theta t + J_x x_t>; for dx the same with d/dx.  The first term is
-        ``maml_b200_net_backward`` (+ ``net_input_grad``) of dl_t on the operator's handle, the second
-        ``maml_b200_net_hvp_image`` (+ ``net_hvp_input_grad``) on the HVP handle; a term whose tangents are all None is
-        skipped.  A tangent on a BatchNorm gamma / beta input never gets here: ``_FunctionalForward.backward`` refuses it
-        before this node runs."""
-        net, num_step, fwd_ctx = ctx.net, ctx.num_step, ctx.fwd_ctx
+        ``maml_b200_net_backward`` (+ ``net_input_grad``) of dl_t on the first-order handle, the second
+        ``maml_b200_net_hvp_image`` (+ ``net_hvp_input_grad``) on the second-order handle; a term whose tangents are all
+        None is skipped.  A tangent on a BatchNorm gamma / beta input never gets here: ``_FunctionalForward.backward``
+        refuses it before this node runs."""
+        fwd_ctx = ctx.fwd_ctx
         x, dlogits, tensors = ctx.saved_tensors[0], ctx.saved_tensors[1], ctx.saved_tensors[2:]
         need_x = fwd_ctx.needs_input_grad[1]
-        needs = fwd_ctx.needs_input_grad[3:]
-        xin = x.detach().to(torch.float32).contiguous()
         dx_t, grads_t = None, [None] * len(tensors)
-
-        def add(acc, v):
-            return v if acc is None else acc + v
-        with torch.cuda.device(xin.device):
-            if dl_t is not None:                              # J^T dl_t on the operator's handle
-                st, dx_t = _net_backward(fwd_ctx, xin, tensors, dl_t, x.dtype)
-                eng, grad = st["eng"], st["grad"]
-                for k, ((off, size), t) in enumerate(zip(eng.segments, tensors)):
-                    if needs[k]:
-                        grads_t[k] = add(grads_t[k], grad[off:off + size].view(t.shape).clone())
-            if x_t is not None or any(t is not None for t in tangents):    # d/d(theta, x) <dl, J_theta t + J_x x_t>
-                hs = net._hvp_engine(xin)
-                eng, meta_like, v_like, jv, hv = hs["eng"], hs["meta"], hs["v"], hs["jv"], hs["hv"]
-                _fill_meta(eng, meta_like, tensors, v_like, tangents)
-                xdot = None if x_t is None else x_t.detach().to(torch.float32).contiguous()
-                eng.net_hvp_image(1, num_step, meta_like, xin, xdot,
-                                  dlogits.detach().to(torch.float32).contiguous().view(1, *dlogits.shape), v_like, jv, hv)
-                if need_x:
-                    dxdot = hs.setdefault("dxdot", torch.empty((1,) + tuple(xin.shape), dtype=torch.float32, device=xin.device))
-                    eng.net_hvp_input_grad(1, dxdot)
-                    dx_t = add(dx_t, dxdot[0].to(x.dtype, copy=True))
-                for k, ((off, size), t) in enumerate(zip(eng.segments, tensors)):
-                    if needs[k]:
-                        grads_t[k] = add(grads_t[k], hv[off:off + size].view(t.shape).clone())
+        if dl_t is not None:                              # J^T dl_t on the first-order handle
+            dx_t, grads_t = fwd_ctx.ops.backward(fwd_ctx, x, tensors, dl_t)
+        if x_t is not None or any(t is not None for t in tangents):    # d/d(theta, x) <dl, J_theta t + J_x x_t>
+            d_x, _, hv = fwd_ctx.ops.hvp(fwd_ctx.num_step, x, x_t, dlogits, tensors, tangents, need_x,
+                                         fwd_ctx.needs_input_grad[3:])
+            dx_t = _add(dx_t, d_x)
+            grads_t = [_add(g, h) for g, h in zip(grads_t, hv)]
         return (dx_t if need_x else None,) + tuple(grads_t)
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, dx_cotangent, *cotangents):
-        net, num_step = ctx.net, ctx.num_step
+        fwd_ctx = ctx.fwd_ctx
         x, dlogits, tensors = ctx.saved_tensors[0], ctx.saved_tensors[1], ctx.saved_tensors[2:]
         if dx_cotangent is not None:
             raise NotImplementedError(
                 "differentiating through the gradient with respect to the images needs image tangent directions, which "
                 "the engine's tangent pass does not implement")
-        xin = x.detach().to(torch.float32).contiguous()
-        n_conv = 4 * net.num_stages
-        for i, c in enumerate(cotangents[:n_conv]):
+        for i, c in enumerate(cotangents[:4 * fwd_ctx.net.num_stages]):
             if c is not None and i % 4 >= 2:
                 raise NotImplementedError(
                     "differentiating through the gradient of a BatchNorm gamma / beta needs gamma / beta tangent "
@@ -404,24 +413,7 @@ class _FunctionalBackward(torch.autograd.Function):
                     "enable_inner_loop_optimizable_bn_params, are outside the accelerated path)")
         if all(c is None for c in cotangents):
             return (None,) * (3 + len(tensors))
-        hs = net._hvp_engine(xin)
-        eng, meta_like, v_like, jv, hv = hs["eng"], hs["meta"], hs["v"], hs["jv"], hs["hv"]
-        with torch.no_grad():
-            v_like.zero_()
-            for (off, size), t, c in zip(eng.segments, tensors, cotangents):
-                meta_like[off:off + size].copy_(t.reshape(-1).to(torch.float32))
-                if c is not None:
-                    v_like[off:off + size].copy_(c.reshape(-1).to(torch.float32))
-        with torch.cuda.device(xin.device):
-            eng.net_hvp(1, num_step, meta_like, xin, dlogits.to(torch.float32).contiguous().view(1, *dlogits.shape), v_like,
-                        jv, hv)
-            d_x = None
-            if ctx.needs_input_grad[1]:
-                dxdot = hs.setdefault("dxdot", torch.empty((1,) + tuple(xin.shape), dtype=torch.float32, device=xin.device))
-                eng.net_hvp_input_grad(1, dxdot)
-                d_x = dxdot[0].to(x.dtype, copy=True)
-        d_dlogits = jv[0].to(dlogits.dtype).clone() if ctx.needs_input_grad[2] else None
-        grads = []
-        for (off, size), t, need in zip(eng.segments, tensors, ctx.needs_input_grad[3:]):
-            grads.append(hv[off:off + size].view(t.shape).to(t.dtype).clone() if need else None)
-        return (None, d_x, d_dlogits) + tuple(grads)
+        d_x, jv, hv = fwd_ctx.ops.hvp(fwd_ctx.num_step, x, None, dlogits, tensors, cotangents, ctx.needs_input_grad[1],
+                                      ctx.needs_input_grad[3:], cast=True)
+        d_dlogits = jv.to(dlogits.dtype).clone() if ctx.needs_input_grad[2] else None
+        return (None, d_x, d_dlogits) + tuple(hv)

@@ -114,7 +114,9 @@ int maml_b200_net_forward(maml_b200_handle* h, int32_t n_tasks, int32_t num_step
 
 /* Backward of maml_b200_net_forward (so that torch.autograd can differentiate through the functional operator, as the
  * reference's apply_inner_loop_update does with torch.autograd.grad, few_shot_learning_system.py:138-139; first order).
- * Must directly follow maml_b200_net_forward on the same handle with the same (n_tasks, num_step, meta_like).
+ * Must directly follow maml_b200_net_forward (or another maml_b200_net_backward of it) on the same handle with the same
+ * (n_tasks, num_step, meta_like).  Another order, n_tasks or num_step makes it fail with an error and launch nothing (the
+ * handle records its last functional call; meta_like it cannot check).
  *   dlogits  [n_tasks, N*T, N]   d(loss) / d(logits)
  *   grad_out [result_size]       (out) first meta_size floats = d(loss) / d(meta_like) in the meta layout (conv / linear
  *                                weights and biases, BatchNorm beta / gamma rows of num_step; LSLR entries 0), summed over
@@ -167,9 +169,11 @@ int maml_b200_net_input_grad(maml_b200_handle* h, int32_t n_tasks, float* dx_out
 int maml_b200_net_hvp_input_grad(maml_b200_handle* h, int32_t n_tasks, float* dxdot_out, void* stream);
 
 /* EMA side effect of the functional forward (F.batch_norm updating running_mean / running_var at num_step, reference
- * meta_neural_network_architectures.py:226-247) from the batch statistics of the last maml_b200_net_forward call, which
- * must not be followed by a maml_b200_net_hvp call on the same handle before this one (apply it right after the forward).
- * running_mean / running_var: [stages][S][F] device.  No-op without per-step BatchNorm. */
+ * meta_neural_network_architectures.py:226-247) from the batch statistics of the last maml_b200_net_forward call.  Like
+ * maml_b200_net_backward it must follow that forward (or a maml_b200_net_backward of it) with the same n_tasks and
+ * num_step, and otherwise fails with an error and launches nothing: another functional call in between, e.g.
+ * maml_b200_net_hvp, overwrites those statistics.  running_mean / running_var: [stages][S][F] device.  No-op without
+ * per-step BatchNorm. */
 int maml_b200_net_running_update(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, float* running_mean,
                                  float* running_var, void* stream);
 

@@ -1,0 +1,57 @@
+"""Test helpers shared by the functional-network operator tests: cases, models, batches and stand-alone engine handles."""
+import torch
+
+from conftest import load_golden
+from oracle import maml_oracle as O
+
+
+def case(name):
+    """(args, fp32 state, batch) of a golden case, or of synthetic_c<C>[_w<W>]: a seeded model with C input channels and
+    W x W images (14 if not given), so that the register-blocked (C0 = 1, 3) and the generic (C0 = 4) first-block kernels
+    all run, at even and odd widths, where no golden case covers them."""
+    if name.startswith("synthetic_c"):
+        from howtotrainyourmamlpytorch_b200 import make_args
+        parts = name.split("_")
+        c = int(parts[1][1:])
+        w = int(parts[2][1:]) if len(parts) > 2 else 14
+        a = make_args("omniglot_mamlpp_5w1s", image_channels=c, image_height=w, image_width=w,
+                      cnn_num_filters=32, num_stages=3, number_of_training_steps_per_iter=2,
+                      number_of_evaluation_steps_per_iter=2, batch_size=2, num_target_samples=3)
+        return a, O.init_state(a), O.synthetic_batch(a, iteration=5, kind="normal")
+    g = load_golden(name)
+    return g.args, g.state(), g.batch(0)
+
+
+def model(a, state, device):
+    from howtotrainyourmamlpytorch_b200 import MAMLFewShotClassifier
+    m = MAMLFewShotClassifier(im_shape=(2, a.image_channels, a.image_height, a.image_width), device=device, args=a)
+    m.load_state_dict(state)
+    return m
+
+
+def images(batch, which, b=0):
+    xs, xt, ys, yt = batch
+    x, y = (xs, ys) if which == "support" else (xt, yt)
+    return x[b].reshape(-1, *x.shape[-3:]).float(), y[b].reshape(-1).long()
+
+
+def bn_names(state):
+    return [k for k in state if k.endswith("norm_layer.weight") or k.endswith("norm_layer.bias")]
+
+
+def engine(a, k_shot, t_target, max_tasks, device):
+    """A stand-alone engine handle for a's network, with batches of N * k_shot support and N * t_target target images."""
+    from howtotrainyourmamlpytorch_b200 import _native
+    with torch.cuda.device(device):
+        return _native.Engine(n_way=int(a.num_classes_per_set), k_shot=k_shot, t_target=t_target, channels=int(a.image_channels),
+                              height=int(a.image_height), width=int(a.image_width), filters=int(a.cnn_num_filters),
+                              num_stages=int(a.num_stages), inner_steps=int(a.number_of_training_steps_per_iter),
+                              per_step_bn=bool(a.per_step_bn_statistics), max_tasks=max_tasks)
+
+
+def meta_like(m, eng, device):
+    """m's own weights in the engine's meta layout."""
+    meta = torch.zeros(eng.meta_size, dtype=torch.float32, device=device)
+    for (off, size), t in zip(eng.segments, m.classifier._segment_tensors(None)):
+        meta[off:off + size] = t.detach().reshape(-1)
+    return meta

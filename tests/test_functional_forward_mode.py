@@ -8,6 +8,7 @@ import torch.nn.functional as Fnn
 
 from conftest import load_golden
 from engine_layout import rel_err
+import functional_cases as fc
 from oracle import maml_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -21,47 +22,13 @@ DIRECTIONS = ["weights", "gamma_beta", "images", "all"]
 B1_REL = 5e-5          # B1 policy (DESIGN.md section 6): 5e-5 of the fp64 reference's max-norm
 
 
-def _case(case):
-    """(args, fp32 state, batch).  synthetic_c<C>[_w<W>]: seeded models with C input channels and W x W images (14 if not
-    given), so that the register-blocked (C0 = 1, 3) and the generic (C0 = 4) first-block kernels all run with an image
-    tangent, at even and odd widths."""
-    if case.startswith("synthetic_c"):
-        from howtotrainyourmamlpytorch_b200 import make_args
-        parts = case.split("_")
-        c = int(parts[1][1:])
-        w = int(parts[2][1:]) if len(parts) > 2 else 14
-        a = make_args("omniglot_mamlpp_5w1s", image_channels=c, image_height=w, image_width=w,
-                      cnn_num_filters=32, num_stages=3, number_of_training_steps_per_iter=2,
-                      number_of_evaluation_steps_per_iter=2, batch_size=2, num_target_samples=3)
-        return a, O.init_state(a), O.synthetic_batch(a, iteration=5, kind="normal")
-    g = load_golden(case)
-    return g.args, g.state(), g.batch(0)
-
-
-def _model(a, state, device):
-    from howtotrainyourmamlpytorch_b200 import MAMLFewShotClassifier
-    m = MAMLFewShotClassifier(im_shape=(2, a.image_channels, a.image_height, a.image_width), device=device, args=a)
-    m.load_state_dict(state)
-    return m
-
-
-def _images(batch, which, b=0):
-    xs, xt, ys, yt = batch
-    x, y = (xs, ys) if which == "support" else (xt, yt)
-    return x[b].reshape(-1, *x.shape[-3:]).float(), y[b].reshape(-1).long()
-
-
-def _bn_names(state):
-    return [k for k in state if k.endswith("norm_layer.weight") or k.endswith("norm_layer.bias")]
-
-
 def _tangents(a, state, x, direction, seed=7):
     """(weight tangents, gamma / beta tangents, image tangent) in fp64 on the CPU; the parts `direction` leaves out are {} /
     None."""
     gen = torch.Generator().manual_seed(seed)
     rnd = lambda t: torch.randn(t.shape, generator=gen, dtype=torch.float64)   # noqa: E731
     w = {n: rnd(state[n]) for n in O.inner_param_names(a)} if direction in ("weights", "all") else {}
-    gb = {n: rnd(state[n]) for n in _bn_names(state)} if direction in ("gamma_beta", "all") else {}
+    gb = {n: rnd(state[n]) for n in fc.bn_names(state)} if direction in ("gamma_beta", "all") else {}
     xd = rnd(x) if direction in ("images", "all") else None
     return w, gb, xd
 
@@ -69,7 +36,7 @@ def _tangents(a, state, x, direction, seed=7):
 def _oracle_jt(a, state, x, step, w, gb, xd, device, dtype=torch.float64):
     """J t through the oracle network with torch.func.jvp."""
     st = {k: t.to(device, dtype) for k, t in state.items()}
-    inner, bn = O.inner_param_names(a), _bn_names(state)
+    inner, bn = O.inner_param_names(a), fc.bn_names(state)
 
     def f(x_, fast, bnp):
         return O._net_forward(x_, fast, {**st, **bnp}, a, step)
@@ -88,7 +55,7 @@ def _op_jt(m, a, x, step, w, gb, xd, device):
         for n in O.inner_param_names(a):
             p = named[n].detach().clone().unsqueeze(0)
             params[n[len(PREFIX):]] = fwAD.make_dual(p, w[n].to(device, torch.float32).unsqueeze(0)) if n in w else p
-        for n in _bn_names(dict(m.state_dict())):
+        for n in fc.bn_names(dict(m.state_dict())):
             p = named[n].detach().clone()
             params[n[len(PREFIX):]] = fwAD.make_dual(p, gb[n].to(device, torch.float32)) if n in gb else p
         xin = x.to(device)
@@ -103,12 +70,12 @@ def _op_jt(m, a, x, step, w, gb, xd, device):
 def test_jvp_matches_fp64_autograd(case, direction, cuda_device):
     """J t (logits tangent) against torch.func.jvp in float64 through the oracle's network, at the first and last step, on
     the support and the target batch shape."""
-    a, state, batch = _case(case)
-    m = _model(a, state, cuda_device)
+    a, state, batch = fc.case(case)
+    m = fc.model(a, state, cuda_device)
     S = int(a.number_of_training_steps_per_iter)
     rows, worst = [], 0.0
     for which in ("support", "target"):
-        x, _ = _images(batch, which)
+        x, _ = fc.images(batch, which)
         w, gb, xd = _tangents(a, state, x, direction)
         for step in sorted({0, S - 1}):
             got = _op_jt(m, a, x, step, w, gb, xd, cuda_device)
@@ -124,14 +91,14 @@ def test_jvp_matches_fp64_autograd(case, direction, cuda_device):
 def test_forward_over_reverse_matches_fp64_autograd(case, cuda_device):
     """Tangents of the weight gradients and of dx of CE(op(x, fast)) along (x_dot, theta_dot) -- with the d(logits) tangent
     that cross-entropy's backward produces -- against torch.func.jvp(torch.func.grad(...)) in float64."""
-    a, state, batch = _case(case)
-    m = _model(a, state, cuda_device)
+    a, state, batch = fc.case(case)
+    m = fc.model(a, state, cuda_device)
     inner = O.inner_param_names(a)
     named = dict(m.named_parameters())
     S = int(a.number_of_training_steps_per_iter)
     rows, bad = [], []
     for which in ("support", "target"):
-        x, y = _images(batch, which)
+        x, y = fc.images(batch, which)
         w, _, xd = _tangents(a, state, x, "all")
         for step in sorted({0, S - 1}):
             with fwAD.dual_level():
@@ -205,7 +172,7 @@ def test_forward_mode_hypergradient_of_meta_loop(case, cuda_device):
     g = load_golden(case)
     a, state, batch = g.args, g.state(), g.batch(0)
     epoch = g.iters[0][0]
-    m = _model(a, state, cuda_device)
+    m = fc.model(a, state, cuda_device)
     named = dict(m.named_parameters())
     gen = torch.Generator().manual_seed(5)
     alpha_dot = {n: torch.randn(state[n].shape, generator=gen, dtype=torch.float64) for n in _lslr_names(a)}
@@ -235,9 +202,9 @@ def test_forward_mode_hypergradient_of_meta_loop(case, cuda_device):
 def test_jvp_full_size(case, cuda_device):
     """J t along (weights, gamma / beta, images) on the full-size target batch: max(3 x |oracle32 - oracle64|, 5e-5) of
     max-norm, as the full-size image-gradient test bounds it (pooling / leaky-ReLU flips between fp32 evaluations)."""
-    a, state, batch = _case(case)
-    m = _model(a, state, cuda_device)
-    x, _ = _images(batch, "target")
+    a, state, batch = fc.case(case)
+    m = fc.model(a, state, cuda_device)
+    x, _ = fc.images(batch, "target")
     w, gb, xd = _tangents(a, state, x, "all")
     tf32 = torch.backends.cudnn.allow_tf32
     rows, bad = [], []
@@ -262,20 +229,13 @@ def test_c_abi_tasks_and_zero_image_tangent(cuda_device):
     """Through the C ABI: n_tasks = 2 gives the two n_tasks = 1 per-batch results bit for bit (net_jvp's J t; net_hvp_image's
     J v and, through net_hvp_input_grad, its image part), and net_hvp_image with x_dot = 0 gives net_hvp's J v and H v bit
     for bit.  H v is summed over the batches, so its n_tasks = 2 form is compared to the sum of the two to fp32 rounding."""
-    from howtotrainyourmamlpytorch_b200 import _native
-    a, state, batch = _case("tiny_pp")
-    m = _model(a, state, cuda_device)
+    a, state, batch = fc.case("tiny_pp")
+    m = fc.model(a, state, cuda_device)
     xt = batch[1].float()
     x2 = torch.stack([xt[0].reshape(-1, *xt.shape[-3:]), xt[1 % xt.shape[0]].reshape(-1, *xt.shape[-3:]) * 0.5 + 0.1]).to(cuda_device)
     n, N, step = x2.shape[1], int(a.num_classes_per_set), int(a.number_of_training_steps_per_iter) - 1
-    with torch.cuda.device(cuda_device):
-        eng = _native.Engine(n_way=N, k_shot=n // N, t_target=1, channels=int(a.image_channels), height=int(a.image_height),
-                             width=int(a.image_width), filters=int(a.cnn_num_filters), num_stages=int(a.num_stages),
-                             inner_steps=int(a.number_of_training_steps_per_iter), per_step_bn=bool(a.per_step_bn_statistics),
-                             max_tasks=2)
-    meta = torch.zeros(eng.meta_size, dtype=torch.float32, device=cuda_device)
-    for (off, size), t in zip(eng.segments, m.classifier._segment_tensors(None)):
-        meta[off:off + size] = t.detach().reshape(-1)
+    eng = fc.engine(a, n // N, 1, 2, cuda_device)
+    meta = fc.meta_like(m, eng, cuda_device)
     gen = torch.Generator().manual_seed(3)
     t_like = torch.randn(eng.meta_size, generator=gen).to(cuda_device)
     xdot = torch.randn(x2.shape, generator=gen).to(cuda_device)
@@ -312,25 +272,25 @@ def test_c_abi_tasks_and_zero_image_tangent(cuda_device):
     assert torch.equal(jv_a, jv_b) and torch.equal(hv_a, hv_b)
 
 
-def test_gamma_beta_tangent_through_the_gradient_is_refused(cuda_device):
+def test_gamma_beta_tangent_through_the_gradient_is_refused_before_any_launch(cuda_device):
     """A forward-mode tangent on a BatchNorm gamma / beta that reaches the operator's BACKWARD (forward-over-reverse) needs
     gamma / beta tangent directions in the backward tangent: refused before any launch.  (J t along gamma / beta itself,
     without the backward, is supported: test_jvp_matches_fp64_autograd.)"""
-    a, state, batch = _case("tiny_pp")
-    m = _model(a, state, cuda_device)
-    x, y = _images(batch, "support")
+    a, state, batch = fc.case("tiny_pp")
+    m = fc.model(a, state, cuda_device)
+    x, y = fc.images(batch, "support")
     named = dict(m.named_parameters())
-    bn = _bn_names(state)[0]
+    bn = fc.bn_names(state)[0]
     with fwAD.dual_level():
         params = {n[len(PREFIX):]: named[n].detach().clone().unsqueeze(0).requires_grad_(True) for n in O.inner_param_names(a)}
         params[bn[len(PREFIX):]] = fwAD.make_dual(named[bn].detach().clone(), torch.ones_like(named[bn]))
         loss = Fnn.cross_entropy(m.classifier.forward(x.to(cuda_device), num_step=0, params=params, training=True),
                                  y.to(cuda_device))
-        cache = m.classifier._engines[(x.shape[0], cuda_device.index)]
-        hvp_before = "hvp" in cache
-        gen_before = cache["gen"]
+        ops = m.classifier._operator_handles[(x.shape[0], cuda_device.index)]
+        second_before = ops.second_order is not None
+        gen_before = ops.gen
         torch.cuda.synchronize()
         with pytest.raises(NotImplementedError, match="gamma / beta"):
             torch.autograd.grad(loss, list(params.values())[:1], create_graph=True)
-    # the refusal comes before the operator's handles are touched: no replayed forward, no HVP handle created by it
-    assert cache["gen"] == gen_before and ("hvp" in cache) == hvp_before
+    # the refusal comes before the operator's handles are touched: no replayed forward, no second-order handle created by it
+    assert ops.gen == gen_before and (ops.second_order is not None) == second_before

@@ -8,6 +8,7 @@ import torch.nn.functional as Fnn
 
 from conftest import load_golden, grad_tolerance
 from engine_layout import rel_err
+import functional_cases as fc
 from oracle import maml_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -16,32 +17,6 @@ PREFIX = "classifier."
 TINY = ["tiny_pp", "tiny_maml", "tiny_bern", "synthetic_c4"]
 # B1 backward policy (DESIGN.md section 6): 5e-5 of the fp64 reference's max-norm
 B1_REL = 5e-5
-
-
-def _case(case):
-    """(args, fp32 state, batch).  synthetic_c4: a seeded model with four input channels -- the geometry of the generic
-    first-block kernels (conv0_kernel / wgrad0_kernel) -- that no golden case covers."""
-    if case == "synthetic_c4":
-        from howtotrainyourmamlpytorch_b200 import make_args
-        a = make_args("omniglot_mamlpp_5w1s", image_channels=4, image_height=14, image_width=14, cnn_num_filters=32,
-                      num_stages=3, number_of_training_steps_per_iter=2, number_of_evaluation_steps_per_iter=2,
-                      batch_size=2, num_target_samples=3)
-        return a, O.init_state(a), O.synthetic_batch(a, iteration=5, kind="normal")
-    g = load_golden(case)
-    return g.args, g.state(), g.batch(0)
-
-
-def _model(a, state, device):
-    from howtotrainyourmamlpytorch_b200 import MAMLFewShotClassifier
-    m = MAMLFewShotClassifier(im_shape=(2, a.image_channels, a.image_height, a.image_width), device=device, args=a)
-    m.load_state_dict(state)
-    return m
-
-
-def _images(batch, which, b=0):
-    xs, xt, ys, yt = batch
-    x, y = (xs, ys) if which == "support" else (xt, yt)
-    return x[b].reshape(-1, *x.shape[-3:]).float(), y[b].reshape(-1).long()
 
 
 def _direction(a, state, seed=11):
@@ -77,13 +52,13 @@ def _op_dx(m, a, x, y, step, v, device):
 
 
 def _per_call(case, order, device):
-    a, state, batch = _case(case)
-    m = _model(a, state, device)
+    a, state, batch = fc.case(case)
+    m = fc.model(a, state, device)
     v = _direction(a, state) if order == 2 else None
     S = int(a.number_of_training_steps_per_iter)
     rows, worst = [], 0.0
     for which in ("target", "support"):
-        x, y = _images(batch, which)
+        x, y = fc.images(batch, which)
         for step in sorted({0, S - 1}):
             got = _op_dx(m, a, x, y, step, v, device)
             want = _oracle_dx(a, state, x, y, step, v, device)
@@ -118,17 +93,17 @@ def test_mixed_second_order_input_grad_matches_fp64_autograd(case, cuda_device):
 #    batch (75 images of 84x84x3) the fp32 oracle itself lands 5e-2 away from fp64 and this operator 4.8e-2, with 309 of
 #    1.6e6 values off by more than 1e-4.  On Omniglot both sit near 3e-7.
 @pytest.mark.parametrize("case", ["omniglot_mamlpp_5w1s", "mini_imagenet_mamlpp_5w1s"])
-def test_input_grad_full_size(case, cuda_device):
-    a, state, batch = _case(case)
-    m = _model(a, state, cuda_device)
-    x, y = _images(batch, "target")
+def test_input_grad_full_size_vs_own_dz0_and_oracle(case, cuda_device):
+    a, state, batch = fc.case(case)
+    m = fc.model(a, state, cuda_device)
+    x, y = fc.images(batch, "target")
     rows, bad = [], []
     n, C, H, W = x.shape
     w0 = state["classifier.layer_dict.conv0.conv.weight"].double().to(cuda_device)
     tf32 = torch.backends.cudnn.allow_tf32
     for step in (0, int(a.number_of_training_steps_per_iter) - 1):
         got = _op_dx(m, a, x, y, step, None, cuda_device)
-        eng = m.classifier._engines[(n, cuda_device.index)]["eng"]
+        eng = m.classifier._operator_handles[(n, cuda_device.index)].first_order
         dz0 = torch.from_numpy(eng.debug_read("tgt_dz", 0, 0, 0)).to(cuda_device, torch.float64)
         dz0 = dz0.view(n, H + 1, W + 1, -1)[:, 1:, 1:, :].permute(0, 3, 1, 2)      # padded grid -> NCHW
         own = Fnn.conv_transpose2d(dz0, w0, padding=1).cpu()
@@ -186,7 +161,7 @@ def test_meta_loop_image_gradients_match_oracle(case, cuda_device):
     g = load_golden(case)
     a, state, batch = g.args, g.state(), g.batch(0)
     epoch = g.iters[0][0]
-    m = _model(a, state, cuda_device)
+    m = fc.model(a, state, cuda_device)
     named = dict(m.named_parameters())
 
     def op(x, fast, s):
@@ -210,33 +185,18 @@ def test_meta_loop_image_gradients_match_oracle(case, cuda_device):
     assert not bad, rows
 
 
-def _engines(a, n, max_tasks, device):
-    from howtotrainyourmamlpytorch_b200 import _native
-    N = int(a.num_classes_per_set)
-    kw = dict(n_way=N, channels=int(a.image_channels), height=int(a.image_height), width=int(a.image_width),
-              filters=int(a.cnn_num_filters), num_stages=int(a.num_stages), inner_steps=int(a.number_of_training_steps_per_iter),
-              per_step_bn=bool(a.per_step_bn_statistics), max_tasks=max_tasks)
-    with torch.cuda.device(device):
-        return _native.Engine(k_shot=1, t_target=n // N, **kw), _native.Engine(k_shot=n // N, t_target=1, **kw)
-
-
-def _meta_like(m, eng, device):
-    meta = torch.zeros(eng.meta_size, dtype=torch.float32, device=device)
-    for (off, size), t in zip(eng.segments, m.classifier._segment_tensors(None)):
-        meta[off:off + size] = t.detach().reshape(-1)
-    return meta
-
-
 def test_c_abi_tasks_and_call_order(cuda_device):
-    """n_tasks = 2 gives the two n_tasks = 1 results bit for bit (both entries), and an entry that does not immediately
-    follow its call (after net_forward, after the other kind, with another n_tasks) fails and writes nothing."""
-    a, state, batch = _case("tiny_pp")
-    m = _model(a, state, cuda_device)
+    """n_tasks = 2 gives the two n_tasks = 1 results bit for bit (both entries), and an entry that does not follow the call
+    whose buffers it reads fails and writes nothing: the image-gradient entries after net_forward, after the other kind or
+    with another n_tasks; net_backward and net_running_update on a fresh handle, after a net_hvp or with another n_tasks /
+    num_step.  A repeated net_backward of one forward is accepted."""
+    a, state, batch = fc.case("tiny_pp")
+    m = fc.model(a, state, cuda_device)
     xs, xt = batch[0].float(), batch[1].float()
     x2 = torch.stack([xt[0].reshape(-1, *xt.shape[-3:]), xt[1 % xt.shape[0]].reshape(-1, *xt.shape[-3:]) * 0.5 + 0.1]).to(cuda_device)
     n, N, step = x2.shape[1], int(a.num_classes_per_set), int(a.number_of_training_steps_per_iter) - 1
-    fwd, hvp = _engines(a, n, 2, cuda_device)
-    meta = _meta_like(m, fwd, cuda_device)
+    fwd, hvp = fc.engine(a, 1, n // N, 2, cuda_device), fc.engine(a, n // N, 1, 2, cuda_device)
+    meta = fc.meta_like(m, fwd, cuda_device)
     gen = torch.Generator().manual_seed(3)
     dl = torch.randn(2, n, N, generator=gen).to(cuda_device)
     v = torch.randn(fwd.meta_size, generator=gen).to(cuda_device)
@@ -265,19 +225,42 @@ def test_c_abi_tasks_and_call_order(cuda_device):
         assert float(both.abs().max()) > 0
 
     sentinel = torch.full((2, n) + tuple(x2.shape[2:]), float("nan"), device=cuda_device)
+    grad_sentinel = torch.full((fwd.result_size,), float("nan"), device=cuda_device)
+    # running statistics: an EMA of NaN stays NaN, so these are finite and must keep their bits
+    S, F = int(a.number_of_training_steps_per_iter), int(a.cnn_num_filters)
+    run_mean = torch.zeros(int(a.num_stages), S, F, device=cuda_device)
+    run_var = torch.ones_like(run_mean)
 
-    def refused(call, match):
+    def refused(call, match, *outs):
+        outs = outs or (sentinel,)
+        before = [o.clone() for o in outs]
         with pytest.raises(RuntimeError, match=match):
             call()
         torch.cuda.synchronize()
-        assert torch.isnan(sentinel).all(), "a refused call wrote its output"
+        for o, b in zip(outs, before):
+            assert torch.equal(o.view(torch.int32), b.view(torch.int32)), "a refused call wrote its output"
 
+    fresh = fc.engine(a, 1, n // N, 2, cuda_device)
+    order = "must immediately follow maml_b200_net_forward or maml_b200_net_backward"
+    refused(lambda: fresh.net_backward(2, step, meta, dl, grad_sentinel), order, grad_sentinel)
+    refused(lambda: fresh.net_running_update(2, step, run_mean, run_var), order, run_mean, run_var)
+    fresh.close()
     fwd.net_forward(2, step, meta, x2, logits)
     refused(lambda: fwd.net_input_grad(2, sentinel), "must immediately follow maml_b200_net_backward")
     refused(lambda: fwd.net_hvp_input_grad(2, sentinel), "must immediately follow maml_b200_net_hvp")
+    refused(lambda: fwd.net_backward(2, (step + 1) % S, meta, dl, grad_sentinel), "num_step differs", grad_sentinel)
+    refused(lambda: fwd.net_backward(1, step, meta, dl[:1].contiguous(), grad_sentinel), "n_tasks differs", grad_sentinel)
     fwd.net_backward(2, step, meta, dl, grad)
+    again = torch.empty_like(grad)
+    fwd.net_backward(2, step, meta, dl, again)       # a repeated backward of one forward is accepted and gives the same
+    assert torch.equal(grad, again)
     refused(lambda: fwd.net_hvp_input_grad(2, sentinel), "must immediately follow maml_b200_net_hvp")
     refused(lambda: fwd.net_input_grad(1, sentinel), "n_tasks differs")
+    # a net_hvp on the first-order handle (support shape: N images per batch) overwrites the forward's weights and statistics
+    fwd.net_hvp(2, step, meta, x2[:, :N].contiguous(), dl[:, :N].contiguous(), v, torch.empty(2, N, N, device=cuda_device),
+                torch.empty(fwd.result_size, device=cuda_device))
+    refused(lambda: fwd.net_backward(2, step, meta, dl, grad_sentinel), order, grad_sentinel)
+    refused(lambda: fwd.net_running_update(2, step, run_mean, run_var), order, run_mean, run_var)
     hvp.net_hvp(2, step, meta, x2, dl, v, jv, hv)
     refused(lambda: hvp.net_input_grad(2, sentinel), "must immediately follow maml_b200_net_backward")
     refused(lambda: hvp.net_hvp_input_grad(1, sentinel), "n_tasks differs")
@@ -306,9 +289,9 @@ def test_weight_derivatives_unchanged_by_image_gradients(cuda_device, monkeypatc
     """With x not requiring grad the operator never calls the image-gradient entries, and its weight gradients, Hv and
     J v are bit-identical to those computed with x requiring grad."""
     from howtotrainyourmamlpytorch_b200 import _native
-    a, state, batch = _case("tiny_pp")
-    m = _model(a, state, cuda_device)
-    x, y = _images(batch, "support")
+    a, state, batch = fc.case("tiny_pp")
+    m = fc.model(a, state, cuda_device)
+    x, y = fc.images(batch, "support")
     x, y = x.to(cuda_device), y.to(cuda_device)
     v = _direction(a, state)
     cvec = torch.randn(x.shape[0], int(a.num_classes_per_set), generator=torch.Generator().manual_seed(5)).to(cuda_device)
@@ -328,10 +311,10 @@ def test_weight_derivatives_unchanged_by_image_gradients(cuda_device, monkeypatc
 def test_image_gradient_output_is_not_differentiable(cuda_device):
     """A cotangent on the image gradient (e.g. a penalty on |dL/dx| differentiated again) needs image tangent directions,
     which the engine does not have: NotImplementedError, not a wrong number."""
-    a, state, batch = _case("tiny_pp")
-    m = _model(a, state, cuda_device)
+    a, state, batch = fc.case("tiny_pp")
+    m = fc.model(a, state, cuda_device)
     named = dict(m.named_parameters())
-    x, y = _images(batch, "target")
+    x, y = fc.images(batch, "target")
     x = x.to(cuda_device).requires_grad_(True)
     params = {n[len(PREFIX):]: named[n].detach().clone().unsqueeze(0).requires_grad_(True) for n in O.inner_param_names(a)}
     loss = Fnn.cross_entropy(m.classifier.forward(x, num_step=0, params=params), y.to(cuda_device))

@@ -11,23 +11,12 @@ import torch.nn.functional as Fnn
 
 from conftest import BERNOULLI_CASES, BIG_CASES, TINY_CASES, load_golden, grad_tolerance
 from engine_layout import rel_err
+import functional_cases as fc
 from oracle import maml_oracle as O
 
 pytestmark = pytest.mark.gpu
 
 PREFIX = "classifier."
-
-
-def _model(g, device):
-    from howtotrainyourmamlpytorch_b200 import MAMLFewShotClassifier
-    a = g.args
-    m = MAMLFewShotClassifier(im_shape=(2, a.image_channels, a.image_height, a.image_width), device=device, args=a)
-    m.load_state_dict(g.state())
-    return m
-
-
-def _bn_names(a):
-    return [n for n in O.trainable_names(a) if "norm_layer" in n]
 
 
 def _check(rows, name, got, want, conv_bias_abs):
@@ -52,13 +41,13 @@ def test_double_backward_matches_fp64_autograd(case, cuda_device):
     torch.func.jvp of the oracle logits.  The gamma / beta rows pin the sign (+H_gamma v)."""
     g = load_golden(case)
     a = g.args
-    m = _model(g, cuda_device)
+    state = g.state()
+    m = fc.model(a, state, cuda_device)
     named = dict(m.named_parameters())
     xs, xt, ys, yt = g.batch(0)
     x = xs[0].reshape(-1, *xs.shape[-3:])
     y = ys[0].reshape(-1).long()
-    state = g.state()
-    inner, bn = O.inner_param_names(a), _bn_names(a)
+    inner, bn = O.inner_param_names(a), fc.bn_names(state)
     gen = torch.Generator().manual_seed(7)
     v = {n: torch.randn(state[n].shape, generator=gen, dtype=torch.float64) for n in inner}
     c = torch.randn(x.shape[0], int(a.num_classes_per_set), generator=gen, dtype=torch.float64)
@@ -148,7 +137,7 @@ def test_reference_loop_on_operator_matches_goldens(case, cuda_device):
     the meta-gradient vs the fused iteration on the same batch.  tiny_pp_first pins the first-order route."""
     g = load_golden(case)
     a = g.args
-    m = _model(g, cuda_device)
+    m = fc.model(a, g.state(), cuda_device)
     batch, epoch = g.batch(0), g.iters[0][0]
     state = g.state()
     loss, logits, grads, stats = _reference_loop_on_operator(m, a, batch, epoch, cuda_device)
@@ -164,7 +153,7 @@ def test_reference_loop_on_operator_matches_goldens(case, cuda_device):
     for k in run:
         assert torch.allclose(run[k], ref_run[k].float(), rtol=5e-5, atol=5e-6), k
     g32, g64 = g.grads(0, ""), g.grads(0, "64")
-    _, _, fused = _model(g, cuda_device).meta_gradient(batch, epoch)
+    _, _, fused = fc.model(a, g.state(), cuda_device).meta_gradient(batch, epoch)
     rows, bad = [], []
     for n in g64:
         got = grads[n].double()
@@ -234,14 +223,14 @@ def test_batchnorm_gradient_output_is_not_differentiable(cuda_device):
     does not have: NotImplementedError, not a wrong number."""
     g = load_golden("tiny_pp")
     a = g.args
-    m = _model(g, cuda_device)
+    m = fc.model(a, g.state(), cuda_device)
     named = dict(m.named_parameters())
     xs, xt, ys, yt = g.batch(0)
     x = xs[0].reshape(-1, *xs.shape[-3:]).to(cuda_device)
     y = ys[0].reshape(-1).long().to(cuda_device)
     inner = O.inner_param_names(a)
     params = {n[len(PREFIX):]: named[n].detach().clone().unsqueeze(0).requires_grad_(True) for n in inner}
-    gamma = named[_bn_names(a)[-1]]
+    gamma = named[fc.bn_names(g.state())[-1]]
     loss = Fnn.cross_entropy(m.classifier.forward(x, num_step=0, params=params), y)
     g_gamma, = torch.autograd.grad(loss, [gamma], create_graph=True)
     with pytest.raises(NotImplementedError, match="gamma / beta"):
