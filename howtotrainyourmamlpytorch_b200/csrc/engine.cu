@@ -260,10 +260,13 @@ static void plan_chunks(maml_b200_handle* h, int n, ChunkPlan* cp) {
     if (l == 0) {
       nch = (int)std::min<long long>(512, std::max<long long>(1, (rows + 63) / 64));
     } else {
-      // ONE wgrad CTA per SM (wgrad_row_kernel<4,4>: 105 registers x 256 threads; its 48 independent accumulators per thread keep
-      // the FMA pipe fed with 8 warps): a second CTA per SM would take the register file away from the main chain's kernels
-      // running beside it; 3 filter rows x tasks x
-      // chunks should just fill one slot per SM -- 720 CTAs (128-row chunks at 8 tasks) ran as 1.2 waves = 2x the time
+      // ONE wgrad CTA per SM, and 3 filter rows x tasks x chunks should just fill one slot per SM -- 720 CTAs (128-row
+      // chunks at 8 tasks) ran as 1.2 waves = 2x the time.  wgrad_tc_row_kernel: a CTA holds its SM's whole register file
+      // (384 threads x 168 registers), so a second CTA could only run behind the first.  wgrad_row_kernel<4,4>: 105
+      // registers x 256 threads, whose 48 independent accumulators per thread keep the FMA pipe fed with 8 warps; a
+      // second CTA per SM would take the register file away from the main chain's kernels running beside it.
+      // Chunks are multiples of 16 rows: a partial 32-row stage of the tensor-core kernel costs a full one, but the rows
+      // of a chunk (and so the summation order of the gradient) do not depend on which kernel runs
       long long want = std::max<long long>(1, num_sms() / (3LL * h->maxT));
       nch = (int)std::min<long long>(std::min<long long>(64, want), std::max<long long>(1, (rows + 15) / 16));
     }
@@ -337,7 +340,7 @@ static int make_all_maps(maml_b200_handle* h) {
     if (make_map(&h->theta_map[pl], h->pack_theta + pl * h->pack_theta_plane, h->pack_theta_plane / h->F, h->F, h->F)) return 1;
     if (make_map(&h->u_map[pl], h->pack_u + pl * h->pack_u_plane, h->pack_u_plane / h->F, h->F, h->F)) return 1;
   }
-  if (tc_conv_prepare()) return fail("cudaFuncSetAttribute(max dynamic shared memory) failed for the wgmma conv kernel");
+  if (tc_conv_prepare()) return fail("cudaFuncSetAttribute(max dynamic shared memory) failed for the wgmma conv / weight-gradient kernels");
   return 0;
 }
 

@@ -106,7 +106,7 @@ __device__ __forceinline__ void wgmma_tf32_n64(float (&d)[32], uint64_t adesc, u
                : "l"(adesc), "l"(bdesc), "r"(1) : "memory");
 }
 
-// the same with the A fragment in registers (m64k8 tf32 layout per warp: see wgrad_tc_kernel)
+// the same with the A fragment in registers (m64k8 tf32 layout per warp: see wgrad_tc_row_kernel)
 __device__ __forceinline__ void wgmma_tf32_rs_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t bdesc) {
   asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
                "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
@@ -477,16 +477,26 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
 // ---------------------------------------------------------------------------------------------
 // wgmma weight gradient of the 3x3 convolutions of blocks l >= 1, fp32-faithful via the 3xTF32 operand split:
 //
-//   dW[tap][c][f] = sum_src sum_j  A_src[j + s_tap, c] * D_src[j, f]            (+ db[f] = sum_j D_0[j, f])
+//   partial[chunk][tap][c][f] = sum_src sum_{j in chunk} A_src[j + s_tap, c] * D_src[j, f]
+//   partial[chunk][bias][f]   = sum_{j in chunk} D_0[j, f]                 (centre filter row CTA, fp32)
 //
 // GEMM M = c, N = f, K = j (pixels).  Both operands are stored pixel-major ([grid row][channel], common.cuh), i.e.
-// MN-major for this GEMM, and TF32 wgmma reads shared-memory operands K-major only.  So A comes from REGISTERS (any
-// layout: each thread loads its m64k8 fragment straight from the hi / lo planes, the tap shift is a row offset) and the
-// warpgroup transposes every 32-row stage of D into K-major SWIZZLE_128B tiles ([f][32 j], the conv kernel's B layout).
-// CTA = one warpgroup per (row chunk, tap, task).  Per K step of 8 rows: A_hi*D_hi into one accumulator, A_hi*D_lo and
-// A_lo*D_hi into a second; after every 32-row stage (4 K steps) both are drained into fp32 register totals with IEEE adds
-// (the tensor core's accumulation truncates, so no accumulator takes more than 8 accumulations).  The dead conv-bias gradient (column sums
-// of D_0) is summed in fp32 by the centre-tap CTA.
+// MN-major for this GEMM, and TF32 wgmma reads shared-memory operands K-major only.  So A comes from REGISTERS (m64k8
+// fragments loaded from shared memory with ld.shared) and every 32-row stage of D is transposed into K-major
+// SWIZZLE_128B tiles ([f][32 j], the conv kernel's B layout).
+//
+// CTA = one (row chunk, filter row ky, task), the grid of wgrad_row_kernel, and three warpgroups: warpgroup kx computes
+// tap (ky, kx).  The three taps of a filter row read A rows shifted by sh - 1, sh, sh + 1, so ONE staged window of
+// 32 + 2 rows serves all three.  Every 32-row stage (A window and D rows, hi and lo; the fp32 D_0 rows too in the bias
+// CTA) streams into a ring of WG_NS slots with cp.async, zero-filled outside the guarded A matrix and past the chunk
+// end; each thread issues a share and its completions arrive on the slot's mbarrier.  There is no producer warp: a
+// 13th warp would put 4 warps on one SM sub-partition and cap every thread at 128 registers (the accumulators need
+// ~150); with 12 warps the cap is 168.
+// Per stage the threads transpose D ONCE (each a share) into the slot's B tiles and one named barrier publishes them.
+// The same barrier shows that every warpgroup has drained the previous stage, so its slot is refilled right after it.
+// Each warpgroup then issues its 4 K steps -- A_hi*D_hi into one accumulator, A_hi*D_lo + A_lo*D_hi into a second --,
+// transposes the NEXT stage while they run, and only then waits and drains both into fp32 register totals with IEEE
+// adds (the tensor core's accumulation truncates, so no accumulator takes more than 8 MMAs).
 // ---------------------------------------------------------------------------------------------
 template <int NC>
 __device__ __forceinline__ void wgmma_tf32_rs(float (&d)[NC / 2], const uint32_t (&a)[4], uint64_t bdesc) {
@@ -496,120 +506,171 @@ __device__ __forceinline__ void wgmma_tf32_rs(float (&d)[NC / 2], const uint32_t
   else wgmma_tf32_rs_n64(d, a, bdesc);
 }
 
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool ok) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(ok ? 16 : 0) : "memory");
+}
+// arrives on `bar` once every cp.async this thread has issued so far has landed (counts toward the init count)
+__device__ __forceinline__ void cp_async_arrive(uint64_t* bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+
+constexpr int WG_NS = 3;                   // ring slots
+constexpr int WG_THREADS = 384;            // 3 warpgroups, one per tap kx
+
+// one ring slot (bytes, 1024-aligned: the B tiles lead): B_hi, B_lo [NC][32] swizzled | A window hi, lo [34][NC + 8] |
+// D hi, lo [32][NC] | fp32 D_0 [32][NC]
+template <int NC> struct WgSlot {
+  static constexpr int BT = NC * 128;
+  static constexpr int AP = NC + 8;        // window pitch (floats): the fragment loads of a warp hit 32 distinct banks
+  static constexpr int AW = 34 * AP * 4;
+  static constexpr int DW = 32 * NC * 4;
+  static constexpr int A_OFF = 2 * BT, D_OFF = A_OFF + 2 * AW, DF_OFF = D_OFF + 2 * DW;
+  static constexpr int BYTES = (DF_OFF + DW + 1023) / 1024 * 1024;
+};
+template <int NC> constexpr size_t wgrad_tc_smem() { return (size_t)WG_NS * WgSlot<NC>::BYTES + 1024; }
+
 template <int NC>
-__global__ void __launch_bounds__(128) wgrad_tc_kernel(const WgradArgs a) {
+__global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_row_kernel(const WgradArgs a) {
   pdl_prologue(27, a.tag);
+  using S = WgSlot<NC>;
   constexpr int R = NC / 2;
-  constexpr int BT = NC * 128;                   // one K-major [NC][32] SWIZZLE_128B tile (bytes)
-  constexpr int DV = NC / 16;                    // float4 of one 32-row D stage per thread and plane
+  constexpr int Q = NC / 4;                // float4 per row
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  __shared__ uint64_t full[WG_NS];
   const int task = blockIdx.y;
-  const int chunk = blockIdx.x / 9, tap = blockIdx.x - chunk * 9;
-  const int ky = tap / 3, kx = tap - 3 * ky;
-  const int sh = (ky - 1) * a.gw + (kx - 1);
+  const int chunk = blockIdx.x / 3, ky = blockIdx.x - chunk * 3;
+  const int sh0 = (ky - 1) * a.gw - 1;     // window row 0 = output row + sh0 (tap kx = 0)
   const int r_begin = chunk * a.rows_per_chunk;
   const int r_end = min(a.rows, r_begin + a.rows_per_chunk);
   const int guard = a.gw + 2;
-  const int KC = a.kc;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int c0 = 16 * warp + (lane >> 2), t4 = lane & 3;   // A fragment: channels c0 (+8), pixels t4 (+4) of a K step
-  const int steps = (r_end - r_begin + 31) / 32;
+  const int steps = r_end > r_begin ? (r_end - r_begin + 31) / 32 : 0;
   const int nit = steps * a.nsrc;
+  const bool bias_cta = (ky == 1);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
+  if (tid == 0) {
+    for (int s = 0; s < WG_NS; ++s) mbar_init(&full[s], WG_THREADS);
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  // this thread's share of stage `it` -> its slot
+  auto load_stage = [&](int it) {
+    const int slot = it % WG_NS;
+    const int s = it / steps;
+    const int r0 = r_begin + (it - s * steps) * 32;
+    const float* Ah = a.A[s] + (long long)task * a.a_stride[s] + a.a_plane[s];
+    const float* Al = Ah + a.a_plane[s];
+    const float* Df = a.D[s] + (long long)task * a.d_stride[s];
+    const float* Dh = Df + a.d_plane[s];
+    const float* Dl = Dh + a.d_plane[s];
+    const uint32_t base = smem_u32(smem + (size_t)slot * S::BYTES);
+    for (int e = tid; e < 34 * Q; e += WG_THREADS) {
+      const int r = e / Q, c4 = e - r * Q;
+      const int jr = r0 + sh0 + r;
+      const bool ok = jr >= -guard && jr < a.rows + guard;
+      const long long go = ok ? (long long)jr * NC + c4 * 4 : 0;
+      const uint32_t so = (uint32_t)((r * S::AP + c4 * 4) * 4);
+      cp_async16(base + S::A_OFF + so, Ah + go, ok);
+      cp_async16(base + S::A_OFF + S::AW + so, Al + go, ok);
+    }
+    const bool want_f = bias_cta && s == 0;
+    for (int e = tid; e < 32 * Q; e += WG_THREADS) {
+      const int r = e / Q;
+      const int jr = r0 + r;
+      const bool ok = jr < r_end;
+      const long long go = ok ? (long long)jr * NC + (e - r * Q) * 4 : 0;
+      cp_async16(base + S::D_OFF + e * 16, Dh + go, ok);
+      cp_async16(base + S::D_OFF + S::DW + e * 16, Dl + go, ok);
+      if (want_f) cp_async16(base + S::DF_OFF + e * 16, Df + go, ok);
+    }
+    cp_async_arrive(&full[slot]);
+  };
+
+  const int kx = warp >> 2;
+  const int c0 = 16 * (warp & 3) + (lane >> 2), t4 = lane & 3;   // A fragment: channels c0 (+8), pixels t4 (+4) of a K step
+  const bool c_ok = c0 < NC;                                      // NC < 64: the upper fragment rows are zero
   float big[R], small[R], tot[R];
 #pragma unroll
   for (int i = 0; i < R; ++i) { big[i] = 0.f; small[i] = 0.f; tot[i] = 0.f; }
-  float4 dh[DV], dl[DV];
-  auto fetch_d = [&](int it) {
-    const int s = it / steps;
-    const int r0 = r_begin + (it - s * steps) * 32;
-    const float* Dh = a.D[s] + (long long)task * a.d_stride[s] + a.d_plane[s];
-    const float* Dl = Dh + a.d_plane[s];
-#pragma unroll
-    for (int v = 0; v < DV; ++v) {
-      const int e = tid + 128 * v, r = e / (NC / 4), f4 = e - r * (NC / 4);
-      const int jr = r0 + r;
-      const bool ok = jr < r_end;
-      dh[v] = ok ? *reinterpret_cast<const float4*>(Dh + (long long)jr * NC + f4 * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
-      dl[v] = ok ? *reinterpret_cast<const float4*>(Dl + (long long)jr * NC + f4 * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-  };
-  auto drain = [&]() {
-    wgmma_wait<0>();
-    reg_fence<R>(big);
-    reg_fence<R>(small);
-#pragma unroll
-    for (int i = 0; i < R; ++i) { tot[i] += big[i] + small[i]; big[i] = 0.f; small[i] = 0.f; }
-  };
+  float bacc = 0.f;
 
-  const uint64_t desc_h = make_desc_sw128(smem_u32(smem)), desc_l = desc_h + (uint64_t)(BT >> 4);
-  if (nit > 0) fetch_d(0);
-  for (int it = 0; it < nit; ++it) {
-    const int s = it / steps;
-    const int r0 = r_begin + (it - s * steps) * 32;
-    // D stage -> K-major tiles: element (f, j) at f * 128 + ((j / 4) ^ (f % 8)) * 16 + (j % 4) * 4
-#pragma unroll
-    for (int v = 0; v < DV; ++v) {
-      const int e = tid + 128 * v, r = e / (NC / 4), f4 = e - r * (NC / 4);
-      const float hv[4] = {dh[v].x, dh[v].y, dh[v].z, dh[v].w}, lv[4] = {dl[v].x, dl[v].y, dl[v].z, dl[v].w};
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const int f = f4 * 4 + q;
-        const int off = f * 128 + (((r >> 2) ^ (f & 7)) << 4) + (r & 3) * 4;
-        *reinterpret_cast<float*>(smem + off) = hv[q];
-        *reinterpret_cast<float*>(smem + BT + off) = lv[q];
-      }
+  // D stage of `slot` -> K-major tiles: element (f, j) at f * 128 + ((j / 4) ^ (f % 8)) * 16 + (j % 4) * 4.  Item =
+  // (plane, j / 4, f), f fastest: four column reads of the row-major stage, one 16-byte store (8 consecutive f of a
+  // quarter warp land in 8 distinct 16-byte bank groups)
+  auto transpose = [&](int it) {
+    const int slot = it % WG_NS;
+    uint8_t* sb = smem + (size_t)slot * S::BYTES;
+    mbar_wait(&full[slot], (uint32_t)(it / WG_NS) & 1u);
+    for (int e = tid; e < 2 * 8 * NC; e += WG_THREADS) {
+      const int pl = e / (8 * NC), rem = e - pl * 8 * NC;
+      const int j4 = rem / NC, f = rem - j4 * NC;
+      const float* src = reinterpret_cast<const float*>(sb + S::D_OFF + pl * S::DW) + (4 * j4) * NC + f;
+      const float4 v = make_float4(src[0], src[NC], src[2 * NC], src[3 * NC]);
+      *reinterpret_cast<float4*>(sb + pl * S::BT + f * 128 + ((j4 ^ (f & 7)) << 4)) = v;
+    }
+    if (bias_cta && tid < NC && it < steps) {        // bias: fp32 column sums of D_0, rows in order
+      const float* df = reinterpret_cast<const float*>(sb + S::DF_OFF) + tid;
+#pragma unroll 8
+      for (int r = 0; r < 32; ++r) bacc += df[r * NC];
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma
+  };
+
+  for (int i = 0; i < WG_NS - 1 && i < nit; ++i) load_stage(i);
+  if (nit > 0) transpose(0);
+  for (int it = 0; it < nit; ++it) {
+    const uint8_t* sb = smem + (size_t)(it % WG_NS) * S::BYTES;
+    // stage it's B tiles are complete, and every warpgroup has drained stage it - 1: refill its slot
     __syncthreads();
-    // A fragments of the stage's 4 K steps (m64k8 tf32: a0 (c0, t4), a1 (c0 + 8, t4), a2 (c0, t4 + 4), a3 (c0 + 8, t4 + 4))
-    const float* Ah = a.A[s] + (long long)task * a.a_stride[s] + a.a_plane[s];
-    const float* Al = Ah + a.a_plane[s];
+    if (it + WG_NS - 1 < nit) load_stage(it + WG_NS - 1);
+    // fragments of the stage's 4 K steps (m64k8 tf32: a0 (c0, t4), a1 (c0 + 8, t4), a2 (c0, t4 + 4), a3 (c0 + 8, t4 + 4));
+    // tap kx reads window rows shifted by kx
+    const float* wh = reinterpret_cast<const float*>(sb + S::A_OFF) + (kx + t4) * S::AP + c0;
+    const float* wl = wh + S::AW / 4;
     uint32_t ah[4][4], al[4][4];
 #pragma unroll
     for (int k = 0; k < 4; ++k)
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
-        const int row = r0 + 8 * k + t4 + ((q & 2) ? 4 : 0);
-        const int c = c0 + ((q & 1) ? 8 : 0);
-        const int jr = row + sh;
-        const bool ok = row < r_end && c < KC && jr >= -guard && jr < a.rows + guard;
-        ah[k][q] = ok ? __float_as_uint(Ah[(long long)jr * KC + c]) : 0u;
-        al[k][q] = ok ? __float_as_uint(Al[(long long)jr * KC + c]) : 0u;
+        const int o = (8 * k + ((q & 2) ? 4 : 0)) * S::AP + ((q & 1) ? 8 : 0);
+        ah[k][q] = c_ok ? __float_as_uint(wh[o]) : 0u;
+        al[k][q] = c_ok ? __float_as_uint(wl[o]) : 0u;
       }
-    const int ks = min(4, (r_end - r0 + 7) >> 3);
+    const uint64_t desc_h = make_desc_sw128(smem_u32(sb)), desc_l = desc_h + (uint64_t)(S::BT >> 4);
+    wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      if (k < ks) {
-        wgmma_fence();
-        wgmma_tf32_rs<NC>(big, ah[k], desc_h + 2 * k);       // K step: +32 B = +2 in the 16-byte address field
-        wgmma_tf32_rs<NC>(small, ah[k], desc_l + 2 * k);
-        wgmma_tf32_rs<NC>(small, al[k], desc_h + 2 * k);
-        wgmma_commit();
-      }
+    for (int k = 0; k < 4; ++k) {                      // rows past the chunk end are zero in D
+      wgmma_tf32_rs<NC>(big, ah[k], desc_h + 2 * k);   // K step: +32 B = +2 in the 16-byte address field
+      wgmma_tf32_rs<NC>(small, ah[k], desc_l + 2 * k);
+      wgmma_tf32_rs<NC>(small, al[k], desc_h + 2 * k);
     }
-    if (it + 1 < nit) fetch_d(it + 1);           // next stage's global loads overlap this stage's MMAs
-    drain();
-    __syncthreads();                             // every MMA has read the tiles before they are overwritten
+    wgmma_commit();
+    if (it + 1 < nit) transpose(it + 1);             // overlaps this stage's MMAs
+    wgmma_wait<0>();
+    reg_fence<R>(big);
+    reg_fence<R>(small);
+#pragma unroll
+    for (int i = 0; i < R; ++i) { tot[i] += big[i] + small[i]; big[i] = 0.f; small[i] = 0.f; }
+    // hide the zeros from the compiler: an accumulator it knows to be zero turns the first MMA into a non-accumulating
+    // one and serialises the next on it
+    reg_fence<R>(big);
+    reg_fence<R>(small);
   }
 
-  float* P = a.partial + (long long)task * a.partial_task_stride + (long long)chunk * a.chunk_stride;
+  float* P = a.partial + (long long)task * a.partial_task_stride + (long long)a.chunk_stride * chunk;
+  const int tap = ky * 3 + kx;
   // accumulator register 4 i + 2 h + e: channel c0 + 8 h, filter 8 i + 2 t4 + e
 #pragma unroll
   for (int i = 0; i < NC / 8; ++i)
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
       const int c = c0 + 8 * hh;
-      if (c < KC)
-        *reinterpret_cast<float2*>(P + (long long)(tap * KC + c) * NC + 8 * i + 2 * t4) = make_float2(tot[4 * i + 2 * hh], tot[4 * i + 2 * hh + 1]);
+      if (c < NC)
+        *reinterpret_cast<float2*>(P + (long long)(tap * NC + c) * NC + 8 * i + 2 * t4) = make_float2(tot[4 * i + 2 * hh], tot[4 * i + 2 * hh + 1]);
     }
-  if (tap == 4 && tid < NC) {
-    const float* D0 = a.D[0] + (long long)task * a.d_stride[0];
-    float bacc = 0.f;
-    for (int j = r_begin; j < r_end; ++j) bacc += D0[(long long)j * NC + tid];
-    P[(long long)9 * KC * NC + tid] = bacc;
-  }
+  if (bias_cta && tid < NC) P[(long long)9 * NC * NC + tid] = bacc;
 }
 
 
@@ -617,14 +678,14 @@ __global__ void __launch_bounds__(128) wgrad_tc_kernel(const WgradArgs a) {
 
 int tc_read_timeline(long long* out16) { return cudaMemcpyFromSymbol(out16, g_tc_timeline, 16 * sizeof(long long)) == cudaSuccess ? 0 : 1; }
 
+// blocks l >= 1 only: kc == ncols (both are F)
 void launch_wgrad_tc(const WgradArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_WGRAD, a.alg_flops, st);
-  dim3 grid(a.nchunks * 9, a.tasks);
-  const size_t smem = (size_t)2 * a.ncols * 128 + 1024;
-  if (a.ncols == 64) launch_pdl(wgrad_tc_kernel<64>, grid, dim3(128), smem, st, tagged(a));
-  else if (a.ncols == 48) launch_pdl(wgrad_tc_kernel<48>, grid, dim3(128), smem, st, tagged(a));
-  else if (a.ncols == 32) launch_pdl(wgrad_tc_kernel<32>, grid, dim3(128), smem, st, tagged(a));
-  else launch_pdl(wgrad_tc_kernel<16>, grid, dim3(128), smem, st, tagged(a));
+  dim3 grid(a.nchunks * 3, a.tasks);
+  if (a.ncols == 64) launch_pdl(wgrad_tc_row_kernel<64>, grid, dim3(WG_THREADS), wgrad_tc_smem<64>(), st, tagged(a));
+  else if (a.ncols == 48) launch_pdl(wgrad_tc_row_kernel<48>, grid, dim3(WG_THREADS), wgrad_tc_smem<48>(), st, tagged(a));
+  else if (a.ncols == 32) launch_pdl(wgrad_tc_row_kernel<32>, grid, dim3(WG_THREADS), wgrad_tc_smem<32>(), st, tagged(a));
+  else launch_pdl(wgrad_tc_row_kernel<16>, grid, dim3(WG_THREADS), wgrad_tc_smem<16>(), st, tagged(a));
   CUDA_CHECK_LAUNCH();
 }
 
@@ -652,7 +713,12 @@ int tc_conv_prepare() {
   cudaError_t e2 = cudaFuncSetAttribute(conv_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxs);
   cudaError_t e3 = cudaFuncSetAttribute(conv_tc_kernel<48>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxs);
   cudaError_t e4 = cudaFuncSetAttribute(conv_tc_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxs);
-  return (e1 == cudaSuccess && e2 == cudaSuccess && e3 == cudaSuccess && e4 == cudaSuccess) ? 0 : 1;
+  cudaError_t w1 = cudaFuncSetAttribute(wgrad_tc_row_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wgrad_tc_smem<64>());
+  cudaError_t w2 = cudaFuncSetAttribute(wgrad_tc_row_kernel<48>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wgrad_tc_smem<48>());
+  cudaError_t w3 = cudaFuncSetAttribute(wgrad_tc_row_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wgrad_tc_smem<32>());
+  cudaError_t w4 = cudaFuncSetAttribute(wgrad_tc_row_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wgrad_tc_smem<16>());
+  return (e1 == cudaSuccess && e2 == cudaSuccess && e3 == cudaSuccess && e4 == cudaSuccess && w1 == cudaSuccess &&
+          w2 == cudaSuccess && w3 == cudaSuccess && w4 == cudaSuccess) ? 0 : 1;
 }
 
 // Split-K factor: small layers have fewer tiles than SMs (Omniglot block 3: 8 tiles, block 2: 32), and one tile's

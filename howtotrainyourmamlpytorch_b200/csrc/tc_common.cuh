@@ -1,4 +1,4 @@
-// Declarations shared by the wgmma conv kernel (kernels_tc.cu) and the engine.
+// Declarations shared by the wgmma conv and weight-gradient kernels (kernels_tc.cu) and the engine.
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
@@ -26,7 +26,7 @@ struct TcConvArgs {
 int tc_conv_rpad(int gw);
 int tc_conv_ring(int ncols, int gw, size_t extra = 0);
 size_t tc_conv_extra_bytes(int ncols, int S, bool tangent);
-int tc_conv_prepare();
+int tc_conv_prepare();     // shared-memory opt-in of the wgmma conv and weight-gradient kernels
 int tc_read_timeline(long long* out16);
 void launch_conv_tc(const TcMaps& maps, const TcConvArgs& a, cudaStream_t st);
 void launch_pack_weights(const ParamLayout& pl, const float* theta, long long theta_task_stride, float* pack,
