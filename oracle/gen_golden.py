@@ -11,7 +11,7 @@ Each ``tests/golden/<case>.npz`` holds: the args (JSON string), the initial ``st
 the fp32 reference outputs (loss, accuracy, last-step logits, every outer gradient captured
 just before ``optimizer.step``, the post-Adam ``state_dict`` incl. running statistics, the
 logged ``learning_rate``), and the fp64 reference loss / gradients (noise-floor anchor for
-the tolerance policy, SURVEY.md appendix C).  Inputs are stored only for the tiny cases; the
+the tolerance policy, SURVEY.md appendix C).  Inputs are stored only for the tiny and envelope cases; the
 full-size ones are regenerated from their seed by ``oracle.maml_oracle.synthetic_batch``.
 
 The reference cannot travel to the GPU box (``/root/reference`` does not exist there), so
@@ -72,6 +72,68 @@ CASES = {
     # BASELINE configs[3] shape (Mini-ImageNet 5-way 5-shot), one task
     "mini_imagenet_mamlpp_5w5s": ("mini_imagenet_mamlpp_5w5s", dict(batch_size=1), [(0, 0)]),
 }
+
+
+def _envelope(base, hwc, f, l, s, nkt, b, iters, kind=KIND, **over):
+    """One envelope case: H x W x C images, F filters, L stages, S inner steps, N-way K-shot with T targets, B tasks."""
+    (h, w, c), (n, k, t) = hwc, nkt
+    d = dict(_TINY, image_height=h, image_width=w, image_channels=c, cnn_num_filters=f, num_stages=l,
+             number_of_training_steps_per_iter=s, number_of_evaluation_steps_per_iter=s, num_classes_per_set=n,
+             num_samples_per_class=k, num_target_samples=t, batch_size=b)
+    if c != 3:
+        d["dataset_name"] = "omniglot_tiny"
+    d.update(over)
+    return (base, d, iters, kind)
+
+
+# Envelope cases: one seeded configuration per corner of what maml_b200_create admits (filters 16..64, 1..4 stages,
+# 1..8 inner steps, 1..4 channels, 2..32 ways, batches up to 128 images, any H x W), each named for the axis it exists
+# for (DESIGN.md section 6).  Inputs are stored like the tiny cases'.  Most cases record a second iteration, so that
+# the post-Adam state is checked after Adam's second step too.  Where the default inner LR of 0.1 throws the inner loop
+# far out (the 1-shot cases: losses of 20-60, or the reference's own fp32 run 1e-3 of max-norm away from its fp64 run on
+# 2-way), the case uses 0.02, so that the comparison with fp64 stays a statement about rounding.  Every fixture holds
+# about eight copies of the weights (state, gradients in fp32 and fp64, post-Adam state per iteration), so wide filter
+# banks go with few stages or one iteration: each file stays under 1 MB.
+ENVELOPE_CASES = {
+    # H != W; odd H at block 0 (21: a pooled row is dropped), odd W at block 1 (15)
+    "env_nonsquare_odd": _envelope("mini_imagenet_mamlpp_5w1s", (21, 30, 3), 16, 3, 2, (3, 2, 2), 2, [(0, 0), (0, 1)]),
+    # C0 = 2 on the generic first-block kernels; a tall image pooled down to 5 x 1; MSL weights between the extremes.
+    # Episode 6, not 0: episode 0 holds a leaky-ReLU pre-activation and a pooling pair 2e-7 from a tie (fp64), which fp32
+    # evaluations resolve either way (the decision-forced test pins it; the direct comparisons cannot)
+    "env_tall_c2": _envelope("omniglot_mamlpp_5w1s", (40, 13, 2), 32, 3, 3, (3, 2, 2), 2, [(3, 6), (3, 1)]),
+    # L = 2 and C0 = 4 in the fused iteration (the generic weight gradient's widest channel count).  One iteration: after
+    # a second one, any fp32 restatement (the CPU oracle included) sits up to 1e-4 away from the reference on 0.5-1.5 %
+    # of some tensors' elements (Adam's second step divides small, noisy gradient elements by their own magnitude)
+    "env_c4_two_stages": _envelope("omniglot_mamlpp_5w1s", (10, 14, 4), 64, 2, 2, (3, 2, 2), 2, [(0, 0)]),
+    # L = 1: no tensor-core block, the first block is the last block, the fused tail runs on block 0
+    "env_one_stage": _envelope("omniglot_mamlpp_5w1s", (12, 12, 1), 16, 1, 2, (3, 2, 2), 2, [(0, 0), (0, 1)],
+                               task_learning_rate=0.02),
+    # S = 8 = MAML_MAX_STEPS with the multi-step loss on: eight target passes, LSLR vectors of 9
+    "env_eight_steps": _envelope("omniglot_mamlpp_5w1s", (16, 16, 1), 32, 4, 8, (3, 2, 2), 2, [(0, 0), (0, 1)]),
+    # S = 1, second order, multi-step loss off: one target slot
+    "env_one_step": _envelope("mini_imagenet_mamlpp_5w1s", (14, 18, 3), 32, 3, 1, (3, 2, 2), 2, [(20, 0), (20, 1)]),
+    # 32-way 4-shot: a support batch of 128 images (the cap), 32 head row groups
+    "env_way32": _envelope("omniglot_mamlpp_5w1s", (8, 8, 1), 16, 3, 2, (32, 4, 1), 1, [(0, 0)]),
+    # the two sides of head_rows / tail_fusable: 17 support rows (head kernel) and 16 (fused tail), 24 target rows
+    "env_way17": _envelope("omniglot_mamlpp_5w1s", (8, 8, 1), 16, 2, 2, (17, 1, 1), 1, [(0, 0)]),
+    "env_way16": _envelope("omniglot_mamlpp_5w1s", (8, 8, 1), 16, 2, 2, (8, 2, 3), 1, [(0, 0), (0, 1)]),
+    # 2-way 1-shot: the smallest batches; the last block's BatchNorm sees 2 x 3 x 3 = 18 values per channel
+    "env_way2": _envelope("omniglot_mamlpp_5w1s", (28, 28, 1), 16, 4, 2, (2, 1, 1), 2, [(0, 0)], task_learning_rate=0.02),
+    # block 1 is 65 wide (grid 66): the halo tile does not fit, so the handle itself runs the FFMA convolutions
+    "env_ffma_wide": _envelope("omniglot_mamlpp_5w1s", (8, 130, 1), 16, 2, 2, (3, 1, 1), 1, [(0, 0)], task_learning_rate=0.02),
+    # block 1 is 62 wide (grid 63): the largest halo the tensor-core convolution admits, a B ring of exactly 2 stages
+    # next to split-K 2 in tangent mode
+    "env_ring_edge": _envelope("mini_imagenet_mamlpp_5w1s", (6, 124, 3), 64, 2, 2, (3, 1, 1), 1, [(0, 0)], task_learning_rate=0.02),
+    # 48 tasks: one weight-gradient chunk per block (num_sms / (3 * 48) rounds to 0), many tasks in every grid
+    "env_many_tasks": _envelope("omniglot_mamlpp_5w1s", (8, 8, 1), 16, 3, 2, (3, 1, 1), 48, [(0, 0)]),
+    # Bernoulli(0.93) images on a non-square odd image: exact pooling ties next to the dropped row
+    "env_bern_nonsquare": _envelope("omniglot_mamlpp_5w1s", (27, 20, 1), 32, 4, 2, (3, 2, 2), 2, [(0, 0)], "bernoulli"),
+    # plain MAML: shared BatchNorm statistics, no LSLR, no multi-step loss, non-square; F = 48 on the tensor cores, and
+    # the head kernel after the last block (5 x 7 pooling windows per image are too many for the fused tail)
+    "env_maml_shared_bn": _envelope("omniglot_maml_5w1s", (18, 26, 3), 48, 2, 4, (3, 2, 2), 2, [(0, 0)],
+                                    dataset_name="omniglot_tiny"),
+}
+CASES.update(ENVELOPE_CASES)
 
 
 def case_kind(case):
@@ -299,7 +361,7 @@ def main():
     for case in which:
         args, argdict, iters = make_args(case)
         kind = case_kind(case)
-        big = not case.startswith("tiny_")
+        big = not case.startswith("tiny_") and case not in ENVELOPE_CASES
         blob = run_reference_fp32(args, iters, store_inputs=not big, kind=kind)
         state32 = {k[len("state/"):]: v for k, v in blob.items() if k.startswith("state/")}
         blob.update(run_reference_validation(args, iters, state32, kind))

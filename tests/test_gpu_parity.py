@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from conftest import ALL_CASES, BERNOULLI_CASES, BIG_CASES, TINY_CASES, load_golden, grad_tolerance
-from engine_layout import geometry, grid_to_nchw, flat_to_nchw, theta_to_ref, rel_err
+from engine_layout import geometry, grid_to_nchw, flat_to_nchw, theta_to_ref, rel_err, gpu_decisions as _gpu_decisions
 from oracle import maml_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -399,41 +399,6 @@ def test_properties_full_size(cuda_device):
             continue
         assert rel_err(gp[n], g1[n]) <= 1e-5, ("task permutation", n)
     assert np.isfinite(float(l1["loss"]))
-
-
-def _gpu_decisions(m, g, batch, epoch):
-    """The discrete decisions the GPU actually took (leaky-ReLU branch per element, arg-max per pooling
-    window), reconstructed bit-exactly from the engine's normalised activations zh:
-    y = fmaf(gamma, zh, beta) (exact product + one rounding == fp64 evaluation rounded to fp32),
-    a = y > 0 ? y : 0.01f * y (fp32), first-max-wins in window order (what F.max_pool2d does on CPU)."""
-    import torch.nn.functional as Fnn
-    a = g.args
-    eng = m._engine
-    geo, _ = geometry(a)
-    F = int(a.cnn_num_filters)
-    N, K, T = int(a.num_classes_per_set), int(a.num_samples_per_class), int(a.num_target_samples)
-    S = int(a.number_of_training_steps_per_iter)
-    B = batch[0].shape[0]
-    sched = O.target_pass_schedule(a, epoch, True, S)
-    sd = {k: v.detach().cpu() for k, v in m.state_dict().items()}
-    dec = {}
-    for b in range(B):
-        for s in range(S):
-            for kind, n in (("sup", N * K), ("tgt", N * T)):
-                if kind == "tgt" and sched[s] is None:
-                    continue
-                per_layer = []
-                for l, gl in enumerate(geo):
-                    zh = grid_to_nchw(eng.debug_read(kind + "_zh", b, s, l), n, gl["h"], gl["w"], F)
-                    _, _, gn, btn, _, _ = O.conv_names(l)
-                    gam, bet = (sd[gn][s], sd[btn][s]) if a.per_step_bn_statistics else (sd[gn], sd[btn])
-                    y = (gam.double()[None, :, None, None] * zh.double() + bet.double()[None, :, None, None]).float()
-                    slope = torch.where(y > 0, torch.ones_like(y), torch.full_like(y, 0.01))
-                    act = torch.where(y > 0, y, torch.tensor(0.01, dtype=torch.float32) * y)
-                    _, idx = Fnn.max_pool2d(act, 2, 2, return_indices=True)
-                    per_layer.append((slope, idx))
-                dec[(b, kind, s)] = per_layer
-    return dec
 
 
 @pytest.mark.parametrize("case", ALL_CASES)
