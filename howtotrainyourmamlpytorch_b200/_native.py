@@ -13,7 +13,7 @@ LIB_PATH = os.environ.get("MAML_B200_LIB") or os.path.join(_PKG, "lib", "libmaml
 
 MAX_STAGES = 4
 MAX_STEPS = 8
-ABI_VERSION = 1
+ABI_VERSION = 2
 
 EXPORTED_SYMBOLS = [
     "maml_b200_abi_version", "maml_b200_last_error", "maml_b200_create", "maml_b200_destroy",
@@ -25,7 +25,8 @@ EXPORTED_SYMBOLS = [
     "maml_b200_comm_init", "maml_b200_comm_connect", "maml_b200_comm_world", "maml_b200_all_reduce",
     "maml_b200_comm_status", "maml_b200_net_backward", "maml_b200_net_running_update", "maml_b200_episode_gather",
     "maml_b200_net_hvp", "maml_b200_net_input_grad", "maml_b200_net_hvp_input_grad",
-    "maml_b200_net_hvp_image", "maml_b200_net_jvp",
+    "maml_b200_net_hvp_image", "maml_b200_net_jvp", "maml_b200_net_forward_tasks", "maml_b200_net_backward_tasks",
+    "maml_b200_net_hvp_image_tasks",
 ]
 PROF_CATS = ["conv_igemm", "conv_first_block", "wgrad", "wgrad_first_block", "bn_act_pool", "head", "param"]
 
@@ -88,6 +89,12 @@ def load_library():
     lib.maml_b200_net_hvp_image.restype = ctypes.c_int
     lib.maml_b200_net_jvp.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp]
     lib.maml_b200_net_jvp.restype = ctypes.c_int
+    lib.maml_b200_net_forward_tasks.argtypes = [vp, i32, i32, vp, i64, vp, vp, vp]
+    lib.maml_b200_net_forward_tasks.restype = ctypes.c_int
+    lib.maml_b200_net_backward_tasks.argtypes = [vp, i32, i32, vp, i64, vp, vp, i32, vp]
+    lib.maml_b200_net_backward_tasks.restype = ctypes.c_int
+    lib.maml_b200_net_hvp_image_tasks.argtypes = [vp, i32, i32, vp, i64, vp, vp, vp, vp, i64, vp, vp, i32, vp]
+    lib.maml_b200_net_hvp_image_tasks.restype = ctypes.c_int
     lib.maml_b200_net_input_grad.argtypes = [vp, i32, vp, vp]
     lib.maml_b200_net_input_grad.restype = ctypes.c_int
     lib.maml_b200_net_hvp_input_grad.argtypes = [vp, i32, vp, vp]
@@ -238,6 +245,29 @@ class Engine(object):
                                         t_like.data_ptr(), None if xdot is None else xdot.data_ptr(), jv_out.data_ptr(),
                                         self._stream())
         _check(self.lib, rc, "maml_b200_net_jvp")
+
+    def net_forward_tasks(self, n_tasks, num_step, meta_like, meta_stride, x, logits):
+        """``net_forward`` with task t's weights at ``meta_like`` + t * meta_stride floats (0: shared)."""
+        rc = self.lib.maml_b200_net_forward_tasks(self.h, int(n_tasks), int(num_step), meta_like.data_ptr(), int(meta_stride),
+                                                  x.data_ptr(), logits.data_ptr(), self._stream())
+        _check(self.lib, rc, "maml_b200_net_forward_tasks")
+
+    def net_backward_tasks(self, n_tasks, num_step, meta_like, meta_stride, dlogits, grad_out, sum_tasks=False):
+        """``net_backward`` with per-task weights; grad_out [n_tasks, result_size] (one vector per task) unless sum_tasks."""
+        rc = self.lib.maml_b200_net_backward_tasks(self.h, int(n_tasks), int(num_step), meta_like.data_ptr(), int(meta_stride),
+                                                   dlogits.data_ptr(), grad_out.data_ptr(), int(bool(sum_tasks)),
+                                                   self._stream())
+        _check(self.lib, rc, "maml_b200_net_backward_tasks")
+
+    def net_hvp_image_tasks(self, n_tasks, num_step, meta_like, meta_stride, x, xdot, dlogits, v_like, dir_stride, jv_out,
+                            hv_out, sum_tasks=False):
+        """``net_hvp_image`` with per-task weights and directions; hv_out [n_tasks, result_size] unless sum_tasks."""
+        rc = self.lib.maml_b200_net_hvp_image_tasks(self.h, int(n_tasks), int(num_step), meta_like.data_ptr(),
+                                                    int(meta_stride), x.data_ptr(), None if xdot is None else xdot.data_ptr(),
+                                                    dlogits.data_ptr(), v_like.data_ptr(), int(dir_stride),
+                                                    jv_out.data_ptr(), hv_out.data_ptr(), int(bool(sum_tasks)),
+                                                    self._stream())
+        _check(self.lib, rc, "maml_b200_net_hvp_image_tasks")
 
     def net_input_grad(self, n_tasks, dx_out):
         rc = self.lib.maml_b200_net_input_grad(self.h, int(n_tasks), dx_out.data_ptr(), self._stream())

@@ -228,8 +228,9 @@ void launch_tail_fused(const BnActArgs& fa, const HeadArgs& ha, const BnBwdArgs&
 void launch_tail_tan_fused(const BnActTanArgs& fa, const HeadArgs& ha, const BnBwdTanArgs& ba, cudaStream_t st);
 void launch_head(const HeadArgs& a, cudaStream_t st);
 
+// meta_task_stride: floats between consecutive tasks' source vectors (0: every task imports the same vector)
 void launch_import_theta(const ParamLayout& pl, const float* meta, float* theta0, long long theta_task_stride,
-                         int tasks, cudaStream_t st);
+                         int tasks, cudaStream_t st, long long meta_task_stride = 0);
 void launch_param_reduce(const ParamLayout& pl, const PartialDesc& pd, const float* partial, int mode,
                          const float* theta_in, float* theta_out, float* g_out, float* tbar,
                          const float* meta, int step, long long task_stride, int tasks, cudaStream_t st,
@@ -268,6 +269,9 @@ struct ExportArgs {
   int n_s, n_t;
   int hw[MAML_MAX_LAYERS];                           // h*w per block
   float* result;
+  // 0: one result vector, summed over the tasks; 1: task t's entries, not summed, at result + t * result_stride (grid.y =
+  // tasks; functional calls only, never with a communicator)
+  int per_task; long long result_stride;
   int tag;          // launch sequence number inside the iteration (device trace)
 };
 void launch_export(const ExportArgs& a, cudaStream_t st);

@@ -980,8 +980,9 @@ static int fork_direction(maml_b200_handle* h, int T, cudaStream_t st, cudaStrea
 }
 
 // Export of a functional call: a plain sum over the n_tasks batches (tasks_global 1, no 1/B) into `result`, no target
-// losses.  The fused iteration sets its schedule on top.
-static ExportArgs export_args(const maml_b200_handle* h, int T, float* result) {
+// losses; with per_task, one unsummed result vector per batch at result + t * result_size.  The fused iteration sets its
+// schedule on top.
+static ExportArgs export_args(const maml_b200_handle* h, int T, float* result, bool per_task = false) {
   ExportArgs e{};
   e.pl = h->pl;
   e.tbar = h->tbar; e.task_stride = h->Ppad;
@@ -993,6 +994,7 @@ static ExportArgs export_args(const maml_b200_handle* h, int T, float* result) {
   e.n_s = h->n_s; e.n_t = h->n_t;
   for (int l = 0; l < h->L; ++l) e.hw[l] = h->geo[l].h * h->geo[l].w;
   e.result = result;
+  e.per_task = per_task ? 1 : 0; e.result_stride = maml_b200_result_size(h);
   return e;
 }
 
@@ -1205,14 +1207,16 @@ static int check_call(const maml_b200_handle* h, bool ptrs, int n_tasks, int num
 
 // Stages a functional call's batch and runs its primal forward on pass set `ps` at `slot`: x (and the image tangent xdot,
 // support grid only) onto the block-0 grid, meta_like into theta slot `slot` (and dir_like into u), the tensor-core packs
-// of that slot, then the forward with the BatchNorm gamma / beta of num_step.  Returns the theta slot.
+// of that slot, then the forward with the BatchNorm gamma / beta of num_step (read from task 0's meta_like).  meta_stride /
+// dir_stride: floats between consecutive tasks' vectors (0: one vector for all tasks).  Returns the theta slot.
 static const float* stage_forward(maml_b200_handle* h, const PassSet& ps, int slot, int stat_kind, int num_step, const float* meta_like,
-                                  const float* x, const float* xdot, const float* dir_like, int T, cudaStream_t st) {
+                                  long long meta_stride, const float* x, const float* xdot, const float* dir_like, long long dir_stride,
+                                  int T, cudaStream_t st) {
   float* th = h->theta + (long long)slot * h->maxT * h->Ppad;
   launch_prep_x(x, ps.xg, ps.xg_stride, T, ps.n, h->C, h->H, h->W, st);
   if (xdot) launch_prep_x(xdot, h->xdot_g, ps.xg_stride, T, ps.n, h->C, h->H, h->W, st);
-  launch_import_theta(h->pl, meta_like, th, h->Ppad, T, st);
-  if (dir_like) launch_import_theta(h->pl, dir_like, h->u, h->Ppad, T, st);
+  launch_import_theta(h->pl, meta_like, th, h->Ppad, T, st, meta_stride);
+  if (dir_like) launch_import_theta(h->pl, dir_like, h->u, h->Ppad, T, st, dir_stride);
   pack_theta_step(h, slot, T, st);
   forward_pass(h, ps, slot, th, slot, meta_like, num_step, stat_kind, T, st);
   return th;
@@ -1242,9 +1246,17 @@ static void external_backward(maml_b200_handle* h, const PassSet& ps, int slot, 
 // under externally supplied weights.  `meta_like` has the layout of the meta vector (conv / linear entries = the
 // weights to use, BatchNorm entries = gamma / beta; LSLR entries ignored).  BatchNorm uses batch statistics and the
 // gamma / beta of `num_step`, exactly like reference VGGReLUNormNetwork.forward (training flag is ignored there too).
-extern "C" int maml_b200_net_forward(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
-                                    const float* x, float* logits, void* stream) {
+static int check_strides(long long meta_stride, long long dir_stride, int64_t meta_size) {
+  if (meta_stride < 0 || dir_stride < 0) return fail("negative task stride");
+  if ((meta_stride > 0 && meta_stride < meta_size) || (dir_stride > 0 && dir_stride < meta_size))
+    return fail("task stride smaller than meta_size (consecutive tasks' vectors would overlap)");
+  return 0;
+}
+
+extern "C" int maml_b200_net_forward_tasks(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
+                                          int64_t meta_stride, const float* x, float* logits, void* stream) {
   if (check_call(h, meta_like && x && logits, n_tasks, num_step)) return 1;
+  if (check_strides(meta_stride, 0, h->pl.meta_size)) return 1;
   cudaStream_t st = (cudaStream_t)stream;
   LaunchScope launch_scope(h, st);
   const int T = n_tasks;
@@ -1252,7 +1264,7 @@ extern "C" int maml_b200_net_forward(maml_b200_handle* h, int32_t n_tasks, int32
   CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
   CK(cudaMemsetAsync(h->losses, 0, (size_t)h->maxT * MAML_MAX_STEPS * sizeof(float), st));
   CK(cudaMemsetAsync(h->correct, 0, (size_t)h->maxT * sizeof(float), st));
-  stage_forward(h, h->tgt, 0, PASS_TGT_FWD, num_step, meta_like, x, nullptr, nullptr, T, st);
+  stage_forward(h, h->tgt, 0, PASS_TGT_FWD, num_step, meta_like, meta_stride, x, nullptr, nullptr, 0, T, st);
   HeadArgs a{};
   a.mode = HEAD_TARGET_FWD; a.n = h->n_t; a.N = h->N; a.D = h->D; a.scale = 1.f;
   a.f = AIN(h->tgt, h->L, 0); a.f_stride = STRIDE(h->tgt, ain, h->L);
@@ -1267,16 +1279,24 @@ extern "C" int maml_b200_net_forward(maml_b200_handle* h, int32_t n_tasks, int32
   return 0;
 }
 
+extern "C" int maml_b200_net_forward(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
+                                    const float* x, float* logits, void* stream) {
+  return maml_b200_net_forward_tasks(h, n_tasks, num_step, meta_like, 0, x, logits, stream);
+}
+
 // Backward of the functional forward above (level B1: lets torch.autograd differentiate through the operator, the way the
 // reference's apply_inner_loop_update does with torch.autograd.grad, few_shot_learning_system.py:138-139, first order).
 // Must follow maml_b200_net_forward (or another net_backward of it) on the same handle with the same (n_tasks, num_step,
 // meta_like): the activations of that call are what this one differentiates.  The handle's call record refuses another
 // order, n_tasks or num_step (meta_like it cannot check).  dlogits [n_tasks, N*T, N] = d(loss)/d(logits).  grad_out:
 // result_size floats; the first meta_size hold d(loss)/d(meta_like) in the meta layout (conv / linear weights and biases,
-// BatchNorm beta / gamma of `num_step`; LSLR entries 0), summed over the n_tasks batches.  No gradient w.r.t. the images.
-extern "C" int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
-                                     const float* dlogits, float* grad_out, void* stream) {
+// BatchNorm beta / gamma of `num_step`; LSLR entries 0), summed over the n_tasks batches (sum_tasks) or one vector per batch
+// at grad_out + t * result_size.  No gradient w.r.t. the images.
+extern "C" int maml_b200_net_backward_tasks(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
+                                           int64_t meta_stride, const float* dlogits, float* grad_out, int32_t sum_tasks,
+                                           void* stream) {
   if (check_call(h, meta_like && dlogits && grad_out, n_tasks, num_step)) return 1;
+  if (check_strides(meta_stride, 0, h->pl.meta_size)) return 1;
   if (require_call(h, FN_FORWARD | FN_BACKWARD, n_tasks, num_step, "maml_b200_net_backward")) return 1;
   cudaStream_t st = (cudaStream_t)stream;
   LaunchScope launch_scope(h, st);
@@ -1292,10 +1312,15 @@ extern "C" int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int3
   external_backward(h, h->tgt, 0, num_step, PASS_TGT_FWD, PASS_TGT_BWD, meta_like, dlogits, h->tgt_partial, h->plan_tgt, T, st);
   launch_param_reduce(h->pl, h->plan_tgt.pd, h->tgt_partial, PR_STORE, nullptr, nullptr, h->tbar, nullptr, meta_like, num_step,
                       h->Ppad, T, st);
-  launch_export(export_args(h, T, grad_out), st);
+  launch_export(export_args(h, T, grad_out, !sum_tasks), st);
   CK(cudaGetLastError());
   record_call(h, FN_BACKWARD, T, num_step);
   return 0;
+}
+
+extern "C" int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
+                                     const float* dlogits, float* grad_out, void* stream) {
+  return maml_b200_net_backward_tasks(h, n_tasks, num_step, meta_like, 0, dlogits, grad_out, 1, stream);
 }
 
 // A forward-mode buffer allocated on first use and zeroed on the call's stream (the kernels that read it run there; a
@@ -1328,9 +1353,12 @@ static int ensure_xdot(maml_b200_handle* h, cudaStream_t st) {
 // tbar by the parameter reduction, the BatchNorm gamma / beta sums go to the PASS_TGT_BWD statistics, which export adds
 // (+H_gamma v, +H_beta v); LSLR entries 0.  v_like's BatchNorm and LSLR entries are not read.  Overwrites the batch
 // statistics maml_b200_net_running_update reads; no running-statistics side effect of its own.
-static int net_hvp_impl(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
-                        const float* xdot, const float* dlogits, const float* v_like, float* jv_out, float* hv_out, void* stream) {
+// meta_stride / dir_stride / sum_tasks: as in maml_b200_net_hvp_image_tasks.
+static int net_hvp_impl(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, long long meta_stride,
+                        const float* x, const float* xdot, const float* dlogits, const float* v_like, long long dir_stride,
+                        float* jv_out, float* hv_out, bool sum_tasks, void* stream) {
   if (check_call(h, meta_like && x && dlogits && v_like && jv_out && hv_out, n_tasks, num_step)) return 1;
+  if (check_strides(meta_stride, dir_stride, h->pl.meta_size)) return 1;
   cudaStream_t st = (cudaStream_t)stream;
   LaunchScope launch_scope(h, st);
   const int T = n_tasks, s = num_step;
@@ -1340,7 +1368,7 @@ static int net_hvp_impl(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, 
   CK(cudaMemsetAsync(h->abar, 0, (size_t)h->maxT * h->pl.nseg_inner * MAML_MAX_STEPS * sizeof(double), st));
   CK(cudaMemsetAsync(h->losses, 0, (size_t)h->maxT * MAML_MAX_STEPS * sizeof(float), st));
   CK(cudaMemsetAsync(h->correct, 0, (size_t)h->maxT * sizeof(float), st));
-  const float* th = stage_forward(h, h->sup, s, PASS_SUP_FWD, s, meta_like, x, xdot, v_like, T, st);
+  const float* th = stage_forward(h, h->sup, s, PASS_SUP_FWD, s, meta_like, meta_stride, x, xdot, v_like, dir_stride, T, st);
   // the tangent pass reads this backward's dz / dp and statistics; its weight-gradient chunks are overwritten unread
   external_backward(h, h->sup, s, s, PASS_SUP_FWD, PASS_SUP_BWD, meta_like, dlogits, h->sup_partial, h->plan_sup, T, st);
   cudaStream_t spre;
@@ -1349,7 +1377,7 @@ static int net_hvp_impl(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, 
   tangent_pass(h, s, th, h->u, meta_like, TangentHead{HEAD_EXTERNAL_TAN, nullptr, dlogits, jv_out, PASS_TGT_BWD}, T, st, rs, spre,
                xdot ? h->xdot_g : nullptr);
   join_pending(h, st);
-  launch_export(export_args(h, T, hv_out), st);
+  launch_export(export_args(h, T, hv_out, !sum_tasks), st);
   CK(cudaGetLastError());
   record_call(h, FN_HVP, T, num_step);
   return 0;
@@ -1357,7 +1385,7 @@ static int net_hvp_impl(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, 
 
 extern "C" int maml_b200_net_hvp(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
                                  const float* dlogits, const float* v_like, float* jv_out, float* hv_out, void* stream) {
-  return net_hvp_impl(h, n_tasks, num_step, meta_like, x, nullptr, dlogits, v_like, jv_out, hv_out, stream);
+  return net_hvp_impl(h, n_tasks, num_step, meta_like, 0, x, nullptr, dlogits, v_like, 0, jv_out, hv_out, true, stream);
 }
 
 // maml_b200_net_hvp along the images too: the tangent direction is (v_like's weights, xdot).  jv_out = J_theta v +
@@ -1366,7 +1394,17 @@ extern "C" int maml_b200_net_hvp(maml_b200_handle* h, int32_t n_tasks, int32_t n
 extern "C" int maml_b200_net_hvp_image(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
                                        const float* x, const float* xdot, const float* dlogits, const float* v_like, float* jv_out,
                                        float* hv_out, void* stream) {
-  return net_hvp_impl(h, n_tasks, num_step, meta_like, x, xdot, dlogits, v_like, jv_out, hv_out, stream);
+  return net_hvp_impl(h, n_tasks, num_step, meta_like, 0, x, xdot, dlogits, v_like, 0, jv_out, hv_out, true, stream);
+}
+
+// Per-task form of maml_b200_net_hvp_image: task t's weights at meta_like + t * meta_stride and its direction at
+// v_like + t * dir_stride (0: shared); hv_out summed over the tasks (sum_tasks) or one vector per task.
+extern "C" int maml_b200_net_hvp_image_tasks(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
+                                             int64_t meta_stride, const float* x, const float* xdot, const float* dlogits,
+                                             const float* v_like, int64_t dir_stride, float* jv_out, float* hv_out,
+                                             int32_t sum_tasks, void* stream) {
+  return net_hvp_impl(h, n_tasks, num_step, meta_like, meta_stride, x, xdot, dlogits, v_like, dir_stride, jv_out, hv_out,
+                      sum_tasks != 0, stream);
 }
 
 // Forward mode of the functional operator: jv_out [n_tasks, N*K, N] = J_theta t + J_x xdot at the weights meta_like, for
@@ -1386,7 +1424,7 @@ extern "C" int maml_b200_net_jvp(maml_b200_handle* h, int32_t n_tasks, int32_t n
   // zero d(logits) of one batch, read with a task stride of 0
   if (!h->zero_dl && alloc_zeroed(&h->zero_dl, (size_t)h->n_s * h->N * sizeof(float), st)) return 1;
   CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
-  const float* th = stage_forward(h, h->sup, s, PASS_SUP_FWD, s, meta_like, x, xdot, t_like, T, st);
+  const float* th = stage_forward(h, h->sup, s, PASS_SUP_FWD, s, meta_like, 0, x, xdot, t_like, 0, T, st);
   cudaStream_t spre;
   if (fork_direction(h, T, st, &spre)) return 1;
   tangent_forward(h, s, th, h->u, meta_like, xdot ? h->xdot_g : nullptr, t_like, T, st, spre, false, nullptr);

@@ -38,20 +38,22 @@ __device__ __forceinline__ long long internal_to_meta(const ParamLayout& pl, lon
   return pl.m_fcb + (i - pl.fcb_off);
 }
 
+// src_stride 0: one meta vector broadcast to every task; otherwise task t reads meta + t * src_stride
 __global__ void import_theta_kernel(ParamLayout pl, const float* __restrict__ meta, float* __restrict__ theta0,
-                                    long long stride, int tasks, int tag) {
+                                    long long stride, int tasks, long long src_stride, int tag) {
   pdl_prologue(15, tag);
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= pl.P) return;
   int seg;
-  const float v = meta[internal_to_meta(pl, i, &seg)];
-  for (int t = 0; t < tasks; ++t) theta0[(long long)t * stride + i] = v;
+  const long long mi = internal_to_meta(pl, i, &seg);
+  for (int t = 0; t < tasks; ++t) theta0[(long long)t * stride + i] = meta[(long long)t * src_stride + mi];
 }
 
 void launch_import_theta(const ParamLayout& pl, const float* meta, float* theta0, long long stride, int tasks,
-                         cudaStream_t st) {
+                         cudaStream_t st, long long meta_task_stride) {
   ProfScope prof_scope__(PROF_PARAM, 0.0, st);
-  launch_pdl(import_theta_kernel, dim3((unsigned)((pl.P + 255) / 256)), dim3(256), (size_t)(0), st, pl, meta, theta0, stride, tasks, launch_tag());
+  launch_pdl(import_theta_kernel, dim3((unsigned)((pl.P + 255) / 256)), dim3(256), (size_t)(0), st, pl, meta, theta0, stride, tasks,
+             meta_task_stride, launch_tag());
   CUDA_CHECK_LAUNCH();
 }
 
@@ -222,6 +224,9 @@ __device__ __forceinline__ void export_body(const ExportArgs& a, float* __restri
   const long long LSF = (long long)pl.L * pl.S * pl.F;
   const double invB = 1.0 / (double)a.tasks_global;
   const long long nb1 = export_range1_blocks(pl);
+  // the tasks this block adds up: all of them, or (per-task mode) task blockIdx.y alone
+  const int t0 = a.per_task ? (int)blockIdx.y : 0, nt = a.per_task ? 1 : a.tasks;
+  if (a.per_task) result += (long long)t0 * a.result_stride;
   // ---- range 1: the inner (fast-weight) tensors, walked in the INTERNAL order so that the per-task reads are coalesced
   // (the reference layout is a transposition of it: [F][C][3][3] vs [tap][c][f]); one scattered 4-byte store per element
   if ((long long)blockIdx.x < nb1) {
@@ -231,7 +236,7 @@ __device__ __forceinline__ void export_body(const ExportArgs& a, float* __restri
     const long long mi = internal_to_meta(pl, gid, &seg);
     double val = 0.0;
     if (a.training)
-      for (int t = 0; t < a.tasks; ++t) val += (double)a.tbar[(long long)t * a.task_stride + gid];
+      for (int t = t0; t < t0 + nt; ++t) val += (double)a.tbar[(long long)t * a.task_stride + gid];
     result[mi] = (float)(val * invB);
     return;
   }
@@ -253,8 +258,8 @@ __device__ __forceinline__ void export_body(const ExportArgs& a, float* __restri
       const int f = (int)(rel % pl.F), s_sel = (int)(rel / pl.F), which = is_gamma ? 1 : 0;
       const int per = pl.per_step_bn ? 1 : a.num_steps;               // steps that feed this entry
       if (!pl.per_step_bn || s_sel < a.num_steps) {
-        for (int k = lane; k < a.tasks * per; k += 32) {
-          const int t = k / per, s = pl.per_step_bn ? s_sel : k - t * per;
+        for (int k = lane; k < nt * per; k += 32) {
+          const int tk = k / per, t = t0 + tk, s = pl.per_step_bn ? s_sel : k - tk * per;
           val += stat_ptr(a, t, PASS_TGT_BWD, s, l)[f * 2 + which];
           val -= stat_ptr(a, t, PASS_TAN_BWD, s, l)[f * 2 + which];
         }
@@ -264,16 +269,16 @@ __device__ __forceinline__ void export_body(const ExportArgs& a, float* __restri
     const int seg = (int)(e / (pl.S + 1)), s = (int)(e % (pl.S + 1));
     dst = pl.m_lslr + e;
     if (a.training && s < a.num_steps)
-      for (int t = lane; t < a.tasks; t += 32) val += a.abar[((long long)t * pl.nseg_inner + seg) * MAML_MAX_STEPS + s];
+      for (int t = t0 + lane; t < t0 + nt; t += 32) val += a.abar[((long long)t * pl.nseg_inner + seg) * MAML_MAX_STEPS + s];
   } else if ((e -= E_lslr) < 2) {
     dst = pl.meta_size + e;
     if (e == 0) {
-      for (int k = lane; k < a.tasks * a.num_steps; k += 32) {
-        const int t = k / a.num_steps, s = k - t * a.num_steps;
+      for (int k = lane; k < nt * a.num_steps; k += 32) {
+        const int tk = k / a.num_steps, t = t0 + tk, s = k - tk * a.num_steps;
         if (a.target_mask & (1u << s)) val += (double)a.weights[s] * (double)a.losses[(long long)t * MAML_MAX_STEPS + s];
       }
     } else {
-      for (int t = lane; t < a.tasks; t += 32) val += (double)a.correct[t];
+      for (int t = t0 + lane; t < t0 + nt; t += 32) val += (double)a.correct[t];
       scale = 1.0;
     }
   } else if ((e -= 2) < E_run) {
@@ -293,8 +298,8 @@ __device__ __forceinline__ void export_body(const ExportArgs& a, float* __restri
       const bool has_t = (a.target_mask >> s) & 1u;
       const int c = has_t ? 2 : 1;
       const int U = c * a.tasks_global;
-      for (int kk = lane; kk < a.tasks * c; kk += 32) {
-        const int t = kk / c, j = kk - t * c;
+      for (int kk = lane; kk < nt * c; kk += 32) {
+        const int tk = kk / c, t = t0 + tk, j = kk - tk * c;
         const int k = c * (a.task_offset + t) + j;
         const double wgt = 0.1 * pow(0.9, (double)(U - 1 - k));
         const double* sp = stat_ptr(a, t, j == 0 ? PASS_SUP_FWD : PASS_TGT_FWD, s, l);
@@ -321,7 +326,7 @@ void launch_export(const ExportArgs& a, cudaStream_t st) {
   const long long bnsz = (long long)(pl.per_step_bn ? pl.S : 1) * pl.F;
   const long long entries = 2LL * pl.L * bnsz + (long long)pl.nseg_inner * (pl.S + 1) + 2 + (pl.per_step_bn ? 2LL * pl.L * pl.S * pl.F : 0);
   const long long blocks = (pl.P + 255) / 256 + (entries + 7) / 8;        // range 1: thread per element; range 2: warp per entry
-  launch_pdl(export_kernel, dim3((unsigned)blocks), dim3(256), (size_t)(0), st, tagged(a));
+  launch_pdl(export_kernel, dim3((unsigned)blocks, a.per_task ? (unsigned)a.tasks : 1u), dim3(256), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();
 }
 

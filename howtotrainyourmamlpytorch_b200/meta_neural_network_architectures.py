@@ -14,6 +14,8 @@ Initialisation restates reference ``:62-66`` (xavier_uniform_ conv weight, zero 
 ``:114-118`` (xavier_uniform_ linear weights), ``:177-192`` (running_mean zeros; running_var ones
 per-step but ZEROS in shared mode; beta zeros; gamma ones).
 """
+import itertools
+
 import torch
 import torch.autograd.forward_ad as fwAD
 import torch.nn as nn
@@ -123,12 +125,15 @@ class VGGReLUNormNetwork(nn.Module):
             out.append(fast.get(n, own[n]))
         return out
 
-    def _handles(self, x):
-        """The operator's engine handles for x's batch size and device (``_OperatorHandles``), created on first use."""
+    def _handles(self, x, spec=None):
+        """The operator's engine handles for x's batch size, device and number of tasks (``spec``: None = one batch, else
+        a ``_Tasks``; x then may carry a leading task dim), created on first use.  Each task count torch.func.vmap runs
+        with keeps handles sized for it; ``vmap(..., chunk_size=)`` bounds that count, and with it the memory."""
         cache = self.__dict__.setdefault("_operator_handles", {})
-        key = (int(x.shape[0]), x.device.index)
+        tasks = 1 if spec is None else spec.B
+        key = (int(x.shape[-4]), x.device.index) + ((tasks,) if tasks > 1 else ())
         if key not in cache:
-            cache[key] = _OperatorHandles(self, x)
+            cache[key] = _OperatorHandles(self, x, tasks)
         return cache[key]
 
     def forward(self, x, num_step, params=None, training=False, backup_running_statistics=False):
@@ -149,7 +154,15 @@ class VGGReLUNormNetwork(nn.Module):
         (``maml_b200_net_input_grad``), and with ``create_graph=True`` the weight gradients are differentiable w.r.t. ``x``
         (``maml_b200_net_hvp_input_grad``: the mixed term an outer loss needs to reach support images through the inner
         loop); the image gradient itself is not differentiable again.  With ``x`` not requiring grad none of this runs.
-        The batch size must be a multiple of the number of classes (episode shaped)."""
+        The batch size must be a multiple of the number of classes (episode shaped).
+
+        ``torch.func`` transforms work too: ``grad`` / ``vjp`` / ``jacrev`` (up to second order) and ``vmap`` over tasks,
+        which runs the B mapped calls as ONE engine call with n_tasks = B (``maml_b200_net_*_tasks``) -- images, fast
+        weights and upstream cotangents may each be batched or shared.  BatchNorm gamma / beta stay shared by the tasks (a
+        batched gamma / beta raises NotImplementedError), as do ``torch.func.jvp`` / ``jacfwd`` / ``hessian`` (forward
+        mode runs through ``torch.autograd.forward_ad``) and third order.  A vmapped forward leaves the EMA of its B
+        batches in task order, so a vmapped inner loop updates the running statistics step-major (every task's support
+        pass at step s, then every target pass), not task-major as the reference's loop over tasks does."""
         from . import _native
         if x.device.type != "cuda":
             raise _native.NativeLibraryError("VGGReLUNormNetwork.forward needs a CUDA (sm_90a) device: no CPU fallback")
@@ -157,7 +170,7 @@ class VGGReLUNormNetwork(nn.Module):
         if n % self.num_output_classes != 0:
             raise ValueError("batch size %d is not a multiple of num_output_classes %d" % (n, self.num_output_classes))
         tensors = self._segment_tensors(params)
-        return _FunctionalForward.apply(self, x, int(num_step), *tensors)
+        return _FunctionalForward.apply(self, None, x, int(num_step), *tensors)
 
     def zero_grad(self, params=None):
         """Reference :662-677: clears the gradients of ``params`` (or of the module's own parameters)."""
@@ -181,52 +194,144 @@ def _f32(t):
     return t.detach().to(torch.float32).contiguous()
 
 
-def _fill(eng, meta_like, tensors, v_like=None, directions=None):
-    """meta_like <- the tensors and, with v_like, v_like <- the directions (None: zero) in the engine's meta layout."""
+class _Tasks:
+    """B independent problems run as ONE engine call (what ``torch.func.vmap`` over the operator becomes): which operands
+    carry a leading task dim (the others are shared by every task).  Every output of a call with a ``_Tasks`` is per task
+    ([B, ...]); a node's backward sums the per-task gradients of a shared operand."""
+
+    def __init__(self, B, x, tensors, directions=()):
+        self.B, self.x = int(B), bool(x)
+        self.tensors, self.directions = tuple(bool(b) for b in tensors), tuple(bool(b) for b in directions)
+
+
+class _Needs:
+    """Which of d/dx, d/d(dlogits) and the per-tensor d/dtheta a ``_FunctionalHvp`` call computes."""
+
+    def __init__(self, x, dl, tensors):
+        self.x, self.dl, self.tensors = bool(x), bool(dl), tuple(bool(b) for b in tensors)
+
+
+# every engine forward of the operator gets a number, so that a backward can tell whether its forward's activations are
+# still the ones a handle holds (and replay the forward first if not)
+_FORWARDS = itertools.count(1)
+
+
+def _batched(spec, n):
+    return spec.tensors if spec is not None else (False,) * n
+
+
+def _images(x, spec, B):
+    """x as the engine reads it: [B, n, C, H, W] float32 (a shared batch copied per task) or, without spec, [n, C, H, W]."""
+    return _f32(x if spec is None or spec.x else x.expand(B, *x.shape))
+
+
+def _fill(eng, buf, tensors, batched):
+    """buf[t] <- task t's tensors (None: zeros) in the engine's meta layout.  With no tensor batched only row 0 is
+    written and every task reads it (task stride 0); a shared tensor among batched ones is broadcast into every row.
+    Returns the task stride in floats."""
+    stride = eng.meta_size if any(batched) else 0
+    rows = buf if stride else buf[:1]
     with torch.no_grad():
-        if v_like is not None:
-            v_like.zero_()
-        for (off, size), t, d in zip(eng.segments, tensors, directions or [None] * len(tensors)):
-            meta_like[off:off + size].copy_(t.detach().reshape(-1).to(torch.float32))
-            if d is not None:
-                v_like[off:off + size].copy_(d.detach().reshape(-1).to(torch.float32))
+        for (off, size), t, b in zip(eng.segments, tensors, batched):
+            if t is None:
+                rows[:, off:off + size].zero_()
+            else:
+                rows[:, off:off + size].copy_(t.detach().reshape(rows.shape[0] if b else 1, size).to(torch.float32))
+    return stride
 
 
-def _unpack(eng, buf, tensors, needs, cast=False):
-    """A meta-layout buffer cut into per-tensor copies (None where not needed), in each tensor's dtype when `cast`."""
-    return [buf[off:off + size].view(t.shape).to(t.dtype if cast else buf.dtype, copy=True) if need else None
-            for (off, size), t, need in zip(eng.segments, tensors, needs)]
+def _unpack(eng, buf, tensors, needs, spec, cast=False):
+    """Per-tensor copies of an engine result buffer [B, result_size] (None where not needed): [B, *shape] per task with a
+    spec, the tensor's own shape without; in each tensor's dtype when `cast`."""
+    out = []
+    for (off, size), t, need, b in zip(eng.segments, tensors, needs, _batched(spec, len(tensors))):
+        if not need:
+            out.append(None)
+            continue
+        v = buf[0, off:off + size].view(t.shape) if spec is None else buf[:, off:off + size].view(-1, *t.shape[int(b):])
+        out.append(v.to(t.dtype if cast else buf.dtype, copy=True))
+    return out
 
 
-def _image_buffer(buf, x):
-    """`buf`, or on first use an engine output buffer for the image gradient of x (one batch)."""
-    return buf if buf is not None else torch.empty((1,) + tuple(x.shape), dtype=torch.float32, device=x.device)
+def _image_buffer(buf, x, B):
+    """`buf`, or on first use an engine output buffer for the image gradients of B batches shaped like x's."""
+    return buf if buf is not None else torch.empty((B,) + tuple(x.shape[-4:]), dtype=torch.float32, device=x.device)
 
 
 def _add(a, b):
     return a if b is None else b if a is None else a + b
 
 
+def _per_task(t, batched, B):
+    """t with a leading task dim: itself when batched, else a stride-0 view."""
+    return t if batched else t.unsqueeze(0).expand(B, *t.shape)
+
+
+def _to_front(t, dim):
+    return t if t is None or dim is None else t.movedim(dim, 0)
+
+
+def _shared_sum(g, batched):
+    """The gradient of an operand from per-task gradients g [B, ...]: g itself if the operand is batched, else (shared by
+    the tasks) their sum."""
+    return g if g is None or batched else g.sum(0)
+
+
+def _refuse_nested(spec):
+    if spec is not None:
+        raise NotImplementedError("nested torch.func.vmap over the functional network operator is not supported: the "
+                                  "engine has one task dimension (flatten the task dims into one vmap)")
+
+
+def _refuse_batched_bn(net, dims):
+    for i, d in enumerate(dims[:4 * net.num_stages]):
+        if d is not None and i % 4 >= 2:
+            raise NotImplementedError(
+                "a BatchNorm gamma / beta batched under torch.func.vmap: the engine shares gamma / beta between the tasks "
+                "of a call (per-task gamma / beta are inner-loop BatchNorm parameters, "
+                "enable_inner_loop_optimizable_bn_params, which are outside the accelerated path)")
+
+
+def _refuse_functorch_jvp(ctx, *tensors):
+    if getattr(ctx, "spec", None) is not None or any(
+            isinstance(t, torch.Tensor) and torch._C._functorch.is_functorch_wrapped_tensor(t)
+            for t in tuple(ctx.saved_tensors) + tensors):
+        raise NotImplementedError(
+            "torch.func.jvp / jacfwd / hessian through the functional network operator are not supported: its forward "
+            "mode runs through torch.autograd.forward_ad (fwAD.dual_level / make_dual), and reverse mode through "
+            "torch.func.grad / vjp / jacrev")
+
+
+def _refuse_third_order():
+    raise NotImplementedError("third-order derivatives of the functional network operator are not supported (the "
+                              "engine differentiates its backward once: second-order MAML)")
+
+
 class _OperatorHandles:
-    """The engine handles behind ``VGGReLUNormNetwork.forward`` for one batch size on one device, one method per use.
+    """The engine handles behind ``VGGReLUNormNetwork.forward`` for one batch size, device and task count B (1, or the
+    batch size of a ``torch.func.vmap`` over tasks), one method per use.
 
-    The first-order handle holds the batch as its target pass (``maml_b200_net_forward`` / ``net_backward`` /
-    ``net_input_grad``, the running-statistics update).  It keeps the activations of its LAST forward only: ``gen`` counts
-    its forwards, so that a backward of an older forward replays it first.  The second-order handle, created on first use,
-    holds the batch as its SUPPORT pass, the buffers the tangent pass runs on (``net_hvp_image`` /
-    ``net_hvp_input_grad`` / ``net_jvp``): a model that is only differentiated once pays nothing for it."""
+    The first-order handle holds the batch as its target pass (``maml_b200_net_forward_tasks`` / ``net_backward_tasks``
+    / ``net_input_grad``, the running-statistics update).  It keeps the activations of its LAST forward only: ``token``
+    names that forward, so that a backward of another one replays its own first (``gen`` counts the forwards it ran).  The second-order handle, created on first
+    use, holds the batch as its SUPPORT pass, the buffers the tangent pass runs on (``net_hvp_image_tasks`` /
+    ``net_hvp_input_grad`` / ``net_jvp``): a model that is only differentiated once pays nothing for it.  Every call runs
+    the per-task entries with per-task results; for B = 1 and shared weights they compute what ``net_forward`` /
+    ``net_backward`` / ``net_hvp_image`` do, bit for bit."""
 
-    def __init__(self, net, x):
+    def __init__(self, net, x, tasks):
         a = net.args
-        self.n, self.N, self.device = int(x.shape[0]), net.num_output_classes, x.device
-        self.cfg = dict(n_way=self.N, channels=int(x.shape[1]), height=int(x.shape[2]), width=int(x.shape[3]),
+        self.B = int(tasks)
+        self.n, self.N, self.device = int(x.shape[-4]), net.num_output_classes, x.device
+        self.cfg = dict(n_way=self.N, channels=int(x.shape[-3]), height=int(x.shape[-2]), width=int(x.shape[-1]),
                         filters=net.cnn_filters, num_stages=net.num_stages, inner_steps=int(a.number_of_training_steps_per_iter),
-                        per_step_bn=bool(a.per_step_bn_statistics), max_tasks=1)
+                        per_step_bn=bool(a.per_step_bn_statistics), max_tasks=self.B)
         self.first_order = eng = self._engine(k_shot=1, t_target=self.n // self.N)
-        self.gen = 0
-        self.meta = torch.zeros(eng.meta_size, dtype=torch.float32, device=self.device)
-        self.logits = torch.empty(1, self.n, self.N, dtype=torch.float32, device=self.device)
-        self.grad = torch.zeros(eng.result_size, dtype=torch.float32, device=self.device)
+        self.token, self.gen = None, 0
+        self.meta = torch.zeros(self.B, eng.meta_size, dtype=torch.float32, device=self.device)
+        self.meta_stride = 0
+        self.logits = torch.empty(self.B, self.n, self.N, dtype=torch.float32, device=self.device)
+        self.grad = torch.zeros(self.B, eng.result_size, dtype=torch.float32, device=self.device)
         S = int(a.number_of_training_steps_per_iter) if a.per_step_bn_statistics else 1
         self.run = torch.zeros(2, net.num_stages, S, net.cnn_filters, dtype=torch.float32, device=self.device)
         self.dx = self.second_order = self.dxdot = None
@@ -239,93 +344,113 @@ class _OperatorHandles:
     def _second(self):
         if self.second_order is None:
             eng = self._engine(k_shot=self.n // self.N, t_target=1)
-            self.meta2 = torch.zeros(eng.meta_size, dtype=torch.float32, device=self.device)
-            self.v = torch.zeros(eng.meta_size, dtype=torch.float32, device=self.device)
-            self.jv = torch.empty(1, self.n, self.N, dtype=torch.float32, device=self.device)
-            self.hv = torch.zeros(eng.result_size, dtype=torch.float32, device=self.device)
+            self.meta2 = torch.zeros(self.B, eng.meta_size, dtype=torch.float32, device=self.device)
+            self.v = torch.zeros(self.B, eng.meta_size, dtype=torch.float32, device=self.device)
+            self.jv = torch.empty(self.B, self.n, self.N, dtype=torch.float32, device=self.device)
+            self.hv = torch.zeros(self.B, eng.result_size, dtype=torch.float32, device=self.device)
             self.second_order = eng
         return self.second_order
 
-    def forward(self, net, x, num_step, tensors):
-        """The logits (``net_forward``), and F.batch_norm's EMA of net's running statistics at num_step (per-step
-        BatchNorm only)."""
+    def _out(self, buf, spec, dtype=None):
+        """An engine output [B, ...] as the caller's copy: per task with a spec, else batch 0's."""
+        return (buf if spec is not None else buf[0]).to(dtype or buf.dtype, copy=True)
+
+    def _run_forward(self, spec, x, num_step, tensors):
         eng = self.first_order
-        _fill(eng, self.meta, tensors)
+        self.meta_stride = _fill(eng, self.meta, tensors, _batched(spec, len(tensors)))
+        eng.net_forward_tasks(self.B, num_step, self.meta, self.meta_stride, _images(x, spec, self.B), self.logits)
+        self.gen += 1
+
+    def forward(self, net, spec, x, num_step, tensors):
+        """The logits (``net_forward_tasks``), and F.batch_norm's EMA of net's running statistics at num_step from the B
+        batches in task order (per-step BatchNorm only)."""
+        eng = self.first_order
         with torch.cuda.device(self.device):
-            eng.net_forward(1, num_step, self.meta, _f32(x), self.logits)
+            self._run_forward(spec, x, num_step, tensors)
             if net.args.per_step_bn_statistics:
                 bns = [net.layer_dict["conv%d" % l].norm_layer for l in range(net.num_stages)]
                 with torch.no_grad():
                     for l, bn in enumerate(bns):
                         self.run[0, l].copy_(bn.running_mean.data)
                         self.run[1, l].copy_(bn.running_var.data)
-                    eng.net_running_update(1, num_step, self.run[0], self.run[1])
+                    eng.net_running_update(self.B, num_step, self.run[0], self.run[1])
                     for l, bn in enumerate(bns):
                         bn.running_mean.data.copy_(self.run[0, l])
                         bn.running_var.data.copy_(self.run[1, l])
-        self.gen += 1
-        return self.logits[0].clone()
+        self.token = next(_FORWARDS)
+        net.__dict__["_operator_forward"] = self.token
+        return self._out(self.logits, spec)
 
-    def backward(self, fwd_ctx, x, tensors, dl):
-        """J^T dl (``net_backward``) at the forward of ``fwd_ctx``, replayed first when another forward of this shape ran
-        since (the replay has no EMA side effect), and J_x^T dl (``net_input_grad``) when x requires grad.  Returns (dx or
-        None, the per-tensor gradients in float32, None where not needed)."""
-        eng, num_step = self.first_order, fwd_ctx.num_step
+    def backward(self, token, num_step, spec, x, tensors, dl, need_x, needs):
+        """J^T dl (``net_backward_tasks``) at the forward named `token`, replayed first when this handle's last forward was
+        another one (the replay has no EMA side effect), and J_x^T dl (``net_input_grad``) when need_x.  Returns (dx or
+        None, the per-tensor gradients in float32, None where not needed), per task with a spec."""
+        eng = self.first_order
         with torch.no_grad(), torch.cuda.device(self.device):
-            if self.gen != fwd_ctx.gen:
-                _fill(eng, self.meta, tensors)
-                eng.net_forward(1, num_step, self.meta, _f32(x), self.logits)
-                self.gen += 1
-                fwd_ctx.gen = self.gen
-            eng.net_backward(1, num_step, self.meta, _f32(dl).view(1, *dl.shape), self.grad)
+            if self.token != token:
+                self._run_forward(spec, x, num_step, tensors)
+                self.token = token
+            eng.net_backward_tasks(self.B, num_step, self.meta, self.meta_stride, _f32(dl).view(self.B, self.n, self.N),
+                                   self.grad)
             dx = None
-            if fwd_ctx.needs_input_grad[1]:
-                self.dx = _image_buffer(self.dx, x)
-                eng.net_input_grad(1, self.dx)
-                dx = self.dx[0].to(x.dtype, copy=True)
-            return dx, _unpack(eng, self.grad, tensors, fwd_ctx.needs_input_grad[3:])
+            if need_x:
+                self.dx = _image_buffer(self.dx, x, self.B)
+                eng.net_input_grad(self.B, self.dx)
+                dx = self._out(self.dx, spec, x.dtype)
+            return dx, _unpack(eng, self.grad, tensors, needs, spec)
 
-    def hvp(self, num_step, x, xdot, dlogits, tensors, directions, need_x, needs, cast=False):
-        """Along the weight directions and the image tangent xdot (None: none; then this is ``net_hvp``): J v and
-        d/dtheta <dlogits, J v> (``net_hvp_image``), and d/dx <dlogits, J v> (``net_hvp_input_grad``) when need_x.  Returns
-        (d/dx or None, J v as float32 [n, N], the per-tensor d/dtheta as by ``_unpack(..., needs, cast)``)."""
+    def hvp(self, num_step, spec, x, xdot, dlogits, tensors, directions, need_x, needs, cast=False):
+        """Along the weight directions and the image tangent xdot (None: none): J v and d/dtheta <dlogits, J v>
+        (``net_hvp_image_tasks``), and d/dx <dlogits, J v> (``net_hvp_input_grad``) when need_x.  Returns (d/dx or None,
+        J v as float32 [(B,) n, N], the per-tensor d/dtheta as by ``_unpack(..., needs, spec, cast)``)."""
         eng = self._second()
-        _fill(eng, self.meta2, tensors, self.v, directions)
+        dirs = spec.directions if spec is not None else (False,) * len(directions)
+        ms = _fill(eng, self.meta2, tensors, _batched(spec, len(tensors)))
+        ds = _fill(eng, self.v, directions, dirs)
         with torch.cuda.device(self.device):
-            eng.net_hvp_image(1, num_step, self.meta2, _f32(x), None if xdot is None else _f32(xdot),
-                              _f32(dlogits).view(1, *dlogits.shape), self.v, self.jv, self.hv)
+            eng.net_hvp_image_tasks(self.B, num_step, self.meta2, ms, _images(x, spec, self.B),
+                                    None if xdot is None else _f32(xdot), _f32(dlogits).view(self.B, self.n, self.N),
+                                    self.v, ds, self.jv, self.hv)
             d_x = None
             if need_x:
-                self.dxdot = _image_buffer(self.dxdot, x)
-                eng.net_hvp_input_grad(1, self.dxdot)
-                d_x = self.dxdot[0].to(x.dtype, copy=True)
-        return d_x, self.jv[0], _unpack(eng, self.hv, tensors, needs, cast)
+                self.dxdot = _image_buffer(self.dxdot, x, self.B)
+                eng.net_hvp_input_grad(self.B, self.dxdot)
+                d_x = self._out(self.dxdot, spec, x.dtype)
+        return d_x, (self.jv if spec is not None else self.jv[0]), _unpack(eng, self.hv, tensors, needs, spec, cast)
 
     def jvp(self, num_step, x, xdot, tensors, tangents):
-        """The logits tangent J_theta t + J_x xdot (``net_jvp``; xdot may be None)."""
+        """The logits tangent J_theta t + J_x xdot (``net_jvp``; xdot may be None; one batch)."""
         eng = self._second()
-        _fill(eng, self.meta2, tensors, self.v, tangents)
+        _fill(eng, self.meta2, tensors, (False,) * len(tensors))
+        _fill(eng, self.v, tangents, (False,) * len(tangents))
         with torch.cuda.device(self.device):
             eng.net_jvp(1, num_step, self.meta2, _f32(x), self.v, None if xdot is None else _f32(xdot), self.jv)
         return self.jv[0].clone()
 
 
 class _FunctionalForward(torch.autograd.Function):
-    """``VGGReLUNormNetwork.forward`` as an autograd node: forward = ``maml_b200_net_forward``, backward =
-    ``_FunctionalBackward`` (``maml_b200_net_backward``: head backward for an external d(logits), BatchNorm / pool / leaky-ReLU
-    backward, dgrad and wgrad kernels of the engine), itself differentiable once more.  The engine keeps the activations of
-    its LAST forward only, so a backward that arrives after another forward of the same shape first replays its own forward
-    (cheap) -- correctness does not depend on the call order."""
+    """``VGGReLUNormNetwork.forward`` as an autograd node: forward = ``maml_b200_net_forward_tasks``, backward =
+    ``_FunctionalBackward`` (``maml_b200_net_backward_tasks``: head backward for an external d(logits), BatchNorm / pool /
+    leaky-ReLU backward, dgrad and wgrad kernels of the engine), itself differentiable once more.  The engine keeps the
+    activations of its LAST forward only, so a backward that arrives after another forward of the same shape first replays
+    its own forward (cheap) -- correctness does not depend on the call order.
+
+    ``spec`` is None for one batch, or a ``_Tasks`` when the ``vmap`` rule below runs B mapped calls as one: the rule moves
+    the batch dims to the front and calls this node again with the spec at the level below, so that the levels above
+    (an outer ``torch.autograd`` or ``torch.func.grad``) see a graph.  In ``setup_context`` form for ``torch.func``."""
 
     @staticmethod
-    def forward(ctx, net, x, num_step, *tensors):
-        ops = net._handles(x)
-        logits = ops.forward(net, x, num_step, tensors)
-        ctx.net, ctx.ops, ctx.num_step, ctx.gen = net, ops, num_step, ops.gen
+    def forward(net, spec, x, num_step, *tensors):
+        return net._handles(x, spec).forward(net, spec, x, num_step, tensors)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        net, spec, x, num_step, *tensors = inputs
+        # the forward that produced `output` ran last: a torch.func level calls this right after it
+        ctx.net, ctx.spec, ctx.num_step, ctx.token = net, spec, num_step, net.__dict__["_operator_forward"]
         # x and the weights themselves: a double backward differentiates w.r.t. them, forward mode at them
         ctx.save_for_backward(x, *tensors)
         ctx.save_for_forward(x, *tensors)
-        return logits
 
     @staticmethod
     def backward(ctx, dlogits):
@@ -337,15 +462,29 @@ class _FunctionalForward(torch.autograd.Function):
                     "tangent directions in the backward tangent pass, which the engine does not implement (BatchNorm "
                     "parameters as inner-loop fast weights, enable_inner_loop_optimizable_bn_params, are outside the "
                     "accelerated path)")
-        out = _FunctionalBackward.apply(ctx, x, dlogits, *tensors)
-        return (None, out[0], None) + tuple(out[1:])
+        out = _FunctionalBackward.apply(ctx, ctx.spec, x, dlogits, *tensors)
+        if ctx.spec is not None:
+            out = [_shared_sum(o, b) for o, b in zip(out, (ctx.spec.x,) + ctx.spec.tensors)]
+        return (None, None, out[0], None) + tuple(out[1:])
 
     @staticmethod
-    def jvp(ctx, _net_t, x_t, _step_t, *tangents):
+    def jvp(ctx, _net_t, _spec_t, x_t, _step_t, *tangents):
         """Forward mode (``torch.autograd.forward_ad``): the logits tangent J_theta t + J_x x_t through
         ``maml_b200_net_jvp`` on the second-order handle -- one primal forward and one tangent forward.  Tangents may sit
         on the images, the conv / linear weights and the BatchNorm gamma / beta."""
-        return ctx.ops.jvp(ctx.num_step, ctx.saved_tensors[0], x_t, ctx.saved_tensors[1:], tangents)
+        _refuse_functorch_jvp(ctx, x_t, *tangents)
+        x = ctx.saved_tensors[0]
+        return ctx.net._handles(x).jvp(ctx.num_step, x, x_t, ctx.saved_tensors[1:], tangents)
+
+    @staticmethod
+    def vmap(info, in_dims, net, spec, x, num_step, *tensors):
+        _refuse_nested(spec)
+        dims = in_dims[4:]
+        _refuse_batched_bn(net, dims)
+        spec = _Tasks(info.batch_size, in_dims[2] is not None, [d is not None for d in dims])
+        logits = _FunctionalForward.apply(net, spec, _to_front(x, in_dims[2]), num_step,
+                                          *[_to_front(t, d) for t, d in zip(tensors, dims)])
+        return logits, 0
 
 
 class _FunctionalBackward(torch.autograd.Function):
@@ -353,51 +492,54 @@ class _FunctionalBackward(torch.autograd.Function):
     create_graph=True)`` of a loss on the operator's logits can be differentiated again (second-order MAML, reference
     few_shot_learning_system.py:138-139 and the outer ``loss.backward()``).
 
-    forward  = ``maml_b200_net_backward``: B(dl, theta) = J^T dl for every tensor (conv / linear, BatchNorm gamma / beta of
-               ``num_step``), and -- only when x requires grad -- ``maml_b200_net_input_grad``: J_x^T dl (else None).  With
-               grad mode off this is the whole first-order backward.
-    backward = ``maml_b200_net_hvp`` along the cotangents v of the conv / linear gradients: one forward-over-reverse pass with
-               dl held constant gives J v (the cotangent of dl) and d/dtheta <dl, J v> (that of every tensor); when x
-               requires grad, ``maml_b200_net_hvp_input_grad`` on the same handle gives d/dx <dl, J v> (that of x).  torch
-               carries J v on through the loss's own double backward.  Third order is not supported.
+    forward  = ``maml_b200_net_backward_tasks``: B(dl, theta) = J^T dl for every tensor (conv / linear, BatchNorm gamma /
+               beta of ``num_step``), and -- only when x requires grad -- ``maml_b200_net_input_grad``: J_x^T dl (else
+               None).  With grad mode off this is the whole first-order backward.
+    backward = ``_FunctionalHvp`` along the cotangents v of the conv / linear gradients.  Third order is not supported.
     A cotangent on a BatchNorm gamma / beta GRADIENT would need gamma / beta tangent directions, and one on the image
     gradient dx would need image tangent directions (the first conv's tangent driven by x-dot); the engine's tangent pass
     has neither: both are refused (the first only arises when BatchNorm parameters are inner-loop fast weights,
     enable_inner_loop_optimizable_bn_params, which the network refuses too; the second e.g. for a penalty on the image
-    gradient's norm that is differentiated again)."""
+    gradient's norm that is differentiated again).  ``spec`` and the ``vmap`` rule as in ``_FunctionalForward``; with a
+    spec, dlogits is [B, n, N] and every gradient is per task."""
 
     @staticmethod
-    def forward(ctx, fwd_ctx, x, dlogits, *tensors):
-        dx, grads = fwd_ctx.ops.backward(fwd_ctx, x, tensors, dlogits)
-        ctx.set_materialize_grads(False)
-        ctx.fwd_ctx = fwd_ctx
-        ctx.save_for_backward(x, dlogits, *tensors)
-        ctx.save_for_forward(x, dlogits, *tensors)
+    def forward(fwd_ctx, spec, x, dlogits, *tensors):
+        need = fwd_ctx.needs_input_grad
+        dx, grads = fwd_ctx.net._handles(x, spec).backward(fwd_ctx.token, fwd_ctx.num_step, spec, x, tensors, dlogits,
+                                                           need[2], need[4:])
         return (dx,) + tuple(grads)
 
     @staticmethod
-    def jvp(ctx, _fwd_ctx_t, x_t, dl_t, *tangents):
-        """Forward-over-reverse: the tangent of every gradient this node returned, along (x_t, dl_t, tangents).  For a
-        weight gradient J_theta^T dl_t + d/dtheta <dl, J_theta t + J_x x_t>; for dx the same with d/dx.  The first term is
-        ``maml_b200_net_backward`` (+ ``net_input_grad``) of dl_t on the first-order handle, the second
-        ``maml_b200_net_hvp_image`` (+ ``net_hvp_input_grad``) on the second-order handle; a term whose tangents are all
-        None is skipped.  A tangent on a BatchNorm gamma / beta input never gets here: ``_FunctionalForward.backward``
-        refuses it before this node runs."""
-        fwd_ctx = ctx.fwd_ctx
-        x, dlogits, tensors = ctx.saved_tensors[0], ctx.saved_tensors[1], ctx.saved_tensors[2:]
-        need_x = fwd_ctx.needs_input_grad[1]
-        dx_t, grads_t = None, [None] * len(tensors)
-        if dl_t is not None:                              # J^T dl_t on the first-order handle
-            dx_t, grads_t = fwd_ctx.ops.backward(fwd_ctx, x, tensors, dl_t)
-        if x_t is not None or any(t is not None for t in tangents):    # d/d(theta, x) <dl, J_theta t + J_x x_t>
-            d_x, _, hv = fwd_ctx.ops.hvp(fwd_ctx.num_step, x, x_t, dlogits, tensors, tangents, need_x,
-                                         fwd_ctx.needs_input_grad[3:])
-            dx_t = _add(dx_t, d_x)
-            grads_t = [_add(g, h) for g, h in zip(grads_t, hv)]
-        return (dx_t if need_x else None,) + tuple(grads_t)
+    def setup_context(ctx, inputs, output):
+        fwd_ctx, spec, x, dlogits, *tensors = inputs
+        ctx.set_materialize_grads(False)
+        ctx.fwd_ctx, ctx.spec = fwd_ctx, spec
+        ctx.save_for_backward(x, dlogits, *tensors)
+        ctx.save_for_forward(x, dlogits, *tensors)
 
     @staticmethod
-    @torch.autograd.function.once_differentiable
+    def jvp(ctx, _fwd_ctx_t, _spec_t, x_t, dl_t, *tangents):
+        """Forward-over-reverse: the tangent of every gradient this node returned, along (x_t, dl_t, tangents).  For a
+        weight gradient J_theta^T dl_t + d/dtheta <dl, J_theta t + J_x x_t>; for dx the same with d/dx.  The first term is
+        ``maml_b200_net_backward_tasks`` (+ ``net_input_grad``) of dl_t on the first-order handle, the second
+        ``maml_b200_net_hvp_image_tasks`` (+ ``net_hvp_input_grad``) on the second-order handle; a term whose tangents are
+        all None is skipped.  A tangent on a BatchNorm gamma / beta input never gets here: ``_FunctionalForward.backward``
+        refuses it before this node runs."""
+        _refuse_functorch_jvp(ctx, x_t, dl_t, *tangents)
+        fwd_ctx = ctx.fwd_ctx
+        x, dlogits, tensors = ctx.saved_tensors[0], ctx.saved_tensors[1], ctx.saved_tensors[2:]
+        ops, need = fwd_ctx.net._handles(x), fwd_ctx.needs_input_grad
+        dx_t, grads_t = None, [None] * len(tensors)
+        if dl_t is not None:                              # J^T dl_t on the first-order handle
+            dx_t, grads_t = ops.backward(fwd_ctx.token, fwd_ctx.num_step, None, x, tensors, dl_t, need[2], need[4:])
+        if x_t is not None or any(t is not None for t in tangents):    # d/d(theta, x) <dl, J_theta t + J_x x_t>
+            d_x, _, hv = ops.hvp(fwd_ctx.num_step, None, x, x_t, dlogits, tensors, tangents, need[2], need[4:])
+            dx_t = _add(dx_t, d_x)
+            grads_t = [_add(g, h) for g, h in zip(grads_t, hv)]
+        return (dx_t if need[2] else None,) + tuple(grads_t)
+
+    @staticmethod
     def backward(ctx, dx_cotangent, *cotangents):
         fwd_ctx = ctx.fwd_ctx
         x, dlogits, tensors = ctx.saved_tensors[0], ctx.saved_tensors[1], ctx.saved_tensors[2:]
@@ -412,8 +554,61 @@ class _FunctionalBackward(torch.autograd.Function):
                     "directions, which the engine does not implement (BatchNorm parameters as inner-loop fast weights, "
                     "enable_inner_loop_optimizable_bn_params, are outside the accelerated path)")
         if all(c is None for c in cotangents):
-            return (None,) * (3 + len(tensors))
-        d_x, jv, hv = fwd_ctx.ops.hvp(fwd_ctx.num_step, x, None, dlogits, tensors, cotangents, ctx.needs_input_grad[1],
-                                      ctx.needs_input_grad[3:], cast=True)
-        d_dlogits = jv.to(dlogits.dtype).clone() if ctx.needs_input_grad[2] else None
-        return (None, d_x, d_dlogits) + tuple(hv)
+            return (None,) * (4 + len(tensors))
+        need = ctx.needs_input_grad
+        spec = ctx.spec
+        if spec is not None:       # the cotangents of per-task gradients are per task
+            spec = _Tasks(spec.B, spec.x, spec.tensors, [True] * len(tensors))
+        out = _FunctionalHvp.apply(fwd_ctx, spec, _Needs(need[2], need[3], need[4:]), x, dlogits, *tensors, *cotangents)
+        if spec is not None:
+            out = [_shared_sum(out[0], spec.x), out[1]] + [_shared_sum(o, b) for o, b in zip(out[2:], spec.tensors)]
+        return (None, None) + tuple(out)
+
+    @staticmethod
+    def vmap(info, in_dims, fwd_ctx, spec, x, dlogits, *tensors):
+        _refuse_nested(spec)
+        dims = in_dims[4:]
+        _refuse_batched_bn(fwd_ctx.net, dims)
+        B = info.batch_size
+        spec = _Tasks(B, in_dims[2] is not None, [d is not None for d in dims])
+        out = _FunctionalBackward.apply(fwd_ctx, spec, _to_front(x, in_dims[2]),
+                                        _per_task(_to_front(dlogits, in_dims[3]), in_dims[3] is not None, B),
+                                        *[_to_front(t, d) for t, d in zip(tensors, dims)])
+        return out, tuple(None if o is None else 0 for o in out)
+
+
+class _FunctionalHvp(torch.autograd.Function):
+    """Backward of ``_FunctionalBackward``: along the cotangents v of the conv / linear gradients,
+    ``maml_b200_net_hvp_image_tasks`` -- one forward-over-reverse pass with dl held constant -- gives J v (the cotangent of
+    dl) and d/dtheta <dl, J v> (that of every tensor); ``maml_b200_net_hvp_input_grad`` on the same handle gives
+    d/dx <dl, J v> (that of x) when ``needs.x``.  torch carries J v on through the loss's own double backward.  A node of its
+    own so that ``torch.func.vmap`` can run it per task; its own backward (third order) is refused."""
+
+    @staticmethod
+    def forward(fwd_ctx, spec, needs, x, dlogits, *tensors_and_directions):
+        k = len(tensors_and_directions) // 2
+        tensors, directions = tensors_and_directions[:k], tensors_and_directions[k:]
+        d_x, jv, hv = fwd_ctx.net._handles(x, spec).hvp(fwd_ctx.num_step, spec, x, None, dlogits, tensors, directions,
+                                                        needs.x, needs.tensors, cast=True)
+        return (d_x, jv.to(dlogits.dtype).clone() if needs.dl else None) + tuple(hv)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        pass
+
+    @staticmethod
+    def backward(ctx, *cotangents):
+        _refuse_third_order()
+
+    @staticmethod
+    def vmap(info, in_dims, fwd_ctx, spec, needs, x, dlogits, *tensors_and_directions):
+        _refuse_nested(spec)
+        k = len(tensors_and_directions) // 2
+        dims = in_dims[5:]
+        _refuse_batched_bn(fwd_ctx.net, dims[:k])
+        B = info.batch_size
+        spec = _Tasks(B, in_dims[3] is not None, [d is not None for d in dims[:k]], [d is not None for d in dims[k:]])
+        out = _FunctionalHvp.apply(fwd_ctx, spec, needs, _to_front(x, in_dims[3]),
+                                   _per_task(_to_front(dlogits, in_dims[4]), in_dims[4] is not None, B),
+                                   *[_to_front(t, d) for t, d in zip(tensors_and_directions, dims)])
+        return out, tuple(None if o is None else 0 for o in out)

@@ -28,7 +28,7 @@ extern "C" {
 
 #define MAML_B200_MAX_STAGES 4
 #define MAML_B200_MAX_STEPS 8
-#define MAML_B200_ABI_VERSION 1
+#define MAML_B200_ABI_VERSION 2
 
 /* Static shape of the path.  Mirrors the args the reference reads on this path:
  * num_classes_per_set, num_samples_per_class, num_target_samples, image_{channels,height,width},
@@ -158,6 +158,27 @@ int maml_b200_net_hvp_image(maml_b200_handle* h, int32_t n_tasks, int32_t num_st
  * buffers (zero d(logits), the image tangent) are allocated by the first call that needs them, outside the workspace. */
 int maml_b200_net_jvp(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
                       const float* t_like, const float* xdot, float* jv_out, void* stream);
+
+/* Per-task forms of net_forward / net_backward / net_hvp_image: n_tasks independent problems in one call, each with its
+ * own weights (what torch.func.vmap over tasks runs as one call).  Same shapes, ordering rules and side effects as the
+ * entries above, plus:
+ *   meta_stride  floats between consecutive tasks' meta_like vectors: task t's conv / linear weights are at
+ *                meta_like + t * meta_stride; 0 = one vector shared by every task (the entries above)
+ *   dir_stride   the same for v_like (0 = shared)
+ *   sum_tasks    1: grad_out / hv_out = result_size floats summed over the tasks (the entries above);
+ *                0: n_tasks x result_size floats, task t's vector (not summed) at + t * result_size
+ * BatchNorm gamma / beta are shared by the tasks of a call: they are read from task 0's vector (meta_like's own rows),
+ * whatever meta_stride is.  A stride that is neither 0 nor >= meta_size is an error.
+ * maml_b200_net_input_grad, maml_b200_net_hvp_input_grad and maml_b200_net_running_update already work per task and follow
+ * these entries as they follow the ones above. */
+int maml_b200_net_forward_tasks(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
+                                int64_t meta_stride, const float* x, float* logits, void* stream);
+int maml_b200_net_backward_tasks(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
+                                 int64_t meta_stride, const float* dlogits, float* grad_out, int32_t sum_tasks, void* stream);
+int maml_b200_net_hvp_image_tasks(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
+                                  int64_t meta_stride, const float* x, const float* xdot, const float* dlogits,
+                                  const float* v_like, int64_t dir_stride, float* jv_out, float* hv_out, int32_t sum_tasks,
+                                  void* stream);
 
 /* Gradients with respect to the images.  Each reads the buffers of the functional call that ran last on this handle and
  * must follow it immediately, with the same n_tasks: another call on the handle in between (a functional call, an

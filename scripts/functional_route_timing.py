@@ -5,9 +5,14 @@ meta-batch 8, second order) three ways, on one GPU:
             update, MSL target losses; then the outer backward) on this repository's VGGReLUNormNetwork.forward
             (integration route B1: engine forward / backward / Hessian-vector product);
   torch     the same loop on torch ops on the GPU (oracle._net_forward: F.conv2d / F.batch_norm / ..., fp32, TF32 off);
-  fused     MAMLFewShotClassifier.run_train_iter (route B0: the whole iteration as one engine call, Adam step included).
+  fused     MAMLFewShotClassifier.run_train_iter (route B0: the whole iteration as one engine call, Adam step included);
+  operator_vmap  the functorch MAML recipe on the operator: torch.func.vmap over the meta-batch, inner torch.func.grad
+            steps with the LSLR update, MSL target losses, outer torch.autograd.grad -- every operator call runs the
+            meta-batch as one engine call (n_tasks = 8);
+  torch_vmap     the same functorch loop on torch ops (oracle._net_forward under vmap); reported as skipped, with the
+            error, if torch.func cannot run it.
 
-Warm-up first; every timed iteration ends in a device synchronise; the three legs alternate within each repeat.  Prints
+Warm-up first; every timed iteration ends in a device synchronise; the legs alternate within each repeat.  Prints
 one JSON line: per leg the median / min / max milliseconds per iteration, plus the GPU name and power limit read in
 the same run.
 
@@ -57,6 +62,36 @@ def reference_loop(net_forward, params, a, batch, epoch, O):
     return torch.autograd.grad(loss, [params[n] for n in names], allow_unused=True)
 
 
+def functorch_loop(net_forward, params, a, batch, epoch, O):
+    """The loop above written the torch.func way: vmap over the tasks, torch.func.grad for the inner steps (its result
+    detached for first order), the outer gradient through torch.autograd."""
+    S = int(a.number_of_training_steps_per_iter)
+    second_order = bool(a.second_order) and epoch > a.first_order_to_second_order_epoch
+    sched = O.target_pass_schedule(a, epoch, True, S)
+    w_msl = torch.from_numpy(O.msl_weights(a, epoch)).to(batch[0].device)
+    inner = O.inner_param_names(a)
+    xs, xt, ys, yt = batch
+    B = xs.shape[0]
+
+    def task(fast, x_s, y_s, x_t, y_t):
+        task_losses = []
+        for s in range(S):
+            g = torch.func.grad(lambda p, s=s: Fnn.cross_entropy(net_forward(x_s, p, s), y_s))(fast)
+            if not second_order:
+                g = {n: v.detach() for n, v in g.items()}
+            fast = {n: fast[n] - params[O.lslr_name(n)][s] * g[n] for n in inner}
+            if sched[s] is not None:
+                loss_t = Fnn.cross_entropy(net_forward(x_t, fast, s), y_t)
+                task_losses.append(w_msl[s] * loss_t if sched[s] == "msl" else loss_t)
+        return torch.stack(task_losses).sum()
+
+    per_task = [t.reshape(B, -1, *t.shape[-3:]) for t in (xs, xt)] + [t.reshape(B, -1) for t in (ys, yt)]
+    loss = torch.func.vmap(task, in_dims=(None, 0, 0, 0, 0))({n: params[n] for n in inner}, per_task[0], per_task[2],
+                                                             per_task[1], per_task[3]).mean()
+    names = O.trainable_names(a)
+    return torch.autograd.grad(loss, [params[n] for n in names], allow_unused=True)
+
+
 def gpu_info():
     out = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True).stdout.strip()
@@ -99,7 +134,15 @@ def main():
         "operator": lambda: reference_loop(op_forward, op_params, a, dbatch, epoch, O),
         "torch": lambda: reference_loop(torch_forward, t_params, a, dbatch, epoch, O),
         "fused": lambda: m_fused.run_train_iter(batch, epoch),
+        "operator_vmap": lambda: functorch_loop(op_forward, op_params, a, dbatch, epoch, O),
+        "torch_vmap": lambda: functorch_loop(torch_forward, t_params, a, dbatch, epoch, O),
     }
+    skipped = {}
+    try:
+        legs["torch_vmap"]()
+    except Exception as e:                  # torch.func cannot run the torch-op network: report, do not time
+        skipped["torch_vmap"] = "%s: %s" % (type(e).__name__, str(e).splitlines()[0] if str(e) else "")
+        del legs["torch_vmap"]
     for _ in range(cli.warmup):
         for f in legs.values():
             f()
@@ -120,7 +163,7 @@ def main():
 
     print(json.dumps({"config": CONFIG, "meta_batch": META_BATCH, "second_order": True, "gpu": name,
                       "power_limit": power, "repeats": cli.repeats, "warmup": cli.warmup,
-                      "legs": {k: summary(v) for k, v in times.items()}}))
+                      "legs": {k: summary(v) for k, v in times.items()}, "skipped": skipped}))
 
 
 if __name__ == "__main__":
