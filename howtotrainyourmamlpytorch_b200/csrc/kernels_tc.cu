@@ -794,34 +794,43 @@ __device__ __forceinline__ float tf32_rna(float x) {
   return __uint_as_float(r);
 }
 
-__global__ void pack_weights_kernel(ParamLayout pl, const float* __restrict__ theta, long long theta_task_stride,
-                                    float* __restrict__ pack, long long pack_task_stride, long long plane_stride, int tag) {
+// One CTA per (block, tap, task): the F x F tile [c][f] is read once (coalesced), written to the W planes as it is and
+// to the WT planes through a shared-memory transpose, so every global access is a full line.  One thread per element
+// with the transposed 4-byte stores going straight to global memory (a 256-byte stride between lanes) took 33 us per
+// launch at F = 64, L = 4, 8 tasks and flooded every SM with 3456 CTAs while the main chain's next kernel waited for
+// slots; the packs run at the head of every support and tangent pass.
+__global__ void __launch_bounds__(256) pack_weights_kernel(ParamLayout pl, const float* __restrict__ theta,
+                                                           long long theta_task_stride, float* __restrict__ pack,
+                                                           long long pack_task_stride, long long plane_stride, int tag) {
   pdl_prologue(21, tag);
-  const int task = blockIdx.y;
-  const long long per_layer = 9LL * pl.F * pl.F;
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= per_layer * (pl.L - 1)) return;
-  const int l = 1 + (int)(i / per_layer);
-  const long long rel = i - (long long)(l - 1) * per_layer;      // (tap, c, f)
-  const int f = (int)(rel % pl.F);
-  const int c = (int)((rel / pl.F) % pl.F);
-  const int tap = (int)(rel / ((long long)pl.F * pl.F));
-  const float x = theta[(long long)task * theta_task_stride + pl.w_off[l] + rel];
-  const float hi = tf32_rna(x), lo = tf32_rna(x - hi);
-  float* p = pack + (long long)task * pack_task_stride + (long long)(l - 1) * per_layer;
-  p[rel] = hi;
-  p[plane_stride + rel] = lo;
-  const long long t = ((long long)tap * pl.F + f) * pl.F + c;
-  p[2 * plane_stride + t] = hi;
-  p[3 * plane_stride + t] = lo;
+  __shared__ float s_hi[64 * 65], s_lo[64 * 65];              // F <= 64 (maml_b200_create); pitch F + 1: no bank conflicts
+  const int F = pl.F, FF = F * F, task = blockIdx.y;
+  const int l = 1 + blockIdx.x / 9, tap = blockIdx.x % 9;
+  const long long tile = (long long)tap * FF;                  // (tap, c, f) -> tile + c * F + f inside W_l
+  const float* src = theta + (long long)task * theta_task_stride + pl.w_off[l] + tile;
+  float* p = pack + (long long)task * pack_task_stride + (long long)(l - 1) * 9 * FF + tile;
+  for (int i = threadIdx.x; i < FF; i += blockDim.x) {
+    const int c = i / F, f = i - c * F;
+    const float x = src[i];
+    const float hi = tf32_rna(x), lo = tf32_rna(x - hi);
+    p[i] = hi;
+    p[plane_stride + i] = lo;
+    s_hi[f * (F + 1) + c] = hi;
+    s_lo[f * (F + 1) + c] = lo;
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < FF; i += blockDim.x) {        // WT: (tap, f, c) -> tile + f * F + c
+    const int f = i / F, c = i - f * F;
+    p[2 * plane_stride + i] = s_hi[f * (F + 1) + c];
+    p[3 * plane_stride + i] = s_lo[f * (F + 1) + c];
+  }
 }
 
 void launch_pack_weights(const ParamLayout& pl, const float* theta, long long theta_task_stride, float* pack,
                          long long pack_task_stride, long long plane_stride, int tasks, cudaStream_t st) {
   ProfScope prof_scope__(PROF_PARAM, 0.0, st);
-  const long long n = 9LL * pl.F * pl.F * (pl.L - 1);
-  if (n <= 0) return;
-  dim3 grid((unsigned)((n + 255) / 256), tasks);
+  if (pl.L <= 1) return;
+  dim3 grid(9 * (pl.L - 1), tasks);
   launch_pdl(pack_weights_kernel, dim3(grid), dim3(256), (size_t)(0), st, pl, theta, theta_task_stride, pack, pack_task_stride, plane_stride, launch_tag());
   CUDA_CHECK_LAUNCH();
 }
