@@ -4,7 +4,7 @@
 // meta_neural_network_architectures.py:89-97 (F.conv2d) and its autograd derivatives
 // (convolution_backward / double backward) -- see SURVEY.md appendix A1-A3.
 //
-// These kernels are the exact-fp32 path: used for the first block (K = 9*C_in is 9 or 27) and
+// These kernels are the exact-fp32 path: used for the first block (K = 9*C_in, 9 to 36) and
 // for shapes the wgmma 3xTF32 kernel (kernels_tc.cu) does not cover.
 #include <algorithm>
 #include "common.cuh"
@@ -200,101 +200,16 @@ void launch_conv_rows(const ConvArgs& a, cudaStream_t st) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// first block: K = 9 * C0 (9 or 27) -- all weights and the image window live in shared memory
-// The two-pair instantiations (NSRC = 2: the image tangent of the functional operator) repeat the staging and the inner
-// loop of the first pair in `if constexpr (NSRC == 2)` blocks.  The copies are deliberate: one force-inlined helper or
-// lambda called once per pair changes the register allocation and instruction order of the one-pair instantiations,
-// which the fused iteration runs.
+// first block: K = 9 * C0 (C0 = 1..4) -- all weights and the image window live in shared memory
+// The two-pair instantiations of conv0_rb_kernel and wgrad0_rb_kernel (NSRC = 2: the image tangent of the functional
+// operator) repeat the staging and the inner loop of the first pair in `if constexpr (NSRC == 2)` blocks.  The copies are
+// deliberate: one force-inlined helper or lambda called once per pair changes the register allocation and instruction
+// order of the one-pair instantiations, which the fused iteration runs.
 // ---------------------------------------------------------------------------------------------
-// NSRC = 2 adds the pair (X2, W2) (image tangent): its weights and window are staged behind the first pair's
-template <int FN, int NSRC>
-__global__ void __launch_bounds__(256) conv0_kernel(Conv0Args a, const float* X2, const float* W2) {
-  pdl_prologue(2, a.tag);
-  constexpr int NC = 16 * FN;
-  extern __shared__ float sm0[];
-  __shared__ double sred[8 * NC * 2];
-  const int task = blockIdx.y;
-  const int j0 = blockIdx.x * 64;
-  const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
-  const int c0 = a.c0;
-  float* Ws = sm0;                       // [9*c0][NC]
-  float* xs = sm0 + 9 * c0 * NC;         // [(64 + 2*(gw+1))][c0]
-  const int halo = a.gw + 1;
-  const int wrows = 64 + 2 * halo;
-  const float* W = a.W + (long long)task * a.w_stride;
-  for (int i = tid; i < 9 * c0 * NC; i += 256) Ws[i] = W[i];
-  const float* X = a.X + (long long)task * a.x_stride;
-  const int guard = a.gw + 2;
-  for (int i = tid; i < wrows * c0; i += 256) {
-    const int r = j0 - halo + i / c0;
-    float v = 0.f;
-    if (r >= -guard && r < a.rows + guard) v = X[(long long)(j0 - halo) * c0 + i];
-    xs[i] = v;
-  }
-  if constexpr (NSRC == 2) {
-    float* Ws2 = xs + wrows * c0;        // [9*c0][NC], then the window [(64 + 2*(gw+1))][c0]
-    float* xs2 = Ws2 + 9 * c0 * NC;
-    const float* W2t = W2 + (long long)task * a.w_stride;
-    for (int i = tid; i < 9 * c0 * NC; i += 256) Ws2[i] = W2t[i];
-    const float* X2t = X2 + (long long)task * a.x_stride;
-    for (int i = tid; i < wrows * c0; i += 256) {
-      const int r = j0 - halo + i / c0;
-      float v = 0.f;
-      if (r >= -guard && r < a.rows + guard) v = X2t[(long long)(j0 - halo) * c0 + i];
-      xs2[i] = v;
-    }
-  }
-  __syncthreads();
-
-  float acc[4][FN];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int jn = 0; jn < FN; ++jn) acc[i][jn] = 0.f;
-
-  for (int tap = 0; tap < 9; ++tap) {
-    const int sh = tap_shift(tap, a.gw) + halo;
-    for (int c = 0; c < c0; ++c) {
-      float b[FN];
-#pragma unroll
-      for (int jn = 0; jn < FN; ++jn) b[jn] = Ws[(tap * c0 + c) * NC + tx * FN + jn];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float av = xs[(ty * 4 + i + sh) * c0 + c];
-#pragma unroll
-        for (int jn = 0; jn < FN; ++jn) acc[i][jn] = fmaf(av, b[jn], acc[i][jn]);
-      }
-    }
-  }
-  if constexpr (NSRC == 2) {                 // the second pair: the same loop over its staged weights and window
-    const float* Ws2 = xs + wrows * c0;
-    const float* xs2 = Ws2 + 9 * c0 * NC;
-    for (int tap = 0; tap < 9; ++tap) {
-      const int sh = tap_shift(tap, a.gw) + halo;
-      for (int c = 0; c < c0; ++c) {
-        float b[FN];
-#pragma unroll
-        for (int jn = 0; jn < FN; ++jn) b[jn] = Ws2[(tap * c0 + c) * NC + tx * FN + jn];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float av = xs2[(ty * 4 + i + sh) * c0 + c];
-#pragma unroll
-          for (int jn = 0; jn < FN; ++jn) acc[i][jn] = fmaf(av, b[jn], acc[i][jn]);
-        }
-      }
-    }
-  }
-  conv_epilogue<FN>(acc, j0, a.rows, a.gw, a.G, a.h, a.w, a.mode,
-                    a.bias ? a.bias + (long long)task * a.bias_stride : nullptr,
-                    a.out + (long long)task * a.out_stride,
-                    a.zh ? a.zh + (long long)task * a.zh_stride : nullptr,
-                    a.stats ? a.stats + (long long)task * a.stats_stride : nullptr, sred);
-}
-
-// Register-blocked first-block conv (C0 = 1 or 3): a thread owns 8 CONSECUTIVE grid rows x FN columns.  For a filter row
+// Register-blocked first-block conv: a thread owns 8 CONSECUTIVE grid rows x FN columns.  For a filter row
 // ky the inputs of those 8 rows and the three kx taps are 10 consecutive grid positions: they are read once into
 // registers (10 * C0 broadcast loads) and feed 8 x 3 x C0 x FN FMAs, the weights of the row come as 3 * C0 vector loads
-// -- ~4 FMAs per shared-memory load instead of 12 per 7 in conv0_kernel, 128 rows per CTA instead of 64.
+// -- ~4 FMAs per shared-memory load, 128 rows per tile.
 // Measured on Mini-ImageNet target passes (75 images of 84x84x3 -> 48 channels per task): see DESIGN.md.
 // NSRC = 2 adds the pair (X2, W2) (image tangent): its weights and window are staged behind the first pair's
 template <int FN, int C0, int NSRC>
@@ -460,7 +375,7 @@ __global__ void __launch_bounds__(256) conv0_rb_kernel(Conv0Args a, int tiles, c
   }
 }
 
-// dynamic shared memory beyond the default 48 KB (two-pair launches of large windows) has to be opted into per kernel
+// dynamic shared memory beyond the default 48 KB has to be opted into per kernel; below it this does nothing
 template <class K>
 static K smem_optin(K kernel, size_t smem) {
   if (smem > 48 * 1024) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -473,7 +388,7 @@ static void launch_conv0_k(K kernel, dim3 grid, size_t smem, cudaStream_t st, co
 }
 
 template <int C0, int NSRC>
-static bool launch_conv0_rb(const Conv0Args& a, cudaStream_t st, const float* X2, const float* W2) {
+static void launch_conv0_rb(const Conv0Args& a, cudaStream_t st, const float* X2, const float* W2) {
   // tiles per CTA: as many as keep >= ~3 CTAs per SM in flight (fixed per-CTA cost -- weights, window, fp64 statistics
   // reduction -- is then paid once per `tiles` x 128 rows); 1 for the small launches that sit on the latency-critical chain
   const long long t128 = (a.rows + 127) / 128;
@@ -486,22 +401,15 @@ static bool launch_conv0_rb(const Conv0Args& a, cudaStream_t st, const float* X2
     case 3: launch_conv0_k(conv0_rb_kernel<3, C0, NSRC>, grid, smem, st, a, tiles, X2, W2); break;
     default: launch_conv0_k(conv0_rb_kernel<4, C0, NSRC>, grid, smem, st, a, tiles, X2, W2); break;
   }
-  return true;
 }
 
 template <int NSRC>
 static void launch_conv0_n(const Conv0Args& a, cudaStream_t st, const float* X2, const float* W2) {
-  if (a.c0 == 1 || a.c0 == 3) {
-    if (a.c0 == 1) launch_conv0_rb<1, NSRC>(a, st, X2, W2); else launch_conv0_rb<3, NSRC>(a, st, X2, W2);
-    return;
-  }
-  dim3 grid((a.rows + 63) / 64, a.tasks);
-  const size_t smem = (size_t)NSRC * (9 * a.c0 * a.ncols + (64 + 2 * (a.gw + 1)) * a.c0) * sizeof(float);
-  switch (a.ncols / 16) {
-    case 1: launch_pdl(smem_optin(conv0_kernel<1, NSRC>, smem), dim3(grid), dim3(256), (size_t)(smem), st, tagged(a), X2, W2); break;
-    case 2: launch_pdl(smem_optin(conv0_kernel<2, NSRC>, smem), dim3(grid), dim3(256), (size_t)(smem), st, tagged(a), X2, W2); break;
-    case 3: launch_pdl(smem_optin(conv0_kernel<3, NSRC>, smem), dim3(grid), dim3(256), (size_t)(smem), st, tagged(a), X2, W2); break;
-    default: launch_pdl(smem_optin(conv0_kernel<4, NSRC>, smem), dim3(grid), dim3(256), (size_t)(smem), st, tagged(a), X2, W2); break;
+  switch (a.c0) {
+    case 1: launch_conv0_rb<1, NSRC>(a, st, X2, W2); break;
+    case 2: launch_conv0_rb<2, NSRC>(a, st, X2, W2); break;
+    case 3: launch_conv0_rb<3, NSRC>(a, st, X2, W2); break;
+    default: launch_conv0_rb<4, NSRC>(a, st, X2, W2); break;
   }
 }
 
@@ -639,106 +547,12 @@ void launch_wgrad(const WgradArgs& a, cudaStream_t st) {
 #undef WGR_CASE
 }
 
-// first block wgrad: A = image matrix [rows][c0] (c0 <= 4), D = dz [rows][F].
-// Per 64-row sub-tile the dz rows and the image window (rows +/- halo) are staged in shared memory; thread
-// (grp, f) accumulates the (tap, c) combinations q = grp, grp + NG, ... for output channel f.
-// NSRC = 2 adds pair 1, A[1] (x) D[1], staged behind pair 0's arrays (the bias row sums D[0] only)
-template <int MAXQ, int NSRC>
-__global__ void __launch_bounds__(256) wgrad0_kernel(WgradArgs a) {
-  pdl_prologue(4, a.tag);
-  extern __shared__ float smw[];
-  const int task = blockIdx.y, chunk = blockIdx.x;
-  const int tid = threadIdx.x;
-  const int Fc = a.ncols, c0 = a.kc;
-  const int NG = 256 / Fc;
-  const int grp = tid / Fc, f = tid - grp * Fc;
-  const bool active = grp < NG;
-  const int ncombo = 9 * c0;            // host guarantees MAXQ * NG >= ncombo
-  constexpr int RT = 64;
-  const int halo = a.gw + 1;
-  float* Ds = smw;                       // [RT][Fc]
-  float* Xs = smw + RT * Fc;             // [(RT + 2*halo)][c0]
-  float acc[MAXQ];
-  int off[MAXQ];
-#pragma unroll
-  for (int i = 0; i < MAXQ; ++i) {
-    acc[i] = 0.f;
-    const int q = grp + i * NG;
-    off[i] = (q < ncombo) ? (tap_shift(q / c0, a.gw) + halo) * c0 + (q % c0) : 0;
-  }
-  float bacc = 0.f;
-  const int r_begin = chunk * a.rows_per_chunk;
-  const int r_end = min(a.rows, r_begin + a.rows_per_chunk);
-  const float* A = a.A[0] + (long long)task * a.a_stride[0];
-  const float* D = a.D[0] + (long long)task * a.d_stride[0];
-  const int guard = a.gw + 2;
-  for (int r0 = r_begin; r0 < r_end; r0 += RT) {
-    const int nr = min(RT, r_end - r0);
-    for (int i = tid; i < RT * Fc / 4; i += 256) {
-      const int r = (i * 4) / Fc;
-      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (r < nr) v = *reinterpret_cast<const float4*>(D + (long long)r0 * Fc + (long long)i * 4);
-      *reinterpret_cast<float4*>(Ds + i * 4) = v;
-    }
-    for (int i = tid; i < (RT + 2 * halo) * c0; i += 256) {
-      const int r = r0 - halo + i / c0;
-      float v = 0.f;
-      if (r >= -guard && r < a.rows + guard) v = A[(long long)(r0 - halo) * c0 + i];
-      Xs[i] = v;
-    }
-    if constexpr (NSRC == 2) {
-      float* Ds2 = Xs + (((RT + 2 * halo) * c0 + 3) & ~3);   // [RT][Fc], then [(RT + 2*halo)][c0] (pair 0's window padded)
-      float* Xs2 = Ds2 + RT * Fc;
-      const float* A2 = a.A[1] + (long long)task * a.a_stride[1];
-      const float* D2 = a.D[1] + (long long)task * a.d_stride[1];
-      for (int i = tid; i < RT * Fc; i += 256) Ds2[i] = (i / Fc < nr) ? D2[(long long)r0 * Fc + i] : 0.f;
-      for (int i = tid; i < (RT + 2 * halo) * c0; i += 256) {
-        const int r = r0 - halo + i / c0;
-        Xs2[i] = (r >= -guard && r < a.rows + guard) ? A2[(long long)(r0 - halo) * c0 + i] : 0.f;
-      }
-    }
-    __syncthreads();
-    if (active) {
-      for (int r = 0; r < nr; ++r) {
-        const float d = Ds[r * Fc + f];
-        const float* xr = Xs + r * c0;
-#pragma unroll
-        for (int i = 0; i < MAXQ; ++i) {
-          const int q = grp + i * NG;
-          if (q < ncombo) acc[i] = fmaf(xr[off[i]], d, acc[i]);
-        }
-        if constexpr (NSRC == 2) {
-          const float* Ds2 = Xs + (((RT + 2 * halo) * c0 + 3) & ~3);
-          const float d2 = Ds2[r * Fc + f];
-          const float* xr2 = Ds2 + RT * Fc + r * c0;
-#pragma unroll
-          for (int i = 0; i < MAXQ; ++i) {
-            const int q = grp + i * NG;
-            if (q < ncombo) acc[i] = fmaf(xr2[off[i]], d2, acc[i]);
-          }
-        }
-        bacc += d;
-      }
-    }
-    __syncthreads();
-  }
-  if (active) {
-    float* P = a.partial + (long long)task * a.partial_task_stride + (long long)chunk * a.chunk_stride;
-#pragma unroll
-    for (int i = 0; i < MAXQ; ++i) {
-      const int q = grp + i * NG;
-      if (q < ncombo) P[(long long)q * Fc + f] = acc[i];
-    }
-    if (grp == 0) P[(long long)ncombo * Fc + f] = bacc;
-  }
-}
-
-// Register-blocked first-block weight gradient (C0 = 1 or 3).  Per grid row the update is the outer product
-// x[27 = tap x c] (x) dz[F]; a thread owns one filter row ky (3 kx x C0 taps) and 4 output channels: 12 * C0 accumulators.
+// Register-blocked first-block weight gradient.  Per grid row the update is the outer product
+// x[9 * C0 = tap x c] (x) dz[F]; a thread owns one filter row ky (3 kx x C0 taps) and 4 output channels: 12 * C0 accumulators.
 // The CTA's threads form NS "row streams" of 3 * F/4 threads; a stream walks CONSECUTIVE rows of the staged tile, so the
-// three x positions of a row slide by one per row: per row C0 broadcast loads + one LDS.128 of dz feed 12 * C0 FMAs
-// (wgrad0_kernel: 7 loads per 6 FMAs).  Streams are summed through shared memory in stream order (deterministic).
-// C0 = 1 is held to 48 registers (5 CTAs per SM); left to itself ptxas gives it 58 (4 CTAs).  0: no bound for C0 = 3.
+// three x positions of a row slide by one per row: per row C0 broadcast loads + one LDS.128 of dz feed 12 * C0 FMAs.
+// Streams are summed through shared memory in stream order (deterministic).
+// C0 = 1 is held to 48 registers (5 CTAs per SM); left to itself ptxas gives it 58 (4 CTAs).  0: no bound for C0 > 1.
 // NSRC = 2 adds pair 1, A[1] (x) D[1] (forward-over-reverse with an image tangent), staged behind pair 0 and walked by the
 // same row streams; the bias row sums D[0] only.  No register bound: it is not on the fused iteration's path.
 template <int C0, int NSRC>
@@ -876,38 +690,25 @@ __global__ void __launch_bounds__(256, (C0 == 1 && NSRC == 1) ? 5 : 0) wgrad0_rb
   }
 }
 
+template <int C0>
+static void launch_wgrad0_rb(const WgradArgs& a, dim3 grid, size_t smem, cudaStream_t st) {
+  if (a.nsrc == 2) launch_pdl(smem_optin(wgrad0_rb_kernel<C0, 2>, smem), grid, dim3(256), smem, st, tagged(a));
+  else launch_pdl(smem_optin(wgrad0_rb_kernel<C0, 1>, smem), grid, dim3(256), smem, st, tagged(a));
+}
+
 void launch_wgrad0(const WgradArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_WGRAD0, a.alg_flops, st);
   dim3 grid(a.nchunks, a.tasks);
-  if ((a.kc == 1 || a.kc == 3) && (a.ncols % 4) == 0) {
-    const int tps = 3 * (a.ncols / 4), ns = 256 / tps, rt = ns * 16;
-    const size_t win = (size_t)(rt + 2 * (a.gw + 1)) * a.kc;      // a second pair starts at a 4-float boundary
-    const size_t stage = (rt * a.ncols + win + (a.nsrc == 2 ? rt * a.ncols + ((win + 3) & ~(size_t)3) : 0)) * sizeof(float);
-    const size_t red = (size_t)ns * (9 * a.kc + 1) * a.ncols * sizeof(float);
-    const size_t smem = stage > red ? stage : red;
-    if (a.nsrc == 2) {
-      if (a.kc == 1) launch_pdl(smem_optin(wgrad0_rb_kernel<1, 2>, smem), dim3(grid), dim3(256), smem, st, tagged(a));
-      else launch_pdl(smem_optin(wgrad0_rb_kernel<3, 2>, smem), dim3(grid), dim3(256), smem, st, tagged(a));
-    } else {
-      if (a.kc == 1) launch_pdl(wgrad0_rb_kernel<1, 1>, dim3(grid), dim3(256), smem, st, tagged(a));
-      else launch_pdl(wgrad0_rb_kernel<3, 1>, dim3(grid), dim3(256), smem, st, tagged(a));
-    }
-    CUDA_CHECK_LAUNCH();
-    return;
-  }
-  const size_t win = (size_t)(64 + 2 * (a.gw + 1)) * a.kc;        // a second pair starts at a 4-float boundary
-  const size_t smem = (64 * a.ncols + win + (a.nsrc == 2 ? 64 * a.ncols + ((win + 3) & ~(size_t)3) : 0)) * sizeof(float);
-  const int need = (9 * a.kc + (256 / a.ncols) - 1) / (256 / a.ncols);      // (tap, c) combinations per thread
-  if (a.nsrc == 2) {
-    if (need <= 3) launch_pdl(smem_optin(wgrad0_kernel<3, 2>, smem), dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
-    else if (need <= 6) launch_pdl(smem_optin(wgrad0_kernel<6, 2>, smem), dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
-    // F <= 64 and C0 <= 4 (maml_b200_create) give need <= 9: the two-pair form has no MAXQ = 36 instantiation
-    else launch_pdl(smem_optin(wgrad0_kernel<9, 2>, smem), dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
-  } else {
-    if (need <= 3) launch_pdl(wgrad0_kernel<3, 1>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
-    else if (need <= 6) launch_pdl(wgrad0_kernel<6, 1>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
-    else if (need <= 9) launch_pdl(wgrad0_kernel<9, 1>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
-    else launch_pdl(wgrad0_kernel<36, 1>, dim3(grid), dim3(256), (size_t)(smem), st, tagged(a));
+  const int tps = 3 * (a.ncols / 4), ns = 256 / tps, rt = ns * 16;
+  const size_t win = (size_t)(rt + 2 * (a.gw + 1)) * a.kc;      // a second pair starts at a 4-float boundary
+  const size_t stage = (rt * a.ncols + win + (a.nsrc == 2 ? rt * a.ncols + ((win + 3) & ~(size_t)3) : 0)) * sizeof(float);
+  const size_t red = (size_t)ns * (9 * a.kc + 1) * a.ncols * sizeof(float);
+  const size_t smem = stage > red ? stage : red;
+  switch (a.kc) {
+    case 1: launch_wgrad0_rb<1>(a, grid, smem, st); break;
+    case 2: launch_wgrad0_rb<2>(a, grid, smem, st); break;
+    case 3: launch_wgrad0_rb<3>(a, grid, smem, st); break;
+    default: launch_wgrad0_rb<4>(a, grid, smem, st); break;
   }
   CUDA_CHECK_LAUNCH();
 }

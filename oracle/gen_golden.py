@@ -97,11 +97,11 @@ def _envelope(base, hwc, f, l, s, nkt, b, iters, kind=KIND, **over):
 ENVELOPE_CASES = {
     # H != W; odd H at block 0 (21: a pooled row is dropped), odd W at block 1 (15)
     "env_nonsquare_odd": _envelope("mini_imagenet_mamlpp_5w1s", (21, 30, 3), 16, 3, 2, (3, 2, 2), 2, [(0, 0), (0, 1)]),
-    # C0 = 2 on the generic first-block kernels; a tall image pooled down to 5 x 1; MSL weights between the extremes.
+    # C0 = 2; a tall image pooled down to 5 x 1; MSL weights between the extremes.
     # Episode 6, not 0: episode 0 holds a leaky-ReLU pre-activation and a pooling pair 2e-7 from a tie (fp64), which fp32
     # evaluations resolve either way (the decision-forced test pins it; the direct comparisons cannot)
     "env_tall_c2": _envelope("omniglot_mamlpp_5w1s", (40, 13, 2), 32, 3, 3, (3, 2, 2), 2, [(3, 6), (3, 1)]),
-    # L = 2 and C0 = 4 in the fused iteration (the generic weight gradient's widest channel count).  One iteration: after
+    # L = 2 and C0 = 4 (the widest channel count) in the fused iteration.  One iteration: after
     # a second one, any fp32 restatement (the CPU oracle included) sits up to 1e-4 away from the reference on 0.5-1.5 %
     # of some tensors' elements (Adam's second step divides small, noisy gradient elements by their own magnitude)
     "env_c4_two_stages": _envelope("omniglot_mamlpp_5w1s", (10, 14, 4), 64, 2, 2, (3, 2, 2), 2, [(0, 0)]),

@@ -6,16 +6,18 @@ from oracle import maml_oracle as O
 
 
 def case(name):
-    """(args, fp32 state, batch) of a golden case, or of synthetic_c<C>[_w<W>]: a seeded model with C input channels and
-    W x W images (14 if not given), so that the register-blocked (C0 = 1, 3) and the generic (C0 = 4) first-block kernels
-    all run, at even and odd widths, where no golden case covers them."""
+    """(args, fp32 state, batch) of a golden case, or of synthetic_c<C>[_w<W>][_f<F>]: a seeded model with C input
+    channels, W x W images (14 if not given) and F filters (32 if not given), so that the first-block kernels run at every
+    channel count, at even and odd widths and at filter counts where no golden case covers them."""
     if name.startswith("synthetic_c"):
         from howtotrainyourmamlpytorch_b200 import make_args
         parts = name.split("_")
         c = int(parts[1][1:])
-        w = int(parts[2][1:]) if len(parts) > 2 else 14
+        opt = {p[0]: int(p[1:]) for p in parts[2:]}
+        w, f = opt.pop("w", 14), opt.pop("f", 32)
+        assert not opt, name
         a = make_args("omniglot_mamlpp_5w1s", image_channels=c, image_height=w, image_width=w,
-                      cnn_num_filters=32, num_stages=3, number_of_training_steps_per_iter=2,
+                      cnn_num_filters=f, num_stages=3, number_of_training_steps_per_iter=2,
                       number_of_evaluation_steps_per_iter=2, batch_size=2, num_target_samples=3)
         return a, O.init_state(a), O.synthetic_batch(a, iteration=5, kind="normal")
     g = load_golden(name)

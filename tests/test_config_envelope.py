@@ -26,26 +26,25 @@ gpu = pytest.mark.gpu
 # case -> (the axis it exists for, the engine paths it must reach).  Path keys:
 #   tc:    blocks l >= 1 run the tensor-core convolution / weight gradient (else the FFMA kernels, or no such block)
 #   tail:  the support pass runs the fused last block + head (tail_fused / tail_onchip) instead of head_kernel
-#   c0:    "rb" = register-blocked first-block kernels (C0 in {1, 3}), "generic" = conv0_kernel / wgrad0_kernel
 #   ring:  depth of the tensor-core conv's B ring next to split-K 2 in tangent mode (only where it is the point)
 #   chunks: weight-gradient chunks per block l >= 1 on an H100 (132 SMs) (only where it is the point)
 ENVELOPE = {
-    "env_nonsquare_odd": ("H != W, odd H at block 0, odd W at block 1", dict(tc=True, tail=True, c0="rb")),
-    "env_tall_c2": ("C0 = 2, pooled 5 x 1, MSL between its extremes", dict(tc=True, tail=True, c0="generic")),
-    "env_c4_two_stages": ("L = 2, C0 = 4 in the fused iteration", dict(tc=True, tail=False, c0="generic")),
-    "env_one_stage": ("L = 1: first block = last block, no tensor-core block", dict(tc=False, tail=True, c0="rb")),
-    "env_eight_steps": ("S = 8 = MAML_MAX_STEPS, MSL on", dict(tc=True, tail=True, c0="rb")),
-    "env_one_step": ("S = 1, second order, one target slot", dict(tc=True, tail=True, c0="rb")),
-    "env_way32": ("N*K = 128 (the cap), 32 head groups", dict(tc=True, tail=False, c0="rb")),
-    "env_way17": ("17 support rows: head kernel", dict(tc=True, tail=False, c0="rb")),
-    "env_way16": ("16 support rows: fused tail; 24 target rows", dict(tc=True, tail=True, c0="rb")),
-    "env_way2": ("2-way 1-shot: last-block BatchNorm over 18 values", dict(tc=True, tail=True, c0="rb")),
-    "env_ffma_wide": ("block 1 65 wide: the handle turns the tensor cores off", dict(tc=False, tail=True, c0="rb")),
-    "env_ring_edge": ("block 1 62 wide: largest halo, ring depth 2", dict(tc=True, tail=False, c0="rb", ring=2)),
-    "env_many_tasks": ("48 tasks: one weight-gradient chunk per block", dict(tc=True, tail=True, c0="rb", chunks=1)),
-    "env_bern_nonsquare": ("Bernoulli images, exact ties next to the dropped row", dict(tc=True, tail=True, c0="rb")),
+    "env_nonsquare_odd": ("H != W, odd H at block 0, odd W at block 1", dict(tc=True, tail=True)),
+    "env_tall_c2": ("C0 = 2, pooled 5 x 1, MSL between its extremes", dict(tc=True, tail=True)),
+    "env_c4_two_stages": ("L = 2, C0 = 4 in the fused iteration", dict(tc=True, tail=False)),
+    "env_one_stage": ("L = 1: first block = last block, no tensor-core block", dict(tc=False, tail=True)),
+    "env_eight_steps": ("S = 8 = MAML_MAX_STEPS, MSL on", dict(tc=True, tail=True)),
+    "env_one_step": ("S = 1, second order, one target slot", dict(tc=True, tail=True)),
+    "env_way32": ("N*K = 128 (the cap), 32 head groups", dict(tc=True, tail=False)),
+    "env_way17": ("17 support rows: head kernel", dict(tc=True, tail=False)),
+    "env_way16": ("16 support rows: fused tail; 24 target rows", dict(tc=True, tail=True)),
+    "env_way2": ("2-way 1-shot: last-block BatchNorm over 18 values", dict(tc=True, tail=True)),
+    "env_ffma_wide": ("block 1 65 wide: the handle turns the tensor cores off", dict(tc=False, tail=True)),
+    "env_ring_edge": ("block 1 62 wide: largest halo, ring depth 2", dict(tc=True, tail=False, ring=2)),
+    "env_many_tasks": ("48 tasks: one weight-gradient chunk per block", dict(tc=True, tail=True, chunks=1)),
+    "env_bern_nonsquare": ("Bernoulli images, exact ties next to the dropped row", dict(tc=True, tail=True)),
     "env_maml_shared_bn": ("plain MAML: shared BatchNorm, no LSLR, non-square, F = 48",
-                           dict(tc=True, tail=False, c0="rb")),
+                           dict(tc=True, tail=False)),
 }
 CASES = list(ENVELOPE)
 BERNOULLI = ["env_bern_nonsquare"]
@@ -86,8 +85,7 @@ def host_plan(a, tasks, num_sms=H100_SMS):
         nch = min(64, max(1, num_sms // (3 * tasks)), max(1, (rows + 15) // 16))
         rpc = ((rows + nch - 1) // nch + 15) // 16 * 16
         chunks.append((rows + rpc - 1) // rpc)
-    return dict(tc=tc, tail=tail, c0="rb" if int(a.image_channels) in (1, 3) else "generic",
-                ring=min(rings) if rings else None, chunks=max(chunks) if chunks else None)
+    return dict(tc=tc, tail=tail, ring=min(rings) if rings else None, chunks=max(chunks) if chunks else None)
 
 
 def _tasks(g):
@@ -207,9 +205,8 @@ def test_path_reached(case, cuda_device):
         assert ids & {K_TAIL, K_TAIL_ONCHIP} and K_TAIL_TAN in ids, sorted(ids)
     else:
         assert not ids & {K_TAIL, K_TAIL_ONCHIP, K_TAIL_TAN}, sorted(ids)
-    # conv0_rb / conv0_kernel and wgrad0_rb / wgrad0_kernel share their ids: the host rule (C0 in {1, 3}) tells them
-    # apart, the ring depth and the chunk count have no id at all
-    for k in ("c0", "ring", "chunks"):
+    # the ring depth and the chunk count have no kernel id: the host rule stands in for them
+    for k in ("ring", "chunks"):
         if k in want:
             assert plan[k] == want[k], (k, plan[k], want[k])
 
