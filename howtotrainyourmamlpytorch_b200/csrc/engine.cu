@@ -650,36 +650,126 @@ static void tc_conv(maml_b200_handle* h, int l, int n, const TcOp& op, const flo
   launch_conv_tc(maps, a, st);
 }
 
+// one operand pair of an FFMA conv of block l: A (row 0 of a guarded pass buffer) times the block-l weights of the
+// fast-weight vector `wv`, as stored (wt 0, conv: sign +1) or transposed (wt 1, dgrad: sign -1)
+struct FfmaOp { const float* A; long long a_stride; const float* wv; int wt, sign; };
+
+// FFMA conv of block l over n images per task: the sum of the operand pairs plus the block-l bias of `bias_vec`
+// (nullable).  The caller sets the output and, in the statistics modes, the sums' address (and zh).
+static ConvArgs ffma_conv(const maml_b200_handle* h, int l, int n, int mode, std::initializer_list<FfmaOp> ops,
+                          const float* bias_vec, int T) {
+  const LayerGeom& g = h->geo[l];
+  ConvArgs a{};
+  for (const FfmaOp& o : ops) a.src[a.nsrc++] = ConvSrc{o.A, o.a_stride, o.wv + h->pl.w_off[l], h->Ppad, h->F, o.wt, o.sign};
+  if (bias_vec) { a.bias = bias_vec + h->pl.b_off[l]; a.bias_stride = h->Ppad; }
+  a.rows = n * g.G; a.gw = g.gw; a.G = g.G; a.h = g.h; a.w = g.w; a.ncols = h->F; a.mode = mode;
+  if (mode != CONV_PLAIN) a.stats_stride = h->stats_task_stride;
+  a.tasks = T;
+  a.alg_flops = conv_flops(h, l, n, T, a.nsrc);
+  return a;
+}
+
+// First-block conv of pass `ps`'s images with the block-0 weights and bias of the fast-weight vector `wv` (nsrc = 2: the
+// caller's second operand pair, see launch_conv0).  The caller sets the output and the statistics' address (and zh).
+static Conv0Args conv0_args(const maml_b200_handle* h, const PassSet& ps, const float* wv, int mode, int nsrc, int T) {
+  const LayerGeom& g = h->geo[0];
+  Conv0Args a{};
+  a.X = ps.xg; a.x_stride = ps.xg_stride;
+  a.W = wv + h->pl.w_off[0]; a.w_stride = h->Ppad;
+  a.bias = wv + h->pl.b_off[0]; a.bias_stride = h->Ppad;
+  a.rows = ps.n * g.G; a.gw = g.gw; a.G = g.G; a.h = g.h; a.w = g.w; a.c0 = h->C; a.ncols = h->F; a.mode = mode;
+  a.stats_stride = h->stats_task_stride; a.tasks = T;
+  a.alg_flops = conv_flops(h, 0, ps.n, T, nsrc);
+  return a;
+}
+
+// Weight gradient of block l over n images per task into that block's chunks of the partial buffer `partial` (laid out by
+// `cp`).  The caller sets the operand pairs and alg_flops (launch_wgrad_upper does for blocks l >= 1).
+static WgradArgs wgrad_args(const maml_b200_handle* h, int l, int n, const ChunkPlan& cp, float* partial, int T) {
+  const LayerGeom& g = h->geo[l];
+  WgradArgs w{};
+  w.kc = l == 0 ? h->C : h->F; w.ncols = h->F; w.rows = n * g.G; w.gw = g.gw;
+  w.rows_per_chunk = cp.rows_per_chunk[l]; w.nchunks = cp.nchunks[l];
+  w.partial = partial + cp.pd.off[2 * l]; w.partial_task_stride = cp.pd.task_stride; w.chunk_stride = cp.pd.cstride[2 * l];
+  w.tasks = T;
+  return w;
+}
+
+// one operand pair of the weight gradient of a block l >= 1: the conv input of `a` times the output gradient of `d`
+struct WgPair { Slot a, d; };
+
+// Weight gradient of block l >= 1, summed over the operand pairs: the tensor-core kernel (reading both operands' TF32
+// planes) when the handle runs the tensor-core path and the option allows it, else the FFMA kernel.
+static void launch_wgrad_upper(const maml_b200_handle* h, int l, int n, const ChunkPlan& cp, float* partial, int T,
+                               std::initializer_list<WgPair> pairs, cudaStream_t st) {
+  const bool tc = h->use_tc && h->opt.wgrad_tc;
+  WgradArgs w = wgrad_args(h, l, n, cp, partial, T);
+  for (const WgPair& p : pairs) {
+    const PassSet& pa = *p.a.ps; const PassSet& pd = *p.d.ps;
+    const int k = w.nsrc++;
+    w.A[k] = AIN(pa, l, p.a.slot); w.a_stride[k] = STRIDE(pa, ain, l);
+    w.D[k] = DZ(pd, l, p.d.slot); w.d_stride[k] = STRIDE(pd, dz, l);
+    if (tc) { w.a_plane[k] = pa.ain_plane[l]; w.d_plane[k] = pd.dz_plane[l]; }
+  }
+  w.alg_flops = conv_flops(h, l, n, T, w.nsrc);
+  if (tc) launch_wgrad_tc(w, st);
+  else launch_wgrad(w, st);
+}
+
+// Head launch on the features of pass `ps` at `slot` (linear layer of the fast weights `theta`, zero labels); every mode
+// but the target forward writes d(features) into the pass's DP(L-1).  The caller sets labels, outputs and (head_grad)
+// where the linear layer's gradient goes.
+static HeadArgs head_args(const maml_b200_handle* h, int mode, const PassSet& ps, int slot, const float* theta, int T) {
+  HeadArgs a{};
+  a.mode = mode; a.n = ps.n; a.N = h->N; a.D = h->D; a.scale = 1.f;
+  a.f = AIN(ps, h->L, slot); a.f_stride = STRIDE(ps, ain, h->L);
+  a.Wfc = theta + h->pl.fcw_off; a.bfc = theta + h->pl.fcb_off; a.theta_stride = h->Ppad;
+  a.y = h->zero_labels; a.y_stride = 0;
+  a.rows_per_cta = head_rows(ps.n);
+  if (mode != HEAD_TARGET_FWD) { a.df = DP(ps, h->L - 1, slot); a.df_stride = STRIDE(ps, dp, h->L - 1); }
+  a.tasks = T;
+  return a;
+}
+
+// the head's gradient goes to the linear layer's chunks (one per row group) of the partial buffer `partial`
+static void head_grad(const maml_b200_handle* h, HeadArgs& a, float* partial, const ChunkPlan& cp) {
+  a.gW = partial + cp.pd.off[2 * h->L]; a.gb = partial + cp.pd.off[2 * h->L + 1];
+  a.g_stride = cp.pd.task_stride; a.g_chunk_stride = cp.pd.cstride[2 * h->L];
+}
+
+// the last block of the support batch, the head and that block's BatchNorm backward run as one kernel
+static bool support_tail_fused(const maml_b200_handle* h) {
+  return h->opt.tail_fuse && tail_fusable(bn_geom(h, h->L - 1, h->n_s), h->n_s, head_rows(h->n_s));
+}
+
+enum { CLR_STATS = 1, CLR_ABAR = 2, CLR_LOSSES = 4, CLR_CORRECT = 8 };
+// zeroes the accumulators in `what` (CLR_* bits) for all maxT tasks on `st`
+static int clear_accumulators(maml_b200_handle* h, unsigned what, cudaStream_t st) {
+  if (what & CLR_STATS) CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
+  if (what & CLR_ABAR) CK(cudaMemsetAsync(h->abar, 0, (size_t)h->maxT * h->pl.nseg_inner * MAML_MAX_STEPS * sizeof(double), st));
+  if (what & CLR_LOSSES) CK(cudaMemsetAsync(h->losses, 0, (size_t)h->maxT * MAML_MAX_STEPS * sizeof(float), st));
+  if (what & CLR_CORRECT) CK(cudaMemsetAsync(h->correct, 0, (size_t)h->maxT * sizeof(float), st));
+  return 0;
+}
+
 // primal forward of one pass: conv -> stats -> BN/leaky/pool for every block
 static void forward_pass(maml_b200_handle* h, const PassSet& ps, int slot, const float* theta, int th_step, const float* meta,
                          int bn_step, int stat_kind, int T, cudaStream_t st, BnActArgs* defer_last = nullptr) {
   for (int l = 0; l < h->L; ++l) {
-    const LayerGeom& g = h->geo[l];
     if (l == 1 && st != h->s_tgt && st != h->s_tgt2) join_pending(h, st);
     if (l == 0) {
-      Conv0Args a{};
-      a.X = ps.xg; a.x_stride = ps.xg_stride;
-      a.W = theta + h->pl.w_off[0]; a.w_stride = h->Ppad;
-      a.bias = theta + h->pl.b_off[0]; a.bias_stride = h->Ppad;
+      Conv0Args a = conv0_args(h, ps, theta, CONV_FWD_STATS, 1, T);
       a.out = ZH(ps, 0, slot); a.out_stride = STRIDE(ps, zh, 0);
-      a.rows = ps.n * g.G; a.gw = g.gw; a.G = g.G; a.h = g.h; a.w = g.w; a.c0 = h->C; a.ncols = h->F; a.mode = CONV_FWD_STATS;
-      a.stats = stat_at(h, stat_kind, bn_step, 0); a.stats_stride = h->stats_task_stride; a.tasks = T;
-      a.alg_flops = conv_flops(h, 0, ps.n, T, 1);
+      a.stats = stat_at(h, stat_kind, bn_step, 0);
       launch_conv0(a, st);
     } else if (h->use_tc) {
       tc_conv(h, l, ps.n, tc_op_ain(h, ps, l, slot, h->theta_map, th_step, +1, 2), theta + h->pl.b_off[l], h->Ppad,
               ZH(ps, l, slot), STRIDE(ps, zh, l), CONV_FWD_STATS, nullptr, 0,
               stat_at(h, stat_kind, bn_step, l), T, st);
     } else {
-      ConvArgs a{};
-      a.nsrc = 1;
-      a.src[0].A = AIN(ps, l, slot); a.src[0].a_stride = STRIDE(ps, ain, l);
-      a.src[0].W = theta + h->pl.w_off[l]; a.src[0].w_stride = h->Ppad; a.src[0].kc = h->F; a.src[0].wt = 0; a.src[0].sign = 1;
-      a.bias = theta + h->pl.b_off[l]; a.bias_stride = h->Ppad;
+      ConvArgs a = ffma_conv(h, l, ps.n, CONV_FWD_STATS, {{AIN(ps, l, slot), STRIDE(ps, ain, l), theta, 0, +1}}, theta, T);
       a.out = ZH(ps, l, slot); a.out_stride = STRIDE(ps, zh, l);
-      a.rows = ps.n * g.G; a.gw = g.gw; a.G = g.G; a.h = g.h; a.w = g.w; a.ncols = h->F; a.mode = CONV_FWD_STATS;
-      a.stats = stat_at(h, stat_kind, bn_step, l); a.stats_stride = h->stats_task_stride; a.tasks = T;
-      a.alg_flops = conv_flops(h, l, ps.n, T, 1);
+      a.stats = stat_at(h, stat_kind, bn_step, l);
       launch_conv_rows(a, st);
     }
     BnActArgs b{};
@@ -705,7 +795,6 @@ static void backward_pass(maml_b200_handle* h, const PassSet& ps, int slot, cons
   cudaStream_t wst = fork_wgrad ? h->s_wg : st;
   const bool split = fork_wgrad && rs != nullptr;
   for (int l = h->L - 1; l >= 0; --l) {
-    const LayerGeom& g = h->geo[l];
     BnBwdArgs b{};
     b.dp = DP(ps, l, slot); b.dp_stride = STRIDE(ps, dp, l);
     b.zh = ZH(ps, l, slot); b.zh_stride = STRIDE(ps, zh, l);
@@ -719,41 +808,25 @@ static void backward_pass(maml_b200_handle* h, const PassSet& ps, int slot, cons
     else launch_bnbwd(b, st);
     if (fork_wgrad) { cudaEventRecord(h->ev_fork, st); cudaStreamWaitEvent(h->s_wg, h->ev_fork, 0); }
 
-    WgradArgs w{};
-    w.nsrc = 1;
-    w.D[0] = DZ(ps, l, slot); w.d_stride[0] = STRIDE(ps, dz, l);
-    w.ncols = h->F; w.rows = ps.n * g.G; w.gw = g.gw;
-    w.rows_per_chunk = cp.rows_per_chunk[l]; w.nchunks = cp.nchunks[l];
-    w.partial = partial + cp.pd.off[2 * l]; w.partial_task_stride = cp.pd.task_stride; w.chunk_stride = cp.pd.cstride[2 * l];
-    w.tasks = T;
     if (l == 0) {
-      w.A[0] = ps.xg; w.a_stride[0] = ps.xg_stride; w.kc = h->C;
+      WgradArgs w = wgrad_args(h, 0, ps.n, cp, partial, T);
+      w.nsrc = 1;
+      w.A[0] = ps.xg; w.a_stride[0] = ps.xg_stride;
+      w.D[0] = DZ(ps, 0, slot); w.d_stride[0] = STRIDE(ps, dz, 0);
       w.alg_flops = conv_flops(h, 0, ps.n, T, 1);
       if (split && h->L == 1) reduce_upper_on_side(h, *rs, cp.pd, partial, meta, T);
       launch_wgrad0(w, split ? st : wst);
     } else {
-      w.A[0] = AIN(ps, l, slot); w.a_stride[0] = STRIDE(ps, ain, l); w.kc = h->F;
-      w.alg_flops = conv_flops(h, l, ps.n, T, 1);
       // dgrad (critical path) is enqueued before the side-stream wgrad so that its CTAs get SMs first
       if (h->use_tc) {
         tc_conv(h, l, ps.n, tc_op_dz(h, ps, l, slot, h->theta_map, th_step, -1, 0), nullptr, 0, DP(ps, l - 1, slot),
                 STRIDE(ps, dp, l - 1), CONV_PLAIN, nullptr, 0, nullptr, T, st);
       } else {
-        ConvArgs a{};
-        a.nsrc = 1;
-        a.src[0].A = DZ(ps, l, slot); a.src[0].a_stride = STRIDE(ps, dz, l);
-        a.src[0].W = theta + h->pl.w_off[l]; a.src[0].w_stride = h->Ppad; a.src[0].kc = h->F; a.src[0].wt = 1; a.src[0].sign = -1;
+        ConvArgs a = ffma_conv(h, l, ps.n, CONV_PLAIN, {{DZ(ps, l, slot), STRIDE(ps, dz, l), theta, 1, -1}}, nullptr, T);
         a.out = DP(ps, l - 1, slot); a.out_stride = STRIDE(ps, dp, l - 1);
-        a.rows = ps.n * g.G; a.gw = g.gw; a.G = g.G; a.h = g.h; a.w = g.w; a.ncols = h->F; a.mode = CONV_PLAIN; a.tasks = T;
-        a.alg_flops = conv_flops(h, l, ps.n, T, 1);
         launch_conv_rows(a, st);
       }
-      if (h->use_tc && h->opt.wgrad_tc) {
-        w.a_plane[0] = ps.ain_plane[l]; w.d_plane[0] = ps.dz_plane[l];
-        launch_wgrad_tc(w, wst);
-      } else {
-        launch_wgrad(w, wst);
-      }
+      launch_wgrad_upper(h, l, ps.n, cp, partial, T, {{{&ps, slot}, {&ps, slot}}}, wst);
       if (split && l == 1) reduce_upper_on_side(h, *rs, cp.pd, partial, meta, T);
     }
   }
@@ -764,14 +837,33 @@ static void backward_pass(maml_b200_handle* h, const PassSet& ps, int slot, cons
 // What a tangent pass differentiates at its head, and where its BatchNorm gamma / beta sums go (export adds the
 // PASS_TGT_BWD sums and subtracts the PASS_TAN_BWD ones).
 //   fused iteration:       HEAD_TANGENT, support labels y, PASS_TAN_BWD   (gamma-bar -= H_gamma u)
-//   functional operator:   HEAD_EXTERNAL_TAN, dl_ext held constant, the logits tangent into jv_out, PASS_TGT_BWD
-//                          (+H_gamma v)
+//   functional operator:   HEAD_EXTERNAL_TAN, dl_ext (floats between tasks: dl_ext_stride) held constant, the logits
+//                          tangent into jv_out, PASS_TGT_BWD (+H_gamma v)
 struct TangentHead {
   int mode;
   const long long* y;
-  const float* dl_ext; float* jv_out;
+  const float* dl_ext; long long dl_ext_stride; float* jv_out;
   int kind_tbwd;
 };
+
+// Head of the tangent pass at support slot s in direction u: the support features and their tangent in tan, d(features)-dot
+// into tan's DP(L-1), the tangent of the linear layer's gradient into the support chunks.
+static HeadArgs tangent_head_args(const maml_b200_handle* h, int s, const float* theta, const float* u, const TangentHead& th,
+                                  int T) {
+  const PassSet& tn = h->tan;
+  HeadArgs a = head_args(h, th.mode, h->sup, s, theta, T);
+  a.fdot = AIN(tn, h->L, 0); a.fdot_stride = STRIDE(tn, ain, h->L);
+  a.uW = u + h->pl.fcw_off; a.ub = u + h->pl.fcb_off; a.u_stride = h->Ppad;
+  if (th.mode == HEAD_TANGENT) {
+    a.y = th.y; a.y_stride = h->n_s;
+  } else {
+    a.dl_ext = th.dl_ext; a.dl_ext_stride = th.dl_ext_stride;
+    a.logits_out = th.jv_out; a.logits_stride = (long long)h->n_s * h->N;
+  }
+  head_grad(h, a, h->sup_partial, h->plan_sup);
+  a.df = DP(tn, h->L - 1, 0); a.df_stride = STRIDE(tn, dp, h->L - 1);
+  return a;
+}
 
 // Forward half of the tangent pass at support slot s: the tangent of the support forward in direction u (weights), plus
 // the image tangent xdot_g (padded grid, nullable: W_0 applied to it joins block 0's tangent conv as a second operand
@@ -802,18 +894,12 @@ static void tangent_forward(maml_b200_handle* h, int s, const float* theta, cons
     }
   }
   for (int l = 0; l < h->L; ++l) {
-    const LayerGeom& g = h->geo[l];
     if (l == 1) join_pending(h, st);
     if (l == 0) {
-      Conv0Args a{};
-      a.X = sp.xg; a.x_stride = sp.xg_stride;
-      a.W = u + h->pl.w_off[0]; a.w_stride = h->Ppad;
-      a.bias = u + h->pl.b_off[0]; a.bias_stride = h->Ppad;
+      Conv0Args a = conv0_args(h, sp, u, CONV_TAN_STATS, xdot_g ? 2 : 1, T);
       a.out = ZH(tn, 0, 0); a.out_stride = STRIDE(tn, zh, 0);
-      a.rows = sp.n * g.G; a.gw = g.gw; a.G = g.G; a.h = g.h; a.w = g.w; a.c0 = h->C; a.ncols = h->F; a.mode = CONV_TAN_STATS;
       a.zh = ZH(sp, 0, s); a.zh_stride = STRIDE(sp, zh, 0);
-      a.stats = stat_at(h, PASS_TAN_FWD, s, 0); a.stats_stride = h->stats_task_stride; a.tasks = T;
-      a.alg_flops = conv_flops(h, 0, sp.n, T, xdot_g ? 2 : 1);
+      a.stats = stat_at(h, PASS_TAN_FWD, s, 0);
       launch_conv0(a, st, xdot_g, xdot_g ? theta + h->pl.w_off[0] : nullptr);     // + conv(x_dot, W_0)
     } else if (h->use_tc) {
       tc_conv(h, l, sp.n, tc_op_ain(h, tn, l, 0, h->theta_map, s, +1, 2),       // conv(a_in_dot, W); the other addend is in tan2
@@ -821,18 +907,11 @@ static void tangent_forward(maml_b200_handle* h, int s, const float* theta, cons
               STRIDE(sp, zh, l), stat_at(h, PASS_TAN_FWD, s, l), T, st);
       cudaStreamWaitEvent(st, h->ev_pre[l], 0);
     } else {
-      ConvArgs a{};
-      a.nsrc = 2;
-      a.src[0].A = AIN(sp, l, s); a.src[0].a_stride = STRIDE(sp, ain, l);
-      a.src[0].W = u + h->pl.w_off[l]; a.src[0].w_stride = h->Ppad; a.src[0].kc = h->F; a.src[0].wt = 0; a.src[0].sign = 1;
-      a.src[1].A = AIN(tn, l, 0); a.src[1].a_stride = STRIDE(tn, ain, l);
-      a.src[1].W = theta + h->pl.w_off[l]; a.src[1].w_stride = h->Ppad; a.src[1].kc = h->F; a.src[1].wt = 0; a.src[1].sign = 1;
-      a.bias = u + h->pl.b_off[l]; a.bias_stride = h->Ppad;
+      ConvArgs a = ffma_conv(h, l, sp.n, CONV_TAN_STATS,
+                             {{AIN(sp, l, s), STRIDE(sp, ain, l), u, 0, +1}, {AIN(tn, l, 0), STRIDE(tn, ain, l), theta, 0, +1}}, u, T);
       a.out = ZH(tn, l, 0); a.out_stride = STRIDE(tn, zh, l);
-      a.rows = sp.n * g.G; a.gw = g.gw; a.G = g.G; a.h = g.h; a.w = g.w; a.ncols = h->F; a.mode = CONV_TAN_STATS;
       a.zh = ZH(sp, l, s); a.zh_stride = STRIDE(sp, zh, l);
-      a.stats = stat_at(h, PASS_TAN_FWD, s, l); a.stats_stride = h->stats_task_stride; a.tasks = T;
-      a.alg_flops = conv_flops(h, l, sp.n, T, 2);
+      a.stats = stat_at(h, PASS_TAN_FWD, s, l);
       launch_conv_rows(a, st);
     }
     BnActTanArgs b{};
@@ -857,34 +936,14 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
                          const float* xdot_g = nullptr) {
   const PassSet& sp = h->sup; const PassSet& tn = h->tan; const PassSet& t2 = h->tan2;
   // the fused last-block kernels implement the cross-entropy tangent head only
-  const bool fuse_tail = th.mode == HEAD_TANGENT && h->opt.tail_fuse && tail_fusable(bn_geom(h, h->L - 1, sp.n), sp.n, head_rows(sp.n));
+  const bool fuse_tail = th.mode == HEAD_TANGENT && support_tail_fused(h);
   BnActTanArgs last_act{};
-  HeadArgs hd{};
   tangent_forward(h, s, theta, u, meta, xdot_g, nullptr, T, st, spre, true, fuse_tail ? &last_act : nullptr);
   const ChunkPlan& cp = h->plan_sup;
   join_pending(h, st);
-  {
-    HeadArgs& a = hd;
-    a.mode = th.mode; a.n = h->n_s; a.N = h->N; a.D = h->D; a.scale = 1.f;
-    a.f = AIN(sp, h->L, s); a.f_stride = STRIDE(sp, ain, h->L);
-    a.fdot = AIN(tn, h->L, 0); a.fdot_stride = STRIDE(tn, ain, h->L);
-    a.Wfc = theta + h->pl.fcw_off; a.bfc = theta + h->pl.fcb_off; a.theta_stride = h->Ppad;
-    a.uW = u + h->pl.fcw_off; a.ub = u + h->pl.fcb_off; a.u_stride = h->Ppad;
-    if (th.mode == HEAD_TANGENT) {
-      a.y = th.y; a.y_stride = h->n_s;
-    } else {
-      a.y = h->zero_labels; a.y_stride = 0;
-      a.dl_ext = th.dl_ext; a.dl_ext_stride = (long long)h->n_s * h->N;
-      a.logits_out = th.jv_out; a.logits_stride = (long long)h->n_s * h->N;
-    }
-    a.gW = h->sup_partial + cp.pd.off[2 * h->L]; a.gb = h->sup_partial + cp.pd.off[2 * h->L + 1]; a.g_stride = cp.pd.task_stride;
-    a.g_chunk_stride = cp.pd.cstride[2 * h->L]; a.rows_per_cta = head_rows(a.n);
-    a.df = DP(tn, h->L - 1, 0); a.df_stride = STRIDE(tn, dp, h->L - 1);
-    a.tasks = T;
-    if (!fuse_tail) launch_head(a, st);
-  }
+  const HeadArgs hd = tangent_head_args(h, s, theta, u, th, T);
+  if (!fuse_tail) launch_head(hd, st);
   for (int l = h->L - 1; l >= 0; --l) {
-    const LayerGeom& g = h->geo[l];
     BnBwdTanArgs b{};
     b.dp = DP(sp, l, s); b.dp_stride = STRIDE(sp, dp, l);
     b.dpdot = DP(tn, l, 0); b.dpdot_stride = STRIDE(tn, dp, l);
@@ -904,15 +963,11 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
     else launch_bnbwd_tan(b, st);
     cudaEventRecord(h->ev_fork, st); cudaStreamWaitEvent(h->s_wg, h->ev_fork, 0);
 
-    WgradArgs w{};
-    w.D[0] = DZ(tn, l, 0); w.d_stride[0] = STRIDE(tn, dz, l);
-    w.ncols = h->F; w.rows = sp.n * g.G; w.gw = g.gw;
-    w.rows_per_chunk = cp.rows_per_chunk[l]; w.nchunks = cp.nchunks[l];
-    w.partial = h->sup_partial + cp.pd.off[2 * l]; w.partial_task_stride = cp.pd.task_stride; w.chunk_stride = cp.pd.cstride[2 * l];
-    w.tasks = T;
     if (l == 0) {
+      WgradArgs w = wgrad_args(h, 0, sp.n, cp, h->sup_partial, T);
       w.nsrc = 1;
-      w.A[0] = sp.xg; w.a_stride[0] = sp.xg_stride; w.kc = h->C;
+      w.A[0] = sp.xg; w.a_stride[0] = sp.xg_stride;
+      w.D[0] = DZ(tn, 0, 0); w.d_stride[0] = STRIDE(tn, dz, 0);
       if (xdot_g) {                                                    // + x_dot (x) dz: the image tangent's part
         w.nsrc = 2;
         w.A[1] = xdot_g; w.a_stride[1] = sp.xg_stride;
@@ -922,33 +977,16 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
       if (h->L == 1) reduce_upper_on_side(h, rs, cp.pd, h->sup_partial, meta, T);
       launch_wgrad0(w, st);
     } else {
-      w.nsrc = 2;
-      w.A[0] = AIN(sp, l, s); w.a_stride[0] = STRIDE(sp, ain, l); w.kc = h->F;
-      w.A[1] = AIN(tn, l, 0); w.a_stride[1] = STRIDE(tn, ain, l);
-      w.D[1] = DZ(sp, l, s); w.d_stride[1] = STRIDE(sp, dz, l);
-      w.alg_flops = conv_flops(h, l, sp.n, T, 2);
       if (h->use_tc) {
         tc_conv(h, l, sp.n, tc_op_dz(h, tn, l, 0, h->theta_map, s, -1, 0),      // dgrad(W, dz_dot); the other addend is in tan2
                 nullptr, 0, DP(tn, l - 1, 0), STRIDE(tn, dp, l - 1), CONV_PLAIN, nullptr, 0, nullptr, T, st);
       } else {
-        ConvArgs a{};
-        a.nsrc = 2;
-        a.src[0].A = DZ(tn, l, 0); a.src[0].a_stride = STRIDE(tn, dz, l);
-        a.src[0].W = theta + h->pl.w_off[l]; a.src[0].w_stride = h->Ppad; a.src[0].kc = h->F; a.src[0].wt = 1; a.src[0].sign = -1;
-        a.src[1].A = DZ(sp, l, s); a.src[1].a_stride = STRIDE(sp, dz, l);
-        a.src[1].W = u + h->pl.w_off[l]; a.src[1].w_stride = h->Ppad; a.src[1].kc = h->F; a.src[1].wt = 1; a.src[1].sign = -1;
+        ConvArgs a = ffma_conv(h, l, sp.n, CONV_PLAIN,
+                               {{DZ(tn, l, 0), STRIDE(tn, dz, l), theta, 1, -1}, {DZ(sp, l, s), STRIDE(sp, dz, l), u, 1, -1}}, nullptr, T);
         a.out = DP(tn, l - 1, 0); a.out_stride = STRIDE(tn, dp, l - 1);
-        a.rows = sp.n * g.G; a.gw = g.gw; a.G = g.G; a.h = g.h; a.w = g.w; a.ncols = h->F; a.mode = CONV_PLAIN; a.tasks = T;
-        a.alg_flops = conv_flops(h, l, sp.n, T, 2);
         launch_conv_rows(a, st);
       }
-      if (h->use_tc && h->opt.wgrad_tc) {
-        w.a_plane[0] = sp.ain_plane[l]; w.d_plane[0] = tn.dz_plane[l];
-        w.a_plane[1] = tn.ain_plane[l]; w.d_plane[1] = sp.dz_plane[l];
-        launch_wgrad_tc(w, h->s_wg);
-      } else {
-        launch_wgrad(w, h->s_wg);
-      }
+      launch_wgrad_upper(h, l, sp.n, cp, h->sup_partial, T, {{{&sp, s}, {&tn, 0}}, {{&tn, 0}, {&sp, s}}}, h->s_wg);
       if (l == 1) reduce_upper_on_side(h, rs, cp.pd, h->sup_partial, meta, T);
     }
   }
@@ -1018,10 +1056,7 @@ static int enqueue_iteration(maml_b200_handle* h, const maml_b200_iter_args* it,
   int last_t = 0;
   for (int s = 0; s < it->num_steps; ++s) if (mask & (1u << s)) last_t = s;
 
-  CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
-  CK(cudaMemsetAsync(h->abar, 0, (size_t)h->maxT * h->pl.nseg_inner * MAML_MAX_STEPS * sizeof(double), st));
-  CK(cudaMemsetAsync(h->losses, 0, (size_t)h->maxT * MAML_MAX_STEPS * sizeof(float), st));
-  CK(cudaMemsetAsync(h->correct, 0, (size_t)h->maxT * sizeof(float), st));
+  if (clear_accumulators(h, CLR_STATS | CLR_ABAR | CLR_LOSSES | CLR_CORRECT, st)) return 1;
 
   launch_prep_x(x_support, h->sup.xg, h->sup.xg_stride, T, h->n_s, h->C, h->H, h->W, st);
   launch_import_theta(h->pl, meta, h->theta, h->Ppad, T, st);
@@ -1040,24 +1075,14 @@ static int enqueue_iteration(maml_b200_handle* h, const maml_b200_iter_args* it,
   for (int s = 0; s < it->num_steps; ++s) {
     const float* th = h->theta + (long long)s * TP;
     float* th_next = h->theta + (long long)(s + 1) * TP;
-    const bool fuse_tail = h->opt.tail_fuse && tail_fusable(bn_geom(h, h->L - 1, h->n_s), h->n_s, head_rows(h->n_s));
+    const bool fuse_tail = support_tail_fused(h);
     BnActArgs last_act{};
     forward_pass(h, h->sup, s, th, s, meta, s, PASS_SUP_FWD, T, st, fuse_tail ? &last_act : nullptr);
     join_pending(h, st);
-    HeadArgs hd{};
-    {
-      HeadArgs& a = hd;
-      a.mode = HEAD_SUPPORT; a.n = h->n_s; a.N = h->N; a.D = h->D; a.scale = 1.f;
-      a.f = AIN(h->sup, h->L, s); a.f_stride = STRIDE(h->sup, ain, h->L);
-      a.Wfc = th + h->pl.fcw_off; a.bfc = th + h->pl.fcb_off; a.theta_stride = h->Ppad;
-      a.y = ys; a.y_stride = h->n_s;
-      a.gW = h->sup_partial + h->plan_sup.pd.off[2 * h->L]; a.gb = h->sup_partial + h->plan_sup.pd.off[2 * h->L + 1];
-      a.g_stride = h->plan_sup.pd.task_stride;
-      a.g_chunk_stride = h->plan_sup.pd.cstride[2 * h->L]; a.rows_per_cta = head_rows(a.n);
-      a.df = DP(h->sup, h->L - 1, s); a.df_stride = STRIDE(h->sup, dp, h->L - 1);
-      a.tasks = T;
-      if (!fuse_tail) launch_head(a, st);
-    }
+    HeadArgs hd = head_args(h, HEAD_SUPPORT, h->sup, s, th, T);
+    hd.y = ys; hd.y_stride = h->n_s;
+    head_grad(h, hd, h->sup_partial, h->plan_sup);
+    if (!fuse_tail) launch_head(hd, st);
     // LSLR update theta^{s+1} = theta^s - alpha[.][s] * g and the tensor-core packs of theta^{s+1}: blocks >= 1 and the
     // linear layer on the side stream, block 0 at the end of the main chain
     ReduceSpec rs{PR_UPDATE, th, th_next, h->g + (long long)s * TP, nullptr, s, s + 1};
@@ -1074,26 +1099,18 @@ static int enqueue_iteration(maml_b200_handle* h, const maml_b200_iter_args* it,
       CK(cudaStreamWaitEvent(ts_, h->ev_wg, 0));         // everything else + packs (side stream)
       const int ts = (h->cfg.reserved & 1) ? s : tpar;
       forward_pass(h, h->tgt, ts, th_next, s + 1, meta, s, PASS_TGT_FWD, T, ts_);
-      HeadArgs a{};
-      a.mode = HEAD_TARGET_FWD; a.n = h->n_t; a.N = h->N; a.D = h->D; a.scale = 1.f;
-      a.f = AIN(h->tgt, h->L, ts); a.f_stride = STRIDE(h->tgt, ain, h->L);
-      a.Wfc = th_next + h->pl.fcw_off; a.bfc = th_next + h->pl.fcb_off; a.theta_stride = h->Ppad;
+      HeadArgs a = head_args(h, HEAD_TARGET_FWD, h->tgt, ts, th_next, T);
       a.y = yt; a.y_stride = h->n_t;
-      a.loss_out = h->losses + s; a.loss_stride = MAML_MAX_STEPS; a.rows_per_cta = head_rows(a.n);
+      a.loss_out = h->losses + s; a.loss_stride = MAML_MAX_STEPS;
       if (s == last_t) {
         a.logits_out = last_logits; a.logits_stride = (long long)h->n_t * h->N;
         a.correct_out = h->correct; a.correct_stride = 1;
       }
-      a.tasks = T;
       launch_head(a, ts_);
       if (it->training) {
-        HeadArgs bqa = a;
-        bqa.mode = HEAD_TARGET_BWD; bqa.scale = it->target_weight[s];
-        bqa.logits_out = nullptr; bqa.correct_out = nullptr; bqa.loss_out = nullptr;
-        bqa.gW = tpart + h->plan_tgt.pd.off[2 * h->L]; bqa.gb = tpart + h->plan_tgt.pd.off[2 * h->L + 1];
-        bqa.g_stride = h->plan_tgt.pd.task_stride;
-        bqa.g_chunk_stride = h->plan_tgt.pd.cstride[2 * h->L];
-        bqa.df = DP(h->tgt, h->L - 1, ts); bqa.df_stride = STRIDE(h->tgt, dp, h->L - 1);
+        HeadArgs bqa = head_args(h, HEAD_TARGET_BWD, h->tgt, ts, th_next, T);
+        bqa.y = yt; bqa.y_stride = h->n_t; bqa.scale = it->target_weight[s];
+        head_grad(h, bqa, tpart, h->plan_tgt);
         launch_head(bqa, ts_);
         backward_pass(h, h->tgt, ts, th_next, s + 1, meta, s, PASS_TGT_FWD, PASS_TGT_BWD, tpart, h->plan_tgt, T, ts_, false);
         launch_param_reduce(h->pl, h->plan_tgt.pd, tpart, PR_STORE, nullptr, nullptr, h->tgrad + (long long)s * TP, nullptr,
@@ -1116,7 +1133,7 @@ static int enqueue_iteration(maml_b200_handle* h, const maml_b200_iter_args* it,
         cudaStream_t spre;
         if (fork_direction(h, T, st, &spre)) return 1;
         ReduceSpec rs{PR_SUB, nullptr, nullptr, nullptr, h->tbar, s, -1};
-        tangent_pass(h, s, th, h->u, meta, TangentHead{HEAD_TANGENT, ys, nullptr, nullptr, PASS_TAN_BWD}, T, st, rs, spre);
+        tangent_pass(h, s, th, h->u, meta, TangentHead{HEAD_TANGENT, ys, nullptr, 0, nullptr, PASS_TAN_BWD}, T, st, rs, spre);
       }
     }
     join_pending(h, st);
@@ -1227,17 +1244,9 @@ static const float* stage_forward(maml_b200_handle* h, const PassSet& ps, int sl
 static void external_backward(maml_b200_handle* h, const PassSet& ps, int slot, int num_step, int kind_fwd, int kind_bwd,
                               const float* meta_like, const float* dlogits, float* partial, const ChunkPlan& cp, int T, cudaStream_t st) {
   const float* th = h->theta + (long long)slot * h->maxT * h->Ppad;
-  HeadArgs a{};
-  a.mode = HEAD_EXTERNAL_BWD; a.n = ps.n; a.N = h->N; a.D = h->D; a.scale = 1.f;
-  a.f = AIN(ps, h->L, slot); a.f_stride = STRIDE(ps, ain, h->L);
-  a.Wfc = th + h->pl.fcw_off; a.bfc = th + h->pl.fcb_off; a.theta_stride = h->Ppad;
-  a.y = h->zero_labels; a.y_stride = 0;
+  HeadArgs a = head_args(h, HEAD_EXTERNAL_BWD, ps, slot, th, T);
   a.dl_ext = dlogits; a.dl_ext_stride = (long long)ps.n * h->N;
-  a.gW = partial + cp.pd.off[2 * h->L]; a.gb = partial + cp.pd.off[2 * h->L + 1];
-  a.g_stride = cp.pd.task_stride; a.g_chunk_stride = cp.pd.cstride[2 * h->L];
-  a.rows_per_cta = head_rows(a.n);
-  a.df = DP(ps, h->L - 1, slot); a.df_stride = STRIDE(ps, dp, h->L - 1);
-  a.tasks = T;
+  head_grad(h, a, partial, cp);
   launch_head(a, st);
   backward_pass(h, ps, slot, th, slot, meta_like, num_step, kind_fwd, kind_bwd, partial, cp, T, st, false);
 }
@@ -1261,18 +1270,11 @@ extern "C" int maml_b200_net_forward_tasks(maml_b200_handle* h, int32_t n_tasks,
   LaunchScope launch_scope(h, st);
   const int T = n_tasks;
   record_call(h, FN_NONE, 0, 0);
-  CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
-  CK(cudaMemsetAsync(h->losses, 0, (size_t)h->maxT * MAML_MAX_STEPS * sizeof(float), st));
-  CK(cudaMemsetAsync(h->correct, 0, (size_t)h->maxT * sizeof(float), st));
-  stage_forward(h, h->tgt, 0, PASS_TGT_FWD, num_step, meta_like, meta_stride, x, nullptr, nullptr, 0, T, st);
-  HeadArgs a{};
-  a.mode = HEAD_TARGET_FWD; a.n = h->n_t; a.N = h->N; a.D = h->D; a.scale = 1.f;
-  a.f = AIN(h->tgt, h->L, 0); a.f_stride = STRIDE(h->tgt, ain, h->L);
-  a.Wfc = h->theta + h->pl.fcw_off; a.bfc = h->theta + h->pl.fcb_off; a.theta_stride = h->Ppad;
-  a.y = h->zero_labels; a.y_stride = 0;
-  a.loss_out = h->losses; a.loss_stride = MAML_MAX_STEPS; a.rows_per_cta = head_rows(a.n);
+  if (clear_accumulators(h, CLR_STATS | CLR_LOSSES | CLR_CORRECT, st)) return 1;
+  const float* th = stage_forward(h, h->tgt, 0, PASS_TGT_FWD, num_step, meta_like, meta_stride, x, nullptr, nullptr, 0, T, st);
+  HeadArgs a = head_args(h, HEAD_TARGET_FWD, h->tgt, 0, th, T);
+  a.loss_out = h->losses; a.loss_stride = MAML_MAX_STEPS;
   a.logits_out = logits; a.logits_stride = (long long)h->n_t * h->N;
-  a.tasks = T;
   launch_head(a, st);
   CK(cudaGetLastError());
   record_call(h, FN_FORWARD, T, num_step);
@@ -1306,9 +1308,7 @@ extern "C" int maml_b200_net_backward_tasks(maml_b200_handle* h, int32_t n_tasks
   for (int kind : {PASS_TGT_BWD, PASS_TAN_BWD})
     CK(cudaMemset2DAsync(h->stats + (long long)kind * MAML_MAX_STEPS * h->st_pass_stride, (size_t)h->stats_task_stride * sizeof(double), 0,
                          (size_t)MAML_MAX_STEPS * h->st_pass_stride * sizeof(double), (size_t)T, st));
-  CK(cudaMemsetAsync(h->abar, 0, (size_t)h->maxT * h->pl.nseg_inner * MAML_MAX_STEPS * sizeof(double), st));
-  CK(cudaMemsetAsync(h->losses, 0, (size_t)h->maxT * MAML_MAX_STEPS * sizeof(float), st));
-  CK(cudaMemsetAsync(h->correct, 0, (size_t)h->maxT * sizeof(float), st));
+  if (clear_accumulators(h, CLR_ABAR | CLR_LOSSES | CLR_CORRECT, st)) return 1;
   external_backward(h, h->tgt, 0, num_step, PASS_TGT_FWD, PASS_TGT_BWD, meta_like, dlogits, h->tgt_partial, h->plan_tgt, T, st);
   launch_param_reduce(h->pl, h->plan_tgt.pd, h->tgt_partial, PR_STORE, nullptr, nullptr, h->tbar, nullptr, meta_like, num_step,
                       h->Ppad, T, st);
@@ -1364,18 +1364,15 @@ static int net_hvp_impl(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, 
   const int T = n_tasks, s = num_step;
   record_call(h, FN_NONE, 0, 0);                 // at num_step 0 this overwrites the weights net_forward imported
   if (xdot && ensure_xdot(h, st)) return 1;
-  CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
-  CK(cudaMemsetAsync(h->abar, 0, (size_t)h->maxT * h->pl.nseg_inner * MAML_MAX_STEPS * sizeof(double), st));
-  CK(cudaMemsetAsync(h->losses, 0, (size_t)h->maxT * MAML_MAX_STEPS * sizeof(float), st));
-  CK(cudaMemsetAsync(h->correct, 0, (size_t)h->maxT * sizeof(float), st));
+  if (clear_accumulators(h, CLR_STATS | CLR_ABAR | CLR_LOSSES | CLR_CORRECT, st)) return 1;
   const float* th = stage_forward(h, h->sup, s, PASS_SUP_FWD, s, meta_like, meta_stride, x, xdot, v_like, dir_stride, T, st);
   // the tangent pass reads this backward's dz / dp and statistics; its weight-gradient chunks are overwritten unread
   external_backward(h, h->sup, s, s, PASS_SUP_FWD, PASS_SUP_BWD, meta_like, dlogits, h->sup_partial, h->plan_sup, T, st);
   cudaStream_t spre;
   if (fork_direction(h, T, st, &spre)) return 1;
   ReduceSpec rs{PR_STORE, nullptr, nullptr, h->tbar, nullptr, s, -1};
-  tangent_pass(h, s, th, h->u, meta_like, TangentHead{HEAD_EXTERNAL_TAN, nullptr, dlogits, jv_out, PASS_TGT_BWD}, T, st, rs, spre,
-               xdot ? h->xdot_g : nullptr);
+  const TangentHead th_ext{HEAD_EXTERNAL_TAN, nullptr, dlogits, (long long)h->n_s * h->N, jv_out, PASS_TGT_BWD};
+  tangent_pass(h, s, th, h->u, meta_like, th_ext, T, st, rs, spre, xdot ? h->xdot_g : nullptr);
   join_pending(h, st);
   launch_export(export_args(h, T, hv_out, !sum_tasks), st);
   CK(cudaGetLastError());
@@ -1423,28 +1420,13 @@ extern "C" int maml_b200_net_jvp(maml_b200_handle* h, int32_t n_tasks, int32_t n
   if (xdot && ensure_xdot(h, st)) return 1;
   // zero d(logits) of one batch, read with a task stride of 0
   if (!h->zero_dl && alloc_zeroed(&h->zero_dl, (size_t)h->n_s * h->N * sizeof(float), st)) return 1;
-  CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
+  if (clear_accumulators(h, CLR_STATS, st)) return 1;
   const float* th = stage_forward(h, h->sup, s, PASS_SUP_FWD, s, meta_like, 0, x, xdot, t_like, 0, T, st);
   cudaStream_t spre;
   if (fork_direction(h, T, st, &spre)) return 1;
   tangent_forward(h, s, th, h->u, meta_like, xdot ? h->xdot_g : nullptr, t_like, T, st, spre, false, nullptr);
   join_pending(h, st);
-  const PassSet& sp = h->sup; const PassSet& tn = h->tan;
-  HeadArgs a{};
-  a.mode = HEAD_EXTERNAL_TAN; a.n = h->n_s; a.N = h->N; a.D = h->D; a.scale = 1.f;
-  a.f = AIN(sp, h->L, s); a.f_stride = STRIDE(sp, ain, h->L);
-  a.fdot = AIN(tn, h->L, 0); a.fdot_stride = STRIDE(tn, ain, h->L);
-  a.Wfc = th + h->pl.fcw_off; a.bfc = th + h->pl.fcb_off; a.theta_stride = h->Ppad;
-  a.uW = h->u + h->pl.fcw_off; a.ub = h->u + h->pl.fcb_off; a.u_stride = h->Ppad;
-  a.y = h->zero_labels; a.y_stride = 0;
-  a.dl_ext = h->zero_dl; a.dl_ext_stride = 0;
-  a.logits_out = jv_out; a.logits_stride = (long long)h->n_s * h->N;
-  a.gW = h->sup_partial + h->plan_sup.pd.off[2 * h->L]; a.gb = h->sup_partial + h->plan_sup.pd.off[2 * h->L + 1];
-  a.g_stride = h->plan_sup.pd.task_stride; a.g_chunk_stride = h->plan_sup.pd.cstride[2 * h->L];
-  a.rows_per_cta = head_rows(a.n);
-  a.df = DP(tn, h->L - 1, 0); a.df_stride = STRIDE(tn, dp, h->L - 1);
-  a.tasks = T;
-  launch_head(a, st);
+  launch_head(tangent_head_args(h, s, th, h->u, TangentHead{HEAD_EXTERNAL_TAN, nullptr, h->zero_dl, 0, jv_out, PASS_TGT_BWD}, T), st);
   CK(cudaGetLastError());
   return 0;
 }

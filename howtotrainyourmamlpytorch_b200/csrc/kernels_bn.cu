@@ -57,6 +57,20 @@ struct WinIter {
     hc = (g.h + 1) >> 1; wc = (g.w + 1) >> 1; NW = g.n * hc * wc; F4 = g.F >> 2;
     WPB = blockDim.x / F4; q = threadIdx.x % F4; lane = threadIdx.x / F4;
   }
+  // work item wi -> image, window row, window column
+  __device__ __forceinline__ void window(int wi, int& img, int& wy, int& wx) const {
+    img = wi / (hc * wc);
+    const int rem = wi - img * hc * wc;
+    wy = rem / wc; wx = rem - wy * wc;
+  }
+  // offset of this thread's channel quad at pixel (yy, xx) of image img on the block's padded grid
+  __device__ __forceinline__ long long grid(const BnGeom& g, int img, int yy, int xx) const {
+    return ((long long)img * g.G + (yy + 1) * g.gw + (xx + 1)) * g.F + q * 4;
+  }
+  // offset of this thread's channel quad at window (wy, wx) of image img on the grid of the pooled output
+  __device__ __forceinline__ long long pooled(const BnGeom& g, int img, int wy, int wx) const {
+    return ((long long)img * g.pG + (wy + g.pb) * g.pgw + (wx + g.pb)) * g.F + q * 4;
+  }
 };
 
 // ------------------------------------------------------------------------------- forward
@@ -67,15 +81,13 @@ __device__ __forceinline__ void bnact_phase(const BnActArgs& a, const BnGeom& g,
   float* z = a.z + (long long)task * a.z_stride;
   float* p = a.p + (long long)task * a.p_stride;
   for (int wi = cta * it.WPB + it.lane; wi < it.NW; wi += ncta * it.WPB) {
-    const int img = wi / (it.hc * it.wc);
-    const int rem = wi - img * it.hc * it.wc;
-    const int wy = rem / it.wc, wx = rem - wy * it.wc;
+    int img, wy, wx; it.window(wi, img, wy, wx);
     float4 best = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
       if (yy < g.h && xx < g.w) {
-        const long long idx = ((long long)img * g.G + (yy + 1) * g.gw + (xx + 1)) * g.F + it.q * 4;
+        const long long idx = it.grid(g, img, yy, xx);
         const float4 zv = ld4(z + idx);
         float4 zh, act;
         zh.x = (zv.x - mu.x) * r.x; zh.y = (zv.y - mu.y) * r.y; zh.z = (zv.z - mu.z) * r.z; zh.w = (zv.w - mu.w) * r.w;
@@ -92,7 +104,7 @@ __device__ __forceinline__ void bnact_phase(const BnActArgs& a, const BnGeom& g,
       }
     }
     if (wy < g.ph && wx < g.pw) {
-      const long long pidx = ((long long)img * g.pG + (wy + g.pb) * g.pgw + (wx + g.pb)) * g.F + it.q * 4;
+      const long long pidx = it.pooled(g, img, wy, wx);
       st4(p + pidx, best);
       if (a.p_hi) st4_split(a.p_hi + (long long)task * a.p_stride, a.p_lo + (long long)task * a.p_stride, pidx, best);
     }
@@ -110,12 +122,17 @@ __global__ void __launch_bounds__(256) bnact_kernel(BnActArgs a) {
   bnact_phase(a, g, task, blockIdx.x, gridDim.x, it, s_mu, s_r, s_g, s_b);
 }
 
+// Host side of WinIter: the pooling windows of one task (NW) and the windows a 256-thread CTA works on at once (wpb, one
+// thread per channel quad)
+struct WinGeom { int NW, wpb; };
+static inline WinGeom win_geom(const BnGeom& g) {
+  return WinGeom{g.n * ((g.h + 1) / 2) * ((g.w + 1) / 2), 256 / (g.F / 4)};
+}
+
 static inline dim3 bn_grid(const BnGeom& g, int tasks, int* block) {
-  const int F4 = g.F / 4;
-  const int wpb = 256 / F4;
-  *block = wpb * F4;
-  const int NW = g.n * ((g.h + 1) / 2) * ((g.w + 1) / 2);
-  int bx = (NW + wpb - 1) / wpb;
+  const WinGeom wg = win_geom(g);
+  *block = wg.wpb * (g.F / 4);
+  int bx = (wg.NW + wg.wpb - 1) / wg.wpb;
   if (bx > 4 * num_sms()) bx = 4 * num_sms();
   if (bx < 1) bx = 1;
   return dim3(bx, tasks);
@@ -131,16 +148,16 @@ void launch_bnact(const BnActArgs& a, cudaStream_t st) {
 // value of one window position: loads zh, recomputes y; used by all backward-type kernels
 struct WinPos { float4 zh; float4 y; bool ok; long long idx; };
 
-__device__ __forceinline__ void argmax_window(const float* __restrict__ zhp, const BnGeom& g, int img, int wy, int wx, int q,
-                                              const float4& ga, const float4& be, float4 (&zh)[4], long long (&idx)[4],
-                                              int4& arg, float4& slope_at) {
+__device__ __forceinline__ void argmax_window(const float* __restrict__ zhp, const BnGeom& g, int img, int wy, int wx,
+                                              const WinIter& it, const float4& ga, const float4& be, float4 (&zh)[4],
+                                              long long (&idx)[4], int4& arg, float4& slope_at) {
   float4 best = make_float4(0.f, 0.f, 0.f, 0.f);
   float4 ybest = best;
   arg = make_int4(0, 0, 0, 0);
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
-    idx[k] = ((long long)img * g.G + (yy + 1) * g.gw + (xx + 1)) * g.F + q * 4;
+    idx[k] = it.grid(g, img, yy, xx);
     zh[k] = ld4(zhp + idx[k]);
     float4 y, act;
     y.x = fmaf(ga.x, zh[k].x, be.x); y.y = fmaf(ga.y, zh[k].y, be.y);
@@ -244,13 +261,11 @@ __device__ __forceinline__ void bnbwd_reduce_phase(const BnBwdArgs& a, const BnG
   const float* zhp = a.zh + (long long)task * a.zh_stride;
   const float* dp = a.dp + (long long)task * a.dp_stride;
   for (int wi = cta * it.WPB + it.lane; wi < it.NW; wi += ncta * it.WPB) {
-    const int img = wi / (it.hc * it.wc);
-    const int rem = wi - img * it.hc * it.wc;
-    const int wy = rem / it.wc, wx = rem - wy * it.wc;
+    int img, wy, wx; it.window(wi, img, wy, wx);
     if (wy >= g.ph || wx >= g.pw) continue;
     float4 zh[4]; long long idx[4]; int4 arg; float4 sl;
-    argmax_window(zhp, g, img, wy, wx, it.q, ga, be, zh, idx, arg, sl);
-    const float4 d = ld4(dp + ((long long)img * g.pG + (wy + g.pb) * g.pgw + (wx + g.pb)) * g.F + it.q * 4);
+    argmax_window(zhp, g, img, wy, wx, it, ga, be, zh, idx, arg, sl);
+    const float4 d = ld4(dp + it.pooled(g, img, wy, wx));
     const float dy0 = d.x * sl.x, dy1 = d.y * sl.y, dy2 = d.z * sl.z, dy3 = d.w * sl.w;
     s1[0] += dy0; s2[0] += (double)dy0 * (double)pick(zh, arg.x, 0);
     s1[1] += dy1; s2[1] += (double)dy1 * (double)pick(zh, arg.y, 1);
@@ -292,14 +307,12 @@ __device__ __forceinline__ void bnbwd_apply_phase(const BnBwdArgs& a, const BnGe
   const float* dp = a.dp + (long long)task * a.dp_stride;
   float* dz = a.dz + (long long)task * a.dz_stride;
   for (int wi = cta * it.WPB + it.lane; wi < it.NW; wi += ncta * it.WPB) {
-    const int img = wi / (it.hc * it.wc);
-    const int rem = wi - img * it.hc * it.wc;
-    const int wy = rem / it.wc, wx = rem - wy * it.wc;
+    int img, wy, wx; it.window(wi, img, wy, wx);
     const bool full = (wy < g.ph && wx < g.pw);
     if (full) {
       float4 zh[4]; long long idx[4]; int4 arg; float4 sl;
-      argmax_window(zhp, g, img, wy, wx, it.q, ga, be, zh, idx, arg, sl);
-      const float4 d = ld4(dp + ((long long)img * g.pG + (wy + g.pb) * g.pgw + (wx + g.pb)) * g.F + it.q * 4);
+      argmax_window(zhp, g, img, wy, wx, it, ga, be, zh, idx, arg, sl);
+      const float4 d = ld4(dp + it.pooled(g, img, wy, wx));
       const float4 dyv = make_float4(d.x * sl.x, d.y * sl.y, d.z * sl.z, d.w * sl.w);
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
@@ -316,7 +329,7 @@ __device__ __forceinline__ void bnbwd_apply_phase(const BnBwdArgs& a, const BnGe
       for (int k = 0; k < 4; ++k) {
         const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
         if (yy < g.h && xx < g.w) {
-          const long long idx = ((long long)img * g.G + (yy + 1) * g.gw + (xx + 1)) * g.F + it.q * 4;
+          const long long idx = it.grid(g, img, yy, xx);
           const float4 zh = ld4(zhp + idx);
           float4 o;
           o.x = rg.x * (-c1.x - zh.x * c2.x); o.y = rg.y * (-c1.y - zh.y * c2.y);
@@ -369,9 +382,8 @@ __global__ void __launch_bounds__(256) bnbwd_fused_kernel(BnBwdArgs a) {
 // more than 32 CTAs at one window per thread, or the handle's BN_FUSE option is off)
 static inline int bn_fused_cluster(const BnGeom& g) {
   if (!launch_ctx().opt->bn_fuse) return 0;
-  const int F4 = g.F / 4, wpb = 256 / F4;
-  const int NW = g.n * ((g.h + 1) / 2) * ((g.w + 1) / 2);
-  const int need = (NW + wpb - 1) / wpb;
+  const WinGeom wg = win_geom(g);
+  const int need = (wg.NW + wg.wpb - 1) / wg.wpb;
   if (need > 32) return 0;
   int cl = 1;
   while (cl < need && cl < 8) cl <<= 1;
@@ -431,15 +443,13 @@ __device__ __forceinline__ void bnact_tan_phase(const BnActTanArgs& a, const BnG
   const float* zhp = a.zh + (long long)task * a.zh_stride;
   float* pd = a.pdot + (long long)task * a.pdot_stride;
   for (int wi = cta * it.WPB + it.lane; wi < it.NW; wi += ncta * it.WPB) {
-    const int img = wi / (it.hc * it.wc);
-    const int rem = wi - img * it.hc * it.wc;
-    const int wy = rem / it.wc, wx = rem - wy * it.wc;
+    int img, wy, wx; it.window(wi, img, wy, wx);
     float4 best = make_float4(0.f, 0.f, 0.f, 0.f), pbest = best;
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
       if (yy < g.h && xx < g.w) {
-        const long long idx = ((long long)img * g.G + (yy + 1) * g.gw + (xx + 1)) * g.F + it.q * 4;
+        const long long idx = it.grid(g, img, yy, xx);
         const float4 zh = ld4(zhp + idx);
         float4 zv = ld4(zd + idx);
         if (zd2) { const float4 z2 = ld4(zd2 + idx); zv.x += z2.x; zv.y += z2.y; zv.z += z2.z; zv.w += z2.w; }
@@ -467,7 +477,7 @@ __device__ __forceinline__ void bnact_tan_phase(const BnActTanArgs& a, const BnG
       }
     }
     if (wy < g.ph && wx < g.pw) {
-      const long long pidx = ((long long)img * g.pG + (wy + g.pb) * g.pgw + (wx + g.pb)) * g.F + it.q * 4;
+      const long long pidx = it.pooled(g, img, wy, wx);
       st4(pd + pidx, pbest);
       if (a.pdot_hi) st4_split(a.pdot_hi + (long long)task * a.pdot_stride, a.pdot_lo + (long long)task * a.pdot_stride, pidx, pbest);
     }
@@ -519,13 +529,11 @@ __device__ __forceinline__ void bnbwd_tan_reduce_phase(const BnBwdTanArgs& a, co
   const float* dp = a.dp + (long long)task * a.dp_stride;
   const float* dpd = a.dpdot + (long long)task * a.dpdot_stride;
   for (int wi = cta * it.WPB + it.lane; wi < it.NW; wi += ncta * it.WPB) {
-    const int img = wi / (it.hc * it.wc);
-    const int rem = wi - img * it.hc * it.wc;
-    const int wy = rem / it.wc, wx = rem - wy * it.wc;
+    int img, wy, wx; it.window(wi, img, wy, wx);
     if (wy >= g.ph || wx >= g.pw) continue;
     float4 zh[4]; long long idx[4]; int4 arg; float4 sl;
-    argmax_window(zhp, g, img, wy, wx, it.q, ga, be, zh, idx, arg, sl);
-    const long long pidx = ((long long)img * g.pG + (wy + g.pb) * g.pgw + (wx + g.pb)) * g.F + it.q * 4;
+    argmax_window(zhp, g, img, wy, wx, it, ga, be, zh, idx, arg, sl);
+    const long long pidx = it.pooled(g, img, wy, wx);
     const float4 d = ld4(dp + pidx);
     float4 dd = ld4(dpd + pidx);
     if (a.dpdot2) {
@@ -584,16 +592,14 @@ __device__ __forceinline__ void bnbwd_tan_apply_phase(const BnBwdTanArgs& a, con
   const float* dpd = a.dpdot + (long long)task * a.dpdot_stride;
   float* dzd = a.dzdot + (long long)task * a.dzdot_stride;
   for (int wi = cta * it.WPB + it.lane; wi < it.NW; wi += ncta * it.WPB) {
-    const int img = wi / (it.hc * it.wc);
-    const int rem = wi - img * it.hc * it.wc;
-    const int wy = rem / it.wc, wx = rem - wy * it.wc;
+    int img, wy, wx; it.window(wi, img, wy, wx);
     const bool full = (wy < g.ph && wx < g.pw);
     int4 arg = make_int4(-1, -1, -1, -1);
     float4 dyd = make_float4(0.f, 0.f, 0.f, 0.f);
     if (full) {
       float4 zh[4]; long long idx[4]; float4 sl;
-      argmax_window(zhp, g, img, wy, wx, it.q, ga, be, zh, idx, arg, sl);
-      const long long pidx = ((long long)img * g.pG + (wy + g.pb) * g.pgw + (wx + g.pb)) * g.F + it.q * 4;
+      argmax_window(zhp, g, img, wy, wx, it, ga, be, zh, idx, arg, sl);
+      const long long pidx = it.pooled(g, img, wy, wx);
       float4 dd = ld4(dpd + pidx);
       if (a.dpdot2) {
         const float4 d2 = ld4(a.dpdot2 + (long long)task * a.dpdot_stride + pidx);
@@ -605,7 +611,7 @@ __device__ __forceinline__ void bnbwd_tan_apply_phase(const BnBwdTanArgs& a, con
     for (int k = 0; k < 4; ++k) {
       const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
       if (yy < g.h && xx < g.w) {
-        const long long idx = ((long long)img * g.G + (yy + 1) * g.gw + (xx + 1)) * g.F + it.q * 4;
+        const long long idx = it.grid(g, img, yy, xx);
         const float4 zh = ld4(zhp + idx), zd = ld4(zhd + idx), dzv = ld4(dzp + idx);
         float4 o;
         o.x = rq.x * dzv.x + rg.x * ((arg.x == k ? dyd.x : 0.f) - t1.x - zd.x * c2.x - zh.x * t2.x);
@@ -784,9 +790,7 @@ __global__ void __launch_bounds__(256) tail_onchip_kernel(BnActArgs fa, HeadArgs
     have[i] = worker && wi < it.NW;
     full[i] = false;
     if (!have[i]) continue;
-    const int img = wi / (it.hc * it.wc);
-    const int rem = wi - img * it.hc * it.wc;
-    const int wy = rem / it.wc, wx = rem - wy * it.wc;
+    int img, wy, wx; it.window(wi, img, wy, wx);
     img_[i] = img; wy_[i] = wy; wx_[i] = wx;
     float4 best = make_float4(0.f, 0.f, 0.f, 0.f), ybest = best;
     int4 am = make_int4(0, 0, 0, 0);
@@ -795,7 +799,7 @@ __global__ void __launch_bounds__(256) tail_onchip_kernel(BnActArgs fa, HeadArgs
       const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
       zh[i][k] = make_float4(0.f, 0.f, 0.f, 0.f);
       if (yy < g.h && xx < g.w) {
-        const long long idx = ((long long)img * g.G + (yy + 1) * g.gw + (xx + 1)) * g.F + it.q * 4;
+        const long long idx = it.grid(g, img, yy, xx);
         const float4 zv = ld4(z + idx);
         float4 zz, y, act;
         zz.x = (zv.x - mu.x) * r.x; zz.y = (zv.y - mu.y) * r.y; zz.z = (zv.z - mu.z) * r.z; zz.w = (zv.w - mu.w) * r.w;
@@ -816,7 +820,7 @@ __global__ void __launch_bounds__(256) tail_onchip_kernel(BnActArgs fa, HeadArgs
     sl[i] = make_float4(slope_of(ybest.x), slope_of(ybest.y), slope_of(ybest.z), slope_of(ybest.w));
     full[i] = (wy < g.ph && wx < g.pw);
     if (full[i]) {
-      const long long pidx = ((long long)img * g.pG + (wy + g.pb) * g.pgw + (wx + g.pb)) * g.F + it.q * 4;
+      const long long pidx = it.pooled(g, img, wy, wx);
       st4(pg + pidx, best);
       st4(s_f + pidx, best);                       // pb = 0 on the last block: pidx is the feature index img * D + ...
     }
@@ -842,7 +846,7 @@ __global__ void __launch_bounds__(256) tail_onchip_kernel(BnActArgs fa, HeadArgs
   for (int i = 0; i < MAXI; ++i) {
     dyv[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     if (!have[i] || !full[i]) continue;
-    const long long pidx = ((long long)img_[i] * g.pG + (wy_[i] + g.pb) * g.pgw + (wx_[i] + g.pb)) * g.F + it.q * 4;
+    const long long pidx = it.pooled(g, img_[i], wy_[i], wx_[i]);
     const float4 d = ld4(s_df + pidx);
     dyv[i] = make_float4(d.x * sl[i].x, d.y * sl[i].y, d.z * sl[i].z, d.w * sl[i].w);
     s1[0] += dyv[i].x; s2[0] += (double)dyv[i].x * (double)pick(zh[i], arg[i].x, 0);
@@ -867,7 +871,7 @@ __global__ void __launch_bounds__(256) tail_onchip_kernel(BnActArgs fa, HeadArgs
     for (int k = 0; k < 4; ++k) {
       const int yy = 2 * wy_[i] + (k >> 1), xx = 2 * wx_[i] + (k & 1);
       if (yy < g.h && xx < g.w) {
-        const long long idx = ((long long)img_[i] * g.G + (yy + 1) * g.gw + (xx + 1)) * g.F + it.q * 4;
+        const long long idx = it.grid(g, img_[i], yy, xx);
         float4 o;
         o.x = rg.x * ((full[i] && arg[i].x == k ? dyv[i].x : 0.f) - c1.x - zh[i][k].x * c2.x);
         o.y = rg.y * ((full[i] && arg[i].y == k ? dyv[i].y : 0.f) - c1.y - zh[i][k].y * c2.y);
@@ -937,12 +941,10 @@ __global__ void __launch_bounds__(256) tail_tan_onchip_kernel(BnActTanArgs fa, H
     full[i] = false;
     dprim[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     if (!have[i]) continue;
-    const int img = wi / (it.hc * it.wc);
-    const int rem = wi - img * it.hc * it.wc;
-    const int wy = rem / it.wc, wx = rem - wy * it.wc;
+    int img, wy, wx; it.window(wi, img, wy, wx);
     img_[i] = img; wy_[i] = wy; wx_[i] = wx;
     full[i] = (wy < g.ph && wx < g.pw);
-    const long long pidx = ((long long)img * g.pG + (wy + g.pb) * g.pgw + (wx + g.pb)) * g.F + it.q * 4;
+    const long long pidx = it.pooled(g, img, wy, wx);
     if (full[i]) dprim[i] = ld4(dpp + pidx);                 // primal d(loss)/d(pooled), written in phase A
     float4 best = make_float4(0.f, 0.f, 0.f, 0.f), ybest = best, pbest = best;
     int4 am = make_int4(0, 0, 0, 0);
@@ -952,7 +954,7 @@ __global__ void __launch_bounds__(256) tail_tan_onchip_kernel(BnActTanArgs fa, H
       zh[i][k] = make_float4(0.f, 0.f, 0.f, 0.f);
       zhd[i][k] = make_float4(0.f, 0.f, 0.f, 0.f);
       if (yy < g.h && xx < g.w) {
-        const long long idx = ((long long)img * g.G + (yy + 1) * g.gw + (xx + 1)) * g.F + it.q * 4;
+        const long long idx = it.grid(g, img, yy, xx);
         const float4 z = ld4(zhp + idx);
         float4 zv = ld4(zd + idx);
         if (zd2) { const float4 z2 = ld4(zd2 + idx); zv.x += z2.x; zv.y += z2.y; zv.z += z2.z; zv.w += z2.w; }
@@ -1007,7 +1009,7 @@ __global__ void __launch_bounds__(256) tail_tan_onchip_kernel(BnActTanArgs fa, H
   for (int i = 0; i < MAXI; ++i) {
     dydv[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     if (!have[i] || !full[i]) continue;
-    const long long pidx = ((long long)img_[i] * g.pG + (wy_[i] + g.pb) * g.pgw + (wx_[i] + g.pb)) * g.F + it.q * 4;
+    const long long pidx = it.pooled(g, img_[i], wy_[i], wx_[i]);
     const float4 dd = ld4(s_dfd + pidx);
     const int ar[4] = {arg[i].x, arg[i].y, arg[i].z, arg[i].w};
     const float slv[4] = {sl[i].x, sl[i].y, sl[i].z, sl[i].w};
@@ -1043,7 +1045,7 @@ __global__ void __launch_bounds__(256) tail_tan_onchip_kernel(BnActTanArgs fa, H
     for (int k = 0; k < 4; ++k) {
       const int yy = 2 * wy_[i] + (k >> 1), xx = 2 * wx_[i] + (k & 1);
       if (yy < g.h && xx < g.w) {
-        const long long idx = ((long long)img_[i] * g.G + (yy + 1) * g.gw + (xx + 1)) * g.F + it.q * 4;
+        const long long idx = it.grid(g, img_[i], yy, xx);
         const float4 dzv = ld4(dzp + idx);
         const float4 z = zh[i][k], zdk = zhd[i][k];
         float4 o;
@@ -1060,44 +1062,38 @@ __global__ void __launch_bounds__(256) tail_tan_onchip_kernel(BnActTanArgs fa, H
 
 // the last block of `n` images is small enough for the fused kernels
 bool tail_fusable(const BnGeom& g, int n_rows, int rows_per_cta) {
-  const int F4 = g.F / 4, wpb = 256 / F4;
-  const int NW = g.n * ((g.h + 1) / 2) * ((g.w + 1) / 2);
-  return launch_ctx().opt->bn_fuse && g.F <= 64 && n_rows <= rows_per_cta && NW <= 4 * wpb;
+  const WinGeom wg = win_geom(g);
+  return launch_ctx().opt->bn_fuse && g.F <= 64 && n_rows <= rows_per_cta && wg.NW <= 4 * wg.wpb;
+}
+
+// Windows per thread (MAXI) of the on-chip tail kernel, 0: the global-memory one.  On chip needs option bit `onchip_bit`,
+// no pooled border, none of the inputs / outputs it lacks (`other_io`: TF32 planes, a second tangent addend), <= 2 windows
+// per thread and its `words` floats of dynamic shared memory within 40 KB.
+static int tail_onchip_items(const BnGeom& g, int onchip_bit, bool other_io, size_t words) {
+  const WinGeom wg = win_geom(g);
+  if (!(launch_ctx().opt->tail_onchip & onchip_bit) || g.pb != 0 || other_io || wg.NW > 2 * wg.wpb ||
+      words * sizeof(float) > 40 * 1024)
+    return 0;
+  return wg.NW <= wg.wpb ? 1 : 2;
 }
 
 void launch_tail_fused(const BnActArgs& fa, const HeadArgs& ha, const BnBwdArgs& ba, cudaStream_t st) {
   ProfScope prof_scope__(PROF_HEAD, 0.0, st);
-  {
-    const int F4 = fa.g.F / 4, wpb = 256 / F4;
-    const int NW = fa.g.n * ((fa.g.h + 1) / 2) * ((fa.g.w + 1) / 2);
-    const size_t words = (size_t)5 * ha.rows_per_cta * ha.N + 2 * (size_t)ha.n * ha.D + (size_t)ha.N * ha.D + ha.N;
-    if ((launch_ctx().opt->tail_onchip & 1) && fa.g.pb == 0 && fa.p_hi == nullptr && NW <= 2 * wpb && words * sizeof(float) <= 40 * 1024) {
-      if (NW <= wpb) launch_pdl(tail_onchip_kernel<1>, dim3(1, fa.tasks), dim3(256), words * sizeof(float), st, tagged(fa), ha, ba);
-      else launch_pdl(tail_onchip_kernel<2>, dim3(1, fa.tasks), dim3(256), words * sizeof(float), st, tagged(fa), ha, ba);
-      CUDA_CHECK_LAUNCH();
-      return;
-    }
-  }
-  const size_t smem = (size_t)5 * ha.rows_per_cta * ha.N * sizeof(float);
-  launch_pdl(tail_fused_kernel, dim3(1, fa.tasks), dim3(256), smem, st, tagged(fa), ha, ba);
+  const size_t words = (size_t)5 * ha.rows_per_cta * ha.N + 2 * (size_t)ha.n * ha.D + (size_t)ha.N * ha.D + ha.N;
+  const int items = tail_onchip_items(fa.g, 1, fa.p_hi != nullptr, words);
+  auto kernel = items == 0 ? tail_fused_kernel : items == 1 ? tail_onchip_kernel<1> : tail_onchip_kernel<2>;
+  const size_t smem = (items ? words : (size_t)5 * ha.rows_per_cta * ha.N) * sizeof(float);
+  launch_pdl(kernel, dim3(1, fa.tasks), dim3(256), smem, st, tagged(fa), ha, ba);
   CUDA_CHECK_LAUNCH();
 }
 
 void launch_tail_tan_fused(const BnActTanArgs& fa, const HeadArgs& ha, const BnBwdTanArgs& ba, cudaStream_t st) {
   ProfScope prof_scope__(PROF_HEAD, 0.0, st);
-  {
-    const int F4 = fa.g.F / 4, wpb = 256 / F4;
-    const int NW = fa.g.n * ((fa.g.h + 1) / 2) * ((fa.g.w + 1) / 2);
-    const size_t words = (size_t)5 * ha.rows_per_cta * ha.N + 3 * (size_t)ha.n * ha.D + 2 * (size_t)ha.N * ha.D + 2 * ha.N;
-    if ((launch_ctx().opt->tail_onchip & 2) && fa.g.pb == 0 && fa.pdot_hi == nullptr && ba.dpdot2 == nullptr && NW <= 2 * wpb && words * sizeof(float) <= 40 * 1024) {
-      if (NW <= wpb) launch_pdl(tail_tan_onchip_kernel<1>, dim3(1, fa.tasks), dim3(256), words * sizeof(float), st, tagged(fa), ha, ba);
-      else launch_pdl(tail_tan_onchip_kernel<2>, dim3(1, fa.tasks), dim3(256), words * sizeof(float), st, tagged(fa), ha, ba);
-      CUDA_CHECK_LAUNCH();
-      return;
-    }
-  }
-  const size_t smem = (size_t)5 * ha.rows_per_cta * ha.N * sizeof(float);
-  launch_pdl(tail_tan_fused_kernel, dim3(1, fa.tasks), dim3(256), smem, st, tagged(fa), ha, ba);
+  const size_t words = (size_t)5 * ha.rows_per_cta * ha.N + 3 * (size_t)ha.n * ha.D + 2 * (size_t)ha.N * ha.D + 2 * ha.N;
+  const int items = tail_onchip_items(fa.g, 2, fa.pdot_hi != nullptr || ba.dpdot2 != nullptr, words);
+  auto kernel = items == 0 ? tail_tan_fused_kernel : items == 1 ? tail_tan_onchip_kernel<1> : tail_tan_onchip_kernel<2>;
+  const size_t smem = (items ? words : (size_t)5 * ha.rows_per_cta * ha.N) * sizeof(float);
+  launch_pdl(kernel, dim3(1, fa.tasks), dim3(256), smem, st, tagged(fa), ha, ba);
   CUDA_CHECK_LAUNCH();
 }
 
