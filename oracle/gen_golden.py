@@ -74,8 +74,9 @@ CASES = {
 }
 
 
-def _envelope(base, hwc, f, l, s, nkt, b, iters, kind=KIND, **over):
-    """One envelope case: H x W x C images, F filters, L stages, S inner steps, N-way K-shot with T targets, B tasks."""
+def _envelope(base, hwc, f, l, s, nkt, b, iters, kind=KIND, moved=None, **over):
+    """One envelope case: H x W x C images, F filters, L stages, S inner steps, N-way K-shot with T targets, B tasks.
+    ``moved``: a seed of ``maml_oracle.moved_state``, applied to the reference model before anything is recorded."""
     (h, w, c), (n, k, t) = hwc, nkt
     d = dict(_TINY, image_height=h, image_width=w, image_channels=c, cnn_num_filters=f, num_stages=l,
              number_of_training_steps_per_iter=s, number_of_evaluation_steps_per_iter=s, num_classes_per_set=n,
@@ -83,7 +84,7 @@ def _envelope(base, hwc, f, l, s, nkt, b, iters, kind=KIND, **over):
     if c != 3:
         d["dataset_name"] = "omniglot_tiny"
     d.update(over)
-    return (base, d, iters, kind)
+    return (base, d, iters, kind) if moved is None else (base, d, iters, kind, moved)
 
 
 # Envelope cases: one seeded configuration per corner of what maml_b200_create admits (filters 16..64, 1..4 stages,
@@ -133,12 +134,46 @@ ENVELOPE_CASES = {
     "env_maml_shared_bn": _envelope("omniglot_maml_5w1s", (18, 26, 3), 48, 2, 4, (3, 2, 2), 2, [(0, 0)],
                                     dataset_name="omniglot_tiny"),
 }
+
+# Moved-state envelope cases (maml_oracle.moved_state, applied to the reference model before anything is recorded):
+# distinct gamma / beta per step and block, one LSLR rate per tensor and step, nonzero biases and running statistics.
+# At the initialisation every one of these is uniform, so a kernel that reads them from the wrong step, block or tensor
+# computes the right numbers there.  Same fixture layout and test battery as ENVELOPE_CASES (which keeps the shape
+# corners, all at the initialisation); one case per path that reads gamma / beta / alpha differently:
+MOVED_CASES = {
+    # MAML++ second order, MSL weights between their extremes, fused tail, tensor cores, two iterations
+    "env_moved_pp": _envelope("mini_imagenet_mamlpp_5w1s", (14, 14, 3), 32, 3, 3, (3, 2, 2), 2, [(3, 0), (3, 1)],
+                              moved=1),
+    # a first-order epoch with the multi-step loss off (one target pass, at the last step).  One iteration: one block-2
+    # weight-gradient element is 7e-8 of max-norm and has opposite signs in the reference's fp32 and fp64 runs; Adam's
+    # first step turns that into +-lr, which moves a second iteration's loss by 3e-4 (fp64 restatements land where the
+    # engine does, the reference's fp32 run does not)
+    "env_moved_first": _envelope("mini_imagenet_mamlpp_5w1s", (16, 16, 3), 32, 3, 3, (3, 2, 2), 2, [(12, 0)],
+                                 moved=2, second_order=False),
+    # plain MAML: shared BatchNorm, the head kernel after the last block (5 x 7 pooling windows per image)
+    "env_moved_maml": _envelope("omniglot_maml_5w1s", (18, 26, 3), 32, 2, 3, (3, 2, 2), 2, [(0, 0)], moved=3,
+                                dataset_name="omniglot_tiny"),
+    # L = 1: the fused tail runs on block 0
+    "env_moved_one_stage": _envelope("omniglot_mamlpp_5w1s", (12, 12, 1), 16, 1, 3, (3, 2, 2), 2, [(3, 0), (3, 1)],
+                                     moved=4),
+    # block 1 65 wide: the handle itself runs the FFMA convolutions
+    "env_moved_ffma": _envelope("omniglot_mamlpp_5w1s", (8, 130, 1), 16, 2, 3, (3, 1, 1), 1, [(3, 0)], moved=5),
+    # S = 8: the largest step-row and LSLR index space
+    "env_moved_eight": _envelope("omniglot_mamlpp_5w1s", (16, 16, 1), 16, 4, 8, (3, 2, 2), 2, [(3, 0), (3, 1)], moved=6),
+}
 CASES.update(ENVELOPE_CASES)
+CASES.update(MOVED_CASES)
 
 
 def case_kind(case):
     c = CASES[case]
     return c[3] if len(c) > 3 else KIND
+
+
+def case_moved(case):
+    """The ``moved_state`` seed of a case, or None (the reference's initialisation)."""
+    c = CASES[case]
+    return c[4] if len(c) > 4 else None
 
 
 def make_args(case):
@@ -161,16 +196,18 @@ def build_reference(args, dtype):
     return model
 
 
-def run_reference_fp32(args, iters, store_inputs, kind=KIND):
+def run_reference_fp32(args, iters, store_inputs, kind=KIND, moved=None):
     """fp32 reference run.  The true model gives the losses / logits / post-Adam state.  The outer
     gradients are captured on a twin model whose ``dataset_name`` lacks 'imagenet' -- the reference clamps
     ``param.grad`` in place between ``backward`` and ``optimizer.step`` (:332-335), so the twin is the only
     way to see the UNCLAMPED gradients without editing the reference.  The twin is reloaded from the true
-    model's parameters before every iteration."""
+    model's parameters before every iteration.  ``moved``: a ``moved_state`` seed applied to the model first."""
     import copy
     import warnings
     warnings.filterwarnings("ignore")
     model = build_reference(args, torch.float32)
+    if moved is not None:
+        model.load_state_dict(O.moved_state(model.state_dict(), args, moved))
     args_nc = copy.copy(args)
     args_nc.dataset_name = args.dataset_name.replace("imagenet", "imgnet")
     twin = build_reference(args_nc, torch.float32)
@@ -361,18 +398,25 @@ def main():
     for case in which:
         args, argdict, iters = make_args(case)
         kind = case_kind(case)
-        big = not case.startswith("tiny_") and case not in ENVELOPE_CASES
-        blob = run_reference_fp32(args, iters, store_inputs=not big, kind=kind)
+        big = not case.startswith("tiny_") and case not in ENVELOPE_CASES and case not in MOVED_CASES
+        moved = case_moved(case)
+        blob = run_reference_fp32(args, iters, store_inputs=not big, kind=kind, moved=moved)
         state32 = {k[len("state/"):]: v for k, v in blob.items() if k.startswith("state/")}
         blob.update(run_reference_validation(args, iters, state32, kind))
         blob.update(run_reference_fp64(args, iters, state32, big, kind))
         blob["args_json"] = np.array(json.dumps(argdict))
         blob["iters_json"] = np.array(json.dumps(iters))
         blob["kind"] = np.array(kind)
+        if moved is not None:
+            blob["moved"] = np.array(moved)
         path = os.path.join(ROOT, "tests", "golden", case + ".npz")
         np.savez_compressed(path, **blob)
         worst = check_against_oracle(args, blob, iters, kind)
-        print(case, "%.1f KB" % (os.path.getsize(path) / 1024.0),
+        # the reference's own fp32-vs-fp64 distance (live tensors, of max-norm): how tame the inner loop is
+        own = max(float(np.abs(blob[k].astype(np.float64) - blob[k.replace("/grad/", "/grad64/")]).max())
+                  / max(float(np.abs(blob[k.replace("/grad/", "/grad64/")]).max()), 1e-30)
+                  for k in blob if k.startswith("it0/grad/") and "conv.bias" not in k and "conv-bias" not in k)
+        print(case, "%.1f KB" % (os.path.getsize(path) / 1024.0), "fp32 vs fp64 %.1e" % own,
               {k: ("%.1e" % a, "%.1e" % b) for k, (a, b) in worst.items()}, flush=True)
 
 

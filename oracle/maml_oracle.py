@@ -150,6 +150,36 @@ def init_state(args, dtype=torch.float32):
     return OrderedDict((k, v.to(dtype)) for k, v in st.items())
 
 
+def moved_state(state, args, seed):
+    """``state`` moved away from the reference's initialisation, seeded and deterministic: BatchNorm gamma ~ U(0.6, 1.4)
+    and beta ~ 0.2 N(0, 1) per (step, channel), one LSLR rate ~ U(0.02, 0.1) per (tensor, step), conv and linear biases
+    ~ 0.1 N(0, 1), running means ~ 0.1 N(0, 1) and variances ~ U(0.5, 1.5) per (step, channel).  Weights are kept.
+    At the initialisation gamma = 1, beta = 0, the biases are 0 and every rate is equal, so a kernel that reads gamma /
+    beta / alpha from the wrong step, block or tensor, or drops a gamma factor or a bias, computes the right numbers
+    there; here it does not.  The ranges keep the inner loop tame (the reference's own fp32 run stays 1e-6 to 1.6e-5 of
+    max-norm from its fp64 run on the envelope shapes)."""
+    gen = torch.Generator().manual_seed(int(seed))
+    out = OrderedDict()
+    for k, v in state.items():
+        shape = v.shape
+        if k.endswith("norm_layer.weight"):
+            new = 0.6 + 0.8 * torch.rand(shape, generator=gen, dtype=torch.float64)
+        elif k.endswith("norm_layer.bias"):
+            new = 0.2 * torch.randn(shape, generator=gen, dtype=torch.float64)
+        elif k.endswith("running_mean"):
+            new = 0.1 * torch.randn(shape, generator=gen, dtype=torch.float64)
+        elif k.endswith("running_var"):
+            new = 0.5 + torch.rand(shape, generator=gen, dtype=torch.float64)
+        elif k.endswith("conv.bias") or k == LIN_B:
+            new = 0.1 * torch.randn(shape, generator=gen, dtype=torch.float64)
+        elif k.startswith("inner_loop_optimizer."):
+            new = 0.02 + 0.08 * torch.rand(shape, generator=gen, dtype=torch.float64)
+        else:
+            new = v.detach().clone()
+        out[k] = new.to(v.dtype)
+    return out
+
+
 def msl_weights(args, current_epoch):
     """Per-step loss importance vector (reference few_shot_learning_system.py:83-103),
     float64 arithmetic then rounded to float32 exactly like ``torch.Tensor(np_array)``."""
@@ -547,10 +577,12 @@ def manual_train_iter(state, args, batch, epoch, training_phase=True, current_ep
                 continue
             # ---- phase B: reverse sweep
             tbar = {n: torch.zeros_like(state[n]) for n in inner}
+            tgt_b, tgt_g = [None] * num_steps, [None] * num_steps
             for s in reversed(range(num_steps)):
                 if tgt_f[s] is not None:
                     tf_, wgt = tgt_f[s]
-                    tg, tbn, _ = net_backward_manual(tf_, theta[s + 1], state, args, s, y_t, scale=float(wgt))
+                    tg, tbn, tsaved = net_backward_manual(tf_, theta[s + 1], state, args, s, y_t, scale=float(wgt))
+                    tgt_b[s], tgt_g[s] = tsaved, tg
                     for n in inner:
                         tbar[n] = tbar[n] + tg[n]
                     for n, gval in tbn.items():
@@ -560,6 +592,8 @@ def manual_train_iter(state, args, batch, epoch, training_phase=True, current_ep
                             outer[n] += gval
                 for n in inner:
                     outer[lslr_name(n)][s] += -(tbar[n] * sup_g[s][n]).sum()
+                if keep_intermediates and s == 0:
+                    tbar_before0 = dict(tbar)
                 if second_order:
                     u = {n: state[lslr_name(n)][s] * tbar[n] for n in inner}
                     Hu, mixed, tint = tangent_pass(sup_f[s], sup_b[s], theta[s], u, state, args, s, y_s)
@@ -575,8 +609,10 @@ def manual_train_iter(state, args, batch, epoch, training_phase=True, current_ep
             for n in inner:
                 outer[n] += tbar[n]
             if keep_intermediates:
+                # tgt_b / tgt_g: the target backward records and the weighted target gradients per step (None where
+                # the step has no target pass); tbar0: theta-bar before step 0's Hessian term, tbar: after it
                 inter.append({"task": b, "theta": theta, "sup_f": sup_f, "sup_b": sup_b, "sup_g": sup_g,
-                              "tgt_f": tgt_f})
+                              "tgt_f": tgt_f, "tgt_b": tgt_b, "tgt_g": tgt_g, "tbar0": tbar_before0, "tbar": dict(tbar)})
     loss = torch.stack(losses).mean()
     out = {"loss": loss, "accuracy": float(torch.cat(corrects).mean()), "logits": torch.stack(logits_out),
            "msl_weights": w_msl}

@@ -5,10 +5,17 @@ from conftest import load_golden
 from oracle import maml_oracle as O
 
 
+MOVED_SEED = 7
+
+
 def case(name):
     """(args, fp32 state, batch) of a golden case, or of synthetic_c<C>[_w<W>][_f<F>]: a seeded model with C input
     channels, W x W images (14 if not given) and F filters (32 if not given), so that the first-block kernels run at every
-    channel count, at even and odd widths and at filter counts where no golden case covers them."""
+    channel count, at even and odd widths and at filter counts where no golden case covers them.  A ``_moved`` suffix
+    moves the case's state off the initialisation (``maml_oracle.moved_state``): distinct gamma / beta per step."""
+    if name.endswith("_moved"):
+        a, state, batch = case(name[:-len("_moved")])
+        return a, O.moved_state(state, a, MOVED_SEED), batch
     if name.startswith("synthetic_c"):
         from howtotrainyourmamlpytorch_b200 import make_args
         parts = name.split("_")

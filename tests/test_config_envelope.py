@@ -1,12 +1,14 @@
 """The engine across the configurations ``maml_b200_create`` admits (filters 16..64, 1..4 stages, 1..8 inner steps,
 1..4 input channels, 2..32 ways, batches of up to 128 images, any H x W that survives the halvings).
 
-Every envelope case (``oracle/gen_golden.py`` ENVELOPE_CASES, fixtures generated from the unmodified reference) names
-the axis it exists for and the engine paths it has to reach.  Per case:
+Every envelope case (``oracle/gen_golden.py`` ENVELOPE_CASES and, at moved states, MOVED_CASES; fixtures generated from
+the unmodified reference) names the axis it exists for and the engine paths it has to reach.  Per case:
   * CPU: the fp64 oracle (autograd and manual) reproduces the reference's fp64 run to 1e-12, and the validation leg;
-  * GPU: the path the handle takes (device trace of one iteration), every intermediate of task 0 at the first and last
-    inner step against the fp64 oracle with the GPU's decisions pinned, the decision-forced meta-gradient, the direct
-    golden comparison, the validation leg, the post-Adam state, the functional operator and tensor cores vs FFMA.
+    on the moved-state cases, the fp64 oracle with a gamma / beta / alpha indexing bug lands far from the reference;
+  * GPU: the path the handle takes (device trace of one iteration), every intermediate of task 0 (support and target
+    passes at every inner step, the reverse sweep, step 0's tangent pass) against the fp64 oracle with the GPU's
+    decisions pinned, the decision-forced meta-gradient, the direct golden comparison, the validation leg, the post-Adam
+    state, the functional operator and tensor cores vs FFMA.
 Tolerances are those of the tiny cases in test_gpu_parity.py / test_oracle_golden.py and of the functional-operator
 tests (DESIGN.md section 6)."""
 import json
@@ -45,10 +47,19 @@ ENVELOPE = {
     "env_bern_nonsquare": ("Bernoulli images, exact ties next to the dropped row", dict(tc=True, tail=True)),
     "env_maml_shared_bn": ("plain MAML: shared BatchNorm, no LSLR, non-square, F = 48",
                            dict(tc=True, tail=False)),
+    # moved states (oracle.maml_oracle.moved_state): per-step gamma / beta, per-(tensor, step) LSLR rates, nonzero biases
+    "env_moved_pp": ("moved state: MAML++ second order, MSL between its extremes", dict(tc=True, tail=True)),
+    "env_moved_first": ("moved state: first order, MSL off", dict(tc=True, tail=True)),
+    "env_moved_maml": ("moved state: plain MAML, shared BatchNorm, head kernel", dict(tc=True, tail=False)),
+    "env_moved_one_stage": ("moved state: L = 1, fused tail on block 0", dict(tc=False, tail=True)),
+    "env_moved_ffma": ("moved state: block 1 65 wide, FFMA convolutions", dict(tc=False, tail=True)),
+    "env_moved_eight": ("moved state: S = 8, the largest step and LSLR index space", dict(tc=True, tail=True)),
 }
 CASES = list(ENVELOPE)
+MOVED = [c for c in CASES if c.startswith("env_moved_")]
 BERNOULLI = ["env_bern_nonsquare"]
 H100_SMS = 132
+SWEEP_TOL = 5e-5       # reverse sweep and tangent pass taps, of max-norm (test_stagewise_with_gpu_decisions)
 
 # kernel ids of the device trace (scripts/trace_kernel_ids.json)
 K_CONV_ROWS, K_CONV0, K_WGRAD_ROW, K_WGRAD0 = 1, 2, 3, 4
@@ -110,9 +121,11 @@ def _dead(n):
 # CPU
 # ----------------------------------------------------------------------------------------------------------------------
 def test_case_table_matches_the_generator():
-    """This module's list and the generator's table name the same cases, and every fixture carries its case's args."""
+    """This module's list and the generator's tables name the same cases, and every fixture carries its case's args (and
+    the moved-state cases their moved state)."""
     from oracle import gen_golden
-    assert sorted(CASES) == sorted(gen_golden.ENVELOPE_CASES)
+    assert sorted(c for c in CASES if c not in MOVED) == sorted(gen_golden.ENVELOPE_CASES)
+    assert sorted(MOVED) == sorted(gen_golden.MOVED_CASES)
     for case in CASES:
         _, argdict, iters = gen_golden.make_args(case)
         g = load_golden(case)
@@ -120,6 +133,48 @@ def test_case_table_matches_the_generator():
         assert [list(i) for i in iters] == g.iters, case
         assert g.kind == gen_golden.case_kind(case), case
         assert "it0/xs" in g.blob.files and g.blob["it0/grad64/" + O.LIN_W].dtype == np.float64, case
+        moved = int(g.blob["moved"]) if "moved" in g.blob.files else None
+        assert moved == gen_golden.case_moved(case) and (moved is not None) == (case in MOVED), case
+        if moved is not None:
+            init = O.init_state(g.args)
+            want = O.moved_state(init, g.args, moved)
+            st = g.state()
+            assert list(st) == list(want), case
+            for k in want:
+                assert torch.equal(st[k], want[k]), (case, k)
+
+
+def _mutants(state, args):
+    """The moved state with one indexing bug each, as the engine would see it: gamma / beta of step 0 at every step
+    (per-step BatchNorm only), alpha of step 0 at every step, alpha of the first tensor for every tensor, gamma = 1 and
+    beta = 0."""
+    out = {}
+    bn = [k for k in state if k.endswith("norm_layer.weight") or k.endswith("norm_layer.bias")]
+    lslr = [O.lslr_name(n) for n in O.inner_param_names(args)]
+    if args.per_step_bn_statistics:
+        out["gamma/beta of step 0"] = dict(state, **{k: state[k][:1].expand_as(state[k]).clone() for k in bn})
+    out["alpha of step 0"] = dict(state, **{k: state[k][:1].expand_as(state[k]).clone() for k in lslr})
+    out["alpha of tensor 0"] = dict(state, **{k: state[lslr[0]].clone() for k in lslr})
+    out["gamma = 1, beta = 0"] = dict(state, **{k: (torch.ones_like(state[k]) if k.endswith("weight")
+                                                   else torch.zeros_like(state[k])) for k in bn})
+    return out
+
+
+@pytest.mark.parametrize("case", MOVED)
+def test_moved_state_tells_indexing_bugs_apart(case):
+    """At a moved state, the fp64 oracle with any one of the indexing bugs above lands >= 1e-3 of max-norm away from the
+    reference's fp64 meta-gradient on some live tensor (at the reference's initialisation the same bugs agree to ~1e-14):
+    a regenerated fixture that drifts back to an uninformative state fails here."""
+    g = load_golden(case)
+    state, ref = g.state(torch.float64), g.grads(0, "64")
+    rows = []
+    for name, st in _mutants(state, g.args).items():
+        res = O.autograd_train_iter(st, g.args, g.batch(0), g.iters[0][0])
+        dist = max(float((res["grads"][n] - ref[n]).abs().max()) / float(ref[n].abs().max())
+                   for n in ref if not _dead(n))
+        rows.append((name, dist))
+    print("\n[%s] mutant distance to the reference (of max-norm): %s" % (case, ", ".join("%s %.2e" % r for r in rows)))
+    assert all(d >= 1e-3 for _, d in rows), rows
 
 
 @pytest.mark.parametrize("case", CASES)
@@ -200,9 +255,11 @@ def test_path_reached(case, cuda_device):
         assert {K_CONV_ROWS, K_WGRAD_ROW} <= ids and not ids & {K_CONV_TC, K_WGRAD_TC}, sorted(ids)
     else:
         assert not ids & {K_CONV_ROWS, K_WGRAD_ROW, K_CONV_TC, K_WGRAD_TC}, sorted(ids)
+    second_order = bool(a.second_order) and epoch > a.first_order_to_second_order_epoch
     if want["tail"]:
-        # support passes through tail_fused or tail_onchip, tangent passes through tail_tan_fused (second order)
-        assert ids & {K_TAIL, K_TAIL_ONCHIP} and K_TAIL_TAN in ids, sorted(ids)
+        # support passes through tail_fused or tail_onchip, tangent passes through tail_tan_fused (second order only:
+        # a first-order iteration runs no tangent pass)
+        assert ids & {K_TAIL, K_TAIL_ONCHIP} and (K_TAIL_TAN in ids) == second_order, sorted(ids)
     else:
         assert not ids & {K_TAIL, K_TAIL_ONCHIP, K_TAIL_TAN}, sorted(ids)
     # the ring depth and the chunk count have no kernel id: the host rule stands in for them
@@ -239,8 +296,9 @@ def _decision_flips(intermediates):
 
 def _forced_run(case, device):
     """One meta_gradient with every target pass kept, the GPU's decisions, and the fp64 oracle with them pinned.  Kept
-    per case for the stage-wise and the decision-forced test: the engine's task-0 taps at the first and last step, the
-    oracle's task-0 intermediates, the decision statistics and both results."""
+    per case for the stage-wise and the decision-forced test: the engine's task-0 taps (every support and target pass,
+    every tgrad[s], u and theta-bar after the reverse sweep, the tangent pass of step 0), the oracle's task-0
+    intermediates, the decision statistics and both results."""
     if case not in _RUNS:
         g = load_golden(case)
         a = g.args
@@ -250,15 +308,28 @@ def _forced_run(case, device):
         dec = gpu_decisions(m, g, batch, epoch)
         ref = O.manual_train_iter(g.state(torch.float64), a, batch, epoch, decisions=dec, keep_intermediates=True)
         eng, L, S = m._engine, int(a.num_stages), int(a.number_of_training_steps_per_iter)
+        sched = O.target_pass_schedule(a, epoch, True, S)
         taps = {}
-        for s in sorted({0, S - 1}):
+        for s in range(S):
             taps[("theta", s, 0)] = eng.debug_read("theta", 0, s, 0)
             taps[("g", s, 0)] = eng.debug_read("g", 0, s, 0)
-            for l in range(L):
-                for name in ("sup_zh", "sup_dp", "sup_dz"):
-                    taps[(name, s, l)] = eng.debug_read(name, 0, s, l)
-                taps[("sup_ain", s, l + 1)] = eng.debug_read("sup_ain", 0, s, l + 1)
+            passes = ("sup", "tgt") if sched[s] is not None else ("sup",)
+            if sched[s] is not None:
+                taps[("tgrad", s, 0)] = eng.debug_read("tgrad", 0, s, 0)
+            for p in passes:
+                for l in range(L):
+                    for name in ("_zh", "_dp", "_dz"):
+                        taps[(p + name, s, l)] = eng.debug_read(p + name, 0, s, l)
+                    taps[(p + "_ain", s, l + 1)] = eng.debug_read(p + "_ain", 0, s, l + 1)
+        taps[("u", 0, 0)] = eng.debug_read("u", 0, 0, 0)
+        taps[("tbar", 0, 0)] = eng.debug_read("tbar", 0, 0, 0)
+        for l in range(L):                          # the tangent pass buffers hold step 0's, the last one run
+            for name in ("tan_zh", "tan_dp", "tan_dz"):
+                taps[(name, 0, l)] = eng.debug_read(name, 0, 0, l)
+            taps[("tan_ain", 0, l + 1)] = eng.debug_read("tan_ain", 0, 0, l + 1)
+        tang0 = [x for x in ref["intermediates"] if "Hu" in x and x["task"] == 0 and x["step"] == 0]
         _RUNS[case] = dict(taps=taps, inter0=[x for x in ref["intermediates"] if "theta" in x and x["task"] == 0][0],
+                           tang0=tang0[0] if tang0 else None, sched=sched,
                            flips=_decision_flips(ref["intermediates"]), loss=float(losses["loss"]),
                            logits=np.stack(preds), grads={n: t.detach().cpu() for n, t in grads.items()},
                            ref_loss=float(ref["loss"]), ref_grads=ref["grads"], ref_logits=ref["logits"])
@@ -269,15 +340,19 @@ def _forced_run(case, device):
 @gpu
 @pytest.mark.parametrize("case", CASES)
 def test_stagewise_with_gpu_decisions(case, cuda_device):
-    """theta, zh, pool, dp, dz and g of every block of task 0 at the first and the last inner step against the fp64
-    oracle with the GPU's decisions pinned: what locates a fault.  Tolerances of test_stagewise_against_oracle."""
+    """Every materialised intermediate of task 0 against the fp64 oracle with the GPU's decisions pinned: what locates a
+    fault.  Phase A: theta, zh, pool, dp, dz and g of every block at every inner step, and the same of every target pass
+    with its weighted gradient tgrad[s].  Phase B: u = alpha[.][0] * theta-bar and theta-bar after the sweep, H u of step
+    0 (= u / alpha[.][0] - theta-bar), and the tangent pass of step 0 (zh-dot, p-dot, dz-dot, dp-dot).  Tolerances of
+    test_stagewise_against_oracle for the passes; the reverse sweep's are set from measured errors (see below)."""
     g = load_golden(case)
     a = g.args
     run = _forced_run(case, cuda_device)
-    taps, inter = run["taps"], run["inter0"]
+    taps, inter, tang0 = run["taps"], run["inter0"], run["tang0"]
     geo, (ph, pw) = geometry(a)
     F = int(a.cnn_num_filters)
-    n_s = int(a.num_classes_per_set) * int(a.num_samples_per_class)
+    n_of = {"sup": int(a.num_classes_per_set) * int(a.num_samples_per_class),
+            "tgt": int(a.num_classes_per_set) * int(a.num_target_samples)}
     S = int(a.number_of_training_steps_per_iter)
     L = len(geo)
     rows, worst, worst_name = [], 0.0, ""
@@ -290,38 +365,67 @@ def test_stagewise_with_gpu_decisions(case, cuda_device):
         if r > worst:
             worst, worst_name = r, name
 
-    for s in sorted({0, S - 1}):
-        th = theta_to_ref(taps[("theta", s, 0)], a)
-        for n, v in inter["theta"][s].items():
-            chk("theta[%d] %s" % (s, n[-22:]), th[n], v, absolute=1e-5 if "conv.bias" in n else None)
-        fwd = inter["sup_f"][s]
-        for l in range(L):
-            gl = geo[l]
-            zh = grid_to_nchw(taps[("sup_zh", s, l)], n_s, gl["h"], gl["w"], F)
-            chk("sup zh   s%d l%d" % (s, l), zh, fwd["blocks"][l]["zh"], tol=2e-5)
-            if l + 1 < L:
-                p = grid_to_nchw(taps[("sup_ain", s, l + 1)], n_s, gl["h"] // 2, gl["w"] // 2, F)
-            else:
-                p = flat_to_nchw(taps[("sup_ain", s, L)], n_s, ph, pw, F)
-            chk("sup pool s%d l%d" % (s, l), p, fwd["blocks"][l]["p"], tol=2e-5)
-        bwd = inter["sup_b"][s]
-        for l in reversed(range(L)):
-            gl = geo[l]
-            if l + 1 < L:
-                dp = grid_to_nchw(taps[("sup_dp", s, l)], n_s, gl["h"] // 2, gl["w"] // 2, F)
-            else:
-                dp = flat_to_nchw(taps[("sup_dp", s, l)], n_s, ph, pw, F)
-            chk("sup dp   s%d l%d" % (s, l), dp, bwd["blocks"][l]["dp"], tol=5e-5)
-            dz = grid_to_nchw(taps[("sup_dz", s, l)], n_s, gl["h"], gl["w"], F)
-            chk("sup dz   s%d l%d" % (s, l), dz, bwd["blocks"][l]["dz"], tol=5e-5)
-        gg = theta_to_ref(taps[("g", s, 0)], a)
-        for n, v in inter["sup_g"][s].items():
+    def chk_params(what, got, want, tol, bias_tol, dead_abs):
+        """One parameter-shaped vector: conv biases (dead) absolutely, the linear bias (a sum of softmax - onehot rows
+        that cancels to ~1e-2 of its terms) at bias_tol."""
+        for n, v in want.items():
             if "conv.bias" in n:
-                chk("g[%d] %s" % (s, n[-22:]), gg[n], v, absolute=1e-5)
-            elif "linear.bias" in n:
-                chk("g[%d] %s" % (s, n[-22:]), gg[n], v, tol=2e-4)
+                chk("%s %s" % (what, n[-22:]), got[n], v, absolute=dead_abs)
             else:
-                chk("g[%d] %s" % (s, n[-22:]), gg[n], v, tol=5e-5)
+                chk("%s %s" % (what, n[-22:]), got[n], v, tol=bias_tol if "linear.bias" in n else tol)
+
+    def grid(buf, n, l, pooled):
+        """A tap of block l (pooled: its output / its dp) in NCHW: padded grid, or the flat features after the last."""
+        gl = geo[l]
+        if not pooled:
+            return grid_to_nchw(buf, n, gl["h"], gl["w"], F)
+        if l + 1 < L:
+            return grid_to_nchw(buf, n, gl["h"] // 2, gl["w"] // 2, F)
+        return flat_to_nchw(buf, n, ph, pw, F)
+
+    def chk_pass(p, s, fwd, bwd):
+        n = n_of[p]
+        for l in range(L):
+            chk("%s zh   s%d l%d" % (p, s, l), grid(taps[(p + "_zh", s, l)], n, l, False), fwd["blocks"][l]["zh"], tol=2e-5)
+            chk("%s pool s%d l%d" % (p, s, l), grid(taps[(p + "_ain", s, l + 1)], n, l, True), fwd["blocks"][l]["p"],
+                tol=2e-5)
+        for l in reversed(range(L)):
+            chk("%s dp   s%d l%d" % (p, s, l), grid(taps[(p + "_dp", s, l)], n, l, True), bwd["blocks"][l]["dp"], tol=5e-5)
+            chk("%s dz   s%d l%d" % (p, s, l), grid(taps[(p + "_dz", s, l)], n, l, False), bwd["blocks"][l]["dz"], tol=5e-5)
+
+    for s in range(S):
+        chk_params("theta[%d]" % s, theta_to_ref(taps[("theta", s, 0)], a), inter["theta"][s], 1e-5, 1e-5, 1e-5)
+        chk_pass("sup", s, inter["sup_f"][s], inter["sup_b"][s])
+        chk_params("g[%d]" % s, theta_to_ref(taps[("g", s, 0)], a), inter["sup_g"][s], 5e-5, 2e-4, 1e-5)
+        if run["sched"][s] is not None:
+            chk_pass("tgt", s, inter["tgt_f"][s][0], inter["tgt_b"][s])
+            chk_params("tgrad[%d]" % s, theta_to_ref(taps[("tgrad", s, 0)], a), inter["tgt_g"][s], 5e-5, 2e-4, 1e-5)
+
+    # reverse sweep: u and theta-bar after it, H u of step 0 = u / alpha - theta-bar (theta-bar's own error cancels
+    # there: what is left is the tangent pass's error and one rounding of theta-bar), and step 0's tangent pass.
+    # Measured on an H100 over every envelope case: <= 6.6e-6 of max-norm -> SWEEP_TOL = 5e-5, a margin of 7x or more
+    state64 = g.state(torch.float64)
+    alpha0 = {n: float(state64[O.lslr_name(n)][0]) for n in inter["tbar"]}
+    u = theta_to_ref(taps[("u", 0, 0)], a)
+    tbar = theta_to_ref(taps[("tbar", 0, 0)], a)
+    dead = 1e-5 * max(1.0, max(float(v.abs().max()) for n, v in inter["tbar"].items() if "conv.bias" not in n))
+    chk_params("u", u, {n: alpha0[n] * v for n, v in inter["tbar0"].items()}, SWEEP_TOL, SWEEP_TOL, dead)
+    chk_params("tbar", tbar, inter["tbar"], SWEEP_TOL, SWEEP_TOL, dead)
+    if tang0 is not None:
+        chk_params("Hu[0]", {n: u[n].double() / alpha0[n] - tbar[n].double() for n in u}, tang0["Hu"], SWEEP_TOL,
+                   SWEEP_TOL, dead / min(alpha0.values()))
+        # with the tensor cores, dp-dot of the blocks below the last holds only the addend dgrad(W, dz-dot); the other,
+        # dgrad(u_W, dz), is computed on a side stream into a buffer of its own
+        tf, tb, theta0, n = tang0["tangent"]["fwd"], tang0["tangent"]["bwd"], inter["theta"][0], n_of["sup"]
+        for l in range(L):
+            chk("tan zh   l%d" % l, grid(taps[("tan_zh", 0, l)], n, l, False), tf[l]["zh_dot"], tol=SWEEP_TOL)
+            chk("tan pool l%d" % l, grid(taps[("tan_ain", 0, l + 1)], n, l, True), tf[l]["p_dot"], tol=SWEEP_TOL)
+        for l in reversed(range(L)):
+            want = tb[l]["dp_dot"]
+            if ENVELOPE[case][1]["tc"] and l + 1 < L:
+                want = Fnn.conv_transpose2d(tb[l + 1]["dz_dot"], theta0[O.conv_names(l + 1)[0]], stride=1, padding=1)
+            chk("tan dp   l%d" % l, grid(taps[("tan_dp", 0, l)], n, l, True), want, tol=SWEEP_TOL)
+            chk("tan dz   l%d" % l, grid(taps[("tan_dz", 0, l)], n, l, False), tb[l]["dz_dot"], tol=SWEEP_TOL)
     print("\n[%s stagewise, GPU decisions pinned] worst %.2f x tolerance at %s\n   %s"
           % (case, worst, worst_name, "\n   ".join(rows)))
     assert worst <= 1.0, "stage mismatch (see report above): worst = %.2f x tolerance at %s" % (worst, worst_name)

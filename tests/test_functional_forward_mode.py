@@ -14,7 +14,8 @@ from oracle import maml_oracle as O
 pytestmark = pytest.mark.gpu
 
 PREFIX = "classifier."
-TINY = ["tiny_pp", "tiny_maml", "tiny_bern", "synthetic_c2", "synthetic_c3", "synthetic_c4"]
+# tiny_pp_moved: distinct gamma / beta per step (the gamma / beta tangent directions scale with the primal gamma)
+TINY = ["tiny_pp", "tiny_maml", "tiny_bern", "synthetic_c2", "synthetic_c3", "synthetic_c4", "tiny_pp_moved"]
 # odd image width: the first block's padded grid rows have an odd length, so every shared-memory tile staged behind an
 # image window must be re-aligned (the two-pair weight-gradient kernels read their second dz tile as float4)
 ODD_WIDTH = ["synthetic_c1_w15", "synthetic_c3_w15"]

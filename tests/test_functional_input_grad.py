@@ -15,7 +15,7 @@ pytestmark = pytest.mark.gpu
 
 PREFIX = "classifier."
 # synthetic_c4_f48: the C0 = 4 weight gradient's stream reduction needs more than the default 48 KB of shared memory
-TINY = ["tiny_pp", "tiny_maml", "tiny_bern", "synthetic_c2", "synthetic_c4", "synthetic_c4_f48"]
+TINY = ["tiny_pp", "tiny_maml", "tiny_bern", "synthetic_c2", "synthetic_c4", "synthetic_c4_f48", "tiny_pp_moved"]
 # B1 backward policy (DESIGN.md section 6): 5e-5 of the fp64 reference's max-norm
 B1_REL = 5e-5
 

@@ -32,19 +32,18 @@ def _check(rows, name, got, want, conv_bias_abs):
     return e <= 5e-5
 
 
-@pytest.mark.parametrize("case", ["tiny_pp", "tiny_maml", "tiny_bern"])
+@pytest.mark.parametrize("case", ["tiny_pp", "tiny_maml", "tiny_bern", "tiny_pp_moved"])
 def test_double_backward_matches_fp64_autograd(case, cuda_device):
     """g = autograd.grad(CE(op(x, fast)), fast, create_graph=True), then autograd.grad(sum <g_i, v_i>) w.r.t. the fast
     weights AND the BatchNorm gamma / beta the module owns, against the same expression through the oracle's
     F.conv2d / F.batch_norm / ... network in float64.  The logits tangent J v reaches the weights through the
     cross-entropy's Hessian, so this exercises both outputs of the engine's pass; it is also compared on its own against
-    torch.func.jvp of the oracle logits.  The gamma / beta rows pin the sign (+H_gamma v)."""
-    g = load_golden(case)
-    a = g.args
-    state = g.state()
+    torch.func.jvp of the oracle logits.  The gamma / beta rows pin the sign (+H_gamma v).  ``tiny_pp_moved``: distinct
+    gamma / beta per step, nonzero biases."""
+    a, state, batch = fc.case(case)
     m = fc.model(a, state, cuda_device)
     named = dict(m.named_parameters())
-    xs, xt, ys, yt = g.batch(0)
+    xs, xt, ys, yt = batch
     x = xs[0].reshape(-1, *xs.shape[-3:])
     y = ys[0].reshape(-1).long()
     inner, bn = O.inner_param_names(a), fc.bn_names(state)

@@ -115,7 +115,8 @@ def test_per_task_entries_at_the_c_abi(case, cuda_device):
 
 
 # ---- 2. vmap of the forward ---------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("case", ["tiny_pp", "tiny_maml", "tiny_bern", "env_nonsquare_odd", "env_c4_two_stages"])
+@pytest.mark.parametrize("case", ["tiny_pp", "tiny_maml", "tiny_bern", "env_nonsquare_odd", "env_c4_two_stages",
+                                  "tiny_pp_moved"])
 def test_vmap_forward_matches_fp64_oracle(case, cuda_device):
     """vmap over B tasks with the weights batched or shared and x batched or shared, against the fp64 oracle per task at
     the B1 policy (5e-5 of max-norm)."""
@@ -169,7 +170,7 @@ def _close(rows, name, got, want):
     return e <= 5e-5
 
 
-@pytest.mark.parametrize("case", ["tiny_pp", "tiny_maml"])
+@pytest.mark.parametrize("case", ["tiny_pp", "tiny_maml", "tiny_pp_moved"])
 def test_vmap_grad_and_grad_of_summed_vmap(case, cuda_device):
     """Per-task gradients of the fast weights, of the module's BatchNorm gamma / beta (shared, passed unbatched) and of x
     (batched), through vmap(grad(loss)) and through grad of the summed vmap, against fp64 autograd per task."""

@@ -63,7 +63,6 @@ def test_stagewise_against_oracle(case, cuda_device):
     eng = m._engine
     ref = O.manual_train_iter(g.state(dtype=torch.float64), a, batch, epoch, keep_intermediates=True)
     inter = [x for x in ref["intermediates"] if "theta" in x and x["task"] == 0][0]
-    tang = {x["step"]: x for x in ref["intermediates"] if "Hu" in x and x["task"] == 0}
     geo, (ph, pw) = geometry(a)
     F = int(a.cnn_num_filters)
     n_s = int(a.num_classes_per_set) * int(a.num_samples_per_class)
