@@ -2,10 +2,15 @@
 import torch
 
 from conftest import load_golden
+from oracle import gen_golden
 from oracle import maml_oracle as O
 
 
 MOVED_SEED = 7
+# Every envelope case and every moved-state case of the fused iteration's fixtures, in the generator's order: the
+# functional-operator tests run on each, so that the operator's own launch plans (sized for n images and B tasks, not for
+# the fused iteration's support + target batch) meet every shape maml_b200_create admits and every moved state
+ENVELOPE = list(gen_golden.ENVELOPE_CASES) + list(gen_golden.MOVED_CASES)
 
 
 def case(name):
@@ -29,6 +34,22 @@ def case(name):
         return a, O.init_state(a), O.synthetic_batch(a, iteration=5, kind="normal")
     g = load_golden(name)
     return g.args, g.state(), g.batch(0)
+
+
+def widen(batch, tasks=3):
+    """The batch with at least `tasks` tasks, for the tests of the per-task entries: task b >= B (the fixture's B) is
+    task b % B with its images at x * 0.5^k + 0.1 k, k = b - B + 1, and its labels.  A batch of `tasks` or more tasks is
+    returned as it is."""
+    xs, xt, ys, yt = batch
+    B = xs.shape[0]
+
+    def more(t, images):
+        rows = [t]
+        for b in range(B, tasks):
+            k = b - B + 1
+            rows.append(t[b % B:b % B + 1] * 0.5 ** k + 0.1 * k if images else t[b % B:b % B + 1])
+        return torch.cat(rows)
+    return more(xs, True), more(xt, True), more(ys, False), more(yt, False)
 
 
 def model(a, state, device):

@@ -121,11 +121,13 @@ def _dead(n):
 # CPU
 # ----------------------------------------------------------------------------------------------------------------------
 def test_case_table_matches_the_generator():
-    """This module's list and the generator's tables name the same cases, and every fixture carries its case's args (and
-    the moved-state cases their moved state)."""
+    """This module's list, the functional-operator tests' list (functional_cases.ENVELOPE) and the generator's tables name
+    the same cases, and every fixture carries its case's args (and the moved-state cases their moved state)."""
     from oracle import gen_golden
     assert sorted(c for c in CASES if c not in MOVED) == sorted(gen_golden.ENVELOPE_CASES)
     assert sorted(MOVED) == sorted(gen_golden.MOVED_CASES)
+    assert fc.ENVELOPE == list(gen_golden.ENVELOPE_CASES) + list(gen_golden.MOVED_CASES)
+    assert sorted(fc.ENVELOPE) == sorted(CASES)
     for case in CASES:
         _, argdict, iters = gen_golden.make_args(case)
         g = load_golden(case)

@@ -67,7 +67,7 @@ def _op_jt(m, a, x, step, w, gb, xd, device):
 
 
 @pytest.mark.parametrize("direction", DIRECTIONS)
-@pytest.mark.parametrize("case", TINY)
+@pytest.mark.parametrize("case", TINY + fc.ENVELOPE)
 def test_jvp_matches_fp64_autograd(case, direction, cuda_device):
     """J t (logits tangent) against torch.func.jvp in float64 through the oracle's network, at the first and last step, on
     the support and the target batch shape."""
@@ -88,7 +88,7 @@ def test_jvp_matches_fp64_autograd(case, direction, cuda_device):
     assert worst <= B1_REL, rows
 
 
-@pytest.mark.parametrize("case", TINY + ODD_WIDTH)
+@pytest.mark.parametrize("case", TINY + ODD_WIDTH + fc.ENVELOPE)
 def test_forward_over_reverse_matches_fp64_autograd(case, cuda_device):
     """Tangents of the weight gradients and of dx of CE(op(x, fast)) along (x_dot, theta_dot) -- with the d(logits) tangent
     that cross-entropy's backward produces -- against torch.func.jvp(torch.func.grad(...)) in float64."""
@@ -271,6 +271,47 @@ def test_c_abi_tasks_and_zero_image_tangent(cuda_device):
     eng.net_hvp(2, step, meta, x2, dl, t_like, jv_a, hv_a)
     eng.net_hvp_image(2, step, meta, x2, torch.zeros_like(x2), dl, t_like, jv_b, hv_b)
     assert torch.equal(jv_a, jv_b) and torch.equal(hv_a, hv_b)
+
+
+# kernel ids of the device trace (scripts/trace_kernel_ids.json)
+K_CONV0, K_WGRAD0, K_INPUT_GRAD0, K_BNACT_TAN_GB = 2, 4, 31, 32
+
+
+@pytest.mark.parametrize("case, call", [("env_c4_two_stages", "hvp_image"), ("env_ring_edge", "hvp_image"),
+                                        ("env_one_stage", "jvp")])
+def test_envelope_calls_reach_their_kernels(case, call, cuda_device):
+    """The device trace of one call at the shapes the envelope parametrizations above exist for: net_hvp_image with
+    x_dot != 0 and then net_hvp_input_grad run the first-block convolution and weight gradient and the image-gradient
+    kernel, here in their two-pair forms (C0 = 4 with F = 64; C0 = 3 with F = 64 on 124-wide images, where the image
+    gradient needs more than 48 KB of shared memory); net_jvp at L = 1 runs the gamma / beta-tangent BatchNorm kernel on
+    block 0, whose pooled tangent is the head's input."""
+    a, state, batch = fc.case(case)
+    m = fc.model(a, state, cuda_device)
+    x, _ = fc.images(batch, "support")
+    x = x.unsqueeze(0).contiguous().to(cuda_device)
+    n, N, step = x.shape[1], int(a.num_classes_per_set), int(a.number_of_training_steps_per_iter) - 1
+    eng = fc.engine(a, n // N, 1, 1, cuda_device)
+    meta = fc.meta_like(m, eng, cuda_device)
+    gen = torch.Generator().manual_seed(3)
+    t_like = torch.randn(eng.meta_size, generator=gen).to(cuda_device)
+    xdot = torch.randn(x.shape, generator=gen).to(cuda_device)
+    dl = torch.randn(1, n, N, generator=gen).to(cuda_device)
+    jv = torch.empty(1, n, N, device=cuda_device)
+    eng.trace(True)
+    if call == "jvp":
+        eng.net_jvp(1, step, meta, x, t_like, None, jv)
+        want = {K_BNACT_TAN_GB}
+    else:
+        eng.net_hvp_image(1, step, meta, x, xdot, dl, t_like, jv, torch.empty(eng.result_size, device=cuda_device))
+        eng.net_hvp_input_grad(1, torch.empty_like(x))
+        want = {K_CONV0, K_WGRAD0, K_INPUT_GRAD0}
+    torch.cuda.synchronize()
+    ids = {k for _, k, _ in eng.trace_read(capacity=1 << 14) if not (k & 0x80)}
+    eng.trace(False)
+    eng.close()
+    print("\n[%s %s] kernel ids %s" % (case, call, sorted(ids)))
+    assert want <= ids, sorted(ids)
+    assert float(jv.abs().max()) > 0
 
 
 def test_gamma_beta_tangent_through_the_gradient_is_refused_before_any_launch(cuda_device):

@@ -71,14 +71,14 @@ def _per_call(case, order, device):
     return worst
 
 
-@pytest.mark.parametrize("case", TINY)
+@pytest.mark.parametrize("case", TINY + fc.ENVELOPE)
 def test_input_grad_matches_fp64_autograd(case, cuda_device):
     """dL/dx of CE(op(x, fast)) against float64 autograd through the oracle's F.conv2d / F.batch_norm / ... network, at the
     first and last step, on the target and the support batch shape."""
     assert _per_call(case, 1, cuda_device) <= B1_REL
 
 
-@pytest.mark.parametrize("case", TINY)
+@pytest.mark.parametrize("case", TINY + fc.ENVELOPE)
 def test_mixed_second_order_input_grad_matches_fp64_autograd(case, cuda_device):
     """d/dx <grad_theta L, v> for a random direction v over the conv / linear fast weights (the backward of the operator's
     backward, taken w.r.t. the images) against float64 autograd."""

@@ -9,7 +9,7 @@ import pytest
 import torch
 import torch.nn.functional as Fnn
 
-from conftest import BERNOULLI_CASES, BIG_CASES, TINY_CASES, load_golden, grad_tolerance
+from conftest import BIG_CASES, TINY_CASES, load_golden, grad_tolerance
 from engine_layout import rel_err
 import functional_cases as fc
 from oracle import maml_oracle as O
@@ -32,7 +32,7 @@ def _check(rows, name, got, want, conv_bias_abs):
     return e <= 5e-5
 
 
-@pytest.mark.parametrize("case", ["tiny_pp", "tiny_maml", "tiny_bern", "tiny_pp_moved"])
+@pytest.mark.parametrize("case", ["tiny_pp", "tiny_maml", "tiny_bern", "tiny_pp_moved"] + fc.ENVELOPE)
 def test_double_backward_matches_fp64_autograd(case, cuda_device):
     """g = autograd.grad(CE(op(x, fast)), fast, create_graph=True), then autograd.grad(sum <g_i, v_i>) w.r.t. the fast
     weights AND the BatchNorm gamma / beta the module owns, against the same expression through the oracle's
@@ -128,7 +128,7 @@ def _reference_loop_on_operator(m, a, batch, epoch, device):
     return float(loss.detach()), torch.stack(logits_out), grads, stats
 
 
-@pytest.mark.parametrize("case", TINY_CASES + ["omniglot_mamlpp_5w1s"])
+@pytest.mark.parametrize("case", TINY_CASES + ["omniglot_mamlpp_5w1s"] + fc.ENVELOPE)
 def test_reference_loop_on_operator_matches_goldens(case, cuda_device):
     """The reference's training loop, second order where the config says so, with the network replaced by this
     operator: loss, last-step logits and every meta-gradient (LSLR included) vs the golden fixtures of the unmodified
@@ -156,7 +156,7 @@ def test_reference_loop_on_operator_matches_goldens(case, cuda_device):
     rows, bad = [], []
     for n in g64:
         got = grads[n].double()
-        if case in BERNOULLI_CASES and not big and not ("conv.bias" in n or "conv-bias" in n):
+        if g.kind == "bernoulli" and not big and not ("conv.bias" in n or "conv-bias" in n):
             e32 = float((got - g32[n].double()).abs().max())
             own = float((g32[n].double() - g64[n].double()).abs().max())
             if e32 > max(3.0 * own, 2e-5 * float(g32[n].abs().max())) + 1e-7:
