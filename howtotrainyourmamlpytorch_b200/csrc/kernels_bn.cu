@@ -11,8 +11,6 @@
 #include "common.cuh"
 #include "head_body.cuh"
 
-struct Chan4 { float4 mu, r, g, b; };
-
 __device__ __forceinline__ float leaky(float y) { return y > 0.f ? y : LEAKY_SLOPE_F * y; }
 __device__ __forceinline__ float slope_of(float y) { return y > 0.f ? 1.f : LEAKY_SLOPE_F; }
 
@@ -48,8 +46,129 @@ __device__ __forceinline__ void st4_split(float* hi, float* lo, long long idx, f
   st4(lo + idx, l);
 }
 __device__ __forceinline__ float4 ld4s(const float* s, int q) { return make_float4(s[q * 4], s[q * 4 + 1], s[q * 4 + 2], s[q * 4 + 3]); }
+// p[i] + p2[i]: a tangent that arrives as two addends; p2 may be null (one addend)
+__device__ __forceinline__ float4 ld4_sum(const float* p, const float* p2, long long i) {
+  float4 v = ld4(p + i);
+  if (p2) { const float4 v2 = ld4(p2 + i); v.x += v2.x; v.y += v2.y; v.z += v2.z; v.w += v2.w; }
+  return v;
+}
+// channel c of a quad; c is a constant at every use (the loops over channels are unrolled)
+template <class V> __device__ __forceinline__ auto comp(const V& v, int c) { return c == 0 ? v.x : c == 1 ? v.y : c == 2 ? v.z : v.w; }
+// f applied channel by channel to the quads v...: make_float4(f(v.x...), f(v.y...), f(v.z...), f(v.w...))
+template <class F, class... V> __device__ __forceinline__ float4 map4(F f, const V&... v) {
+  return make_float4(f(v.x...), f(v.y...), f(v.z...), f(v.w...));
+}
+__device__ __forceinline__ float4 mul4(const float4& a, const float4& b) { return make_float4(a.x * b.x, a.y * b.y, a.z * b.z, a.w * b.w); }
+__device__ __forceinline__ float4 slope_of(const float4& y) { return make_float4(slope_of(y.x), slope_of(y.y), slope_of(y.z), slope_of(y.w)); }
 
-#define F4_OP(out, expr) { out.x = expr(x); out.y = expr(y); out.z = expr(z); out.w = expr(w); }
+// a_k for the run-time arg-max position k, as a select chain: indexing a register array with k would move it to local
+// memory (STL / LDL in the middle of latency-bound kernels)
+template <class T> __device__ __forceinline__ T select4(int k, T a0, T a1, T a2, T a3) { return k == 0 ? a0 : k == 1 ? a1 : k == 2 ? a2 : a3; }
+template <class T> __device__ __forceinline__ T pick(const T (&v)[4], int k) { return select4(k, v[0], v[1], v[2], v[3]); }
+// channel c of v[k]
+__device__ __forceinline__ float pick(const float4 (&v)[4], int k, int c) {
+  return select4(k, comp(v[0], c), comp(v[1], c), comp(v[2], c), comp(v[3], c));
+}
+
+// ------------------------------------------------------------------------------- per-element formulas
+// Every kernel below computes these through the functions here, so the forward and the backward-type kernels agree by
+// construction.
+
+// zh = (z - mu) * r
+__device__ __forceinline__ float4 bn_normalize(const float4& z, const float4& mu, const float4& r) {
+  return map4([](float z, float mu, float r) { return (z - mu) * r; }, z, mu, r);
+}
+
+// y = gamma * zh + beta (one explicit fma) and act = leaky(y) at one window position
+struct BnAct { float4 y, act; };
+__device__ __forceinline__ BnAct bn_act(const float4& ga, const float4& zh, const float4& be) {
+  BnAct v;
+  v.y = map4([](float ga, float zh, float be) { return fmaf(ga, zh, be); }, ga, zh, be);
+  v.act = map4([](float y) { return leaky(y); }, v.y);
+  return v;
+}
+
+// The max-pool decision.  The positions k = 0..3 of a window are offered in order (k = 0 is always inside the image); per
+// channel, a position replaces the maximum so far only if its act is strictly greater, so the first maximum wins, as in
+// F.max_pool2d.  No mask is stored: every backward-type kernel recomputes the decision from zh through bn_act and this
+// function, and so reaches the forward's decision.  The maximum carries the winner's y, position and p (a value of the
+// caller's: the tangent of the pooled value).  A window starts from WinMax{} (arg = 0 for position 0).
+struct WinMax { int4 arg; float4 p, y, act; };
+__device__ __forceinline__ void keep_first_max(int k, const BnAct& v, WinMax& w, const float4& p = float4()) {
+  if (k == 0) { w.act = v.act; w.y = v.y; w.p = p; }
+  else {
+    if (v.act.x > w.act.x) { w.act.x = v.act.x; w.y.x = v.y.x; w.p.x = p.x; w.arg.x = k; }
+    if (v.act.y > w.act.y) { w.act.y = v.act.y; w.y.y = v.y.y; w.p.y = p.y; w.arg.y = k; }
+    if (v.act.z > w.act.z) { w.act.z = v.act.z; w.y.z = v.y.z; w.p.z = p.z; w.arg.z = k; }
+    if (v.act.w > w.act.w) { w.act.w = v.act.w; w.y.w = v.y.w; w.p.w = p.w; w.arg.w = k; }
+  }
+}
+
+// tangent of act at one position: slope * gamma * zhdot; GB (gamma / beta carry tangents gd, bd):
+// slope * (gamma zhdot + gd zh + bd).  Two formulas: the first is not the second with gd = bd = 0 (rounding).
+template <bool GB>
+__device__ __forceinline__ float4 act_tangent(const BnAct& v, const float4& ga, const float4& zhd, const float4& zh,
+                                              const float4& gd = float4(), const float4& bd = float4()) {
+  return map4([](float y, float ga, float zhd, float zh, float gd, float bd) {
+    return GB ? slope_of(y) * (ga * zhd + fmaf(gd, zh, bd)) : slope_of(y) * ga * zhd;
+  }, v.y, ga, zhd, zh, gd, bd);
+}
+
+// tangent of zh: zhdot = r * (zdot - mean(zdot) - zh * q), q = mean(zh * zdot)
+__device__ __forceinline__ float4 bn_tan_normalize(const float4& zd, const float4& zh, const float4& r, const float4& md,
+                                                   const float4& qq) {
+  return map4([](float zd, float zh, float r, float md, float q) { return r * (zd - md - zh * q); }, zd, zh, r, md, qq);
+}
+
+// backward sums of a full window at its arg-max: S1 += dy, S2 += dy * zh (fp64), dy = dp * slope.  Returns dy.
+__device__ __forceinline__ float4 bn_bwd_sums(const float4& dp, const float4& sl, const float4 (&zh)[4], const int4& arg,
+                                              double (&s1)[4], double (&s2)[4]) {
+  const float4 dy = mul4(dp, sl);
+  s1[0] += dy.x; s2[0] += (double)dy.x * (double)pick(zh, arg.x, 0);
+  s1[1] += dy.y; s2[1] += (double)dy.y * (double)pick(zh, arg.y, 1);
+  s1[2] += dy.z; s2[2] += (double)dy.z * (double)pick(zh, arg.z, 2);
+  s1[3] += dy.w; s2[3] += (double)dy.w * (double)pick(zh, arg.w, 3);
+  return dy;
+}
+
+// tangent backward sums of a full window at its arg-max: T1 += dydot, T2 += dydot * zh + dy * zhdot (fp64), with
+// dy = dp * slope, dydot = dpdot * slope and zhd_at(k, c) = zhdot of channel c at position k.  Returns dydot.
+template <class ZhdAt>
+__device__ __forceinline__ float4 bn_tan_bwd_sums(const float4& dp, const float4& dpd, const float4& sl, const float4 (&zh)[4],
+                                                  const int4& arg, ZhdAt zhd_at, double (&s1)[4], double (&s2)[4]) {
+  float dyd[4];
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+    const int k = comp(arg, c);
+    const float zhk = pick(zh, k, c), zhdk = zhd_at(k, c);
+    const float dy = comp(dp, c) * comp(sl, c);
+    dyd[c] = comp(dpd, c) * comp(sl, c);
+    s1[c] += dyd[c];
+    s2[c] += (double)dyd[c] * (double)zhk + (double)dy * (double)zhdk;
+  }
+  return make_float4(dyd[0], dyd[1], dyd[2], dyd[3]);
+}
+
+// dz = r * gamma * (dy - S1/m - zh * S2/m) at window position k, rg = r * gamma, c1 / c2 = S1/m / S2/m; dy (the pooled
+// gradient times the slope) reaches only the arg-max of a full window.  NO_DY: a position of a partial window,
+// r * gamma * (-S1/m - zh * S2/m); its zero results can differ in sign from those of 0 - S1/m - ...
+template <bool NO_DY = false>
+__device__ __forceinline__ float4 bn_bwd_dz(const float4& rg, const float4& c1, const float4& zh, const float4& c2, int k = 0,
+                                            const int4& arg = int4(), const float4& dy = float4(), bool full = true) {
+  return map4([k, full](float rg, float c1, float zh, float c2, int arg, float dy) {
+    return rg * ((NO_DY ? -c1 : (full && arg == k ? dy : 0.f) - c1) - zh * c2);
+  }, rg, c1, zh, c2, arg, dy);
+}
+
+// dzdot = -r * q * dz + r * gamma * (dydot - T1/m - zhdot * S2/m - zh * T2/m) at window position k, rq = -r * q; dydot
+// reaches only the arg-max of a full window
+__device__ __forceinline__ float4 bn_tan_bwd_dz(const float4& rq, const float4& dz, const float4& rg, const float4& t1,
+                                                const float4& zhd, const float4& c2, const float4& zh, const float4& t2, int k,
+                                                const int4& arg, const float4& dyd, bool full = true) {
+  return map4([k, full](float rq, float dz, float rg, float t1, float zhd, float c2, float zh, float t2, int arg, float dyd) {
+    return rq * dz + rg * ((full && arg == k ? dyd : 0.f) - t1 - zhd * c2 - zh * t2);
+  }, rq, dz, rg, t1, zhd, c2, zh, t2, arg, dyd);
+}
 
 struct WinIter {
   int hc, wc, NW, F4, WPB, q, lane;
@@ -82,31 +201,21 @@ __device__ __forceinline__ void bnact_phase(const BnActArgs& a, const BnGeom& g,
   float* p = a.p + (long long)task * a.p_stride;
   for (int wi = cta * it.WPB + it.lane; wi < it.NW; wi += ncta * it.WPB) {
     int img, wy, wx; it.window(wi, img, wy, wx);
-    float4 best = make_float4(0.f, 0.f, 0.f, 0.f);
+    WinMax w{};
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
       if (yy < g.h && xx < g.w) {
         const long long idx = it.grid(g, img, yy, xx);
-        const float4 zv = ld4(z + idx);
-        float4 zh, act;
-        zh.x = (zv.x - mu.x) * r.x; zh.y = (zv.y - mu.y) * r.y; zh.z = (zv.z - mu.z) * r.z; zh.w = (zv.w - mu.w) * r.w;
+        const float4 zh = bn_normalize(ld4(z + idx), mu, r);
         st4(z + idx, zh);
-        act.x = leaky(fmaf(ga.x, zh.x, be.x)); act.y = leaky(fmaf(ga.y, zh.y, be.y));
-        act.z = leaky(fmaf(ga.z, zh.z, be.z)); act.w = leaky(fmaf(ga.w, zh.w, be.w));
-        if (k == 0) best = act;
-        else {
-          if (act.x > best.x) best.x = act.x;
-          if (act.y > best.y) best.y = act.y;
-          if (act.z > best.z) best.z = act.z;
-          if (act.w > best.w) best.w = act.w;
-        }
+        keep_first_max(k, bn_act(ga, zh, be), w);
       }
     }
     if (wy < g.ph && wx < g.pw) {
       const long long pidx = it.pooled(g, img, wy, wx);
-      st4(p + pidx, best);
-      if (a.p_hi) st4_split(a.p_hi + (long long)task * a.p_stride, a.p_lo + (long long)task * a.p_stride, pidx, best);
+      st4(p + pidx, w.act);
+      if (a.p_hi) st4_split(a.p_hi + (long long)task * a.p_stride, a.p_lo + (long long)task * a.p_stride, pidx, w.act);
     }
   }
 }
@@ -145,59 +254,20 @@ void launch_bnact(const BnActArgs& a, cudaStream_t st) {
   CUDA_CHECK_LAUNCH();
 }
 
-// value of one window position: loads zh, recomputes y; used by all backward-type kernels
-struct WinPos { float4 zh; float4 y; bool ok; long long idx; };
-
+// a full window of the backward-type kernels: loads zh at its four positions and recomputes the forward's pooling decision
 __device__ __forceinline__ void argmax_window(const float* __restrict__ zhp, const BnGeom& g, int img, int wy, int wx,
                                               const WinIter& it, const float4& ga, const float4& be, float4 (&zh)[4],
                                               long long (&idx)[4], int4& arg, float4& slope_at) {
-  float4 best = make_float4(0.f, 0.f, 0.f, 0.f);
-  float4 ybest = best;
-  arg = make_int4(0, 0, 0, 0);
+  WinMax w{};
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
     idx[k] = it.grid(g, img, yy, xx);
     zh[k] = ld4(zhp + idx[k]);
-    float4 y, act;
-    y.x = fmaf(ga.x, zh[k].x, be.x); y.y = fmaf(ga.y, zh[k].y, be.y);
-    y.z = fmaf(ga.z, zh[k].z, be.z); y.w = fmaf(ga.w, zh[k].w, be.w);
-    act.x = leaky(y.x); act.y = leaky(y.y); act.z = leaky(y.z); act.w = leaky(y.w);
-    if (k == 0) { best = act; ybest = y; }
-    else {
-      if (act.x > best.x) { best.x = act.x; ybest.x = y.x; arg.x = k; }
-      if (act.y > best.y) { best.y = act.y; ybest.y = y.y; arg.y = k; }
-      if (act.z > best.z) { best.z = act.z; ybest.z = y.z; arg.z = k; }
-      if (act.w > best.w) { best.w = act.w; ybest.w = y.w; arg.w = k; }
-    }
+    keep_first_max(k, bn_act(ga, zh[k], be), w);
   }
-  slope_at.x = slope_of(ybest.x); slope_at.y = slope_of(ybest.y); slope_at.z = slope_of(ybest.z); slope_at.w = slope_of(ybest.w);
-}
-
-// component `comp` (a literal at every call site) of v[k], k = the run-time arg-max position: a select chain -- indexing
-// the register array with k would move it to local memory (STL / LDL in the middle of latency-bound kernels)
-__device__ __forceinline__ float pick(const float4 (&v)[4], int k, int comp) {
-  const float a0 = comp == 0 ? v[0].x : comp == 1 ? v[0].y : comp == 2 ? v[0].z : v[0].w;
-  const float a1 = comp == 0 ? v[1].x : comp == 1 ? v[1].y : comp == 2 ? v[1].z : v[1].w;
-  const float a2 = comp == 0 ? v[2].x : comp == 1 ? v[2].y : comp == 2 ? v[2].z : v[2].w;
-  const float a3 = comp == 0 ? v[3].x : comp == 1 ? v[3].y : comp == 2 ? v[3].z : v[3].w;
-  return k == 0 ? a0 : k == 1 ? a1 : k == 2 ? a2 : a3;
-}
-
-// block-level reduction of per-thread (4 channels x 2 sums) fp64 partials, then one atomic per channel
-__device__ __forceinline__ void block_reduce_stats(double (&s1)[4], double (&s2)[4], const WinIter& it, double* stats, int F) {
-  __shared__ double red[256 * 8];
-  const int tid = threadIdx.x;
-#pragma unroll
-  for (int c = 0; c < 4; ++c) { red[tid * 8 + c * 2] = s1[c]; red[tid * 8 + c * 2 + 1] = s2[c]; }
-  __syncthreads();
-  for (int o = tid; o < F * 2; o += blockDim.x) {
-    const int ch = o >> 1, which = o & 1;
-    const int q = ch >> 2, comp = ch & 3;
-    double t = 0.0;
-    for (int l = 0; l < it.WPB; ++l) t += red[(l * it.F4 + q) * 8 + comp * 2 + which];
-    atomicAdd(&stats[ch * 2 + which], t);
-  }
+  arg = w.arg;
+  slope_at = slope_of(w.y);
 }
 
 // ---- thread-block-cluster helpers for the fused (reduce -> cluster all-reduce -> apply) backward kernels
@@ -216,18 +286,32 @@ __device__ __forceinline__ void bn_dsmem_st_f64(double* local, uint32_t rank, do
 // CTA totals of the per-thread partials (fixed summation order): thread o < 2F returns the total of (channel o/2,
 // sum o%2); other threads return 0
 __device__ __forceinline__ double block_reduce_totals(double (&s1)[4], double (&s2)[4], const WinIter& it, int F) {
-  __shared__ double red2[256 * 8];
+  __shared__ double red[256 * 8];
   const int tid = threadIdx.x;
 #pragma unroll
-  for (int c = 0; c < 4; ++c) { red2[tid * 8 + c * 2] = s1[c]; red2[tid * 8 + c * 2 + 1] = s2[c]; }
+  for (int c = 0; c < 4; ++c) { red[tid * 8 + c * 2] = s1[c]; red[tid * 8 + c * 2 + 1] = s2[c]; }
   __syncthreads();
   double t = 0.0;
   if (tid < F * 2) {
     const int ch = tid >> 1, which = tid & 1;
     const int q = ch >> 2, comp = ch & 3;
-    for (int l = 0; l < it.WPB; ++l) t += red2[(l * it.F4 + q) * 8 + comp * 2 + which];
+    for (int l = 0; l < it.WPB; ++l) t += red[(l * it.F4 + q) * 8 + comp * 2 + which];
   }
   return t;
+}
+// CTA totals added to the statistics arena: one atomic per (channel, sum)
+__device__ __forceinline__ void block_reduce_stats(double (&s1)[4], double (&s2)[4], const WinIter& it, double* stats, int F) {
+  const double t = block_reduce_totals(s1, s2, it, F);
+  if (threadIdx.x < F * 2) atomicAdd(&stats[threadIdx.x], t);
+}
+// CTA totals of a kernel that needs no cluster: publishes sums / m in shared memory and the raw sums in the statistics row
+__device__ __forceinline__ void publish_totals(double t, int F, double m, float* s_a, float* s_b2, double* row) {
+  const int tid = threadIdx.x;
+  if (tid < F * 2) {
+    ((tid & 1) ? s_b2 : s_a)[tid >> 1] = (float)(t / m);
+    row[tid] = t;
+  }
+  __syncthreads();
 }
 // All-reduce of the CTA totals over the cluster with ONE barrier: every CTA pushes its totals into slot [own rank] of
 // every CTA's `gather` array (remote shared-memory stores), barrier.cluster (release / acquire), then each CTA sums its
@@ -265,12 +349,7 @@ __device__ __forceinline__ void bnbwd_reduce_phase(const BnBwdArgs& a, const BnG
     if (wy >= g.ph || wx >= g.pw) continue;
     float4 zh[4]; long long idx[4]; int4 arg; float4 sl;
     argmax_window(zhp, g, img, wy, wx, it, ga, be, zh, idx, arg, sl);
-    const float4 d = ld4(dp + it.pooled(g, img, wy, wx));
-    const float dy0 = d.x * sl.x, dy1 = d.y * sl.y, dy2 = d.z * sl.z, dy3 = d.w * sl.w;
-    s1[0] += dy0; s2[0] += (double)dy0 * (double)pick(zh, arg.x, 0);
-    s1[1] += dy1; s2[1] += (double)dy1 * (double)pick(zh, arg.y, 1);
-    s1[2] += dy2; s2[2] += (double)dy2 * (double)pick(zh, arg.z, 2);
-    s1[3] += dy3; s2[3] += (double)dy3 * (double)pick(zh, arg.w, 3);
+    bn_bwd_sums(ld4(dp + it.pooled(g, img, wy, wx)), sl, zh, arg, s1, s2);
   }
 }
 
@@ -302,7 +381,7 @@ __device__ __forceinline__ void bnbwd_apply_phase(const BnBwdArgs& a, const BnGe
                                                   const float* s_c2) {
   if (it.lane >= it.WPB) return;
   const float4 r = ld4s(s_r, it.q), ga = ld4s(s_g, it.q), be = ld4s(s_b, it.q), c1 = ld4s(s_c1, it.q), c2 = ld4s(s_c2, it.q);
-  const float4 rg = make_float4(r.x * ga.x, r.y * ga.y, r.z * ga.z, r.w * ga.w);
+  const float4 rg = mul4(r, ga);
   const float* zhp = a.zh + (long long)task * a.zh_stride;
   const float* dp = a.dp + (long long)task * a.dp_stride;
   float* dz = a.dz + (long long)task * a.dz_stride;
@@ -312,15 +391,10 @@ __device__ __forceinline__ void bnbwd_apply_phase(const BnBwdArgs& a, const BnGe
     if (full) {
       float4 zh[4]; long long idx[4]; int4 arg; float4 sl;
       argmax_window(zhp, g, img, wy, wx, it, ga, be, zh, idx, arg, sl);
-      const float4 d = ld4(dp + it.pooled(g, img, wy, wx));
-      const float4 dyv = make_float4(d.x * sl.x, d.y * sl.y, d.z * sl.z, d.w * sl.w);
+      const float4 dyv = mul4(ld4(dp + it.pooled(g, img, wy, wx)), sl);
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        float4 o;
-        o.x = rg.x * ((arg.x == k ? dyv.x : 0.f) - c1.x - zh[k].x * c2.x);
-        o.y = rg.y * ((arg.y == k ? dyv.y : 0.f) - c1.y - zh[k].y * c2.y);
-        o.z = rg.z * ((arg.z == k ? dyv.z : 0.f) - c1.z - zh[k].z * c2.z);
-        o.w = rg.w * ((arg.w == k ? dyv.w : 0.f) - c1.w - zh[k].w * c2.w);
+        const float4 o = bn_bwd_dz(rg, c1, zh[k], c2, k, arg, dyv);
         st4(dz + idx[k], o);
         if (a.dz_hi) st4_split(a.dz_hi + (long long)task * a.dz_stride, a.dz_lo + (long long)task * a.dz_stride, idx[k], o);
       }
@@ -330,10 +404,7 @@ __device__ __forceinline__ void bnbwd_apply_phase(const BnBwdArgs& a, const BnGe
         const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
         if (yy < g.h && xx < g.w) {
           const long long idx = it.grid(g, img, yy, xx);
-          const float4 zh = ld4(zhp + idx);
-          float4 o;
-          o.x = rg.x * (-c1.x - zh.x * c2.x); o.y = rg.y * (-c1.y - zh.y * c2.y);
-          o.z = rg.z * (-c1.z - zh.z * c2.z); o.w = rg.w * (-c1.w - zh.w * c2.w);
+          const float4 o = bn_bwd_dz<true>(rg, c1, ld4(zhp + idx), c2);
           st4(dz + idx, o);
           if (a.dz_hi) st4_split(a.dz_hi + (long long)task * a.dz_stride, a.dz_lo + (long long)task * a.dz_stride, idx, o);
         }
@@ -444,42 +515,23 @@ __device__ __forceinline__ void bnact_tan_phase(const BnActTanArgs& a, const BnG
   float* pd = a.pdot + (long long)task * a.pdot_stride;
   for (int wi = cta * it.WPB + it.lane; wi < it.NW; wi += ncta * it.WPB) {
     int img, wy, wx; it.window(wi, img, wy, wx);
-    float4 best = make_float4(0.f, 0.f, 0.f, 0.f), pbest = best;
+    WinMax w{};
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
       if (yy < g.h && xx < g.w) {
         const long long idx = it.grid(g, img, yy, xx);
         const float4 zh = ld4(zhp + idx);
-        float4 zv = ld4(zd + idx);
-        if (zd2) { const float4 z2 = ld4(zd2 + idx); zv.x += z2.x; zv.y += z2.y; zv.z += z2.z; zv.w += z2.w; }
-        float4 zhd;
-        zhd.x = r.x * (zv.x - md.x - zh.x * qq.x); zhd.y = r.y * (zv.y - md.y - zh.y * qq.y);
-        zhd.z = r.z * (zv.z - md.z - zh.z * qq.z); zhd.w = r.w * (zv.w - md.w - zh.w * qq.w);
+        const float4 zhd = bn_tan_normalize(ld4_sum(zd, zd2, idx), zh, r, md, qq);
         st4(zd + idx, zhd);
-        float4 y, act, pdv;
-        y.x = fmaf(ga.x, zh.x, be.x); y.y = fmaf(ga.y, zh.y, be.y); y.z = fmaf(ga.z, zh.z, be.z); y.w = fmaf(ga.w, zh.w, be.w);
-        act.x = leaky(y.x); act.y = leaky(y.y); act.z = leaky(y.z); act.w = leaky(y.w);
-        if constexpr (GB) {
-          pdv.x = slope_of(y.x) * (ga.x * zhd.x + fmaf(gd.x, zh.x, bd.x)); pdv.y = slope_of(y.y) * (ga.y * zhd.y + fmaf(gd.y, zh.y, bd.y));
-          pdv.z = slope_of(y.z) * (ga.z * zhd.z + fmaf(gd.z, zh.z, bd.z)); pdv.w = slope_of(y.w) * (ga.w * zhd.w + fmaf(gd.w, zh.w, bd.w));
-        } else {
-          pdv.x = slope_of(y.x) * ga.x * zhd.x; pdv.y = slope_of(y.y) * ga.y * zhd.y;
-          pdv.z = slope_of(y.z) * ga.z * zhd.z; pdv.w = slope_of(y.w) * ga.w * zhd.w;
-        }
-        if (k == 0) { best = act; pbest = pdv; }
-        else {
-          if (act.x > best.x) { best.x = act.x; pbest.x = pdv.x; }
-          if (act.y > best.y) { best.y = act.y; pbest.y = pdv.y; }
-          if (act.z > best.z) { best.z = act.z; pbest.z = pdv.z; }
-          if (act.w > best.w) { best.w = act.w; pbest.w = pdv.w; }
-        }
+        const BnAct v = bn_act(ga, zh, be);
+        keep_first_max(k, v, w, act_tangent<GB>(v, ga, zhd, zh, gd, bd));
       }
     }
     if (wy < g.ph && wx < g.pw) {
       const long long pidx = it.pooled(g, img, wy, wx);
-      st4(pd + pidx, pbest);
-      if (a.pdot_hi) st4_split(a.pdot_hi + (long long)task * a.pdot_stride, a.pdot_lo + (long long)task * a.pdot_stride, pidx, pbest);
+      st4(pd + pidx, w.p);
+      if (a.pdot_hi) st4_split(a.pdot_hi + (long long)task * a.pdot_stride, a.pdot_lo + (long long)task * a.pdot_stride, pidx, w.p);
     }
   }
 }
@@ -528,6 +580,7 @@ __device__ __forceinline__ void bnbwd_tan_reduce_phase(const BnBwdTanArgs& a, co
   const float* zhd = a.zhdot + (long long)task * a.zhdot_stride;
   const float* dp = a.dp + (long long)task * a.dp_stride;
   const float* dpd = a.dpdot + (long long)task * a.dpdot_stride;
+  const float* dpd2 = a.dpdot2 ? a.dpdot2 + (long long)task * a.dpdot_stride : nullptr;
   for (int wi = cta * it.WPB + it.lane; wi < it.NW; wi += ncta * it.WPB) {
     int img, wy, wx; it.window(wi, img, wy, wx);
     if (wy >= g.ph || wx >= g.pw) continue;
@@ -535,23 +588,8 @@ __device__ __forceinline__ void bnbwd_tan_reduce_phase(const BnBwdTanArgs& a, co
     argmax_window(zhp, g, img, wy, wx, it, ga, be, zh, idx, arg, sl);
     const long long pidx = it.pooled(g, img, wy, wx);
     const float4 d = ld4(dp + pidx);
-    float4 dd = ld4(dpd + pidx);
-    if (a.dpdot2) {
-      const float4 d2 = ld4(a.dpdot2 + (long long)task * a.dpdot_stride + pidx);
-      dd.x += d2.x; dd.y += d2.y; dd.z += d2.z; dd.w += d2.w;
-    }
-    const int ar[4] = {arg.x, arg.y, arg.z, arg.w};
-    const float slv[4] = {sl.x, sl.y, sl.z, sl.w};
-    const float dv[4] = {d.x, d.y, d.z, d.w};
-    const float ddv[4] = {dd.x, dd.y, dd.z, dd.w};
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      const float zhk = pick(zh, ar[c], c);
-      const float zhdk = zhd[idx[ar[c]] + c];
-      const float dy = dv[c] * slv[c], dyd = ddv[c] * slv[c];
-      s1[c] += dyd;
-      s2[c] += (double)dyd * (double)zhk + (double)dy * (double)zhdk;
-    }
+    const float4 dd = ld4_sum(dpd, dpd2, pidx);
+    bn_tan_bwd_sums(d, dd, sl, zh, arg, [&](int k, int c) { return zhd[pick(idx, k) + c]; }, s1, s2);
   }
 }
 
@@ -584,12 +622,13 @@ __device__ __forceinline__ void bnbwd_tan_apply_phase(const BnBwdTanArgs& a, con
   if (it.lane >= it.WPB) return;
   const float4 r = ld4s(s_r, it.q), ga = ld4s(s_g, it.q), be = ld4s(s_b, it.q);
   const float4 qq = ld4s(s_q, it.q), c2 = ld4s(s_c2, it.q), t1 = ld4s(s_t1, it.q), t2 = ld4s(s_t2, it.q);
-  const float4 rg = make_float4(r.x * ga.x, r.y * ga.y, r.z * ga.z, r.w * ga.w);
+  const float4 rg = mul4(r, ga);
   const float4 rq = make_float4(-r.x * qq.x, -r.y * qq.y, -r.z * qq.z, -r.w * qq.w);
   const float* zhp = a.zh + (long long)task * a.zh_stride;
   const float* zhd = a.zhdot + (long long)task * a.zhdot_stride;
   const float* dzp = a.dz + (long long)task * a.dz_stride;
   const float* dpd = a.dpdot + (long long)task * a.dpdot_stride;
+  const float* dpd2 = a.dpdot2 ? a.dpdot2 + (long long)task * a.dpdot_stride : nullptr;
   float* dzd = a.dzdot + (long long)task * a.dzdot_stride;
   for (int wi = cta * it.WPB + it.lane; wi < it.NW; wi += ncta * it.WPB) {
     int img, wy, wx; it.window(wi, img, wy, wx);
@@ -599,13 +638,7 @@ __device__ __forceinline__ void bnbwd_tan_apply_phase(const BnBwdTanArgs& a, con
     if (full) {
       float4 zh[4]; long long idx[4]; float4 sl;
       argmax_window(zhp, g, img, wy, wx, it, ga, be, zh, idx, arg, sl);
-      const long long pidx = it.pooled(g, img, wy, wx);
-      float4 dd = ld4(dpd + pidx);
-      if (a.dpdot2) {
-        const float4 d2 = ld4(a.dpdot2 + (long long)task * a.dpdot_stride + pidx);
-        dd.x += d2.x; dd.y += d2.y; dd.z += d2.z; dd.w += d2.w;
-      }
-      dyd = make_float4(dd.x * sl.x, dd.y * sl.y, dd.z * sl.z, dd.w * sl.w);
+      dyd = mul4(ld4_sum(dpd, dpd2, it.pooled(g, img, wy, wx)), sl);
     }
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
@@ -613,11 +646,7 @@ __device__ __forceinline__ void bnbwd_tan_apply_phase(const BnBwdTanArgs& a, con
       if (yy < g.h && xx < g.w) {
         const long long idx = it.grid(g, img, yy, xx);
         const float4 zh = ld4(zhp + idx), zd = ld4(zhd + idx), dzv = ld4(dzp + idx);
-        float4 o;
-        o.x = rq.x * dzv.x + rg.x * ((arg.x == k ? dyd.x : 0.f) - t1.x - zd.x * c2.x - zh.x * t2.x);
-        o.y = rq.y * dzv.y + rg.y * ((arg.y == k ? dyd.y : 0.f) - t1.y - zd.y * c2.y - zh.y * t2.y);
-        o.z = rq.z * dzv.z + rg.z * ((arg.z == k ? dyd.z : 0.f) - t1.z - zd.z * c2.z - zh.z * t2.z);
-        o.w = rq.w * dzv.w + rg.w * ((arg.w == k ? dyd.w : 0.f) - t1.w - zd.w * c2.w - zh.w * t2.w);
+        const float4 o = bn_tan_bwd_dz(rq, dzv, rg, t1, zd, c2, zh, t2, k, arg, dyd);
         st4(dzd + idx, o);
         if (a.dzdot_hi) st4_split(a.dzdot_hi + (long long)task * a.dzdot_stride, a.dzdot_lo + (long long)task * a.dzdot_stride, idx, o);
       }
@@ -711,12 +740,7 @@ __global__ void __launch_bounds__(256) tail_fused_kernel(BnActArgs fa, HeadArgs 
   __syncthreads();
   double s1[4] = {0, 0, 0, 0}, s2[4] = {0, 0, 0, 0};
   bnbwd_reduce_phase(ba, g, task, 0, 1, it, s_g, s_b, s1, s2);
-  const double t = block_reduce_totals(s1, s2, it, g.F);
-  if (threadIdx.x < g.F * 2) {
-    ((threadIdx.x & 1) ? s_c2 : s_c1)[threadIdx.x >> 1] = (float)(t / m);
-    (ba.stats_bwd + (long long)task * ba.stats_bwd_stride)[threadIdx.x] = t;
-  }
-  __syncthreads();
+  publish_totals(block_reduce_totals(s1, s2, it, g.F), g.F, m, s_c1, s_c2, ba.stats_bwd + (long long)task * ba.stats_bwd_stride);
   bnbwd_apply_phase(ba, g, task, 0, 1, it, s_r, s_g, s_b, s_c1, s_c2);
 }
 
@@ -738,12 +762,7 @@ __global__ void __launch_bounds__(256) tail_tan_fused_kernel(BnActTanArgs fa, He
   __syncthreads();
   double s1[4] = {0, 0, 0, 0}, s2[4] = {0, 0, 0, 0};
   bnbwd_tan_reduce_phase(ba, g, task, 0, 1, it, s_g, s_b, s1, s2);
-  const double t = block_reduce_totals(s1, s2, it, g.F);
-  if (threadIdx.x < g.F * 2) {
-    ((threadIdx.x & 1) ? s_t2 : s_t1)[threadIdx.x >> 1] = (float)(t / m);
-    (ba.stats_tbwd + (long long)task * ba.stats_tbwd_stride)[threadIdx.x] = t;
-  }
-  __syncthreads();
+  publish_totals(block_reduce_totals(s1, s2, it, g.F), g.F, m, s_t1, s_t2, ba.stats_tbwd + (long long)task * ba.stats_tbwd_stride);
   bnbwd_tan_apply_phase(ba, g, task, 0, 1, it, s_r, s_g, s_b, s_q, s_c2, s_t1, s_t2);
 }
 
@@ -792,37 +811,26 @@ __global__ void __launch_bounds__(256) tail_onchip_kernel(BnActArgs fa, HeadArgs
     if (!have[i]) continue;
     int img, wy, wx; it.window(wi, img, wy, wx);
     img_[i] = img; wy_[i] = wy; wx_[i] = wx;
-    float4 best = make_float4(0.f, 0.f, 0.f, 0.f), ybest = best;
-    int4 am = make_int4(0, 0, 0, 0);
+    WinMax w{};
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
       zh[i][k] = make_float4(0.f, 0.f, 0.f, 0.f);
       if (yy < g.h && xx < g.w) {
         const long long idx = it.grid(g, img, yy, xx);
-        const float4 zv = ld4(z + idx);
-        float4 zz, y, act;
-        zz.x = (zv.x - mu.x) * r.x; zz.y = (zv.y - mu.y) * r.y; zz.z = (zv.z - mu.z) * r.z; zz.w = (zv.w - mu.w) * r.w;
+        const float4 zz = bn_normalize(ld4(z + idx), mu, r);
         st4(z + idx, zz);
         zh[i][k] = zz;
-        y.x = fmaf(ga.x, zz.x, be.x); y.y = fmaf(ga.y, zz.y, be.y); y.z = fmaf(ga.z, zz.z, be.z); y.w = fmaf(ga.w, zz.w, be.w);
-        act.x = leaky(y.x); act.y = leaky(y.y); act.z = leaky(y.z); act.w = leaky(y.w);
-        if (k == 0) { best = act; ybest = y; }
-        else {
-          if (act.x > best.x) { best.x = act.x; ybest.x = y.x; am.x = k; }
-          if (act.y > best.y) { best.y = act.y; ybest.y = y.y; am.y = k; }
-          if (act.z > best.z) { best.z = act.z; ybest.z = y.z; am.z = k; }
-          if (act.w > best.w) { best.w = act.w; ybest.w = y.w; am.w = k; }
-        }
+        keep_first_max(k, bn_act(ga, zz, be), w);
       }
     }
-    arg[i] = am;
-    sl[i] = make_float4(slope_of(ybest.x), slope_of(ybest.y), slope_of(ybest.z), slope_of(ybest.w));
+    arg[i] = w.arg;
+    sl[i] = slope_of(w.y);
     full[i] = (wy < g.ph && wx < g.pw);
     if (full[i]) {
       const long long pidx = it.pooled(g, img, wy, wx);
-      st4(pg + pidx, best);
-      st4(s_f + pidx, best);                       // pb = 0 on the last block: pidx is the feature index img * D + ...
+      st4(pg + pidx, w.act);
+      st4(s_f + pidx, w.act);                      // pb = 0 on the last block: pidx is the feature index img * D + ...
     }
   }
   __syncthreads();
@@ -847,22 +855,12 @@ __global__ void __launch_bounds__(256) tail_onchip_kernel(BnActArgs fa, HeadArgs
     dyv[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     if (!have[i] || !full[i]) continue;
     const long long pidx = it.pooled(g, img_[i], wy_[i], wx_[i]);
-    const float4 d = ld4(s_df + pidx);
-    dyv[i] = make_float4(d.x * sl[i].x, d.y * sl[i].y, d.z * sl[i].z, d.w * sl[i].w);
-    s1[0] += dyv[i].x; s2[0] += (double)dyv[i].x * (double)pick(zh[i], arg[i].x, 0);
-    s1[1] += dyv[i].y; s2[1] += (double)dyv[i].y * (double)pick(zh[i], arg[i].y, 1);
-    s1[2] += dyv[i].z; s2[2] += (double)dyv[i].z * (double)pick(zh[i], arg[i].z, 2);
-    s1[3] += dyv[i].w; s2[3] += (double)dyv[i].w * (double)pick(zh[i], arg[i].w, 3);
+    dyv[i] = bn_bwd_sums(ld4(s_df + pidx), sl[i], zh[i], arg[i], s1, s2);
   }
-  const double t = block_reduce_totals(s1, s2, it, g.F);
-  if (tid < g.F * 2) {
-    ((tid & 1) ? s_c2 : s_c1)[tid >> 1] = (float)(t / m);
-    (ba.stats_bwd + (long long)task * ba.stats_bwd_stride)[tid] = t;
-  }
-  __syncthreads();
+  publish_totals(block_reduce_totals(s1, s2, it, g.F), g.F, m, s_c1, s_c2, ba.stats_bwd + (long long)task * ba.stats_bwd_stride);
   if (!worker) return;
   const float4 c1 = ld4s(s_c1, it.q), c2 = ld4s(s_c2, it.q);
-  const float4 rg = make_float4(r.x * ga.x, r.y * ga.y, r.z * ga.z, r.w * ga.w);
+  const float4 rg = mul4(r, ga);
   float* dz = ba.dz + (long long)task * ba.dz_stride;
 #pragma unroll
   for (int i = 0; i < MAXI; ++i) {
@@ -872,11 +870,7 @@ __global__ void __launch_bounds__(256) tail_onchip_kernel(BnActArgs fa, HeadArgs
       const int yy = 2 * wy_[i] + (k >> 1), xx = 2 * wx_[i] + (k & 1);
       if (yy < g.h && xx < g.w) {
         const long long idx = it.grid(g, img_[i], yy, xx);
-        float4 o;
-        o.x = rg.x * ((full[i] && arg[i].x == k ? dyv[i].x : 0.f) - c1.x - zh[i][k].x * c2.x);
-        o.y = rg.y * ((full[i] && arg[i].y == k ? dyv[i].y : 0.f) - c1.y - zh[i][k].y * c2.y);
-        o.z = rg.z * ((full[i] && arg[i].z == k ? dyv[i].z : 0.f) - c1.z - zh[i][k].z * c2.z);
-        o.w = rg.w * ((full[i] && arg[i].w == k ? dyv[i].w : 0.f) - c1.w - zh[i][k].w * c2.w);
+        const float4 o = bn_bwd_dz(rg, c1, zh[i][k], c2, k, arg[i], dyv[i], full[i]);
         st4(dz + idx, o);
         if (ba.dz_hi) st4_split(ba.dz_hi + (long long)task * ba.dz_stride, ba.dz_lo + (long long)task * ba.dz_stride, idx, o);
       }
@@ -946,8 +940,7 @@ __global__ void __launch_bounds__(256) tail_tan_onchip_kernel(BnActTanArgs fa, H
     full[i] = (wy < g.ph && wx < g.pw);
     const long long pidx = it.pooled(g, img, wy, wx);
     if (full[i]) dprim[i] = ld4(dpp + pidx);                 // primal d(loss)/d(pooled), written in phase A
-    float4 best = make_float4(0.f, 0.f, 0.f, 0.f), ybest = best, pbest = best;
-    int4 am = make_int4(0, 0, 0, 0);
+    WinMax w{};
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
@@ -956,32 +949,18 @@ __global__ void __launch_bounds__(256) tail_tan_onchip_kernel(BnActTanArgs fa, H
       if (yy < g.h && xx < g.w) {
         const long long idx = it.grid(g, img, yy, xx);
         const float4 z = ld4(zhp + idx);
-        float4 zv = ld4(zd + idx);
-        if (zd2) { const float4 z2 = ld4(zd2 + idx); zv.x += z2.x; zv.y += z2.y; zv.z += z2.z; zv.w += z2.w; }
-        float4 d;
-        d.x = r.x * (zv.x - md.x - z.x * qq.x); d.y = r.y * (zv.y - md.y - z.y * qq.y);
-        d.z = r.z * (zv.z - md.z - z.z * qq.z); d.w = r.w * (zv.w - md.w - z.w * qq.w);
+        const float4 d = bn_tan_normalize(ld4_sum(zd, zd2, idx), z, r, md, qq);
         st4(zd + idx, d);
         zh[i][k] = z; zhd[i][k] = d;
-        float4 y, act, pdv;
-        y.x = fmaf(ga.x, z.x, be.x); y.y = fmaf(ga.y, z.y, be.y); y.z = fmaf(ga.z, z.z, be.z); y.w = fmaf(ga.w, z.w, be.w);
-        act.x = leaky(y.x); act.y = leaky(y.y); act.z = leaky(y.z); act.w = leaky(y.w);
-        pdv.x = slope_of(y.x) * ga.x * d.x; pdv.y = slope_of(y.y) * ga.y * d.y;
-        pdv.z = slope_of(y.z) * ga.z * d.z; pdv.w = slope_of(y.w) * ga.w * d.w;
-        if (k == 0) { best = act; ybest = y; pbest = pdv; }
-        else {
-          if (act.x > best.x) { best.x = act.x; ybest.x = y.x; pbest.x = pdv.x; am.x = k; }
-          if (act.y > best.y) { best.y = act.y; ybest.y = y.y; pbest.y = pdv.y; am.y = k; }
-          if (act.z > best.z) { best.z = act.z; ybest.z = y.z; pbest.z = pdv.z; am.z = k; }
-          if (act.w > best.w) { best.w = act.w; ybest.w = y.w; pbest.w = pdv.w; am.w = k; }
-        }
+        const BnAct v = bn_act(ga, z, be);
+        keep_first_max(k, v, w, act_tangent<false>(v, ga, d, z));
       }
     }
-    arg[i] = am;
-    sl[i] = make_float4(slope_of(ybest.x), slope_of(ybest.y), slope_of(ybest.z), slope_of(ybest.w));
+    arg[i] = w.arg;
+    sl[i] = slope_of(w.y);
     if (full[i]) {
-      st4(pdg + pidx, pbest);
-      st4(s_fd + pidx, pbest);                     // pb = 0 on the last block: pidx is the feature index img * D + ...
+      st4(pdg + pidx, w.p);
+      st4(s_fd + pidx, w.p);                       // pb = 0 on the last block: pidx is the feature index img * D + ...
     }
   }
   __syncthreads();
@@ -1010,32 +989,13 @@ __global__ void __launch_bounds__(256) tail_tan_onchip_kernel(BnActTanArgs fa, H
     dydv[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     if (!have[i] || !full[i]) continue;
     const long long pidx = it.pooled(g, img_[i], wy_[i], wx_[i]);
-    const float4 dd = ld4(s_dfd + pidx);
-    const int ar[4] = {arg[i].x, arg[i].y, arg[i].z, arg[i].w};
-    const float slv[4] = {sl[i].x, sl[i].y, sl[i].z, sl[i].w};
-    const float dv[4] = {dprim[i].x, dprim[i].y, dprim[i].z, dprim[i].w};
-    const float ddv[4] = {dd.x, dd.y, dd.z, dd.w};
-    float dydc[4];
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      const float zhk = pick(zh[i], ar[c], c);
-      const float zhdk = pick(zhd[i], ar[c], c);
-      const float dy = dv[c] * slv[c], dyd = ddv[c] * slv[c];
-      dydc[c] = dyd;
-      s1[c] += dyd;
-      s2[c] += (double)dyd * (double)zhk + (double)dy * (double)zhdk;
-    }
-    dydv[i] = make_float4(dydc[0], dydc[1], dydc[2], dydc[3]);
+    dydv[i] = bn_tan_bwd_sums(dprim[i], ld4(s_dfd + pidx), sl[i], zh[i], arg[i], [&](int k, int c) { return pick(zhd[i], k, c); },
+                              s1, s2);
   }
-  const double t = block_reduce_totals(s1, s2, it, g.F);
-  if (tid < g.F * 2) {
-    ((tid & 1) ? s_t2 : s_t1)[tid >> 1] = (float)(t / m);
-    (ba.stats_tbwd + (long long)task * ba.stats_tbwd_stride)[tid] = t;
-  }
-  __syncthreads();
+  publish_totals(block_reduce_totals(s1, s2, it, g.F), g.F, m, s_t1, s_t2, ba.stats_tbwd + (long long)task * ba.stats_tbwd_stride);
   if (!worker) return;
   const float4 c2 = ld4s(s_c2, it.q), t1 = ld4s(s_t1, it.q), t2 = ld4s(s_t2, it.q);
-  const float4 rg = make_float4(r.x * ga.x, r.y * ga.y, r.z * ga.z, r.w * ga.w);
+  const float4 rg = mul4(r, ga);
   const float4 rq = make_float4(-r.x * qq.x, -r.y * qq.y, -r.z * qq.z, -r.w * qq.w);
   float* dzd = ba.dzdot + (long long)task * ba.dzdot_stride;
 #pragma unroll
@@ -1047,12 +1007,7 @@ __global__ void __launch_bounds__(256) tail_tan_onchip_kernel(BnActTanArgs fa, H
       if (yy < g.h && xx < g.w) {
         const long long idx = it.grid(g, img_[i], yy, xx);
         const float4 dzv = ld4(dzp + idx);
-        const float4 z = zh[i][k], zdk = zhd[i][k];
-        float4 o;
-        o.x = rq.x * dzv.x + rg.x * ((full[i] && arg[i].x == k ? dydv[i].x : 0.f) - t1.x - zdk.x * c2.x - z.x * t2.x);
-        o.y = rq.y * dzv.y + rg.y * ((full[i] && arg[i].y == k ? dydv[i].y : 0.f) - t1.y - zdk.y * c2.y - z.y * t2.y);
-        o.z = rq.z * dzv.z + rg.z * ((full[i] && arg[i].z == k ? dydv[i].z : 0.f) - t1.z - zdk.z * c2.z - z.z * t2.z);
-        o.w = rq.w * dzv.w + rg.w * ((full[i] && arg[i].w == k ? dydv[i].w : 0.f) - t1.w - zdk.w * c2.w - z.w * t2.w);
+        const float4 o = bn_tan_bwd_dz(rq, dzv, rg, t1, zhd[i][k], c2, zh[i][k], t2, k, arg[i], dydv[i], full[i]);
         st4(dzd + idx, o);
         if (ba.dzdot_hi) st4_split(ba.dzdot_hi + (long long)task * ba.dzdot_stride, ba.dzdot_lo + (long long)task * ba.dzdot_stride, idx, o);
       }
