@@ -148,6 +148,29 @@ struct BnBwdTanArgs {             // backward reduce / apply (tangent)
   int tag;          // launch sequence number inside the iteration (device trace)
 };
 
+// Layer norm (norm_layer "layer_norm"): statistics per IMAGE over its F*h*w conv outputs, y = zh + bias[c][y][x] (the
+// reference's frozen weight is all ones), then leaky-ReLU and max-pool as with BatchNorm.  One argument block for the LN
+// kernels; each reads the fields its comment names.  Per-image fp64 sums: [task][img][2] at `st_*` + task * st_stride.
+struct LnArgs {
+  float* z; long long z_stride;          // stats / act: z (act: -> zh in place); tangent: zdot (-> zhdot in place)
+  const float* z2;                       // tangent: optional second addend of zdot (same stride)
+  const float* zh; long long zh_stride;  // primal zh (tangent and backward kernels)
+  const float* zhd; long long zhd_stride;            // tangent backward: zhdot
+  const float* dp; long long dp_stride;              // pooled gradient (backward), primal dp (tangent backward)
+  const float* dpd; const float* dpd2; long long dpd_stride;   // tangent backward: dpdot (+ optional second addend)
+  const float* dz; long long dz_stride;              // tangent backward: primal dz
+  float* out; float* out_hi; float* out_lo; long long out_stride;   // act: p (+ TF32 planes); backward: dz (+ planes)
+  const double* st_fwd;                  // (sum z, sum z^2) of the primal forward
+  const double* st_tan;                  // (sum zdot, sum zh * zdot)
+  const double* st_bwd;                  // (sum dy, sum dy * zh)
+  double* st_out;                        // the sums a stats / reduce kernel accumulates
+  long long st_stride;
+  const float* bias;                     // [F][h][w] layer-norm bias (act kernels)
+  float* db; long long db_stride;        // bias gradient: [F][h][w] per task (stored, not accumulated)
+  BnGeom g; int tasks;
+  int tag;          // launch sequence number inside the iteration (device trace)
+};
+
 enum { HEAD_SUPPORT = 0, HEAD_TARGET_FWD = 1, HEAD_TARGET_BWD = 2, HEAD_TANGENT = 3,
        HEAD_EXTERNAL_BWD = 4,       // backward of the linear layer for an externally supplied d(loss)/d(logits) (functional operator)
        HEAD_EXTERNAL_TAN = 5 };     // tangent of HEAD_EXTERNAL_BWD with d(loss)/d(logits) held constant; the logits tangent
@@ -190,6 +213,10 @@ struct ParamLayout {
   // per inner segment: internal offset / size and number of gradient chunks in a partial buffer
   long long seg_off[2 * MAML_MAX_LAYERS + 2];
   long long seg_size[2 * MAML_MAX_LAYERS + 2];
+  // layer norm (ln = 1; then per_step_bn = 0 and m_beta / m_gamma are unused): block l's bias [F][h_l][w_l] sits at m_lnb[l]
+  // of the meta vector and at lnb_off[l] of a per-task bias-gradient row of lnb_off[L] floats
+  int ln;
+  long long m_lnb[MAML_MAX_LAYERS], lnb_off[MAML_MAX_LAYERS + 1];
 };
 
 enum { PR_UPDATE = 0, PR_STORE = 1, PR_SUB = 2 };
@@ -223,6 +250,11 @@ void launch_bnbwd_tan_reduce(const BnBwdTanArgs& a, cudaStream_t st);
 void launch_bnbwd_tan_apply(const BnBwdTanArgs& a, cudaStream_t st);
 void launch_bnbwd(const BnBwdArgs& a, cudaStream_t st);          // reduce + apply (one cluster kernel for small blocks)
 void launch_bnbwd_tan(const BnBwdTanArgs& a, cudaStream_t st);
+// layer norm (kernels_bn.cu).  tan = false: primal forward / backward; true: their forward-mode tangents
+void launch_ln_stats(const LnArgs& a, bool tan, cudaStream_t st);   // per-image sums of z (or of zdot and zh * zdot)
+void launch_ln_act(const LnArgs& a, bool tan, cudaStream_t st);     // normalise, + bias, leaky-ReLU, max-pool
+void launch_ln_bwd(const LnArgs& a, bool tan, cudaStream_t st);     // per-image backward sums, then dz (or dzdot)
+void launch_ln_bias_grad(const LnArgs& a, bool tan, cudaStream_t st);  // sum over the images of dy (or dydot)
 bool tail_fusable(const BnGeom& g, int n_rows, int rows_per_cta);
 void launch_tail_fused(const BnActArgs& fa, const HeadArgs& ha, const BnBwdArgs& ba, cudaStream_t st);
 void launch_tail_tan_fused(const BnActTanArgs& fa, const HeadArgs& ha, const BnBwdTanArgs& ba, cudaStream_t st);
@@ -272,6 +304,9 @@ struct ExportArgs {
   // 0: one result vector, summed over the tasks; 1: task t's entries, not summed, at result + t * result_stride (grid.y =
   // tasks; functional calls only, never with a communicator)
   int per_task; long long result_stride;
+  // layer norm: bias-gradient rows [tasks][2][S][pl.lnb_off[L]]: [.][0][s] the target pass of step s (loss weight
+  // included), [.][1][s] H_b u of step s's tangent pass
+  const float* lnb;
   int tag;          // launch sequence number inside the iteration (device trace)
 };
 void launch_export(const ExportArgs& a, cudaStream_t st);

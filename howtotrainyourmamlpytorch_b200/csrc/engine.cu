@@ -109,6 +109,11 @@ struct maml_b200_handle {
   double* stats = nullptr; long long stats_task_stride = 0, st_pass_stride = 0, st_layer_stride = 0, stats_count = 0;
   float *losses = nullptr, *correct = nullptr, *decay_dev = nullptr;
   double* abar = nullptr;
+  // layer-norm handles (cfg.norm_layer = 1): per-image sums [task][pass kind][step][block][image][2] and the bias-gradient
+  // rows [task][2][S][pl.lnb_off[L]] (see ExportArgs::lnb)
+  bool ln = false;
+  double* ln_stats = nullptr; long long ln_task_stride = 0, ln_pass_stride = 0;
+  float* lnb = nullptr;
   long long* zero_labels = nullptr;   // [max(n_s, n_t)] zeros (label-free forward)
   float* pinned = nullptr;            // host staging ring for small per-call scalars (16 slots x 32 floats)
   int pin_slot = 0;
@@ -222,7 +227,9 @@ static void build_geometry(maml_b200_handle* h) {
 static void build_layout(maml_b200_handle* h) {
   ParamLayout& pl = h->pl;
   memset(&pl, 0, sizeof(pl));
-  pl.L = h->L; pl.F = h->F; pl.N = h->N; pl.S = h->S; pl.per_step_bn = h->cfg.per_step_bn; pl.pix = h->pix;
+  pl.L = h->L; pl.F = h->F; pl.N = h->N; pl.S = h->S; pl.pix = h->pix;
+  pl.ln = h->ln ? 1 : 0;
+  pl.per_step_bn = h->ln ? 0 : h->cfg.per_step_bn;       // layer norm: no per-step parameters, no running statistics
   long long o = 0, m = 0;
   const long long bnsz = (long long)(pl.per_step_bn ? h->S : 1) * h->F;
   for (int l = 0; l < h->L; ++l) {
@@ -232,8 +239,15 @@ static void build_layout(maml_b200_handle* h) {
     pl.b_off[l] = o; o += h->F;
     pl.m_w[l] = m; h->seg_off.push_back(m); h->seg_size.push_back(wsz); m += wsz;
     pl.m_b[l] = m; h->seg_off.push_back(m); h->seg_size.push_back(h->F); m += h->F;
-    pl.m_beta[l] = m; h->seg_off.push_back(m); h->seg_size.push_back(bnsz); m += bnsz;
-    pl.m_gamma[l] = m; h->seg_off.push_back(m); h->seg_size.push_back(bnsz); m += bnsz;
+    if (h->ln) {
+      // norm_layer.bias [F, h_l, w_l]; the frozen all-ones weight is not a meta-parameter (the reference's Adam skips it)
+      const long long lsz = (long long)h->F * h->geo[l].h * h->geo[l].w;
+      pl.m_lnb[l] = m; h->seg_off.push_back(m); h->seg_size.push_back(lsz); m += lsz;
+      pl.lnb_off[l + 1] = pl.lnb_off[l] + lsz;
+    } else {
+      pl.m_beta[l] = m; h->seg_off.push_back(m); h->seg_size.push_back(bnsz); m += bnsz;
+      pl.m_gamma[l] = m; h->seg_off.push_back(m); h->seg_size.push_back(bnsz); m += bnsz;
+    }
     pl.seg_off[2 * l] = pl.w_off[l]; pl.seg_size[2 * l] = wsz;
     pl.seg_off[2 * l + 1] = pl.b_off[l]; pl.seg_size[2 * l + 1] = h->F;
   }
@@ -412,6 +426,12 @@ static void carve(maml_b200_handle* h, Bump& b) {
   h->abar = b.d(T * h->pl.nseg_inner * MAML_MAX_STEPS);
   h->decay_dev = b.f(MAML_MAX_STEPS);
   h->zero_labels = (long long*)b.d(std::max(h->n_s, h->n_t));
+  if (h->ln) {
+    h->ln_pass_stride = (long long)MAML_MAX_STEPS * h->L * std::max(h->n_s, h->n_t) * 2;
+    h->ln_task_stride = PASS_KINDS * h->ln_pass_stride;
+    h->ln_stats = b.d(h->ln_task_stride * T);
+    h->lnb = b.f(T * 2 * h->S * h->pl.lnb_off[h->L]);
+  }
 }
 
 extern "C" int maml_b200_create(const maml_b200_config* cfg, maml_b200_handle** out) {
@@ -421,6 +441,7 @@ extern "C" int maml_b200_create(const maml_b200_config* cfg, maml_b200_handle** 
   if (cfg->inner_steps < 1 || cfg->inner_steps > MAML_MAX_STEPS) return fail("inner_steps must be in [1, 8]");
   if (cfg->channels < 1 || cfg->channels > 4) return fail("channels must be in [1, 4]");
   if (cfg->max_tasks < 1) return fail("max_tasks must be >= 1");
+  if (cfg->norm_layer != 0 && cfg->norm_layer != 1) return fail("norm_layer must be 0 (batch norm) or 1 (layer norm)");
   if (cfg->n_way < 2 || cfg->n_way > 32) return fail("n_way must be in [2, 32]");
   const int n_s = cfg->n_way * cfg->k_shot, n_t = cfg->n_way * cfg->t_target;
   if (n_s < 1 || n_t < 1 || n_s > 128 || n_t > 128) return fail("N*K and N*T must be in [1, 128]");
@@ -433,6 +454,7 @@ extern "C" int maml_b200_create(const maml_b200_config* cfg, maml_b200_handle** 
   h->opt = read_options();
   h->L = cfg->num_stages; h->F = cfg->filters; h->N = cfg->n_way; h->S = cfg->inner_steps;
   h->C = cfg->channels; h->H = cfg->height; h->W = cfg->width; h->n_s = n_s; h->n_t = n_t; h->maxT = cfg->max_tasks;
+  h->ln = cfg->norm_layer == 1;
   build_geometry(h);
   build_layout(h);
   // tensor-core (wgmma / TMA, 3xTF32) convolutions for blocks l >= 1; reserved bit 1 forces the fp32 FFMA kernels (tests)
@@ -529,7 +551,7 @@ extern "C" int maml_b200_segment(const maml_b200_handle* h, int32_t idx, int64_t
 extern "C" int64_t maml_b200_meta_size(const maml_b200_handle* h) { return h ? h->pl.meta_size : -1; }
 extern "C" int64_t maml_b200_result_size(const maml_b200_handle* h) {
   if (!h) return -1;
-  return h->pl.meta_size + 2 + (h->cfg.per_step_bn ? 2LL * h->L * h->S * h->F : 0);
+  return h->pl.meta_size + 2 + (h->pl.per_step_bn ? 2LL * h->L * h->S * h->F : 0);
 }
 extern "C" int64_t maml_b200_last_launch_count(const maml_b200_handle* h) { return h ? h->last_launches : -1; }
 
@@ -549,6 +571,23 @@ static double conv_flops(const maml_b200_handle* h, int l, int n, int T, int nsr
 static double* stat_at(const maml_b200_handle* h, int kind, int step, int layer) {
   return h->stats + ((long long)kind * MAML_MAX_STEPS + step) * h->st_pass_stride + (long long)layer * h->st_layer_stride;
 }
+// layer norm: the per-image sums of (pass kind, step, block), task 0; and the arguments every LN launch of block l over n
+// images per task shares
+static double* ln_stat_at(const maml_b200_handle* h, int kind, int step, int layer) {
+  return h->ln_stats + (long long)kind * h->ln_pass_stride + ((long long)step * h->L + layer) * std::max(h->n_s, h->n_t) * 2;
+}
+static LnArgs ln_args(const maml_b200_handle* h, int l, int n, const float* meta, int T) {
+  LnArgs a{};
+  a.st_stride = h->ln_task_stride;
+  a.bias = meta + h->pl.m_lnb[l];
+  a.g = bn_geom(h, l, n); a.tasks = T;
+  return a;
+}
+// bias-gradient row of (task 0, kind 0: target pass / 1: tangent pass, step)
+static float* lnb_at(const maml_b200_handle* h, int kind, int step) {
+  return h->lnb + ((long long)kind * h->S + step) * h->pl.lnb_off[h->L];
+}
+
 static const float* gamma_at(const maml_b200_handle* h, const float* meta, int l, int step) {
   return meta + h->pl.m_gamma[l] + (h->cfg.per_step_bn ? (long long)step * h->F : 0);
 }
@@ -739,13 +778,17 @@ static void head_grad(const maml_b200_handle* h, HeadArgs& a, float* partial, co
 
 // the last block of the support batch, the head and that block's BatchNorm backward run as one kernel
 static bool support_tail_fused(const maml_b200_handle* h) {
-  return h->opt.tail_fuse && tail_fusable(bn_geom(h, h->L - 1, h->n_s), h->n_s, head_rows(h->n_s));
+  return h->opt.tail_fuse && !h->ln && tail_fusable(bn_geom(h, h->L - 1, h->n_s), h->n_s, head_rows(h->n_s));
 }
 
 enum { CLR_STATS = 1, CLR_ABAR = 2, CLR_LOSSES = 4, CLR_CORRECT = 8 };
 // zeroes the accumulators in `what` (CLR_* bits) for all maxT tasks on `st`
 static int clear_accumulators(maml_b200_handle* h, unsigned what, cudaStream_t st) {
   if (what & CLR_STATS) CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
+  if ((what & CLR_STATS) && h->ln) {
+    CK(cudaMemsetAsync(h->ln_stats, 0, (size_t)h->ln_task_stride * h->maxT * sizeof(double), st));
+    CK(cudaMemsetAsync(h->lnb, 0, (size_t)h->maxT * 2 * h->S * h->pl.lnb_off[h->L] * sizeof(float), st));
+  }
   if (what & CLR_ABAR) CK(cudaMemsetAsync(h->abar, 0, (size_t)h->maxT * h->pl.nseg_inner * MAML_MAX_STEPS * sizeof(double), st));
   if (what & CLR_LOSSES) CK(cudaMemsetAsync(h->losses, 0, (size_t)h->maxT * MAML_MAX_STEPS * sizeof(float), st));
   if (what & CLR_CORRECT) CK(cudaMemsetAsync(h->correct, 0, (size_t)h->maxT * sizeof(float), st));
@@ -772,6 +815,16 @@ static void forward_pass(maml_b200_handle* h, const PassSet& ps, int slot, const
       a.stats = stat_at(h, stat_kind, bn_step, l);
       launch_conv_rows(a, st);
     }
+    if (h->ln) {                   // per-image sums of z, then normalise / bias / leaky-ReLU / pool
+      LnArgs a = ln_args(h, l, ps.n, meta, T);
+      a.z = ZH(ps, l, slot); a.z_stride = STRIDE(ps, zh, l);
+      a.st_fwd = a.st_out = ln_stat_at(h, stat_kind, bn_step, l);
+      launch_ln_stats(a, false, st);
+      a.out = AIN(ps, l + 1, slot); a.out_stride = STRIDE(ps, ain, l + 1);
+      if (h->use_tc && l + 1 < h->L) { a.out_hi = AIN_HI(ps, l + 1, slot); a.out_lo = AIN_LO(ps, l + 1, slot); }
+      launch_ln_act(a, false, st);
+      continue;
+    }
     BnActArgs b{};
     b.z = ZH(ps, l, slot); b.z_stride = STRIDE(ps, zh, l);
     b.stats = stat_at(h, stat_kind, bn_step, l); b.stats_stride = h->stats_task_stride;
@@ -795,6 +848,19 @@ static void backward_pass(maml_b200_handle* h, const PassSet& ps, int slot, cons
   cudaStream_t wst = fork_wgrad ? h->s_wg : st;
   const bool split = fork_wgrad && rs != nullptr;
   for (int l = h->L - 1; l >= 0; --l) {
+    if (h->ln) {
+      LnArgs a = ln_args(h, l, ps.n, meta, T);
+      a.dp = DP(ps, l, slot); a.dp_stride = STRIDE(ps, dp, l);
+      a.zh = ZH(ps, l, slot); a.zh_stride = STRIDE(ps, zh, l);
+      a.st_fwd = ln_stat_at(h, kind_fwd, bn_step, l); a.st_out = ln_stat_at(h, kind_bwd, bn_step, l);
+      a.out = DZ(ps, l, slot); a.out_stride = STRIDE(ps, dz, l);
+      if (h->use_tc && l >= 1) { a.out_hi = DZ_HI(ps, l, slot); a.out_lo = DZ_LO(ps, l, slot); }
+      launch_ln_bwd(a, false, st);
+      if (kind_bwd == PASS_TGT_BWD) {    // the bias is an outer parameter only: its gradient comes from the target loss
+        a.db = lnb_at(h, 0, bn_step) + h->pl.lnb_off[l]; a.db_stride = 2LL * h->S * h->pl.lnb_off[h->L];
+        launch_ln_bias_grad(a, false, st);
+      }
+    } else {
     BnBwdArgs b{};
     b.dp = DP(ps, l, slot); b.dp_stride = STRIDE(ps, dp, l);
     b.zh = ZH(ps, l, slot); b.zh_stride = STRIDE(ps, zh, l);
@@ -806,6 +872,7 @@ static void backward_pass(maml_b200_handle* h, const PassSet& ps, int slot, cons
     b.g = bn_geom(h, l, ps.n); b.tasks = T;
     if (fused_head && l == h->L - 1) launch_tail_fused(*fused_act, *fused_head, b, st);
     else launch_bnbwd(b, st);
+    }
     if (fork_wgrad) { cudaEventRecord(h->ev_fork, st); cudaStreamWaitEvent(h->s_wg, h->ev_fork, 0); }
 
     if (l == 0) {
@@ -914,6 +981,18 @@ static void tangent_forward(maml_b200_handle* h, int s, const float* theta, cons
       a.stats = stat_at(h, PASS_TAN_FWD, s, l);
       launch_conv_rows(a, st);
     }
+    if (h->ln) {                   // zdot (+ the side stream's addend) -> per-image sums -> zhdot, pdot
+      LnArgs a = ln_args(h, l, sp.n, meta, T);
+      a.z = ZH(tn, l, 0); a.z_stride = STRIDE(tn, zh, l);
+      if (h->use_tc && l >= 1) a.z2 = ZH(t2, l, 0);
+      a.zh = ZH(sp, l, s); a.zh_stride = STRIDE(sp, zh, l);
+      a.st_fwd = ln_stat_at(h, PASS_SUP_FWD, s, l); a.st_tan = a.st_out = ln_stat_at(h, PASS_TAN_FWD, s, l);
+      launch_ln_stats(a, true, st);
+      a.out = AIN(tn, l + 1, 0); a.out_stride = STRIDE(tn, ain, l + 1);
+      if (h->use_tc && l + 1 < h->L) { a.out_hi = AIN_HI(tn, l + 1, 0); a.out_lo = AIN_LO(tn, l + 1, 0); }
+      launch_ln_act(a, true, st);
+      continue;
+    }
     BnActTanArgs b{};
     b.zdot = ZH(tn, l, 0); b.zdot_stride = STRIDE(tn, zh, l);
     if (h->use_tc && l >= 1) b.zdot2 = ZH(t2, l, 0);
@@ -944,10 +1023,27 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
   const HeadArgs hd = tangent_head_args(h, s, theta, u, th, T);
   if (!fuse_tail) launch_head(hd, st);
   for (int l = h->L - 1; l >= 0; --l) {
+    if (h->use_tc && l + 1 < h->L) cudaStreamWaitEvent(st, h->ev_pre[MAML_MAX_LAYERS + l + 1], 0);
+    if (h->ln) {
+      LnArgs a = ln_args(h, l, sp.n, meta, T);
+      a.dp = DP(sp, l, s); a.dp_stride = STRIDE(sp, dp, l);
+      a.dpd = DP(tn, l, 0); a.dpd_stride = STRIDE(tn, dp, l);
+      if (h->use_tc && l + 1 < h->L) a.dpd2 = DP(t2, l, 0);
+      a.zh = ZH(sp, l, s); a.zh_stride = STRIDE(sp, zh, l);
+      a.zhd = ZH(tn, l, 0); a.zhd_stride = STRIDE(tn, zh, l);
+      a.dz = DZ(sp, l, s); a.dz_stride = STRIDE(sp, dz, l);
+      a.st_fwd = ln_stat_at(h, PASS_SUP_FWD, s, l); a.st_bwd = ln_stat_at(h, PASS_SUP_BWD, s, l);
+      a.st_tan = ln_stat_at(h, PASS_TAN_FWD, s, l); a.st_out = ln_stat_at(h, th.kind_tbwd, s, l);
+      a.out = DZ(tn, l, 0); a.out_stride = STRIDE(tn, dz, l);
+      if (h->use_tc && l >= 1) { a.out_hi = DZ_HI(tn, l, 0); a.out_lo = DZ_LO(tn, l, 0); }
+      launch_ln_bwd(a, true, st);
+      a.db = lnb_at(h, 1, s) + h->pl.lnb_off[l]; a.db_stride = 2LL * h->S * h->pl.lnb_off[h->L];
+      launch_ln_bias_grad(a, true, st);                  // H_b u: the tangent of the support loss's bias gradient
+    } else {
     BnBwdTanArgs b{};
     b.dp = DP(sp, l, s); b.dp_stride = STRIDE(sp, dp, l);
     b.dpdot = DP(tn, l, 0); b.dpdot_stride = STRIDE(tn, dp, l);
-    if (h->use_tc && l + 1 < h->L) { b.dpdot2 = DP(t2, l, 0); cudaStreamWaitEvent(st, h->ev_pre[MAML_MAX_LAYERS + l + 1], 0); }
+    if (h->use_tc && l + 1 < h->L) b.dpdot2 = DP(t2, l, 0);
     b.zh = ZH(sp, l, s); b.zh_stride = STRIDE(sp, zh, l);
     b.zhdot = ZH(tn, l, 0); b.zhdot_stride = STRIDE(tn, zh, l);
     b.dz = DZ(sp, l, s); b.dz_stride = STRIDE(sp, dz, l);
@@ -961,6 +1057,7 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
     b.g = bn_geom(h, l, sp.n); b.tasks = T;
     if (fuse_tail && l == h->L - 1) launch_tail_tan_fused(last_act, hd, b, st);
     else launch_bnbwd_tan(b, st);
+    }
     cudaEventRecord(h->ev_fork, st); cudaStreamWaitEvent(h->s_wg, h->ev_fork, 0);
 
     if (l == 0) {
@@ -1033,6 +1130,7 @@ static ExportArgs export_args(const maml_b200_handle* h, int T, float* result, b
   for (int l = 0; l < h->L; ++l) e.hw[l] = h->geo[l].h * h->geo[l].w;
   e.result = result;
   e.per_task = per_task ? 1 : 0; e.result_stride = maml_b200_result_size(h);
+  e.lnb = h->lnb;
   return e;
 }
 
@@ -1219,6 +1317,8 @@ static int check_call(const maml_b200_handle* h, bool ptrs, int n_tasks, int num
   if (!h || !ptrs) return fail("null argument");
   if (n_tasks < 1 || n_tasks > h->maxT) return fail("n_tasks out of range");
   if (num_step < 0 || num_step >= h->S) return fail("num_step out of range");
+  if (h->ln) return fail("the functional network operator does not support layer norm (norm_layer = 1): only "
+                         "maml_b200_meta_batch_fwd_bwd runs the layer-norm network");
   return 0;
 }
 
@@ -1511,7 +1611,8 @@ extern "C" int maml_b200_adam_step(maml_b200_handle* h, float* meta, const float
 extern "C" int maml_b200_running_stats_update(maml_b200_handle* h, const float* result, float* running_mean, float* running_var,
                                               const float* decay_host, void* stream) {
   if (!h || !result || !running_mean || !running_var || !decay_host) return fail("null argument");
-  if (!h->cfg.per_step_bn) return 0;    // shared-BN mode passes running stats = None in the reference: no update
+  // shared-BN mode passes running stats = None in the reference, and layer norm has none: no update
+  if (!h->pl.per_step_bn) return 0;
   LaunchScope launch_scope(h);
   cudaStream_t st = (cudaStream_t)stream;
   float* pin = h->pinned + 32 * (h->pin_slot++ & 15);

@@ -1053,3 +1053,303 @@ void launch_tail_tan_fused(const BnActTanArgs& fa, const HeadArgs& ha, const BnB
 }
 
 MAML_TRACE_SETTER(trace_set_bn)
+
+// ---------------------------------------------------------------------------------------------------------------
+// Layer norm (reference MetaLayerNormLayer, meta_neural_network_architectures.py:261-322: F.layer_norm over the conv
+// output [F, h, w] of each image, eps 1e-5, frozen all-ones weight, learnable bias [F, h, w]).  The statistics are per
+// image, so a query image's output does not depend on the other images of the batch.  The per-element formulas are the
+// BatchNorm ones above with gamma = 1 and per-image constants: bn_act(1, zh, b) = fmaf(1, zh, b) = zh + b exactly, and the
+// pooling decision is keep_first_max's.  Every reduction is spread over several CTAs per image (grid (CTAs per image,
+// images, tasks)); each CTA adds its two fp64 totals to the image's sums with one atomic each.  The bias gradient (sum over
+// the images of dy at each position) runs one thread per (window, channel quad) over the images in order: deterministic.
+// ---------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float4 ones4() { return make_float4(1.f, 1.f, 1.f, 1.f); }
+__device__ __forceinline__ float4 splat4(float v) { return make_float4(v, v, v, v); }
+
+// per-image constants from fp64 sums (m = F h w): mean and r = 1 / sqrt(var + eps), as chan_setup does per channel
+__device__ __forceinline__ void ln_image_consts(const double* st, double m, float& mu, float& r) {
+  const double mean = st[0] / m;
+  double var = st[1] / m - mean * mean;
+  if (var < 0.0) var = 0.0;
+  mu = (float)mean;
+  r = (float)(1.0 / sqrt(var + BN_EPS_D));
+}
+__device__ __forceinline__ const double* ln_st(const double* base, long long stride, int task, int img) {
+  return base + (long long)task * stride + 2LL * img;
+}
+// the layer-norm bias of channel quad q at pixel (yy, xx): [F][h][w]
+__device__ __forceinline__ float4 ln_bias4(const float* b, const BnGeom& g, int q, int yy, int xx) {
+  const long long hw = (long long)g.h * g.w, o = (long long)(q * 4) * hw + (long long)yy * g.w + xx;
+  return make_float4(b[o], b[o + hw], b[o + 2 * hw], b[o + 3 * hw]);
+}
+// CTA totals of (s1, s2) added to one image's sums (fixed order inside the CTA, one fp64 atomic per sum)
+__device__ __forceinline__ void ln_block_add(double s1, double s2, double* dst) {
+  __shared__ double red[2][32];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { s1 += __shfl_xor_sync(0xffffffffu, s1, o); s2 += __shfl_xor_sync(0xffffffffu, s2, o); }
+  const int w = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
+  if ((threadIdx.x & 31) == 0) { red[0][w] = s1; red[1][w] = s2; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t1 = 0.0, t2 = 0.0;
+    for (int k = 0; k < nw; ++k) { t1 += red[0][k]; t2 += red[1][k]; }
+    atomicAdd(dst, t1);
+    atomicAdd(dst + 1, t2);
+  }
+}
+// The windows of image blockIdx.y handled by this thread: wi = blockIdx.x * WPB + lane, stride gridDim.x * WPB
+#define LN_FOR_WINDOWS(it, wy, wx)                                                                          \
+  for (int wi_ = blockIdx.x * (it).WPB + (it).lane, wy = 0, wx = 0; wi_ < (it).hc * (it).wc;                \
+       wi_ += gridDim.x * (it).WPB)                                                                         \
+    if ((wy = wi_ / (it).wc, wx = wi_ - wy * (it).wc), true)
+
+// sums of one image: primal (sum z, sum z^2); tangent (sum zdot, sum zh * zdot) with zdot = z + z2
+template <bool TAN>
+__global__ void __launch_bounds__(256) ln_stats_kernel(LnArgs a) {
+  pdl_prologue(TAN ? 34 : 33, a.tag);
+  const BnGeom g = a.g;
+  const int img = blockIdx.y, task = blockIdx.z;
+  WinIter it(g);
+  double s1 = 0.0, s2 = 0.0;
+  if (it.lane < it.WPB) {
+    const float* z = a.z + (long long)task * a.z_stride;
+    const float* z2 = a.z2 ? a.z2 + (long long)task * a.z_stride : nullptr;
+    const float* zhp = TAN ? a.zh + (long long)task * a.zh_stride : nullptr;
+    LN_FOR_WINDOWS(it, wy, wx) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
+        if (yy < g.h && xx < g.w) {
+          const long long idx = it.grid(g, img, yy, xx);
+          const float4 v = TAN ? ld4_sum(z, z2, idx) : ld4(z + idx);
+          const float4 w = TAN ? ld4(zhp + idx) : v;
+#pragma unroll
+          for (int c = 0; c < 4; ++c) { s1 += (double)comp(v, c); s2 += (double)comp(v, c) * (double)comp(w, c); }
+        }
+      }
+    }
+  }
+  ln_block_add(s1, s2, a.st_out + (long long)task * a.st_stride + 2LL * img);
+}
+
+// primal: zh = (z - mu) r in place, y = zh + b, p = max-pool(leaky(y)).  Tangent (z = zdot):
+// zhdot = r (zdot - mean zdot - zh mean(zh zdot)) in place, pdot = slope * zhdot at the arg-max.
+template <bool TAN>
+__global__ void __launch_bounds__(256) ln_act_kernel(LnArgs a) {
+  pdl_prologue(TAN ? 36 : 35, a.tag);
+  const BnGeom g = a.g;
+  const int img = blockIdx.y, task = blockIdx.z;
+  const double m = (double)g.F * g.h * g.w;
+  WinIter it(g);
+  if (it.lane >= it.WPB) return;
+  float mu, r;
+  ln_image_consts(ln_st(a.st_fwd, a.st_stride, task, img), m, mu, r);
+  float md = 0.f, qq = 0.f;
+  if (TAN) {
+    const double* stt = ln_st(a.st_tan, a.st_stride, task, img);
+    md = (float)(stt[0] / m); qq = (float)(stt[1] / m);
+  }
+  const float4 one = ones4();
+  float* z = a.z + (long long)task * a.z_stride;
+  const float* z2 = a.z2 ? a.z2 + (long long)task * a.z_stride : nullptr;
+  const float* zhp = TAN ? a.zh + (long long)task * a.zh_stride : nullptr;
+  float* p = a.out + (long long)task * a.out_stride;
+  LN_FOR_WINDOWS(it, wy, wx) {
+    WinMax w{};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
+      if (yy < g.h && xx < g.w) {
+        const long long idx = it.grid(g, img, yy, xx);
+        const float4 be = ln_bias4(a.bias, g, it.q, yy, xx);
+        if (TAN) {
+          const float4 zh = ld4(zhp + idx);
+          const float4 zhd = bn_tan_normalize(ld4_sum(z, z2, idx), zh, splat4(r), splat4(md), splat4(qq));
+          st4(z + idx, zhd);
+          const BnAct v = bn_act(one, zh, be);
+          keep_first_max(k, v, w, act_tangent<false>(v, one, zhd, zh));
+        } else {
+          const float4 zh = bn_normalize(ld4(z + idx), splat4(mu), splat4(r));
+          st4(z + idx, zh);
+          keep_first_max(k, bn_act(one, zh, be), w);
+        }
+      }
+    }
+    if (wy < g.ph && wx < g.pw) {
+      const long long pidx = it.pooled(g, img, wy, wx);
+      const float4 o = TAN ? w.p : w.act;
+      st4(p + pidx, o);
+      if (a.out_hi) st4_split(a.out_hi + (long long)task * a.out_stride, a.out_lo + (long long)task * a.out_stride, pidx, o);
+    }
+  }
+}
+
+// the arg-max window of the backward-type kernels, with the per-position layer-norm bias in place of beta
+__device__ __forceinline__ void ln_argmax_window(const float* __restrict__ zhp, const float* bias, const BnGeom& g, int img,
+                                                 int wy, int wx, const WinIter& it, float4 (&zh)[4], long long (&idx)[4],
+                                                 int4& arg, float4& slope_at) {
+  WinMax w{};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
+    idx[k] = it.grid(g, img, yy, xx);
+    zh[k] = ld4(zhp + idx[k]);
+    keep_first_max(k, bn_act(ones4(), zh[k], ln_bias4(bias, g, it.q, yy, xx)), w);
+  }
+  arg = w.arg;
+  slope_at = slope_of(w.y);
+}
+
+// per-image backward sums: primal (S1 = sum dy, S2 = sum dy zh); tangent (T1 = sum dydot, T2 = sum dydot zh + dy zhdot)
+template <bool TAN>
+__global__ void __launch_bounds__(256) ln_bwd_reduce_kernel(LnArgs a) {
+  pdl_prologue(TAN ? 38 : 37, a.tag);
+  const BnGeom g = a.g;
+  const int img = blockIdx.y, task = blockIdx.z;
+  WinIter it(g);
+  double s1[4] = {0, 0, 0, 0}, s2[4] = {0, 0, 0, 0};
+  if (it.lane < it.WPB) {
+    const float* zhp = a.zh + (long long)task * a.zh_stride;
+    const float* dp = a.dp + (long long)task * a.dp_stride;
+    LN_FOR_WINDOWS(it, wy, wx) {
+      if (wy >= g.ph || wx >= g.pw) continue;
+      float4 zh[4]; long long idx[4]; int4 arg; float4 sl;
+      ln_argmax_window(zhp, a.bias, g, img, wy, wx, it, zh, idx, arg, sl);
+      const long long pidx = it.pooled(g, img, wy, wx);
+      if (TAN) {
+        const float* zhd = a.zhd + (long long)task * a.zhd_stride;
+        const float4 dd = ld4_sum(a.dpd + (long long)task * a.dpd_stride, a.dpd2 ? a.dpd2 + (long long)task * a.dpd_stride : nullptr, pidx);
+        bn_tan_bwd_sums(ld4(dp + pidx), dd, sl, zh, arg, [&](int k, int c) { return zhd[pick(idx, k) + c]; }, s1, s2);
+      } else {
+        bn_bwd_sums(ld4(dp + pidx), sl, zh, arg, s1, s2);
+      }
+    }
+  }
+  ln_block_add(s1[0] + s1[1] + s1[2] + s1[3], s2[0] + s2[1] + s2[2] + s2[3],
+               a.st_out + (long long)task * a.st_stride + 2LL * img);
+}
+
+// primal: dz = r (dy - S1/m - zh S2/m); tangent: dzdot = -r q dz + r (dydot - T1/m - zhdot S2/m - zh T2/m)
+template <bool TAN>
+__global__ void __launch_bounds__(256) ln_bwd_apply_kernel(LnArgs a) {
+  pdl_prologue(TAN ? 40 : 39, a.tag);
+  const BnGeom g = a.g;
+  const int img = blockIdx.y, task = blockIdx.z;
+  const double m = (double)g.F * g.h * g.w;
+  WinIter it(g);
+  if (it.lane >= it.WPB) return;
+  float mu, r;
+  ln_image_consts(ln_st(a.st_fwd, a.st_stride, task, img), m, mu, r);
+  // this pass's sums (primal S1, S2; tangent T1, T2) are in st_out; the tangent also reads the primal S2 and q
+  const double* sc = ln_st(a.st_out, a.st_stride, task, img);
+  const float4 rr = splat4(r);
+  float4 c1 = splat4((float)(sc[0] / m)), c2 = splat4((float)(sc[1] / m)), rq = float4(), t1 = float4(), t2 = float4();
+  if (TAN) {
+    t1 = c1; t2 = c2;
+    c2 = splat4((float)(ln_st(a.st_bwd, a.st_stride, task, img)[1] / m));
+    rq = splat4(-r * (float)(ln_st(a.st_tan, a.st_stride, task, img)[1] / m));
+  }
+  const float* zhp = a.zh + (long long)task * a.zh_stride;
+  float* dz = a.out + (long long)task * a.out_stride;
+  LN_FOR_WINDOWS(it, wy, wx) {
+    const bool full = (wy < g.ph && wx < g.pw);
+    int4 arg = make_int4(-1, -1, -1, -1);
+    float4 dy = float4();
+    if (full) {
+      float4 zh[4]; long long idx[4]; float4 sl;
+      ln_argmax_window(zhp, a.bias, g, img, wy, wx, it, zh, idx, arg, sl);
+      const long long pidx = it.pooled(g, img, wy, wx);
+      dy = TAN ? mul4(ld4_sum(a.dpd + (long long)task * a.dpd_stride, a.dpd2 ? a.dpd2 + (long long)task * a.dpd_stride : nullptr, pidx), sl)
+               : mul4(ld4(a.dp + (long long)task * a.dp_stride + pidx), sl);
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
+      if (yy < g.h && xx < g.w) {
+        const long long idx = it.grid(g, img, yy, xx);
+        const float4 zh = ld4(zhp + idx);
+        float4 o;
+        if (TAN) {
+          o = bn_tan_bwd_dz(rq, ld4(a.dz + (long long)task * a.dz_stride + idx), rr, t1,
+                            ld4(a.zhd + (long long)task * a.zhd_stride + idx), c2, zh, t2, k, arg, dy, full);
+        } else {
+          o = full ? bn_bwd_dz(rr, c1, zh, c2, k, arg, dy) : bn_bwd_dz<true>(rr, c1, zh, c2);
+        }
+        st4(dz + idx, o);
+        if (a.out_hi) st4_split(a.out_hi + (long long)task * a.out_stride, a.out_lo + (long long)task * a.out_stride, idx, o);
+      }
+    }
+  }
+}
+
+// bias gradient of one pass: db[c][y][x] = sum over the images (in order) of dy (tangent: dydot) at (c, y, x); dy reaches
+// only the arg-max of a full window.  One thread per (window, channel quad); grid (window groups, tasks).
+template <bool TAN>
+__global__ void __launch_bounds__(256) ln_bias_grad_kernel(LnArgs a) {
+  pdl_prologue(TAN ? 42 : 41, a.tag);
+  const BnGeom g = a.g;
+  const int task = blockIdx.y;
+  WinIter it(g);
+  const int wi = blockIdx.x * it.WPB + it.lane;
+  if (it.lane >= it.WPB || wi >= it.hc * it.wc) return;
+  const int wy = wi / it.wc, wx = wi - wy * it.wc;
+  float4 acc[4] = {float4(), float4(), float4(), float4()};
+  if (wy < g.ph && wx < g.pw) {
+    const float* zhp = a.zh + (long long)task * a.zh_stride;
+    const float* src = TAN ? a.dpd + (long long)task * a.dpd_stride : a.dp + (long long)task * a.dp_stride;
+    const float* src2 = TAN && a.dpd2 ? a.dpd2 + (long long)task * a.dpd_stride : nullptr;
+    for (int img = 0; img < g.n; ++img) {
+      float4 zh[4]; long long idx[4]; int4 arg; float4 sl;
+      ln_argmax_window(zhp, a.bias, g, img, wy, wx, it, zh, idx, arg, sl);
+      const float4 dy = mul4(ld4_sum(src, src2, it.pooled(g, img, wy, wx)), sl);
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        acc[k] = map4([k](float s, int ar, float d) { return ar == k ? s + d : s; }, acc[k], arg, dy);
+    }
+  }
+  float* db = a.db + (long long)task * a.db_stride;
+  const long long hw = (long long)g.h * g.w;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
+    if (yy < g.h && xx < g.w) {
+      const long long o = (long long)(it.q * 4) * hw + (long long)yy * g.w + xx;
+#pragma unroll
+      for (int c = 0; c < 4; ++c) db[o + c * hw] = comp(acc[k], c);
+    }
+  }
+}
+
+// grid of the per-image kernels: (CTAs per image, images, tasks), at most about 4 CTAs per SM in all
+static inline dim3 ln_grid(const BnGeom& g, int tasks, int* block) {
+  const WinGeom wg = win_geom(g);
+  *block = wg.wpb * (g.F / 4);
+  const int per_img = ((g.h + 1) / 2) * ((g.w + 1) / 2);
+  int bx = (per_img + wg.wpb - 1) / wg.wpb;
+  const int cap = std::max(1, 4 * num_sms() / std::max(1, g.n * tasks));
+  if (bx > cap) bx = cap;
+  return dim3(bx, g.n, tasks);
+}
+
+template <class K>
+static void ln_launch(K kernel, const LnArgs& a, cudaStream_t st) {
+  ProfScope prof_scope__(PROF_BN, 0.0, st);
+  int block; const dim3 grid = ln_grid(a.g, a.tasks, &block);
+  launch_pdl(kernel, grid, dim3(block), (size_t)(0), st, tagged(a));
+  CUDA_CHECK_LAUNCH();
+}
+
+void launch_ln_stats(const LnArgs& a, bool tan, cudaStream_t st) { ln_launch(tan ? ln_stats_kernel<true> : ln_stats_kernel<false>, a, st); }
+void launch_ln_act(const LnArgs& a, bool tan, cudaStream_t st) { ln_launch(tan ? ln_act_kernel<true> : ln_act_kernel<false>, a, st); }
+void launch_ln_bwd(const LnArgs& a, bool tan, cudaStream_t st) {
+  ln_launch(tan ? ln_bwd_reduce_kernel<true> : ln_bwd_reduce_kernel<false>, a, st);
+  ln_launch(tan ? ln_bwd_apply_kernel<true> : ln_bwd_apply_kernel<false>, a, st);
+}
+void launch_ln_bias_grad(const LnArgs& a, bool tan, cudaStream_t st) {
+  ProfScope prof_scope__(PROF_BN, 0.0, st);
+  const WinGeom wg = win_geom(a.g);
+  const int per_img = ((a.g.h + 1) / 2) * ((a.g.w + 1) / 2);
+  const dim3 grid((per_img + wg.wpb - 1) / wg.wpb, a.tasks);
+  launch_pdl(tan ? ln_bias_grad_kernel<true> : ln_bias_grad_kernel<false>, grid, dim3(wg.wpb * (a.g.F / 4)), (size_t)(0), st, tagged(a));
+  CUDA_CHECK_LAUNCH();
+}

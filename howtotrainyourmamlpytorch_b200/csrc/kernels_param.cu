@@ -244,7 +244,7 @@ __device__ __forceinline__ void export_body(const ExportArgs& a, float* __restri
   const int lane = threadIdx.x & 31;
   long long e = ((long long)blockIdx.x - nb1) * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const long long bnsz = (long long)(pl.per_step_bn ? pl.S : 1) * pl.F;
-  const long long E_bn = 2LL * pl.L * bnsz, E_lslr = (long long)pl.nseg_inner * (pl.S + 1), E_run = pl.per_step_bn ? 2 * LSF : 0;
+  const long long E_bn = pl.ln ? 0 : 2LL * pl.L * bnsz, E_lslr = (long long)pl.nseg_inner * (pl.S + 1), E_run = pl.per_step_bn ? 2 * LSF : 0;
   double val = 0.0, scale = invB;
   long long dst;
   if (e < E_bn) {
@@ -313,6 +313,19 @@ __device__ __forceinline__ void export_body(const ExportArgs& a, float* __restri
         }
       }
     }
+  } else if (pl.ln && (e -= E_run) < pl.lnb_off[pl.L]) {
+    // layer-norm bias: target-pass gradients minus the Hessian-vector terms of every step (one step-independent tensor)
+    int l = 0;
+    while (e >= pl.lnb_off[l + 1]) ++l;
+    dst = pl.m_lnb[l] + (e - pl.lnb_off[l]);
+    if (a.training) {
+      const long long row = pl.lnb_off[pl.L];
+      for (int k = lane; k < nt * a.num_steps; k += 32) {
+        const int tk = k / a.num_steps, t = t0 + tk, s = k - tk * a.num_steps;
+        const float* r = a.lnb + ((long long)t * 2 * pl.S + s) * row + e;
+        val += (double)r[0] - (double)r[(long long)pl.S * row];
+      }
+    }
   } else {
     return;                                        // warp-uniform
   }
@@ -324,7 +337,8 @@ void launch_export(const ExportArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_PARAM, 0.0, st);
   const ParamLayout& pl = a.pl;
   const long long bnsz = (long long)(pl.per_step_bn ? pl.S : 1) * pl.F;
-  const long long entries = 2LL * pl.L * bnsz + (long long)pl.nseg_inner * (pl.S + 1) + 2 + (pl.per_step_bn ? 2LL * pl.L * pl.S * pl.F : 0);
+  const long long entries = (pl.ln ? pl.lnb_off[pl.L] : 2LL * pl.L * bnsz) + (long long)pl.nseg_inner * (pl.S + 1) + 2 +
+                            (pl.per_step_bn ? 2LL * pl.L * pl.S * pl.F : 0);
   const long long blocks = (pl.P + 255) / 256 + (entries + 7) / 8;        // range 1: thread per element; range 2: warp per entry
   launch_pdl(export_kernel, dim3((unsigned)blocks, a.per_task ? (unsigned)a.tasks : 1u), dim3(256), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();

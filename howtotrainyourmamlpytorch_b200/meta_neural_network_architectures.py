@@ -70,17 +70,47 @@ class MetaBatchNormLayer(nn.Module):
                     self.running_var[0].mul_(1.0 - momentum)
 
 
+class MetaLayerNormLayer(nn.Module):
+    """Reference ``MetaLayerNormLayer`` (:261-322): ``F.layer_norm`` over the conv output [F, h, w] of each image (the size
+    BEFORE pooling), eps 1e-5.  ``weight`` is registered first, as ones with ``requires_grad=False``: the reference never
+    trains it, but ``F.layer_norm`` multiplies by it, so the engine accepts only all-ones weights (it adds the bias to the
+    normalised values).  ``bias`` [F, h, w] is an outer (Adam) parameter, not adapted in the inner loop.  No running
+    statistics, no per-step index."""
+
+    def __init__(self, input_feature_shape, eps=1e-5, elementwise_affine=True):
+        super().__init__()
+        if not elementwise_affine:
+            raise NotImplementedError("MetaLayerNormLayer without elementwise_affine is not on the accelerated path "
+                                      "(the reference network always builds it with the affine parameters)")
+        self.normalized_shape = torch.Size(int(d) for d in input_feature_shape)
+        self.eps = eps
+        self.elementwise_affine = True
+        self.weight = nn.Parameter(torch.ones(self.normalized_shape), requires_grad=False)
+        self.bias = nn.Parameter(torch.zeros(self.normalized_shape))
+
+    def restore_backup_stats(self):
+        pass
+
+
 class MetaConvNormLayerReLU(nn.Module):
     def __init__(self, input_shape, num_filters, kernel_size, stride, padding, use_bias, args, normalization=True,
                  meta_layer=True, no_bn_learnable_params=False, device=None):
         super().__init__()
-        if not normalization or getattr(args, "norm_layer", "batch_norm") != "batch_norm":
-            raise NotImplementedError("only norm_layer='batch_norm' is on the accelerated path")
+        norm = getattr(args, "norm_layer", "batch_norm")
+        if not normalization or norm not in ("batch_norm", "layer_norm"):
+            raise NotImplementedError("only norm_layer='batch_norm' or 'layer_norm' is on the accelerated path")
         self.layer_dict = nn.ModuleDict()
         self.conv = MetaConv2dLayer(in_channels=int(input_shape[1]), out_channels=num_filters, kernel_size=kernel_size,
                                     stride=stride, padding=padding, use_bias=use_bias)
-        self.norm_layer = MetaBatchNormLayer(num_filters, device=device, args=args,
-                                             use_per_step_bn_statistics=args.per_step_bn_statistics)
+        if norm == "layer_norm":
+            if getattr(args, "enable_inner_loop_optimizable_bn_params", False):
+                raise NotImplementedError("enable_inner_loop_optimizable_bn_params with norm_layer='layer_norm' is "
+                                          "outside the accelerated path")
+            # normalized_shape = the conv output of one image: 3x3 / stride 1 / padding 1 keeps h x w
+            self.norm_layer = MetaLayerNormLayer(input_feature_shape=(num_filters, int(input_shape[2]), int(input_shape[3])))
+        else:
+            self.norm_layer = MetaBatchNormLayer(num_filters, device=device, args=args,
+                                                 use_per_step_bn_statistics=args.per_step_bn_statistics)
 
 
 class VGGReLUNormNetwork(nn.Module):
@@ -164,6 +194,9 @@ class VGGReLUNormNetwork(nn.Module):
         batches in task order, so a vmapped inner loop updates the running statistics step-major (every task's support
         pass at step s, then every target pass), not task-major as the reference's loop over tasks does."""
         from . import _native
+        if getattr(self.args, "norm_layer", "batch_norm") == "layer_norm":
+            raise NotImplementedError("VGGReLUNormNetwork.forward (the functional network operator) does not run the "
+                                      "layer-norm network; MAMLFewShotClassifier.run_train_iter / run_validation_iter do")
         if x.device.type != "cuda":
             raise _native.NativeLibraryError("VGGReLUNormNetwork.forward needs a CUDA (sm_90a) device: no CPU fallback")
         n = int(x.shape[0])

@@ -10,6 +10,8 @@ vector finishes the iteration:
         r_new = 0.9^U r_old + sum_k 0.1 * 0.9^(U-1-k) stat_k,      U = updates at that step,
     so each rank pre-weights its own statistics by their (static) position k and the same all-reduce
     reproduces the sequential result.  (csrc/kernels_param.cu: export_kernel computes the weighted sums.)
+    The layer-norm network (norm_layer "layer_norm") has no running statistics: its result vector ends after the
+    number of correct predictions, and nothing here applies to it.
 """
 
 BN_MOMENTUM = 0.1

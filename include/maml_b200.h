@@ -28,11 +28,11 @@ extern "C" {
 
 #define MAML_B200_MAX_STAGES 4
 #define MAML_B200_MAX_STEPS 8
-#define MAML_B200_ABI_VERSION 2
+#define MAML_B200_ABI_VERSION 3
 
 /* Static shape of the path.  Mirrors the args the reference reads on this path:
  * num_classes_per_set, num_samples_per_class, num_target_samples, image_{channels,height,width},
- * cnn_num_filters, num_stages, number_of_training_steps_per_iter, per_step_bn_statistics. */
+ * cnn_num_filters, num_stages, number_of_training_steps_per_iter, per_step_bn_statistics, norm_layer. */
 typedef struct maml_b200_config {
   int32_t n_way;        /* N  classes per task                         */
   int32_t k_shot;       /* K  support samples per class                */
@@ -47,6 +47,10 @@ typedef struct maml_b200_config {
   int32_t max_tasks;    /* max tasks per call on this GPU (workspace)  */
   int32_t reserved;     /* test switches. bit 0: keep the activations of EVERY target pass for debug_read;
                            bit 1: run blocks l >= 1 on the fp32 FFMA kernels instead of wgmma 3xTF32 */
+  int32_t norm_layer;   /* 0: batch norm; 1: layer norm (reference MetaLayerNormLayer: statistics per image over
+                           [F, h, w], frozen all-ones weight, learnable bias [F, h, w]; per_step_bn is then ignored,
+                           there are no running statistics).  Layer-norm handles run maml_b200_meta_batch_fwd_bwd and
+                           the parameter entries; the functional entries (maml_b200_net_*) refuse them. */
 } maml_b200_config;
 
 /* Per-call schedule: what reference forward(...) derives from epoch / phase (:232-244,:304-305). */
@@ -74,8 +78,9 @@ int64_t maml_b200_workspace_bytes(const maml_b200_handle* h);
 
 /* Flat meta-parameter vector ("meta"), reference layout and reference Adam order
  * (reference few_shot_learning_system.py:288-294): per block conv.weight[F,Cin,3,3],
- * conv.bias[F], norm_layer.bias[S|1,F], norm_layer.weight[S|1,F]; then linear.weights[N,D],
- * linear.bias[N]; then the 2*stages+2 LSLR vectors [S+1] in inner-parameter order. */
+ * conv.bias[F], norm_layer.bias[S|1,F], norm_layer.weight[S|1,F] (layer norm: conv.weight, conv.bias,
+ * norm_layer.bias[F,h_l,w_l]); then linear.weights[N,D], linear.bias[N]; then the 2*stages+2 LSLR
+ * vectors [S+1] in inner-parameter order. */
 int32_t maml_b200_num_segments(const maml_b200_handle* h);
 int maml_b200_segment(const maml_b200_handle* h, int32_t idx, int64_t* offset, int64_t* size);
 int64_t maml_b200_meta_size(const maml_b200_handle* h);
@@ -85,8 +90,8 @@ int64_t maml_b200_meta_size(const maml_b200_handle* h);
  *                                      and summed over the LOCAL tasks (all-reduce SUM completes it)
  *   [meta_size]                        sum over local tasks of task_loss / B
  *   [meta_size + 1]                    number of correct last-step target predictions (local)
- *   [meta_size + 2, +stages*S*F)       running-mean EMA partial sums   (per_step_bn only)
- *   [.. , +stages*S*F)                 running-var  EMA partial sums   (per_step_bn only)
+ *   [meta_size + 2, +stages*S*F)       running-mean EMA partial sums   (per_step_bn batch norm only)
+ *   [.. , +stages*S*F)                 running-var  EMA partial sums   (per_step_bn batch norm only)
  * The whole vector is linear in the tasks, so ONE all-reduce(sum) over ranks finishes it. */
 int64_t maml_b200_result_size(const maml_b200_handle* h);
 
