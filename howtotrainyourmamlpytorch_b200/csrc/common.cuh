@@ -166,6 +166,7 @@ struct LnArgs {
   double* st_out;                        // the sums a stats / reduce kernel accumulates
   long long st_stride;
   const float* bias;                     // [F][h][w] layer-norm bias (act kernels)
+  const float* bdot; long long bdot_stride;   // tangent act: nullable bias tangent [F][h][w] per task (stride 0: shared)
   float* db; long long db_stride;        // bias gradient: [F][h][w] per task (stored, not accumulated)
   BnGeom g; int tasks;
   int tag;          // launch sequence number inside the iteration (device trace)
@@ -252,7 +253,7 @@ void launch_bnbwd(const BnBwdArgs& a, cudaStream_t st);          // reduce + app
 void launch_bnbwd_tan(const BnBwdTanArgs& a, cudaStream_t st);
 // layer norm (kernels_bn.cu).  tan = false: primal forward / backward; true: their forward-mode tangents
 void launch_ln_stats(const LnArgs& a, bool tan, cudaStream_t st);   // per-image sums of z (or of zdot and zh * zdot)
-void launch_ln_act(const LnArgs& a, bool tan, cudaStream_t st);     // normalise, + bias, leaky-ReLU, max-pool
+void launch_ln_act(const LnArgs& a, bool tan, cudaStream_t st);     // normalise, + bias, leaky-ReLU, max-pool (+ bdot)
 void launch_ln_bwd(const LnArgs& a, bool tan, cudaStream_t st);     // per-image backward sums, then dz (or dzdot)
 void launch_ln_bias_grad(const LnArgs& a, bool tan, cudaStream_t st);  // sum over the images of dy (or dydot)
 bool tail_fusable(const BnGeom& g, int n_rows, int rows_per_cta);

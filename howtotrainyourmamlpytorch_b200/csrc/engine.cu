@@ -934,13 +934,14 @@ static HeadArgs tangent_head_args(const maml_b200_handle* h, int s, const float*
 
 // Forward half of the tangent pass at support slot s: the tangent of the support forward in direction u (weights), plus
 // the image tangent xdot_g (padded grid, nullable: W_0 applied to it joins block 0's tangent conv as a second operand
-// pair) and the BatchNorm gamma / beta tangents of step s read from the meta-layout vector t_bn (nullable).  Leaves the
-// normalised tangents in tan.zh and the pooled ones in tan.ain; the features' tangent is tan.ain[L].
+// pair) and the norm tangents read from the meta-layout vector t_bn (nullable): BatchNorm gamma / beta of step s (shared by
+// the tasks), or the layer-norm biases (t_stride floats between tasks, 0: shared).  Leaves the normalised tangents in
+// tan.zh and the pooled ones in tan.ain; the features' tangent is tan.ain[L].
 // pre_dgrad: also enqueue the u-weight dgrad convs of the backward half on spre, right behind the forward ones.
 // defer_last: the last block's BatchNorm tangent is not launched but returned (the fused last-block kernel runs it).
 static void tangent_forward(maml_b200_handle* h, int s, const float* theta, const float* u, const float* meta,
-                            const float* xdot_g, const float* t_bn, int T, cudaStream_t st, cudaStream_t spre, bool pre_dgrad,
-                            BnActTanArgs* defer_last) {
+                            const float* xdot_g, const float* t_bn, long long t_stride, int T, cudaStream_t st,
+                            cudaStream_t spre, bool pre_dgrad, BnActTanArgs* defer_last) {
   const PassSet& sp = h->sup; const PassSet& tn = h->tan; const PassSet& t2 = h->tan2;
   // Tangent convs of blocks >= 1 have two operand pairs; the pair (primal activation, u weights) depends only on u and
   // on what phase A saved, not on the tangent chain.  It is computed up front on the side stream (right behind the
@@ -990,6 +991,7 @@ static void tangent_forward(maml_b200_handle* h, int s, const float* theta, cons
       launch_ln_stats(a, true, st);
       a.out = AIN(tn, l + 1, 0); a.out_stride = STRIDE(tn, ain, l + 1);
       if (h->use_tc && l + 1 < h->L) { a.out_hi = AIN_HI(tn, l + 1, 0); a.out_lo = AIN_LO(tn, l + 1, 0); }
+      if (t_bn) { a.bdot = t_bn + h->pl.m_lnb[l]; a.bdot_stride = t_stride; }
       launch_ln_act(a, true, st);
       continue;
     }
@@ -1009,15 +1011,17 @@ static void tangent_forward(maml_b200_handle* h, int s, const float* theta, cons
 }
 
 // forward-mode tangent of (support forward + support backward) at step s in direction u (and, with xdot_g, in the
-// images' direction x-dot: pass the padded grid of x-dot)  =>  H u into `partial`
+// images' direction x-dot: pass the padded grid of x-dot; with t_ln, a layer-norm handle's bias directions in the meta
+// layout, t_ln_stride floats between tasks)  =>  H u into `partial`
 static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const float* u, const float* meta,
                          const TangentHead& th, int T, cudaStream_t st, const ReduceSpec& rs, cudaStream_t spre,
-                         const float* xdot_g = nullptr) {
+                         const float* xdot_g = nullptr, const float* t_ln = nullptr, long long t_ln_stride = 0) {
   const PassSet& sp = h->sup; const PassSet& tn = h->tan; const PassSet& t2 = h->tan2;
   // the fused last-block kernels implement the cross-entropy tangent head only
   const bool fuse_tail = th.mode == HEAD_TANGENT && support_tail_fused(h);
   BnActTanArgs last_act{};
-  tangent_forward(h, s, theta, u, meta, xdot_g, nullptr, T, st, spre, true, fuse_tail ? &last_act : nullptr);
+  tangent_forward(h, s, theta, u, meta, xdot_g, h->ln ? t_ln : nullptr, t_ln_stride, T, st, spre, true,
+                  fuse_tail ? &last_act : nullptr);
   const ChunkPlan& cp = h->plan_sup;
   join_pending(h, st);
   const HeadArgs hd = tangent_head_args(h, s, theta, u, th, T);
@@ -1037,8 +1041,11 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
       a.out = DZ(tn, l, 0); a.out_stride = STRIDE(tn, dz, l);
       if (h->use_tc && l >= 1) { a.out_hi = DZ_HI(tn, l, 0); a.out_lo = DZ_LO(tn, l, 0); }
       launch_ln_bwd(a, true, st);
-      a.db = lnb_at(h, 1, s) + h->pl.lnb_off[l]; a.db_stride = 2LL * h->S * h->pl.lnb_off[h->L];
-      launch_ln_bias_grad(a, true, st);                  // H_b u: the tangent of the support loss's bias gradient
+      // H_b u, the tangent of the support loss's bias gradient: export subtracts kind 1 (fused iteration, b-bar -= H_b u)
+      // and adds kind 0 (functional operator, +H_b v), as it does with the BatchNorm gamma / beta sums of kind_tbwd
+      a.db = lnb_at(h, th.kind_tbwd == PASS_TGT_BWD ? 0 : 1, s) + h->pl.lnb_off[l];
+      a.db_stride = 2LL * h->S * h->pl.lnb_off[h->L];
+      launch_ln_bias_grad(a, true, st);
     } else {
     BnBwdTanArgs b{};
     b.dp = DP(sp, l, s); b.dp_stride = STRIDE(sp, dp, l);
@@ -1317,8 +1324,6 @@ static int check_call(const maml_b200_handle* h, bool ptrs, int n_tasks, int num
   if (!h || !ptrs) return fail("null argument");
   if (n_tasks < 1 || n_tasks > h->maxT) return fail("n_tasks out of range");
   if (num_step < 0 || num_step >= h->S) return fail("num_step out of range");
-  if (h->ln) return fail("the functional network operator does not support layer norm (norm_layer = 1): only "
-                         "maml_b200_meta_batch_fwd_bwd runs the layer-norm network");
   return 0;
 }
 
@@ -1404,10 +1409,16 @@ extern "C" int maml_b200_net_backward_tasks(maml_b200_handle* h, int32_t n_tasks
   LaunchScope launch_scope(h, st);
   const int T = n_tasks;
   record_call(h, FN_NONE, 0, 0);
-  // backward statistics (and the tangent ones export subtracts) start from zero; forward statistics are kept
-  for (int kind : {PASS_TGT_BWD, PASS_TAN_BWD})
+  // backward statistics (and the tangent ones export subtracts) start from zero; forward statistics are kept.  Layer norm:
+  // its backward sums are added to with atomics, and export sums both kinds of bias-gradient rows over every step
+  for (int kind : {PASS_TGT_BWD, PASS_TAN_BWD}) {
     CK(cudaMemset2DAsync(h->stats + (long long)kind * MAML_MAX_STEPS * h->st_pass_stride, (size_t)h->stats_task_stride * sizeof(double), 0,
                          (size_t)MAML_MAX_STEPS * h->st_pass_stride * sizeof(double), (size_t)T, st));
+    if (h->ln)
+      CK(cudaMemset2DAsync(h->ln_stats + (long long)kind * h->ln_pass_stride, (size_t)h->ln_task_stride * sizeof(double), 0,
+                           (size_t)h->ln_pass_stride * sizeof(double), (size_t)T, st));
+  }
+  if (h->ln) CK(cudaMemsetAsync(h->lnb, 0, (size_t)T * 2 * h->S * h->pl.lnb_off[h->L] * sizeof(float), st));
   if (clear_accumulators(h, CLR_ABAR | CLR_LOSSES | CLR_CORRECT, st)) return 1;
   external_backward(h, h->tgt, 0, num_step, PASS_TGT_FWD, PASS_TGT_BWD, meta_like, dlogits, h->tgt_partial, h->plan_tgt, T, st);
   launch_param_reduce(h->pl, h->plan_tgt.pd, h->tgt_partial, PR_STORE, nullptr, nullptr, h->tbar, nullptr, meta_like, num_step,
@@ -1451,8 +1462,10 @@ static int ensure_xdot(maml_b200_handle* h, cudaStream_t st) {
 // N*K images (the handle's support shape).  jv_out [n_tasks, N*K, N] = J v.  hv_out: result_size floats; the first meta_size
 // hold d/d(meta_like) <dlogits, J v> in the meta layout, summed over the batches: conv / linear entries are stored into
 // tbar by the parameter reduction, the BatchNorm gamma / beta sums go to the PASS_TGT_BWD statistics, which export adds
-// (+H_gamma v, +H_beta v); LSLR entries 0.  v_like's BatchNorm and LSLR entries are not read.  Overwrites the batch
-// statistics maml_b200_net_running_update reads; no running-statistics side effect of its own.
+// (+H_gamma v, +H_beta v), and a layer-norm handle's bias sums to the bias-gradient rows export adds (+H_b v); LSLR
+// entries 0.  v_like's BatchNorm and LSLR entries are not read; on a layer-norm handle its bias entries are the bias
+// directions (the tangent forward's b-dot).  Overwrites the batch statistics maml_b200_net_running_update reads; no
+// running-statistics side effect of its own.
 // meta_stride / dir_stride / sum_tasks: as in maml_b200_net_hvp_image_tasks.
 static int net_hvp_impl(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, long long meta_stride,
                         const float* x, const float* xdot, const float* dlogits, const float* v_like, long long dir_stride,
@@ -1472,7 +1485,7 @@ static int net_hvp_impl(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, 
   if (fork_direction(h, T, st, &spre)) return 1;
   ReduceSpec rs{PR_STORE, nullptr, nullptr, h->tbar, nullptr, s, -1};
   const TangentHead th_ext{HEAD_EXTERNAL_TAN, nullptr, dlogits, (long long)h->n_s * h->N, jv_out, PASS_TGT_BWD};
-  tangent_pass(h, s, th, h->u, meta_like, th_ext, T, st, rs, spre, xdot ? h->xdot_g : nullptr);
+  tangent_pass(h, s, th, h->u, meta_like, th_ext, T, st, rs, spre, xdot ? h->xdot_g : nullptr, v_like, dir_stride);
   join_pending(h, st);
   launch_export(export_args(h, T, hv_out, !sum_tasks), st);
   CK(cudaGetLastError());
@@ -1524,7 +1537,7 @@ extern "C" int maml_b200_net_jvp(maml_b200_handle* h, int32_t n_tasks, int32_t n
   const float* th = stage_forward(h, h->sup, s, PASS_SUP_FWD, s, meta_like, 0, x, xdot, t_like, 0, T, st);
   cudaStream_t spre;
   if (fork_direction(h, T, st, &spre)) return 1;
-  tangent_forward(h, s, th, h->u, meta_like, xdot ? h->xdot_g : nullptr, t_like, T, st, spre, false, nullptr);
+  tangent_forward(h, s, th, h->u, meta_like, xdot ? h->xdot_g : nullptr, t_like, 0, T, st, spre, false, nullptr);
   join_pending(h, st);
   launch_head(tangent_head_args(h, s, th, h->u, TangentHead{HEAD_EXTERNAL_TAN, nullptr, h->zero_dl, 0, jv_out, PASS_TGT_BWD}, T), st);
   CK(cudaGetLastError());
@@ -1583,7 +1596,7 @@ extern "C" int maml_b200_net_running_update(maml_b200_handle* h, int32_t n_tasks
                                            float* running_var, void* stream) {
   if (check_call(h, running_mean && running_var, n_tasks, num_step)) return 1;
   if (require_call(h, FN_FORWARD | FN_BACKWARD, n_tasks, num_step, "maml_b200_net_running_update")) return 1;
-  if (!h->cfg.per_step_bn) return 0;
+  if (!h->pl.per_step_bn) return 0;      // shared BatchNorm, and layer norm (no running statistics)
   LaunchScope launch_scope(h);
   int hw[MAML_MAX_LAYERS];
   for (int l = 0; l < h->L; ++l) hw[l] = h->geo[l].h * h->geo[l].w;

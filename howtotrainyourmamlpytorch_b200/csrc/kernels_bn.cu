@@ -1133,8 +1133,9 @@ __global__ void __launch_bounds__(256) ln_stats_kernel(LnArgs a) {
 }
 
 // primal: zh = (z - mu) r in place, y = zh + b, p = max-pool(leaky(y)).  Tangent (z = zdot):
-// zhdot = r (zdot - mean zdot - zh mean(zh zdot)) in place, pdot = slope * zhdot at the arg-max.
-template <bool TAN>
+// zhdot = r (zdot - mean zdot - zh mean(zh zdot)) in place, pdot = slope * ydot at the arg-max, ydot = zhdot (+ bdot with
+// BDOT: a bias tangent, read like the bias; b enters after the normalisation, so the statistics and zhdot do not see it).
+template <bool TAN, bool BDOT = false>
 __global__ void __launch_bounds__(256) ln_act_kernel(LnArgs a) {
   pdl_prologue(TAN ? 36 : 35, a.tag);
   const BnGeom g = a.g;
@@ -1153,6 +1154,7 @@ __global__ void __launch_bounds__(256) ln_act_kernel(LnArgs a) {
   float* z = a.z + (long long)task * a.z_stride;
   const float* z2 = a.z2 ? a.z2 + (long long)task * a.z_stride : nullptr;
   const float* zhp = TAN ? a.zh + (long long)task * a.zh_stride : nullptr;
+  const float* bd = BDOT ? a.bdot + (long long)task * a.bdot_stride : nullptr;
   float* p = a.out + (long long)task * a.out_stride;
   LN_FOR_WINDOWS(it, wy, wx) {
     WinMax w{};
@@ -1167,7 +1169,7 @@ __global__ void __launch_bounds__(256) ln_act_kernel(LnArgs a) {
           const float4 zhd = bn_tan_normalize(ld4_sum(z, z2, idx), zh, splat4(r), splat4(md), splat4(qq));
           st4(z + idx, zhd);
           const BnAct v = bn_act(one, zh, be);
-          keep_first_max(k, v, w, act_tangent<false>(v, one, zhd, zh));
+          keep_first_max(k, v, w, act_tangent<BDOT>(v, one, zhd, zh, float4(), BDOT ? ln_bias4(bd, g, it.q, yy, xx) : float4()));
         } else {
           const float4 zh = bn_normalize(ld4(z + idx), splat4(mu), splat4(r));
           st4(z + idx, zh);
@@ -1340,7 +1342,9 @@ static void ln_launch(K kernel, const LnArgs& a, cudaStream_t st) {
 }
 
 void launch_ln_stats(const LnArgs& a, bool tan, cudaStream_t st) { ln_launch(tan ? ln_stats_kernel<true> : ln_stats_kernel<false>, a, st); }
-void launch_ln_act(const LnArgs& a, bool tan, cudaStream_t st) { ln_launch(tan ? ln_act_kernel<true> : ln_act_kernel<false>, a, st); }
+void launch_ln_act(const LnArgs& a, bool tan, cudaStream_t st) {
+  ln_launch(!tan ? ln_act_kernel<false> : a.bdot ? ln_act_kernel<true, true> : ln_act_kernel<true>, a, st);
+}
 void launch_ln_bwd(const LnArgs& a, bool tan, cudaStream_t st) {
   ln_launch(tan ? ln_bwd_reduce_kernel<true> : ln_bwd_reduce_kernel<false>, a, st);
   ln_launch(tan ? ln_bwd_apply_kernel<true> : ln_bwd_apply_kernel<false>, a, st);

@@ -138,22 +138,56 @@ class VGGReLUNormNetwork(nn.Module):
         self.layer_dict["linear"] = MetaLinearLayer(input_shape=(shape[0], feat), num_filters=self.num_output_classes,
                                                     use_bias=True)
 
+    def _layer_norm(self):
+        return getattr(self.args, "norm_layer", "batch_norm") == "layer_norm"
+
+    def _segment_names(self):
+        """The operator's tensors in the engine's meta-vector order: per block conv.weight, conv.bias, then BatchNorm's
+        norm_layer.bias / norm_layer.weight (beta / gamma) or the layer norm's norm_layer.bias [F, h, w] alone (its frozen
+        all-ones weight is not a segment); then the linear layer."""
+        norm = ("norm_layer.bias",) if self._layer_norm() else ("norm_layer.bias", "norm_layer.weight")
+        names = []
+        for i in range(self.num_stages):
+            names += ["layer_dict.conv%d.%s" % (i, n) for n in ("conv.weight", "conv.bias") + norm]
+        return names + ["layer_dict.linear.weights", "layer_dict.linear.bias"]
+
+    def _norm_segments(self):
+        """(indices of the norm parameters among ``_segment_names``, whether the engine's tangent passes take directions
+        along them).  The layer-norm biases do (a bias tangent enters after the normalisation); BatchNorm gamma / beta do
+        not (they would be inner-loop fast weights, enable_inner_loop_optimizable_bn_params)."""
+        idx = tuple(i for i, n in enumerate(self._segment_names()) if ".norm_layer." in n)
+        return idx, self._layer_norm()
+
     def _segment_tensors(self, params):
-        """Tensors in the engine's meta-vector order (conv.weight, conv.bias, norm.bias, norm.weight per block; linear)."""
+        """Tensors in the engine's meta-vector order (``_segment_names``): ``params``' entries, else the module's own."""
+        own = dict(self.named_parameters())
+        fast = self._fast(params)
+        return [fast.get(n, own[n]) for n in self._segment_names()]
+
+    def _fast(self, params):
+        """``params`` keyed like the module's own parameters, without the reference's replica dim."""
         own = dict(self.named_parameters())
         fast = {}
         if params is not None:
             for k, v in params.items():
                 k = k.replace("module.", "")
                 fast[k] = v[0] if v.dim() == own[k].dim() + 1 else v   # strip the reference's replica dim
-        out = []
-        for i in range(self.num_stages):
-            p = "layer_dict.conv%d." % i
-            for n in (p + "conv.weight", p + "conv.bias", p + "norm_layer.bias", p + "norm_layer.weight"):
-                out.append(fast.get(n, own[n]))
-        for n in ("layer_dict.linear.weights", "layer_dict.linear.bias"):
-            out.append(fast.get(n, own[n]))
-        return out
+        return fast
+
+    def _check_layer_norm_weights(self, params):
+        """The engine applies the layer norm's frozen weight as ones (the reference creates it so and never trains it):
+        any other value, in ``params`` or in the module, is refused before anything runs.  The module's own weights are
+        checked again only when replaced or modified in place."""
+        fast, own = self._fast(params), dict(self.named_parameters())
+        ws = [(n, fast.get(n, own[n])) for n in ("layer_dict.conv%d.norm_layer.weight" % l for l in range(self.num_stages))]
+        key = tuple((n in fast, w.data_ptr(), w._version) for n, w in ws)
+        if not any(n in fast for n, _ in ws) and key == self.__dict__.get("_ln_weight_key"):
+            return
+        for n, w in ws:
+            if not bool(torch.all(w.detach() == 1)):
+                raise ValueError("%s is not all ones: the layer-norm network runs with the reference's frozen all-ones "
+                                 "weight only" % n)
+        self.__dict__["_ln_weight_key"] = key
 
     def _handles(self, x, spec=None):
         """The operator's engine handles for x's batch size, device and number of tasks (``spec``: None = one batch, else
@@ -173,14 +207,17 @@ class VGGReLUNormNetwork(nn.Module):
         or not; missing entries fall back to the module's own parameters.  BatchNorm always uses batch statistics
         (the reference hard-codes ``training=True``, :246-247) with the gamma / beta of ``num_step``, and -- like
         ``F.batch_norm`` there -- leaves its EMA update in ``running_mean / running_var[num_step]`` (per-step BN only).
+        The layer-norm network (``norm_layer: "layer_norm"``) normalises each image on its own, adds the bias
+        [F, h, w] (an outer parameter: differentiable, and a valid tangent or cotangent direction wherever the weights
+        are), has no running statistics and ignores ``num_step``; its frozen weight must be all ones (ValueError).
 
         Runs on the CUDA engine (C ABI ``maml_b200_net_forward`` / ``maml_b200_net_backward``) and is differentiable
         through ``torch.autograd`` with respect to every weight it uses (conv / linear fast weights, BatchNorm gamma /
         beta), which is what the reference's ``apply_inner_loop_update`` needs (``torch.autograd.grad`` of the support
         loss, few_shot_learning_system.py:138-139).  Twice differentiable: with ``create_graph=True`` the returned
         gradients are differentiable w.r.t. the weights (and the upstream d(logits)) through ``maml_b200_net_hvp``, so the
-        reference's second-order loop runs on this operator; a BatchNorm gamma / beta gradient is not (see
-        ``_FunctionalBackward``).  When ``x`` requires grad the operator is differentiable w.r.t. the images too
+        reference's second-order loop runs on this operator (a layer-norm bias gradient too); a BatchNorm gamma / beta
+        gradient is not (see ``_FunctionalBackward``).  When ``x`` requires grad the operator is differentiable w.r.t. the images too
         (``maml_b200_net_input_grad``), and with ``create_graph=True`` the weight gradients are differentiable w.r.t. ``x``
         (``maml_b200_net_hvp_input_grad``: the mixed term an outer loss needs to reach support images through the inner
         loop); the image gradient itself is not differentiable again.  With ``x`` not requiring grad none of this runs.
@@ -188,20 +225,23 @@ class VGGReLUNormNetwork(nn.Module):
 
         ``torch.func`` transforms work too: ``grad`` / ``vjp`` / ``jacrev`` (up to second order) and ``vmap`` over tasks,
         which runs the B mapped calls as ONE engine call with n_tasks = B (``maml_b200_net_*_tasks``) -- images, fast
-        weights and upstream cotangents may each be batched or shared.  BatchNorm gamma / beta stay shared by the tasks (a
-        batched gamma / beta raises NotImplementedError), as do ``torch.func.jvp`` / ``jacfwd`` / ``hessian`` (forward
-        mode runs through ``torch.autograd.forward_ad``) and third order.  A vmapped forward leaves the EMA of its B
-        batches in task order, so a vmapped inner loop updates the running statistics step-major (every task's support
-        pass at step s, then every target pass), not task-major as the reference's loop over tasks does."""
+        weights and upstream cotangents may each be batched or shared.  BatchNorm gamma / beta and the layer-norm biases
+        stay shared by the tasks (a batched one raises NotImplementedError); ``torch.func.jvp`` / ``jacfwd`` /
+        ``hessian`` (forward mode runs through ``torch.autograd.forward_ad``) and third order raise it too.  A vmapped
+        forward leaves the EMA of its B batches in task order, so a vmapped inner loop updates the running statistics
+        step-major (every task's support pass at step s, then every target pass), not task-major as the reference's loop
+        over tasks does."""
         from . import _native
-        if getattr(self.args, "norm_layer", "batch_norm") == "layer_norm":
-            raise NotImplementedError("VGGReLUNormNetwork.forward (the functional network operator) does not run the "
-                                      "layer-norm network; MAMLFewShotClassifier.run_train_iter / run_validation_iter do")
         if x.device.type != "cuda":
+            if self._layer_norm():
+                raise NotImplementedError("VGGReLUNormNetwork.forward on the layer-norm network runs on the CUDA engine "
+                                          "only (sm_90a): no CPU fallback")
             raise _native.NativeLibraryError("VGGReLUNormNetwork.forward needs a CUDA (sm_90a) device: no CPU fallback")
         n = int(x.shape[0])
         if n % self.num_output_classes != 0:
             raise ValueError("batch size %d is not a multiple of num_output_classes %d" % (n, self.num_output_classes))
+        if self._layer_norm():
+            self._check_layer_norm_weights(params)
         tensors = self._segment_tensors(params)
         return _FunctionalForward.apply(self, None, x, int(num_step), *tensors)
 
@@ -316,13 +356,16 @@ def _refuse_nested(spec):
                                   "engine has one task dimension (flatten the task dims into one vmap)")
 
 
-def _refuse_batched_bn(net, dims):
-    for i, d in enumerate(dims[:4 * net.num_stages]):
-        if d is not None and i % 4 >= 2:
+def _refuse_batched_norm(net, dims):
+    if any(dims[i] is not None for i in net._norm_segments()[0]):
+        if net._layer_norm():
             raise NotImplementedError(
-                "a BatchNorm gamma / beta batched under torch.func.vmap: the engine shares gamma / beta between the tasks "
-                "of a call (per-task gamma / beta are inner-loop BatchNorm parameters, "
-                "enable_inner_loop_optimizable_bn_params, which are outside the accelerated path)")
+                "a layer-norm bias batched under torch.func.vmap: the engine shares the layer-norm biases between the "
+                "tasks of a call (they are outer parameters, the same for every task)")
+        raise NotImplementedError(
+            "a BatchNorm gamma / beta batched under torch.func.vmap: the engine shares gamma / beta between the tasks "
+            "of a call (per-task gamma / beta are inner-loop BatchNorm parameters, "
+            "enable_inner_loop_optimizable_bn_params, which are outside the accelerated path)")
 
 
 def _refuse_functorch_jvp(ctx, *tensors):
@@ -356,6 +399,7 @@ class _OperatorHandles:
         a = net.args
         self.B = int(tasks)
         self.n, self.N, self.device = int(x.shape[-4]), net.num_output_classes, x.device
+        self.layer_norm = net._layer_norm()
         self.cfg = dict(n_way=self.N, channels=int(x.shape[-3]), height=int(x.shape[-2]), width=int(x.shape[-1]),
                         filters=net.cnn_filters, num_stages=net.num_stages, inner_steps=int(a.number_of_training_steps_per_iter),
                         per_step_bn=bool(a.per_step_bn_statistics), max_tasks=self.B)
@@ -372,7 +416,7 @@ class _OperatorHandles:
     def _engine(self, **shape):
         from . import _native
         with torch.cuda.device(self.device):
-            return _native.Engine(**shape, **self.cfg)
+            return _native.Engine(**shape, **self.cfg, layer_norm=self.layer_norm)
 
     def _second(self):
         if self.second_order is None:
@@ -396,11 +440,11 @@ class _OperatorHandles:
 
     def forward(self, net, spec, x, num_step, tensors):
         """The logits (``net_forward_tasks``), and F.batch_norm's EMA of net's running statistics at num_step from the B
-        batches in task order (per-step BatchNorm only)."""
+        batches in task order (per-step BatchNorm only; the layer norm has no running statistics)."""
         eng = self.first_order
         with torch.cuda.device(self.device):
             self._run_forward(spec, x, num_step, tensors)
-            if net.args.per_step_bn_statistics:
+            if net.args.per_step_bn_statistics and not self.layer_norm:
                 bns = [net.layer_dict["conv%d" % l].norm_layer for l in range(net.num_stages)]
                 with torch.no_grad():
                     for l, bn in enumerate(bns):
@@ -488,8 +532,9 @@ class _FunctionalForward(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dlogits):
         x, tensors = ctx.saved_tensors[0], ctx.saved_tensors[1:]
-        for i, t in enumerate(tensors[:4 * ctx.net.num_stages]):
-            if i % 4 >= 2 and fwAD.unpack_dual(t).tangent is not None:
+        norm, directions = ctx.net._norm_segments()
+        for i in () if directions else norm:
+            if fwAD.unpack_dual(tensors[i]).tangent is not None:
                 raise NotImplementedError(
                     "differentiating the gradient in forward mode along a BatchNorm gamma / beta tangent needs gamma / beta "
                     "tangent directions in the backward tangent pass, which the engine does not implement (BatchNorm "
@@ -504,7 +549,7 @@ class _FunctionalForward(torch.autograd.Function):
     def jvp(ctx, _net_t, _spec_t, x_t, _step_t, *tangents):
         """Forward mode (``torch.autograd.forward_ad``): the logits tangent J_theta t + J_x x_t through
         ``maml_b200_net_jvp`` on the second-order handle -- one primal forward and one tangent forward.  Tangents may sit
-        on the images, the conv / linear weights and the BatchNorm gamma / beta."""
+        on the images, the conv / linear weights and the BatchNorm gamma / beta or layer-norm biases."""
         _refuse_functorch_jvp(ctx, x_t, *tangents)
         x = ctx.saved_tensors[0]
         return ctx.net._handles(x).jvp(ctx.num_step, x, x_t, ctx.saved_tensors[1:], tangents)
@@ -513,7 +558,7 @@ class _FunctionalForward(torch.autograd.Function):
     def vmap(info, in_dims, net, spec, x, num_step, *tensors):
         _refuse_nested(spec)
         dims = in_dims[4:]
-        _refuse_batched_bn(net, dims)
+        _refuse_batched_norm(net, dims)
         spec = _Tasks(info.batch_size, in_dims[2] is not None, [d is not None for d in dims])
         logits = _FunctionalForward.apply(net, spec, _to_front(x, in_dims[2]), num_step,
                                           *[_to_front(t, d) for t, d in zip(tensors, dims)])
@@ -526,9 +571,11 @@ class _FunctionalBackward(torch.autograd.Function):
     few_shot_learning_system.py:138-139 and the outer ``loss.backward()``).
 
     forward  = ``maml_b200_net_backward_tasks``: B(dl, theta) = J^T dl for every tensor (conv / linear, BatchNorm gamma /
-               beta of ``num_step``), and -- only when x requires grad -- ``maml_b200_net_input_grad``: J_x^T dl (else
+               beta of ``num_step`` or the layer-norm biases), and -- only when x requires grad -- ``maml_b200_net_input_grad``: J_x^T dl (else
                None).  With grad mode off this is the whole first-order backward.
-    backward = ``_FunctionalHvp`` along the cotangents v of the conv / linear gradients.  Third order is not supported.
+    backward = ``_FunctionalHvp`` along the cotangents v of the conv / linear gradients (and of the layer-norm bias
+               gradients: bias directions, which the engine's tangent forward adds after the normalisation).  Third order
+               is not supported.
     A cotangent on a BatchNorm gamma / beta GRADIENT would need gamma / beta tangent directions, and one on the image
     gradient dx would need image tangent directions (the first conv's tangent driven by x-dot); the engine's tangent pass
     has neither: both are refused (the first only arises when BatchNorm parameters are inner-loop fast weights,
@@ -557,7 +604,8 @@ class _FunctionalBackward(torch.autograd.Function):
         weight gradient J_theta^T dl_t + d/dtheta <dl, J_theta t + J_x x_t>; for dx the same with d/dx.  The first term is
         ``maml_b200_net_backward_tasks`` (+ ``net_input_grad``) of dl_t on the first-order handle, the second
         ``maml_b200_net_hvp_image_tasks`` (+ ``net_hvp_input_grad``) on the second-order handle; a term whose tangents are
-        all None is skipped.  A tangent on a BatchNorm gamma / beta input never gets here: ``_FunctionalForward.backward``
+        all None is skipped.  A layer-norm bias tangent is a bias direction of that pass.  A tangent on a BatchNorm
+        gamma / beta input never gets here: ``_FunctionalForward.backward``
         refuses it before this node runs."""
         _refuse_functorch_jvp(ctx, x_t, dl_t, *tangents)
         fwd_ctx = ctx.fwd_ctx
@@ -580,8 +628,9 @@ class _FunctionalBackward(torch.autograd.Function):
             raise NotImplementedError(
                 "differentiating through the gradient with respect to the images needs image tangent directions, which "
                 "the engine's tangent pass does not implement")
-        for i, c in enumerate(cotangents[:4 * fwd_ctx.net.num_stages]):
-            if c is not None and i % 4 >= 2:
+        norm, directions = fwd_ctx.net._norm_segments()
+        for i in () if directions else norm:
+            if cotangents[i] is not None:
                 raise NotImplementedError(
                     "differentiating through the gradient of a BatchNorm gamma / beta needs gamma / beta tangent "
                     "directions, which the engine does not implement (BatchNorm parameters as inner-loop fast weights, "
@@ -601,7 +650,7 @@ class _FunctionalBackward(torch.autograd.Function):
     def vmap(info, in_dims, fwd_ctx, spec, x, dlogits, *tensors):
         _refuse_nested(spec)
         dims = in_dims[4:]
-        _refuse_batched_bn(fwd_ctx.net, dims)
+        _refuse_batched_norm(fwd_ctx.net, dims)
         B = info.batch_size
         spec = _Tasks(B, in_dims[2] is not None, [d is not None for d in dims])
         out = _FunctionalBackward.apply(fwd_ctx, spec, _to_front(x, in_dims[2]),
@@ -611,7 +660,7 @@ class _FunctionalBackward(torch.autograd.Function):
 
 
 class _FunctionalHvp(torch.autograd.Function):
-    """Backward of ``_FunctionalBackward``: along the cotangents v of the conv / linear gradients,
+    """Backward of ``_FunctionalBackward``: along the cotangents v of the conv / linear (and layer-norm bias) gradients,
     ``maml_b200_net_hvp_image_tasks`` -- one forward-over-reverse pass with dl held constant -- gives J v (the cotangent of
     dl) and d/dtheta <dl, J v> (that of every tensor); ``maml_b200_net_hvp_input_grad`` on the same handle gives
     d/dx <dl, J v> (that of x) when ``needs.x``.  torch carries J v on through the loss's own double backward.  A node of its
@@ -638,7 +687,7 @@ class _FunctionalHvp(torch.autograd.Function):
         _refuse_nested(spec)
         k = len(tensors_and_directions) // 2
         dims = in_dims[5:]
-        _refuse_batched_bn(fwd_ctx.net, dims[:k])
+        _refuse_batched_norm(fwd_ctx.net, dims[:k])
         B = info.batch_size
         spec = _Tasks(B, in_dims[3] is not None, [d is not None for d in dims[:k]], [d is not None for d in dims[k:]])
         out = _FunctionalHvp.apply(fwd_ctx, spec, needs, _to_front(x, in_dims[3]),

@@ -49,8 +49,9 @@ typedef struct maml_b200_config {
                            bit 1: run blocks l >= 1 on the fp32 FFMA kernels instead of wgmma 3xTF32 */
   int32_t norm_layer;   /* 0: batch norm; 1: layer norm (reference MetaLayerNormLayer: statistics per image over
                            [F, h, w], frozen all-ones weight, learnable bias [F, h, w]; per_step_bn is then ignored,
-                           there are no running statistics).  Layer-norm handles run maml_b200_meta_batch_fwd_bwd and
-                           the parameter entries; the functional entries (maml_b200_net_*) refuse them. */
+                           there are no running statistics).  Layer-norm handles run every entry; the layer norm has
+                           no per-step rows, so the functional entries (maml_b200_net_*) compute the same at every
+                           num_step, and maml_b200_net_running_update is a no-op. */
 } maml_b200_config;
 
 /* Per-call schedule: what reference forward(...) derives from epoch / phase (:232-244,:304-305). */
@@ -112,7 +113,7 @@ int maml_b200_meta_batch_fwd_bwd(maml_b200_handle* h, const maml_b200_iter_args*
 
 /* Stand-alone functional forward: replaces reference VGGReLUNormNetwork.forward(x, num_step, params)
  * (meta_neural_network_architectures.py:620-660) for batches of N*T images: conv / BatchNorm(batch statistics, gamma and
- * beta of `num_step`) / leaky-ReLU / maxpool x stages, flatten, linear.  `meta_like`: same layout as the meta vector,
+ * beta of `num_step`) or layer norm (per-image statistics, + bias) / leaky-ReLU / maxpool x stages, flatten, linear.  `meta_like`: same layout as the meta vector,
  * conv / linear entries = the (fast) weights to use.  x [n_tasks, N*T, C, H, W]; logits [n_tasks, N*T, N] (out). */
 int maml_b200_net_forward(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
                           const float* x, float* logits, void* stream);
@@ -124,7 +125,8 @@ int maml_b200_net_forward(maml_b200_handle* h, int32_t n_tasks, int32_t num_step
  * handle records its last functional call; meta_like it cannot check).
  *   dlogits  [n_tasks, N*T, N]   d(loss) / d(logits)
  *   grad_out [result_size]       (out) first meta_size floats = d(loss) / d(meta_like) in the meta layout (conv / linear
- *                                weights and biases, BatchNorm beta / gamma rows of num_step; LSLR entries 0), summed over
+ *                                weights and biases, BatchNorm beta / gamma rows of num_step or the layer-norm biases;
+ *                                LSLR entries 0), summed over
  *                                the n_tasks batches.  The gradient with respect to the images is a separate call,
  *                                maml_b200_net_input_grad. */
 int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
@@ -132,14 +134,14 @@ int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int32_t num_ste
 
 /* Second-order companion of maml_b200_net_backward: for the batch x, weights meta_like and upstream dlogits, one
  * forward-over-reverse pass along v_like (meta layout; its BatchNorm and LSLR entries are not read: there are no
- * gamma / beta tangent directions).  Self-contained: it recomputes the forward and the backward of dlogits itself, so it
+ * gamma / beta tangent directions; on a layer-norm handle its bias entries are bias directions).  Self-contained: it recomputes the forward and the backward of dlogits itself, so it
  * needs no earlier call.  The batch has the handle's SUPPORT shape: N*K images (create the handle with k_shot = batch / N).
  *   x          [n_tasks, N*K, C, H, W]
  *   dlogits    [n_tasks, N*K, N]  d(loss) / d(logits), held constant along v
  *   jv_out     [n_tasks, N*K, N]  = J(meta_like) v           (tangent of the logits)
  *   hv_out     result_size floats; first meta_size = d/d(meta_like) <dlogits, J v> in the meta layout
- *              (conv / linear weights and biases, BatchNorm gamma / beta of num_step; LSLR entries 0), summed over the
- *              n_tasks batches
+ *              (conv / linear weights and biases, BatchNorm gamma / beta of num_step or the layer-norm biases, +H v;
+ *              LSLR entries 0), summed over the n_tasks batches
  * No running-statistics side effect; it overwrites the batch statistics maml_b200_net_running_update reads. */
 int maml_b200_net_hvp(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
                       const float* dlogits, const float* v_like, float* jv_out, float* hv_out, void* stream);
@@ -156,8 +158,8 @@ int maml_b200_net_hvp_image(maml_b200_handle* h, int32_t n_tasks, int32_t num_st
 /* Forward mode of the functional operator: the logits tangent J_theta t + J_x xdot at the weights meta_like, for batches of
  * the handle's SUPPORT shape (N*K images).  Self-contained: one primal forward, then one tangent forward; no backward.
  *   x, xdot    [n_tasks, N*K, C, H, W]; xdot may be NULL (no image tangent)
- *   t_like     meta layout: conv / linear tangents and the BatchNorm beta / gamma tangents of num_step; LSLR entries
- *              are not read
+ *   t_like     meta layout: conv / linear tangents and the BatchNorm beta / gamma tangents of num_step (layer norm: the
+ *              bias tangents); LSLR entries are not read
  *   jv_out     [n_tasks, N*K, N]
  * No running-statistics side effect; it overwrites the batch statistics maml_b200_net_running_update reads.  Its small
  * buffers (zero d(logits), the image tangent) are allocated by the first call that needs them, outside the workspace. */
@@ -172,8 +174,9 @@ int maml_b200_net_jvp(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, co
  *   dir_stride   the same for v_like (0 = shared)
  *   sum_tasks    1: grad_out / hv_out = result_size floats summed over the tasks (the entries above);
  *                0: n_tasks x result_size floats, task t's vector (not summed) at + t * result_size
- * BatchNorm gamma / beta are shared by the tasks of a call: they are read from task 0's vector (meta_like's own rows),
- * whatever meta_stride is.  A stride that is neither 0 nor >= meta_size is an error.
+ * BatchNorm gamma / beta and the layer-norm biases are shared by the tasks of a call: they are read from task 0's vector
+ * (meta_like's own rows), whatever meta_stride is.  The layer-norm bias DIRECTIONS of net_hvp_image_tasks follow
+ * dir_stride (per task), and each task's bias gradient goes to its own result vector.  A stride that is neither 0 nor >= meta_size is an error.
  * maml_b200_net_input_grad, maml_b200_net_hvp_input_grad and maml_b200_net_running_update already work per task and follow
  * these entries as they follow the ones above. */
 int maml_b200_net_forward_tasks(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
@@ -199,7 +202,7 @@ int maml_b200_net_hvp_input_grad(maml_b200_handle* h, int32_t n_tasks, float* dx
  * maml_b200_net_backward it must follow that forward (or a maml_b200_net_backward of it) with the same n_tasks and
  * num_step, and otherwise fails with an error and launches nothing: another functional call in between, e.g.
  * maml_b200_net_hvp, overwrites those statistics.  running_mean / running_var: [stages][S][F] device.  No-op without
- * per-step BatchNorm. */
+ * per-step BatchNorm (shared BatchNorm, layer norm). */
 int maml_b200_net_running_update(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, float* running_mean,
                                  float* running_var, void* stream);
 

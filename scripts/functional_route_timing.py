@@ -14,9 +14,10 @@ meta-batch 8, second order) three ways, on one GPU:
 
 Warm-up first; every timed iteration ends in a device synchronise; the legs alternate within each repeat.  Prints
 one JSON line: per leg the median / min / max milliseconds per iteration, plus the GPU name and power limit read in
-the same run.
+the same run.  ``--norm-layer layer_norm`` runs the same config with the layer-norm network (its torch legs on
+oracle.ln_oracle._net_forward) and adds "norm_layer" to the line.
 
-  python scripts/functional_route_timing.py [--repeats 20] [--warmup 3]
+  python scripts/functional_route_timing.py [--repeats 20] [--warmup 3] [--norm-layer {batch_norm,layer_norm}]
 """
 import argparse
 import json
@@ -35,7 +36,7 @@ import torch.nn.functional as Fnn                    # noqa: E402
 CONFIG, META_BATCH = "omniglot_mamlpp_5w1s", 8
 
 
-def reference_loop(net_forward, params, a, batch, epoch, O):
+def reference_loop(net_forward, params, a, batch, epoch, O, names):
     """oracle.autograd_train_iter's loop with a pluggable network forward; returns the outer gradients."""
     S = int(a.number_of_training_steps_per_iter)
     second_order = bool(a.second_order) and epoch > a.first_order_to_second_order_epoch
@@ -58,11 +59,10 @@ def reference_loop(net_forward, params, a, batch, epoch, O):
                 task_losses.append(w_msl[s] * loss_t if sched[s] == "msl" else loss_t)
         total.append(torch.stack(task_losses).sum())
     loss = torch.stack(total).mean()
-    names = O.trainable_names(a)
     return torch.autograd.grad(loss, [params[n] for n in names], allow_unused=True)
 
 
-def functorch_loop(net_forward, params, a, batch, epoch, O):
+def functorch_loop(net_forward, params, a, batch, epoch, O, names):
     """The loop above written the torch.func way: vmap over the tasks, torch.func.grad for the inner steps (its result
     detached for first order), the outer gradient through torch.autograd."""
     S = int(a.number_of_training_steps_per_iter)
@@ -88,7 +88,6 @@ def functorch_loop(net_forward, params, a, batch, epoch, O):
     per_task = [t.reshape(B, -1, *t.shape[-3:]) for t in (xs, xt)] + [t.reshape(B, -1) for t in (ys, yt)]
     loss = torch.func.vmap(task, in_dims=(None, 0, 0, 0, 0))({n: params[n] for n in inner}, per_task[0], per_task[2],
                                                              per_task[1], per_task[3]).mean()
-    names = O.trainable_names(a)
     return torch.autograd.grad(loss, [params[n] for n in names], allow_unused=True)
 
 
@@ -103,15 +102,19 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--repeats", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--norm-layer", default="batch_norm", choices=["batch_norm", "layer_norm"])
     cli = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("functional_route_timing.py needs a CUDA device")
     from howtotrainyourmamlpytorch_b200 import MAMLFewShotClassifier, make_args, synthetic_batch
+    from oracle import ln_oracle as LN
     from oracle import maml_oracle as O
+    layer_norm = cli.norm_layer == "layer_norm"
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
     dev = torch.device("cuda", 0)
-    a = make_args(CONFIG, batch_size=META_BATCH)
+    a = make_args(CONFIG, batch_size=META_BATCH, **({"norm_layer": "layer_norm"} if layer_norm else {}))
+    names = LN.trainable_names(a) if layer_norm else O.trainable_names(a)
     epoch = 0
     batch = synthetic_batch(a, iteration=0)
     dbatch = tuple(t.to(dev) for t in batch)
@@ -120,7 +123,7 @@ def main():
     m_fused = MAMLFewShotClassifier(im_shape=(2, a.image_channels, a.image_height, a.image_width), device=dev, args=a)
     m_fused.load_state_dict(m_op.state_dict())
     op_params = dict(m_op.named_parameters())
-    t_params = {k: v.detach().clone().requires_grad_(v.requires_grad) for k, v in m_op.state_dict().items()}
+    t_params = {k: v.detach().clone().to(dev).requires_grad_(v.requires_grad) for k, v in m_op.state_dict().items()}
     t_params.update({k: v.detach().clone().requires_grad_(True) for k, v in op_params.items() if v.requires_grad})
     pre = len("classifier.")
 
@@ -128,14 +131,14 @@ def main():
         return m_op.classifier.forward(x, num_step=s, training=True, params={n[pre:]: w.unsqueeze(0) for n, w in fast.items()})
 
     def torch_forward(x, fast, s):
-        return O._net_forward(x, fast, t_params, a, s)
+        return LN._net_forward(x, fast, t_params, a) if layer_norm else O._net_forward(x, fast, t_params, a, s)
 
     legs = {
-        "operator": lambda: reference_loop(op_forward, op_params, a, dbatch, epoch, O),
-        "torch": lambda: reference_loop(torch_forward, t_params, a, dbatch, epoch, O),
+        "operator": lambda: reference_loop(op_forward, op_params, a, dbatch, epoch, O, names),
+        "torch": lambda: reference_loop(torch_forward, t_params, a, dbatch, epoch, O, names),
         "fused": lambda: m_fused.run_train_iter(batch, epoch),
-        "operator_vmap": lambda: functorch_loop(op_forward, op_params, a, dbatch, epoch, O),
-        "torch_vmap": lambda: functorch_loop(torch_forward, t_params, a, dbatch, epoch, O),
+        "operator_vmap": lambda: functorch_loop(op_forward, op_params, a, dbatch, epoch, O, names),
+        "torch_vmap": lambda: functorch_loop(torch_forward, t_params, a, dbatch, epoch, O, names),
     }
     skipped = {}
     try:
@@ -161,9 +164,12 @@ def main():
         v = sorted(v)
         return {"median_ms": round(v[len(v) // 2], 3), "min_ms": round(v[0], 3), "max_ms": round(v[-1], 3)}
 
-    print(json.dumps({"config": CONFIG, "meta_batch": META_BATCH, "second_order": True, "gpu": name,
-                      "power_limit": power, "repeats": cli.repeats, "warmup": cli.warmup,
-                      "legs": {k: summary(v) for k, v in times.items()}, "skipped": skipped}))
+    line = {"config": CONFIG, "meta_batch": META_BATCH, "second_order": True, "gpu": name,
+            "power_limit": power, "repeats": cli.repeats, "warmup": cli.warmup,
+            "legs": {k: summary(v) for k, v in times.items()}, "skipped": skipped}
+    if layer_norm:
+        line["norm_layer"] = "layer_norm"
+    print(json.dumps(line))
 
 
 if __name__ == "__main__":
