@@ -149,8 +149,9 @@ struct BnBwdTanArgs {             // backward reduce / apply (tangent)
 };
 
 // Layer norm (norm_layer "layer_norm"): statistics per IMAGE over its F*h*w conv outputs, y = zh + bias[c][y][x] (the
-// reference's frozen weight is all ones), then leaky-ReLU and max-pool as with BatchNorm.  One argument block for the LN
-// kernels; each reads the fields its comment names.  Per-image fp64 sums: [task][img][2] at `st_*` + task * st_stride.
+// reference's frozen weight is all ones), then leaky-ReLU and max-pool through the BatchNorm window bodies, with per-image
+// constants and beta = the bias at each position.  One argument block for the LN kernels; each reads the fields its
+// comment names.  Per-image fp64 sums: [task][img][2] at `st_*` + task * st_stride.
 struct LnArgs {
   float* z; long long z_stride;          // stats / act: z (act: -> zh in place); tangent: zdot (-> zhdot in place)
   const float* z2;                       // tangent: optional second addend of zdot (same stride)
@@ -165,7 +166,7 @@ struct LnArgs {
   const double* st_bwd;                  // (sum dy, sum dy * zh)
   double* st_out;                        // the sums a stats / reduce kernel accumulates
   long long st_stride;
-  const float* bias;                     // [F][h][w] layer-norm bias (act kernels)
+  const float* bias;                     // [F][h][w] layer-norm bias (every kernel but stats)
   const float* bdot; long long bdot_stride;   // tangent act: nullable bias tangent [F][h][w] per task (stride 0: shared)
   float* db; long long db_stride;        // bias gradient: [F][h][w] per task (stored, not accumulated)
   BnGeom g; int tasks;

@@ -781,18 +781,154 @@ static bool support_tail_fused(const maml_b200_handle* h) {
   return h->opt.tail_fuse && !h->ln && tail_fusable(bn_geom(h, h->L - 1, h->n_s), h->n_s, head_rows(h->n_s));
 }
 
-enum { CLR_STATS = 1, CLR_ABAR = 2, CLR_LOSSES = 4, CLR_CORRECT = 8 };
-// zeroes the accumulators in `what` (CLR_* bits) for all maxT tasks on `st`
-static int clear_accumulators(maml_b200_handle* h, unsigned what, cudaStream_t st) {
+enum { CLR_STATS = 1, CLR_ABAR = 2, CLR_LOSSES = 4, CLR_CORRECT = 8, CLR_BWD_STATS = 16 };
+// zeroes the accumulators in `what` (CLR_* bits) for all maxT tasks on `st`; CLR_BWD_STATS: only the backward sums (kinds
+// PASS_TGT_BWD / PASS_TAN_BWD) of the first bwd_tasks tasks.  Layer norm: both sums clear the bias-gradient rows too.
+static int clear_accumulators(maml_b200_handle* h, unsigned what, cudaStream_t st, int bwd_tasks = 0) {
   if (what & CLR_STATS) CK(cudaMemsetAsync(h->stats, 0, (size_t)h->stats_count * sizeof(double), st));
-  if ((what & CLR_STATS) && h->ln) {
-    CK(cudaMemsetAsync(h->ln_stats, 0, (size_t)h->ln_task_stride * h->maxT * sizeof(double), st));
-    CK(cudaMemsetAsync(h->lnb, 0, (size_t)h->maxT * 2 * h->S * h->pl.lnb_off[h->L] * sizeof(float), st));
+  if ((what & CLR_STATS) && h->ln) CK(cudaMemsetAsync(h->ln_stats, 0, (size_t)h->ln_task_stride * h->maxT * sizeof(double), st));
+  if (what & CLR_BWD_STATS)
+    for (int kind : {PASS_TGT_BWD, PASS_TAN_BWD}) {
+      CK(cudaMemset2DAsync(h->stats + (long long)kind * MAML_MAX_STEPS * h->st_pass_stride, (size_t)h->stats_task_stride * sizeof(double),
+                           0, (size_t)MAML_MAX_STEPS * h->st_pass_stride * sizeof(double), (size_t)bwd_tasks, st));
+      if (h->ln)
+        CK(cudaMemset2DAsync(h->ln_stats + (long long)kind * h->ln_pass_stride, (size_t)h->ln_task_stride * sizeof(double), 0,
+                             (size_t)h->ln_pass_stride * sizeof(double), (size_t)bwd_tasks, st));
+    }
+  if ((what & (CLR_STATS | CLR_BWD_STATS)) && h->ln) {
+    const int tasks = (what & CLR_STATS) ? h->maxT : bwd_tasks;
+    CK(cudaMemsetAsync(h->lnb, 0, (size_t)tasks * 2 * h->S * h->pl.lnb_off[h->L] * sizeof(float), st));
   }
   if (what & CLR_ABAR) CK(cudaMemsetAsync(h->abar, 0, (size_t)h->maxT * h->pl.nseg_inner * MAML_MAX_STEPS * sizeof(double), st));
   if (what & CLR_LOSSES) CK(cudaMemsetAsync(h->losses, 0, (size_t)h->maxT * MAML_MAX_STEPS * sizeof(float), st));
   if (what & CLR_CORRECT) CK(cudaMemsetAsync(h->correct, 0, (size_t)h->maxT * sizeof(float), st));
   return 0;
+}
+
+// The normalisation (+ leaky-ReLU + max-pool) of block l in each kind of pass, BatchNorm or layer norm.  defer_last: the
+// last block's BatchNorm is not launched but returned; fused_head: it runs in the fused last-block kernel.
+static void norm_forward(maml_b200_handle* h, const PassSet& ps, int slot, const float* meta, int l, int step, int stat_kind,
+                         int T, cudaStream_t st, BnActArgs* defer_last) {
+  if (h->ln) {                   // per-image sums of z, then normalise / bias / leaky-ReLU / pool
+    LnArgs a = ln_args(h, l, ps.n, meta, T);
+    a.z = ZH(ps, l, slot); a.z_stride = STRIDE(ps, zh, l);
+    a.st_fwd = a.st_out = ln_stat_at(h, stat_kind, step, l);
+    launch_ln_stats(a, false, st);
+    a.out = AIN(ps, l + 1, slot); a.out_stride = STRIDE(ps, ain, l + 1);
+    if (h->use_tc && l + 1 < h->L) { a.out_hi = AIN_HI(ps, l + 1, slot); a.out_lo = AIN_LO(ps, l + 1, slot); }
+    launch_ln_act(a, false, st);
+    return;
+  }
+  BnActArgs b{};
+  b.z = ZH(ps, l, slot); b.z_stride = STRIDE(ps, zh, l);
+  b.stats = stat_at(h, stat_kind, step, l); b.stats_stride = h->stats_task_stride;
+  b.gamma = gamma_at(h, meta, l, step); b.beta = beta_at(h, meta, l, step);
+  b.p = AIN(ps, l + 1, slot); b.p_stride = STRIDE(ps, ain, l + 1);
+  if (h->use_tc && l + 1 < h->L) { b.p_hi = AIN_HI(ps, l + 1, slot); b.p_lo = AIN_LO(ps, l + 1, slot); }
+  b.g = bn_geom(h, l, ps.n); b.tasks = T;
+  if (defer_last && l == h->L - 1) *defer_last = b;
+  else launch_bnact(b, st);
+}
+
+static void norm_backward(maml_b200_handle* h, const PassSet& ps, int slot, const float* meta, int l, int step, int kind_fwd,
+                          int kind_bwd, int T, cudaStream_t st, const BnActArgs* fused_act, const HeadArgs* fused_head) {
+  if (h->ln) {
+    LnArgs a = ln_args(h, l, ps.n, meta, T);
+    a.dp = DP(ps, l, slot); a.dp_stride = STRIDE(ps, dp, l);
+    a.zh = ZH(ps, l, slot); a.zh_stride = STRIDE(ps, zh, l);
+    a.st_fwd = ln_stat_at(h, kind_fwd, step, l); a.st_out = ln_stat_at(h, kind_bwd, step, l);
+    a.out = DZ(ps, l, slot); a.out_stride = STRIDE(ps, dz, l);
+    if (h->use_tc && l >= 1) { a.out_hi = DZ_HI(ps, l, slot); a.out_lo = DZ_LO(ps, l, slot); }
+    launch_ln_bwd(a, false, st);
+    if (kind_bwd == PASS_TGT_BWD) {    // the bias is an outer parameter only: its gradient comes from the target loss
+      a.db = lnb_at(h, 0, step) + h->pl.lnb_off[l]; a.db_stride = 2LL * h->S * h->pl.lnb_off[h->L];
+      launch_ln_bias_grad(a, false, st);
+    }
+    return;
+  }
+  BnBwdArgs b{};
+  b.dp = DP(ps, l, slot); b.dp_stride = STRIDE(ps, dp, l);
+  b.zh = ZH(ps, l, slot); b.zh_stride = STRIDE(ps, zh, l);
+  b.stats_fwd = stat_at(h, kind_fwd, step, l); b.stats_fwd_stride = h->stats_task_stride;
+  b.stats_bwd = stat_at(h, kind_bwd, step, l); b.stats_bwd_stride = h->stats_task_stride;
+  b.gamma = gamma_at(h, meta, l, step); b.beta = beta_at(h, meta, l, step);
+  b.dz = DZ(ps, l, slot); b.dz_stride = STRIDE(ps, dz, l);
+  if (h->use_tc && l >= 1) { b.dz_hi = DZ_HI(ps, l, slot); b.dz_lo = DZ_LO(ps, l, slot); }
+  b.g = bn_geom(h, l, ps.n); b.tasks = T;
+  if (fused_head && l == h->L - 1) launch_tail_fused(*fused_act, *fused_head, b, st);
+  else launch_bnbwd(b, st);
+}
+
+static void norm_tangent_forward(maml_b200_handle* h, int s, const float* meta, int l, const float* t_norm, long long t_stride,
+                                 int T, cudaStream_t st, BnActTanArgs* defer_last) {
+  const PassSet& sp = h->sup; const PassSet& tn = h->tan; const PassSet& t2 = h->tan2;
+  if (h->ln) {                   // zdot (+ the side stream's addend) -> per-image sums -> zhdot, pdot
+    LnArgs a = ln_args(h, l, sp.n, meta, T);
+    a.z = ZH(tn, l, 0); a.z_stride = STRIDE(tn, zh, l);
+    if (h->use_tc && l >= 1) a.z2 = ZH(t2, l, 0);
+    a.zh = ZH(sp, l, s); a.zh_stride = STRIDE(sp, zh, l);
+    a.st_fwd = ln_stat_at(h, PASS_SUP_FWD, s, l); a.st_tan = a.st_out = ln_stat_at(h, PASS_TAN_FWD, s, l);
+    launch_ln_stats(a, true, st);
+    a.out = AIN(tn, l + 1, 0); a.out_stride = STRIDE(tn, ain, l + 1);
+    if (h->use_tc && l + 1 < h->L) { a.out_hi = AIN_HI(tn, l + 1, 0); a.out_lo = AIN_LO(tn, l + 1, 0); }
+    if (t_norm) { a.bdot = t_norm + h->pl.m_lnb[l]; a.bdot_stride = t_stride; }
+    launch_ln_act(a, true, st);
+    return;
+  }
+  BnActTanArgs b{};
+  b.zdot = ZH(tn, l, 0); b.zdot_stride = STRIDE(tn, zh, l);
+  if (h->use_tc && l >= 1) b.zdot2 = ZH(t2, l, 0);
+  b.zh = ZH(sp, l, s); b.zh_stride = STRIDE(sp, zh, l);
+  b.stats_fwd = stat_at(h, PASS_SUP_FWD, s, l); b.stats_fwd_stride = h->stats_task_stride;
+  b.stats_tan = stat_at(h, PASS_TAN_FWD, s, l); b.stats_tan_stride = h->stats_task_stride;
+  b.gamma = gamma_at(h, meta, l, s); b.beta = beta_at(h, meta, l, s);
+  b.pdot = AIN(tn, l + 1, 0); b.pdot_stride = STRIDE(tn, ain, l + 1);
+  if (h->use_tc && l + 1 < h->L) { b.pdot_hi = AIN_HI(tn, l + 1, 0); b.pdot_lo = AIN_LO(tn, l + 1, 0); }
+  b.g = bn_geom(h, l, sp.n); b.tasks = T;
+  if (defer_last && l == h->L - 1) *defer_last = b;
+  else launch_bnact_tan(b, st, t_norm ? gamma_at(h, t_norm, l, s) : nullptr, t_norm ? beta_at(h, t_norm, l, s) : nullptr);
+}
+
+static void norm_tangent_backward(maml_b200_handle* h, int s, const float* meta, int l, int kind_tbwd, int T, cudaStream_t st,
+                                  const BnActTanArgs* fused_act, const HeadArgs* fused_head) {
+  const PassSet& sp = h->sup; const PassSet& tn = h->tan; const PassSet& t2 = h->tan2;
+  if (h->ln) {
+    LnArgs a = ln_args(h, l, sp.n, meta, T);
+    a.dp = DP(sp, l, s); a.dp_stride = STRIDE(sp, dp, l);
+    a.dpd = DP(tn, l, 0); a.dpd_stride = STRIDE(tn, dp, l);
+    if (h->use_tc && l + 1 < h->L) a.dpd2 = DP(t2, l, 0);
+    a.zh = ZH(sp, l, s); a.zh_stride = STRIDE(sp, zh, l);
+    a.zhd = ZH(tn, l, 0); a.zhd_stride = STRIDE(tn, zh, l);
+    a.dz = DZ(sp, l, s); a.dz_stride = STRIDE(sp, dz, l);
+    a.st_fwd = ln_stat_at(h, PASS_SUP_FWD, s, l); a.st_bwd = ln_stat_at(h, PASS_SUP_BWD, s, l);
+    a.st_tan = ln_stat_at(h, PASS_TAN_FWD, s, l); a.st_out = ln_stat_at(h, kind_tbwd, s, l);
+    a.out = DZ(tn, l, 0); a.out_stride = STRIDE(tn, dz, l);
+    if (h->use_tc && l >= 1) { a.out_hi = DZ_HI(tn, l, 0); a.out_lo = DZ_LO(tn, l, 0); }
+    launch_ln_bwd(a, true, st);
+    // H_b u, the tangent of the support loss's bias gradient: export subtracts kind 1 (fused iteration, b-bar -= H_b u)
+    // and adds kind 0 (functional operator, +H_b v), as it does with the BatchNorm gamma / beta sums of kind_tbwd
+    a.db = lnb_at(h, kind_tbwd == PASS_TGT_BWD ? 0 : 1, s) + h->pl.lnb_off[l];
+    a.db_stride = 2LL * h->S * h->pl.lnb_off[h->L];
+    launch_ln_bias_grad(a, true, st);
+    return;
+  }
+  BnBwdTanArgs b{};
+  b.dp = DP(sp, l, s); b.dp_stride = STRIDE(sp, dp, l);
+  b.dpdot = DP(tn, l, 0); b.dpdot_stride = STRIDE(tn, dp, l);
+  if (h->use_tc && l + 1 < h->L) b.dpdot2 = DP(t2, l, 0);
+  b.zh = ZH(sp, l, s); b.zh_stride = STRIDE(sp, zh, l);
+  b.zhdot = ZH(tn, l, 0); b.zhdot_stride = STRIDE(tn, zh, l);
+  b.dz = DZ(sp, l, s); b.dz_stride = STRIDE(sp, dz, l);
+  b.stats_fwd = stat_at(h, PASS_SUP_FWD, s, l); b.stats_fwd_stride = h->stats_task_stride;
+  b.stats_bwd = stat_at(h, PASS_SUP_BWD, s, l); b.stats_bwd_stride = h->stats_task_stride;
+  b.stats_tan = stat_at(h, PASS_TAN_FWD, s, l); b.stats_tan_stride = h->stats_task_stride;
+  b.stats_tbwd = stat_at(h, kind_tbwd, s, l); b.stats_tbwd_stride = h->stats_task_stride;
+  b.gamma = gamma_at(h, meta, l, s); b.beta = beta_at(h, meta, l, s);
+  b.dzdot = DZ(tn, l, 0); b.dzdot_stride = STRIDE(tn, dz, l);
+  if (h->use_tc && l >= 1) { b.dzdot_hi = DZ_HI(tn, l, 0); b.dzdot_lo = DZ_LO(tn, l, 0); }
+  b.g = bn_geom(h, l, sp.n); b.tasks = T;
+  if (fused_head && l == h->L - 1) launch_tail_tan_fused(*fused_act, *fused_head, b, st);
+  else launch_bnbwd_tan(b, st);
 }
 
 // primal forward of one pass: conv -> stats -> BN/leaky/pool for every block
@@ -815,25 +951,7 @@ static void forward_pass(maml_b200_handle* h, const PassSet& ps, int slot, const
       a.stats = stat_at(h, stat_kind, bn_step, l);
       launch_conv_rows(a, st);
     }
-    if (h->ln) {                   // per-image sums of z, then normalise / bias / leaky-ReLU / pool
-      LnArgs a = ln_args(h, l, ps.n, meta, T);
-      a.z = ZH(ps, l, slot); a.z_stride = STRIDE(ps, zh, l);
-      a.st_fwd = a.st_out = ln_stat_at(h, stat_kind, bn_step, l);
-      launch_ln_stats(a, false, st);
-      a.out = AIN(ps, l + 1, slot); a.out_stride = STRIDE(ps, ain, l + 1);
-      if (h->use_tc && l + 1 < h->L) { a.out_hi = AIN_HI(ps, l + 1, slot); a.out_lo = AIN_LO(ps, l + 1, slot); }
-      launch_ln_act(a, false, st);
-      continue;
-    }
-    BnActArgs b{};
-    b.z = ZH(ps, l, slot); b.z_stride = STRIDE(ps, zh, l);
-    b.stats = stat_at(h, stat_kind, bn_step, l); b.stats_stride = h->stats_task_stride;
-    b.gamma = gamma_at(h, meta, l, bn_step); b.beta = beta_at(h, meta, l, bn_step);
-    b.p = AIN(ps, l + 1, slot); b.p_stride = STRIDE(ps, ain, l + 1);
-    if (h->use_tc && l + 1 < h->L) { b.p_hi = AIN_HI(ps, l + 1, slot); b.p_lo = AIN_LO(ps, l + 1, slot); }
-    b.g = bn_geom(h, l, ps.n); b.tasks = T;
-    if (defer_last && l == h->L - 1) *defer_last = b;      // launched by the fused last-block kernel
-    else launch_bnact(b, st);
+    norm_forward(h, ps, slot, meta, l, bn_step, stat_kind, T, st, defer_last);
   }
 }
 
@@ -848,31 +966,7 @@ static void backward_pass(maml_b200_handle* h, const PassSet& ps, int slot, cons
   cudaStream_t wst = fork_wgrad ? h->s_wg : st;
   const bool split = fork_wgrad && rs != nullptr;
   for (int l = h->L - 1; l >= 0; --l) {
-    if (h->ln) {
-      LnArgs a = ln_args(h, l, ps.n, meta, T);
-      a.dp = DP(ps, l, slot); a.dp_stride = STRIDE(ps, dp, l);
-      a.zh = ZH(ps, l, slot); a.zh_stride = STRIDE(ps, zh, l);
-      a.st_fwd = ln_stat_at(h, kind_fwd, bn_step, l); a.st_out = ln_stat_at(h, kind_bwd, bn_step, l);
-      a.out = DZ(ps, l, slot); a.out_stride = STRIDE(ps, dz, l);
-      if (h->use_tc && l >= 1) { a.out_hi = DZ_HI(ps, l, slot); a.out_lo = DZ_LO(ps, l, slot); }
-      launch_ln_bwd(a, false, st);
-      if (kind_bwd == PASS_TGT_BWD) {    // the bias is an outer parameter only: its gradient comes from the target loss
-        a.db = lnb_at(h, 0, bn_step) + h->pl.lnb_off[l]; a.db_stride = 2LL * h->S * h->pl.lnb_off[h->L];
-        launch_ln_bias_grad(a, false, st);
-      }
-    } else {
-    BnBwdArgs b{};
-    b.dp = DP(ps, l, slot); b.dp_stride = STRIDE(ps, dp, l);
-    b.zh = ZH(ps, l, slot); b.zh_stride = STRIDE(ps, zh, l);
-    b.stats_fwd = stat_at(h, kind_fwd, bn_step, l); b.stats_fwd_stride = h->stats_task_stride;
-    b.stats_bwd = stat_at(h, kind_bwd, bn_step, l); b.stats_bwd_stride = h->stats_task_stride;
-    b.gamma = gamma_at(h, meta, l, bn_step); b.beta = beta_at(h, meta, l, bn_step);
-    b.dz = DZ(ps, l, slot); b.dz_stride = STRIDE(ps, dz, l);
-    if (h->use_tc && l >= 1) { b.dz_hi = DZ_HI(ps, l, slot); b.dz_lo = DZ_LO(ps, l, slot); }
-    b.g = bn_geom(h, l, ps.n); b.tasks = T;
-    if (fused_head && l == h->L - 1) launch_tail_fused(*fused_act, *fused_head, b, st);
-    else launch_bnbwd(b, st);
-    }
+    norm_backward(h, ps, slot, meta, l, bn_step, kind_fwd, kind_bwd, T, st, fused_act, fused_head);
     if (fork_wgrad) { cudaEventRecord(h->ev_fork, st); cudaStreamWaitEvent(h->s_wg, h->ev_fork, 0); }
 
     if (l == 0) {
@@ -934,13 +1028,13 @@ static HeadArgs tangent_head_args(const maml_b200_handle* h, int s, const float*
 
 // Forward half of the tangent pass at support slot s: the tangent of the support forward in direction u (weights), plus
 // the image tangent xdot_g (padded grid, nullable: W_0 applied to it joins block 0's tangent conv as a second operand
-// pair) and the norm tangents read from the meta-layout vector t_bn (nullable): BatchNorm gamma / beta of step s (shared by
-// the tasks), or the layer-norm biases (t_stride floats between tasks, 0: shared).  Leaves the normalised tangents in
+// pair) and the norm parameters' tangents read from the meta-layout vector t_norm (nullable): BatchNorm gamma / beta of step
+// s (shared by the tasks), or the layer-norm biases (t_stride floats between tasks, 0: shared).  Leaves the normalised tangents in
 // tan.zh and the pooled ones in tan.ain; the features' tangent is tan.ain[L].
 // pre_dgrad: also enqueue the u-weight dgrad convs of the backward half on spre, right behind the forward ones.
 // defer_last: the last block's BatchNorm tangent is not launched but returned (the fused last-block kernel runs it).
 static void tangent_forward(maml_b200_handle* h, int s, const float* theta, const float* u, const float* meta,
-                            const float* xdot_g, const float* t_bn, long long t_stride, int T, cudaStream_t st,
+                            const float* xdot_g, const float* t_norm, long long t_stride, int T, cudaStream_t st,
                             cudaStream_t spre, bool pre_dgrad, BnActTanArgs* defer_last) {
   const PassSet& sp = h->sup; const PassSet& tn = h->tan; const PassSet& t2 = h->tan2;
   // Tangent convs of blocks >= 1 have two operand pairs; the pair (primal activation, u weights) depends only on u and
@@ -982,45 +1076,21 @@ static void tangent_forward(maml_b200_handle* h, int s, const float* theta, cons
       a.stats = stat_at(h, PASS_TAN_FWD, s, l);
       launch_conv_rows(a, st);
     }
-    if (h->ln) {                   // zdot (+ the side stream's addend) -> per-image sums -> zhdot, pdot
-      LnArgs a = ln_args(h, l, sp.n, meta, T);
-      a.z = ZH(tn, l, 0); a.z_stride = STRIDE(tn, zh, l);
-      if (h->use_tc && l >= 1) a.z2 = ZH(t2, l, 0);
-      a.zh = ZH(sp, l, s); a.zh_stride = STRIDE(sp, zh, l);
-      a.st_fwd = ln_stat_at(h, PASS_SUP_FWD, s, l); a.st_tan = a.st_out = ln_stat_at(h, PASS_TAN_FWD, s, l);
-      launch_ln_stats(a, true, st);
-      a.out = AIN(tn, l + 1, 0); a.out_stride = STRIDE(tn, ain, l + 1);
-      if (h->use_tc && l + 1 < h->L) { a.out_hi = AIN_HI(tn, l + 1, 0); a.out_lo = AIN_LO(tn, l + 1, 0); }
-      if (t_bn) { a.bdot = t_bn + h->pl.m_lnb[l]; a.bdot_stride = t_stride; }
-      launch_ln_act(a, true, st);
-      continue;
-    }
-    BnActTanArgs b{};
-    b.zdot = ZH(tn, l, 0); b.zdot_stride = STRIDE(tn, zh, l);
-    if (h->use_tc && l >= 1) b.zdot2 = ZH(t2, l, 0);
-    b.zh = ZH(sp, l, s); b.zh_stride = STRIDE(sp, zh, l);
-    b.stats_fwd = stat_at(h, PASS_SUP_FWD, s, l); b.stats_fwd_stride = h->stats_task_stride;
-    b.stats_tan = stat_at(h, PASS_TAN_FWD, s, l); b.stats_tan_stride = h->stats_task_stride;
-    b.gamma = gamma_at(h, meta, l, s); b.beta = beta_at(h, meta, l, s);
-    b.pdot = AIN(tn, l + 1, 0); b.pdot_stride = STRIDE(tn, ain, l + 1);
-    if (h->use_tc && l + 1 < h->L) { b.pdot_hi = AIN_HI(tn, l + 1, 0); b.pdot_lo = AIN_LO(tn, l + 1, 0); }
-    b.g = bn_geom(h, l, sp.n); b.tasks = T;
-    if (defer_last && l == h->L - 1) *defer_last = b;
-    else launch_bnact_tan(b, st, t_bn ? gamma_at(h, t_bn, l, s) : nullptr, t_bn ? beta_at(h, t_bn, l, s) : nullptr);
+    norm_tangent_forward(h, s, meta, l, t_norm, t_stride, T, st, defer_last);
   }
 }
 
 // forward-mode tangent of (support forward + support backward) at step s in direction u (and, with xdot_g, in the
-// images' direction x-dot: pass the padded grid of x-dot; with t_ln, a layer-norm handle's bias directions in the meta
-// layout, t_ln_stride floats between tasks)  =>  H u into `partial`
+// images' direction x-dot: pass the padded grid of x-dot; with t_norm, along the norm parameters' tangents, as in
+// tangent_forward)  =>  H u into `partial`
 static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const float* u, const float* meta,
                          const TangentHead& th, int T, cudaStream_t st, const ReduceSpec& rs, cudaStream_t spre,
-                         const float* xdot_g = nullptr, const float* t_ln = nullptr, long long t_ln_stride = 0) {
-  const PassSet& sp = h->sup; const PassSet& tn = h->tan; const PassSet& t2 = h->tan2;
+                         const float* xdot_g = nullptr, const float* t_norm = nullptr, long long t_stride = 0) {
+  const PassSet& sp = h->sup; const PassSet& tn = h->tan;
   // the fused last-block kernels implement the cross-entropy tangent head only
   const bool fuse_tail = th.mode == HEAD_TANGENT && support_tail_fused(h);
   BnActTanArgs last_act{};
-  tangent_forward(h, s, theta, u, meta, xdot_g, h->ln ? t_ln : nullptr, t_ln_stride, T, st, spre, true,
+  tangent_forward(h, s, theta, u, meta, xdot_g, t_norm, t_stride, T, st, spre, true,
                   fuse_tail ? &last_act : nullptr);
   const ChunkPlan& cp = h->plan_sup;
   join_pending(h, st);
@@ -1028,43 +1098,7 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
   if (!fuse_tail) launch_head(hd, st);
   for (int l = h->L - 1; l >= 0; --l) {
     if (h->use_tc && l + 1 < h->L) cudaStreamWaitEvent(st, h->ev_pre[MAML_MAX_LAYERS + l + 1], 0);
-    if (h->ln) {
-      LnArgs a = ln_args(h, l, sp.n, meta, T);
-      a.dp = DP(sp, l, s); a.dp_stride = STRIDE(sp, dp, l);
-      a.dpd = DP(tn, l, 0); a.dpd_stride = STRIDE(tn, dp, l);
-      if (h->use_tc && l + 1 < h->L) a.dpd2 = DP(t2, l, 0);
-      a.zh = ZH(sp, l, s); a.zh_stride = STRIDE(sp, zh, l);
-      a.zhd = ZH(tn, l, 0); a.zhd_stride = STRIDE(tn, zh, l);
-      a.dz = DZ(sp, l, s); a.dz_stride = STRIDE(sp, dz, l);
-      a.st_fwd = ln_stat_at(h, PASS_SUP_FWD, s, l); a.st_bwd = ln_stat_at(h, PASS_SUP_BWD, s, l);
-      a.st_tan = ln_stat_at(h, PASS_TAN_FWD, s, l); a.st_out = ln_stat_at(h, th.kind_tbwd, s, l);
-      a.out = DZ(tn, l, 0); a.out_stride = STRIDE(tn, dz, l);
-      if (h->use_tc && l >= 1) { a.out_hi = DZ_HI(tn, l, 0); a.out_lo = DZ_LO(tn, l, 0); }
-      launch_ln_bwd(a, true, st);
-      // H_b u, the tangent of the support loss's bias gradient: export subtracts kind 1 (fused iteration, b-bar -= H_b u)
-      // and adds kind 0 (functional operator, +H_b v), as it does with the BatchNorm gamma / beta sums of kind_tbwd
-      a.db = lnb_at(h, th.kind_tbwd == PASS_TGT_BWD ? 0 : 1, s) + h->pl.lnb_off[l];
-      a.db_stride = 2LL * h->S * h->pl.lnb_off[h->L];
-      launch_ln_bias_grad(a, true, st);
-    } else {
-    BnBwdTanArgs b{};
-    b.dp = DP(sp, l, s); b.dp_stride = STRIDE(sp, dp, l);
-    b.dpdot = DP(tn, l, 0); b.dpdot_stride = STRIDE(tn, dp, l);
-    if (h->use_tc && l + 1 < h->L) b.dpdot2 = DP(t2, l, 0);
-    b.zh = ZH(sp, l, s); b.zh_stride = STRIDE(sp, zh, l);
-    b.zhdot = ZH(tn, l, 0); b.zhdot_stride = STRIDE(tn, zh, l);
-    b.dz = DZ(sp, l, s); b.dz_stride = STRIDE(sp, dz, l);
-    b.stats_fwd = stat_at(h, PASS_SUP_FWD, s, l); b.stats_fwd_stride = h->stats_task_stride;
-    b.stats_bwd = stat_at(h, PASS_SUP_BWD, s, l); b.stats_bwd_stride = h->stats_task_stride;
-    b.stats_tan = stat_at(h, PASS_TAN_FWD, s, l); b.stats_tan_stride = h->stats_task_stride;
-    b.stats_tbwd = stat_at(h, th.kind_tbwd, s, l); b.stats_tbwd_stride = h->stats_task_stride;
-    b.gamma = gamma_at(h, meta, l, s); b.beta = beta_at(h, meta, l, s);
-    b.dzdot = DZ(tn, l, 0); b.dzdot_stride = STRIDE(tn, dz, l);
-    if (h->use_tc && l >= 1) { b.dzdot_hi = DZ_HI(tn, l, 0); b.dzdot_lo = DZ_LO(tn, l, 0); }
-    b.g = bn_geom(h, l, sp.n); b.tasks = T;
-    if (fuse_tail && l == h->L - 1) launch_tail_tan_fused(last_act, hd, b, st);
-    else launch_bnbwd_tan(b, st);
-    }
+    norm_tangent_backward(h, s, meta, l, th.kind_tbwd, T, st, &last_act, fuse_tail ? &hd : nullptr);
     cudaEventRecord(h->ev_fork, st); cudaStreamWaitEvent(h->s_wg, h->ev_fork, 0);
 
     if (l == 0) {
@@ -1409,17 +1443,9 @@ extern "C" int maml_b200_net_backward_tasks(maml_b200_handle* h, int32_t n_tasks
   LaunchScope launch_scope(h, st);
   const int T = n_tasks;
   record_call(h, FN_NONE, 0, 0);
-  // backward statistics (and the tangent ones export subtracts) start from zero; forward statistics are kept.  Layer norm:
-  // its backward sums are added to with atomics, and export sums both kinds of bias-gradient rows over every step
-  for (int kind : {PASS_TGT_BWD, PASS_TAN_BWD}) {
-    CK(cudaMemset2DAsync(h->stats + (long long)kind * MAML_MAX_STEPS * h->st_pass_stride, (size_t)h->stats_task_stride * sizeof(double), 0,
-                         (size_t)MAML_MAX_STEPS * h->st_pass_stride * sizeof(double), (size_t)T, st));
-    if (h->ln)
-      CK(cudaMemset2DAsync(h->ln_stats + (long long)kind * h->ln_pass_stride, (size_t)h->ln_task_stride * sizeof(double), 0,
-                           (size_t)h->ln_pass_stride * sizeof(double), (size_t)T, st));
-  }
-  if (h->ln) CK(cudaMemsetAsync(h->lnb, 0, (size_t)T * 2 * h->S * h->pl.lnb_off[h->L] * sizeof(float), st));
-  if (clear_accumulators(h, CLR_ABAR | CLR_LOSSES | CLR_CORRECT, st)) return 1;
+  // backward sums (and the tangent ones export subtracts) start from zero; the forward sums of net_forward are kept.  Layer
+  // norm: export sums both kinds of bias-gradient rows over every step
+  if (clear_accumulators(h, CLR_BWD_STATS | CLR_ABAR | CLR_LOSSES | CLR_CORRECT, st, T)) return 1;
   external_backward(h, h->tgt, 0, num_step, PASS_TGT_FWD, PASS_TGT_BWD, meta_like, dlogits, h->tgt_partial, h->plan_tgt, T, st);
   launch_param_reduce(h->pl, h->plan_tgt.pd, h->tgt_partial, PR_STORE, nullptr, nullptr, h->tbar, nullptr, meta_like, num_step,
                       h->Ppad, T, st);
@@ -1485,7 +1511,9 @@ static int net_hvp_impl(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, 
   if (fork_direction(h, T, st, &spre)) return 1;
   ReduceSpec rs{PR_STORE, nullptr, nullptr, h->tbar, nullptr, s, -1};
   const TangentHead th_ext{HEAD_EXTERNAL_TAN, nullptr, dlogits, (long long)h->n_s * h->N, jv_out, PASS_TGT_BWD};
-  tangent_pass(h, s, th, h->u, meta_like, th_ext, T, st, rs, spre, xdot ? h->xdot_g : nullptr, v_like, dir_stride);
+  // the HVP has no BatchNorm gamma / beta directions: only a layer-norm handle's tangent pass reads v_like's norm entries
+  tangent_pass(h, s, th, h->u, meta_like, th_ext, T, st, rs, spre, xdot ? h->xdot_g : nullptr, h->ln ? v_like : nullptr,
+               dir_stride);
   join_pending(h, st);
   launch_export(export_args(h, T, hv_out, !sum_tasks), st);
   CK(cudaGetLastError());

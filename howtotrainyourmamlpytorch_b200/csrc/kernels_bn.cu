@@ -14,17 +14,22 @@
 __device__ __forceinline__ float leaky(float y) { return y > 0.f ? y : LEAKY_SLOPE_F * y; }
 __device__ __forceinline__ float slope_of(float y) { return y > 0.f ? 1.f : LEAKY_SLOPE_F; }
 
+// mean and r = 1 / sqrt(var + eps) of m values from their fp64 sums st[0] = sum z, st[1] = sum z^2
+__device__ __forceinline__ void norm_consts(const double* __restrict__ st, double m, float& mu, float& r) {
+  const double mean = st[0] / m;
+  double var = st[1] / m - mean * mean;
+  if (var < 0.0) var = 0.0;
+  mu = (float)mean;
+  r = (float)(1.0 / sqrt(var + BN_EPS_D));
+}
+
 // per-channel constants from the fp64 sums (sum z, sum z^2)
 __device__ __forceinline__ void chan_setup(const double* __restrict__ st, const float* __restrict__ gamma,
                                            const float* __restrict__ beta, double m, int F, float* s_mu, float* s_r,
                                            float* s_g, float* s_b) {
   const int tid = threadIdx.x;
   if (tid < F) {
-    const double mean = st[tid * 2 + 0] / m;
-    double var = st[tid * 2 + 1] / m - mean * mean;
-    if (var < 0.0) var = 0.0;
-    s_mu[tid] = (float)mean;
-    s_r[tid] = (float)(1.0 / sqrt(var + BN_EPS_D));
+    norm_consts(st + tid * 2, m, s_mu[tid], s_r[tid]);
     s_g[tid] = gamma[tid];
     s_b[tid] = beta[tid];
   }
@@ -192,6 +197,102 @@ struct WinIter {
   }
 };
 
+// ------------------------------------------------------------------------------- per-window bodies
+// One pooling window (wy, wx) of image img for this thread's channel quad, shared by the BatchNorm phases and the layer-norm
+// kernels.  The constants (mu, r, gamma, the sums / m) are per channel for BatchNorm and per image for layer norm (gamma =
+// 1); be_at(yy, xx) is beta at pixel (yy, xx): BatchNorm's per-channel quad at every position, layer norm's bias there.
+
+// v at idx, and its TF32 split into the planes hi / lo (nullable) `toff` floats from their task's start
+__device__ __forceinline__ void st4_out(float* p, float* hi, float* lo, long long toff, long long idx, float4 v) {
+  st4(p + idx, v);
+  if (hi) st4_split(hi + toff, lo + toff, idx, v);
+}
+
+// a full window of the backward-type kernels: loads zh at its four positions and recomputes the forward's pooling decision
+template <class BeAt>
+__device__ __forceinline__ void argmax_window(const float* __restrict__ zhp, const BnGeom& g, int img, int wy, int wx,
+                                              const WinIter& it, const float4& ga, BeAt be_at, float4 (&zh)[4],
+                                              long long (&idx)[4], int4& arg, float4& slope_at) {
+  WinMax w{};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
+    idx[k] = it.grid(g, img, yy, xx);
+    zh[k] = ld4(zhp + idx[k]);
+    keep_first_max(k, bn_act(ga, zh[k], be_at(yy, xx)), w);
+  }
+  arg = w.arg;
+  slope_at = slope_of(w.y);
+}
+
+// forward: zh = (z - mu) * r in place, p = max-pool(leaky(gamma * zh + beta)) at a full window
+template <class BeAt>
+__device__ __forceinline__ void act_window(const WinIter& it, const BnGeom& g, int img, int wy, int wx, float* z, const float4& mu,
+                                           const float4& r, const float4& ga, BeAt be_at, float* p, float* p_hi, float* p_lo,
+                                           long long p_toff) {
+  WinMax w{};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
+    if (yy < g.h && xx < g.w) {
+      const long long idx = it.grid(g, img, yy, xx);
+      const float4 zh = bn_normalize(ld4(z + idx), mu, r);
+      st4(z + idx, zh);
+      keep_first_max(k, bn_act(ga, zh, be_at(yy, xx)), w);
+    }
+  }
+  if (wy < g.ph && wx < g.pw) st4_out(p, p_hi, p_lo, p_toff, it.pooled(g, img, wy, wx), w.act);
+}
+
+// backward sums of a full window at its arg-max (partial windows add nothing): S1 += dy, S2 += dy * zh
+template <class BeAt>
+__device__ __forceinline__ void bwd_reduce_window(const WinIter& it, const BnGeom& g, int img, int wy, int wx, const float* zhp,
+                                                  const float4& ga, BeAt be_at, const float* dp, double (&s1)[4], double (&s2)[4]) {
+  if (wy >= g.ph || wx >= g.pw) return;
+  float4 zh[4]; long long idx[4]; int4 arg; float4 sl;
+  argmax_window(zhp, g, img, wy, wx, it, ga, be_at, zh, idx, arg, sl);
+  bn_bwd_sums(ld4(dp + it.pooled(g, img, wy, wx)), sl, zh, arg, s1, s2);
+}
+
+// tangent backward sums of a full window at its arg-max: T1 += dydot, T2 += dydot * zh + dy * zhdot; dpdot = dpd (+ dpd2)
+template <class BeAt>
+__device__ __forceinline__ void bwd_tan_reduce_window(const WinIter& it, const BnGeom& g, int img, int wy, int wx, const float* zhp,
+                                                      const float4& ga, BeAt be_at, const float* zhd, const float* dp,
+                                                      const float* dpd, const float* dpd2, double (&s1)[4], double (&s2)[4]) {
+  if (wy >= g.ph || wx >= g.pw) return;
+  float4 zh[4]; long long idx[4]; int4 arg; float4 sl;
+  argmax_window(zhp, g, img, wy, wx, it, ga, be_at, zh, idx, arg, sl);
+  const long long pidx = it.pooled(g, img, wy, wx);
+  const float4 d = ld4(dp + pidx);
+  const float4 dd = ld4_sum(dpd, dpd2, pidx);
+  bn_tan_bwd_sums(d, dd, sl, zh, arg, [&](int k, int c) { return zhd[pick(idx, k) + c]; }, s1, s2);
+}
+
+// dz = r * gamma * (dy - S1/m - zh * S2/m) at every position inside the image (dy != 0 only at the arg-max); rg = r * gamma,
+// c1 = S1/m, c2 = S2/m
+template <class BeAt>
+__device__ __forceinline__ void bwd_apply_window(const WinIter& it, const BnGeom& g, int img, int wy, int wx, const float* zhp,
+                                                 const float4& ga, BeAt be_at, const float* dp, const float4& rg, const float4& c1,
+                                                 const float4& c2, float* dz, float* dz_hi, float* dz_lo, long long dz_toff) {
+  const bool full = (wy < g.ph && wx < g.pw);
+  if (full) {
+    float4 zh[4]; long long idx[4]; int4 arg; float4 sl;
+    argmax_window(zhp, g, img, wy, wx, it, ga, be_at, zh, idx, arg, sl);
+    const float4 dyv = mul4(ld4(dp + it.pooled(g, img, wy, wx)), sl);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) st4_out(dz, dz_hi, dz_lo, dz_toff, idx[k], bn_bwd_dz(rg, c1, zh[k], c2, k, arg, dyv));
+  } else {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
+      if (yy < g.h && xx < g.w) {
+        const long long idx = it.grid(g, img, yy, xx);
+        st4_out(dz, dz_hi, dz_lo, dz_toff, idx, bn_bwd_dz<true>(rg, c1, ld4(zhp + idx), c2));
+      }
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------- forward
 __device__ __forceinline__ void bnact_phase(const BnActArgs& a, const BnGeom& g, int task, int cta, int ncta, const WinIter& it,
                                             const float* s_mu, const float* s_r, const float* s_g, const float* s_b) {
@@ -201,22 +302,7 @@ __device__ __forceinline__ void bnact_phase(const BnActArgs& a, const BnGeom& g,
   float* p = a.p + (long long)task * a.p_stride;
   for (int wi = cta * it.WPB + it.lane; wi < it.NW; wi += ncta * it.WPB) {
     int img, wy, wx; it.window(wi, img, wy, wx);
-    WinMax w{};
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
-      if (yy < g.h && xx < g.w) {
-        const long long idx = it.grid(g, img, yy, xx);
-        const float4 zh = bn_normalize(ld4(z + idx), mu, r);
-        st4(z + idx, zh);
-        keep_first_max(k, bn_act(ga, zh, be), w);
-      }
-    }
-    if (wy < g.ph && wx < g.pw) {
-      const long long pidx = it.pooled(g, img, wy, wx);
-      st4(p + pidx, w.act);
-      if (a.p_hi) st4_split(a.p_hi + (long long)task * a.p_stride, a.p_lo + (long long)task * a.p_stride, pidx, w.act);
-    }
+    act_window(it, g, img, wy, wx, z, mu, r, ga, [&](int, int) { return be; }, p, a.p_hi, a.p_lo, (long long)task * a.p_stride);
   }
 }
 
@@ -252,22 +338,6 @@ void launch_bnact(const BnActArgs& a, cudaStream_t st) {
   int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
   launch_pdl(bnact_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
   CUDA_CHECK_LAUNCH();
-}
-
-// a full window of the backward-type kernels: loads zh at its four positions and recomputes the forward's pooling decision
-__device__ __forceinline__ void argmax_window(const float* __restrict__ zhp, const BnGeom& g, int img, int wy, int wx,
-                                              const WinIter& it, const float4& ga, const float4& be, float4 (&zh)[4],
-                                              long long (&idx)[4], int4& arg, float4& slope_at) {
-  WinMax w{};
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
-    idx[k] = it.grid(g, img, yy, xx);
-    zh[k] = ld4(zhp + idx[k]);
-    keep_first_max(k, bn_act(ga, zh[k], be), w);
-  }
-  arg = w.arg;
-  slope_at = slope_of(w.y);
 }
 
 // ---- thread-block-cluster helpers for the fused (reduce -> cluster all-reduce -> apply) backward kernels
@@ -346,10 +416,7 @@ __device__ __forceinline__ void bnbwd_reduce_phase(const BnBwdArgs& a, const BnG
   const float* dp = a.dp + (long long)task * a.dp_stride;
   for (int wi = cta * it.WPB + it.lane; wi < it.NW; wi += ncta * it.WPB) {
     int img, wy, wx; it.window(wi, img, wy, wx);
-    if (wy >= g.ph || wx >= g.pw) continue;
-    float4 zh[4]; long long idx[4]; int4 arg; float4 sl;
-    argmax_window(zhp, g, img, wy, wx, it, ga, be, zh, idx, arg, sl);
-    bn_bwd_sums(ld4(dp + it.pooled(g, img, wy, wx)), sl, zh, arg, s1, s2);
+    bwd_reduce_window(it, g, img, wy, wx, zhp, ga, [&](int, int) { return be; }, dp, s1, s2);
   }
 }
 
@@ -387,29 +454,8 @@ __device__ __forceinline__ void bnbwd_apply_phase(const BnBwdArgs& a, const BnGe
   float* dz = a.dz + (long long)task * a.dz_stride;
   for (int wi = cta * it.WPB + it.lane; wi < it.NW; wi += ncta * it.WPB) {
     int img, wy, wx; it.window(wi, img, wy, wx);
-    const bool full = (wy < g.ph && wx < g.pw);
-    if (full) {
-      float4 zh[4]; long long idx[4]; int4 arg; float4 sl;
-      argmax_window(zhp, g, img, wy, wx, it, ga, be, zh, idx, arg, sl);
-      const float4 dyv = mul4(ld4(dp + it.pooled(g, img, wy, wx)), sl);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const float4 o = bn_bwd_dz(rg, c1, zh[k], c2, k, arg, dyv);
-        st4(dz + idx[k], o);
-        if (a.dz_hi) st4_split(a.dz_hi + (long long)task * a.dz_stride, a.dz_lo + (long long)task * a.dz_stride, idx[k], o);
-      }
-    } else {
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
-        if (yy < g.h && xx < g.w) {
-          const long long idx = it.grid(g, img, yy, xx);
-          const float4 o = bn_bwd_dz<true>(rg, c1, ld4(zhp + idx), c2);
-          st4(dz + idx, o);
-          if (a.dz_hi) st4_split(a.dz_hi + (long long)task * a.dz_stride, a.dz_lo + (long long)task * a.dz_stride, idx, o);
-        }
-      }
-    }
+    bwd_apply_window(it, g, img, wy, wx, zhp, ga, [&](int, int) { return be; }, dp, rg, c1, c2, dz, a.dz_hi, a.dz_lo,
+                     (long long)task * a.dz_stride);
   }
 }
 
@@ -583,13 +629,7 @@ __device__ __forceinline__ void bnbwd_tan_reduce_phase(const BnBwdTanArgs& a, co
   const float* dpd2 = a.dpdot2 ? a.dpdot2 + (long long)task * a.dpdot_stride : nullptr;
   for (int wi = cta * it.WPB + it.lane; wi < it.NW; wi += ncta * it.WPB) {
     int img, wy, wx; it.window(wi, img, wy, wx);
-    if (wy >= g.ph || wx >= g.pw) continue;
-    float4 zh[4]; long long idx[4]; int4 arg; float4 sl;
-    argmax_window(zhp, g, img, wy, wx, it, ga, be, zh, idx, arg, sl);
-    const long long pidx = it.pooled(g, img, wy, wx);
-    const float4 d = ld4(dp + pidx);
-    const float4 dd = ld4_sum(dpd, dpd2, pidx);
-    bn_tan_bwd_sums(d, dd, sl, zh, arg, [&](int k, int c) { return zhd[pick(idx, k) + c]; }, s1, s2);
+    bwd_tan_reduce_window(it, g, img, wy, wx, zhp, ga, [&](int, int) { return be; }, zhd, dp, dpd, dpd2, s1, s2);
   }
 }
 
@@ -637,7 +677,7 @@ __device__ __forceinline__ void bnbwd_tan_apply_phase(const BnBwdTanArgs& a, con
     float4 dyd = make_float4(0.f, 0.f, 0.f, 0.f);
     if (full) {
       float4 zh[4]; long long idx[4]; float4 sl;
-      argmax_window(zhp, g, img, wy, wx, it, ga, be, zh, idx, arg, sl);
+      argmax_window(zhp, g, img, wy, wx, it, ga, [&](int, int) { return be; }, zh, idx, arg, sl);
       dyd = mul4(ld4_sum(dpd, dpd2, it.pooled(g, img, wy, wx)), sl);
     }
 #pragma unroll
@@ -1066,14 +1106,6 @@ MAML_TRACE_SETTER(trace_set_bn)
 __device__ __forceinline__ float4 ones4() { return make_float4(1.f, 1.f, 1.f, 1.f); }
 __device__ __forceinline__ float4 splat4(float v) { return make_float4(v, v, v, v); }
 
-// per-image constants from fp64 sums (m = F h w): mean and r = 1 / sqrt(var + eps), as chan_setup does per channel
-__device__ __forceinline__ void ln_image_consts(const double* st, double m, float& mu, float& r) {
-  const double mean = st[0] / m;
-  double var = st[1] / m - mean * mean;
-  if (var < 0.0) var = 0.0;
-  mu = (float)mean;
-  r = (float)(1.0 / sqrt(var + BN_EPS_D));
-}
 __device__ __forceinline__ const double* ln_st(const double* base, long long stride, int task, int img) {
   return base + (long long)task * stride + 2LL * img;
 }
@@ -1097,11 +1129,7 @@ __device__ __forceinline__ void ln_block_add(double s1, double s2, double* dst) 
     atomicAdd(dst + 1, t2);
   }
 }
-// The windows of image blockIdx.y handled by this thread: wi = blockIdx.x * WPB + lane, stride gridDim.x * WPB
-#define LN_FOR_WINDOWS(it, wy, wx)                                                                          \
-  for (int wi_ = blockIdx.x * (it).WPB + (it).lane, wy = 0, wx = 0; wi_ < (it).hc * (it).wc;                \
-       wi_ += gridDim.x * (it).WPB)                                                                         \
-    if ((wy = wi_ / (it).wc, wx = wi_ - wy * (it).wc), true)
+// Every per-image kernel below runs the windows of image blockIdx.y: wi = blockIdx.x * WPB + lane, stride gridDim.x * WPB.
 
 // sums of one image: primal (sum z, sum z^2); tangent (sum zdot, sum zh * zdot) with zdot = z + z2
 template <bool TAN>
@@ -1115,7 +1143,8 @@ __global__ void __launch_bounds__(256) ln_stats_kernel(LnArgs a) {
     const float* z = a.z + (long long)task * a.z_stride;
     const float* z2 = a.z2 ? a.z2 + (long long)task * a.z_stride : nullptr;
     const float* zhp = TAN ? a.zh + (long long)task * a.zh_stride : nullptr;
-    LN_FOR_WINDOWS(it, wy, wx) {
+    for (int wi = blockIdx.x * it.WPB + it.lane; wi < it.hc * it.wc; wi += gridDim.x * it.WPB) {
+      const int wy = wi / it.wc, wx = wi - wy * it.wc;
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
@@ -1144,62 +1173,41 @@ __global__ void __launch_bounds__(256) ln_act_kernel(LnArgs a) {
   WinIter it(g);
   if (it.lane >= it.WPB) return;
   float mu, r;
-  ln_image_consts(ln_st(a.st_fwd, a.st_stride, task, img), m, mu, r);
+  norm_consts(ln_st(a.st_fwd, a.st_stride, task, img), m, mu, r);
   float md = 0.f, qq = 0.f;
   if (TAN) {
     const double* stt = ln_st(a.st_tan, a.st_stride, task, img);
     md = (float)(stt[0] / m); qq = (float)(stt[1] / m);
   }
-  const float4 one = ones4();
   float* z = a.z + (long long)task * a.z_stride;
   const float* z2 = a.z2 ? a.z2 + (long long)task * a.z_stride : nullptr;
   const float* zhp = TAN ? a.zh + (long long)task * a.zh_stride : nullptr;
   const float* bd = BDOT ? a.bdot + (long long)task * a.bdot_stride : nullptr;
   float* p = a.out + (long long)task * a.out_stride;
-  LN_FOR_WINDOWS(it, wy, wx) {
+  const long long toff = (long long)task * a.out_stride;
+  for (int wi = blockIdx.x * it.WPB + it.lane; wi < it.hc * it.wc; wi += gridDim.x * it.WPB) {
+    const int wy = wi / it.wc, wx = wi - wy * it.wc;
+    if (!TAN) {
+      act_window(it, g, img, wy, wx, z, splat4(mu), splat4(r), ones4(), [&](int yy, int xx) { return ln_bias4(a.bias, g, it.q, yy, xx); },
+                 p, a.out_hi, a.out_lo, toff);
+      continue;
+    }
+    // the tangent, like bnact_tan_phase (whose code is kept apart: sharing it changes the BatchNorm kernels' SASS)
     WinMax w{};
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
       if (yy < g.h && xx < g.w) {
         const long long idx = it.grid(g, img, yy, xx);
-        const float4 be = ln_bias4(a.bias, g, it.q, yy, xx);
-        if (TAN) {
-          const float4 zh = ld4(zhp + idx);
-          const float4 zhd = bn_tan_normalize(ld4_sum(z, z2, idx), zh, splat4(r), splat4(md), splat4(qq));
-          st4(z + idx, zhd);
-          const BnAct v = bn_act(one, zh, be);
-          keep_first_max(k, v, w, act_tangent<BDOT>(v, one, zhd, zh, float4(), BDOT ? ln_bias4(bd, g, it.q, yy, xx) : float4()));
-        } else {
-          const float4 zh = bn_normalize(ld4(z + idx), splat4(mu), splat4(r));
-          st4(z + idx, zh);
-          keep_first_max(k, bn_act(one, zh, be), w);
-        }
+        const float4 zh = ld4(zhp + idx);
+        const float4 zhd = bn_tan_normalize(ld4_sum(z, z2, idx), zh, splat4(r), splat4(md), splat4(qq));
+        st4(z + idx, zhd);
+        const BnAct v = bn_act(ones4(), zh, ln_bias4(a.bias, g, it.q, yy, xx));
+        keep_first_max(k, v, w, act_tangent<BDOT>(v, ones4(), zhd, zh, float4(), BDOT ? ln_bias4(bd, g, it.q, yy, xx) : float4()));
       }
     }
-    if (wy < g.ph && wx < g.pw) {
-      const long long pidx = it.pooled(g, img, wy, wx);
-      const float4 o = TAN ? w.p : w.act;
-      st4(p + pidx, o);
-      if (a.out_hi) st4_split(a.out_hi + (long long)task * a.out_stride, a.out_lo + (long long)task * a.out_stride, pidx, o);
-    }
+    if (wy < g.ph && wx < g.pw) st4_out(p, a.out_hi, a.out_lo, toff, it.pooled(g, img, wy, wx), w.p);
   }
-}
-
-// the arg-max window of the backward-type kernels, with the per-position layer-norm bias in place of beta
-__device__ __forceinline__ void ln_argmax_window(const float* __restrict__ zhp, const float* bias, const BnGeom& g, int img,
-                                                 int wy, int wx, const WinIter& it, float4 (&zh)[4], long long (&idx)[4],
-                                                 int4& arg, float4& slope_at) {
-  WinMax w{};
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
-    idx[k] = it.grid(g, img, yy, xx);
-    zh[k] = ld4(zhp + idx[k]);
-    keep_first_max(k, bn_act(ones4(), zh[k], ln_bias4(bias, g, it.q, yy, xx)), w);
-  }
-  arg = w.arg;
-  slope_at = slope_of(w.y);
 }
 
 // per-image backward sums: primal (S1 = sum dy, S2 = sum dy zh); tangent (T1 = sum dydot, T2 = sum dydot zh + dy zhdot)
@@ -1213,18 +1221,15 @@ __global__ void __launch_bounds__(256) ln_bwd_reduce_kernel(LnArgs a) {
   if (it.lane < it.WPB) {
     const float* zhp = a.zh + (long long)task * a.zh_stride;
     const float* dp = a.dp + (long long)task * a.dp_stride;
-    LN_FOR_WINDOWS(it, wy, wx) {
-      if (wy >= g.ph || wx >= g.pw) continue;
-      float4 zh[4]; long long idx[4]; int4 arg; float4 sl;
-      ln_argmax_window(zhp, a.bias, g, img, wy, wx, it, zh, idx, arg, sl);
-      const long long pidx = it.pooled(g, img, wy, wx);
-      if (TAN) {
-        const float* zhd = a.zhd + (long long)task * a.zhd_stride;
-        const float4 dd = ld4_sum(a.dpd + (long long)task * a.dpd_stride, a.dpd2 ? a.dpd2 + (long long)task * a.dpd_stride : nullptr, pidx);
-        bn_tan_bwd_sums(ld4(dp + pidx), dd, sl, zh, arg, [&](int k, int c) { return zhd[pick(idx, k) + c]; }, s1, s2);
-      } else {
-        bn_bwd_sums(ld4(dp + pidx), sl, zh, arg, s1, s2);
-      }
+    const auto be_at = [&](int yy, int xx) { return ln_bias4(a.bias, g, it.q, yy, xx); };
+    for (int wi = blockIdx.x * it.WPB + it.lane; wi < it.hc * it.wc; wi += gridDim.x * it.WPB) {
+      const int wy = wi / it.wc, wx = wi - wy * it.wc;
+      if constexpr (TAN)
+        bwd_tan_reduce_window(it, g, img, wy, wx, zhp, ones4(), be_at, a.zhd + (long long)task * a.zhd_stride, dp,
+                              a.dpd + (long long)task * a.dpd_stride, a.dpd2 ? a.dpd2 + (long long)task * a.dpd_stride : nullptr,
+                              s1, s2);
+      else
+        bwd_reduce_window(it, g, img, wy, wx, zhp, ones4(), be_at, dp, s1, s2);
     }
   }
   ln_block_add(s1[0] + s1[1] + s1[2] + s1[3], s2[0] + s2[1] + s2[2] + s2[3],
@@ -1241,7 +1246,7 @@ __global__ void __launch_bounds__(256) ln_bwd_apply_kernel(LnArgs a) {
   WinIter it(g);
   if (it.lane >= it.WPB) return;
   float mu, r;
-  ln_image_consts(ln_st(a.st_fwd, a.st_stride, task, img), m, mu, r);
+  norm_consts(ln_st(a.st_fwd, a.st_stride, task, img), m, mu, r);
   // this pass's sums (primal S1, S2; tangent T1, T2) are in st_out; the tangent also reads the primal S2 and q
   const double* sc = ln_st(a.st_out, a.st_stride, task, img);
   const float4 rr = splat4(r);
@@ -1253,32 +1258,32 @@ __global__ void __launch_bounds__(256) ln_bwd_apply_kernel(LnArgs a) {
   }
   const float* zhp = a.zh + (long long)task * a.zh_stride;
   float* dz = a.out + (long long)task * a.out_stride;
-  LN_FOR_WINDOWS(it, wy, wx) {
-    const bool full = (wy < g.ph && wx < g.pw);
+  const long long toff = (long long)task * a.out_stride;
+  const auto be_at = [&](int yy, int xx) { return ln_bias4(a.bias, g, it.q, yy, xx); };
+  for (int wi = blockIdx.x * it.WPB + it.lane; wi < it.hc * it.wc; wi += gridDim.x * it.WPB) {
+    const int wy = wi / it.wc, wx = wi - wy * it.wc;
+    if (!TAN) {
+      bwd_apply_window(it, g, img, wy, wx, zhp, ones4(), be_at, a.dp + (long long)task * a.dp_stride, rr, c1, c2, dz, a.out_hi,
+                       a.out_lo, toff);
+      continue;
+    }
+    // the tangent, like bnbwd_tan_apply_phase (whose code is kept apart: sharing it changes the BatchNorm kernels' SASS)
     int4 arg = make_int4(-1, -1, -1, -1);
     float4 dy = float4();
-    if (full) {
+    if (wy < g.ph && wx < g.pw) {
       float4 zh[4]; long long idx[4]; float4 sl;
-      ln_argmax_window(zhp, a.bias, g, img, wy, wx, it, zh, idx, arg, sl);
-      const long long pidx = it.pooled(g, img, wy, wx);
-      dy = TAN ? mul4(ld4_sum(a.dpd + (long long)task * a.dpd_stride, a.dpd2 ? a.dpd2 + (long long)task * a.dpd_stride : nullptr, pidx), sl)
-               : mul4(ld4(a.dp + (long long)task * a.dp_stride + pidx), sl);
+      argmax_window(zhp, g, img, wy, wx, it, ones4(), be_at, zh, idx, arg, sl);
+      dy = mul4(ld4_sum(a.dpd + (long long)task * a.dpd_stride, a.dpd2 ? a.dpd2 + (long long)task * a.dpd_stride : nullptr,
+                        it.pooled(g, img, wy, wx)), sl);
     }
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const int yy = 2 * wy + (k >> 1), xx = 2 * wx + (k & 1);
       if (yy < g.h && xx < g.w) {
         const long long idx = it.grid(g, img, yy, xx);
-        const float4 zh = ld4(zhp + idx);
-        float4 o;
-        if (TAN) {
-          o = bn_tan_bwd_dz(rq, ld4(a.dz + (long long)task * a.dz_stride + idx), rr, t1,
-                            ld4(a.zhd + (long long)task * a.zhd_stride + idx), c2, zh, t2, k, arg, dy, full);
-        } else {
-          o = full ? bn_bwd_dz(rr, c1, zh, c2, k, arg, dy) : bn_bwd_dz<true>(rr, c1, zh, c2);
-        }
-        st4(dz + idx, o);
-        if (a.out_hi) st4_split(a.out_hi + (long long)task * a.out_stride, a.out_lo + (long long)task * a.out_stride, idx, o);
+        st4_out(dz, a.out_hi, a.out_lo, toff, idx,
+                bn_tan_bwd_dz(rq, ld4(a.dz + (long long)task * a.dz_stride + idx), rr, t1, ld4(a.zhd + (long long)task * a.zhd_stride + idx),
+                              c2, ld4(zhp + idx), t2, k, arg, dy));
       }
     }
   }
@@ -1302,7 +1307,8 @@ __global__ void __launch_bounds__(256) ln_bias_grad_kernel(LnArgs a) {
     const float* src2 = TAN && a.dpd2 ? a.dpd2 + (long long)task * a.dpd_stride : nullptr;
     for (int img = 0; img < g.n; ++img) {
       float4 zh[4]; long long idx[4]; int4 arg; float4 sl;
-      ln_argmax_window(zhp, a.bias, g, img, wy, wx, it, zh, idx, arg, sl);
+      argmax_window(zhp, g, img, wy, wx, it, ones4(), [&](int yy, int xx) { return ln_bias4(a.bias, g, it.q, yy, xx); }, zh, idx,
+                    arg, sl);
       const float4 dy = mul4(ld4_sum(src, src2, it.pooled(g, img, wy, wx)), sl);
 #pragma unroll
       for (int k = 0; k < 4; ++k)

@@ -129,38 +129,13 @@ class MAMLFewShotClassifier(nn.Module):
         return [(n, p) for n, p in self.named_parameters() if p.requires_grad]
 
     def _meta_param_names(self):
-        """Flat-buffer order = engine segment order: per block conv.weight, conv.bias, norm.bias, norm.weight (layer norm:
-        conv.weight, conv.bias, norm.bias -- its frozen weight is no meta-parameter); linear.weights, linear.bias; LSLR
-        vectors.  (Equals the reference's Adam parameter order.)"""
-        names = []
-        L = int(self.args.num_stages)
-        for l in range(L):
-            p = "classifier.layer_dict.conv%d." % l
-            names += [p + "conv.weight", p + "conv.bias", p + "norm_layer.bias"]
-            if not self._layer_norm():
-                names.append(p + "norm_layer.weight")
-        names += ["classifier.layer_dict.linear.weights", "classifier.layer_dict.linear.bias"]
+        """Flat-buffer order = the network's engine segment order (``_segment_names``), then the LSLR vectors.  (Equals
+        the reference's Adam parameter order.)"""
+        names = ["classifier." + n for n in self.classifier._segment_names()]
         inner = [n for n in names if "norm_layer" not in n]
         names += ["inner_loop_optimizer.names_learning_rates_dict." + n[len("classifier."):].replace(".", "-")
                   for n in inner]
         return names
-
-    def _layer_norm(self):
-        return getattr(self.args, "norm_layer", "batch_norm") == "layer_norm"
-
-    def _check_layer_norm_weights(self):
-        """The engine applies the layer norm's frozen weight as ones (the reference creates it so and never trains it).
-        Any other value -- e.g. from a loaded state_dict -- is refused rather than silently ignored.  Checked again
-        whenever a weight tensor is replaced or modified in place."""
-        norms = [self.classifier.layer_dict["conv%d" % l].norm_layer for l in range(int(self.args.num_stages))]
-        key = tuple((m.weight.data_ptr(), m.weight._version) for m in norms)
-        if key == getattr(self, "_ln_weight_key", None):
-            return
-        for l, m in enumerate(norms):
-            if not bool(torch.all(m.weight.detach() == 1)):
-                raise ValueError("classifier.layer_dict.conv%d.norm_layer.weight is not all ones: the layer-norm network "
-                                 "runs with the reference's frozen all-ones weight only" % l)
-        self._ln_weight_key = key
 
     def _build_flat_storage(self):
         named = dict(self.named_parameters())
@@ -181,7 +156,7 @@ class MAMLFewShotClassifier(nn.Module):
             p.data = flat[off:off + size].view(p.shape)
             self._flat_slices[n] = (off, size)
             off += size
-        for l in range(L if not self._layer_norm() else 0):      # layer norm keeps no running statistics
+        for l in range(L if not self.classifier._layer_norm() else 0):      # layer norm keeps no running statistics
             bn = self.classifier.layer_dict["conv%d" % l].norm_layer
             run[0, l].copy_(bn.running_mean.data.reshape(run_rows, F))
             run[1, l].copy_(bn.running_var.data.reshape(run_rows, F))
@@ -302,7 +277,7 @@ class MAMLFewShotClassifier(nn.Module):
                     inner_steps=int(a.number_of_training_steps_per_iter), per_step_bn=bool(a.per_step_bn_statistics),
                     max_tasks=int(n_tasks), keep_target_passes=bool(getattr(self, "_debug_keep_target_passes", False)),
                     force_fp32_convs=bool(getattr(self, "_debug_force_fp32_convs", False)),
-                    layer_norm=self._layer_norm())
+                    layer_norm=self.classifier._layer_norm())
             self._engine_tasks = int(n_tasks)
             if self._engine.meta_size != self._flat.numel():
                 raise RuntimeError("engine / module parameter layout mismatch (%d vs %d floats)" %
@@ -409,8 +384,8 @@ class MAMLFewShotClassifier(nn.Module):
         # _shard_override = (rank, world): test hook -- act as one rank of a sharded job without a process group
         self.rank, self.world_size = getattr(self, "_shard_override", None) or self._dist()
         xs, xt, ys, yt = self._stage_batch(data_batch)
-        if self._layer_norm():
-            self._check_layer_norm_weights()
+        if self.classifier._layer_norm():
+            self.classifier._check_layer_norm_weights()
         B = xs.shape[0]
         n_t = xt.shape[1] * xt.shape[2]
         N = int(self.args.num_classes_per_set)
@@ -443,7 +418,7 @@ class MAMLFewShotClassifier(nn.Module):
                 eng.adam_step(self._flat, reduced, self._exp_avg, self._exp_avg_sq, lr=self._current_lr,
                               step=self.optimizer.step_count, trainable_mask=self._trainable_mask,
                               clamp_mask=self._clamp_mask)
-            if self.args.per_step_bn_statistics and not self._layer_norm() and (apply_update or not training_phase):
+            if self.args.per_step_bn_statistics and not self.classifier._layer_norm() and (apply_update or not training_phase):
                 # F.batch_norm's EMA side effect on running_*[step].  Evaluation passes leave it behind as well: the
                 # reference's backup is copy(tensor.data), an alias, so restore_backup_stats restores the mutated values
                 # (meta_neural_network_architectures.py:240-255; pinned by the val/ golden entries).

@@ -174,7 +174,7 @@ class VGGReLUNormNetwork(nn.Module):
                 fast[k] = v[0] if v.dim() == own[k].dim() + 1 else v   # strip the reference's replica dim
         return fast
 
-    def _check_layer_norm_weights(self, params):
+    def _check_layer_norm_weights(self, params=None):
         """The engine applies the layer norm's frozen weight as ones (the reference creates it so and never trains it):
         any other value, in ``params`` or in the module, is refused before anything runs.  The module's own weights are
         checked again only when replaced or modified in place."""

@@ -115,12 +115,12 @@ def test_refusals():
     with pytest.raises(NotImplementedError, match="layer_norm"):
         MAMLFewShotClassifier(im_shape=(2, a.image_channels, a.image_height, a.image_width), device="cpu",
                               args=args_from_json(None, **d))
-    m._check_layer_norm_weights()                      # all ones: accepted
+    m.classifier._check_layer_norm_weights()           # all ones: accepted
     sd = m.state_dict()
     sd["classifier.layer_dict.conv1.norm_layer.weight"] = torch.full_like(sd["classifier.layer_dict.conv1.norm_layer.weight"], 2.0)
     m.load_state_dict(sd)
     with pytest.raises(ValueError, match="conv1.norm_layer.weight is not all ones"):
-        m._check_layer_norm_weights()
+        m.classifier._check_layer_norm_weights()
 
 
 # ------------------------------------------------------------------------------------------------ GPU
