@@ -13,7 +13,7 @@ LIB_PATH = os.environ.get("MAML_B200_LIB") or os.path.join(_PKG, "lib", "libmaml
 
 MAX_STAGES = 4
 MAX_STEPS = 8
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 EXPORTED_SYMBOLS = [
     "maml_b200_abi_version", "maml_b200_last_error", "maml_b200_create", "maml_b200_destroy",
@@ -34,7 +34,7 @@ PROF_CATS = ["conv_igemm", "conv_first_block", "wgrad", "wgrad_first_block", "bn
 class Config(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in (
         "n_way", "k_shot", "t_target", "channels", "height", "width", "filters", "num_stages",
-        "inner_steps", "per_step_bn", "max_tasks", "reserved", "norm_layer")]
+        "inner_steps", "per_step_bn", "max_tasks", "reserved", "norm_layer", "inner_bn")]
 
 
 class IterArgs(ctypes.Structure):
@@ -104,7 +104,7 @@ def load_library():
     lib.maml_b200_episode_gather.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, ctypes.POINTER(f32),
                                              ctypes.POINTER(f32), vp, vp, vp, vp, vp]
     lib.maml_b200_episode_gather.restype = ctypes.c_int
-    lib.maml_b200_adam_step.argtypes = [vp, vp, vp, vp, vp, f32, i32, u32, u32, vp]
+    lib.maml_b200_adam_step.argtypes = [vp, vp, vp, vp, vp, f32, i32, ctypes.c_uint64, ctypes.c_uint64, vp]
     lib.maml_b200_adam_step.restype = ctypes.c_int
     lib.maml_b200_running_stats_update.argtypes = [vp, vp, vp, vp, ctypes.POINTER(f32), vp]
     lib.maml_b200_running_stats_update.restype = ctypes.c_int
@@ -160,7 +160,8 @@ class Engine(object):
     """Owns one ``maml_b200_handle`` (one static task shape on the current CUDA device)."""
 
     def __init__(self, n_way, k_shot, t_target, channels, height, width, filters, num_stages, inner_steps,
-                 per_step_bn, max_tasks, keep_target_passes=False, force_fp32_convs=False, layer_norm=False):
+                 per_step_bn, max_tasks, keep_target_passes=False, force_fp32_convs=False, layer_norm=False,
+                 inner_bn=False):
         import torch
         if not torch.cuda.is_available():
             raise NativeLibraryError("the MAML engine needs a CUDA (sm_90a) device; there is no CPU fallback")
@@ -169,7 +170,7 @@ class Engine(object):
                           filters=filters, num_stages=num_stages, inner_steps=inner_steps,
                           per_step_bn=int(bool(per_step_bn)), max_tasks=max_tasks,
                           reserved=(1 if keep_target_passes else 0) | (2 if force_fp32_convs else 0),
-                          norm_layer=1 if layer_norm else 0)
+                          norm_layer=1 if layer_norm else 0, inner_bn=1 if inner_bn else 0)
         h = ctypes.c_void_p()
         _check(self.lib, self.lib.maml_b200_create(ctypes.byref(self.cfg), ctypes.byref(h)), "maml_b200_create")
         self.h = h

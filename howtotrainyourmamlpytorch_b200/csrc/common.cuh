@@ -202,32 +202,43 @@ struct HeadArgs {
 // ---------------------------------------------------------------------------------------------
 // parameter-space description (internal fast-weight layout)
 // ---------------------------------------------------------------------------------------------
+#define MAML_MAX_INNER_SEGS (4 * MAML_MAX_LAYERS + 2)
 struct ParamLayout {
-  int L, F, N, S, per_step_bn;
+  int L, F, N, S, per_step_bn;    // per_step_bn: per-step running statistics (rows of gamma / beta: per_step_gb)
   int cin[MAML_MAX_LAYERS];
   int pix;                        // pooled pixels of the last block (D = pix * F)
-  // internal (per task) fast-weight vector: W_l [9][cin][F], b_l [F], ..., Wfc [N][pix][F], bfc [N]
+  // internal (per task) fast-weight vector: W_l [9][cin][F], b_l [F], (beta_l [F], gamma_l [F]), ..., Wfc [N][pix][F], bfc [N]
   long long w_off[MAML_MAX_LAYERS], b_off[MAML_MAX_LAYERS], fcw_off, fcb_off, P;
   // reference-layout flat meta vector offsets
   long long m_w[MAML_MAX_LAYERS], m_b[MAML_MAX_LAYERS], m_beta[MAML_MAX_LAYERS], m_gamma[MAML_MAX_LAYERS];
-  long long m_fcw, m_fcb, m_lslr, meta_size;     // lslr: (2L+2) vectors of S+1
-  int nseg_inner;                 // 2L + 2 inner tensors
+  long long m_fcw, m_fcb, m_lslr, meta_size;     // lslr: nseg_inner vectors of S+1
+  int nseg_inner;                 // 2L + 2 inner tensors (4L + 2 with inner_bn), in the reference's inner-loop order
   // per inner segment: internal offset / size and number of gradient chunks in a partial buffer
-  long long seg_off[2 * MAML_MAX_LAYERS + 2];
-  long long seg_size[2 * MAML_MAX_LAYERS + 2];
+  long long seg_off[MAML_MAX_INNER_SEGS];
+  long long seg_size[MAML_MAX_INNER_SEGS];
   // layer norm (ln = 1; then per_step_bn = 0 and m_beta / m_gamma are unused): block l's bias [F][h_l][w_l] sits at m_lnb[l]
   // of the meta vector and at lnb_off[l] of a per-task bias-gradient row of lnb_off[L] floats
   int ln;
   long long m_lnb[MAML_MAX_LAYERS], lnb_off[MAML_MAX_LAYERS + 1];
+  // inner_bn (enable_inner_loop_optimizable_bn_params): block l's BatchNorm beta / gamma [F] are fast weights at
+  // beta_off[l] / gamma_off[l] (right after b_l), inner segments 4l + 2 / 4l + 3.  per_step_gb: the meta vector holds one
+  // gamma / beta row per inner step (per_step_bn without inner_bn), else one row
+  int inner_bn, per_step_gb;
+  long long beta_off[MAML_MAX_LAYERS], gamma_off[MAML_MAX_LAYERS];
 };
+// inner segments per block: conv.weight, conv.bias (+ norm_layer.bias, norm_layer.weight with inner_bn)
+__host__ __device__ __forceinline__ int seg_per_block(const ParamLayout& pl) { return pl.inner_bn ? 4 : 2; }
 
 enum { PR_UPDATE = 0, PR_STORE = 1, PR_SUB = 2 };
 
 struct PartialDesc {              // where each inner segment's gradient chunks live in a partial buffer
-  long long off[2 * MAML_MAX_LAYERS + 2];   // offset (floats) of chunk 0 inside the per-task partial block
-  long long cstride[2 * MAML_MAX_LAYERS + 2];
-  int nchunks[2 * MAML_MAX_LAYERS + 2];
+  long long off[MAML_MAX_INNER_SEGS];   // offset (floats) of chunk 0 inside the per-task partial block
+  long long cstride[MAML_MAX_INNER_SEGS];
+  int nchunks[MAML_MAX_INNER_SEGS];
   long long task_stride;
+  // segments without chunks (nchunks 0: inner-loop BatchNorm beta / gamma) read their gradient from the backward pass's fp64
+  // sums instead: block l's (S1, S2) = (dL/dbeta, dL/dgamma) pairs at bn_sums + task * bn_task_stride + l * bn_layer_stride
+  const double* bn_sums; long long bn_task_stride, bn_layer_stride;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -252,6 +263,13 @@ void launch_bnbwd_tan_reduce(const BnBwdTanArgs& a, cudaStream_t st);
 void launch_bnbwd_tan_apply(const BnBwdTanArgs& a, cudaStream_t st);
 void launch_bnbwd(const BnBwdArgs& a, cudaStream_t st);          // reduce + apply (one cluster kernel for small blocks)
 void launch_bnbwd_tan(const BnBwdTanArgs& a, cudaStream_t st);
+// inner-loop BatchNorm gamma / beta (fast weights, read per task: task t's at gamma / beta + t * gb_stride), always as the
+// unfused streaming kernels.  gdot / bdot: their tangents, same stride; the tangent backward adds r * gdot * (dy - S1/m -
+// zh * S2/m) to dzdot
+void launch_bnact_ibn(const BnActArgs& a, long long gb_stride, cudaStream_t st);
+void launch_bnbwd_ibn(const BnBwdArgs& a, long long gb_stride, cudaStream_t st);
+void launch_bnact_tan_ibn(const BnActTanArgs& a, long long gb_stride, const float* gdot, const float* bdot, cudaStream_t st);
+void launch_bnbwd_tan_ibn(const BnBwdTanArgs& a, long long gb_stride, const float* gdot, cudaStream_t st);
 // layer norm (kernels_bn.cu).  tan = false: primal forward / backward; true: their forward-mode tangents
 void launch_ln_stats(const LnArgs& a, bool tan, cudaStream_t st);   // per-image sums of z (or of zdot and zh * zdot)
 void launch_ln_act(const LnArgs& a, bool tan, cudaStream_t st);     // normalise, + bias, leaky-ReLU, max-pool (+ bdot)

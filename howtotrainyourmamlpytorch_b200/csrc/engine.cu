@@ -230,13 +230,18 @@ static void build_layout(maml_b200_handle* h) {
   pl.L = h->L; pl.F = h->F; pl.N = h->N; pl.S = h->S; pl.pix = h->pix;
   pl.ln = h->ln ? 1 : 0;
   pl.per_step_bn = h->ln ? 0 : h->cfg.per_step_bn;       // layer norm: no per-step parameters, no running statistics
+  // inner-loop gamma / beta are one [F] row each, whatever per_step_bn is (the running statistics stay per step)
+  pl.inner_bn = h->cfg.inner_bn ? 1 : 0;
+  pl.per_step_gb = pl.per_step_bn && !pl.inner_bn;
+  const int spb = seg_per_block(pl);
   long long o = 0, m = 0;
-  const long long bnsz = (long long)(pl.per_step_bn ? h->S : 1) * h->F;
+  const long long bnsz = (long long)(pl.per_step_gb ? h->S : 1) * h->F;
   for (int l = 0; l < h->L; ++l) {
     pl.cin[l] = h->geo[l].cin;
     const long long wsz = 9LL * pl.cin[l] * h->F;
     pl.w_off[l] = o; o += wsz;
     pl.b_off[l] = o; o += h->F;
+    if (pl.inner_bn) { pl.beta_off[l] = o; o += h->F; pl.gamma_off[l] = o; o += h->F; }
     pl.m_w[l] = m; h->seg_off.push_back(m); h->seg_size.push_back(wsz); m += wsz;
     pl.m_b[l] = m; h->seg_off.push_back(m); h->seg_size.push_back(h->F); m += h->F;
     if (h->ln) {
@@ -248,17 +253,21 @@ static void build_layout(maml_b200_handle* h) {
       pl.m_beta[l] = m; h->seg_off.push_back(m); h->seg_size.push_back(bnsz); m += bnsz;
       pl.m_gamma[l] = m; h->seg_off.push_back(m); h->seg_size.push_back(bnsz); m += bnsz;
     }
-    pl.seg_off[2 * l] = pl.w_off[l]; pl.seg_size[2 * l] = wsz;
-    pl.seg_off[2 * l + 1] = pl.b_off[l]; pl.seg_size[2 * l + 1] = h->F;
+    pl.seg_off[spb * l] = pl.w_off[l]; pl.seg_size[spb * l] = wsz;
+    pl.seg_off[spb * l + 1] = pl.b_off[l]; pl.seg_size[spb * l + 1] = h->F;
+    if (pl.inner_bn) {
+      pl.seg_off[spb * l + 2] = pl.beta_off[l]; pl.seg_size[spb * l + 2] = h->F;
+      pl.seg_off[spb * l + 3] = pl.gamma_off[l]; pl.seg_size[spb * l + 3] = h->F;
+    }
   }
   pl.fcw_off = o; o += (long long)h->N * h->D;
   pl.fcb_off = o; o += h->N;
   pl.P = o;
   pl.m_fcw = m; h->seg_off.push_back(m); h->seg_size.push_back((long long)h->N * h->D); m += (long long)h->N * h->D;
   pl.m_fcb = m; h->seg_off.push_back(m); h->seg_size.push_back(h->N); m += h->N;
-  pl.nseg_inner = 2 * h->L + 2;
-  pl.seg_off[2 * h->L] = pl.fcw_off; pl.seg_size[2 * h->L] = (long long)h->N * h->D;
-  pl.seg_off[2 * h->L + 1] = pl.fcb_off; pl.seg_size[2 * h->L + 1] = h->N;
+  pl.nseg_inner = spb * h->L + 2;
+  pl.seg_off[spb * h->L] = pl.fcw_off; pl.seg_size[spb * h->L] = (long long)h->N * h->D;
+  pl.seg_off[spb * h->L + 1] = pl.fcb_off; pl.seg_size[spb * h->L + 1] = h->N;
   pl.m_lslr = m;
   for (int k = 0; k < pl.nseg_inner; ++k) { h->seg_off.push_back(m); h->seg_size.push_back(h->S + 1); m += h->S + 1; }
   pl.meta_size = m;
@@ -267,7 +276,8 @@ static void build_layout(maml_b200_handle* h) {
 
 static void plan_chunks(maml_b200_handle* h, int n, ChunkPlan* cp) {
   long long off = 0;
-  memset(&cp->pd, 0, sizeof(cp->pd));
+  memset(&cp->pd, 0, sizeof(cp->pd));     // inner-loop beta / gamma segments have no chunks (nchunks 0)
+  const int spb = seg_per_block(h->pl);
   for (int l = 0; l < h->L; ++l) {
     const long long rows = (long long)n * h->geo[l].G;
     int nch, rpc;
@@ -288,16 +298,16 @@ static void plan_chunks(maml_b200_handle* h, int n, ChunkPlan* cp) {
     nch = (int)((rows + rpc - 1) / rpc);
     cp->rows_per_chunk[l] = rpc; cp->nchunks[l] = nch;
     const long long cs = 9LL * h->geo[l].cin * h->F + h->F;
-    cp->pd.off[2 * l] = off; cp->pd.cstride[2 * l] = cs; cp->pd.nchunks[2 * l] = nch;
-    cp->pd.off[2 * l + 1] = off + 9LL * h->geo[l].cin * h->F; cp->pd.cstride[2 * l + 1] = cs; cp->pd.nchunks[2 * l + 1] = nch;
+    cp->pd.off[spb * l] = off; cp->pd.cstride[spb * l] = cs; cp->pd.nchunks[spb * l] = nch;
+    cp->pd.off[spb * l + 1] = off + 9LL * h->geo[l].cin * h->F; cp->pd.cstride[spb * l + 1] = cs; cp->pd.nchunks[spb * l + 1] = nch;
     off += cs * nch;
   }
   // head: one gradient chunk per row group of the batch (gW [N][D] followed by gb [N] inside each chunk)
   const int hg = (n + head_rows(n) - 1) / head_rows(n);
   const long long hcs = (long long)h->N * h->D + h->N;
   cp->head_groups = hg;
-  cp->pd.off[2 * h->L] = off; cp->pd.cstride[2 * h->L] = hcs; cp->pd.nchunks[2 * h->L] = hg;
-  cp->pd.off[2 * h->L + 1] = off + (long long)h->N * h->D; cp->pd.cstride[2 * h->L + 1] = hcs; cp->pd.nchunks[2 * h->L + 1] = hg;
+  cp->pd.off[spb * h->L] = off; cp->pd.cstride[spb * h->L] = hcs; cp->pd.nchunks[spb * h->L] = hg;
+  cp->pd.off[spb * h->L + 1] = off + (long long)h->N * h->D; cp->pd.cstride[spb * h->L + 1] = hcs; cp->pd.nchunks[spb * h->L + 1] = hg;
   off += hcs * hg;
   cp->size = rup(off, 64);
   cp->pd.task_stride = cp->size;
@@ -442,6 +452,8 @@ extern "C" int maml_b200_create(const maml_b200_config* cfg, maml_b200_handle** 
   if (cfg->channels < 1 || cfg->channels > 4) return fail("channels must be in [1, 4]");
   if (cfg->max_tasks < 1) return fail("max_tasks must be >= 1");
   if (cfg->norm_layer != 0 && cfg->norm_layer != 1) return fail("norm_layer must be 0 (batch norm) or 1 (layer norm)");
+  if (cfg->inner_bn != 0 && cfg->inner_bn != 1) return fail("inner_bn must be 0 or 1");
+  if (cfg->inner_bn && cfg->norm_layer == 1) return fail("inner_bn (inner-loop BatchNorm gamma / beta) needs norm_layer 0 (batch norm)");
   if (cfg->n_way < 2 || cfg->n_way > 32) return fail("n_way must be in [2, 32]");
   const int n_s = cfg->n_way * cfg->k_shot, n_t = cfg->n_way * cfg->t_target;
   if (n_s < 1 || n_t < 1 || n_s > 128 || n_t > 128) return fail("N*K and N*T must be in [1, 128]");
@@ -589,10 +601,17 @@ static float* lnb_at(const maml_b200_handle* h, int kind, int step) {
 }
 
 static const float* gamma_at(const maml_b200_handle* h, const float* meta, int l, int step) {
-  return meta + h->pl.m_gamma[l] + (h->cfg.per_step_bn ? (long long)step * h->F : 0);
+  return meta + h->pl.m_gamma[l] + (h->pl.per_step_gb ? (long long)step * h->F : 0);
 }
 static const float* beta_at(const maml_b200_handle* h, const float* meta, int l, int step) {
-  return meta + h->pl.m_beta[l] + (h->cfg.per_step_bn ? (long long)step * h->F : 0);
+  return meta + h->pl.m_beta[l] + (h->pl.per_step_gb ? (long long)step * h->F : 0);
+}
+// BatchNorm gamma / beta of block l for a pass at inner step `step`: the meta vector's row, shared by the tasks (stride 0),
+// or with inner_bn the fast weights `theta` (per task, stride Ppad)
+struct NormParams { const float* gamma; const float* beta; long long stride; };
+static NormParams norm_params(const maml_b200_handle* h, const float* meta, const float* theta, int l, int step) {
+  if (h->pl.inner_bn) return NormParams{theta + h->pl.gamma_off[l], theta + h->pl.beta_off[l], h->Ppad};
+  return NormParams{gamma_at(h, meta, l, step), beta_at(h, meta, l, step), 0};
 }
 
 struct Slot { const PassSet* ps; int slot; };
@@ -642,6 +661,7 @@ struct ReduceSpec {
   const float* theta_in; float* theta_out; float* g_out; float* tbar;
   int step;
   int pack_step;                  // >= 0: re-pack theta[pack_step] for the tensor-core convs afterwards
+  const double* bn_sums = nullptr;  // inner_bn: the pass's backward sums (kind, step, block 0, task 0), the beta / gamma gradient
 };
 
 static void pack_theta_step(maml_b200_handle* h, int step, int T, cudaStream_t st);
@@ -650,10 +670,19 @@ static void pack_theta_step(maml_b200_handle* h, int step, int T, cudaStream_t s
 // much earlier.  So the reduction (+ LSLR update + tensor-core weight packing) of blocks >= 1 and the linear layer runs
 // on the wgrad side stream while the main chain finishes block 0; only the 9*C*F + F first-block values are reduced on
 // the critical path.  The main chain joins the side stream lazily (join_pending) before block 1 needs those weights.
+// The partial-buffer description of a reduction: inner-loop beta / gamma read the pass's backward sums.
+static PartialDesc with_bn_sums(const maml_b200_handle* h, const PartialDesc& pd, const double* bn_sums) {
+  PartialDesc d = pd;
+  d.bn_sums = bn_sums; d.bn_task_stride = h->stats_task_stride; d.bn_layer_stride = h->st_layer_stride;
+  return d;
+}
+
 static void reduce_upper_on_side(maml_b200_handle* h, const ReduceSpec& rs, const PartialDesc& pd, const float* partial,
                                  const float* meta, int T) {
-  launch_param_reduce(h->pl, pd, partial, rs.mode, rs.theta_in, rs.theta_out, rs.g_out, rs.tbar, meta, rs.step, h->Ppad, T,
-                      h->s_wg, 2, -1);
+  // the first block's tensors (seg_per_block segments: with inner_bn its beta / gamma too, whose sums the main chain
+  // finishes last) are reduced on the main chain by reduce_lower
+  launch_param_reduce(h->pl, with_bn_sums(h, pd, rs.bn_sums), partial, rs.mode, rs.theta_in, rs.theta_out, rs.g_out, rs.tbar,
+                      meta, rs.step, h->Ppad, T, h->s_wg, seg_per_block(h->pl), -1);
   if (rs.pack_step >= 0) pack_theta_step(h, rs.pack_step, T, h->s_wg);
   cudaEventRecord(h->ev_wg, h->s_wg);
   h->wg_pending = true;
@@ -661,8 +690,8 @@ static void reduce_upper_on_side(maml_b200_handle* h, const ReduceSpec& rs, cons
 
 static void reduce_lower(maml_b200_handle* h, const ReduceSpec& rs, const PartialDesc& pd, const float* partial,
                          const float* meta, int T, cudaStream_t st) {
-  launch_param_reduce(h->pl, pd, partial, rs.mode, rs.theta_in, rs.theta_out, rs.g_out, rs.tbar, meta, rs.step, h->Ppad, T,
-                      st, 0, 2);
+  launch_param_reduce(h->pl, with_bn_sums(h, pd, rs.bn_sums), partial, rs.mode, rs.theta_in, rs.theta_out, rs.g_out, rs.tbar,
+                      meta, rs.step, h->Ppad, T, st, 0, seg_per_block(h->pl));
 }
 static void join_pending(maml_b200_handle* h, cudaStream_t st) {
   if (!h->wg_pending) return;
@@ -729,7 +758,8 @@ static WgradArgs wgrad_args(const maml_b200_handle* h, int l, int n, const Chunk
   WgradArgs w{};
   w.kc = l == 0 ? h->C : h->F; w.ncols = h->F; w.rows = n * g.G; w.gw = g.gw;
   w.rows_per_chunk = cp.rows_per_chunk[l]; w.nchunks = cp.nchunks[l];
-  w.partial = partial + cp.pd.off[2 * l]; w.partial_task_stride = cp.pd.task_stride; w.chunk_stride = cp.pd.cstride[2 * l];
+  const int k = seg_per_block(h->pl) * l;
+  w.partial = partial + cp.pd.off[k]; w.partial_task_stride = cp.pd.task_stride; w.chunk_stride = cp.pd.cstride[k];
   w.tasks = T;
   return w;
 }
@@ -772,13 +802,14 @@ static HeadArgs head_args(const maml_b200_handle* h, int mode, const PassSet& ps
 
 // the head's gradient goes to the linear layer's chunks (one per row group) of the partial buffer `partial`
 static void head_grad(const maml_b200_handle* h, HeadArgs& a, float* partial, const ChunkPlan& cp) {
-  a.gW = partial + cp.pd.off[2 * h->L]; a.gb = partial + cp.pd.off[2 * h->L + 1];
-  a.g_stride = cp.pd.task_stride; a.g_chunk_stride = cp.pd.cstride[2 * h->L];
+  const int k = seg_per_block(h->pl) * h->L;
+  a.gW = partial + cp.pd.off[k]; a.gb = partial + cp.pd.off[k + 1];
+  a.g_stride = cp.pd.task_stride; a.g_chunk_stride = cp.pd.cstride[k];
 }
 
 // the last block of the support batch, the head and that block's BatchNorm backward run as one kernel
 static bool support_tail_fused(const maml_b200_handle* h) {
-  return h->opt.tail_fuse && !h->ln && tail_fusable(bn_geom(h, h->L - 1, h->n_s), h->n_s, head_rows(h->n_s));
+  return h->opt.tail_fuse && !h->ln && !h->pl.inner_bn && tail_fusable(bn_geom(h, h->L - 1, h->n_s), h->n_s, head_rows(h->n_s));
 }
 
 enum { CLR_STATS = 1, CLR_ABAR = 2, CLR_LOSSES = 4, CLR_CORRECT = 8, CLR_BWD_STATS = 16 };
@@ -807,8 +838,8 @@ static int clear_accumulators(maml_b200_handle* h, unsigned what, cudaStream_t s
 
 // The normalisation (+ leaky-ReLU + max-pool) of block l in each kind of pass, BatchNorm or layer norm.  defer_last: the
 // last block's BatchNorm is not launched but returned; fused_head: it runs in the fused last-block kernel.
-static void norm_forward(maml_b200_handle* h, const PassSet& ps, int slot, const float* meta, int l, int step, int stat_kind,
-                         int T, cudaStream_t st, BnActArgs* defer_last) {
+static void norm_forward(maml_b200_handle* h, const PassSet& ps, int slot, const float* theta, const float* meta, int l, int step,
+                         int stat_kind, int T, cudaStream_t st, BnActArgs* defer_last) {
   if (h->ln) {                   // per-image sums of z, then normalise / bias / leaky-ReLU / pool
     LnArgs a = ln_args(h, l, ps.n, meta, T);
     a.z = ZH(ps, l, slot); a.z_stride = STRIDE(ps, zh, l);
@@ -822,16 +853,18 @@ static void norm_forward(maml_b200_handle* h, const PassSet& ps, int slot, const
   BnActArgs b{};
   b.z = ZH(ps, l, slot); b.z_stride = STRIDE(ps, zh, l);
   b.stats = stat_at(h, stat_kind, step, l); b.stats_stride = h->stats_task_stride;
-  b.gamma = gamma_at(h, meta, l, step); b.beta = beta_at(h, meta, l, step);
+  const NormParams np = norm_params(h, meta, theta, l, step);
+  b.gamma = np.gamma; b.beta = np.beta;
   b.p = AIN(ps, l + 1, slot); b.p_stride = STRIDE(ps, ain, l + 1);
   if (h->use_tc && l + 1 < h->L) { b.p_hi = AIN_HI(ps, l + 1, slot); b.p_lo = AIN_LO(ps, l + 1, slot); }
   b.g = bn_geom(h, l, ps.n); b.tasks = T;
   if (defer_last && l == h->L - 1) *defer_last = b;
+  else if (np.stride) launch_bnact_ibn(b, np.stride, st);
   else launch_bnact(b, st);
 }
 
-static void norm_backward(maml_b200_handle* h, const PassSet& ps, int slot, const float* meta, int l, int step, int kind_fwd,
-                          int kind_bwd, int T, cudaStream_t st, const BnActArgs* fused_act, const HeadArgs* fused_head) {
+static void norm_backward(maml_b200_handle* h, const PassSet& ps, int slot, const float* theta, const float* meta, int l, int step,
+                          int kind_fwd, int kind_bwd, int T, cudaStream_t st, const BnActArgs* fused_act, const HeadArgs* fused_head) {
   if (h->ln) {
     LnArgs a = ln_args(h, l, ps.n, meta, T);
     a.dp = DP(ps, l, slot); a.dp_stride = STRIDE(ps, dp, l);
@@ -851,16 +884,19 @@ static void norm_backward(maml_b200_handle* h, const PassSet& ps, int slot, cons
   b.zh = ZH(ps, l, slot); b.zh_stride = STRIDE(ps, zh, l);
   b.stats_fwd = stat_at(h, kind_fwd, step, l); b.stats_fwd_stride = h->stats_task_stride;
   b.stats_bwd = stat_at(h, kind_bwd, step, l); b.stats_bwd_stride = h->stats_task_stride;
-  b.gamma = gamma_at(h, meta, l, step); b.beta = beta_at(h, meta, l, step);
+  const NormParams np = norm_params(h, meta, theta, l, step);
+  b.gamma = np.gamma; b.beta = np.beta;
   b.dz = DZ(ps, l, slot); b.dz_stride = STRIDE(ps, dz, l);
   if (h->use_tc && l >= 1) { b.dz_hi = DZ_HI(ps, l, slot); b.dz_lo = DZ_LO(ps, l, slot); }
   b.g = bn_geom(h, l, ps.n); b.tasks = T;
   if (fused_head && l == h->L - 1) launch_tail_fused(*fused_act, *fused_head, b, st);
+  else if (np.stride) launch_bnbwd_ibn(b, np.stride, st);
   else launch_bnbwd(b, st);
 }
 
-static void norm_tangent_forward(maml_b200_handle* h, int s, const float* meta, int l, const float* t_norm, long long t_stride,
-                                 int T, cudaStream_t st, BnActTanArgs* defer_last) {
+// inner_bn: gamma / beta are theta's and their tangents u's (per task); t_norm is then not read
+static void norm_tangent_forward(maml_b200_handle* h, int s, const float* theta, const float* u, const float* meta, int l,
+                                 const float* t_norm, long long t_stride, int T, cudaStream_t st, BnActTanArgs* defer_last) {
   const PassSet& sp = h->sup; const PassSet& tn = h->tan; const PassSet& t2 = h->tan2;
   if (h->ln) {                   // zdot (+ the side stream's addend) -> per-image sums -> zhdot, pdot
     LnArgs a = ln_args(h, l, sp.n, meta, T);
@@ -881,16 +917,18 @@ static void norm_tangent_forward(maml_b200_handle* h, int s, const float* meta, 
   b.zh = ZH(sp, l, s); b.zh_stride = STRIDE(sp, zh, l);
   b.stats_fwd = stat_at(h, PASS_SUP_FWD, s, l); b.stats_fwd_stride = h->stats_task_stride;
   b.stats_tan = stat_at(h, PASS_TAN_FWD, s, l); b.stats_tan_stride = h->stats_task_stride;
-  b.gamma = gamma_at(h, meta, l, s); b.beta = beta_at(h, meta, l, s);
+  const NormParams np = norm_params(h, meta, theta, l, s);
+  b.gamma = np.gamma; b.beta = np.beta;
   b.pdot = AIN(tn, l + 1, 0); b.pdot_stride = STRIDE(tn, ain, l + 1);
   if (h->use_tc && l + 1 < h->L) { b.pdot_hi = AIN_HI(tn, l + 1, 0); b.pdot_lo = AIN_LO(tn, l + 1, 0); }
   b.g = bn_geom(h, l, sp.n); b.tasks = T;
   if (defer_last && l == h->L - 1) *defer_last = b;
+  else if (np.stride) launch_bnact_tan_ibn(b, np.stride, u + h->pl.gamma_off[l], u + h->pl.beta_off[l], st);
   else launch_bnact_tan(b, st, t_norm ? gamma_at(h, t_norm, l, s) : nullptr, t_norm ? beta_at(h, t_norm, l, s) : nullptr);
 }
 
-static void norm_tangent_backward(maml_b200_handle* h, int s, const float* meta, int l, int kind_tbwd, int T, cudaStream_t st,
-                                  const BnActTanArgs* fused_act, const HeadArgs* fused_head) {
+static void norm_tangent_backward(maml_b200_handle* h, int s, const float* theta, const float* u, const float* meta, int l,
+                                  int kind_tbwd, int T, cudaStream_t st, const BnActTanArgs* fused_act, const HeadArgs* fused_head) {
   const PassSet& sp = h->sup; const PassSet& tn = h->tan; const PassSet& t2 = h->tan2;
   if (h->ln) {
     LnArgs a = ln_args(h, l, sp.n, meta, T);
@@ -923,11 +961,13 @@ static void norm_tangent_backward(maml_b200_handle* h, int s, const float* meta,
   b.stats_bwd = stat_at(h, PASS_SUP_BWD, s, l); b.stats_bwd_stride = h->stats_task_stride;
   b.stats_tan = stat_at(h, PASS_TAN_FWD, s, l); b.stats_tan_stride = h->stats_task_stride;
   b.stats_tbwd = stat_at(h, kind_tbwd, s, l); b.stats_tbwd_stride = h->stats_task_stride;
-  b.gamma = gamma_at(h, meta, l, s); b.beta = beta_at(h, meta, l, s);
+  const NormParams np = norm_params(h, meta, theta, l, s);
+  b.gamma = np.gamma; b.beta = np.beta;
   b.dzdot = DZ(tn, l, 0); b.dzdot_stride = STRIDE(tn, dz, l);
   if (h->use_tc && l >= 1) { b.dzdot_hi = DZ_HI(tn, l, 0); b.dzdot_lo = DZ_LO(tn, l, 0); }
   b.g = bn_geom(h, l, sp.n); b.tasks = T;
   if (fused_head && l == h->L - 1) launch_tail_tan_fused(*fused_act, *fused_head, b, st);
+  else if (np.stride) launch_bnbwd_tan_ibn(b, np.stride, u + h->pl.gamma_off[l], st);
   else launch_bnbwd_tan(b, st);
 }
 
@@ -951,7 +991,7 @@ static void forward_pass(maml_b200_handle* h, const PassSet& ps, int slot, const
       a.stats = stat_at(h, stat_kind, bn_step, l);
       launch_conv_rows(a, st);
     }
-    norm_forward(h, ps, slot, meta, l, bn_step, stat_kind, T, st, defer_last);
+    norm_forward(h, ps, slot, theta, meta, l, bn_step, stat_kind, T, st, defer_last);
   }
 }
 
@@ -966,7 +1006,7 @@ static void backward_pass(maml_b200_handle* h, const PassSet& ps, int slot, cons
   cudaStream_t wst = fork_wgrad ? h->s_wg : st;
   const bool split = fork_wgrad && rs != nullptr;
   for (int l = h->L - 1; l >= 0; --l) {
-    norm_backward(h, ps, slot, meta, l, bn_step, kind_fwd, kind_bwd, T, st, fused_act, fused_head);
+    norm_backward(h, ps, slot, theta, meta, l, bn_step, kind_fwd, kind_bwd, T, st, fused_act, fused_head);
     if (fork_wgrad) { cudaEventRecord(h->ev_fork, st); cudaStreamWaitEvent(h->s_wg, h->ev_fork, 0); }
 
     if (l == 0) {
@@ -1076,7 +1116,7 @@ static void tangent_forward(maml_b200_handle* h, int s, const float* theta, cons
       a.stats = stat_at(h, PASS_TAN_FWD, s, l);
       launch_conv_rows(a, st);
     }
-    norm_tangent_forward(h, s, meta, l, t_norm, t_stride, T, st, defer_last);
+    norm_tangent_forward(h, s, theta, u, meta, l, t_norm, t_stride, T, st, defer_last);
   }
 }
 
@@ -1098,7 +1138,7 @@ static void tangent_pass(maml_b200_handle* h, int s, const float* theta, const f
   if (!fuse_tail) launch_head(hd, st);
   for (int l = h->L - 1; l >= 0; --l) {
     if (h->use_tc && l + 1 < h->L) cudaStreamWaitEvent(st, h->ev_pre[MAML_MAX_LAYERS + l + 1], 0);
-    norm_tangent_backward(h, s, meta, l, th.kind_tbwd, T, st, &last_act, fuse_tail ? &hd : nullptr);
+    norm_tangent_backward(h, s, theta, u, meta, l, th.kind_tbwd, T, st, &last_act, fuse_tail ? &hd : nullptr);
     cudaEventRecord(h->ev_fork, st); cudaStreamWaitEvent(h->s_wg, h->ev_fork, 0);
 
     if (l == 0) {
@@ -1224,7 +1264,7 @@ static int enqueue_iteration(maml_b200_handle* h, const maml_b200_iter_args* it,
     if (!fuse_tail) launch_head(hd, st);
     // LSLR update theta^{s+1} = theta^s - alpha[.][s] * g and the tensor-core packs of theta^{s+1}: blocks >= 1 and the
     // linear layer on the side stream, block 0 at the end of the main chain
-    ReduceSpec rs{PR_UPDATE, th, th_next, h->g + (long long)s * TP, nullptr, s, s + 1};
+    ReduceSpec rs{PR_UPDATE, th, th_next, h->g + (long long)s * TP, nullptr, s, s + 1, stat_at(h, PASS_SUP_BWD, s, 0)};
     backward_pass(h, h->sup, s, th, s, meta, s, PASS_SUP_FWD, PASS_SUP_BWD, h->sup_partial, h->plan_sup, T, st, true, &rs,
                   fuse_tail ? &last_act : nullptr, fuse_tail ? &hd : nullptr);
     if (mask & (1u << s)) {
@@ -1252,8 +1292,8 @@ static int enqueue_iteration(maml_b200_handle* h, const maml_b200_iter_args* it,
         head_grad(h, bqa, tpart, h->plan_tgt);
         launch_head(bqa, ts_);
         backward_pass(h, h->tgt, ts, th_next, s + 1, meta, s, PASS_TGT_FWD, PASS_TGT_BWD, tpart, h->plan_tgt, T, ts_, false);
-        launch_param_reduce(h->pl, h->plan_tgt.pd, tpart, PR_STORE, nullptr, nullptr, h->tgrad + (long long)s * TP, nullptr,
-                            meta, s, h->Ppad, T, ts_);
+        launch_param_reduce(h->pl, with_bn_sums(h, h->plan_tgt.pd, stat_at(h, PASS_TGT_BWD, s, 0)), tpart, PR_STORE, nullptr,
+                            nullptr, h->tgrad + (long long)s * TP, nullptr, meta, s, h->Ppad, T, ts_);
       }
       CK(cudaEventRecord(h->ev_tgt[s], ts_));
     }
@@ -1271,7 +1311,7 @@ static int enqueue_iteration(maml_b200_handle* h, const maml_b200_iter_args* it,
       if (it->second_order) {
         cudaStream_t spre;
         if (fork_direction(h, T, st, &spre)) return 1;
-        ReduceSpec rs{PR_SUB, nullptr, nullptr, nullptr, h->tbar, s, -1};
+        ReduceSpec rs{PR_SUB, nullptr, nullptr, nullptr, h->tbar, s, -1, stat_at(h, PASS_TAN_BWD, s, 0)};
         tangent_pass(h, s, th, h->u, meta, TangentHead{HEAD_TANGENT, ys, nullptr, 0, nullptr, PASS_TAN_BWD}, T, st, rs, spre);
       }
     }
@@ -1356,6 +1396,7 @@ extern "C" int maml_b200_meta_batch_fwd_bwd(maml_b200_handle* h, const maml_b200
 // Argument checks of the functional entries; `ptrs`: the entry's required pointers are all non-null.
 static int check_call(const maml_b200_handle* h, bool ptrs, int n_tasks, int num_step) {
   if (!h || !ptrs) return fail("null argument");
+  if (h->pl.inner_bn) return fail("the functional entries (maml_b200_net_*) do not run inner_bn handles yet");
   if (n_tasks < 1 || n_tasks > h->maxT) return fail("n_tasks out of range");
   if (num_step < 0 || num_step >= h->S) return fail("num_step out of range");
   return 0;
@@ -1635,7 +1676,7 @@ extern "C" int maml_b200_net_running_update(maml_b200_handle* h, int32_t n_tasks
 }
 
 extern "C" int maml_b200_adam_step(maml_b200_handle* h, float* meta, const float* grad, float* exp_avg, float* exp_avg_sq,
-                                   float lr, int32_t step, uint32_t trainable_mask, uint32_t clamp_mask, void* stream) {
+                                   float lr, int32_t step, uint64_t trainable_mask, uint64_t clamp_mask, void* stream) {
   if (!h || !meta || !grad || !exp_avg || !exp_avg_sq) return fail("null argument");
   if (step < 1) return fail("step must be >= 1");
   LaunchScope launch_scope(h);
@@ -1643,8 +1684,15 @@ extern "C" int maml_b200_adam_step(maml_b200_handle* h, float* meta, const float
   for (size_t k = 0; k < h->seg_off.size(); ++k) ends.push_back(h->seg_off[k] + h->seg_size[k]);
   const float bc1 = (float)(1.0 - pow(0.9, (double)step));
   const float bc2 = (float)(1.0 - pow(0.999, (double)step));
-  launch_adam(meta, grad, exp_avg, exp_avg_sq, h->pl.meta_size, lr, bc1, bc2, ends.data(), (int)ends.size(), trainable_mask,
-              clamp_mask, (cudaStream_t)stream);
+  // one launch per 32 segments (the kernel's segment table and masks): an inner_bn handle with 4 blocks has 36
+  for (size_t k0 = 0; k0 < ends.size(); k0 += 32) {
+    const size_t nk = std::min<size_t>(32, ends.size() - k0);
+    const long long base = k0 ? ends[k0 - 1] : 0;
+    std::vector<long long> rel(nk);
+    for (size_t k = 0; k < nk; ++k) rel[k] = ends[k0 + k] - base;
+    launch_adam(meta + base, grad + base, exp_avg + base, exp_avg_sq + base, rel[nk - 1], lr, bc1, bc2, rel.data(), (int)nk,
+                (uint32_t)(trainable_mask >> k0), (uint32_t)(clamp_mask >> k0), (cudaStream_t)stream);
+  }
   CK(cudaGetLastError());
   return 0;
 }

@@ -655,18 +655,37 @@ void launch_bnbwd_tan_reduce(const BnBwdTanArgs& a, cudaStream_t st) {
 }
 
 // ------------------------------------------------------------------------------- tangent backward: apply
+// bn_tan_bwd_dz plus the gamma-tangent term: dzdot = -r q dz + r gamma (dydot - T1/m - zhdot S2/m - zh T2/m)
+//                                                 + r gdot (dy - S1/m - zh S2/m),   rgd = r * gdot, c1 = S1/m
+// dy and dydot reach only the arg-max of a full window
+__device__ __forceinline__ float4 bn_tan_bwd_dz_gd(const float4& rq, const float4& dz, const float4& rg, const float4& t1,
+                                                   const float4& zhd, const float4& c2, const float4& zh, const float4& t2, int k,
+                                                   const int4& arg, const float4& dyd, const float4& rgd, const float4& c1,
+                                                   const float4& dy, bool full) {
+  const float4 base = bn_tan_bwd_dz(rq, dz, rg, t1, zhd, c2, zh, t2, k, arg, dyd, full);
+  return map4([k, full](float b, float rgd, float c1, float zh, float c2, int arg, float dy) {
+    return b + rgd * (((full && arg == k) ? dy : 0.f) - c1 - zh * c2);
+  }, base, rgd, c1, zh, c2, arg, dy);
+}
+
 // dzdot = -r*q*dz + r*gamma*(dydot - T1/m - zhdot*S2/m - zh*T2/m)
+// GD (inner-loop gamma / beta, s_gd = gdot, s_c1 = S1/m): + r*gdot*(dy - S1/m - zh*S2/m), dy from the primal dp
+template <bool GD = false>
 __device__ __forceinline__ void bnbwd_tan_apply_phase(const BnBwdTanArgs& a, const BnGeom& g, int task, int cta, int ncta,
                                                       const WinIter& it, const float* s_r, const float* s_g, const float* s_b,
-                                                      const float* s_q, const float* s_c2, const float* s_t1, const float* s_t2) {
+                                                      const float* s_q, const float* s_c2, const float* s_t1, const float* s_t2,
+                                                      const float* s_gd = nullptr, const float* s_c1 = nullptr) {
   if (it.lane >= it.WPB) return;
   const float4 r = ld4s(s_r, it.q), ga = ld4s(s_g, it.q), be = ld4s(s_b, it.q);
   const float4 qq = ld4s(s_q, it.q), c2 = ld4s(s_c2, it.q), t1 = ld4s(s_t1, it.q), t2 = ld4s(s_t2, it.q);
+  float4 c1 = make_float4(0.f, 0.f, 0.f, 0.f), rgd = c1;
+  if constexpr (GD) { c1 = ld4s(s_c1, it.q); rgd = mul4(r, ld4s(s_gd, it.q)); }
   const float4 rg = mul4(r, ga);
   const float4 rq = make_float4(-r.x * qq.x, -r.y * qq.y, -r.z * qq.z, -r.w * qq.w);
   const float* zhp = a.zh + (long long)task * a.zh_stride;
   const float* zhd = a.zhdot + (long long)task * a.zhdot_stride;
   const float* dzp = a.dz + (long long)task * a.dz_stride;
+  const float* dpp = a.dp + (long long)task * a.dp_stride;
   const float* dpd = a.dpdot + (long long)task * a.dpdot_stride;
   const float* dpd2 = a.dpdot2 ? a.dpdot2 + (long long)task * a.dpdot_stride : nullptr;
   float* dzd = a.dzdot + (long long)task * a.dzdot_stride;
@@ -674,11 +693,13 @@ __device__ __forceinline__ void bnbwd_tan_apply_phase(const BnBwdTanArgs& a, con
     int img, wy, wx; it.window(wi, img, wy, wx);
     const bool full = (wy < g.ph && wx < g.pw);
     int4 arg = make_int4(-1, -1, -1, -1);
-    float4 dyd = make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 dyd = make_float4(0.f, 0.f, 0.f, 0.f), dy = dyd;
     if (full) {
       float4 zh[4]; long long idx[4]; float4 sl;
       argmax_window(zhp, g, img, wy, wx, it, ga, [&](int, int) { return be; }, zh, idx, arg, sl);
-      dyd = mul4(ld4_sum(dpd, dpd2, it.pooled(g, img, wy, wx)), sl);
+      const long long pidx = it.pooled(g, img, wy, wx);
+      dyd = mul4(ld4_sum(dpd, dpd2, pidx), sl);
+      if constexpr (GD) dy = mul4(ld4(dpp + pidx), sl);
     }
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
@@ -686,7 +707,9 @@ __device__ __forceinline__ void bnbwd_tan_apply_phase(const BnBwdTanArgs& a, con
       if (yy < g.h && xx < g.w) {
         const long long idx = it.grid(g, img, yy, xx);
         const float4 zh = ld4(zhp + idx), zd = ld4(zhd + idx), dzv = ld4(dzp + idx);
-        const float4 o = bn_tan_bwd_dz(rq, dzv, rg, t1, zd, c2, zh, t2, k, arg, dyd);
+        float4 o;
+        if constexpr (GD) o = bn_tan_bwd_dz_gd(rq, dzv, rg, t1, zd, c2, zh, t2, k, arg, dyd, rgd, c1, dy, full);
+        else o = bn_tan_bwd_dz(rq, dzv, rg, t1, zd, c2, zh, t2, k, arg, dyd);
         st4(dzd + idx, o);
         if (a.dzdot_hi) st4_split(a.dzdot_hi + (long long)task * a.dzdot_stride, a.dzdot_lo + (long long)task * a.dzdot_stride, idx, o);
       }
@@ -753,6 +776,154 @@ void launch_bnbwd_tan(const BnBwdTanArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
   int block; bn_grid(a.g, a.tasks, &block);
   launch_cluster(bnbwd_tan_fused_kernel, tagged(a), cl, a.tasks, block, st);
+  CUDA_CHECK_LAUNCH();
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Inner-loop gamma / beta (enable_inner_loop_optimizable_bn_params): gamma and beta are fast weights, so every task has its
+// own pair, at gamma / beta + task * gbs (gbs: the fast-weight vectors' stride).  The kernels below run the streaming
+// phases above with the task's pair; the tangent backward adds the one term that shared gamma / beta do not have.  Handles
+// without the flag never launch them.
+__device__ __forceinline__ void ibn_load(const float* __restrict__ src, long long gbs, int task, int F, float* s) {
+  if (threadIdx.x < F) s[threadIdx.x] = src[(long long)task * gbs + threadIdx.x];
+}
+
+__global__ void __launch_bounds__(256) bnact_ibn_kernel(BnActArgs a, long long gbs) {
+  pdl_prologue(43, a.tag);
+  __shared__ float s_mu[64], s_r[64], s_g[64], s_b[64];
+  const BnGeom g = a.g;
+  const int task = blockIdx.y;
+  chan_setup(a.stats + (long long)task * a.stats_stride, a.gamma + (long long)task * gbs, a.beta + (long long)task * gbs,
+             (double)g.n * g.h * g.w, g.F, s_mu, s_r, s_g, s_b);
+  __syncthreads();
+  WinIter it(g);
+  bnact_phase(a, g, task, blockIdx.x, gridDim.x, it, s_mu, s_r, s_g, s_b);
+}
+
+__global__ void __launch_bounds__(256) bnbwd_reduce_ibn_kernel(BnBwdArgs a, long long gbs) {
+  pdl_prologue(44, a.tag);
+  __shared__ float s_g[64], s_b[64];
+  const BnGeom g = a.g;
+  const int task = blockIdx.y;
+  ibn_load(a.gamma, gbs, task, g.F, s_g);
+  ibn_load(a.beta, gbs, task, g.F, s_b);
+  __syncthreads();
+  WinIter it(g);
+  double s1[4] = {0, 0, 0, 0}, s2[4] = {0, 0, 0, 0};
+  bnbwd_reduce_phase(a, g, task, blockIdx.x, gridDim.x, it, s_g, s_b, s1, s2);
+  block_reduce_stats(s1, s2, it, a.stats_bwd + (long long)task * a.stats_bwd_stride, g.F);
+}
+
+__global__ void __launch_bounds__(256) bnbwd_apply_ibn_kernel(BnBwdArgs a, long long gbs) {
+  pdl_prologue(45, a.tag);
+  __shared__ float s_mu[64], s_r[64], s_g[64], s_b[64], s_c1[64], s_c2[64];
+  const BnGeom g = a.g;
+  const int task = blockIdx.y;
+  const double m = (double)g.n * g.h * g.w;
+  chan_setup(a.stats_fwd + (long long)task * a.stats_fwd_stride, a.gamma + (long long)task * gbs, a.beta + (long long)task * gbs,
+             m, g.F, s_mu, s_r, s_g, s_b);
+  if (threadIdx.x < g.F) {
+    const double* sb = a.stats_bwd + (long long)task * a.stats_bwd_stride;
+    s_c1[threadIdx.x] = (float)(sb[threadIdx.x * 2] / m);
+    s_c2[threadIdx.x] = (float)(sb[threadIdx.x * 2 + 1] / m);
+  }
+  __syncthreads();
+  WinIter it(g);
+  bnbwd_apply_phase(a, g, task, blockIdx.x, gridDim.x, it, s_r, s_g, s_b, s_c1, s_c2);
+}
+
+void launch_bnact_ibn(const BnActArgs& a, long long gb_stride, cudaStream_t st) {
+  ProfScope prof_scope__(PROF_BN, 0.0, st);
+  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
+  launch_pdl(bnact_ibn_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a), gb_stride);
+  CUDA_CHECK_LAUNCH();
+}
+
+void launch_bnbwd_ibn(const BnBwdArgs& a, long long gb_stride, cudaStream_t st) {
+  ProfScope prof_scope__(PROF_BN, 0.0, st);
+  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
+  dim3 rgrid = grid;
+  if ((int)rgrid.x > num_sms()) rgrid.x = num_sms();
+  launch_pdl(bnbwd_reduce_ibn_kernel, dim3(rgrid), dim3(block), (size_t)(0), st, tagged(a), gb_stride);
+  CUDA_CHECK_LAUNCH();
+  launch_pdl(bnbwd_apply_ibn_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a), gb_stride);
+  CUDA_CHECK_LAUNCH();
+}
+
+// forward tangent along the weights and the task's (gdot, bdot): pdot = slope * (gamma zhdot + gdot zh + bdot)
+__global__ void __launch_bounds__(256) bnact_tan_ibn_kernel(BnActTanArgs a, long long gbs, const float* gdot, const float* bdot) {
+  pdl_prologue(46, a.tag);
+  __shared__ float s_mu[64], s_r[64], s_g[64], s_b[64], s_md[64], s_q[64], s_gd[64], s_bd[64];
+  const BnGeom g = a.g;
+  const int task = blockIdx.y;
+  const double m = (double)g.n * g.h * g.w;
+  chan_setup(a.stats_fwd + (long long)task * a.stats_fwd_stride, a.gamma + (long long)task * gbs, a.beta + (long long)task * gbs,
+             m, g.F, s_mu, s_r, s_g, s_b);
+  if (threadIdx.x < g.F) {
+    const double* stt = a.stats_tan + (long long)task * a.stats_tan_stride;
+    s_md[threadIdx.x] = (float)(stt[threadIdx.x * 2] / m);
+    s_q[threadIdx.x] = (float)(stt[threadIdx.x * 2 + 1] / m);
+  }
+  ibn_load(gdot, gbs, task, g.F, s_gd);
+  ibn_load(bdot, gbs, task, g.F, s_bd);
+  __syncthreads();
+  WinIter it(g);
+  bnact_tan_phase<true>(a, g, task, blockIdx.x, gridDim.x, it, s_r, s_g, s_b, s_md, s_q, s_gd, s_bd);
+}
+
+__global__ void __launch_bounds__(256) bnbwd_tan_reduce_ibn_kernel(BnBwdTanArgs a, long long gbs) {
+  pdl_prologue(47, a.tag);
+  __shared__ float s_g[64], s_b[64];
+  const BnGeom g = a.g;
+  const int task = blockIdx.y;
+  ibn_load(a.gamma, gbs, task, g.F, s_g);
+  ibn_load(a.beta, gbs, task, g.F, s_b);
+  __syncthreads();
+  WinIter it(g);
+  double s1[4] = {0, 0, 0, 0}, s2[4] = {0, 0, 0, 0};
+  bnbwd_tan_reduce_phase(a, g, task, blockIdx.x, gridDim.x, it, s_g, s_b, s1, s2);
+  block_reduce_stats(s1, s2, it, a.stats_tbwd + (long long)task * a.stats_tbwd_stride, g.F);
+}
+
+__global__ void __launch_bounds__(256) bnbwd_tan_apply_ibn_kernel(BnBwdTanArgs a, long long gbs, const float* gdot) {
+  pdl_prologue(48, a.tag);
+  __shared__ float s_mu[64], s_r[64], s_g[64], s_b[64], s_q[64], s_c2[64], s_t1[64], s_t2[64], s_gd[64], s_c1[64];
+  const BnGeom g = a.g;
+  const int task = blockIdx.y;
+  const double m = (double)g.n * g.h * g.w;
+  chan_setup(a.stats_fwd + (long long)task * a.stats_fwd_stride, a.gamma + (long long)task * gbs, a.beta + (long long)task * gbs,
+             m, g.F, s_mu, s_r, s_g, s_b);
+  if (threadIdx.x < g.F) {
+    const int c = threadIdx.x;
+    const double* sb = a.stats_bwd + (long long)task * a.stats_bwd_stride;
+    const double* tb = a.stats_tbwd + (long long)task * a.stats_tbwd_stride;
+    s_q[c] = (float)((a.stats_tan + (long long)task * a.stats_tan_stride)[c * 2 + 1] / m);
+    s_c1[c] = (float)(sb[c * 2] / m);
+    s_c2[c] = (float)(sb[c * 2 + 1] / m);
+    s_t1[c] = (float)(tb[c * 2] / m);
+    s_t2[c] = (float)(tb[c * 2 + 1] / m);
+  }
+  ibn_load(gdot, gbs, task, g.F, s_gd);
+  __syncthreads();
+  WinIter it(g);
+  bnbwd_tan_apply_phase<true>(a, g, task, blockIdx.x, gridDim.x, it, s_r, s_g, s_b, s_q, s_c2, s_t1, s_t2, s_gd, s_c1);
+}
+
+void launch_bnact_tan_ibn(const BnActTanArgs& a, long long gb_stride, const float* gdot, const float* bdot, cudaStream_t st) {
+  ProfScope prof_scope__(PROF_BN, 0.0, st);
+  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
+  launch_pdl(bnact_tan_ibn_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a), gb_stride, gdot, bdot);
+  CUDA_CHECK_LAUNCH();
+}
+
+void launch_bnbwd_tan_ibn(const BnBwdTanArgs& a, long long gb_stride, const float* gdot, cudaStream_t st) {
+  ProfScope prof_scope__(PROF_BN, 0.0, st);
+  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
+  dim3 rgrid = grid;
+  if ((int)rgrid.x > num_sms()) rgrid.x = num_sms();
+  launch_pdl(bnbwd_tan_reduce_ibn_kernel, dim3(rgrid), dim3(block), (size_t)(0), st, tagged(a), gb_stride);
+  CUDA_CHECK_LAUNCH();
+  launch_pdl(bnbwd_tan_apply_ibn_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a), gb_stride, gdot);
   CUDA_CHECK_LAUNCH();
 }
 

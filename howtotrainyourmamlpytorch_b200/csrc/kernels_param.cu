@@ -10,6 +10,7 @@
 
 // internal index (per-task fast-weight vector) -> index in the reference-layout flat meta vector
 __device__ __forceinline__ long long internal_to_meta(const ParamLayout& pl, long long i, int* seg_out) {
+  const int spb = seg_per_block(pl);
   for (int l = 0; l < pl.L; ++l) {
     const long long wsz = 9LL * pl.cin[l] * pl.F;
     if (i >= pl.w_off[l] && i < pl.w_off[l] + wsz) {
@@ -17,12 +18,17 @@ __device__ __forceinline__ long long internal_to_meta(const ParamLayout& pl, lon
       const int f = (int)(rel % pl.F);
       const int c = (int)((rel / pl.F) % pl.cin[l]);
       const int tap = (int)(rel / ((long long)pl.F * pl.cin[l]));
-      *seg_out = 2 * l;
+      *seg_out = spb * l;
       return pl.m_w[l] + ((long long)f * pl.cin[l] + c) * 9 + tap;
     }
     if (i >= pl.b_off[l] && i < pl.b_off[l] + pl.F) {
-      *seg_out = 2 * l + 1;
+      *seg_out = spb * l + 1;
       return pl.m_b[l] + (i - pl.b_off[l]);
+    }
+    if (pl.inner_bn && i >= pl.beta_off[l] && i < pl.beta_off[l] + 2 * pl.F) {     // beta_l, then gamma_l
+      const bool is_gamma = i >= pl.gamma_off[l];
+      *seg_out = spb * l + (is_gamma ? 3 : 2);
+      return is_gamma ? pl.m_gamma[l] + (i - pl.gamma_off[l]) : pl.m_beta[l] + (i - pl.beta_off[l]);
     }
   }
   const long long D = (long long)pl.pix * pl.F;
@@ -31,10 +37,10 @@ __device__ __forceinline__ long long internal_to_meta(const ParamLayout& pl, lon
     const int k = (int)(rel / D);
     const int r2 = (int)(rel % D);
     const int pix = r2 / pl.F, c = r2 % pl.F;
-    *seg_out = 2 * pl.L;
+    *seg_out = spb * pl.L;
     return pl.m_fcw + (long long)k * D + (long long)c * pl.pix + pix;
   }
-  *seg_out = 2 * pl.L + 1;
+  *seg_out = spb * pl.L + 1;
   return pl.m_fcb + (i - pl.fcb_off);
 }
 
@@ -64,7 +70,8 @@ __device__ __forceinline__ int seg_of(const ParamLayout& pl, long long i) {
   return s;
 }
 
-// reduce the gradient chunks of every inner tensor (fixed order) and
+// reduce the gradient chunks of every inner tensor (fixed order; inner-loop BatchNorm beta / gamma: read the fp64 sums, see
+// PartialDesc) and
 //   PR_UPDATE: g_out = sum; theta_out = theta_in - alpha[seg][step] * sum     (LSLR step)
 //   PR_STORE : g_out = sum
 //   PR_SUB   : tbar -= sum
@@ -78,9 +85,17 @@ __global__ void param_reduce_kernel(ParamLayout pl, PartialDesc pd, const float*
   if (i >= i_hi) return;
   const int task = blockIdx.y;
   const int seg = seg_of(pl, i);
-  const float* p = partial + (long long)task * pd.task_stride + pd.off[seg] + (i - pl.seg_off[seg]);
   float s = 0.f;
-  for (int c = 0; c < pd.nchunks[seg]; ++c) s += p[(long long)c * pd.cstride[seg]];   // fixed order: deterministic
+  if (pd.nchunks[seg] == 0) {
+    // beta_l (segment 2 of block l: S1 = sum dy) or gamma_l (segment 3: S2 = sum dy * zh); nothing without sums
+    const int spb = seg_per_block(pl);
+    if (pd.bn_sums)
+      s = (float)pd.bn_sums[(long long)task * pd.bn_task_stride + (long long)(seg / spb) * pd.bn_layer_stride +
+                            (i - pl.seg_off[seg]) * 2 + (seg % spb - 2)];
+  } else {
+    const float* p = partial + (long long)task * pd.task_stride + pd.off[seg] + (i - pl.seg_off[seg]);
+    for (int c = 0; c < pd.nchunks[seg]; ++c) s += p[(long long)c * pd.cstride[seg]];   // fixed order: deterministic
+  }
   const long long o = (long long)task * task_stride + i;
   if (mode == PR_UPDATE) {
     const float alpha = meta[pl.m_lslr + (long long)seg * (pl.S + 1) + step];
@@ -243,8 +258,9 @@ __device__ __forceinline__ void export_body(const ExportArgs& a, float* __restri
   // ---- range 2: one warp per entry
   const int lane = threadIdx.x & 31;
   long long e = ((long long)blockIdx.x - nb1) * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const long long bnsz = (long long)(pl.per_step_bn ? pl.S : 1) * pl.F;
-  const long long E_bn = pl.ln ? 0 : 2LL * pl.L * bnsz, E_lslr = (long long)pl.nseg_inner * (pl.S + 1), E_run = pl.per_step_bn ? 2 * LSF : 0;
+  // BatchNorm beta / gamma rows (per_step_gb: one per step).  Inner-loop beta / gamma are fast weights: range 1 exports them
+  const long long bnsz = (long long)(pl.per_step_gb ? pl.S : 1) * pl.F;
+  const long long E_bn = (pl.ln || pl.inner_bn) ? 0 : 2LL * pl.L * bnsz, E_lslr = (long long)pl.nseg_inner * (pl.S + 1), E_run = pl.per_step_bn ? 2 * LSF : 0;
   double val = 0.0, scale = invB;
   long long dst;
   if (e < E_bn) {
@@ -256,10 +272,10 @@ __device__ __forceinline__ void export_body(const ExportArgs& a, float* __restri
     dst = (is_gamma ? pl.m_gamma[l] : pl.m_beta[l]) + rel;
     if (a.training) {
       const int f = (int)(rel % pl.F), s_sel = (int)(rel / pl.F), which = is_gamma ? 1 : 0;
-      const int per = pl.per_step_bn ? 1 : a.num_steps;               // steps that feed this entry
-      if (!pl.per_step_bn || s_sel < a.num_steps) {
+      const int per = pl.per_step_gb ? 1 : a.num_steps;               // steps that feed this entry
+      if (!pl.per_step_gb || s_sel < a.num_steps) {
         for (int k = lane; k < nt * per; k += 32) {
-          const int tk = k / per, t = t0 + tk, s = pl.per_step_bn ? s_sel : k - tk * per;
+          const int tk = k / per, t = t0 + tk, s = pl.per_step_gb ? s_sel : k - tk * per;
           val += stat_ptr(a, t, PASS_TGT_BWD, s, l)[f * 2 + which];
           val -= stat_ptr(a, t, PASS_TAN_BWD, s, l)[f * 2 + which];
         }
@@ -336,8 +352,8 @@ __device__ __forceinline__ void export_body(const ExportArgs& a, float* __restri
 void launch_export(const ExportArgs& a, cudaStream_t st) {
   ProfScope prof_scope__(PROF_PARAM, 0.0, st);
   const ParamLayout& pl = a.pl;
-  const long long bnsz = (long long)(pl.per_step_bn ? pl.S : 1) * pl.F;
-  const long long entries = (pl.ln ? pl.lnb_off[pl.L] : 2LL * pl.L * bnsz) + (long long)pl.nseg_inner * (pl.S + 1) + 2 +
+  const long long bnsz = (long long)(pl.per_step_gb ? pl.S : 1) * pl.F;
+  const long long entries = (pl.ln ? pl.lnb_off[pl.L] : pl.inner_bn ? 0 : 2LL * pl.L * bnsz) + (long long)pl.nseg_inner * (pl.S + 1) + 2 +
                             (pl.per_step_bn ? 2LL * pl.L * pl.S * pl.F : 0);
   const long long blocks = (pl.P + 255) / 256 + (entries + 7) / 8;        // range 1: thread per element; range 2: warp per entry
   launch_pdl(export_kernel, dim3((unsigned)blocks, a.per_task ? (unsigned)a.tasks : 1u), dim3(256), (size_t)(0), st, tagged(a));

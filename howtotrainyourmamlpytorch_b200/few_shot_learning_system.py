@@ -117,8 +117,9 @@ class MAMLFewShotClassifier(nn.Module):
     # ------------------------------------------------------------------ parameters / flat storage
     def get_inner_loop_parameter_dict(self, params):
         """The tensors adapted in the inner loop (reference :105-120): everything that requires grad
-        except BatchNorm parameters."""
-        return {name: p for name, p in params if p.requires_grad and "norm_layer" not in name}
+        except the norm parameters, which join with enable_inner_loop_optimizable_bn_params."""
+        inner_bn = self.classifier._inner_bn()
+        return {name: p for name, p in params if p.requires_grad and (inner_bn or "norm_layer" not in name)}
 
     def trainable_parameters(self):
         for p in self.parameters():
@@ -132,7 +133,7 @@ class MAMLFewShotClassifier(nn.Module):
         """Flat-buffer order = the network's engine segment order (``_segment_names``), then the LSLR vectors.  (Equals
         the reference's Adam parameter order.)"""
         names = ["classifier." + n for n in self.classifier._segment_names()]
-        inner = [n for n in names if "norm_layer" not in n]
+        inner = [n for n in names if self.classifier._inner_bn() or "norm_layer" not in n]
         names += ["inner_loop_optimizer.names_learning_rates_dict." + n[len("classifier."):].replace(".", "-")
                   for n in inner]
         return names
@@ -277,7 +278,7 @@ class MAMLFewShotClassifier(nn.Module):
                     inner_steps=int(a.number_of_training_steps_per_iter), per_step_bn=bool(a.per_step_bn_statistics),
                     max_tasks=int(n_tasks), keep_target_passes=bool(getattr(self, "_debug_keep_target_passes", False)),
                     force_fp32_convs=bool(getattr(self, "_debug_force_fp32_convs", False)),
-                    layer_norm=self.classifier._layer_norm())
+                    layer_norm=self.classifier._layer_norm(), inner_bn=self.classifier._inner_bn())
             self._engine_tasks = int(n_tasks)
             if self._engine.meta_size != self._flat.numel():
                 raise RuntimeError("engine / module parameter layout mismatch (%d vs %d floats)" %

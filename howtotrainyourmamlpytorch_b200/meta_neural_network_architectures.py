@@ -49,9 +49,10 @@ class MetaBatchNormLayer(nn.Module):
     def __init__(self, num_features, device, args, eps=1e-5, momentum=0.1, affine=True, track_running_stats=True,
                  meta_batch_norm=True, no_learnable_params=False, use_per_step_bn_statistics=False):
         super().__init__()
-        if getattr(args, "enable_inner_loop_optimizable_bn_params", False):
-            raise NotImplementedError("enable_inner_loop_optimizable_bn_params is outside the accelerated path "
-                                      "(no shipped config sets it)")
+        inner_bn = bool(getattr(args, "enable_inner_loop_optimizable_bn_params", False))
+        if inner_bn and not (args.learnable_bn_gamma and args.learnable_bn_beta):
+            raise NotImplementedError("enable_inner_loop_optimizable_bn_params with a frozen BatchNorm gamma or beta "
+                                      "(learnable_bn_gamma / learnable_bn_beta false) is outside the accelerated path")
         self.num_features, self.eps, self.momentum = int(num_features), eps, momentum
         self.use_per_step_bn_statistics = bool(use_per_step_bn_statistics)
         S = int(args.number_of_training_steps_per_iter)
@@ -61,6 +62,11 @@ class MetaBatchNormLayer(nn.Module):
                                         requires_grad=False)
         self.bias = nn.Parameter(torch.zeros(shape), requires_grad=bool(args.learnable_bn_beta))
         self.weight = nn.Parameter(torch.ones(shape), requires_grad=bool(args.learnable_bn_gamma))
+        if inner_bn:
+            # reference :194-198: inner-loop gamma / beta are one [F] row each, even with per-step statistics; re-assigned
+            # into their slots, so the registration order stays running_mean, running_var, bias, weight
+            self.bias = nn.Parameter(torch.zeros(self.num_features), requires_grad=True)
+            self.weight = nn.Parameter(torch.ones(self.num_features), requires_grad=True)
         if self.use_per_step_bn_statistics:
             # Reference quirk: while building itself the reference network pushes an all-zero dummy batch
             # through every block twice with num_step=0 (build_block :365 and build_network :603), and
@@ -140,6 +146,10 @@ class VGGReLUNormNetwork(nn.Module):
 
     def _layer_norm(self):
         return getattr(self.args, "norm_layer", "batch_norm") == "layer_norm"
+
+    def _inner_bn(self):
+        """BatchNorm gamma / beta are inner-loop fast weights (enable_inner_loop_optimizable_bn_params)."""
+        return bool(getattr(self.args, "enable_inner_loop_optimizable_bn_params", False))
 
     def _segment_names(self):
         """The operator's tensors in the engine's meta-vector order: per block conv.weight, conv.bias, then BatchNorm's
@@ -232,6 +242,10 @@ class VGGReLUNormNetwork(nn.Module):
         step-major (every task's support pass at step s, then every target pass), not task-major as the reference's loop
         over tasks does."""
         from . import _native
+        if self._inner_bn():
+            raise NotImplementedError("VGGReLUNormNetwork.forward does not run a network with "
+                                      "enable_inner_loop_optimizable_bn_params yet (inner-loop BatchNorm gamma / beta run in "
+                                      "MAMLFewShotClassifier.run_train_iter / run_validation_iter)")
         if x.device.type != "cuda":
             if self._layer_norm():
                 raise NotImplementedError("VGGReLUNormNetwork.forward on the layer-norm network runs on the CUDA engine "

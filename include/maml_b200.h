@@ -28,11 +28,12 @@ extern "C" {
 
 #define MAML_B200_MAX_STAGES 4
 #define MAML_B200_MAX_STEPS 8
-#define MAML_B200_ABI_VERSION 3
+#define MAML_B200_ABI_VERSION 4
 
 /* Static shape of the path.  Mirrors the args the reference reads on this path:
  * num_classes_per_set, num_samples_per_class, num_target_samples, image_{channels,height,width},
- * cnn_num_filters, num_stages, number_of_training_steps_per_iter, per_step_bn_statistics, norm_layer. */
+ * cnn_num_filters, num_stages, number_of_training_steps_per_iter, per_step_bn_statistics, norm_layer,
+ * enable_inner_loop_optimizable_bn_params. */
 typedef struct maml_b200_config {
   int32_t n_way;        /* N  classes per task                         */
   int32_t k_shot;       /* K  support samples per class                */
@@ -52,6 +53,12 @@ typedef struct maml_b200_config {
                            there are no running statistics).  Layer-norm handles run every entry; the layer norm has
                            no per-step rows, so the functional entries (maml_b200_net_*) compute the same at every
                            num_step, and maml_b200_net_running_update is a no-op. */
+  int32_t inner_bn;     /* 1: enable_inner_loop_optimizable_bn_params (batch norm only: refused with norm_layer = 1).  Each
+                           block's norm_layer.bias / .weight (beta, gamma) are [F] whatever per_step_bn is, and are
+                           inner-loop fast weights: per task, updated by the LSLR rule with their own rate vectors, and
+                           differentiated to second order like the conv weights.  The running statistics keep their
+                           per-step rows when per_step_bn is set.  The functional entries (maml_b200_net_*) refuse these
+                           handles. */
 } maml_b200_config;
 
 /* Per-call schedule: what reference forward(...) derives from epoch / phase (:232-244,:304-305). */
@@ -80,8 +87,11 @@ int64_t maml_b200_workspace_bytes(const maml_b200_handle* h);
 /* Flat meta-parameter vector ("meta"), reference layout and reference Adam order
  * (reference few_shot_learning_system.py:288-294): per block conv.weight[F,Cin,3,3],
  * conv.bias[F], norm_layer.bias[S|1,F], norm_layer.weight[S|1,F] (layer norm: conv.weight, conv.bias,
- * norm_layer.bias[F,h_l,w_l]); then linear.weights[N,D], linear.bias[N]; then the 2*stages+2 LSLR
- * vectors [S+1] in inner-parameter order. */
+ * norm_layer.bias[F,h_l,w_l]; inner_bn: norm_layer.bias[F], norm_layer.weight[F]); then linear.weights[N,D], linear.bias[N];
+ * then the LSLR vectors [S+1] in inner-parameter order (the reference's get_inner_loop_parameter_dict): 2*stages+2 of them
+ * (per block conv.weight, conv.bias; then linear.weights, linear.bias), or with inner_bn 4*stages+2 (per block conv.weight,
+ * conv.bias, norm_layer.bias, norm_layer.weight; then the linear layer's).
+ * Fast weights (per task, inside the engine): the inner tensors in that order, conv weights as [3*3][Cin][F]. */
 int32_t maml_b200_num_segments(const maml_b200_handle* h);
 int maml_b200_segment(const maml_b200_handle* h, int32_t idx, int64_t* offset, int64_t* size);
 int64_t maml_b200_meta_size(const maml_b200_handle* h);
@@ -209,10 +219,10 @@ int maml_b200_net_running_update(maml_b200_handle* h, int32_t n_tasks, int32_t n
 /* Outer step on the flat vectors: optional clamp to [-10,10] (reference :332-335), Adam
  * (betas 0.9/0.999, eps 1e-8, no weight decay; reference :69,:336).  `grad` is the first
  * meta_size floats of (the all-reduced) result.  Bit i of trainable_mask / clamp_mask refers to
- * segment i.  `step` is the 1-based Adam step count of this update. */
+ * segment i (an inner_bn handle with 4 blocks has 36 segments).  `step` is the 1-based Adam step count of this update. */
 int maml_b200_adam_step(maml_b200_handle* h, float* meta, const float* grad,
                         float* exp_avg, float* exp_avg_sq,
-                        float lr, int32_t step, uint32_t trainable_mask, uint32_t clamp_mask,
+                        float lr, int32_t step, uint64_t trainable_mask, uint64_t clamp_mask,
                         void* stream);
 
 /* Running-statistics EMA finalisation (side effect of F.batch_norm in the reference,

@@ -1,0 +1,443 @@
+"""Inner-loop BatchNorm gamma / beta (``enable_inner_loop_optimizable_bn_params``) on the fused training and validation
+iteration, against golden vectors of the unmodified reference (``oracle/gen_golden_ibn.py``) and the fp64 autograd oracle
+(``oracle/ibn_oracle.py``).  With the flag each block's norm_layer.bias / .weight are [F] fast weights: per task, updated by
+the LSLR rule with their own rate vectors, differentiated to second order like the conv weights.
+
+CPU tests: the oracle reproduces each fixture's fp64 reference run, the module's state_dict / LSLR / Adam order match the
+reference's, and the refusals.  GPU tests: the meta-gradient (gamma / beta and their LSLR rates included), the validation
+leg and the post-Adam state against the goldens; tensor cores against FFMA; rank r of G; and, on the fixtures and on a
+seeded full-size case (``FULL``: Omniglot MAML++ 5-way 1-shot at 8 tasks, moved state), every stage of the iteration and the
+meta-gradient against the autograd-free fp64 oracle with the GPU's leaky-ReLU and pooling decisions pinned."""
+import numpy as np
+import pytest
+import torch
+
+from conftest import grad_tolerance, load_golden
+from engine_layout import flat_to_nchw, geometry, grid_to_nchw, rel_err
+from oracle import ibn_oracle as IBN
+from oracle import maml_oracle as O
+
+IBN_CASES = ["ibn_tiny_pp", "ibn_tiny_pp_moved", "ibn_tiny_first", "ibn_tiny_maml", "ibn_one_stage", "ibn_ffma_wide",
+             "ibn_bern"]
+FLAG = "enable_inner_loop_optimizable_bn_params"
+FULL = "ibn_full_omniglot_mamlpp_5w1s"
+
+
+class _Seeded(object):
+    """A full-size case without a fixture: the config's args, a moved state (distinct gamma / beta per block and channel,
+    moved biases and LSLR rates) and seeded N(0, 1) episodes."""
+
+    def __init__(self):
+        from howtotrainyourmamlpytorch_b200 import MAMLFewShotClassifier
+        from howtotrainyourmamlpytorch_b200.configs import CONFIGS
+        from howtotrainyourmamlpytorch_b200.utils.parser_utils import args_from_json
+        self.argdict = dict(CONFIGS["omniglot_mamlpp_5w1s"], batch_size=8, **{FLAG: True})
+        self.args = a = args_from_json(None, **self.argdict)
+        self.iters = [(0, 0)]
+        m = MAMLFewShotClassifier(im_shape=(2, a.image_channels, a.image_height, a.image_width), device="cpu", args=a)
+        self._state = O.moved_state(m.state_dict(), a, 13)
+
+    def state(self, dtype=torch.float32):
+        return {k: v.detach().clone().to(dtype) for k, v in self._state.items()}
+
+    def batch(self, it=0):
+        return O.synthetic_batch(self.args, iteration=self.iters[it][1], kind="normal")
+
+
+def _case(case):
+    return _Seeded() if case == FULL else load_golden(case)
+
+
+def _model(g, device, **debug):
+    from howtotrainyourmamlpytorch_b200 import MAMLFewShotClassifier
+    a = g.args
+    m = MAMLFewShotClassifier(im_shape=(2, a.image_channels, a.image_height, a.image_width), device=device, args=a)
+    for k, v in debug.items():
+        setattr(m, k, v)
+    m.load_state_dict(g.state())
+    return m
+
+
+# ------------------------------------------------------------------------------------------------ CPU
+@pytest.mark.parametrize("oracle", ["autograd", "manual"])
+@pytest.mark.parametrize("case", IBN_CASES)
+def test_oracle_reproduces_fp64_reference(case, oracle):
+    g = load_golden(case)
+    state = {k: v.double() for k, v in g.state(torch.float64).items()}
+    fn = IBN.autograd_train_iter if oracle == "autograd" else IBN.manual_train_iter
+    res = fn(state, g.args, g.batch(0), g.iters[0][0])
+    assert abs(float(res["loss"]) - g.scalar("loss64")) <= 1e-12 * abs(g.scalar("loss64"))
+    ref = g.grads(0, "64")
+    assert list(res["grads"].keys()) == list(ref.keys())
+    for n, got in res["grads"].items():
+        # conv biases are dead under BatchNorm: their reference gradient is rounding noise of ~1e-15 (absolute bound)
+        dead = n.endswith("conv.bias") or "conv-bias" in n
+        tol = 1e-12 if dead else 1e-12 * max(float(ref[n].abs().max()), 1e-30)
+        assert float((got - ref[n].double()).abs().max()) <= tol, n
+
+
+@pytest.mark.parametrize("case", IBN_CASES)
+def test_layout_and_adam_order_match_the_reference(case):
+    g = load_golden(case)
+    m = _model(g, "cpu")
+    sd = m.state_dict()
+    ref = g.state()
+    assert list(sd.keys()) == list(ref.keys())
+    for k in ref:
+        assert tuple(sd[k].shape) == tuple(ref[k].shape), k
+        assert torch.equal(sd[k], ref[k]), k
+    F, S = int(g.args.cnn_num_filters), int(g.args.number_of_training_steps_per_iter)
+    run_shape = (S, F) if g.args.per_step_bn_statistics else (F,)
+    for l in range(int(g.args.num_stages)):
+        p = "classifier.layer_dict.conv%d.norm_layer." % l
+        assert tuple(sd[p + "bias"].shape) == tuple(sd[p + "weight"].shape) == (F,)
+        assert tuple(sd[p + "running_mean"].shape) == run_shape
+        names = [n for n in sd if n.startswith(p)]
+        assert names == [p + n for n in ("running_mean", "running_var", "bias", "weight")]
+    # the inner loop and its LSLR vectors: conv.weight, conv.bias, norm_layer.bias, norm_layer.weight per block, then linear
+    inner = ["classifier." + n for n in m.get_inner_loop_parameter_dict(m.classifier.named_parameters())]
+    assert inner == IBN.inner_param_names(g.args)
+    lslr = list(m.inner_loop_optimizer.names_learning_rates_dict.keys())
+    assert ["inner_loop_optimizer.names_learning_rates_dict." + k for k in lslr] == [O.lslr_name(n) for n in inner]
+    assert all(v.shape == (S + 1,) for v in m.inner_loop_optimizer.names_learning_rates_dict.values())
+    assert [n for n, _ in m._trainable_param_list()] == IBN.trainable_names(g.args) == list(g.grads(0).keys())
+    # the flat buffer holds every LSLR vector (frozen ones too, outside Adam's mask), in inner-loop order
+    assert m._order == IBN.inner_param_names(g.args) + [O.lslr_name(n) for n in inner]
+    group = m.optimizer.state_dict()["param_groups"][0]
+    assert group["params"] == list(range(len(IBN.trainable_names(g.args))))
+
+
+def test_refusals():
+    from howtotrainyourmamlpytorch_b200 import MAMLFewShotClassifier
+    from howtotrainyourmamlpytorch_b200.utils.parser_utils import args_from_json
+    g = load_golden("ibn_tiny_pp")
+    a = g.args
+    shape = (2, a.image_channels, a.image_height, a.image_width)
+    m = MAMLFewShotClassifier(im_shape=shape, device="cpu", args=a)
+    x = torch.zeros(a.num_classes_per_set, a.image_channels, a.image_height, a.image_width)
+    with pytest.raises(NotImplementedError, match=FLAG):
+        m.classifier(x, 0)
+    for frozen in ("learnable_bn_gamma", "learnable_bn_beta"):
+        with pytest.raises(NotImplementedError, match=frozen[:-5]):
+            MAMLFewShotClassifier(im_shape=shape, device="cpu", args=args_from_json(None, **dict(g.argdict, **{frozen: False})))
+    with pytest.raises(NotImplementedError, match="layer_norm"):
+        MAMLFewShotClassifier(im_shape=shape, device="cpu", args=args_from_json(None, **dict(g.argdict, norm_layer="layer_norm")))
+
+
+# ------------------------------------------------------------------------------------------------ GPU
+def _check_grads(grads, g32, g64, big=False):
+    assert set(grads) >= set(g64)
+    bad = []
+    for n in g64:
+        err = float((grads[n].cpu().double() - g64[n].double()).abs().max())
+        tol = grad_tolerance(n, g32[n], g64[n], big)
+        print("%-80s err %.2e tol %.2e" % (n, err, tol))
+        if err > tol:
+            bad.append((n, err, tol))
+    assert not bad, bad
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", IBN_CASES)
+def test_golden_reference_parity(case, cuda_device):
+    """Loss, logits, accuracy and every outer gradient (gamma / beta and their LSLR rates included) vs the reference."""
+    g = load_golden(case)
+    m = _model(g, cuda_device)
+    losses, preds, grads = m.meta_gradient(g.batch(0), g.iters[0][0])
+    ref32, ref64 = g.scalar("loss"), g.scalar("loss64")
+    assert abs(float(losses["loss"]) - ref64) <= max(3 * abs(ref32 - ref64), 2e-5 * abs(ref64))
+    ref_logits = torch.from_numpy(g.array("logits"))
+    assert float((torch.from_numpy(np.stack(preds)) - ref_logits).abs().max()) <= 1e-3 * float(ref_logits.abs().max())
+    assert abs(losses["accuracy"] - g.scalar("accuracy")) <= 1e-6
+    _check_grads(grads, g.grads(0, ""), g.grads(0, "64"))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", IBN_CASES)
+def test_validation_iter(case, cuda_device):
+    """run_validation_iter against the reference's: loss, accuracy, logits, and the running statistics it leaves."""
+    g = load_golden(case)
+    m = _model(g, cuda_device)
+    m.current_epoch = g.iters[0][0]
+    losses, preds = m.run_validation_iter(g.batch(0))
+    ref_loss = float(g.val("loss"))
+    assert abs(float(losses["loss"]) - ref_loss) <= 2e-5 * abs(ref_loss)
+    ref_logits = torch.from_numpy(g.val("logits"))
+    assert float((torch.from_numpy(np.stack(preds)) - ref_logits).abs().max()) <= 2e-4 * float(ref_logits.abs().max())
+    assert abs(float(losses["accuracy"]) - float(g.val("accuracy"))) <= 1e-6
+    post = g.val_post()
+    sd = {k: v.detach().cpu() for k, v in m.state_dict().items()}
+    for k, v in post.items():
+        assert float((sd[k] - v).abs().max()) <= 1e-5 * max(float(v.abs().max()), 1.0), k
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", IBN_CASES)
+def test_train_iterations_post_state(case, cuda_device):
+    """run_train_iter (fwd/bwd, clamp + Adam over every segment) over the recorded iterations: the post-step state_dict
+    must match.  The 4-block cases have 36 meta segments, more than one Adam launch covers."""
+    g = load_golden(case)
+    m = _model(g, cuda_device)
+    for it, (epoch, _) in enumerate(g.iters):
+        losses, _ = m.run_train_iter(g.batch(it), epoch)
+        assert abs(float(losses["loss"]) - g.scalar("loss", it)) <= 1e-4 * abs(g.scalar("loss", it))
+        post = g.post(it)
+        sd = {k: v.detach().cpu() for k, v in m.state_dict().items()}
+        assert list(sd.keys()) == list(post.keys())
+        for k in post:
+            if "conv.bias" in k or "conv-bias" in k:
+                continue   # dead parameter: the reference's update is pure rounding noise through Adam
+            if "running" in k:
+                assert torch.allclose(sd[k], post[k], rtol=1e-4, atol=1e-5), (it, k, float((sd[k] - post[k]).abs().max()))
+                continue
+            # Adam's first steps move every weight by ~lr * g / (|g| + 1e-8): an element whose gradient is at noise level
+            # may move differently; everything else must agree
+            diff = (sd[k] - post[k]).abs()
+            assert float((diff > 2e-5).float().mean()) <= 2e-3 and float(diff.max()) <= 2.5e-3, (it, k, float(diff.max()))
+        # the conv biases shift the batch mean the running statistics record: adopt the reference's before the next iteration
+        with torch.no_grad():
+            for k, p in m.named_parameters():
+                if "conv.bias" in k:
+                    p.copy_(post[k].to(p.device))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", ["ibn_tiny_pp", "ibn_tiny_pp_moved", "ibn_bern"])
+def test_tensor_core_convs_match_fp32_ffma_convs(case, cuda_device):
+    """The wgmma 3xTF32 path against the exact-fp32 FFMA kernels (`reserved` bit 1): the fast weights after the first
+    step (gamma / beta rows included) and the whole meta-gradient, within 3x the reference's own fp32-vs-fp64 distance of
+    each tensor (floor 2e-5 of max-norm)."""
+    g = load_golden(case)
+    g32, g64 = g.grads(0, ""), g.grads(0, "64")
+    outs = []
+    for force in (False, True):
+        m = _model(g, cuda_device, _debug_force_fp32_convs=force)
+        _, _, grads = m.meta_gradient(g.batch(0), g.iters[0][0])
+        taps = {"theta1": torch.from_numpy(m._engine.debug_read("theta", 0, 1, 0)),
+                "g0": torch.from_numpy(m._engine.debug_read("g", 0, 0, 0))}
+        taps.update({n: v.cpu() for n, v in grads.items()})
+        outs.append(taps)
+    for k in outs[0]:
+        tol = 2e-5
+        if k in g64:
+            tol = max(tol, 3 * rel_err(g32[k].double(), g64[k].double()))
+        assert rel_err(outs[0][k], outs[1][k]) <= tol, (k, rel_err(outs[0][k], outs[1][k]))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case,G", [("ibn_tiny_pp", 3), ("ibn_tiny_pp_moved", 3)])
+def test_engine_as_rank_r_of_G_sums_to_single_call(case, G, cuda_device):
+    """Rank r of G, one rank after the other on one GPU: the G result vectors sum to the single call's (gamma / beta and
+    their LSLR rates included, and the per-step running-statistics parts)."""
+    g = load_golden(case)
+    batch, epoch = g.batch(0), g.iters[0][0]
+    B = batch[0].shape[0]
+    Bl = B // G
+    m = _model(g, cuda_device)
+    m.meta_gradient(batch, epoch)
+    full = m._result.detach().double().cpu().clone()
+    acc = torch.zeros_like(full)
+    for r in range(G):
+        mr = _model(g, cuda_device)
+        mr._ensure_engine(B)
+        mr._shard_override = (r, G)
+        mr.meta_gradient(tuple(t[r * Bl:(r + 1) * Bl].contiguous() for t in batch), epoch)
+        acc += mr._result.detach().double().cpu()
+    for (off, size), name in zip(m._engine.segments, m._order):
+        a, b = acc[off:off + size], full[off:off + size]
+        assert float((a - b).abs().max()) <= 2e-6 * float(b.abs().max()) + 1e-9, name
+    ms = m._engine.meta_size
+    assert abs(float(acc[ms] - full[ms])) <= 1e-6 * abs(float(full[ms]))
+    assert float(acc[ms + 1]) == float(full[ms + 1])
+
+
+@pytest.mark.gpu
+def test_functional_entries_refuse_inner_bn_handles(cuda_device):
+    """The functional network operator does not run these handles yet: its C entries fail with an error."""
+    g = load_golden("ibn_tiny_pp")
+    m = _model(g, cuda_device)
+    eng = m._ensure_engine(1)
+    a = g.args
+    x = torch.zeros(1, a.num_classes_per_set * a.num_target_samples, a.image_channels, a.image_height, a.image_width,
+                    device=cuda_device)
+    logits = torch.zeros(1, a.num_classes_per_set * a.num_target_samples, a.num_classes_per_set, device=cuda_device)
+    with pytest.raises(RuntimeError, match="inner_bn"):
+        eng.net_forward(1, 0, m._flat, x, logits)
+
+
+# ------------------------------------------------------------------------------------------------ stages and decisions
+def _theta_ibn(vec, args):
+    """Internal fast-weight vector -> {reference name: tensor}: per block W [3*3][Cin][F], b, beta, gamma [F]; then the
+    linear layer [N][pix][F] and its bias."""
+    geo, (ph, pw) = geometry(args)
+    F, N = int(args.cnn_num_filters), int(args.num_classes_per_set)
+    v, out, o = np.asarray(vec), {}, 0
+    for l, gl in enumerate(geo):
+        wsz = 9 * gl["cin"] * F
+        w = v[o:o + wsz].reshape(3, 3, gl["cin"], F).transpose(3, 2, 0, 1)
+        out["classifier.layer_dict.conv%d.conv.weight" % l] = torch.from_numpy(np.ascontiguousarray(w))
+        o += wsz
+        for n in ("conv.bias", "norm_layer.bias", "norm_layer.weight"):
+            out["classifier.layer_dict.conv%d.%s" % (l, n)] = torch.from_numpy(v[o:o + F].copy())
+            o += F
+    D = ph * pw * F
+    fw = v[o:o + N * D].reshape(N, ph * pw, F).transpose(0, 2, 1).reshape(N, D)
+    out[O.LIN_W] = torch.from_numpy(np.ascontiguousarray(fw))
+    out[O.LIN_B] = torch.from_numpy(v[o + N * D:o + N * D + N].copy())
+    return out
+
+
+def _gpu_decisions(m, g, batch, epoch):
+    """The leaky-ReLU branch per element and the arg-max per pooling window that the GPU took, rebuilt bit-exactly from its
+    normalised activations and the TASK's fast gamma / beta of the pass (theta^s for the support pass of step s,
+    theta^{s+1} for its target pass): y = fmaf(gamma, zh, beta) = the fp64 value rounded once to fp32, first max wins."""
+    import torch.nn.functional as Fnn
+    a, eng = g.args, m._engine
+    geo, _ = geometry(a)
+    F = int(a.cnn_num_filters)
+    N, K, T = int(a.num_classes_per_set), int(a.num_samples_per_class), int(a.num_target_samples)
+    S = int(a.number_of_training_steps_per_iter)
+    sched = O.target_pass_schedule(a, epoch, True, S)
+    dec = {}
+    for b in range(batch[0].shape[0]):
+        thetas = [_theta_ibn(eng.debug_read("theta", b, s, 0), a) for s in range(S + 1)]
+        for s in range(S):
+            for kind, n, th in (("sup", N * K, thetas[s]), ("tgt", N * T, thetas[s + 1])):
+                if kind == "tgt" and sched[s] is None:
+                    continue
+                per_layer = []
+                for l, gl in enumerate(geo):
+                    zh = grid_to_nchw(eng.debug_read(kind + "_zh", b, s, l), n, gl["h"], gl["w"], F)
+                    _, _, gn, btn, _, _ = O.conv_names(l)
+                    y = (th[gn].double()[None, :, None, None] * zh.double() + th[btn].double()[None, :, None, None]).float()
+                    slope = torch.where(y > 0, torch.ones_like(y), torch.full_like(y, 0.01))
+                    act = torch.where(y > 0, y, torch.tensor(0.01, dtype=torch.float32) * y)
+                    _, idx = Fnn.max_pool2d(act, 2, 2, return_indices=True)
+                    per_layer.append((slope, idx))
+                dec[(b, kind, s)] = per_layer
+    return dec
+
+
+def _pinned_run(case, device):
+    """The GPU iteration (every target pass kept) and the fp64 autograd-free oracle with the GPU's decisions pinned."""
+    g = _case(case)
+    m = _model(g, device, _debug_keep_target_passes=True)
+    batch, epoch = g.batch(0), g.iters[0][0]
+    losses, preds, grads = m.meta_gradient(batch, epoch)
+    dec = _gpu_decisions(m, g, batch, epoch)
+    ref = IBN.manual_train_iter(g.state(torch.float64), g.args, batch, epoch, decisions=dec, keep_intermediates=True)
+    return g, m, losses, preds, grads, ref
+
+
+STAGE_CASES = ["ibn_tiny_pp", "ibn_tiny_pp_moved", "ibn_tiny_first", "ibn_tiny_maml", "ibn_one_stage", "ibn_ffma_wide",
+               "ibn_bern", FULL]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", STAGE_CASES)
+def test_stagewise_against_oracle(case, cuda_device):
+    """Every materialised intermediate of tasks 0 and B-1 against the fp64 autograd-free oracle with the GPU's decisions
+    pinned: theta^s (gamma / beta rows included), every support pass (zh, pooled output, dp, dz) and g_s, every target pass
+    (zh, dz) and tgrad[s], theta-bar and u after the reverse sweep, and step 0's tangent pass (zh-dot, dz-dot of every
+    block: the gamma-tangent term of dz-dot included)."""
+    g, m, losses, preds, grads, ref = _pinned_run(case, cuda_device)
+    a, eng = g.args, m._engine
+    geo, (ph, pw) = geometry(a)
+    F = int(a.cnn_num_filters)
+    N, K, T = int(a.num_classes_per_set), int(a.num_samples_per_class), int(a.num_target_samples)
+    S, L, B = int(a.number_of_training_steps_per_iter), len(geo), g.batch(0)[0].shape[0]
+    rows, worst = [], 0.0
+
+    def chk(name, got, want, tol):
+        nonlocal worst
+        e = rel_err(got, want)
+        rows.append("%-44s %.2e%s" % (name, e, "" if e <= tol else "   <-- FAIL"))
+        worst = max(worst, e / tol)
+
+    def chk_vec(tag, vec, want, tol=5e-5):
+        got = _theta_ibn(vec, a)
+        for n, v in want.items():
+            if n.endswith("conv.bias"):
+                continue          # dead under BatchNorm: gradient and tangent are rounding noise
+            chk("%s %s" % (tag, n[-26:]), got[n], v, 2e-4 if n == O.LIN_B and tol > 1e-5 else tol)
+
+    for t in sorted({0, B - 1}):
+        inter = [x for x in ref["intermediates"] if "theta" in x and x["task"] == t][0]
+        tan0 = [x for x in ref["intermediates"] if x.get("step") == 0 and x["task"] == t]
+        for s in range(S):
+            chk_vec("t%d theta[%d]" % (t, s), eng.debug_read("theta", t, s, 0), inter["theta"][s], tol=1e-5)
+            for l in range(L):
+                gl = geo[l]
+                chk("t%d sup zh   s%d l%d" % (t, s, l), grid_to_nchw(eng.debug_read("sup_zh", t, s, l), N * K, gl["h"], gl["w"], F),
+                    inter["sup_f"][s]["blocks"][l]["zh"], 2e-5)
+                p = (grid_to_nchw(eng.debug_read("sup_ain", t, s, l + 1), N * K, gl["h"] // 2, gl["w"] // 2, F) if l + 1 < L
+                     else flat_to_nchw(eng.debug_read("sup_ain", t, s, L), N * K, ph, pw, F))
+                chk("t%d sup pool s%d l%d" % (t, s, l), p, inter["sup_f"][s]["blocks"][l]["p"], 2e-5)
+                dp = (grid_to_nchw(eng.debug_read("sup_dp", t, s, l), N * K, gl["h"] // 2, gl["w"] // 2, F) if l + 1 < L
+                      else flat_to_nchw(eng.debug_read("sup_dp", t, s, l), N * K, ph, pw, F))
+                chk("t%d sup dp   s%d l%d" % (t, s, l), dp, inter["sup_b"][s]["blocks"][l]["dp"], 5e-5)
+                chk("t%d sup dz   s%d l%d" % (t, s, l), grid_to_nchw(eng.debug_read("sup_dz", t, s, l), N * K, gl["h"], gl["w"], F),
+                    inter["sup_b"][s]["blocks"][l]["dz"], 5e-5)
+            chk_vec("t%d g[%d]" % (t, s), eng.debug_read("g", t, s, 0), inter["sup_g"][s])
+            if inter["tgt_f"][s] is not None:
+                for l in range(L):
+                    gl = geo[l]
+                    chk("t%d tgt zh   s%d l%d" % (t, s, l),
+                        grid_to_nchw(eng.debug_read("tgt_zh", t, s, l), N * T, gl["h"], gl["w"], F),
+                        inter["tgt_f"][s][0]["blocks"][l]["zh"], 2e-5)
+                    chk("t%d tgt dz   s%d l%d" % (t, s, l),
+                        grid_to_nchw(eng.debug_read("tgt_dz", t, s, l), N * T, gl["h"], gl["w"], F),
+                        inter["tgt_b"][s]["blocks"][l]["dz"], 5e-5)
+                chk_vec("t%d tgrad[%d]" % (t, s), eng.debug_read("tgrad", t, s, 0), inter["tgt_g"][s])
+        chk_vec("t%d tbar" % t, eng.debug_read("tbar", t, 0, 0), inter["tbar"])
+        if tan0:
+            chk_vec("t%d u[0]" % t, eng.debug_read("u", t, 0, 0), tan0[0]["u"])
+            for l in range(L):
+                gl = geo[l]
+                chk("t%d tan zh-dot l%d" % (t, l), grid_to_nchw(eng.debug_read("tan_zh", t, 0, l), N * K, gl["h"], gl["w"], F),
+                    tan0[0]["tangent"]["fwd"][l]["zh_dot"], 5e-5)
+                chk("t%d tan dz-dot l%d" % (t, l), grid_to_nchw(eng.debug_read("tan_dz", t, 0, l), N * K, gl["h"], gl["w"], F),
+                    tan0[0]["tangent"]["bwd"][l]["dz_dot"], 5e-5)
+    print("\n[%s stagewise]\n   " % case + "\n   ".join(rows))
+    assert worst <= 1.0, "stage mismatch (see report above): worst = %.2f x tolerance" % worst
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", STAGE_CASES)
+def test_decision_forced_parity(case, cuda_device):
+    """(1) Every discrete decision the GPU took (leaky-ReLU branch, pooling arg-max) is consistent with fp64 arithmetic
+    except at margins below 1e-4; (2) with those decisions pinned, the fp64 oracle's loss, logits and every meta-gradient
+    tensor (gamma / beta and their LSLR rates included; conv biases absolute) agree with the GPU's to 1e-4 of max-norm."""
+    import torch.nn.functional as Fnn
+    g, m, losses, preds, grads, ref = _pinned_run(case, cuda_device)
+    n_flip, worst_margin = 0, 0.0
+    for x in [i for i in ref["intermediates"] if "theta" in i]:
+        for f in list(x["sup_f"]) + [t[0] for t in x["tgt_f"] if t is not None]:
+            for blk in f["blocks"]:
+                y = blk["y"]
+                flip = (y > 0) != (blk["slope"] > 0.5)
+                if flip.any():
+                    n_flip += int(flip.sum())
+                    worst_margin = max(worst_margin, float(y[flip].abs().max()))
+                act = y * O._slope(y)
+                n_, c_ = act.shape[:2]
+                gap = Fnn.max_pool2d(act, 2, 2) - act.view(n_, c_, -1).gather(2, blk["idx"].view(n_, c_, -1)).view(
+                    n_, c_, *blk["idx"].shape[2:])
+                if (gap > 0).any():
+                    n_flip += int((gap > 0).sum())
+                    worst_margin = max(worst_margin, float(gap.max()))
+    print("\n[%s] decisions differing from fp64: %d, worst fp64 margin at one: %.2e" % (case, n_flip, worst_margin))
+    assert worst_margin <= 1e-4, worst_margin
+    assert abs(float(losses["loss"]) - float(ref["loss"])) <= 1e-5 * abs(float(ref["loss"]))
+    bad = []
+    for n, v in ref["grads"].items():
+        err = float((grads[n].cpu().double() - v).abs().max())
+        scale = max(float(v.abs().max()), 1e-30)
+        dead = "conv.bias" in n or "conv-bias" in n
+        tol = 1e-5 if dead else 1e-4 * scale + 1e-7
+        print("%-80s err %.2e (%.1e of max)" % (n, err, err / scale))
+        if err > tol:
+            bad.append((n, err, scale))
+    assert not bad, bad
+    got_logits = torch.from_numpy(np.stack(preds)).double()
+    assert float((got_logits - ref["logits"]).abs().max()) <= 1e-4 * float(ref["logits"].abs().max())
