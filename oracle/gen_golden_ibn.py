@@ -47,6 +47,13 @@ IBN_CASES = {
     # Bernoulli images: exact pooling ties
     "ibn_bern": ("omniglot_mamlpp_5w1s", dict(G._TINY, image_height=28, image_width=28, cnn_num_filters=32, batch_size=2,
                                               task_learning_rate=0.02, **dict(_OMNI, **_IBN)), [(0, 0)], "bernoulli", None),
+    # the shape of env_moved_eight: S = 8, so the gamma / beta LSLR vectors (9 entries) and the per-step running-statistics
+    # rows are indexed past step 4
+    "ibn_eight_moved": G._envelope("omniglot_mamlpp_5w1s", (16, 16, 1), 16, 4, 8, (3, 2, 2), 2, [(3, 0), (3, 1)],
+                                   moved=6, **_IBN),
+    # the shape of env_many_tasks at a moved state: 48 tasks, so every task's gamma / beta (theta + task * Ppad) past task 7
+    # is read
+    "ibn_many_tasks": G._envelope("omniglot_mamlpp_5w1s", (8, 8, 1), 16, 3, 2, (3, 1, 1), 48, [(0, 0)], moved=8, **_IBN),
 }
 
 

@@ -35,6 +35,13 @@ LN_CASES = {
     # Bernoulli images: exact pooling ties
     "ln_bern": ("omniglot_mamlpp_5w1s", dict(G._TINY, image_channels=1, image_height=28, image_width=28, batch_size=2,
                                              task_learning_rate=0.02, **_LN), [(0, 0)], "bernoulli", None),
+    # the shape of env_moved_eight: S = 8, so the LSLR vectors (9 entries) and the per-(pass, step) bias-gradient rows are
+    # indexed past step 4
+    "ln_eight_moved": G._envelope("omniglot_mamlpp_5w1s", (16, 16, 1), 16, 4, 8, (3, 2, 2), 2, [(3, 0), (3, 1)],
+                                  moved=6, **_LN),
+    # the shape of env_one_stage: L = 1, the head follows block 0's per-image normalisation
+    "ln_one_stage": G._envelope("omniglot_mamlpp_5w1s", (12, 12, 1), 16, 1, 2, (3, 2, 2), 2, [(0, 0), (0, 1)],
+                                moved=None, task_learning_rate=0.02, **_LN) + (None,),
 }
 
 

@@ -1,6 +1,9 @@
-"""Test helpers: convert the engine's internal layouts (debug taps) to the reference's NCHW / OIHW."""
+"""Test helpers: convert the engine's internal layouts (debug taps) to the reference's NCHW / OIHW, and the host rules
+that choose the engine's launch plans, restated."""
 import numpy as np
 import torch
+
+H100_SMS = 132
 
 
 def geometry(args):
@@ -10,6 +13,110 @@ def geometry(args):
         geo.append(dict(h=h, w=w, cin=cin))
         h, w, cin = h // 2, w // 2, int(args.cnn_num_filters)
     return geo, (h, w)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# the host rules of maml_b200_create / plan_chunks / tail_fusable, restated (engine.cu, kernels_tc.cu, kernels_bn.cu)
+# ----------------------------------------------------------------------------------------------------------------------
+def _tc_rpad(gw):
+    return (128 + 2 * (gw + 1) + 7) // 8 * 8
+
+
+def _tc_ring(F, gw):
+    row = (F + 4) * 4
+    extra = 128 * row + (128 // 2) * row              # split-K over 2 CTAs in tangent mode
+    avail = 227 * 1024 - 4096 - 1024 - 4 * _tc_rpad(gw) * 128 - extra
+    return min(8, avail // (2 * F * 128))
+
+
+def host_plan(a, tasks, num_sms=H100_SMS):
+    geo, _ = geometry(a)
+    L, F = len(geo), int(a.cnn_num_filters)
+    n_s = int(a.num_classes_per_set) * int(a.num_samples_per_class)
+    rings = [_tc_ring(F, geo[l]["w"] + 1) for l in range(1, L)]
+    tc = L > 1 and all(_tc_rpad(geo[l]["w"] + 1) <= 256 for l in range(1, L)) and min(rings) >= 2
+    head_rows = 16 if n_s <= 16 else 4
+    last = geo[-1]
+    windows = n_s * ((last["h"] + 1) // 2) * ((last["w"] + 1) // 2)
+    tail = n_s <= head_rows and windows <= 4 * (256 // (F // 4))
+    chunks = []
+    for l in range(1, L):
+        rows = n_s * (geo[l]["h"] + 1) * (geo[l]["w"] + 1)
+        nch = min(64, max(1, num_sms // (3 * tasks)), max(1, (rows + 15) // 16))
+        rpc = ((rows + nch - 1) // nch + 15) // 16 * 16
+        chunks.append((rows + rpc - 1) // rpc)
+    return dict(tc=tc, tail=tail, ring=min(rings) if rings else None, chunks=max(chunks) if chunks else None)
+
+
+def norm_grid_regimes(a, tasks, num_sms=H100_SMS):
+    """The regimes the grids of the normalisation kernels reach in one iteration (every block, support and target pass),
+    from bn_grid / ln_grid (kernels_bn.cu) and the inner-loop-BatchNorm reduce cap (launch_bnbwd_ibn):
+      ibn_reduce_capped: a BatchNorm pass needs more CTAs per task than num_sms, the reduce's cap;
+      ibn_apply_capped:  it needs more than 4 * num_sms, bn_grid's cap (apply, forward and tangent kernels);
+      ln_one_cta:        ln_grid's cap max(1, 4 * num_sms / (n * tasks)) is 1 and an image needs more;
+      ln_capped:         that cap is above 1 and an image needs more."""
+    geo, _ = geometry(a)
+    F, N = int(a.cnn_num_filters), int(a.num_classes_per_set)
+    wpb = 256 // (F // 4)
+    out = set()
+    for n in (N * int(a.num_samples_per_class), N * int(a.num_target_samples)):
+        for gl in geo:
+            per_img = ((gl["h"] + 1) // 2) * ((gl["w"] + 1) // 2)
+            bx = (n * per_img + wpb - 1) // wpb
+            if bx > num_sms:
+                out.add("ibn_reduce_capped")
+            if bx > 4 * num_sms:
+                out.add("ibn_apply_capped")
+            per_img_ctas = (per_img + wpb - 1) // wpb
+            cap = max(1, 4 * num_sms // max(1, n * tasks))
+            if per_img_ctas > cap:
+                out.add("ln_one_cta" if cap == 1 else "ln_capped")
+    return out
+
+
+def device_sms():
+    """The SM count the host rules see: the GPU's, or an H100's (132) on a machine without one."""
+    return torch.cuda.get_device_properties(0).multi_processor_count if torch.cuda.is_available() else H100_SMS
+
+
+def traced_kernel_ids(m, batch, epoch):
+    """The kernel ids (scripts/trace_kernel_ids.json) of one traced iteration, after an untraced one."""
+    m.meta_gradient(batch, epoch)
+    eng = m._engine
+    eng.trace(True)
+    m.meta_gradient(batch, epoch)
+    tr = eng.trace_read(capacity=1 << 16)
+    eng.trace(False)
+    starts = [k for _, k, _ in tr if not (k & 0x80)]
+    assert len(starts) == eng.last_launch_count()
+    return set(starts)
+
+
+# kernel ids of the device trace: the convolutions, the BatchNorm kernels of the plain path (bnact .. bnbwd_tan_fused,
+# the fused tails, bnact_tan_gb), and the layer-norm (primal, tangent) and inner-loop BatchNorm (primal, tangent) ones
+K_CONV_ROWS, K_WGRAD_ROW, K_CONV_TC, K_WGRAD_TC = 1, 3, 22, 27
+K_BN = set(range(6, 14)) | {23, 24, 25, 32}
+K_LN, K_LN_TAN = {33, 35, 37, 39, 41}, {34, 36, 38, 40, 42}
+K_IBN, K_IBN_TAN = {43, 44, 45}, {46, 47, 48}
+
+
+def check_norm_path(ids, norm, a, epoch, tasks):
+    """The kernel ids of one iteration of a layer-norm (norm "ln") or inner-loop BatchNorm ("ibn") handle: that path's
+    primal kernels, its tangent kernels exactly when the epoch is second order, none of the plain BatchNorm path's or the
+    other path's, and the convolution kernels the host plan chooses."""
+    own, own_tan, other = (K_LN, K_LN_TAN, K_IBN | K_IBN_TAN) if norm == "ln" else (K_IBN, K_IBN_TAN, K_LN | K_LN_TAN)
+    second_order = bool(a.second_order) and epoch > a.first_order_to_second_order_epoch
+    assert own <= ids, sorted(ids)
+    assert (own_tan <= ids) if second_order else not (ids & own_tan), (second_order, sorted(ids))
+    assert not ids & (K_BN | other), sorted(ids & (K_BN | other))
+    plan = host_plan(a, tasks, device_sms())
+    if plan["tc"]:
+        assert {K_CONV_TC, K_WGRAD_TC} <= ids and not ids & {K_CONV_ROWS, K_WGRAD_ROW}, sorted(ids)
+    elif int(a.num_stages) > 1:
+        assert {K_CONV_ROWS, K_WGRAD_ROW} <= ids and not ids & {K_CONV_TC, K_WGRAD_TC}, sorted(ids)
+    else:
+        assert not ids & {K_CONV_ROWS, K_WGRAD_ROW, K_CONV_TC, K_WGRAD_TC}, sorted(ids)
+    return plan
 
 
 def grid_to_nchw(buf, n, h, w, F):

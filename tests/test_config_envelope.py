@@ -20,7 +20,8 @@ import torch.nn.functional as Fnn
 
 import functional_cases as fc
 from conftest import load_golden, grad_tolerance
-from engine_layout import geometry, grid_to_nchw, flat_to_nchw, theta_to_ref, rel_err, gpu_decisions
+from engine_layout import (geometry, grid_to_nchw, flat_to_nchw, theta_to_ref, rel_err, gpu_decisions, host_plan,
+                           traced_kernel_ids)
 from oracle import maml_oracle as O
 
 gpu = pytest.mark.gpu
@@ -58,45 +59,11 @@ ENVELOPE = {
 CASES = list(ENVELOPE)
 MOVED = [c for c in CASES if c.startswith("env_moved_")]
 BERNOULLI = ["env_bern_nonsquare"]
-H100_SMS = 132
 SWEEP_TOL = 5e-5       # reverse sweep and tangent pass taps, of max-norm (test_stagewise_with_gpu_decisions)
 
 # kernel ids of the device trace (scripts/trace_kernel_ids.json)
 K_CONV_ROWS, K_CONV0, K_WGRAD_ROW, K_WGRAD0 = 1, 2, 3, 4
 K_HEAD, K_CONV_TC, K_TAIL, K_TAIL_TAN, K_TAIL_ONCHIP, K_WGRAD_TC = 14, 22, 23, 24, 25, 27
-
-
-# ----------------------------------------------------------------------------------------------------------------------
-# the host rules of maml_b200_create / plan_chunks / tail_fusable, restated (engine.cu, kernels_tc.cu, kernels_bn.cu)
-# ----------------------------------------------------------------------------------------------------------------------
-def _tc_rpad(gw):
-    return (128 + 2 * (gw + 1) + 7) // 8 * 8
-
-
-def _tc_ring(F, gw):
-    row = (F + 4) * 4
-    extra = 128 * row + (128 // 2) * row              # split-K over 2 CTAs in tangent mode
-    avail = 227 * 1024 - 4096 - 1024 - 4 * _tc_rpad(gw) * 128 - extra
-    return min(8, avail // (2 * F * 128))
-
-
-def host_plan(a, tasks, num_sms=H100_SMS):
-    geo, _ = geometry(a)
-    L, F = len(geo), int(a.cnn_num_filters)
-    n_s = int(a.num_classes_per_set) * int(a.num_samples_per_class)
-    rings = [_tc_ring(F, geo[l]["w"] + 1) for l in range(1, L)]
-    tc = L > 1 and all(_tc_rpad(geo[l]["w"] + 1) <= 256 for l in range(1, L)) and min(rings) >= 2
-    head_rows = 16 if n_s <= 16 else 4
-    last = geo[-1]
-    windows = n_s * ((last["h"] + 1) // 2) * ((last["w"] + 1) // 2)
-    tail = n_s <= head_rows and windows <= 4 * (256 // (F // 4))
-    chunks = []
-    for l in range(1, L):
-        rows = n_s * (geo[l]["h"] + 1) * (geo[l]["w"] + 1)
-        nch = min(64, max(1, num_sms // (3 * tasks)), max(1, (rows + 15) // 16))
-        rpc = ((rows + nch - 1) // nch + 15) // 16 * 16
-        chunks.append((rows + rpc - 1) // rpc)
-    return dict(tc=tc, tail=tail, ring=min(rings) if rings else None, chunks=max(chunks) if chunks else None)
 
 
 def _tasks(g):
@@ -235,21 +202,12 @@ def test_path_reached(case, cuda_device):
     """The kernels one iteration actually launches (device trace) are those of the case's declared path."""
     g = load_golden(case)
     a = g.args
-    m = _model(g, cuda_device)
     batch, epoch = g.batch(0), g.iters[0][0]
-    m.meta_gradient(batch, epoch)
-    eng = m._engine
-    eng.trace(True)
-    m.meta_gradient(batch, epoch)
-    tr = eng.trace_read(capacity=1 << 16)
-    eng.trace(False)
-    ids = {k for _, k, _ in tr if not (k & 0x80)}
-    starts = [k for _, k, _ in tr if not (k & 0x80)]
-    assert len(starts) == eng.last_launch_count()
+    ids = traced_kernel_ids(_model(g, cuda_device), batch, epoch)
     want = ENVELOPE[case][1]
     plan = host_plan(a, _tasks(g), torch.cuda.get_device_properties(cuda_device).multi_processor_count)
     L = int(a.num_stages)
-    print("\n[%s] %s: %d launches, kernel ids %s, host plan %s" % (case, ENVELOPE[case][0], len(starts), sorted(ids), plan))
+    print("\n[%s] %s: kernel ids %s, host plan %s" % (case, ENVELOPE[case][0], sorted(ids), plan))
     assert {K_CONV0, K_WGRAD0, K_HEAD} <= ids
     if want["tc"]:
         assert {K_CONV_TC, K_WGRAD_TC} <= ids and not ids & {K_CONV_ROWS, K_WGRAD_ROW}, sorted(ids)

