@@ -254,22 +254,14 @@ void launch_conv0(const Conv0Args& a, cudaStream_t st, const float* X2 = nullptr
 void launch_wgrad(const WgradArgs& a, cudaStream_t st);
 void launch_wgrad0(const WgradArgs& a, cudaStream_t st);     // nsrc = 2: pair 1 adds A[1] (x) D[1]; the bias row sums D[0]
 void launch_input_grad0(const InputGradArgs& a, cudaStream_t st);
-void launch_bnact(const BnActArgs& a, cudaStream_t st);
-// gdot / bdot (nullable, [F]): tangents of gamma / beta, pdot = slope * (gamma zhdot + gdot zh + bdot) at the arg-max
-void launch_bnact_tan(const BnActTanArgs& a, cudaStream_t st, const float* gdot = nullptr, const float* bdot = nullptr);
-void launch_bnbwd_reduce(const BnBwdArgs& a, cudaStream_t st);
-void launch_bnbwd_apply(const BnBwdArgs& a, cudaStream_t st);
-void launch_bnbwd_tan_reduce(const BnBwdTanArgs& a, cudaStream_t st);
-void launch_bnbwd_tan_apply(const BnBwdTanArgs& a, cudaStream_t st);
-void launch_bnbwd(const BnBwdArgs& a, cudaStream_t st);          // reduce + apply (one cluster kernel for small blocks)
-void launch_bnbwd_tan(const BnBwdTanArgs& a, cudaStream_t st);
-// inner-loop BatchNorm gamma / beta (fast weights, read per task: task t's at gamma / beta + t * gb_stride), always as the
-// unfused streaming kernels.  gdot / bdot: their tangents, same stride; the tangent backward adds r * gdot * (dy - S1/m -
-// zh * S2/m) to dzdot
-void launch_bnact_ibn(const BnActArgs& a, long long gb_stride, cudaStream_t st);
-void launch_bnbwd_ibn(const BnBwdArgs& a, long long gb_stride, cudaStream_t st);
-void launch_bnact_tan_ibn(const BnActTanArgs& a, long long gb_stride, const float* gdot, const float* bdot, cudaStream_t st);
-void launch_bnbwd_tan_ibn(const BnBwdTanArgs& a, long long gb_stride, const float* gdot, cudaStream_t st);
+// BatchNorm.  gb_stride 0: gamma / beta shared by the tasks.  Otherwise inner-loop gamma / beta (fast weights), task t's at
+// gamma / beta + t * gb_stride, always on the unfused streaming kernels.  gdot / bdot: tangents of gamma / beta at the same
+// stride, so pdot = slope * (gamma zhdot + gdot zh + bdot) at the arg-max; nullable when gb_stride is 0.  With gb_stride the
+// tangent backward also adds r * gdot * (dy - S1/m - zh * S2/m) to dzdot; without, it reads no gdot.
+void launch_bnact(const BnActArgs& a, long long gb_stride, cudaStream_t st);
+void launch_bnact_tan(const BnActTanArgs& a, const float* gdot, const float* bdot, long long gb_stride, cudaStream_t st);
+void launch_bnbwd(const BnBwdArgs& a, long long gb_stride, cudaStream_t st);   // reduce + apply (one cluster kernel for small blocks)
+void launch_bnbwd_tan(const BnBwdTanArgs& a, const float* gdot, long long gb_stride, cudaStream_t st);
 // layer norm (kernels_bn.cu).  tan = false: primal forward / backward; true: their forward-mode tangents
 void launch_ln_stats(const LnArgs& a, bool tan, cudaStream_t st);   // per-image sums of z (or of zdot and zh * zdot)
 void launch_ln_act(const LnArgs& a, bool tan, cudaStream_t st);     // normalise, + bias, leaky-ReLU, max-pool (+ bdot)

@@ -859,8 +859,7 @@ static void norm_forward(maml_b200_handle* h, const PassSet& ps, int slot, const
   if (h->use_tc && l + 1 < h->L) { b.p_hi = AIN_HI(ps, l + 1, slot); b.p_lo = AIN_LO(ps, l + 1, slot); }
   b.g = bn_geom(h, l, ps.n); b.tasks = T;
   if (defer_last && l == h->L - 1) *defer_last = b;
-  else if (np.stride) launch_bnact_ibn(b, np.stride, st);
-  else launch_bnact(b, st);
+  else launch_bnact(b, np.stride, st);
 }
 
 static void norm_backward(maml_b200_handle* h, const PassSet& ps, int slot, const float* theta, const float* meta, int l, int step,
@@ -890,8 +889,7 @@ static void norm_backward(maml_b200_handle* h, const PassSet& ps, int slot, cons
   if (h->use_tc && l >= 1) { b.dz_hi = DZ_HI(ps, l, slot); b.dz_lo = DZ_LO(ps, l, slot); }
   b.g = bn_geom(h, l, ps.n); b.tasks = T;
   if (fused_head && l == h->L - 1) launch_tail_fused(*fused_act, *fused_head, b, st);
-  else if (np.stride) launch_bnbwd_ibn(b, np.stride, st);
-  else launch_bnbwd(b, st);
+  else launch_bnbwd(b, np.stride, st);
 }
 
 // inner_bn: gamma / beta are theta's and their tangents u's (per task); t_norm is then not read
@@ -922,9 +920,10 @@ static void norm_tangent_forward(maml_b200_handle* h, int s, const float* theta,
   b.pdot = AIN(tn, l + 1, 0); b.pdot_stride = STRIDE(tn, ain, l + 1);
   if (h->use_tc && l + 1 < h->L) { b.pdot_hi = AIN_HI(tn, l + 1, 0); b.pdot_lo = AIN_LO(tn, l + 1, 0); }
   b.g = bn_geom(h, l, sp.n); b.tasks = T;
+  const float* gdot = np.stride ? u + h->pl.gamma_off[l] : t_norm ? gamma_at(h, t_norm, l, s) : nullptr;
+  const float* bdot = np.stride ? u + h->pl.beta_off[l] : t_norm ? beta_at(h, t_norm, l, s) : nullptr;
   if (defer_last && l == h->L - 1) *defer_last = b;
-  else if (np.stride) launch_bnact_tan_ibn(b, np.stride, u + h->pl.gamma_off[l], u + h->pl.beta_off[l], st);
-  else launch_bnact_tan(b, st, t_norm ? gamma_at(h, t_norm, l, s) : nullptr, t_norm ? beta_at(h, t_norm, l, s) : nullptr);
+  else launch_bnact_tan(b, gdot, bdot, np.stride, st);
 }
 
 static void norm_tangent_backward(maml_b200_handle* h, int s, const float* theta, const float* u, const float* meta, int l,
@@ -967,8 +966,7 @@ static void norm_tangent_backward(maml_b200_handle* h, int s, const float* theta
   if (h->use_tc && l >= 1) { b.dzdot_hi = DZ_HI(tn, l, 0); b.dzdot_lo = DZ_LO(tn, l, 0); }
   b.g = bn_geom(h, l, sp.n); b.tasks = T;
   if (fused_head && l == h->L - 1) launch_tail_tan_fused(*fused_act, *fused_head, b, st);
-  else if (np.stride) launch_bnbwd_tan_ibn(b, np.stride, u + h->pl.gamma_off[l], st);
-  else launch_bnbwd_tan(b, st);
+  else launch_bnbwd_tan(b, np.stride ? u + h->pl.gamma_off[l] : nullptr, np.stride, st);
 }
 
 // primal forward of one pass: conv -> stats -> BN/leaky/pool for every block

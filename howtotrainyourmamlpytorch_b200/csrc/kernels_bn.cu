@@ -306,12 +306,17 @@ __device__ __forceinline__ void bnact_phase(const BnActArgs& a, const BnGeom& g,
   }
 }
 
-__global__ void __launch_bounds__(256) bnact_kernel(BnActArgs a) {
-  pdl_prologue(6, a.tag);
+// PT (this kernel and the five streaming kernels below): gamma / beta per task (inner-loop gamma / beta: fast weights), task
+// t's at gamma / beta + t * gbs.  gbs is a trailing kernel parameter, so the Bn*Args structs keep their layout.
+template <bool PT>
+__global__ void __launch_bounds__(256) bnact_kernel(BnActArgs a, long long gbs) {
+  pdl_prologue(PT ? 43 : 6, a.tag);
   __shared__ float s_mu[64], s_r[64], s_g[64], s_b[64];
   const BnGeom g = a.g;
   const int task = blockIdx.y;
-  chan_setup(a.stats + (long long)task * a.stats_stride, a.gamma, a.beta, (double)g.n * g.h * g.w, g.F, s_mu, s_r, s_g, s_b);
+  const long long go = PT ? (long long)task * gbs : 0;
+  chan_setup(a.stats + (long long)task * a.stats_stride, a.gamma + go, a.beta + go, (double)g.n * g.h * g.w, g.F, s_mu, s_r,
+             s_g, s_b);
   __syncthreads();
   WinIter it(g);
   bnact_phase(a, g, task, blockIdx.x, gridDim.x, it, s_mu, s_r, s_g, s_b);
@@ -333,10 +338,10 @@ static inline dim3 bn_grid(const BnGeom& g, int tasks, int* block) {
   return dim3(bx, tasks);
 }
 
-void launch_bnact(const BnActArgs& a, cudaStream_t st) {
+void launch_bnact(const BnActArgs& a, long long gb_stride, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
   int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
-  launch_pdl(bnact_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
+  launch_pdl(gb_stride ? bnact_kernel<true> : bnact_kernel<false>, dim3(grid), dim3(block), (size_t)(0), st, tagged(a), gb_stride);
   CUDA_CHECK_LAUNCH();
 }
 
@@ -420,12 +425,14 @@ __device__ __forceinline__ void bnbwd_reduce_phase(const BnBwdArgs& a, const BnG
   }
 }
 
-__global__ void __launch_bounds__(256) bnbwd_reduce_kernel(BnBwdArgs a) {
-  pdl_prologue(7, a.tag);
+template <bool PT>
+__global__ void __launch_bounds__(256) bnbwd_reduce_kernel(BnBwdArgs a, long long gbs) {
+  pdl_prologue(PT ? 44 : 7, a.tag);
   __shared__ float s_g[64], s_b[64];
   const BnGeom g = a.g;
   const int task = blockIdx.y;
-  if (threadIdx.x < g.F) { s_g[threadIdx.x] = a.gamma[threadIdx.x]; s_b[threadIdx.x] = a.beta[threadIdx.x]; }
+  const long long go = PT ? (long long)task * gbs : 0;
+  if (threadIdx.x < g.F) { s_g[threadIdx.x] = (a.gamma + go)[threadIdx.x]; s_b[threadIdx.x] = (a.beta + go)[threadIdx.x]; }
   __syncthreads();
   WinIter it(g);
   double s1[4] = {0, 0, 0, 0}, s2[4] = {0, 0, 0, 0};
@@ -433,11 +440,12 @@ __global__ void __launch_bounds__(256) bnbwd_reduce_kernel(BnBwdArgs a) {
   block_reduce_stats(s1, s2, it, a.stats_bwd + (long long)task * a.stats_bwd_stride, g.F);
 }
 
-void launch_bnbwd_reduce(const BnBwdArgs& a, cudaStream_t st) {
+static void launch_bnbwd_reduce(const BnBwdArgs& a, long long gb_stride, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
   int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
   if ((int)grid.x > num_sms()) grid.x = num_sms();
-  launch_pdl(bnbwd_reduce_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
+  launch_pdl(gb_stride ? bnbwd_reduce_kernel<true> : bnbwd_reduce_kernel<false>, dim3(grid), dim3(block), (size_t)(0), st,
+             tagged(a), gb_stride);
   CUDA_CHECK_LAUNCH();
 }
 
@@ -459,13 +467,15 @@ __device__ __forceinline__ void bnbwd_apply_phase(const BnBwdArgs& a, const BnGe
   }
 }
 
-__global__ void __launch_bounds__(256) bnbwd_apply_kernel(BnBwdArgs a) {
-  pdl_prologue(8, a.tag);
+template <bool PT>
+__global__ void __launch_bounds__(256) bnbwd_apply_kernel(BnBwdArgs a, long long gbs) {
+  pdl_prologue(PT ? 45 : 8, a.tag);
   __shared__ float s_mu[64], s_r[64], s_g[64], s_b[64], s_c1[64], s_c2[64];
   const BnGeom g = a.g;
   const int task = blockIdx.y;
   const double m = (double)g.n * g.h * g.w;
-  chan_setup(a.stats_fwd + (long long)task * a.stats_fwd_stride, a.gamma, a.beta, m, g.F, s_mu, s_r, s_g, s_b);
+  const long long go = PT ? (long long)task * gbs : 0;
+  chan_setup(a.stats_fwd + (long long)task * a.stats_fwd_stride, a.gamma + go, a.beta + go, m, g.F, s_mu, s_r, s_g, s_b);
   if (threadIdx.x < g.F) {
     const double* sb = a.stats_bwd + (long long)task * a.stats_bwd_stride;
     s_c1[threadIdx.x] = (float)(sb[threadIdx.x * 2] / m);
@@ -517,28 +527,32 @@ static inline void launch_cluster(void (*kernel)(A), const A& a, int cl, int tas
   cudaLaunchKernelEx(&cfg, kernel, a);
 }
 
-// BatchNorm backward of one block (reduce + apply), fused into one cluster kernel when the block is small
-void launch_bnbwd(const BnBwdArgs& a, cudaStream_t st) {
-  const int cl = bn_fused_cluster(a.g);
-  if (cl == 0) { launch_bnbwd_reduce(a, st); launch_bnbwd_apply(a, st); return; }
+static void launch_bnbwd_apply(const BnBwdArgs& a, long long gb_stride, cudaStream_t st) {
+  ProfScope prof_scope__(PROF_BN, 0.0, st);
+  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
+  launch_pdl(gb_stride ? bnbwd_apply_kernel<true> : bnbwd_apply_kernel<false>, dim3(grid), dim3(block), (size_t)(0), st,
+             tagged(a), gb_stride);
+  CUDA_CHECK_LAUNCH();
+}
+
+// BatchNorm backward of one block (reduce + apply), fused into one cluster kernel when the block is small and gamma / beta
+// are shared: the cluster kernels (and the tail kernels) read shared gamma / beta only, so per-task ones (gb_stride != 0)
+// always take the two streaming kernels
+void launch_bnbwd(const BnBwdArgs& a, long long gb_stride, cudaStream_t st) {
+  const int cl = gb_stride ? 0 : bn_fused_cluster(a.g);
+  if (cl == 0) { launch_bnbwd_reduce(a, gb_stride, st); launch_bnbwd_apply(a, gb_stride, st); return; }
   ProfScope prof_scope__(PROF_BN, 0.0, st);
   int block; bn_grid(a.g, a.tasks, &block);
   launch_cluster(bnbwd_fused_kernel, tagged(a), cl, a.tasks, block, st);
   CUDA_CHECK_LAUNCH();
 }
 
-void launch_bnbwd_apply(const BnBwdArgs& a, cudaStream_t st) {
-  ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
-  launch_pdl(bnbwd_apply_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
-  CUDA_CHECK_LAUNCH();
-}
-
 // ------------------------------------------------------------------------------- tangent forward
-// zhdot = r * (zdot - mean(zdot) - zh * mean(zh * zdot));  pdot = slope * gamma * zhdot at the arg-max
+// zhdot = r * (zdot - mean(zdot) - zh * mean(zh * zdot));  pdot = slope * gamma * zhdot at the arg-max.  go: the task's
+// offset of gamma / beta
 __device__ __forceinline__ void bnact_tan_setup(const BnActTanArgs& a, const BnGeom& g, int task, double m, float* s_mu, float* s_r,
-                                                float* s_g, float* s_b, float* s_md, float* s_q) {
-  chan_setup(a.stats_fwd + (long long)task * a.stats_fwd_stride, a.gamma, a.beta, m, g.F, s_mu, s_r, s_g, s_b);
+                                                float* s_g, float* s_b, float* s_md, float* s_q, long long go = 0) {
+  chan_setup(a.stats_fwd + (long long)task * a.stats_fwd_stride, a.gamma + go, a.beta + go, m, g.F, s_mu, s_r, s_g, s_b);
   if (threadIdx.x < g.F) {
     const double* stt = a.stats_tan + (long long)task * a.stats_tan_stride;
     s_md[threadIdx.x] = (float)(stt[threadIdx.x * 2] / m);
@@ -582,36 +596,27 @@ __device__ __forceinline__ void bnact_tan_phase(const BnActTanArgs& a, const BnG
   }
 }
 
-__global__ void __launch_bounds__(256) bnact_tan_kernel(BnActTanArgs a) {
-  pdl_prologue(10, a.tag);
-  __shared__ float s_mu[64], s_r[64], s_g[64], s_b[64], s_md[64], s_q[64];
-  const BnGeom g = a.g;
-  const int task = blockIdx.y;
-  bnact_tan_setup(a, g, task, (double)g.n * g.h * g.w, s_mu, s_r, s_g, s_b, s_md, s_q);
-  __syncthreads();
-  WinIter it(g);
-  bnact_tan_phase(a, g, task, blockIdx.x, gridDim.x, it, s_r, s_g, s_b, s_md, s_q);
-}
-
-// forward tangent with gamma / beta tangents (functional operator's forward mode); a kernel of its own, so that the
-// fused iteration's bnact_tan_kernel keeps its code
-__global__ void __launch_bounds__(256) bnact_tan_gb_kernel(BnActTanArgs a, const float* gdot, const float* bdot) {
-  pdl_prologue(32, a.tag);
+// GB: gamma / beta carry tangents gdot / bdot, read like gamma / beta (the functional operator's forward mode; with PT, the
+// inner loop's gamma / beta along u)
+template <bool GB, bool PT>
+__global__ void __launch_bounds__(256) bnact_tan_kernel(BnActTanArgs a, const float* gdot, const float* bdot, long long gbs) {
+  pdl_prologue(PT ? 46 : GB ? 32 : 10, a.tag);
   __shared__ float s_mu[64], s_r[64], s_g[64], s_b[64], s_md[64], s_q[64], s_gd[64], s_bd[64];
   const BnGeom g = a.g;
   const int task = blockIdx.y;
-  bnact_tan_setup(a, g, task, (double)g.n * g.h * g.w, s_mu, s_r, s_g, s_b, s_md, s_q);
-  if (threadIdx.x < g.F) { s_gd[threadIdx.x] = gdot[threadIdx.x]; s_bd[threadIdx.x] = bdot[threadIdx.x]; }
+  const long long go = PT ? (long long)task * gbs : 0;
+  bnact_tan_setup(a, g, task, (double)g.n * g.h * g.w, s_mu, s_r, s_g, s_b, s_md, s_q, go);
+  if (GB && threadIdx.x < g.F) { s_gd[threadIdx.x] = (gdot + go)[threadIdx.x]; s_bd[threadIdx.x] = (bdot + go)[threadIdx.x]; }
   __syncthreads();
   WinIter it(g);
-  bnact_tan_phase<true>(a, g, task, blockIdx.x, gridDim.x, it, s_r, s_g, s_b, s_md, s_q, s_gd, s_bd);
+  bnact_tan_phase<GB>(a, g, task, blockIdx.x, gridDim.x, it, s_r, s_g, s_b, s_md, s_q, s_gd, s_bd);
 }
 
-void launch_bnact_tan(const BnActTanArgs& a, cudaStream_t st, const float* gdot, const float* bdot) {
+void launch_bnact_tan(const BnActTanArgs& a, const float* gdot, const float* bdot, long long gb_stride, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
   int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
-  if (gdot) launch_pdl(bnact_tan_gb_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a), gdot, bdot);
-  else launch_pdl(bnact_tan_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
+  const auto kernel = gb_stride ? bnact_tan_kernel<true, true> : gdot ? bnact_tan_kernel<true, false> : bnact_tan_kernel<false, false>;
+  launch_pdl(kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a), gdot, bdot, gb_stride);
   CUDA_CHECK_LAUNCH();
 }
 
@@ -633,12 +638,14 @@ __device__ __forceinline__ void bnbwd_tan_reduce_phase(const BnBwdTanArgs& a, co
   }
 }
 
-__global__ void __launch_bounds__(256) bnbwd_tan_reduce_kernel(BnBwdTanArgs a) {
-  pdl_prologue(11, a.tag);
+template <bool PT>
+__global__ void __launch_bounds__(256) bnbwd_tan_reduce_kernel(BnBwdTanArgs a, long long gbs) {
+  pdl_prologue(PT ? 47 : 11, a.tag);
   __shared__ float s_g[64], s_b[64];
   const BnGeom g = a.g;
   const int task = blockIdx.y;
-  if (threadIdx.x < g.F) { s_g[threadIdx.x] = a.gamma[threadIdx.x]; s_b[threadIdx.x] = a.beta[threadIdx.x]; }
+  const long long go = PT ? (long long)task * gbs : 0;
+  if (threadIdx.x < g.F) { s_g[threadIdx.x] = (a.gamma + go)[threadIdx.x]; s_b[threadIdx.x] = (a.beta + go)[threadIdx.x]; }
   __syncthreads();
   WinIter it(g);
   double s1[4] = {0, 0, 0, 0}, s2[4] = {0, 0, 0, 0};
@@ -646,11 +653,12 @@ __global__ void __launch_bounds__(256) bnbwd_tan_reduce_kernel(BnBwdTanArgs a) {
   block_reduce_stats(s1, s2, it, a.stats_tbwd + (long long)task * a.stats_tbwd_stride, g.F);
 }
 
-void launch_bnbwd_tan_reduce(const BnBwdTanArgs& a, cudaStream_t st) {
+static void launch_bnbwd_tan_reduce(const BnBwdTanArgs& a, long long gb_stride, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
   int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
   if ((int)grid.x > num_sms()) grid.x = num_sms();
-  launch_pdl(bnbwd_tan_reduce_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
+  launch_pdl(gb_stride ? bnbwd_tan_reduce_kernel<true> : bnbwd_tan_reduce_kernel<false>, dim3(grid), dim3(block), (size_t)(0),
+             st, tagged(a), gb_stride);
   CUDA_CHECK_LAUNCH();
 }
 
@@ -718,8 +726,8 @@ __device__ __forceinline__ void bnbwd_tan_apply_phase(const BnBwdTanArgs& a, con
 }
 
 __device__ __forceinline__ void bnbwd_tan_setup(const BnBwdTanArgs& a, const BnGeom& g, int task, double m, float* s_mu, float* s_r,
-                                                float* s_g, float* s_b, float* s_q, float* s_c2) {
-  chan_setup(a.stats_fwd + (long long)task * a.stats_fwd_stride, a.gamma, a.beta, m, g.F, s_mu, s_r, s_g, s_b);
+                                                float* s_g, float* s_b, float* s_q, float* s_c2, long long go = 0) {
+  chan_setup(a.stats_fwd + (long long)task * a.stats_fwd_stride, a.gamma + go, a.beta + go, m, g.F, s_mu, s_r, s_g, s_b);
   if (threadIdx.x < g.F) {
     const int c = threadIdx.x;
     s_q[c] = (float)((a.stats_tan + (long long)task * a.stats_tan_stride)[c * 2 + 1] / m);
@@ -727,22 +735,29 @@ __device__ __forceinline__ void bnbwd_tan_setup(const BnBwdTanArgs& a, const BnG
   }
 }
 
-__global__ void __launch_bounds__(256) bnbwd_tan_apply_kernel(BnBwdTanArgs a) {
-  pdl_prologue(12, a.tag);
-  __shared__ float s_mu[64], s_r[64], s_g[64], s_b[64], s_q[64], s_c2[64], s_t1[64], s_t2[64];
+// PT: also the gamma-tangent term (bnbwd_tan_apply_phase<GD>), gdot read like gamma
+template <bool PT>
+__global__ void __launch_bounds__(256) bnbwd_tan_apply_kernel(BnBwdTanArgs a, const float* gdot, long long gbs) {
+  pdl_prologue(PT ? 48 : 12, a.tag);
+  __shared__ float s_mu[64], s_r[64], s_g[64], s_b[64], s_q[64], s_c2[64], s_t1[64], s_t2[64], s_gd[64], s_c1[64];
   const BnGeom g = a.g;
   const int task = blockIdx.y;
   const double m = (double)g.n * g.h * g.w;
-  bnbwd_tan_setup(a, g, task, m, s_mu, s_r, s_g, s_b, s_q, s_c2);
+  const long long go = PT ? (long long)task * gbs : 0;
+  bnbwd_tan_setup(a, g, task, m, s_mu, s_r, s_g, s_b, s_q, s_c2, go);
   if (threadIdx.x < g.F) {
     const int c = threadIdx.x;
     const double* tb = a.stats_tbwd + (long long)task * a.stats_tbwd_stride;
     s_t1[c] = (float)(tb[c * 2] / m);
     s_t2[c] = (float)(tb[c * 2 + 1] / m);
+    if (PT) {
+      s_c1[c] = (float)((a.stats_bwd + (long long)task * a.stats_bwd_stride)[c * 2] / m);
+      s_gd[c] = (gdot + go)[c];
+    }
   }
   __syncthreads();
   WinIter it(g);
-  bnbwd_tan_apply_phase(a, g, task, blockIdx.x, gridDim.x, it, s_r, s_g, s_b, s_q, s_c2, s_t1, s_t2);
+  bnbwd_tan_apply_phase<PT>(a, g, task, blockIdx.x, gridDim.x, it, s_r, s_g, s_b, s_q, s_c2, s_t1, s_t2, s_gd, s_c1);
 }
 
 __global__ void __launch_bounds__(256) bnbwd_tan_fused_kernel(BnBwdTanArgs a) {
@@ -763,167 +778,21 @@ __global__ void __launch_bounds__(256) bnbwd_tan_fused_kernel(BnBwdTanArgs a) {
   bnbwd_tan_apply_phase(a, g, task, blockIdx.x, gridDim.x, it, s_r, s_g, s_b, s_q, s_c2, s_t1, s_t2);
 }
 
-void launch_bnbwd_tan_apply(const BnBwdTanArgs& a, cudaStream_t st) {
+static void launch_bnbwd_tan_apply(const BnBwdTanArgs& a, const float* gdot, long long gb_stride, cudaStream_t st) {
   ProfScope prof_scope__(PROF_BN, 0.0, st);
   int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
-  launch_pdl(bnbwd_tan_apply_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a));
+  launch_pdl(gb_stride ? bnbwd_tan_apply_kernel<true> : bnbwd_tan_apply_kernel<false>, dim3(grid), dim3(block), (size_t)(0), st,
+             tagged(a), gdot, gb_stride);
   CUDA_CHECK_LAUNCH();
 }
 
-void launch_bnbwd_tan(const BnBwdTanArgs& a, cudaStream_t st) {
-  const int cl = bn_fused_cluster(a.g);
-  if (cl == 0) { launch_bnbwd_tan_reduce(a, st); launch_bnbwd_tan_apply(a, st); return; }
+// per-task gamma / beta (gb_stride != 0) take the two streaming kernels, as in launch_bnbwd
+void launch_bnbwd_tan(const BnBwdTanArgs& a, const float* gdot, long long gb_stride, cudaStream_t st) {
+  const int cl = gb_stride ? 0 : bn_fused_cluster(a.g);
+  if (cl == 0) { launch_bnbwd_tan_reduce(a, gb_stride, st); launch_bnbwd_tan_apply(a, gdot, gb_stride, st); return; }
   ProfScope prof_scope__(PROF_BN, 0.0, st);
   int block; bn_grid(a.g, a.tasks, &block);
   launch_cluster(bnbwd_tan_fused_kernel, tagged(a), cl, a.tasks, block, st);
-  CUDA_CHECK_LAUNCH();
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Inner-loop gamma / beta (enable_inner_loop_optimizable_bn_params): gamma and beta are fast weights, so every task has its
-// own pair, at gamma / beta + task * gbs (gbs: the fast-weight vectors' stride).  The kernels below run the streaming
-// phases above with the task's pair; the tangent backward adds the one term that shared gamma / beta do not have.  Handles
-// without the flag never launch them.
-__device__ __forceinline__ void ibn_load(const float* __restrict__ src, long long gbs, int task, int F, float* s) {
-  if (threadIdx.x < F) s[threadIdx.x] = src[(long long)task * gbs + threadIdx.x];
-}
-
-__global__ void __launch_bounds__(256) bnact_ibn_kernel(BnActArgs a, long long gbs) {
-  pdl_prologue(43, a.tag);
-  __shared__ float s_mu[64], s_r[64], s_g[64], s_b[64];
-  const BnGeom g = a.g;
-  const int task = blockIdx.y;
-  chan_setup(a.stats + (long long)task * a.stats_stride, a.gamma + (long long)task * gbs, a.beta + (long long)task * gbs,
-             (double)g.n * g.h * g.w, g.F, s_mu, s_r, s_g, s_b);
-  __syncthreads();
-  WinIter it(g);
-  bnact_phase(a, g, task, blockIdx.x, gridDim.x, it, s_mu, s_r, s_g, s_b);
-}
-
-__global__ void __launch_bounds__(256) bnbwd_reduce_ibn_kernel(BnBwdArgs a, long long gbs) {
-  pdl_prologue(44, a.tag);
-  __shared__ float s_g[64], s_b[64];
-  const BnGeom g = a.g;
-  const int task = blockIdx.y;
-  ibn_load(a.gamma, gbs, task, g.F, s_g);
-  ibn_load(a.beta, gbs, task, g.F, s_b);
-  __syncthreads();
-  WinIter it(g);
-  double s1[4] = {0, 0, 0, 0}, s2[4] = {0, 0, 0, 0};
-  bnbwd_reduce_phase(a, g, task, blockIdx.x, gridDim.x, it, s_g, s_b, s1, s2);
-  block_reduce_stats(s1, s2, it, a.stats_bwd + (long long)task * a.stats_bwd_stride, g.F);
-}
-
-__global__ void __launch_bounds__(256) bnbwd_apply_ibn_kernel(BnBwdArgs a, long long gbs) {
-  pdl_prologue(45, a.tag);
-  __shared__ float s_mu[64], s_r[64], s_g[64], s_b[64], s_c1[64], s_c2[64];
-  const BnGeom g = a.g;
-  const int task = blockIdx.y;
-  const double m = (double)g.n * g.h * g.w;
-  chan_setup(a.stats_fwd + (long long)task * a.stats_fwd_stride, a.gamma + (long long)task * gbs, a.beta + (long long)task * gbs,
-             m, g.F, s_mu, s_r, s_g, s_b);
-  if (threadIdx.x < g.F) {
-    const double* sb = a.stats_bwd + (long long)task * a.stats_bwd_stride;
-    s_c1[threadIdx.x] = (float)(sb[threadIdx.x * 2] / m);
-    s_c2[threadIdx.x] = (float)(sb[threadIdx.x * 2 + 1] / m);
-  }
-  __syncthreads();
-  WinIter it(g);
-  bnbwd_apply_phase(a, g, task, blockIdx.x, gridDim.x, it, s_r, s_g, s_b, s_c1, s_c2);
-}
-
-void launch_bnact_ibn(const BnActArgs& a, long long gb_stride, cudaStream_t st) {
-  ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
-  launch_pdl(bnact_ibn_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a), gb_stride);
-  CUDA_CHECK_LAUNCH();
-}
-
-void launch_bnbwd_ibn(const BnBwdArgs& a, long long gb_stride, cudaStream_t st) {
-  ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
-  dim3 rgrid = grid;
-  if ((int)rgrid.x > num_sms()) rgrid.x = num_sms();
-  launch_pdl(bnbwd_reduce_ibn_kernel, dim3(rgrid), dim3(block), (size_t)(0), st, tagged(a), gb_stride);
-  CUDA_CHECK_LAUNCH();
-  launch_pdl(bnbwd_apply_ibn_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a), gb_stride);
-  CUDA_CHECK_LAUNCH();
-}
-
-// forward tangent along the weights and the task's (gdot, bdot): pdot = slope * (gamma zhdot + gdot zh + bdot)
-__global__ void __launch_bounds__(256) bnact_tan_ibn_kernel(BnActTanArgs a, long long gbs, const float* gdot, const float* bdot) {
-  pdl_prologue(46, a.tag);
-  __shared__ float s_mu[64], s_r[64], s_g[64], s_b[64], s_md[64], s_q[64], s_gd[64], s_bd[64];
-  const BnGeom g = a.g;
-  const int task = blockIdx.y;
-  const double m = (double)g.n * g.h * g.w;
-  chan_setup(a.stats_fwd + (long long)task * a.stats_fwd_stride, a.gamma + (long long)task * gbs, a.beta + (long long)task * gbs,
-             m, g.F, s_mu, s_r, s_g, s_b);
-  if (threadIdx.x < g.F) {
-    const double* stt = a.stats_tan + (long long)task * a.stats_tan_stride;
-    s_md[threadIdx.x] = (float)(stt[threadIdx.x * 2] / m);
-    s_q[threadIdx.x] = (float)(stt[threadIdx.x * 2 + 1] / m);
-  }
-  ibn_load(gdot, gbs, task, g.F, s_gd);
-  ibn_load(bdot, gbs, task, g.F, s_bd);
-  __syncthreads();
-  WinIter it(g);
-  bnact_tan_phase<true>(a, g, task, blockIdx.x, gridDim.x, it, s_r, s_g, s_b, s_md, s_q, s_gd, s_bd);
-}
-
-__global__ void __launch_bounds__(256) bnbwd_tan_reduce_ibn_kernel(BnBwdTanArgs a, long long gbs) {
-  pdl_prologue(47, a.tag);
-  __shared__ float s_g[64], s_b[64];
-  const BnGeom g = a.g;
-  const int task = blockIdx.y;
-  ibn_load(a.gamma, gbs, task, g.F, s_g);
-  ibn_load(a.beta, gbs, task, g.F, s_b);
-  __syncthreads();
-  WinIter it(g);
-  double s1[4] = {0, 0, 0, 0}, s2[4] = {0, 0, 0, 0};
-  bnbwd_tan_reduce_phase(a, g, task, blockIdx.x, gridDim.x, it, s_g, s_b, s1, s2);
-  block_reduce_stats(s1, s2, it, a.stats_tbwd + (long long)task * a.stats_tbwd_stride, g.F);
-}
-
-__global__ void __launch_bounds__(256) bnbwd_tan_apply_ibn_kernel(BnBwdTanArgs a, long long gbs, const float* gdot) {
-  pdl_prologue(48, a.tag);
-  __shared__ float s_mu[64], s_r[64], s_g[64], s_b[64], s_q[64], s_c2[64], s_t1[64], s_t2[64], s_gd[64], s_c1[64];
-  const BnGeom g = a.g;
-  const int task = blockIdx.y;
-  const double m = (double)g.n * g.h * g.w;
-  chan_setup(a.stats_fwd + (long long)task * a.stats_fwd_stride, a.gamma + (long long)task * gbs, a.beta + (long long)task * gbs,
-             m, g.F, s_mu, s_r, s_g, s_b);
-  if (threadIdx.x < g.F) {
-    const int c = threadIdx.x;
-    const double* sb = a.stats_bwd + (long long)task * a.stats_bwd_stride;
-    const double* tb = a.stats_tbwd + (long long)task * a.stats_tbwd_stride;
-    s_q[c] = (float)((a.stats_tan + (long long)task * a.stats_tan_stride)[c * 2 + 1] / m);
-    s_c1[c] = (float)(sb[c * 2] / m);
-    s_c2[c] = (float)(sb[c * 2 + 1] / m);
-    s_t1[c] = (float)(tb[c * 2] / m);
-    s_t2[c] = (float)(tb[c * 2 + 1] / m);
-  }
-  ibn_load(gdot, gbs, task, g.F, s_gd);
-  __syncthreads();
-  WinIter it(g);
-  bnbwd_tan_apply_phase<true>(a, g, task, blockIdx.x, gridDim.x, it, s_r, s_g, s_b, s_q, s_c2, s_t1, s_t2, s_gd, s_c1);
-}
-
-void launch_bnact_tan_ibn(const BnActTanArgs& a, long long gb_stride, const float* gdot, const float* bdot, cudaStream_t st) {
-  ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
-  launch_pdl(bnact_tan_ibn_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a), gb_stride, gdot, bdot);
-  CUDA_CHECK_LAUNCH();
-}
-
-void launch_bnbwd_tan_ibn(const BnBwdTanArgs& a, long long gb_stride, const float* gdot, cudaStream_t st) {
-  ProfScope prof_scope__(PROF_BN, 0.0, st);
-  int block; dim3 grid = bn_grid(a.g, a.tasks, &block);
-  dim3 rgrid = grid;
-  if ((int)rgrid.x > num_sms()) rgrid.x = num_sms();
-  launch_pdl(bnbwd_tan_reduce_ibn_kernel, dim3(rgrid), dim3(block), (size_t)(0), st, tagged(a), gb_stride);
-  CUDA_CHECK_LAUNCH();
-  launch_pdl(bnbwd_tan_apply_ibn_kernel, dim3(grid), dim3(block), (size_t)(0), st, tagged(a), gb_stride, gdot);
   CUDA_CHECK_LAUNCH();
 }
 

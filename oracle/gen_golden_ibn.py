@@ -5,7 +5,7 @@
   python oracle/gen_golden_ibn.py               # every case
   python oracle/gen_golden_ibn.py ibn_tiny_pp   # one case
 
-Writes ``tests/golden/<case>.npz`` (with the validation leg) and checks ``oracle/ibn_oracle.py`` against the fp64
+Writes ``tests/golden/<case>.npz`` (with the validation leg) and checks ``oracle/maml_oracle.py`` against the fp64
 reference run at once."""
 import json
 import os
@@ -18,7 +18,6 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
 from oracle import gen_golden as G  # noqa: E402
-from oracle import ibn_oracle as IBN  # noqa: E402
 from oracle import maml_oracle as O  # noqa: E402
 
 _IBN = dict(enable_inner_loop_optimizable_bn_params=True)
@@ -68,7 +67,7 @@ def check_against_oracle(args, blob, iters, kind):
     reference run."""
     state = {k[len("state/"):]: torch.from_numpy(v).double() for k, v in blob.items() if k.startswith("state/")}
     epoch, seed_it = iters[0]
-    res = IBN.autograd_train_iter(state, args, O.synthetic_batch(args, iteration=seed_it, kind=kind), epoch)
+    res = O.autograd_train_iter(state, args, O.synthetic_batch(args, iteration=seed_it, kind=kind), epoch)
     err = abs(float(res["loss"]) - float(blob["it0/loss64"])) / abs(float(blob["it0/loss64"]))
     gerr = 0.0
     for n, g in res["grads"].items():

@@ -85,11 +85,12 @@ def lslr_name(param_name):
 
 
 def inner_param_names(args):
-    """The 10 adaptable tensors, in reference order (few_shot_learning_system.py:105-120)."""
+    """The adaptable tensors, in reference order (few_shot_learning_system.py:105-120): per block conv.weight, conv.bias
+    (with ``enable_inner_loop_optimizable_bn_params`` also norm_layer.bias, norm_layer.weight), then the linear layer."""
     names = []
     for l in range(num_stages(args)):
-        wn, bn_, _, _, _, _ = conv_names(l)
-        names += [wn, bn_]
+        wn, bn_, gn, btn, _, _ = conv_names(l)
+        names += [wn, bn_, btn, gn] if args.enable_inner_loop_optimizable_bn_params else [wn, bn_]
     names += [LIN_W, LIN_B]
     return names
 
@@ -218,8 +219,13 @@ def target_pass_schedule(args, epoch, training_phase, num_steps):
 # ----------------------------------------------------------------------------------------
 # restatement 1: autograd, call for call
 # ----------------------------------------------------------------------------------------
-def _bn_params(state, args, l, step):
+def _bn_params(state, fast, args, l, step):
+    """Block l's BatchNorm gamma / beta at inner step ``step``.  With ``enable_inner_loop_optimizable_bn_params`` they are
+    fast weights, read from ``fast`` without a step index (reference meta_neural_network_architectures.py:194-198,
+    :229-234); otherwise they are ``state``'s, one row per step with per-step statistics."""
     _, _, gn, btn, _, _ = conv_names(l)
+    if args.enable_inner_loop_optimizable_bn_params:
+        return fast[gn], fast[btn]
     g, b = state[gn], state[btn]
     if args.per_step_bn_statistics:
         return g[step], b[step]
@@ -237,7 +243,7 @@ def _net_forward(x, fast, state, args, step, stats_out=None):
                 mu = out.mean(dim=(0, 2, 3))
                 var_unbiased = out.var(dim=(0, 2, 3), unbiased=True) if m > 1 else out.new_zeros(out.shape[1])
                 stats_out.append((l, step, mu, var_unbiased))
-        g, b = _bn_params(state, args, l, step)
+        g, b = _bn_params(state, fast, args, l, step)
         out = F.batch_norm(out, None, None, g, b, training=True, momentum=BN_MOMENTUM, eps=BN_EPS)
         out = F.leaky_relu(out)
         out = F.max_pool2d(out, kernel_size=(2, 2), stride=2, padding=0)
@@ -422,12 +428,12 @@ def head_backward(f, Wfc, prob, y, scale=1.0):
 
 
 def net_forward_manual(x, theta, state, args, step, y, forced=None):
-    """theta: dict name->tensor for the 10 fast tensors.  forced: optional per-block (slope, idx)."""
+    """theta: dict name->tensor for the fast tensors.  forced: optional per-block (slope, idx)."""
     fws = []
     a = x
     for l in range(num_stages(args)):
         wn, bn_, _, _, _, _ = conv_names(l)
-        g, b = _bn_params(state, args, l, step)
+        g, b = _bn_params(state, theta, args, l, step)
         fw = block_forward(a, theta[wn], theta[bn_], g, b, None if forced is None else forced[l])
         fws.append(fw)
         a = fw["p"]
@@ -437,7 +443,8 @@ def net_forward_manual(x, theta, state, args, step, y, forced=None):
 
 
 def net_backward_manual(fwd, theta, state, args, step, y, scale=1.0):
-    """Gradient of scale*loss w.r.t. the 10 fast tensors and the step's gamma/beta."""
+    """Gradient of scale*loss w.r.t. the fast tensors and gamma/beta: beta's is S1 = sum dy, gamma's S2 = sum dy * zh
+    per channel, among the fast tensors' with inner-loop gamma / beta, else in ``bn_grads`` (the step's)."""
     hb = head_backward(fwd["f"], theta[LIN_W], fwd["prob"], y, scale)
     grads = {LIN_W: hb["dW"], LIN_B: hb["db"]}
     bn_grads = {}
@@ -445,10 +452,11 @@ def net_backward_manual(fwd, theta, state, args, step, y, scale=1.0):
     dp = hb["df"].reshape(fwd["blocks"][-1]["p"].shape)
     for l in reversed(range(num_stages(args))):
         wn, bn_, gn, btn, _, _ = conv_names(l)
-        g, _ = _bn_params(state, args, l, step)
+        g, _ = _bn_params(state, theta, args, l, step)
         bw = block_backward(fwd["blocks"][l], theta[wn], g, dp, need_dgrad=(l > 0))
         grads[wn], grads[bn_] = bw["dW"], bw["db"]
-        bn_grads[gn], bn_grads[btn] = bw["dgamma"], bw["dbeta"]
+        gb_grads = grads if args.enable_inner_loop_optimizable_bn_params else bn_grads
+        gb_grads[gn], gb_grads[btn] = bw["dgamma"], bw["dbeta"]
         saved[l] = dict(bw, dp=dp)
         dp = bw["da_in"]
     return grads, bn_grads, {"head": hb, "blocks": saved}
@@ -456,15 +464,21 @@ def net_backward_manual(fwd, theta, state, args, step, y, scale=1.0):
 
 def tangent_pass(fwd, bwd_saved, theta, u, state, args, step, y):
     """A3: forward-mode derivative of (support forward + support backward) in direction u
-    (dict over the 10 fast tensors; gamma/beta tangents are zero).  Returns (Hu dict,
-    mixed second-derivative terms on this step's gamma / beta, intermediates)."""
+    (dict over the fast tensors).  Returns (Hu dict, mixed second-derivative terms on this
+    step's gamma / beta, intermediates).  Shared gamma / beta have no tangents.  Inner-loop
+    gamma / beta have tangents (gdot, bdot) in u, and with dzh = gamma * dy:
+      ydot   = gamma * zhdot + gdot * zh + bdot
+      dzhdot = gamma * dydot + gdot * dy
+    so dzdot gains r gdot (dy - S1/m - zh S2/m); their sums T1 = sum dydot (beta), T2 =
+    sum dydot zh + dy zhdot (gamma) are then Hu's, and there are no mixed terms."""
+    inner_bn = args.enable_inner_loop_optimizable_bn_params
     L = num_stages(args)
     tf = []
     a_dot = None
     for l in range(L):
-        wn, bn_, _, _, _, _ = conv_names(l)
+        wn, bn_, gn, btn, _, _ = conv_names(l)
         fw = fwd["blocks"][l]
-        g, _ = _bn_params(state, args, l, step)
+        g, _ = _bn_params(state, theta, args, l, step)
         z_dot = F.conv2d(fw["a_in"], u[wn], u[bn_], stride=1, padding=1)
         if a_dot is not None:
             z_dot = z_dot + F.conv2d(a_dot, theta[wn], None, stride=1, padding=1)
@@ -473,6 +487,8 @@ def tangent_pass(fwd, bwd_saved, theta, u, state, args, step, y):
         q = (zh * z_dot).mean(dim=(0, 2, 3))                      # mean(zh * z_dot)
         zh_dot = r[None, :, None, None] * (z_dot - mu_dot - zh * q[None, :, None, None])
         y_dot = g[None, :, None, None] * zh_dot
+        if inner_bn:
+            y_dot = y_dot + u[gn][None, :, None, None] * zh + u[btn][None, :, None, None]
         a_dot_full = y_dot * fw["slope"]
         n, c = a_dot_full.shape[:2]
         p_dot = a_dot_full.view(n, c, -1).gather(2, fw["idx"].view(n, c, -1)).view(fw["p"].shape)
@@ -492,13 +508,15 @@ def tangent_pass(fwd, bwd_saved, theta, u, state, args, step, y):
     for l in reversed(range(L)):
         wn, bn_, gn, btn, _, _ = conv_names(l)
         fw, bw, t = fwd["blocks"][l], bwd_saved["blocks"][l], tf[l]
-        g, _ = _bn_params(state, args, l, step)
+        g, _ = _bn_params(state, theta, args, l, step)
         gg = g[None, :, None, None]
         zh, r, m = fw["zh"], fw["r"], fw["m"]
         dy_dot = _unpool(dp_dot, fw["idx"], zh) * fw["slope"]
         dbeta_dot = dy_dot.sum(dim=(0, 2, 3))
         dgamma_dot = (dy_dot * zh + bw["dy"] * t["zh_dot"]).sum(dim=(0, 2, 3))
         dzh_dot = dy_dot * gg
+        if inner_bn:
+            dzh_dot = dzh_dot + bw["dy"] * u[gn][None, :, None, None]
         m1_dot = dzh_dot.mean(dim=(0, 2, 3))[None, :, None, None]
         m2_dot = (dzh_dot * zh + bw["dzh"] * t["zh_dot"]).mean(dim=(0, 2, 3))[None, :, None, None]
         r_dot_over_r = (-r * t["q"])[None, :, None, None]          # r_dot = -r^2 q
@@ -510,7 +528,8 @@ def tangent_pass(fwd, bwd_saved, theta, u, state, args, step, y):
             dW_dot = dW_dot + torch.nn.grad.conv2d_weight(t["a_in_dot"], W.shape, bw["dz"], stride=1, padding=1)
         Hu[wn] = dW_dot
         Hu[bn_] = dz_dot.sum(dim=(0, 2, 3))
-        mixed[gn], mixed[btn] = dgamma_dot, dbeta_dot
+        gb_dot = Hu if inner_bn else mixed
+        gb_dot[gn], gb_dot[btn] = dgamma_dot, dbeta_dot
         tb[l] = {"dz_dot": dz_dot, "dp_dot": dp_dot, "dy_dot": dy_dot}
         if l > 0:
             dp_dot = F.conv_transpose2d(dz_dot, W, stride=1, padding=1) + \

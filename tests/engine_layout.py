@@ -50,7 +50,8 @@ def host_plan(a, tasks, num_sms=H100_SMS):
 
 def norm_grid_regimes(a, tasks, num_sms=H100_SMS):
     """The regimes the grids of the normalisation kernels reach in one iteration (every block, support and target pass),
-    from bn_grid / ln_grid (kernels_bn.cu) and the inner-loop-BatchNorm reduce cap (launch_bnbwd_ibn):
+    from bn_grid / ln_grid (kernels_bn.cu) and the cap of the BatchNorm backward reduce (launch_bnbwd_reduce), which
+    inner-loop BatchNorm always runs:
       ibn_reduce_capped: a BatchNorm pass needs more CTAs per task than num_sms, the reduce's cap;
       ibn_apply_capped:  it needs more than 4 * num_sms, bn_grid's cap (apply, forward and tangent kernels);
       ln_one_cta:        ln_grid's cap max(1, 4 * num_sms / (n * tasks)) is 1 and an image needs more;
@@ -93,7 +94,7 @@ def traced_kernel_ids(m, batch, epoch):
 
 
 # kernel ids of the device trace: the convolutions, the BatchNorm kernels of the plain path (bnact .. bnbwd_tan_fused,
-# the fused tails, bnact_tan_gb), and the layer-norm (primal, tangent) and inner-loop BatchNorm (primal, tangent) ones
+# the fused tails, bnact_tan<GB>), and the layer-norm (primal, tangent) and inner-loop BatchNorm (PT: primal, tangent) ones
 K_CONV_ROWS, K_WGRAD_ROW, K_CONV_TC, K_WGRAD_TC = 1, 3, 22, 27
 K_BN = set(range(6, 14)) | {23, 24, 25, 32}
 K_LN, K_LN_TAN = {33, 35, 37, 39, 41}, {34, 36, 38, 40, 42}

@@ -1,6 +1,6 @@
 """Inner-loop BatchNorm gamma / beta (``enable_inner_loop_optimizable_bn_params``) on the fused training and validation
 iteration, against golden vectors of the unmodified reference (``oracle/gen_golden_ibn.py``) and the fp64 autograd oracle
-(``oracle/ibn_oracle.py``).  With the flag each block's norm_layer.bias / .weight are [F] fast weights: per task, updated by
+(``oracle/maml_oracle.py``).  With the flag each block's norm_layer.bias / .weight are [F] fast weights: per task, updated by
 the LSLR rule with their own rate vectors, differentiated to second order like the conv weights.
 
 CPU tests: the oracle reproduces each fixture's fp64 reference run, the module's state_dict / LSLR / Adam order match the
@@ -24,7 +24,6 @@ import functional_cases as fc
 from conftest import grad_tolerance, load_golden
 from engine_layout import (check_norm_path, device_sms, flat_to_nchw, geometry, grid_to_nchw, host_plan,
                            norm_grid_regimes, rel_err, traced_kernel_ids)
-from oracle import ibn_oracle as IBN
 from oracle import maml_oracle as O
 
 IBN_CASES = ["ibn_tiny_pp", "ibn_tiny_pp_moved", "ibn_tiny_first", "ibn_tiny_maml", "ibn_one_stage", "ibn_ffma_wide",
@@ -106,7 +105,7 @@ def _model(g, device, **debug):
 def test_oracle_reproduces_fp64_reference(case, oracle):
     g = load_golden(case)
     state = {k: v.double() for k, v in g.state(torch.float64).items()}
-    fn = IBN.autograd_train_iter if oracle == "autograd" else IBN.manual_train_iter
+    fn = O.autograd_train_iter if oracle == "autograd" else O.manual_train_iter
     res = fn(state, g.args, g.batch(0), g.iters[0][0])
     assert abs(float(res["loss"]) - g.scalar("loss64")) <= 1e-12 * abs(g.scalar("loss64"))
     ref = g.grads(0, "64")
@@ -138,15 +137,15 @@ def test_layout_and_adam_order_match_the_reference(case):
         assert names == [p + n for n in ("running_mean", "running_var", "bias", "weight")]
     # the inner loop and its LSLR vectors: conv.weight, conv.bias, norm_layer.bias, norm_layer.weight per block, then linear
     inner = ["classifier." + n for n in m.get_inner_loop_parameter_dict(m.classifier.named_parameters())]
-    assert inner == IBN.inner_param_names(g.args)
+    assert inner == O.inner_param_names(g.args)
     lslr = list(m.inner_loop_optimizer.names_learning_rates_dict.keys())
     assert ["inner_loop_optimizer.names_learning_rates_dict." + k for k in lslr] == [O.lslr_name(n) for n in inner]
     assert all(v.shape == (S + 1,) for v in m.inner_loop_optimizer.names_learning_rates_dict.values())
-    assert [n for n, _ in m._trainable_param_list()] == IBN.trainable_names(g.args) == list(g.grads(0).keys())
+    assert [n for n, _ in m._trainable_param_list()] == O.trainable_names(g.args) == list(g.grads(0).keys())
     # the flat buffer holds every LSLR vector (frozen ones too, outside Adam's mask), in inner-loop order
-    assert m._order == IBN.inner_param_names(g.args) + [O.lslr_name(n) for n in inner]
+    assert m._order == O.inner_param_names(g.args) + [O.lslr_name(n) for n in inner]
     group = m.optimizer.state_dict()["param_groups"][0]
-    assert group["params"] == list(range(len(IBN.trainable_names(g.args))))
+    assert group["params"] == list(range(len(O.trainable_names(g.args))))
 
 
 def test_refusals():
@@ -484,7 +483,7 @@ def _forced_run(case, device):
         batch, epoch = g.batch(0), g.iters[0][0]
         losses, preds, grads = m.meta_gradient(batch, epoch)
         dec = _gpu_decisions(m, g, batch, epoch)
-        ref = IBN.manual_train_iter(g.state(torch.float64), g.args, batch, epoch, decisions=dec, keep_intermediates=True)
+        ref = O.manual_train_iter(g.state(torch.float64), g.args, batch, epoch, decisions=dec, keep_intermediates=True)
         rows, worst = _stage_report(g.args, m._engine, ref, batch[0].shape[0])
         _RUNS[case] = dict(rows=rows, worst=worst, flips=_decision_flips(ref["intermediates"]), loss=float(losses["loss"]),
                            logits=np.stack(preds), grads={n: v.detach().cpu() for n, v in grads.items()},
