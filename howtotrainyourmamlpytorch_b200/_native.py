@@ -13,7 +13,7 @@ LIB_PATH = os.environ.get("MAML_B200_LIB") or os.path.join(_PKG, "lib", "libmaml
 
 MAX_STAGES = 4
 MAX_STEPS = 8
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 EXPORTED_SYMBOLS = [
     "maml_b200_abi_version", "maml_b200_last_error", "maml_b200_create", "maml_b200_destroy",
@@ -26,7 +26,7 @@ EXPORTED_SYMBOLS = [
     "maml_b200_comm_status", "maml_b200_net_backward", "maml_b200_net_running_update", "maml_b200_episode_gather",
     "maml_b200_net_hvp", "maml_b200_net_input_grad", "maml_b200_net_hvp_input_grad",
     "maml_b200_net_hvp_image", "maml_b200_net_jvp", "maml_b200_net_forward_tasks", "maml_b200_net_backward_tasks",
-    "maml_b200_net_hvp_image_tasks",
+    "maml_b200_net_hvp_image_tasks", "maml_b200_net_jvp_tasks",
 ]
 PROF_CATS = ["conv_igemm", "conv_first_block", "wgrad", "wgrad_first_block", "bn_act_pool", "head", "param"]
 
@@ -95,6 +95,8 @@ def load_library():
     lib.maml_b200_net_backward_tasks.restype = ctypes.c_int
     lib.maml_b200_net_hvp_image_tasks.argtypes = [vp, i32, i32, vp, i64, vp, vp, vp, vp, i64, vp, vp, i32, vp]
     lib.maml_b200_net_hvp_image_tasks.restype = ctypes.c_int
+    lib.maml_b200_net_jvp_tasks.argtypes = [vp, i32, i32, vp, i64, vp, vp, i64, vp, vp, vp]
+    lib.maml_b200_net_jvp_tasks.restype = ctypes.c_int
     lib.maml_b200_net_input_grad.argtypes = [vp, i32, vp, vp]
     lib.maml_b200_net_input_grad.restype = ctypes.c_int
     lib.maml_b200_net_hvp_input_grad.argtypes = [vp, i32, vp, vp]
@@ -270,6 +272,14 @@ class Engine(object):
                                                     jv_out.data_ptr(), hv_out.data_ptr(), int(bool(sum_tasks)),
                                                     self._stream())
         _check(self.lib, rc, "maml_b200_net_hvp_image_tasks")
+
+    def net_jvp_tasks(self, n_tasks, num_step, meta_like, meta_stride, x, t_like, dir_stride, xdot, jv_out):
+        """``net_jvp`` with task t's weights at ``meta_like`` + t * meta_stride and its tangent at ``t_like`` + t *
+        dir_stride floats (0: shared)."""
+        rc = self.lib.maml_b200_net_jvp_tasks(self.h, int(n_tasks), int(num_step), meta_like.data_ptr(), int(meta_stride),
+                                              x.data_ptr(), t_like.data_ptr(), int(dir_stride),
+                                              None if xdot is None else xdot.data_ptr(), jv_out.data_ptr(), self._stream())
+        _check(self.lib, rc, "maml_b200_net_jvp_tasks")
 
     def net_input_grad(self, n_tasks, dx_out):
         rc = self.lib.maml_b200_net_input_grad(self.h, int(n_tasks), dx_out.data_ptr(), self._stream())

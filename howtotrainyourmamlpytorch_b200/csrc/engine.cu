@@ -1394,15 +1394,24 @@ extern "C" int maml_b200_meta_batch_fwd_bwd(maml_b200_handle* h, const maml_b200
 // Argument checks of the functional entries; `ptrs`: the entry's required pointers are all non-null.
 static int check_call(const maml_b200_handle* h, bool ptrs, int n_tasks, int num_step) {
   if (!h || !ptrs) return fail("null argument");
-  if (h->pl.inner_bn) return fail("the functional entries (maml_b200_net_*) do not run inner_bn handles yet");
   if (n_tasks < 1 || n_tasks > h->maxT) return fail("n_tasks out of range");
   if (num_step < 0 || num_step >= h->S) return fail("num_step out of range");
   return 0;
 }
 
+// The shared-weight entries (net_forward, net_backward, net_hvp, net_hvp_image, net_jvp) read the BatchNorm gamma / beta of
+// num_step, shared by the tasks; an inner_bn handle has no such rows, its gamma / beta are per-task fast weights.
+static int refuse_inner_bn(const maml_b200_handle* h, const char* entry, const char* per_task) {
+  if (h && h->pl.inner_bn)
+    return fail(std::string("maml_b200_") + entry + " shares BatchNorm gamma / beta between the tasks; an inner_bn handle "
+                "(per-task gamma / beta) runs maml_b200_" + per_task);
+  return 0;
+}
+
 // Stages a functional call's batch and runs its primal forward on pass set `ps` at `slot`: x (and the image tangent xdot,
 // support grid only) onto the block-0 grid, meta_like into theta slot `slot` (and dir_like into u), the tensor-core packs
-// of that slot, then the forward with the BatchNorm gamma / beta of num_step (read from task 0's meta_like).  meta_stride /
+// of that slot, then the forward with the BatchNorm gamma / beta of num_step (read from task 0's meta_like; inner_bn: each
+// task's own, imported into theta with its weights, and their directions into u).  meta_stride /
 // dir_stride: floats between consecutive tasks' vectors (0: one vector for all tasks).  Returns the theta slot.
 static const float* stage_forward(maml_b200_handle* h, const PassSet& ps, int slot, int stat_kind, int num_step, const float* meta_like,
                                   long long meta_stride, const float* x, const float* xdot, const float* dir_like, long long dir_stride,
@@ -1461,6 +1470,7 @@ extern "C" int maml_b200_net_forward_tasks(maml_b200_handle* h, int32_t n_tasks,
 
 extern "C" int maml_b200_net_forward(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
                                     const float* x, float* logits, void* stream) {
+  if (refuse_inner_bn(h, "net_forward", "net_forward_tasks")) return 1;
   return maml_b200_net_forward_tasks(h, n_tasks, num_step, meta_like, 0, x, logits, stream);
 }
 
@@ -1486,8 +1496,9 @@ extern "C" int maml_b200_net_backward_tasks(maml_b200_handle* h, int32_t n_tasks
   // norm: export sums both kinds of bias-gradient rows over every step
   if (clear_accumulators(h, CLR_BWD_STATS | CLR_ABAR | CLR_LOSSES | CLR_CORRECT, st, T)) return 1;
   external_backward(h, h->tgt, 0, num_step, PASS_TGT_FWD, PASS_TGT_BWD, meta_like, dlogits, h->tgt_partial, h->plan_tgt, T, st);
-  launch_param_reduce(h->pl, h->plan_tgt.pd, h->tgt_partial, PR_STORE, nullptr, nullptr, h->tbar, nullptr, meta_like, num_step,
-                      h->Ppad, T, st);
+  // inner_bn: the beta / gamma rows are each task's backward sums S1 / S2 (export has no gamma / beta rows of its own)
+  const PartialDesc pd = h->pl.inner_bn ? with_bn_sums(h, h->plan_tgt.pd, stat_at(h, PASS_TGT_BWD, num_step, 0)) : h->plan_tgt.pd;
+  launch_param_reduce(h->pl, pd, h->tgt_partial, PR_STORE, nullptr, nullptr, h->tbar, nullptr, meta_like, num_step, h->Ppad, T, st);
   launch_export(export_args(h, T, grad_out, !sum_tasks), st);
   CK(cudaGetLastError());
   record_call(h, FN_BACKWARD, T, num_step);
@@ -1496,6 +1507,7 @@ extern "C" int maml_b200_net_backward_tasks(maml_b200_handle* h, int32_t n_tasks
 
 extern "C" int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
                                      const float* dlogits, float* grad_out, void* stream) {
+  if (refuse_inner_bn(h, "net_backward", "net_backward_tasks")) return 1;
   return maml_b200_net_backward_tasks(h, n_tasks, num_step, meta_like, 0, dlogits, grad_out, 1, stream);
 }
 
@@ -1548,9 +1560,11 @@ static int net_hvp_impl(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, 
   external_backward(h, h->sup, s, s, PASS_SUP_FWD, PASS_SUP_BWD, meta_like, dlogits, h->sup_partial, h->plan_sup, T, st);
   cudaStream_t spre;
   if (fork_direction(h, T, st, &spre)) return 1;
-  ReduceSpec rs{PR_STORE, nullptr, nullptr, h->tbar, nullptr, s, -1};
+  // inner_bn: the beta / gamma rows are the tangent backward's sums (kind_tbwd), stored as they are: +H_beta v, +H_gamma v
   const TangentHead th_ext{HEAD_EXTERNAL_TAN, nullptr, dlogits, (long long)h->n_s * h->N, jv_out, PASS_TGT_BWD};
-  // the HVP has no BatchNorm gamma / beta directions: only a layer-norm handle's tangent pass reads v_like's norm entries
+  ReduceSpec rs{PR_STORE, nullptr, nullptr, h->tbar, nullptr, s, -1, h->pl.inner_bn ? stat_at(h, th_ext.kind_tbwd, s, 0) : nullptr};
+  // Norm-parameter directions: an inner_bn handle's gamma / beta directions are u's (imported from v_like per task), a
+  // layer-norm handle's bias directions are read from v_like's norm entries (t_norm); a plain BatchNorm handle has none
   tangent_pass(h, s, th, h->u, meta_like, th_ext, T, st, rs, spre, xdot ? h->xdot_g : nullptr, h->ln ? v_like : nullptr,
                dir_stride);
   join_pending(h, st);
@@ -1562,6 +1576,7 @@ static int net_hvp_impl(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, 
 
 extern "C" int maml_b200_net_hvp(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
                                  const float* dlogits, const float* v_like, float* jv_out, float* hv_out, void* stream) {
+  if (refuse_inner_bn(h, "net_hvp", "net_hvp_image_tasks")) return 1;
   return net_hvp_impl(h, n_tasks, num_step, meta_like, 0, x, nullptr, dlogits, v_like, 0, jv_out, hv_out, true, stream);
 }
 
@@ -1571,6 +1586,7 @@ extern "C" int maml_b200_net_hvp(maml_b200_handle* h, int32_t n_tasks, int32_t n
 extern "C" int maml_b200_net_hvp_image(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
                                        const float* x, const float* xdot, const float* dlogits, const float* v_like, float* jv_out,
                                        float* hv_out, void* stream) {
+  if (refuse_inner_bn(h, "net_hvp_image", "net_hvp_image_tasks")) return 1;
   return net_hvp_impl(h, n_tasks, num_step, meta_like, 0, x, xdot, dlogits, v_like, 0, jv_out, hv_out, true, stream);
 }
 
@@ -1587,12 +1603,16 @@ extern "C" int maml_b200_net_hvp_image_tasks(maml_b200_handle* h, int32_t n_task
 // Forward mode of the functional operator: jv_out [n_tasks, N*K, N] = J_theta t + J_x xdot at the weights meta_like, for
 // batches of N*K images (the handle's support shape).  Self-contained: the primal forward at support slot num_step, then
 // the forward half of the tangent pass (no backward).  t_like in the meta layout: conv / linear entries are the weight
-// tangents, the BatchNorm beta / gamma rows of num_step their tangents; LSLR entries are not read.  xdot may be NULL.
+// tangents, the BatchNorm beta / gamma rows their tangents (inner_bn: per task, as the weights; otherwise those of
+// num_step, shared) or the layer-norm bias tangents; LSLR entries are not read.  xdot may be NULL.  Task t's weights at
+// meta_like + t * meta_stride, its tangent at t_like + t * dir_stride (0: shared).
 // The logits tangent comes from the HEAD_EXTERNAL_TAN head with d(logits) = 0, whose gradient outputs are discarded.
 // Overwrites the batch statistics maml_b200_net_running_update reads; no running-statistics side effect of its own.
-extern "C" int maml_b200_net_jvp(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
-                                 const float* t_like, const float* xdot, float* jv_out, void* stream) {
+extern "C" int maml_b200_net_jvp_tasks(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
+                                       int64_t meta_stride, const float* x, const float* t_like, int64_t dir_stride,
+                                       const float* xdot, float* jv_out, void* stream) {
   if (check_call(h, meta_like && x && t_like && jv_out, n_tasks, num_step)) return 1;
+  if (check_strides(meta_stride, dir_stride, h->pl.meta_size)) return 1;
   cudaStream_t st = (cudaStream_t)stream;
   LaunchScope launch_scope(h, st);
   const int T = n_tasks, s = num_step;
@@ -1601,14 +1621,20 @@ extern "C" int maml_b200_net_jvp(maml_b200_handle* h, int32_t n_tasks, int32_t n
   // zero d(logits) of one batch, read with a task stride of 0
   if (!h->zero_dl && alloc_zeroed(&h->zero_dl, (size_t)h->n_s * h->N * sizeof(float), st)) return 1;
   if (clear_accumulators(h, CLR_STATS, st)) return 1;
-  const float* th = stage_forward(h, h->sup, s, PASS_SUP_FWD, s, meta_like, 0, x, xdot, t_like, 0, T, st);
+  const float* th = stage_forward(h, h->sup, s, PASS_SUP_FWD, s, meta_like, meta_stride, x, xdot, t_like, dir_stride, T, st);
   cudaStream_t spre;
   if (fork_direction(h, T, st, &spre)) return 1;
-  tangent_forward(h, s, th, h->u, meta_like, xdot ? h->xdot_g : nullptr, t_like, 0, T, st, spre, false, nullptr);
+  tangent_forward(h, s, th, h->u, meta_like, xdot ? h->xdot_g : nullptr, t_like, dir_stride, T, st, spre, false, nullptr);
   join_pending(h, st);
   launch_head(tangent_head_args(h, s, th, h->u, TangentHead{HEAD_EXTERNAL_TAN, nullptr, h->zero_dl, 0, jv_out, PASS_TGT_BWD}, T), st);
   CK(cudaGetLastError());
   return 0;
+}
+
+extern "C" int maml_b200_net_jvp(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
+                                 const float* t_like, const float* xdot, float* jv_out, void* stream) {
+  if (refuse_inner_bn(h, "net_jvp", "net_jvp_tasks")) return 1;
+  return maml_b200_net_jvp_tasks(h, n_tasks, num_step, meta_like, 0, x, t_like, 0, xdot, jv_out, stream);
 }
 
 // First-block data gradient of a functional call, straight into NCHW images: dx = sum over the pairs (W_k, D_k) of

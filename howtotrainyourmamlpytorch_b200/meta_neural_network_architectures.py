@@ -163,10 +163,11 @@ class VGGReLUNormNetwork(nn.Module):
 
     def _norm_segments(self):
         """(indices of the norm parameters among ``_segment_names``, whether the engine's tangent passes take directions
-        along them).  The layer-norm biases do (a bias tangent enters after the normalisation); BatchNorm gamma / beta do
-        not (they would be inner-loop fast weights, enable_inner_loop_optimizable_bn_params)."""
+        along them).  The layer-norm biases do (a bias tangent enters after the normalisation), and so do BatchNorm gamma
+        / beta when they are inner-loop fast weights (enable_inner_loop_optimizable_bn_params: per task, like the conv
+        weights); the shared per-step gamma / beta of a plain BatchNorm network do not."""
         idx = tuple(i for i, n in enumerate(self._segment_names()) if ".norm_layer." in n)
-        return idx, self._layer_norm()
+        return idx, self._layer_norm() or self._inner_bn()
 
     def _segment_tensors(self, params):
         """Tensors in the engine's meta-vector order (``_segment_names``): ``params``' entries, else the module's own."""
@@ -217,6 +218,9 @@ class VGGReLUNormNetwork(nn.Module):
         or not; missing entries fall back to the module's own parameters.  BatchNorm always uses batch statistics
         (the reference hard-codes ``training=True``, :246-247) with the gamma / beta of ``num_step``, and -- like
         ``F.batch_norm`` there -- leaves its EMA update in ``running_mean / running_var[num_step]`` (per-step BN only).
+        With ``enable_inner_loop_optimizable_bn_params`` gamma / beta are [F] fast weights, taken from ``params`` (or the
+        module) without a step index, as the reference does (:226-234); ``num_step`` then selects only the running-
+        statistics row.
         The layer-norm network (``norm_layer: "layer_norm"``) normalises each image on its own, adds the bias
         [F, h, w] (an outer parameter: differentiable, and a valid tangent or cotangent direction wherever the weights
         are), has no running statistics and ignores ``num_step``; its frozen weight must be all ones (ValueError).
@@ -226,8 +230,8 @@ class VGGReLUNormNetwork(nn.Module):
         beta), which is what the reference's ``apply_inner_loop_update`` needs (``torch.autograd.grad`` of the support
         loss, few_shot_learning_system.py:138-139).  Twice differentiable: with ``create_graph=True`` the returned
         gradients are differentiable w.r.t. the weights (and the upstream d(logits)) through ``maml_b200_net_hvp``, so the
-        reference's second-order loop runs on this operator (a layer-norm bias gradient too); a BatchNorm gamma / beta
-        gradient is not (see ``_FunctionalBackward``).  When ``x`` requires grad the operator is differentiable w.r.t. the images too
+        reference's second-order loop runs on this operator (a layer-norm bias gradient too, and an inner-loop BatchNorm
+        gamma / beta gradient); a plain BatchNorm network's gamma / beta gradient is not (see ``_FunctionalBackward``).  When ``x`` requires grad the operator is differentiable w.r.t. the images too
         (``maml_b200_net_input_grad``), and with ``create_graph=True`` the weight gradients are differentiable w.r.t. ``x``
         (``maml_b200_net_hvp_input_grad``: the mixed term an outer loss needs to reach support images through the inner
         loop); the image gradient itself is not differentiable again.  With ``x`` not requiring grad none of this runs.
@@ -235,18 +239,19 @@ class VGGReLUNormNetwork(nn.Module):
 
         ``torch.func`` transforms work too: ``grad`` / ``vjp`` / ``jacrev`` (up to second order) and ``vmap`` over tasks,
         which runs the B mapped calls as ONE engine call with n_tasks = B (``maml_b200_net_*_tasks``) -- images, fast
-        weights and upstream cotangents may each be batched or shared.  BatchNorm gamma / beta and the layer-norm biases
-        stay shared by the tasks (a batched one raises NotImplementedError); ``torch.func.jvp`` / ``jacfwd`` /
+        weights and upstream cotangents may each be batched or shared.  A plain BatchNorm network's gamma / beta and the
+        layer-norm biases stay shared by the tasks (a batched one raises NotImplementedError); inner-loop BatchNorm gamma /
+        beta may be batched (per task after the first inner step, as the functorch loop makes them); ``torch.func.jvp`` / ``jacfwd`` /
         ``hessian`` (forward mode runs through ``torch.autograd.forward_ad``) and third order raise it too.  A vmapped
         forward leaves the EMA of its B batches in task order, so a vmapped inner loop updates the running statistics
         step-major (every task's support pass at step s, then every target pass), not task-major as the reference's loop
         over tasks does."""
         from . import _native
-        if self._inner_bn():
-            raise NotImplementedError("VGGReLUNormNetwork.forward does not run a network with "
-                                      "enable_inner_loop_optimizable_bn_params yet (inner-loop BatchNorm gamma / beta run in "
-                                      "MAMLFewShotClassifier.run_train_iter / run_validation_iter)")
         if x.device.type != "cuda":
+            if self._inner_bn():
+                raise NotImplementedError("VGGReLUNormNetwork.forward on a network with "
+                                          "enable_inner_loop_optimizable_bn_params runs on the CUDA engine only (sm_90a): "
+                                          "no CPU fallback")
             if self._layer_norm():
                 raise NotImplementedError("VGGReLUNormNetwork.forward on the layer-norm network runs on the CUDA engine "
                                           "only (sm_90a): no CPU fallback")
@@ -371,6 +376,10 @@ def _refuse_nested(spec):
 
 
 def _refuse_batched_norm(net, dims):
+    """Inner-loop BatchNorm gamma / beta are per-task fast weights: batched ones are what the functorch loop passes after
+    its first inner step.  The other norm parameters are shared by the tasks of a call."""
+    if net._inner_bn():
+        return
     if any(dims[i] is not None for i in net._norm_segments()[0]):
         if net._layer_norm():
             raise NotImplementedError(
@@ -378,8 +387,8 @@ def _refuse_batched_norm(net, dims):
                 "tasks of a call (they are outer parameters, the same for every task)")
         raise NotImplementedError(
             "a BatchNorm gamma / beta batched under torch.func.vmap: the engine shares gamma / beta between the tasks "
-            "of a call (per-task gamma / beta are inner-loop BatchNorm parameters, "
-            "enable_inner_loop_optimizable_bn_params, which are outside the accelerated path)")
+            "of a call (per-task gamma / beta are inner-loop BatchNorm parameters: set "
+            "enable_inner_loop_optimizable_bn_params)")
 
 
 def _refuse_functorch_jvp(ctx, *tensors):
@@ -405,15 +414,16 @@ class _OperatorHandles:
     / ``net_input_grad``, the running-statistics update).  It keeps the activations of its LAST forward only: ``token``
     names that forward, so that a backward of another one replays its own first (``gen`` counts the forwards it ran).  The second-order handle, created on first
     use, holds the batch as its SUPPORT pass, the buffers the tangent pass runs on (``net_hvp_image_tasks`` /
-    ``net_hvp_input_grad`` / ``net_jvp``): a model that is only differentiated once pays nothing for it.  Every call runs
-    the per-task entries with per-task results; for B = 1 and shared weights they compute what ``net_forward`` /
-    ``net_backward`` / ``net_hvp_image`` do, bit for bit."""
+    ``net_hvp_input_grad`` / ``net_jvp_tasks``): a model that is only differentiated once pays nothing for it.  Every call
+    runs the per-task entries with per-task results; for B = 1 and shared weights they compute what ``net_forward`` /
+    ``net_backward`` / ``net_hvp_image`` / ``net_jvp`` do, bit for bit.  A network with inner-loop BatchNorm gamma / beta
+    gets inner_bn handles, which run the per-task entries only: their gamma / beta follow each task's weights."""
 
     def __init__(self, net, x, tasks):
         a = net.args
         self.B = int(tasks)
         self.n, self.N, self.device = int(x.shape[-4]), net.num_output_classes, x.device
-        self.layer_norm = net._layer_norm()
+        self.layer_norm, self.inner_bn = net._layer_norm(), net._inner_bn()
         self.cfg = dict(n_way=self.N, channels=int(x.shape[-3]), height=int(x.shape[-2]), width=int(x.shape[-1]),
                         filters=net.cnn_filters, num_stages=net.num_stages, inner_steps=int(a.number_of_training_steps_per_iter),
                         per_step_bn=bool(a.per_step_bn_statistics), max_tasks=self.B)
@@ -430,7 +440,7 @@ class _OperatorHandles:
     def _engine(self, **shape):
         from . import _native
         with torch.cuda.device(self.device):
-            return _native.Engine(**shape, **self.cfg, layer_norm=self.layer_norm)
+            return _native.Engine(**shape, **self.cfg, layer_norm=self.layer_norm, inner_bn=self.inner_bn)
 
     def _second(self):
         if self.second_order is None:
@@ -510,12 +520,12 @@ class _OperatorHandles:
         return d_x, (self.jv if spec is not None else self.jv[0]), _unpack(eng, self.hv, tensors, needs, spec, cast)
 
     def jvp(self, num_step, x, xdot, tensors, tangents):
-        """The logits tangent J_theta t + J_x xdot (``net_jvp``; xdot may be None; one batch)."""
+        """The logits tangent J_theta t + J_x xdot (``net_jvp_tasks`` at strides 0; xdot may be None; one batch)."""
         eng = self._second()
         _fill(eng, self.meta2, tensors, (False,) * len(tensors))
         _fill(eng, self.v, tangents, (False,) * len(tangents))
         with torch.cuda.device(self.device):
-            eng.net_jvp(1, num_step, self.meta2, _f32(x), self.v, None if xdot is None else _f32(xdot), self.jv)
+            eng.net_jvp_tasks(1, num_step, self.meta2, 0, _f32(x), self.v, 0, None if xdot is None else _f32(xdot), self.jv)
         return self.jv[0].clone()
 
 
@@ -551,9 +561,8 @@ class _FunctionalForward(torch.autograd.Function):
             if fwAD.unpack_dual(tensors[i]).tangent is not None:
                 raise NotImplementedError(
                     "differentiating the gradient in forward mode along a BatchNorm gamma / beta tangent needs gamma / beta "
-                    "tangent directions in the backward tangent pass, which the engine does not implement (BatchNorm "
-                    "parameters as inner-loop fast weights, enable_inner_loop_optimizable_bn_params, are outside the "
-                    "accelerated path)")
+                    "tangent directions in the backward tangent pass, which the engine implements for inner-loop BatchNorm "
+                    "parameters only (enable_inner_loop_optimizable_bn_params), not for the shared per-step gamma / beta")
         out = _FunctionalBackward.apply(ctx, ctx.spec, x, dlogits, *tensors)
         if ctx.spec is not None:
             out = [_shared_sum(o, b) for o, b in zip(out, (ctx.spec.x,) + ctx.spec.tensors)]
@@ -562,7 +571,7 @@ class _FunctionalForward(torch.autograd.Function):
     @staticmethod
     def jvp(ctx, _net_t, _spec_t, x_t, _step_t, *tangents):
         """Forward mode (``torch.autograd.forward_ad``): the logits tangent J_theta t + J_x x_t through
-        ``maml_b200_net_jvp`` on the second-order handle -- one primal forward and one tangent forward.  Tangents may sit
+        ``maml_b200_net_jvp_tasks`` on the second-order handle -- one primal forward and one tangent forward.  Tangents may sit
         on the images, the conv / linear weights and the BatchNorm gamma / beta or layer-norm biases."""
         _refuse_functorch_jvp(ctx, x_t, *tangents)
         x = ctx.saved_tensors[0]
@@ -588,13 +597,14 @@ class _FunctionalBackward(torch.autograd.Function):
                beta of ``num_step`` or the layer-norm biases), and -- only when x requires grad -- ``maml_b200_net_input_grad``: J_x^T dl (else
                None).  With grad mode off this is the whole first-order backward.
     backward = ``_FunctionalHvp`` along the cotangents v of the conv / linear gradients (and of the layer-norm bias
-               gradients: bias directions, which the engine's tangent forward adds after the normalisation).  Third order
-               is not supported.
-    A cotangent on a BatchNorm gamma / beta GRADIENT would need gamma / beta tangent directions, and one on the image
-    gradient dx would need image tangent directions (the first conv's tangent driven by x-dot); the engine's tangent pass
-    has neither: both are refused (the first only arises when BatchNorm parameters are inner-loop fast weights,
-    enable_inner_loop_optimizable_bn_params, which the network refuses too; the second e.g. for a penalty on the image
-    gradient's norm that is differentiated again).  ``spec`` and the ``vmap`` rule as in ``_FunctionalForward``; with a
+               gradients: bias directions, which the engine's tangent forward adds after the normalisation; and of
+               inner-loop BatchNorm gamma / beta gradients: gamma / beta directions).  Third order is not supported.
+    A cotangent on an inner-loop BatchNorm gamma / beta gradient (enable_inner_loop_optimizable_bn_params) is a gamma /
+    beta direction of the tangent pass, per task like the weights' (the engine reads it into the tangent forward's
+    gamma-dot / beta-dot and the tangent backward's gamma-dot term).  A cotangent on a plain BatchNorm network's shared
+    gamma / beta GRADIENT would need gamma / beta tangent directions shared by the tasks, and one on the image gradient dx
+    would need image tangent directions (the first conv's tangent driven by x-dot); the engine's tangent pass has neither:
+    both are refused (the second e.g. for a penalty on the image gradient's norm that is differentiated again).  ``spec`` and the ``vmap`` rule as in ``_FunctionalForward``; with a
     spec, dlogits is [B, n, N] and every gradient is per task."""
 
     @staticmethod
@@ -618,9 +628,9 @@ class _FunctionalBackward(torch.autograd.Function):
         weight gradient J_theta^T dl_t + d/dtheta <dl, J_theta t + J_x x_t>; for dx the same with d/dx.  The first term is
         ``maml_b200_net_backward_tasks`` (+ ``net_input_grad``) of dl_t on the first-order handle, the second
         ``maml_b200_net_hvp_image_tasks`` (+ ``net_hvp_input_grad``) on the second-order handle; a term whose tangents are
-        all None is skipped.  A layer-norm bias tangent is a bias direction of that pass.  A tangent on a BatchNorm
-        gamma / beta input never gets here: ``_FunctionalForward.backward``
-        refuses it before this node runs."""
+        all None is skipped.  A layer-norm bias tangent is a bias direction of that pass, an inner-loop BatchNorm gamma /
+        beta tangent a gamma / beta direction.  A tangent on a plain BatchNorm network's gamma / beta never gets here:
+        ``_FunctionalForward.backward`` refuses it before this node runs."""
         _refuse_functorch_jvp(ctx, x_t, dl_t, *tangents)
         fwd_ctx = ctx.fwd_ctx
         x, dlogits, tensors = ctx.saved_tensors[0], ctx.saved_tensors[1], ctx.saved_tensors[2:]
@@ -647,8 +657,8 @@ class _FunctionalBackward(torch.autograd.Function):
             if cotangents[i] is not None:
                 raise NotImplementedError(
                     "differentiating through the gradient of a BatchNorm gamma / beta needs gamma / beta tangent "
-                    "directions, which the engine does not implement (BatchNorm parameters as inner-loop fast weights, "
-                    "enable_inner_loop_optimizable_bn_params, are outside the accelerated path)")
+                    "directions, which the engine implements for inner-loop BatchNorm parameters only "
+                    "(enable_inner_loop_optimizable_bn_params), not for the shared per-step gamma / beta")
         if all(c is None for c in cotangents):
             return (None,) * (4 + len(tensors))
         need = ctx.needs_input_grad
@@ -674,7 +684,8 @@ class _FunctionalBackward(torch.autograd.Function):
 
 
 class _FunctionalHvp(torch.autograd.Function):
-    """Backward of ``_FunctionalBackward``: along the cotangents v of the conv / linear (and layer-norm bias) gradients,
+    """Backward of ``_FunctionalBackward``: along the cotangents v of the conv / linear (and layer-norm bias, or inner-loop
+    BatchNorm gamma / beta) gradients,
     ``maml_b200_net_hvp_image_tasks`` -- one forward-over-reverse pass with dl held constant -- gives J v (the cotangent of
     dl) and d/dtheta <dl, J v> (that of every tensor); ``maml_b200_net_hvp_input_grad`` on the same handle gives
     d/dx <dl, J v> (that of x) when ``needs.x``.  torch carries J v on through the loss's own double backward.  A node of its

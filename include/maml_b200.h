@@ -28,7 +28,7 @@ extern "C" {
 
 #define MAML_B200_MAX_STAGES 4
 #define MAML_B200_MAX_STEPS 8
-#define MAML_B200_ABI_VERSION 4
+#define MAML_B200_ABI_VERSION 5
 
 /* Static shape of the path.  Mirrors the args the reference reads on this path:
  * num_classes_per_set, num_samples_per_class, num_target_samples, image_{channels,height,width},
@@ -57,8 +57,10 @@ typedef struct maml_b200_config {
                            block's norm_layer.bias / .weight (beta, gamma) are [F] whatever per_step_bn is, and are
                            inner-loop fast weights: per task, updated by the LSLR rule with their own rate vectors, and
                            differentiated to second order like the conv weights.  The running statistics keep their
-                           per-step rows when per_step_bn is set.  The functional entries (maml_b200_net_*) refuse these
-                           handles. */
+                           per-step rows when per_step_bn is set.  Of the functional entries (maml_b200_net_*) these
+                           handles run the per-task ones (maml_b200_net_*_tasks), the image gradients and the running-
+                           statistics update; the shared-weight entries (net_forward, net_backward, net_hvp,
+                           net_hvp_image, net_jvp) refuse them. */
 } maml_b200_config;
 
 /* Per-call schedule: what reference forward(...) derives from epoch / phase (:232-244,:304-305). */
@@ -143,8 +145,9 @@ int maml_b200_net_backward(maml_b200_handle* h, int32_t n_tasks, int32_t num_ste
                            const float* dlogits, float* grad_out, void* stream);
 
 /* Second-order companion of maml_b200_net_backward: for the batch x, weights meta_like and upstream dlogits, one
- * forward-over-reverse pass along v_like (meta layout; its BatchNorm and LSLR entries are not read: there are no
- * gamma / beta tangent directions; on a layer-norm handle its bias entries are bias directions).  Self-contained: it recomputes the forward and the backward of dlogits itself, so it
+ * forward-over-reverse pass along v_like (meta layout; its LSLR entries are not read, nor are its BatchNorm entries on a
+ * plain BatchNorm handle, which has no gamma / beta tangent directions; on a layer-norm handle its bias entries are bias
+ * directions, and an inner_bn handle's gamma / beta directions run through maml_b200_net_hvp_image_tasks).  Self-contained: it recomputes the forward and the backward of dlogits itself, so it
  * needs no earlier call.  The batch has the handle's SUPPORT shape: N*K images (create the handle with k_shot = batch / N).
  *   x          [n_tasks, N*K, C, H, W]
  *   dlogits    [n_tasks, N*K, N]  d(loss) / d(logits), held constant along v
@@ -176,17 +179,21 @@ int maml_b200_net_hvp_image(maml_b200_handle* h, int32_t n_tasks, int32_t num_st
 int maml_b200_net_jvp(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like, const float* x,
                       const float* t_like, const float* xdot, float* jv_out, void* stream);
 
-/* Per-task forms of net_forward / net_backward / net_hvp_image: n_tasks independent problems in one call, each with its
+/* Per-task forms of net_forward / net_backward / net_hvp_image / net_jvp: n_tasks independent problems in one call, each with its
  * own weights (what torch.func.vmap over tasks runs as one call).  Same shapes, ordering rules and side effects as the
  * entries above, plus:
  *   meta_stride  floats between consecutive tasks' meta_like vectors: task t's conv / linear weights are at
  *                meta_like + t * meta_stride; 0 = one vector shared by every task (the entries above)
- *   dir_stride   the same for v_like (0 = shared)
+ *   dir_stride   the same for v_like / t_like (0 = shared)
  *   sum_tasks    1: grad_out / hv_out = result_size floats summed over the tasks (the entries above);
  *                0: n_tasks x result_size floats, task t's vector (not summed) at + t * result_size
  * BatchNorm gamma / beta and the layer-norm biases are shared by the tasks of a call: they are read from task 0's vector
- * (meta_like's own rows), whatever meta_stride is.  The layer-norm bias DIRECTIONS of net_hvp_image_tasks follow
- * dir_stride (per task), and each task's bias gradient goes to its own result vector.  A stride that is neither 0 nor >= meta_size is an error.
+ * (meta_like's own rows), whatever meta_stride is; so are net_jvp_tasks' BatchNorm gamma / beta tangents, whatever
+ * dir_stride is.  The layer-norm bias DIRECTIONS of net_hvp_image_tasks / net_jvp_tasks follow dir_stride (per task), and
+ * each task's bias gradient goes to its own result vector.  On an inner_bn handle gamma / beta are per-task fast weights:
+ * they follow meta_stride (each task's own beta / gamma rows), their directions and tangents follow dir_stride, and each
+ * task's beta / gamma gradient (+H_beta v, +H_gamma v for net_hvp_image_tasks) goes to its own result vector (or into the
+ * sum).  A stride that is neither 0 nor >= meta_size is an error.
  * maml_b200_net_input_grad, maml_b200_net_hvp_input_grad and maml_b200_net_running_update already work per task and follow
  * these entries as they follow the ones above. */
 int maml_b200_net_forward_tasks(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
@@ -197,6 +204,9 @@ int maml_b200_net_hvp_image_tasks(maml_b200_handle* h, int32_t n_tasks, int32_t 
                                   int64_t meta_stride, const float* x, const float* xdot, const float* dlogits,
                                   const float* v_like, int64_t dir_stride, float* jv_out, float* hv_out, int32_t sum_tasks,
                                   void* stream);
+int maml_b200_net_jvp_tasks(maml_b200_handle* h, int32_t n_tasks, int32_t num_step, const float* meta_like,
+                            int64_t meta_stride, const float* x, const float* t_like, int64_t dir_stride, const float* xdot,
+                            float* jv_out, void* stream);
 
 /* Gradients with respect to the images.  Each reads the buffers of the functional call that ran last on this handle and
  * must follow it immediately, with the same n_tasks: another call on the handle in between (a functional call, an

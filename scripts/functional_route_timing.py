@@ -15,9 +15,11 @@ meta-batch 8, second order) three ways, on one GPU:
 Warm-up first; every timed iteration ends in a device synchronise; the legs alternate within each repeat.  Prints
 one JSON line: per leg the median / min / max milliseconds per iteration, plus the GPU name and power limit read in
 the same run.  ``--norm-layer layer_norm`` runs the same config with the layer-norm network (its torch legs on
-oracle.ln_oracle._net_forward) and adds "norm_layer" to the line.
+oracle.ln_oracle._net_forward) and adds "norm_layer" to the line.  ``--inner-bn`` sets
+enable_inner_loop_optimizable_bn_params on the BatchNorm network (BatchNorm gamma / beta adapted per task in the inner
+loop, and differentiated with the other fast weights in every leg) and adds "inner_bn" to the line.
 
-  python scripts/functional_route_timing.py [--repeats 20] [--warmup 3] [--norm-layer {batch_norm,layer_norm}]
+  python scripts/functional_route_timing.py [--repeats 20] [--warmup 3] [--norm-layer {batch_norm,layer_norm}] [--inner-bn]
 """
 import argparse
 import json
@@ -103,7 +105,10 @@ def main():
     ap.add_argument("--repeats", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--norm-layer", default="batch_norm", choices=["batch_norm", "layer_norm"])
+    ap.add_argument("--inner-bn", action="store_true", help="enable_inner_loop_optimizable_bn_params (batch norm only)")
     cli = ap.parse_args()
+    if cli.inner_bn and cli.norm_layer == "layer_norm":
+        ap.error("--inner-bn needs --norm-layer batch_norm")
     if not torch.cuda.is_available():
         raise SystemExit("functional_route_timing.py needs a CUDA device")
     from howtotrainyourmamlpytorch_b200 import MAMLFewShotClassifier, make_args, synthetic_batch
@@ -113,7 +118,10 @@ def main():
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
     dev = torch.device("cuda", 0)
-    a = make_args(CONFIG, batch_size=META_BATCH, **({"norm_layer": "layer_norm"} if layer_norm else {}))
+    extra = {"norm_layer": "layer_norm"} if layer_norm else {}
+    if cli.inner_bn:
+        extra["enable_inner_loop_optimizable_bn_params"] = True
+    a = make_args(CONFIG, batch_size=META_BATCH, **extra)
     names = LN.trainable_names(a) if layer_norm else O.trainable_names(a)
     epoch = 0
     batch = synthetic_batch(a, iteration=0)
@@ -169,6 +177,8 @@ def main():
             "legs": {k: summary(v) for k, v in times.items()}, "skipped": skipped}
     if layer_norm:
         line["norm_layer"] = "layer_norm"
+    if cli.inner_bn:
+        line["inner_bn"] = True
     print(json.dumps(line))
 
 
