@@ -494,12 +494,13 @@ extern "C" int maml_b200_create(const maml_b200_config* cfg, maml_b200_handle** 
   if (e != cudaSuccess) { cudaFree(h->ws); delete h; return fail(std::string("cudaMallocHost: ") + cudaGetErrorString(e)); }
   h->use_graphs = !(cfg->reserved & 4) && !h->opt.no_graph;
   // Two regimes, told apart by whether one iteration's block-1 tiles (support + target, all tasks) fit one wave of SMs.
-  //  * latency-bound (Omniglot 5-way at 8 tasks: 144 tiles): programmatic dependent launch on the MAIN chain only (the next
+  //  * latency-bound (at most one tile per SM; on an H100's 132 SMs Omniglot 5-way up to 7 tasks -- at 8 tasks its 144 tiles
+  //    are more than 132, and it runs throughput-bound): programmatic dependent launch on the MAIN chain only (the next
   //    kernel of the support / tangent chain is scheduled while the current one drains; on every stream, early-launched
   //    CTAs hold the SM slots the other streams want), deep shared-memory rings (all B stages of a short pipeline
   //    prefetched at once).
-  //  * throughput-bound (Mini-ImageNet, 20-way): no PDL, conv ring 4 (the shared memory it gives up lets the BatchNorm /
-  //    first-block kernels of the other streams share the SM).
+  //  * throughput-bound (on an H100 every benchmarked workload: Omniglot at 8 tasks, Mini-ImageNet, 20-way): no PDL, conv
+  //    ring 4 (the shared memory it gives up lets the BatchNorm / first-block kernels of the other streams share the SM).
   {
     const int l1 = h->L > 1 ? 1 : 0;
     const long long tiles = (((long long)h->n_s * h->geo[l1].G + 127) / 128 + ((long long)h->n_t * h->geo[l1].G + 127) / 128) * h->maxT;

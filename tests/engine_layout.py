@@ -30,9 +30,23 @@ def _tc_ring(F, gw):
 
 
 def host_plan(a, tasks, num_sms=H100_SMS):
+    """The plan a handle made for ``tasks`` tasks (its max_tasks) takes, with the switches at their defaults:
+      tc, ring: tensor-core convolutions / weight gradients for blocks l >= 1, and the depth of their ring next to split-K
+                2 in tangent mode;
+      tail:     the support pass's fused last block + head;
+      chunks:   weight-gradient chunks per block l >= 1 (the most of any block);
+      regime:   "latency" when one iteration's block-1 conv tiles (support + target, every task) fit one wave of SMs,
+                else "throughput"; it decides programmatic dependent launch on the main chain (pdl) and the ring depth
+                of the main-chain tensor-core convolutions (nb).
+    The split-K cluster size of conv_tc_kernel comes from the occupancy calculator at launch and is not restated."""
     geo, _ = geometry(a)
     L, F = len(geo), int(a.cnn_num_filters)
     n_s = int(a.num_classes_per_set) * int(a.num_samples_per_class)
+    n_t = int(a.num_classes_per_set) * int(a.num_target_samples)
+    g1 = geo[1 if L > 1 else 0]
+    G1 = (g1["h"] + 1) * (g1["w"] + 1)
+    tiles = ((n_s * G1 + 127) // 128 + (n_t * G1 + 127) // 128) * tasks
+    small = tiles <= num_sms
     rings = [_tc_ring(F, geo[l]["w"] + 1) for l in range(1, L)]
     tc = L > 1 and all(_tc_rpad(geo[l]["w"] + 1) <= 256 for l in range(1, L)) and min(rings) >= 2
     head_rows = 16 if n_s <= 16 else 4
@@ -45,7 +59,8 @@ def host_plan(a, tasks, num_sms=H100_SMS):
         nch = min(64, max(1, num_sms // (3 * tasks)), max(1, (rows + 15) // 16))
         rpc = ((rows + nch - 1) // nch + 15) // 16 * 16
         chunks.append((rows + rpc - 1) // rpc)
-    return dict(tc=tc, tail=tail, ring=min(rings) if rings else None, chunks=max(chunks) if chunks else None)
+    return dict(tc=tc, tail=tail, ring=min(rings) if rings else None, chunks=max(chunks) if chunks else None,
+                tiles=tiles, regime="latency" if small else "throughput", pdl=small, nb=8 if small else 4)
 
 
 def norm_grid_regimes(a, tasks, num_sms=H100_SMS):
@@ -134,9 +149,12 @@ def flat_to_nchw(buf, n, h, w, F):
 
 
 def theta_to_ref(vec, args):
-    """Internal fast-weight vector -> {reference name: tensor in reference layout}."""
+    """Internal fast-weight vector -> {reference name: tensor in reference layout}: per block W [3*3][Cin][F] and b (with
+    inner-loop BatchNorm gamma / beta also beta, gamma [F]), then the linear layer [N][pix][F] and its bias."""
     geo, (ph, pw) = geometry(args)
     F, N = int(args.cnn_num_filters), int(args.num_classes_per_set)
+    per_block = ("conv.bias", "norm_layer.bias", "norm_layer.weight") if args.enable_inner_loop_optimizable_bn_params \
+        else ("conv.bias",)
     out, o = {}, 0
     v = np.asarray(vec)
     for l, g in enumerate(geo):
@@ -145,8 +163,9 @@ def theta_to_ref(vec, args):
         w = v[o:o + wsz].reshape(3, 3, cin, F).transpose(3, 2, 0, 1)     # [tap(ky,kx)][c][f] -> [f][c][ky][kx]
         out["classifier.layer_dict.conv%d.conv.weight" % l] = torch.from_numpy(np.ascontiguousarray(w))
         o += wsz
-        out["classifier.layer_dict.conv%d.conv.bias" % l] = torch.from_numpy(v[o:o + F].copy())
-        o += F
+        for n in per_block:
+            out["classifier.layer_dict.conv%d.%s" % (l, n)] = torch.from_numpy(v[o:o + F].copy())
+            o += F
     pix = ph * pw
     D = pix * F
     fw = v[o:o + N * D].reshape(N, pix, F).transpose(0, 2, 1).reshape(N, D)   # [k][pix][c] -> [k][c*pix + pix]
@@ -161,15 +180,39 @@ def rel_err(a, b):
     return float((a - b).abs().max()) / max(float(b.abs().max()), 1e-30)
 
 
-def gpu_decisions(m, g, batch, epoch):
-    """The discrete decisions the GPU actually took (leaky-ReLU branch per element, arg-max per pooling
-    window), reconstructed bit-exactly from the engine's normalised activations zh:
-    y = fmaf(gamma, zh, beta) (exact product + one rounding == fp64 evaluation rounded to fp32),
-    a = y > 0 ? y : 0.01f * y (fp32), first-max-wins in window order (what F.max_pool2d does on CPU).
-    ``m`` must have run ``meta_gradient`` with ``_debug_keep_target_passes`` set."""
-    import torch.nn.functional as Fnn
+def norm_params(args, state, theta, l, step):
+    """Block l's normalisation scale / shift in one pass at inner step ``step``: BatchNorm gamma / beta [F] (the step's
+    row with per-step statistics; the pass's fast weights ``theta`` with inner-loop gamma / beta), or layer norm's frozen
+    weight and bias [F, h, w]."""
     from oracle import maml_oracle as O
-    a = g.args
+    if getattr(args, "norm_layer", "batch_norm") == "layer_norm":
+        _, _, gn, btn, _, _ = O.conv_names(l)
+        return state[gn], state[btn]
+    return O._bn_params(state, theta, args, l, step)
+
+
+def activate_pool(zh, gamma, beta):
+    """What the GPU computes from its normalised activations zh [n, F, h, w] (fp32), bit for bit:
+    y = fmaf(gamma, zh, beta) (exact product + one rounding == fp64 evaluation rounded to fp32),
+    a = y > 0 ? y : 0.01f * y (fp32), 2x2 max-pool first-max-wins in window order (what F.max_pool2d does on CPU).
+    gamma / beta: [F] (BatchNorm) or [F, h, w] (layer norm).  Returns (leaky-ReLU slope per element, arg-max per pooling
+    window, pooled output)."""
+    import torch.nn.functional as Fnn
+    shape = (1, -1, 1, 1) if gamma.dim() == 1 else (1,) + tuple(gamma.shape)
+    y = (gamma.double().reshape(shape) * zh.double() + beta.double().reshape(shape)).float()
+    slope = torch.where(y > 0, torch.ones_like(y), torch.full_like(y, 0.01))
+    act = torch.where(y > 0, y, torch.tensor(0.01, dtype=torch.float32) * y)
+    p, idx = Fnn.max_pool2d(act, 2, 2, return_indices=True)
+    return slope, idx, p
+
+
+def gpu_decisions(m, args, batch, epoch):
+    """The discrete decisions the GPU actually took (leaky-ReLU branch per element, arg-max per pooling window) in every
+    pass, reconstructed bit-exactly from the engine's normalised activations zh (``activate_pool``) and the pass's
+    scale / shift (``norm_params``; inner-loop gamma / beta: the TASK's fast weights, theta^s in the support pass of step
+    s, theta^{s+1} in its target pass).  ``m`` must have run ``meta_gradient`` with ``_debug_keep_target_passes`` set."""
+    from oracle import maml_oracle as O
+    a = args
     eng = m._engine
     geo, _ = geometry(a)
     F = int(a.cnn_num_filters)
@@ -180,19 +223,16 @@ def gpu_decisions(m, g, batch, epoch):
     sd = {k: v.detach().cpu() for k, v in m.state_dict().items()}
     dec = {}
     for b in range(B):
+        thetas = [theta_to_ref(eng.debug_read("theta", b, s, 0), a) for s in range(S + 1)] \
+            if a.enable_inner_loop_optimizable_bn_params else [None] * (S + 1)
         for s in range(S):
-            for kind, n in (("sup", N * K), ("tgt", N * T)):
+            for kind, n, th in (("sup", N * K, thetas[s]), ("tgt", N * T, thetas[s + 1])):
                 if kind == "tgt" and sched[s] is None:
                     continue
                 per_layer = []
                 for l, gl in enumerate(geo):
                     zh = grid_to_nchw(eng.debug_read(kind + "_zh", b, s, l), n, gl["h"], gl["w"], F)
-                    _, _, gn, btn, _, _ = O.conv_names(l)
-                    gam, bet = (sd[gn][s], sd[btn][s]) if a.per_step_bn_statistics else (sd[gn], sd[btn])
-                    y = (gam.double()[None, :, None, None] * zh.double() + bet.double()[None, :, None, None]).float()
-                    slope = torch.where(y > 0, torch.ones_like(y), torch.full_like(y, 0.01))
-                    act = torch.where(y > 0, y, torch.tensor(0.01, dtype=torch.float32) * y)
-                    _, idx = Fnn.max_pool2d(act, 2, 2, return_indices=True)
+                    slope, idx, _ = activate_pool(zh, *norm_params(a, sd, th, l, s))
                     per_layer.append((slope, idx))
                 dec[(b, kind, s)] = per_layer
     return dec

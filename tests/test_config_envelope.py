@@ -265,7 +265,7 @@ def _forced_run(case, device):
         m = _model(g, device, keep_targets=True)
         batch, epoch = g.batch(0), g.iters[0][0]
         losses, preds, grads = m.meta_gradient(batch, epoch)
-        dec = gpu_decisions(m, g, batch, epoch)
+        dec = gpu_decisions(m, a, batch, epoch)
         ref = O.manual_train_iter(g.state(torch.float64), a, batch, epoch, decisions=dec, keep_intermediates=True)
         eng, L, S = m._engine, int(a.num_stages), int(a.number_of_training_steps_per_iter)
         sched = O.target_pass_schedule(a, epoch, True, S)

@@ -417,7 +417,7 @@ def test_decision_forced_parity(case, cuda_device):
     m.load_state_dict(g.state())
     batch, epoch = g.batch(0), g.iters[0][0]
     losses, preds, grads = m.meta_gradient(batch, epoch)
-    dec = _gpu_decisions(m, g, batch, epoch)
+    dec = _gpu_decisions(m, a, batch, epoch)
     ref = O.manual_train_iter(g.state(torch.float64), a, batch, epoch, decisions=dec, keep_intermediates=True)
     # (2) consistency of the GPU's decisions with exact arithmetic
     n_slope_flip, n_arg_flip, worst_margin, n_dec = 0, 0, 0.0, 0

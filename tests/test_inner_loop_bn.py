@@ -22,8 +22,8 @@ import torch
 
 import functional_cases as fc
 from conftest import grad_tolerance, load_golden
-from engine_layout import (check_norm_path, device_sms, flat_to_nchw, geometry, grid_to_nchw, host_plan,
-                           norm_grid_regimes, rel_err, traced_kernel_ids)
+from engine_layout import (check_norm_path, device_sms, flat_to_nchw, geometry, gpu_decisions, grid_to_nchw,
+                           host_plan, norm_grid_regimes, rel_err, theta_to_ref, traced_kernel_ids)
 from oracle import maml_oracle as O
 
 IBN_CASES = ["ibn_tiny_pp", "ibn_tiny_pp_moved", "ibn_tiny_first", "ibn_tiny_maml", "ibn_one_stage", "ibn_ffma_wide",
@@ -332,58 +332,6 @@ def test_functional_entries_refuse_inner_bn_handles(cuda_device):
 
 
 # ------------------------------------------------------------------------------------------------ stages and decisions
-def _theta_ibn(vec, args):
-    """Internal fast-weight vector -> {reference name: tensor}: per block W [3*3][Cin][F], b, beta, gamma [F]; then the
-    linear layer [N][pix][F] and its bias."""
-    geo, (ph, pw) = geometry(args)
-    F, N = int(args.cnn_num_filters), int(args.num_classes_per_set)
-    v, out, o = np.asarray(vec), {}, 0
-    for l, gl in enumerate(geo):
-        wsz = 9 * gl["cin"] * F
-        w = v[o:o + wsz].reshape(3, 3, gl["cin"], F).transpose(3, 2, 0, 1)
-        out["classifier.layer_dict.conv%d.conv.weight" % l] = torch.from_numpy(np.ascontiguousarray(w))
-        o += wsz
-        for n in ("conv.bias", "norm_layer.bias", "norm_layer.weight"):
-            out["classifier.layer_dict.conv%d.%s" % (l, n)] = torch.from_numpy(v[o:o + F].copy())
-            o += F
-    D = ph * pw * F
-    fw = v[o:o + N * D].reshape(N, ph * pw, F).transpose(0, 2, 1).reshape(N, D)
-    out[O.LIN_W] = torch.from_numpy(np.ascontiguousarray(fw))
-    out[O.LIN_B] = torch.from_numpy(v[o + N * D:o + N * D + N].copy())
-    return out
-
-
-def _gpu_decisions(m, g, batch, epoch):
-    """The leaky-ReLU branch per element and the arg-max per pooling window that the GPU took, rebuilt bit-exactly from its
-    normalised activations and the TASK's fast gamma / beta of the pass (theta^s for the support pass of step s,
-    theta^{s+1} for its target pass): y = fmaf(gamma, zh, beta) = the fp64 value rounded once to fp32, first max wins."""
-    import torch.nn.functional as Fnn
-    a, eng = g.args, m._engine
-    geo, _ = geometry(a)
-    F = int(a.cnn_num_filters)
-    N, K, T = int(a.num_classes_per_set), int(a.num_samples_per_class), int(a.num_target_samples)
-    S = int(a.number_of_training_steps_per_iter)
-    sched = O.target_pass_schedule(a, epoch, True, S)
-    dec = {}
-    for b in range(batch[0].shape[0]):
-        thetas = [_theta_ibn(eng.debug_read("theta", b, s, 0), a) for s in range(S + 1)]
-        for s in range(S):
-            for kind, n, th in (("sup", N * K, thetas[s]), ("tgt", N * T, thetas[s + 1])):
-                if kind == "tgt" and sched[s] is None:
-                    continue
-                per_layer = []
-                for l, gl in enumerate(geo):
-                    zh = grid_to_nchw(eng.debug_read(kind + "_zh", b, s, l), n, gl["h"], gl["w"], F)
-                    _, _, gn, btn, _, _ = O.conv_names(l)
-                    y = (th[gn].double()[None, :, None, None] * zh.double() + th[btn].double()[None, :, None, None]).float()
-                    slope = torch.where(y > 0, torch.ones_like(y), torch.full_like(y, 0.01))
-                    act = torch.where(y > 0, y, torch.tensor(0.01, dtype=torch.float32) * y)
-                    _, idx = Fnn.max_pool2d(act, 2, 2, return_indices=True)
-                    per_layer.append((slope, idx))
-                dec[(b, kind, s)] = per_layer
-    return dec
-
-
 def _decision_flips(intermediates):
     """(#decisions differing from fp64, worst fp64 margin at one) of a pinned run: leaky-ReLU branches and pooling
     arg-maxes."""
@@ -423,7 +371,7 @@ def _stage_report(a, eng, ref, B):
         worst = max(worst, e / tol)
 
     def chk_vec(tag, vec, want, tol=5e-5):
-        got = _theta_ibn(vec, a)
+        got = theta_to_ref(vec, a)
         for n, v in want.items():
             if n.endswith("conv.bias"):
                 continue          # dead under BatchNorm: gradient and tangent are rounding noise
@@ -482,7 +430,7 @@ def _forced_run(case, device):
         m = _model(g, device, _debug_keep_target_passes=True)
         batch, epoch = g.batch(0), g.iters[0][0]
         losses, preds, grads = m.meta_gradient(batch, epoch)
-        dec = _gpu_decisions(m, g, batch, epoch)
+        dec = gpu_decisions(m, g.args, batch, epoch)
         ref = O.manual_train_iter(g.state(torch.float64), g.args, batch, epoch, decisions=dec, keep_intermediates=True)
         rows, worst = _stage_report(g.args, m._engine, ref, batch[0].shape[0])
         _RUNS[case] = dict(rows=rows, worst=worst, flips=_decision_flips(ref["intermediates"]), loss=float(losses["loss"]),

@@ -21,8 +21,8 @@ import torch
 
 import functional_cases as fc
 from conftest import load_golden
-from engine_layout import (check_norm_path, device_sms, flat_to_nchw, geometry, grid_to_nchw, host_plan,
-                           norm_grid_regimes, rel_err, theta_to_ref, traced_kernel_ids)
+from engine_layout import (check_norm_path, device_sms, flat_to_nchw, geometry, gpu_decisions, grid_to_nchw,
+                           host_plan, norm_grid_regimes, rel_err, theta_to_ref, traced_kernel_ids)
 from oracle import ln_oracle as LN
 from oracle import maml_oracle as O
 
@@ -334,35 +334,6 @@ def test_layer_norm_is_not_transductive(cuda_device):
 
 
 # ------------------------------------------------------------------------------------------------ stages and decisions
-def _gpu_decisions(m, g, batch, epoch):
-    """The leaky-ReLU branch per element and the arg-max per pooling window that the GPU took, rebuilt bit-exactly from
-    its normalised activations: y = fmaf(1, zh, b) = zh + b rounded once to fp32, first max wins in window order."""
-    import torch.nn.functional as Fnn
-    a, eng = g.args, m._engine
-    geo, _ = geometry(a)
-    F = int(a.cnn_num_filters)
-    N, K, T = int(a.num_classes_per_set), int(a.num_samples_per_class), int(a.num_target_samples)
-    S = int(a.number_of_training_steps_per_iter)
-    sched = O.target_pass_schedule(a, epoch, True, S)
-    sd = {k: v.detach().cpu() for k, v in m.state_dict().items()}
-    dec = {}
-    for b in range(batch[0].shape[0]):
-        for s in range(S):
-            for kind, n in (("sup", N * K), ("tgt", N * T)):
-                if kind == "tgt" and sched[s] is None:
-                    continue
-                per_layer = []
-                for l, gl in enumerate(geo):
-                    zh = grid_to_nchw(eng.debug_read(kind + "_zh", b, s, l), n, gl["h"], gl["w"], F)
-                    y = (zh.double() + sd[O.conv_names(l)[3]].double()[None]).float()
-                    slope = torch.where(y > 0, torch.ones_like(y), torch.full_like(y, 0.01))
-                    act = torch.where(y > 0, y, torch.tensor(0.01, dtype=torch.float32) * y)
-                    _, idx = Fnn.max_pool2d(act, 2, 2, return_indices=True)
-                    per_layer.append((slope, idx))
-                dec[(b, kind, s)] = per_layer
-    return dec
-
-
 def _decision_flips(intermediates):
     """(#decisions differing from fp64, worst fp64 margin at one) of a pinned run: leaky-ReLU branches and pooling
     arg-maxes."""
@@ -458,7 +429,7 @@ def _forced_run(case, device):
         m = _model(g, device, _debug_keep_target_passes=True)
         batch, epoch = g.batch(0), g.iters[0][0]
         losses, preds, grads = m.meta_gradient(batch, epoch)
-        dec = _gpu_decisions(m, g, batch, epoch)
+        dec = gpu_decisions(m, g.args, batch, epoch)
         ref = LN.manual_train_iter(g.state(torch.float64), g.args, batch, epoch, decisions=dec, keep_intermediates=True)
         rows, worst = _stage_report(g.args, m._engine, ref, batch[0].shape[0])
         _RUNS[case] = dict(rows=rows, worst=worst, flips=_decision_flips(ref["intermediates"]), loss=float(losses["loss"]),
